@@ -46,7 +46,7 @@ WORKLOADS = {
     "c3": (10_000_000, 1024, "f32", 1024, 100, "dot", "configs[2]: N=10M d=1024 fp32 Q=1024 k=100 inner-product"),
     "c4": (10_000_000, 768, "f16", 1, 10, "euclidean", "configs[3]: N=10M d=768 fp16 Q=1 k=10 L2"),
     "c5": (100_000_000, 1024, "f32", 1024, 10, "cosine",
-           "configs[4]: N=100M d=1024 fp32 Q=1024 k=10 cosine, row-sharded (needs >= 4 GPUs: 410 GB of corpus)"),
+           "configs[4]: N=100M d=1024 fp32 Q=1024 k=10 cosine, row-sharded (needs >= 8 GPUs of 80 GB: 410 GB of corpus + its BF16 shadow)"),
     "c1": (100_000, 128, "f32", 1, 10, "cosine", "configs[0]: N=100k d=128 fp32 Q=1 k=10 cosine"),
     "q1": (10_000_000, 1024, "f32", 1, 10, "cosine", "N=10M d=1024 fp32 Q=1 k=10 cosine (single-query latency)"),
     "clustered": (10_000_000, 1024, "f32", 64, 10, "cosine",
@@ -60,9 +60,9 @@ SCAN_DESC = {
     "tensor": "exact 3xTF32 scan over the fp32 rows",
     "simt": "CUDA-core scan over the stored rows",
 }
-KERNEL_NAME = {"tensor": "knn_scan_tc_kernel<3> (tcgen05/TMEM/TMA, 3xTF32 exact)",
-               "filter": "knn_scan_tc_kernel<1> (tcgen05/TMEM/TMA, 1xTF32 filter + exact fp32 rescoring)",
-               "shadow": "knn_scan_shadow_kernel (tcgen05/TMEM/TMA over the 16-bit corpus image + exact fp32 rescoring)",
+KERNEL_NAME = {"tensor": "knn_scan_tc_kernel<3> (wgmma/TMA, 3xTF32 exact)",
+               "filter": "knn_scan_tc_kernel<1> (wgmma/TMA, 1xTF32 filter + exact fp32 rescoring)",
+               "shadow": "knn_scan_shadow_kernel (wgmma/TMA over the 16-bit corpus image + exact fp32 rescoring)",
                "simt": "knn_scan_simt_kernel"}
 
 
@@ -82,12 +82,15 @@ def parse_args():
     ap.add_argument("--no-parity", action="store_true", help="skip the untimed parity post-check")
     ap.add_argument("--exchange", default="peer", choices=["peer", "nccl"],
                     help="N>1 candidate exchange: peer-memory kernels behind the C ABI (default) or NCCL all-gather + merge")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step returned (indices.npy as float64, scores.npy "
+                         "as float32, [Q x k]) to DIR, so that two builds can be compared output for output on identical inputs")
     return ap.parse_args()
 
 
 # ------------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -155,32 +158,19 @@ def load_peaks():
     d = _peaks()
     if d and "hbm_gbs" in d:
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet: 3.35 TB/s HBM3)"
 
 
 def load_tensor_peak(bf16=False):
     """Dense tensor TFLOP/s of the arithmetic the scan uses: BF16 / FP16 (16-bit path), or TF32 = half the bf16 figure
-    (tf32 : bf16 = 1.1 : 2.25 PFLOP/s nominal, B200_PROFILING.md table).  Sustained, because the scan runs inside a
-    long, power-capped step."""
+    (H100 SXM data sheet, dense: 989 TFLOP/s bf16, 495 tf32, at a 700 W power limit)."""
     div = 1.0 if bf16 else 2.0
     what = "" if bf16 else " / 2: dense TF32 runs at half the bf16 rate"
     d = _peaks()
     if d and ("bf16_tflops_sustained" in d or "bf16_tflops" in d):
         return float(d.get("bf16_tflops_sustained", d.get("bf16_tflops"))) / div, \
             f"measured (MEASURED_PEAKS.json bf16_tflops_sustained{what})"
-    return 1590.0 / div, f"fallback (B200_PROFILING.md 1.59 PFLOP/s bf16{what})"
-
-
-def load_traffic(workload: str, path: str):
-    """dram bytes per scan launch from the committed ncu --set full capture (profiles/traffic.json), or None."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.exists(p):
-        try:
-            d = json.load(open(p))
-            return d.get(f"{workload}:{path}", d.get(workload))
-        except Exception:
-            return None
-    return None
+    return 989.0 / div, f"fallback (H100 SXM data sheet: 989 TFLOP/s dense bf16{what})"
 
 
 def scan_bytes(path: str, n: int, dim: int, dtype: str) -> int:
@@ -380,6 +370,7 @@ def measure(run: Runner, ix, n_shard, N_total, dim, dtype, Q, k, metric, steps, 
     t_wall0 = time.perf_counter()
     total_ms = run.timed_steps(lambda s: search_dev(q_all[warmup + s].data_ptr()), steps, flush)
     t_wall = time.perf_counter() - t_wall0
+    last = (out_idx.clone(), out_score.clone())  # what the last timed step returned (later calls overwrite out_*)
     scan_ms, scan_launches = ix.scan_time_ms()
     ix.enable_timing(False)
     launches = ix.stats()["kernel_launches"] - launches0 + (steps if G > 1 and not peer else 0)
@@ -404,8 +395,8 @@ def measure(run: Runner, ix, n_shard, N_total, dim, dtype, Q, k, metric, steps, 
     res = {"value": Q * steps / (total_ms / 1e3), "ms_per_step": total_ms / steps, "steps": steps, "path": used_path,
            "scan_ms": scan_ms, "scan_launches": scan_launches, "launches": int(launches), "wall_s": t_wall, "clocks": clocks,
            "l2": "L2 flushed between steps (256 MB memset, untimed)" if flush is not None
-                 else "corpus shard per GPU >> 126 MB L2 (inputs larger than L2; no flush needed)",
-           "out_idx": out_idx, "out_score": out_score, "q_all": q_all, "search_dev": search_dev}
+                 else "corpus shard per GPU >> 50 MB L2 (inputs larger than L2; no flush needed)",
+           "out_idx": out_idx, "out_score": out_score, "q_all": q_all, "search_dev": search_dev, "last": last}
 
     if want_e2e:
         # e2e: the reference-facing call with HOST buffers (H2D queries + D2H results inside the timed region)
@@ -452,7 +443,7 @@ def roofline_of(res, n_shard, dim, dtype, Q, workload, peak, peak_src):
     avg_ms = res["scan_ms"] / launches
     achieved = algo / (avg_ms / 1e3) / 1e9
     r = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-         "traffic": load_traffic(workload, path), "peak_source": peak_src, "kernel": KERNEL_NAME.get(path, path),
+         "peak_source": peak_src, "kernel": KERNEL_NAME.get(path, path),
          "algorithmic_bytes_per_launch": algo, "avg_launch_ms": avg_ms, "scan_launches_per_step": launches / res["steps"],
          "scan_share_of_step": res["scan_ms"] / (res["ms_per_step"] * res["steps"])}
     fp32_bytes = n_shard * dim * (4 if dtype == "f32" else 2)
@@ -490,6 +481,15 @@ def also_entry(res, n, dim, dtype, Q, desc, peak, peak_src, workload):
     if "e2e" in res:
         e["e2e"] = res["e2e"]
     return e
+
+
+def dump_outputs(out_dir, idx, score):
+    """The last timed step's result as the caller receives it: global row indices ([Q x k], float64 holds every uint32
+    exactly) and scores ([Q x k] float32)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "indices.npy"), idx.cpu().numpy().view(np.uint32).astype(np.float64))
+    np.save(os.path.join(out_dir, "scores.npy"), score.cpu().numpy().astype(np.float32))
 
 
 # ------------------------------------------------------------------------------------------------------
@@ -581,7 +581,7 @@ def parity_check(run: Runner, ix, lo, hi, N_total, dim, dtype, Q, k, metric, res
         if run.rank == 0:
             try:
                 shard_gb = (N_total // G) * dim * (4 if dtype == "f32" else 2) / 1e9
-                tight = shard_gb * 3.0 > 140  # a second shard + shadow would not fit beside this rank's own rows + shadow
+                tight = shard_gb * 3.0 > 75  # a second shard + shadow would not fit beside this rank's own rows + shadow
                 if tight:
                     os.environ["NK_SHADOW"] = "0"  # read at index creation: rows only (TF32 filter path, same exact results)
                 mix = KnnIndex(dim, metric=metric, dtype=dtype, devices=tuple(range(G)))
@@ -644,13 +644,13 @@ def main():
             sys.exit(2)
         G = world
     elem = 2 if dtype != "f32" else 4
-    if N_total // max(G, 1) * dim * elem > 150e9:
+    if N_total // max(G, 1) * dim * elem > 52e9:  # rows + their BF16 shadow (+50%) within an 80 GB GPU
         if rank == 0:
             print(json.dumps({"error": f"workload {args.workload} needs more GPUs: {N_total // max(G, 1) * dim * elem / 1e9:.0f} GB per GPU"}))
         return
     config = {"workload": desc, "N": N_total, "dim": dim, "corpus_dtype": dtype, "Q": Q, "k": k, "metric": metric,
               "sharding": f"row-range x{G}" if G > 1 else "single GPU",
-              "l2": "corpus shard per GPU >> 126 MB L2 (inputs larger than L2; no flush needed)"
+              "l2": "corpus shard per GPU >> 50 MB L2 (inputs larger than L2; no flush needed)"
               if N_total // G * dim * elem > 512e6 else "L2 flushed between steps (256 MB memset)"}
 
     # ------------------------------------------------------------------ reference arm (CPU)
@@ -700,6 +700,8 @@ def main():
 
     res = measure(run, ix, n_shard, N_total, dim, dtype, Q, k, metric, args.steps, args.warmup, want_e2e=True, sample_clocks=True)
     used_path = res["path"]
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, *res["last"])
     roofline = roofline_of(res, n_shard, dim, dtype, Q, args.workload, peak, peak_src)
     algo = roofline["algorithmic_bytes_per_launch"]
     line = {
@@ -724,7 +726,7 @@ def main():
                                   "note": "asynchronous API: a first-stage overflow goes straight to the exact stage (exact_stage_rate); the TF32 retry stage belongs to the host-synchronous nk_search"}
     if not args.no_parity:
         line["parity_check"] = parity_check(run, ix, lo, hi, N_total, dim, dtype, Q, k, metric, res, clustered=clustered)
-    for key in ("out_idx", "out_score", "q_all", "search_dev"):
+    for key in ("out_idx", "out_score", "q_all", "search_dev", "last"):
         res.pop(key, None)
 
     # ---- the rest of the north_star grid (default N=1 line only), same timing rules, device-resident + e2e where cheap
@@ -737,7 +739,7 @@ def main():
                 index.set_path(path)
                 c0, s0 = index.debug_counters(), index.stats()["searches"]
                 r = measure(run, index, n, n, d, dt, q_, k_, m_, steps, warm, want_e2e=e2e)
-                for key in ("out_idx", "out_score", "q_all", "search_dev"):
+                for key in ("out_idx", "out_score", "q_all", "search_dev", "last"):
                     r.pop(key, None)
                 also[name] = also_entry(r, n, d, dt, q_, desc_, peak, peak_src, wl or name)
                 if r["path"] in ("shadow", "filter"):

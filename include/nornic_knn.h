@@ -1,5 +1,5 @@
 /*
- * nornic_knn.h — C ABI of libnornic_knn.so, the B200-native brute-force kNN engine that sits behind
+ * nornic_knn.h — C ABI of libnornic_knn.so, the H100-native brute-force kNN engine that sits behind
  * NornicDB's GPU boundary.
  *
  * Part 1 re-exports, symbol for symbol, the C functions of the cgo preamble in the reference's
@@ -51,7 +51,7 @@ CudaDevice *cuda_create_device(int device_id);       /* cuda_bridge.go:56  (NULL
 void cuda_release_device(CudaDevice *dev);           /* cuda_bridge.go:94  (NULL-safe) */
 const char *cuda_device_name(int device_id);         /* cuda_bridge.go:102 ("Unknown" on error) */
 size_t cuda_device_memory(int device_id);            /* cuda_bridge.go:113 (bytes, 0 on error) */
-int cuda_device_compute_capability(int device_id);   /* cuda_bridge.go:122 (major*10+minor; B200 = 100) */
+int cuda_device_compute_capability(int device_id);   /* cuda_bridge.go:122 (major*10+minor; H100 = 90) */
 
 /* cuda_bridge.go:138.  count is in floats; host_data may be NULL (uninitialised buffer); the copy
  * is synchronous.  memory_type 0 = device, 1 = pinned host. */
@@ -86,7 +86,7 @@ int cuda_topk(CudaDevice *dev, CudaBuffer *scores, unsigned int *out_indices, fl
 enum { NK_METRIC_COSINE = 0, NK_METRIC_DOT = 1, NK_METRIC_EUCLIDEAN = 2 };
 /* Corpus element type held in HBM.  Queries and scores are always fp32.  fp16 / bf16 corpora (SURVEY.md §8(f)3 "fp16/bf16
  * down-conversion at load") are half the bytes; batches of >= 5 queries scan them IN PLACE on the tensor cores
- * (tcgen05.mma.kind::f16 with fp16 or bf16 operands — no shadow copy, no row-side rounding residue). */
+ * (fp16 or bf16 wgmma operands — no shadow copy, no row-side rounding residue). */
 enum { NK_DTYPE_F32 = 0, NK_DTYPE_F16 = 1, NK_DTYPE_BF16 = 2 };
 /* Kernel selection for nk_index_set_path (diagnostics / tests); AUTO picks by Q, dim and dtype. */
 /* TENSOR = exact 3xTF32 tensor-core scan; TENSOR_FILTER = 1xTF32 prefilter over the fp32 rows with rigorous margins +

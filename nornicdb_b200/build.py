@@ -1,4 +1,4 @@
-"""Build libnornic_knn.so (sm_100a) in-tree with nvcc.  No GPU is needed to build.
+"""Build libnornic_knn.so (sm_90a) in-tree with nvcc.  No GPU is needed to build.
 
 The library is plain CUDA C++ + cudart (no torch, no cuBLAS); it is loaded through ctypes by
 nornicdb_b200._lib and is what a cgo / JNI / N-API host would link (INTEGRATION.md)."""
@@ -12,10 +12,10 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libnornic_knn.so")
-SOURCES = ["runtime.cu", "rowops.cu", "merge.cu", "scan_simt.cu", "scan_tensor.cu", "scan_tensor_shadow.cu", "scan_tensor_pair.cu", "assign_tensor.cu", "exchange.cu", "legacy_abi.cu", "index_api.cu"]
+SOURCES = ["runtime.cu", "rowops.cu", "merge.cu", "scan_simt.cu", "scan_tensor.cu", "scan_tensor_shadow.cu", "assign_tensor.cu", "exchange.cu", "legacy_abi.cu", "index_api.cu"]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-O2",
     "--expt-relaxed-constexpr",
@@ -61,7 +61,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
             sys.stderr.write(f"--- nvcc {src} ---\n{out}\n")
     if failed:
         raise RuntimeError("nvcc failed building libnornic_knn.so")
-    link = [NVCC, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-ccbin", "/usr/bin/g++",
+    link = [NVCC, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-ccbin", "/usr/bin/g++",
             "-cudart", "static", "-o", OUT, *objs]
     subprocess.run(link, check=True)
     with open(stamp_file, "w") as f:

@@ -2,10 +2,11 @@
 //
 // nearest centroid of every corpus row = the Q x N^T contraction of the scan with Q = #centroids and an ARGMAX over the
 // centroid columns instead of a per-query top-k.  The kernel reuses the shadow scan's pipeline (scan_tensor_shadow.cu:
-// TMA slabs of the BF16 shadow and of the bf16 centroids, tcgen05.mma.kind::f16 from shared memory, double-buffered TMEM
-// accumulators) with one more loop level — every corpus tile is multiplied with each block of 128 centroids in turn (the
-// tile is re-read from L2, it crossed HBM once) — and a register-only epilogue: thread = corpus row keeps the four best
-// UPPER bounds and the best LOWER bound of its row's scores across all centroid blocks.
+// TMA slabs of the BF16 shadow and of the bf16 centroids, wgmma from shared memory, accumulators in the registers of two
+// consumer warpgroups) with one more loop level — every corpus tile is multiplied with each block of 64 centroids in turn
+// (the tile is re-read from L2, it crossed HBM once) — and a register-only epilogue: each thread keeps, for each of its
+// four fragment rows, the four best UPPER bounds and the best LOWER bound over its columns of every centroid block; the
+// four lanes that share a row merge their lists at the end.
 //   cosine    (assignToCentroidsGPU, kmeans.go:491-546)  score = x.c/|c|            (|x| > 0 does not change the argmax)
 //   euclidean (assignToCentroids,    kmeans.go:458-489)  score = 2 x.c - |c|^2      (argmin |x-c|^2)
 // with the rigorous BF16 bound of scan_tensor_shadow.cu.  A row whose runner-up cannot reach the winner's lower bound is
@@ -15,7 +16,7 @@
 #include <stdlib.h>
 
 #include "kernels.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 #include "scan_tensor_shared.cuh"
 
 namespace nk {
@@ -24,12 +25,12 @@ namespace asg {
 using namespace tc;
 constexpr int NTHREADS = 384;
 constexpr int ROWS = 256;
-constexpr int QT = 128;
+constexpr int QT = 64;
 constexpr int BKB = 64;
 constexpr int ASTAGES = 4;
 constexpr int A_BYTES = ROWS * 128;
 constexpr int B_BYTES = QT * 128;
-constexpr int BSTAGES = 5;
+constexpr int BSTAGES = 8;
 constexpr int RING_BYTES = ASTAGES * A_BYTES + BSTAGES * B_BYTES;
 constexpr int EPI_WARP0 = 4;
 constexpr uint32_t NONE = 0xffffffffu, ALL = 0xfffffffeu;
@@ -47,8 +48,6 @@ struct Params {
 struct __align__(8) Shared {
     uint64_t afull[ASTAGES], aempty[ASTAGES];
     uint64_t bfull[BSTAGES], bempty[BSTAGES];
-    uint64_t accfull[2], accempty[2][2];
-    uint32_t tmem_base;
 };
 }  // namespace asg
 
@@ -66,20 +65,12 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
     if (warp == 0 && lane == 0) {
         ptx::prefetch_tensormap(&map_rows);
         ptx::prefetch_tensormap(&map_q);
-        for (int i = 0; i < ASTAGES; ++i) { ptx::mbar_init(&sh.afull[i], 1); ptx::mbar_init(&sh.aempty[i], 1); }
-        for (int i = 0; i < BSTAGES; ++i) { ptx::mbar_init(&sh.bfull[i], 1); ptx::mbar_init(&sh.bempty[i], 1); }
-        for (int b = 0; b < 2; ++b) {
-            ptx::mbar_init(&sh.accfull[b], 1);
-            ptx::mbar_init(&sh.accempty[b][0], 4);
-            ptx::mbar_init(&sh.accempty[b][1], 4);
-        }
+        // a stage is free again once every consumer warp has seen its MMAs complete
+        for (int i = 0; i < ASTAGES; ++i) { ptx::mbar_init(&sh.afull[i], 1); ptx::mbar_init(&sh.aempty[i], 8); }
+        for (int i = 0; i < BSTAGES; ++i) { ptx::mbar_init(&sh.bfull[i], 1); ptx::mbar_init(&sh.bempty[i], 8); }
         ptx::fence_barrier_init();
     }
-    if (warp == 2) ptx::tmem_alloc(&sh.tmem_base, TMEM_COLS);
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem = sh.tmem_base;
 
     if (warp == 0) {
         // TMA producer: shadow slabs; a tile is streamed once per centroid block (first from HBM, then from L2)
@@ -110,94 +101,111 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                     }
                     __syncwarp();
                 }
-    } else if (warp == 1) {
-        // MMA issuer
-        const uint32_t idesc = ptx::make_idesc_bf16(128, QT);
-        uint32_t g = 0, it = 0;
-        for (uint32_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x)
-            for (uint32_t qbk = 0; qbk < nqb; ++qbk, ++it) {
-                const uint32_t buf = it & 1;
-                ptx::mbar_wait(&sh.accempty[buf][0], ((it >> 1) & 1) ^ 1);
-                ptx::mbar_wait(&sh.accempty[buf][1], ((it >> 1) & 1) ^ 1);
+    } else if (warp >= EPI_WARP0) {
+        // consumers: warpgroup m owns rows [128 m, 128 m + 128) of the tile as two m64 halves h; thread = 4 rows
+        // (rbase + 64 h + 8 r) x QT/4 centroid columns (cbase + 8 (j / 2) + j % 2) of every centroid block
+        const uint32_t ewarp = warp - EPI_WARP0, m = ewarp >> 2, wq = ewarp & 3;
+        const uint32_t rbase = m * 128 + wq * 16 + ((uint32_t)lane >> 2), cbase = 2u * ((uint32_t)lane & 3u);
+        const bool euclid = p.metric == NK_METRIC_EUCLIDEAN;
+        // score = mul * acc - (euclid ? |c|^2 : 0);  bound = ra qa[c] + rb qb[c] (+ 1e-6 |c|^2)
+        const float mul = euclid ? 2.0f : 1.0f;
+        float acc[2][QT / 2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < QT / 2; ++i) acc[h][i] = 0.0f;
+        uint32_t g = 0;
+        for (uint32_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+            float x2[4], ra[4], rb[4], maxlo[4], u[4][4];
+            uint32_t id[4][4];
+#pragma unroll
+            for (int ri = 0; ri < 4; ++ri) {
+                const uint32_t row = tile * ROWS + rbase + 64 * (ri >> 1) + 8 * (ri & 1);
+                x2[ri] = row < p.n ? __ldg(p.xnorm2 + row) : 0.0f;
+                const float dxn = sqrtf(row < p.n ? __ldg(p.dnorm2 + row) : 0.0f) * 1.0001f;
+                ra[ri] = mul * dxn;
+                rb[ri] = mul * sqrtf(x2[ri]);
+                maxlo[ri] = -INFINITY;
+#pragma unroll
+                for (int e = 0; e < 4; ++e) { u[ri][e] = -INFINITY; id[ri][e] = NONE; }
+            }
+            for (uint32_t qbk = 0; qbk < nqb; ++qbk) {
                 for (uint32_t j = 0; j < nslab; ++j, ++g) {
                     const uint32_t sa = g % ASTAGES, sbq = g % BSTAGES;
                     ptx::mbar_wait(&sh.bfull[sbq], (g / BSTAGES) & 1);
                     ptx::mbar_wait(&sh.afull[sa], (g / ASTAGES) & 1);
-                    ptx::tc_fence_after();
-                    if (ptx::elect_one_sync()) {
-                        const uint64_t bdesc = ptx::make_smem_desc_sw128(ptx::smem_u32(b_base + (size_t)sbq * B_BYTES));
-                        const uint32_t abase = ptx::smem_u32(a_base + (size_t)sa * A_BYTES);
+                    const uint64_t bdesc = ptx::make_smem_desc_sw128(ptx::smem_u32(b_base + (size_t)sbq * B_BYTES));
+                    const uint32_t abase = ptx::smem_u32(a_base + (size_t)sa * A_BYTES + (size_t)m * (A_BYTES / 2));
+                    ptx::wgmma_fence();
 #pragma unroll
-                        for (uint32_t m = 0; m < 2; ++m) {
-                            const uint64_t adesc = ptx::make_smem_desc_sw128(abase + m * (A_BYTES / 2));
-                            const uint32_t d = tmem + (buf * 2 + m) * QT;
+                    for (uint32_t h = 0; h < 2; ++h) {
+                        const uint64_t adesc = ptx::make_smem_desc_sw128(abase + h * (A_BYTES / 4));
 #pragma unroll
-                            for (uint32_t kk = 0; kk < 4; ++kk) ptx::mma_bf16_ss(d, adesc + kk * 2, bdesc + kk * 2, idesc, (j | kk) != 0);
-                        }
-                        ptx::tc_commit(&sh.aempty[sa]);
-                        ptx::tc_commit(&sh.bempty[sbq]);
-                        if (j + 1 == nslab) ptx::tc_commit(&sh.accfull[buf]);
+                        for (uint32_t kk = 0; kk < 4; ++kk) ptx::wgmma_bf16_n64(acc[h], adesc + kk * 2, bdesc + kk * 2, (j | kk) != 0);
                     }
+                    ptx::wgmma_commit();
+                    ptx::wgmma_wait_all();
+                    ptx::fence_acc(acc[0]);
+                    ptx::fence_acc(acc[1]);
                     __syncwarp();
+                    if (lane == 0) { ptx::mbar_arrive(&sh.aempty[sa]); ptx::mbar_arrive(&sh.bempty[sbq]); }
                 }
-            }
-    } else if (warp >= EPI_WARP0) {
-        // epilogue: one warpgroup per 128-row M-tile, thread = corpus row; everything stays in registers
-        const uint32_t m = (uint32_t)(warp - EPI_WARP0) >> 2, quad = warp & 3;
-        const uint32_t lane_base = (quad * 32u) << 16;
-        const uint32_t rt = m * 128 + quad * 32 + lane;
-        const bool euclid = p.metric == NK_METRIC_EUCLIDEAN;
-        uint32_t it = 0;
-        for (uint32_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-            const uint32_t row = tile * ROWS + rt;
-            const float x2 = row < p.n ? __ldg(p.xnorm2 + row) : 0.0f;
-            const float xn = sqrtf(x2);
-            const float dxn = sqrtf(row < p.n ? __ldg(p.dnorm2 + row) : 0.0f) * 1.0001f;
-            // score = mul * acc - (euclid ? |c|^2 : 0);  bound = ra qa[c] + rb qb[c] (+ 1e-6 |c|^2)
-            const float mul = euclid ? 2.0f : 1.0f, ra = mul * dxn, rb = mul * xn;
-            float u0 = -INFINITY, u1 = -INFINITY, u2 = -INFINITY, u3 = -INFINITY, maxlo = -INFINITY;
-            uint32_t i0 = NONE, i1 = NONE, i2 = NONE, i3 = NONE;
-            for (uint32_t qbk = 0; qbk < nqb; ++qbk, ++it) {
-                const uint32_t buf = it & 1;
-                ptx::mbar_wait(&sh.accfull[buf], (it >> 1) & 1);
-                ptx::tc_fence_after();
-#pragma unroll 1
-                for (uint32_t chunk = 0; chunk < QT / 64; ++chunk) {
-                    const uint32_t cb = qbk * QT + chunk * 64;
-                    uint32_t v0[32], v1[32];
-                    ptx::tmem_ld_32x32b_x32(tmem + lane_base + (buf * 2 + m) * QT + chunk * 64, v0);
-                    ptx::tmem_ld_32x32b_x32(tmem + lane_base + (buf * 2 + m) * QT + chunk * 64 + 32, v1);
-                    ptx::tmem_wait_ld();
-                    if (chunk + 1 == QT / 64) {
-                        ptx::tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) ptx::mbar_arrive(&sh.accempty[buf][m]);
-                    }
-                    if (cb < p.K) {
 #pragma unroll
-                        for (uint32_t c = 0; c < 64; ++c) {
-                            const uint32_t ci = cb + c;  // centroid index (uniform over the warp)
-                            if (ci < p.K) {
-                                const float acc = __uint_as_float(c < 32 ? v0[c & 31] : v1[c & 31]);
-                                const float qn = __ldg(p.qn + ci);
-                                const float cc = euclid ? qn * qn : 0.0f;
-                                const float s = fmaf(acc, mul, -cc);
-                                const float bnd = fmaf(ra, __ldg(p.qa + ci), rb * __ldg(p.qb + ci)) + 1e-6f * cc;
-                                const float up = s + bnd, lo = s - bnd;
-                                maxlo = fmaxf(maxlo, lo);  // NaN scores never enter: such rows end up in the exact fix-up
-                                if (up > u3) {  // strict: among equal bounds the lower centroid index stays ahead
-                                    u3 = up; i3 = ci;
-                                    if (u3 > u2) { float t = u2; u2 = u3; u3 = t; uint32_t ti = i2; i2 = i3; i3 = ti; }
-                                    if (u2 > u1) { float t = u1; u1 = u2; u2 = t; uint32_t ti = i1; i1 = i2; i2 = ti; }
-                                    if (u1 > u0) { float t = u0; u0 = u1; u1 = t; uint32_t ti = i0; i0 = i1; i1 = ti; }
+                for (int jj = 0; jj < QT / 4; ++jj) {
+                    const uint32_t ci = qbk * QT + cbase + 8 * (jj >> 1) + (jj & 1);  // centroid index, ascending in jj
+                    if (ci >= p.K) continue;
+                    const float qn = __ldg(p.qn + ci), qa = __ldg(p.qa + ci), qb = __ldg(p.qb + ci);
+                    const float cc = euclid ? qn * qn : 0.0f;
+#pragma unroll
+                    for (int ri = 0; ri < 4; ++ri) {
+                        const float s = fmaf(acc[ri >> 1][(jj >> 1) * 4 + (ri & 1) * 2 + (jj & 1)], mul, -cc);
+                        const float bnd = fmaf(ra[ri], qa, rb[ri] * qb) + 1e-6f * cc;
+                        const float up = s + bnd, lo = s - bnd;
+                        maxlo[ri] = fmaxf(maxlo[ri], lo);  // NaN scores never enter: such rows end up in the exact fix-up
+                        if (up > u[ri][3]) {  // strict: among equal bounds the lower centroid index stays ahead
+                            u[ri][3] = up; id[ri][3] = ci;
+#pragma unroll
+                            for (int e = 3; e > 0; --e)
+                                if (u[ri][e] > u[ri][e - 1]) {
+                                    const float t = u[ri][e - 1]; u[ri][e - 1] = u[ri][e]; u[ri][e] = t;
+                                    const uint32_t ti = id[ri][e - 1]; id[ri][e - 1] = id[ri][e]; id[ri][e] = ti;
                                 }
-                            }
                         }
                     }
                 }
             }
-            if (row < p.n) {
-                const bool decided = i0 != NONE && !(u1 >= maxlo) && x2 > 0.0f && x2 < INFINITY;
+#pragma unroll
+            for (int ri = 0; ri < 4; ++ri) {
+                // the four lanes of a row saw disjoint columns: merge their lists, ordered by (bound desc, centroid asc) —
+                // the order the strict insertion above produces over ascending centroids
+#pragma unroll
+                for (int o = 1; o <= 2; o <<= 1) {
+                    float pu[4];
+                    uint32_t pid[4];
+#pragma unroll
+                    for (int e = 0; e < 4; ++e) {
+                        pu[e] = __shfl_xor_sync(0xffffffffu, u[ri][e], o);
+                        pid[e] = __shfl_xor_sync(0xffffffffu, id[ri][e], o);
+                    }
+                    maxlo[ri] = fmaxf(maxlo[ri], __shfl_xor_sync(0xffffffffu, maxlo[ri], o));
+#pragma unroll
+                    for (int f = 0; f < 4; ++f) {
+                        if (pu[f] > u[ri][3] || (pu[f] == u[ri][3] && pid[f] < id[ri][3])) {
+                            u[ri][3] = pu[f]; id[ri][3] = pid[f];
+#pragma unroll
+                            for (int e = 3; e > 0; --e)
+                                if (u[ri][e] > u[ri][e - 1] || (u[ri][e] == u[ri][e - 1] && id[ri][e] < id[ri][e - 1])) {
+                                    const float t = u[ri][e - 1]; u[ri][e - 1] = u[ri][e]; u[ri][e] = t;
+                                    const uint32_t ti = id[ri][e - 1]; id[ri][e - 1] = id[ri][e]; id[ri][e] = ti;
+                                }
+                        }
+                    }
+                }
+                const uint32_t row = tile * ROWS + rbase + 64 * (ri >> 1) + 8 * (ri & 1);
+                if ((lane & 3) != 0 || row >= p.n) continue;
+                const float u1 = u[ri][1], u2 = u[ri][2], u3 = u[ri][3], ml = maxlo[ri], xx = x2[ri];
+                const uint32_t i0 = id[ri][0], i1 = id[ri][1], i2 = id[ri][2];
+                const bool decided = i0 != NONE && !(u1 >= ml) && xx > 0.0f && xx < INFINITY;
                 if (decided) {
                     p.assign[row] = i0;
                 } else {
@@ -205,10 +213,10 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                     const uint32_t pos = atomicAdd(p.amb_count, 1u);
                     if (pos < p.amb_cap) {
                         p.amb_rows[pos] = row;
-                        const bool all = i0 == NONE || u3 >= maxlo || !(x2 > 0.0f) || !(x2 < INFINITY);
+                        const bool all = i0 == NONE || u3 >= ml || !(xx > 0.0f) || !(xx < INFINITY);
                         p.amb_cand[4 * pos + 0] = all ? ALL : i0;
                         p.amb_cand[4 * pos + 1] = all ? NONE : i1;
-                        p.amb_cand[4 * pos + 2] = (all || !(u2 >= maxlo)) ? NONE : i2;
+                        p.amb_cand[4 * pos + 2] = (all || !(u2 >= ml)) ? NONE : i2;
                         p.amb_cand[4 * pos + 3] = NONE;
                     }
                     p.assign[row] = i0 == NONE ? 0u : i0;  // overwritten by the fix-up
@@ -216,9 +224,6 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
             }
         }
     }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) ptx::tmem_dealloc(tmem, TMEM_COLS);
 }
 
 // Exact fp32 decision for the listed rows: one warp per row, candidates in ascending centroid order, strict comparison
@@ -279,7 +284,7 @@ __global__ void assign_fixup_kernel(const float *rows, uint32_t dim, const float
 bool assign_tensor_supported(const DeviceInfo &di, uint32_t dim, uint32_t K, int metric) {
     if (const char *e = getenv("NK_ASSIGN_TENSOR"))
         if (atoi(e) == 0) return false;
-    return di.cc >= 100 && dim % 4 == 0 && dim >= 32 && dim <= 32768 && K >= 1 && (metric == NK_METRIC_COSINE || metric == NK_METRIC_EUCLIDEAN);
+    return di.cc >= 90 && dim % 4 == 0 && dim >= 32 && dim <= 32768 && K >= 1 && (metric == NK_METRIC_COSINE || metric == NK_METRIC_EUCLIDEAN);
 }
 
 // rows / shadow / norms: one shard (device pointers); centroids_dev: [K x dim] fp32 on the same device; assign_dev: [n].

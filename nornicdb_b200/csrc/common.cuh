@@ -1,4 +1,4 @@
-// common.cuh — shared device/host utilities of libnornic_knn (sm_100a only).
+// common.cuh — shared device/host utilities of libnornic_knn (sm_90a only).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_bf16.h>

@@ -301,12 +301,10 @@ static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uin
     a.queries = q_dev; a.Q = Q; a.k = k; a.metric = ix->metric; a.stream = stream;
     a.row_mask = s.mask_on ? s.mask : nullptr;
     a.out_idx = xo.out_idx; a.out_score = xo.out_score; a.min_score = ix->key_floor(); a.defer_tail = xo.defer_tail;
-    // AUTO (measured on B200, N=10M d=1024, ms per batch).  fp32 rows: CUDA-core scan 5.9 / 6.2 / 6.1 / 7.6 at Q = 1 / 2 /
-    // 4 / 8, TF32 tensor filter 5.8 for any Q <= 64 -> CUDA cores keep Q <= 4, tensor cores from 5 queries on.  With a
-    // BF16 shadow the filter streams half the bytes: 2.9-3.1 ms for any Q <= 128, so it serves every batch size once the
-    // shard is large enough for bytes (not launches) to matter; small shards keep the single-kernel CUDA-core scan at
-    // Q <= 4 (N=100k d=128: 86 us vs 89 us).  16-bit shards: the 16-bit tensor pass from 5 queries on (the CUDA-core scan
-    // already streams the minimum bytes at Q <= 4).
+    // AUTO: CUDA cores keep Q <= 4 (the single-kernel scan already streams the fewest bytes), tensor cores from 5 queries
+    // on.  With a BF16 shadow the filter streams half the bytes of the fp32 rows, so it serves every batch size once the
+    // shard is large enough for bytes (not launches) to matter; small shards keep the CUDA-core scan at Q <= 4.  16-bit
+    // shards: the 16-bit tensor pass from 5 queries on.
     nk::ScanArgs as = a;  // with the 16-bit image attached (if the shard has an up-to-date one)
     if (s.xnorm2 && s.shadow_n == s.n) {
         if (ix->dtype == NK_DTYPE_F32) {
@@ -400,7 +398,7 @@ static int finish_deferred(NkIndex *ix, NkShard &s) {
 extern "C" {
 
 const char *nk_last_error(void) { return nk::get_error(); }
-const char *nk_version(void) { return "nornic-knn-b200 0.1 (sm_100a)"; }
+const char *nk_version(void) { return "nornic-knn-b200 0.1 (sm_90a)"; }
 
 NkIndex *nk_index_create(const int *device_ids, int n_devices, uint32_t dim, int dtype, int metric) {
     nk::DeviceGuard _restore_device;

@@ -6,7 +6,7 @@ namespace nk {
 
 struct DeviceInfo {
     int device_id = 0;
-    int num_sms = 148;
+    int num_sms = 132;
     size_t max_smem_optin = 0;
     int cc = 0;
 };

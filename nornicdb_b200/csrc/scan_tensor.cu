@@ -1,13 +1,13 @@
-// scan_tensor.cu — fused distance + top-k scan over the FP32 rows on the 5th-gen tensor cores (tcgen05 + TMEM + TMA):
+// scan_tensor.cu — fused distance + top-k scan over the FP32 rows on the tensor cores (wgmma + TMA + mbarrier):
 // the path of shards without a BF16 shadow, the retry stage of the shadow filter (scan_tensor_shadow.cu), the exact
 // 3xTF32 scan, plus the finish step and the host logic both filters share.
 //
 // For Q > ~16 queries the CUDA-core scan stops being HBM-bound (fp32 FMA ridge ~10 flop/byte, the batch needs
-// Q/2 flop/byte), so the Q x N^T contraction moves to tcgen05.mma.  fp32 inputs on tensor cores mean TF32
+// Q/2 flop/byte), so the Q x N^T contraction moves to wgmma.  fp32 inputs on tensor cores mean TF32
 // (10-bit mantissa), which by itself cannot meet "identical index sets, 1e-4".  Two modes (template NT):
 //
 //   NT = 3  "exact":  3xTF32 split  x*q ~= xl*qh + xh*ql + xh*qh  (xh = rn_tf32(x), xl = x - xh exactly),
-//           fp32 accumulation in TMEM, ~2^-21 relative per product.  Per-CTA exact top-k lists.
+//           fp32 accumulation, ~2^-21 relative per product.  Per-CTA exact top-k lists.
 //   NT = 1  "filter": ONE TF32 product per element (a third of the tensor work and energy — the chip is
 //           power-capped when HBM and the tensor pipes both run flat out) with a RIGOROUS error margin:
 //           |s_hat - s| <= c*|x|*|q|, c = 2^-10 + d*2^-22  (rounding of both operands + fp32 accumulation), so
@@ -17,19 +17,15 @@
 //           is raised ON DEVICE and the NT=3 kernels — enqueued behind, early-exiting when the flag is clear —
 //           redo the search exactly.  No host round trip.
 //
-// One persistent CTA per SM, warp-specialised (16 warps):
-//   warp 0      TMA producer: corpus K-slabs [256 rows x 32 floats] (128B-swizzled), ring released by the split
-//               warps as soon as the slab is in registers (EVICT_FIRST);
-//   warp 3      TMA producer: query slabs (pre-rounded hi [+ lo], [64 x 32 floats] each, L2-resident, EVICT_LAST);
-//   warps 4-11  "split" warps, one thread per corpus row: conflict-free swizzled LDS.128, xh (and xl) with packed
-//               FADD2/FFMA2, |x|^2 on the side (no separate norm pass), tcgen05.st into a TMEM ring: the corpus is
-//               the MMA's A operand FROM TENSOR MEMORY (smem-operand MMAs of this shape are 1.5x slower, see
-//               profiles/experiments/mma_rate.cu);
-//   warps 1,2   MMA issuers, one per 128-row M-tile (tcgen05.mma.kind::tf32 M=128 N=64 K=8, accumulators in TMEM);
-//               two issuers because one warp's per-slab poll/fence/commit overhead lets the shallow MMA queue drain;
-//   warps 12-15 epilogue: tcgen05.ld the [128 rows x 64 queries] accumulator (thread = corpus row), release it,
-//               scale / bound, compare against each query's running threshold with a compact mask pass, append the
-//               few survivors; warp-level register top-k prune.  Distances never go to memory.
+// One persistent CTA per SM, warp-specialised (12 warps):
+//   warp 0      TMA producer: corpus K-slabs [256 rows x 32 floats] (128B-swizzled), ring released once the MMAs that
+//               read the slab have completed (EVICT_FIRST);
+//   warp 3      TMA producer: query slabs (pre-rounded hi [+ lo], [QT x 32 floats] each, L2-resident, EVICT_LAST);
+//   warps 4-11  two consumer warpgroups, one per 128-row M-tile.  Per slab: split (thread = corpus row: swizzled LDS.128,
+//               xh rounded in place, xl into a per-warpgroup tile, |x|^2 on the side), then wgmma.m64nQTk8.tf32 with A
+//               and B from shared memory, fp32 accumulators in registers.  Per tile: scale / bound straight from the
+//               accumulator registers, compare against each query's running threshold with a compact mask pass,
+//               append the few survivors; warp-level register top-k prune.  Distances never go to memory.
 // Exact mode: per-CTA lists are folded by merge_keys().  Filter mode: CTAs share their thresholds through a per-query
 // atomic max, append their survivors to one list per query, and filter_finish_kernel (below) selects, re-scores and
 // sorts.  Large batches: 2 / 4 query groups per launch share every corpus tile through L2 (Params::qgroups).
@@ -44,7 +40,7 @@
 #include <string>
 
 #include "kernels.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 #include "scan_tensor_shared.cuh"
 
 namespace nk {
@@ -54,31 +50,25 @@ constexpr int ROWS = 256;        // corpus rows per tile (2 M-tiles of 128)
 constexpr int QT_MAX = 128;      // queries per launch (MMA N): 64, or 128 for large batches (filter mode)
 constexpr int ASTAGES = 4;       // corpus-slab smem ring
 constexpr int A_BYTES = ROWS * BK * 4;   // 32 KB
-constexpr int ACC_COL = 0;       // [mtile] x QT columns (single-buffered, drained per M-tile); the A ring follows
-constexpr int SPLIT_WARP0 = 4, EPI_WARP0 = 12;
-constexpr int MAX_BSTAGES = 8, MAX_TSTAGES = 6;
-constexpr int XX_RING = 8;       // >= MAX_TSTAGES / 1 slab-per-tile + 2
+constexpr int EPI_WARP0 = 4;     // consumer warpgroups: warps 4-7 (rows 0-127), 8-11 (rows 128-255)
+constexpr int MAX_BSTAGES = 8;
 
 template <int NT, int QT> struct Cfg {
     static constexpr int PARTS = NT == 3 ? 2 : 1;          // hi (+ lo)
     static constexpr int B_BYTES = QT * BK * 4;            // one part of one query slab (8 / 16 KB)
     static constexpr int BST_BYTES = PARTS * B_BYTES;
-    static constexpr int BSTAGES = (80 * 1024) / BST_BYTES > MAX_BSTAGES ? MAX_BSTAGES : (80 * 1024) / BST_BYTES;
-    static constexpr int A_COL = 2 * QT;                   // TMEM: accumulators [2][QT], then the A-operand ring
-    static constexpr int TSTAGES = (TMEM_COLS - A_COL) / (2 * PARTS * BK);  // 3 / 6 (QT=64), 4 (QT=128 filter)
-    static constexpr int RING_BYTES = ASTAGES * A_BYTES + BSTAGES * BST_BYTES;
-    static_assert(BSTAGES >= 2 && TSTAGES >= 2 && TSTAGES <= MAX_TSTAGES, "ring too shallow");
+    static constexpr int B_BUDGET = NT == 3 ? 48 * 1024 : 80 * 1024;  // exact mode also holds the xl tiles (32 KB)
+    static constexpr int BSTAGES = B_BUDGET / BST_BYTES > MAX_BSTAGES ? MAX_BSTAGES : B_BUDGET / BST_BYTES;
+    static constexpr int XL_BYTES = NT == 3 ? A_BYTES : 0;    // xl = x - xh of the current slab, one 16 KB tile per warpgroup
+    static constexpr int RING_BYTES = ASTAGES * A_BYTES + BSTAGES * BST_BYTES + XL_BYTES;
+    static_assert(BSTAGES >= 2, "ring too shallow");
 };
 
 struct __align__(8) Shared {
-    uint64_t afull_s[ASTAGES], aempty_s[ASTAGES];    // corpus slab in smem: TMA -> split warps -> TMA
-    uint64_t bfull[MAX_BSTAGES], bempty[MAX_BSTAGES];  // query slabs in smem: TMA -> MMA -> TMA
-    uint64_t afull[MAX_TSTAGES][2], aempty[MAX_TSTAGES][2];  // A operand in TMEM, per (stage, M-tile)
-    uint64_t accfull[2], accempty[2];                // accumulators, per M-tile
-    uint32_t tmem_base;
+    uint64_t afull_s[ASTAGES], aempty_s[ASTAGES];    // corpus slab in smem: TMA -> consumers -> TMA
+    uint64_t bfull[MAX_BSTAGES], bempty[MAX_BSTAGES];  // query slabs in smem: TMA -> consumers -> TMA
     unsigned int maxxx;       // running max of |x|^2 (float bits) over the rows this CTA has scored
-    float xx[XX_RING][ROWS];  // |x|^2 per row, ring over tiles: the split warps run up to TSTAGES slabs (several tiles when
-                              // dim is small) ahead of the MMA, which runs one tile ahead of the epilogue
+    float xx[ROWS];           // |x|^2 per row of the current tile (split step -> epilogue, same warpgroup)
     float tau[QT_MAX];
     float qn[QT_MAX];
     int cnt[QT_MAX];
@@ -345,7 +335,7 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
     using namespace tc;
     using C = Cfg<NT, QT>;
     constexpr bool FILTER = NT == 1;
-    constexpr int A_COL = C::A_COL, B_BYTES = C::B_BYTES;
+    constexpr int B_BYTES = C::B_BYTES;
     pdl_trigger();
     pdl_wait();
     if (p.only_if && *p.only_if == 0) return;  // exact fallback not needed (uniform over the grid)
@@ -353,7 +343,7 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
     extern __shared__ unsigned char smem_dyn[];
     // 128-byte-swizzled tiles need 1024-byte alignment: align by hand (the launch reserves the slack).
     unsigned char *smem_raw = smem_dyn + ((1024u - (ptx::smem_u32(smem_dyn) & 1023u)) & 1023u);
-    // layout: [ASTAGES x A 32K] [BSTAGES x (Bhi 8K [| Blo 8K])] [Shared]
+    // layout: [ASTAGES x A 32K] [BSTAGES x (Bhi [| Blo])] [xl 2 x 16K (exact mode)] [Shared]
     unsigned char *a_base = smem_raw;
     unsigned char *b_base = smem_raw + (size_t)ASTAGES * A_BYTES;
     Shared &sh = *reinterpret_cast<Shared *>(smem_raw + (size_t)C::RING_BYTES);
@@ -361,7 +351,7 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t num_tiles = (p.n + ROWS - 1) / ROWS;
     // Query groups: CTA b serves query block (b % G) over the tile subset (b / G).  The G sibling CTAs stream the SAME
-    // corpus tiles at the same pace, so a tile crosses HBM once and its other G-1 readers hit the 126 MB L2: large
+    // corpus tiles at the same pace, so a tile crosses HBM once and its other G-1 readers hit the 50 MB L2: large
     // batches (Q > 128) stop being bound by re-reading the corpus once per 128 queries.
     const uint32_t grp = blockIdx.x % p.qgroups, sub = blockIdx.x / p.qgroups, sgrid = gridDim.x / p.qgroups;
     const uint32_t q0 = p.q0 + grp * QT, qpad_off = p.qpad_off + grp * QT;
@@ -375,15 +365,12 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
         ptx::prefetch_tensormap(&map_rows);
         ptx::prefetch_tensormap(&map_qhi);
         if (NT == 3) ptx::prefetch_tensormap(&map_qlo);
+        // a stage is free again once every consumer warp has seen its MMAs complete
         for (int i = 0; i < ASTAGES; ++i) { ptx::mbar_init(&sh.afull_s[i], 1); ptx::mbar_init(&sh.aempty_s[i], 8); }
-        for (int i = 0; i < C::BSTAGES; ++i) { ptx::mbar_init(&sh.bfull[i], 1); ptx::mbar_init(&sh.bempty[i], 2); }
-        for (int i = 0; i < C::TSTAGES; ++i)
-            for (int m = 0; m < 2; ++m) { ptx::mbar_init(&sh.afull[i][m], 4); ptx::mbar_init(&sh.aempty[i][m], 1); }
-        for (int i = 0; i < 2; ++i) { ptx::mbar_init(&sh.accfull[i], 1); ptx::mbar_init(&sh.accempty[i], 4); }
+        for (int i = 0; i < C::BSTAGES; ++i) { ptx::mbar_init(&sh.bfull[i], 1); ptx::mbar_init(&sh.bempty[i], 8); }
         sh.maxxx = 0u;
         ptx::fence_barrier_init();
     }
-    if (warp == 2) ptx::tmem_alloc(&sh.tmem_base, TMEM_COLS);
     if (tid < QT) {
         // start threshold: the caller's score floor and, when the prep kernel sampled the shard, a lower bound of the
         // query's k-th best score (no flood tiles then)
@@ -396,10 +383,7 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
         sh.cnt[tid] = 0;
         sh.qn[tid] = (FILTER && p.qnorm) ? p.qnorm[qpad_off + tid] : 1.0f;
     }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem = sh.tmem_base;
     const bool flood = !(FILTER && p.presampled);  // first two tiles: every (row, query) pair is placed directly
 
     if (warp == 0) {
@@ -434,233 +418,185 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
             }
         }
         if (prof && lane == 0) { g_tc_prof[2] = acc_a; }
-    } else if (warp == 1 || warp == 2) {
-        // ===================================== MMA issuers (one warp per M-tile) ==================
-        const uint32_t m = warp - 1;
-        const uint32_t idesc = ptx::make_idesc_tf32(128, QT);
-        const uint32_t d = tmem + ACC_COL + m * QT;
-        uint32_t g = 0, it = 0;
-        for (uint32_t tile = sub; tile < num_tiles; tile += sgrid, ++it) {
-            for (uint32_t j = 0; j < p.nslab; ++j, ++g) {
-                const uint32_t s = g % C::BSTAGES, ts = g % C::TSTAGES;
-                if (j == 0) { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.accempty[m], (it & 1) ^ 1); TC_PROF_END(b); }  // epilogue drained
-                { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.bfull[s], (g / C::BSTAGES) & 1); TC_PROF_END(a); }  // query slabs landed
-                { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.afull[ts][m], (g / C::TSTAGES) & 1); TC_PROF_END(c); }  // A operand in TMEM
-                ptx::tc_fence_after();
-                if (ptx::elect_one_sync()) {
-                    const uint32_t bhi = ptx::smem_u32(b_base + (size_t)s * C::BST_BYTES);
-                    const uint64_t dhi = ptx::make_smem_desc_sw128(bhi);
-                    const uint32_t ahi = tmem + A_COL + (ts * 2 + m) * C::PARTS * BK;
-                    // K advance per MMA = 8 floats = 32 B = 2 descriptor units = 8 TMEM columns
-                    if (NT == 3) {
-                        const uint64_t dlo = ptx::make_smem_desc_sw128(bhi + B_BYTES);
-                        const uint32_t alo = ahi + BK;
-#pragma unroll
-                        for (uint32_t kk = 0; kk < BK / 8; ++kk) {  // smallest terms first
-                            ptx::mma_tf32_ts(d, alo + kk * 8, dhi + kk * 2, idesc, (j | kk) != 0);
-                            ptx::mma_tf32_ts(d, ahi + kk * 8, dlo + kk * 2, idesc, 1);
-                            ptx::mma_tf32_ts(d, ahi + kk * 8, dhi + kk * 2, idesc, 1);
-                        }
-                    } else {
-#pragma unroll
-                        for (uint32_t kk = 0; kk < BK / 8; ++kk) ptx::mma_tf32_ts(d, ahi + kk * 8, dhi + kk * 2, idesc, (j | kk) != 0);
-                    }
-                    ptx::tc_commit(&sh.aempty[ts][m]);                        // TMEM A slot of this M-tile reusable
-                    ptx::tc_commit(&sh.bempty[s]);                            // query slabs: both issuers must be done
-                    if (j + 1 == p.nslab) ptx::tc_commit(&sh.accfull[m]);     // accumulator of this M-tile complete
-                }
-                __syncwarp();
-            }
-        }
-        if (prof && lane == 0 && warp == 1) { g_tc_prof[4] = acc_a; g_tc_prof[5] = acc_b; g_tc_prof[6] = acc_c; g_tc_prof[7] = clock64() - t_start; }
-    } else if (warp >= SPLIT_WARP0 && warp < SPLIT_WARP0 + 8) {
-        // ===================================== split warps ======================================
-        const uint32_t m = (warp - SPLIT_WARP0) >> 2, quad = warp & 3;
-        const uint32_t r = m * 128 + quad * 32 + lane;  // row within the tile
-        const uint32_t lane_base = (quad * 32u) << 16;
-        uint32_t g = 0, it = 0;
-        for (uint32_t tile = sub; tile < num_tiles; tile += sgrid, ++it) {
-            uint64_t xx2 = 0;  // two partial sums of |x|^2 (packed f32x2)
-            for (uint32_t j = 0; j < p.nslab; ++j, ++g) {
-                const uint32_t s = g % ASTAGES, ts = g % C::TSTAGES;
-                { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.afull_s[s], (g / ASTAGES) & 1); TC_PROF_END(a); }
-                long long _tw = prof ? clock64() : 0;
-                const unsigned char *rowp = a_base + (size_t)s * A_BYTES + (size_t)r * 128;
-                uint32_t hi[32], lo[32];
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    // 128B swizzle: logical 16-byte chunk c of row r sits at chunk c ^ (r & 7)
-                    const uint4 v = *reinterpret_cast<const uint4 *>(rowp + ((c ^ (r & 7)) << 4));
-                    const uint32_t e[4] = {v.x, v.y, v.z, v.w};
-#pragma unroll
-                    for (int u = 0; u < 4; u += 2) {
-                        const uint32_t h0 = ptx::tf32_round_bits(e[u]), h1 = ptx::tf32_round_bits(e[u + 1]);
-                        const uint64_t x2 = ptx::pack2(e[u], e[u + 1]);
-                        xx2 = ptx::fma_f32x2(x2, x2, xx2);  // |x|^2 on the side
-                        hi[c * 4 + u] = h0; hi[c * 4 + u + 1] = h1;
-                        if (NT == 3) {
-                            const uint64_t l2 = ptx::sub_f32x2(x2, ptx::pack2(h0, h1));  // exact residual x - xh
-                            lo[c * 4 + u] = (uint32_t)l2; lo[c * 4 + u + 1] = (uint32_t)(l2 >> 32);
-                        }
-                    }
-                }
-                // the slab now lives in registers: hand the smem slot straight back to the TMA producer
-                __syncwarp();
-                if (lane == 0) ptx::mbar_arrive(&sh.aempty_s[s]);
-                if (prof) acc_c += clock64() - _tw;
-                { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.aempty[ts][m], ((g / C::TSTAGES) & 1) ^ 1); TC_PROF_END(b); }
-                _tw = prof ? clock64() : 0;
-                ptx::tc_fence_after();
-                const uint32_t acol = tmem + lane_base + A_COL + (ts * 2 + m) * C::PARTS * BK;
-                ptx::tmem_st_32x32b_x32(acol, hi);
-                if (NT == 3) ptx::tmem_st_32x32b_x32(acol + BK, lo);
-                ptx::tmem_wait_st();
-                if (j + 1 == p.nslab)  // published by the afull arrive below
-                    sh.xx[it % XX_RING][r] = __uint_as_float((uint32_t)xx2) + __uint_as_float((uint32_t)(xx2 >> 32));
-                ptx::tc_fence_before();
-                __syncwarp();
-                if (lane == 0) ptx::mbar_arrive(&sh.afull[ts][m]);
-                if (prof) acc_d += clock64() - _tw;
-            }
-        }
-        if (prof && lane == 0 && warp == SPLIT_WARP0) { g_tc_prof[8] = acc_a; g_tc_prof[9] = acc_b; g_tc_prof[10] = acc_c; g_tc_prof[11] = acc_d; g_tc_prof[12] = clock64() - t_start; }
-        if (prof && lane == 0 && warp == SPLIT_WARP0 + 4) { g_tc_prof[13] = acc_a; g_tc_prof[14] = acc_b; g_tc_prof[15] = acc_c; g_tc_prof[16] = acc_d; }
     } else if (warp >= EPI_WARP0) {
-        // ===================================== epilogue =========================================
-        const uint32_t quad = warp & 3;
-        const uint32_t lane_base = (quad * 32u) << 16;
+        // ===================================== consumers: split + MMA + epilogue ===================
+        // warpgroup m owns rows [128 m, 128 m + 128) of the tile.  Split step: thread t rounds row 128 m + t of the slab.
+        // MMA / epilogue: two m64 halves h; thread = 4 rows x QT/4 columns of the accumulator fragments: rows
+        // rbase + 64 h + 8 r, columns cbase + 8 (j / 2) + j % 2.
+        const uint32_t ewarp = warp - EPI_WARP0, m = ewarp >> 2, wq = ewarp & 3;
+        const uint32_t srow = m * 128 + ((uint32_t)tid & 127u);  // split row
+        const uint32_t rbase = m * 128 + wq * 16 + ((uint32_t)lane >> 2), cbase = 2u * ((uint32_t)lane & 3u);
+        unsigned char *xl_base = smem_raw + (size_t)ASTAGES * A_BYTES + (size_t)C::BSTAGES * C::BST_BYTES + (size_t)m * (A_BYTES / 2);
         uint64_t *my_cand = p.cand + (size_t)blockIdx.x * QT * P;
         const int prune_at = P - ROWS;
         const bool cosine = p.metric == NK_METRIC_COSINE, euclid = p.metric == NK_METRIC_EUCLIDEAN;
         const float bfac = p.margin_c * (euclid ? 2.0f : 1.0f);  // bound on -dist^2 = -(|x|^2+|q|^2-2x.q) is 2c|x||q|
-        uint32_t it = 0;
+        float acc[2][QT / 2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < QT / 2; ++i) acc[h][i] = 0.0f;
+        uint32_t g = 0, it = 0;
         for (uint32_t tile = sub; tile < num_tiles; tile += sgrid, ++it) {
-#pragma unroll 1
-            for (uint32_t m = 0; m < 2; ++m) {
-                const uint32_t rt = m * 128 + quad * 32 + lane;
+            float xe = 0.0f, xo = 0.0f;  // |x|^2 of the split row: partial sums over even / odd elements
+            for (uint32_t j = 0; j < p.nslab; ++j, ++g) {
+                const uint32_t s = g % ASTAGES, sb = g % C::BSTAGES;
+                { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.afull_s[s], (g / ASTAGES) & 1); TC_PROF_END(a); }
+                if (NT == 3 && j > 0) group_sync(2 + m, 128);  // the previous slab's MMAs no longer read the xl tile
+                // split: xh = rn_tf32(x) in place (the MMA's A operand), xl = x - xh (exact) into this warpgroup's xl tile,
+                // |x|^2 on the side
+                unsigned char *rowp = a_base + (size_t)s * A_BYTES + (size_t)srow * 128;
+#pragma unroll
+                for (int c = 0; c < 8; ++c) {
+                    // 128B swizzle: logical 16-byte chunk c of row r sits at chunk c ^ (r & 7)
+                    const uint32_t off = (uint32_t)(c ^ (int)(srow & 7)) << 4;
+                    const uint4 v = *reinterpret_cast<const uint4 *>(rowp + off);
+                    const uint32_t e[4] = {v.x, v.y, v.z, v.w};
+                    uint32_t hi[4], lo[4];
+#pragma unroll
+                    for (int u = 0; u < 4; ++u) {
+                        const float x = __uint_as_float(e[u]);
+                        if (u & 1) xo = fmaf(x, x, xo); else xe = fmaf(x, x, xe);
+                        hi[u] = ptx::tf32_round_bits(e[u]);
+                        lo[u] = __float_as_uint(x - __uint_as_float(hi[u]));
+                    }
+                    *reinterpret_cast<uint4 *>(rowp + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+                    if (NT == 3) *reinterpret_cast<uint4 *>(xl_base + (size_t)(srow - m * 128) * 128 + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
+                }
+                if (j + 1 == p.nslab) sh.xx[srow] = xe + xo;
+                ptx::fence_proxy_async_smem();
+                group_sync(2 + m, 128);  // every row of this warpgroup's half of the slab is rounded
+                { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.bfull[sb], (g / C::BSTAGES) & 1); TC_PROF_END(b); }
+                const uint32_t bhi = ptx::smem_u32(b_base + (size_t)sb * C::BST_BYTES);
+                const uint64_t dhi = ptx::make_smem_desc_sw128(bhi), dlo = ptx::make_smem_desc_sw128(bhi + B_BYTES);
+                const uint32_t ahi = ptx::smem_u32(a_base + (size_t)s * A_BYTES + (size_t)m * (A_BYTES / 2)), alo = ptx::smem_u32(xl_base);
+                ptx::wgmma_fence();
+                // K advance per MMA = 8 floats = 32 B = 2 descriptor units; M-half h = 64 rows = 8 KB
+#pragma unroll
+                for (uint32_t kk = 0; kk < BK / 8; ++kk) {
+#pragma unroll
+                    for (uint32_t h = 0; h < 2; ++h) {
+                        const uint64_t dah = ptx::make_smem_desc_sw128(ahi + h * (A_BYTES / 4)) + kk * 2;
+                        if (NT == 3) {  // smallest terms first
+                            const uint64_t dal = ptx::make_smem_desc_sw128(alo + h * (A_BYTES / 4)) + kk * 2;
+                            ptx::wgmma_tf32<QT>(acc[h], dal, dhi + kk * 2, (j | kk) != 0);
+                            ptx::wgmma_tf32<QT>(acc[h], dah, dlo + kk * 2, 1);
+                            ptx::wgmma_tf32<QT>(acc[h], dah, dhi + kk * 2, 1);
+                        } else {
+                            ptx::wgmma_tf32<QT>(acc[h], dah, dhi + kk * 2, (j | kk) != 0);
+                        }
+                    }
+                }
+                ptx::wgmma_commit();
+                ptx::wgmma_wait_all();
+                ptx::fence_acc(acc[0]);
+                ptx::fence_acc(acc[1]);
+                __syncwarp();
+                if (lane == 0) { ptx::mbar_arrive(&sh.aempty_s[s]); ptx::mbar_arrive(&sh.bempty[sb]); }
+            }
+            if (flood && it < 2 && ewarp == 0 && lane == 0)
+                for (uint32_t qi = 0; qi < nq; ++qi) sh.cnt[qi] = (int)((it + 1) * ROWS);
+#pragma unroll
+            for (uint32_t ri = 0; ri < 4; ++ri) {
+                const uint32_t h = ri >> 1, r = ri & 1;
+                const uint32_t rt = rbase + 64 * h + 8 * r;  // row within the tile
                 const uint32_t row = tile * ROWS + rt;
                 const bool alive = row < p.n && (!p.mask || ((__ldg(p.mask + (row >> 5)) >> (row & 31)) & 1u));
-                { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.accfull[m], it & 1); TC_PROF_END(a); }
-                ptx::tc_fence_after();
                 // score(row, query c):
                 //   cosine     acc / |x|  (queries pre-normalised)       filter bound c
                 //   dot        acc                                        filter bound c |x| |q|
                 //   euclidean  -(|x|^2 + |q|^2 - 2 acc)   (filter only)   filter bound 2c |x| |q|
                 // filter mode buffers the UPPER bound score + bound.
-                const float x2 = sh.xx[it % XX_RING][rt];
+                const float x2 = sh.xx[rt];
                 const float xn = sqrtf(x2);
                 float mul = 1.0f, bnd = 0.0f;
                 if (cosine) mul = x2 > 0.0f ? 1.0f / xn : 0.0f;
                 if (FILTER) {
                     bnd = cosine ? p.margin_c : bfac * xn;
-                    if (!cosine && alive && x2 < INFINITY) atomicMax(&sh.maxxx, __float_as_uint(x2));  // NaN / Inf rows: kept, judged exactly
+                    if (!cosine && alive && x2 < INFINITY && (lane & 3) == 0) atomicMax(&sh.maxxx, __float_as_uint(x2));  // NaN / Inf rows: kept, judged exactly
                     if (euclid) mul = 2.0f;
                 }
-#pragma unroll 1
-                for (uint32_t half = 0; half < QT / 64; ++half) {
-                    // drain 64 accumulator columns into registers; after the last half hand the accumulator back,
-                    // then score from registers
-                    const uint32_t cb = half * 64;
-                    uint32_t v0[32], v1[32];
-                    ptx::tmem_ld_32x32b_x32(tmem + lane_base + ACC_COL + m * QT + cb, v0);
-                    ptx::tmem_ld_32x32b_x32(tmem + lane_base + ACC_COL + m * QT + cb + 32, v1);
-                    ptx::tmem_wait_ld();
-                    if (half + 1 == QT / 64) {
-                        ptx::tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) ptx::mbar_arrive(&sh.accempty[m]);
+                float v[QT / 4];
+#pragma unroll
+                for (int jj = 0; jj < QT / 4; ++jj) v[jj] = acc[h][(jj >> 1) * 4 + r * 2 + (jj & 1)];
+                if (DUMP && FILTER && row < p.n) {  // tests only: score estimate and error bound per (row, query)
+#pragma unroll
+                    for (int jj = 0; jj < QT / 4; ++jj) {
+                        const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
+                        if (qi >= nq) continue;
+                        const float qn = sh.qn[qi];
+                        float est = v[jj] * mul, b = bnd * qn;
+                        if (euclid) { est -= fmaf(qn, qn, x2); b += EUC_EPS * fmaf(qn, qn, x2); }
+                        p.dump_est[(size_t)row * p.dump_ld + q0 + qi] = est;
+                        p.dump_bnd[(size_t)row * p.dump_ld + q0 + qi] = b;
                     }
-                    if (DUMP && FILTER && row < p.n) {  // tests only: score estimate and error bound per (row, query)
-                        for (uint32_t c = 0; c < 64 && cb + c < nq; ++c) {
-                            uint32_t bits = 0;
+                }
+                if (flood && it < 2) {
+                    // Flood tiles: until the first prune (after this CTA's second tile) every threshold is -inf and
+                    // EVERY (row, query) pair is buffered.  Place them directly - slot = tile-local row, no atomics.
+                    const uint32_t slot = it * ROWS + rt;
+                    const uint32_t grow = (uint32_t)(p.row_base + row);
 #pragma unroll
-                            for (uint32_t i = 0; i < 32; ++i) {
-                                if (c == i) bits = v0[i];
-                                if (c == 32 + i) bits = v1[i];
-                            }
-                            const float qn = sh.qn[cb + c];
-                            float est = __uint_as_float(bits) * mul, b = bnd * qn;
-                            if (euclid) { est -= fmaf(qn, qn, x2); b += EUC_EPS * fmaf(qn, qn, x2); }
-                            p.dump_est[(size_t)row * p.dump_ld + q0 + cb + c] = est;
-                            p.dump_bnd[(size_t)row * p.dump_ld + q0 + cb + c] = b;
-                        }
-                    }
-                    if (flood && it < 2 && cb < nq) {
-                        // Flood tiles: until the first prune (after this CTA's second tile) every threshold is -inf and
-                        // EVERY (row, query) pair is buffered.  Place them directly - slot = tile-local row, no atomics,
-                        // no register select - instead of 256 x QT trips through the rare-push loop (~60 us per launch).
-                        const uint32_t slot = it * ROWS + rt;
-                        const uint32_t grow = (uint32_t)(p.row_base + row);
-#pragma unroll
-                        for (uint32_t c = 0; c < 64; ++c) {
-                            const uint32_t qi = cb + c;
-                            if (qi < nq) {
-                                float sc = __uint_as_float(c < 32 ? v0[c & 31] : v1[c & 31]) * mul;
-                                if (FILTER) {
-                                    const float qn = sh.qn[qi];
-                                    if (euclid) sc -= EUC_KEEP * fmaf(qn, qn, x2);
-                                    sc = fmaf(bnd, qn, sc);
-                                    if (sc != sc) sc = INFINITY;
-                                } else if (sc != sc) {
-                                    sc = -INFINITY;
-                                }
-                                my_cand[(size_t)qi * P + slot] = (alive && sc >= p.min_score) ? make_key(sc, grow) : 0ull;  // 0 = empty slot
-                            }
-                        }
-                        if (rt == 0 && half == 0)
-                            for (uint32_t qi = m == 0 ? 0 : nq; qi < nq; ++qi) sh.cnt[qi] = (int)((it + 1) * ROWS);
-                    } else if (alive && cb < nq) {
-                        // Compact compare pass -> 64-bit mask of columns worth buffering (NaN passes); the rare pushes
-                        // run in a small out-of-line loop so the hot code stays a few hundred instructions (a fully
-                        // unrolled push per column was ~40 KB of SASS: I-cache thrash).
-                        uint32_t pass0 = 0, pass1 = 0;
-#pragma unroll
-                        for (uint32_t c = 0; c < 32; ++c) {
-                            float s0 = __uint_as_float(v0[c]) * mul, s1 = __uint_as_float(v1[c]) * mul;
-                            if (FILTER) {
-                                const float q0n = sh.qn[cb + c], q1n = sh.qn[cb + 32 + c];
-                                if (euclid) { s0 -= EUC_KEEP * fmaf(q0n, q0n, x2); s1 -= EUC_KEEP * fmaf(q1n, q1n, x2); }
-                                s0 = fmaf(bnd, q0n, s0);
-                                s1 = fmaf(bnd, q1n, s1);
-                            }
-                            pass0 |= !(s0 < sh.tau[cb + c]) ? (1u << c) : 0u;
-                            pass1 |= !(s1 < sh.tau[cb + 32 + c]) ? (1u << c) : 0u;
-                        }
-                        uint64_t pass = (uint64_t)pass0 | ((uint64_t)pass1 << 32);
-                        if (nq - cb < 64) pass &= (1ull << (nq - cb)) - 1ull;
-#pragma unroll 1
-                        while (pass) {
-                            const uint32_t c = (uint32_t)__ffsll((long long)pass) - 1u;
-                            pass &= pass - 1ull;
-                            uint32_t bits = 0;
-#pragma unroll
-                            for (uint32_t i = 0; i < 32; ++i) {  // register file is not indexable: select by compare
-                                if (c == i) bits = v0[i];
-                                if (c == 32 + i) bits = v1[i];
-                            }
-                            const uint32_t qi = cb + c;
-                            float sc = __uint_as_float(bits) * mul;
+                    for (int jj = 0; jj < QT / 4; ++jj) {
+                        const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
+                        if (qi < nq) {
+                            float sc = v[jj] * mul;
                             if (FILTER) {
                                 const float qn = sh.qn[qi];
                                 if (euclid) sc -= EUC_KEEP * fmaf(qn, qn, x2);
                                 sc = fmaf(bnd, qn, sc);
-                                if (sc != sc) sc = INFINITY;  // undecidable here: keep it, the exact rescoring judges
+                                if (sc != sc) sc = INFINITY;
                             } else if (sc != sc) {
                                 sc = -INFINITY;
                             }
-                            if (sc >= sh.tau[qi]) {
-                                int pos = atomicAdd(&sh.cnt[qi], 1);
-                                if (pos < P) my_cand[(size_t)qi * P + pos] = make_key(sc, (uint32_t)(p.row_base + row));
-                                else atomicExch(p.flags, 1);
-                            }
+                            my_cand[(size_t)qi * P + slot] = (alive && sc >= p.min_score) ? make_key(sc, grow) : 0ull;  // 0 = empty slot
+                        }
+                    }
+                } else if (alive) {
+                    // Compact compare pass -> mask of columns worth buffering (NaN passes); the rare pushes run in a small
+                    // out-of-line loop so the hot code stays short.
+                    uint32_t pass = 0;
+#pragma unroll
+                    for (int jj = 0; jj < QT / 4; ++jj) {
+                        const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
+                        float s0 = v[jj] * mul;
+                        if (FILTER) {
+                            const float qn = sh.qn[qi];
+                            if (euclid) s0 -= EUC_KEEP * fmaf(qn, qn, x2);
+                            s0 = fmaf(bnd, qn, s0);
+                        }
+                        pass |= (!(s0 < sh.tau[qi]) && qi < nq) ? (1u << jj) : 0u;
+                    }
+#pragma unroll 1
+                    while (pass) {
+                        const uint32_t c = (uint32_t)__ffs((int)pass) - 1u;
+                        pass &= pass - 1u;
+                        float val = 0.0f;
+#pragma unroll
+                        for (uint32_t i = 0; i < (uint32_t)(QT / 4); ++i)  // register file is not indexable: select by compare
+                            if (c == i) val = v[i];
+                        const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
+                        float sc = val * mul;
+                        if (FILTER) {
+                            const float qn = sh.qn[qi];
+                            if (euclid) sc -= EUC_KEEP * fmaf(qn, qn, x2);
+                            sc = fmaf(bnd, qn, sc);
+                            if (sc != sc) sc = INFINITY;  // undecidable here: keep it, the exact rescoring judges
+                        } else if (sc != sc) {
+                            sc = -INFINITY;
+                        }
+                        if (sc >= sh.tau[qi]) {
+                            int pos = atomicAdd(&sh.cnt[qi], 1);
+                            if (pos < P) my_cand[(size_t)qi * P + pos] = make_key(sc, (uint32_t)(p.row_base + row));
+                            else atomicExch(p.flags, 1);
                         }
                     }
                 }
             }
-            // prune any buffer that could overflow during the next tile; the 4 epilogue warps prune different
+            // prune any buffer that could overflow during the next tile; the 8 consumer warps prune different
             // queries concurrently with a register-resident warp selection
             group_sync(EPI_BAR, EPI_THREADS);  // every push of this tile is visible
-            for (uint32_t qi = quad; qi < nq; qi += 4)
+            for (uint32_t qi = ewarp; qi < nq; qi += EPI_THREADS / 32)
                 if (sh.cnt[qi] > prune_at) {
                     const float margin2 = !FILTER ? 0.0f : filter_margin2(p.metric, p.margin_c, __uint_as_float(sh.maxxx), sh.qn[qi]);
                     float floor_tau = p.min_score;
@@ -687,7 +623,7 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
     }
 
     // ---- emit this CTA's list per query: best k (exact) or everything inside the margin (filter).  Every role has
-    // finished its tile loop here, so all 16 warps share the final prunes (4x shorter tail than the epilogue warps alone).
+    // finished its tile loop here, so all 12 warps share the final prunes.
     __syncthreads();
     {
         const bool cosine = p.metric == NK_METRIC_COSINE;
@@ -724,11 +660,7 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
         if (FILTER && !cosine && tid == 0) atomicMax(reinterpret_cast<unsigned int *>(p.flags + 2), sh.maxxx);
     }
 
-    if (prof && tid == EPI_WARP0 * 32) { g_tc_prof[17] = acc_a; g_tc_prof[18] = clock64() - t_start; g_tc_prof[19] = (long long)num_tiles; }
-    // ---- teardown ----------------------------------------------------------------------------------
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) ptx::tmem_dealloc(tmem, TMEM_COLS);
+    if (prof && tid == EPI_WARP0 * 32) { g_tc_prof[4] = acc_a; g_tc_prof[5] = acc_b; g_tc_prof[6] = clock64() - t_start; g_tc_prof[7] = (long long)num_tiles; }
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -1092,7 +1024,7 @@ int tc_ensure_smem(const void *func, int device, size_t smem) {
 }
 
 static bool tc_common_ok(const DeviceInfo &di, const ScanArgs &a) {
-    if (di.cc < 100) return false;
+    if (di.cc < 90) return false;
     if (a.dtype != NK_DTYPE_F32) return false;                      // fp16 / bf16 corpus: 16-bit tensor pass or CUDA cores
     if (a.dim % 4 != 0 || a.dim < 32) return false;                 // TMA: 16-byte global stride
     if ((reinterpret_cast<uintptr_t>(a.rows) & 15) != 0) return false;
@@ -1178,18 +1110,15 @@ static void tc_print_prof(cudaStream_t stream, uint32_t num_tiles, uint32_t grid
     cudaStreamSynchronize(stream);
     cudaMemcpyFromSymbol(h, g_tc_prof, sizeof(h));
     uint32_t slabs = ((num_tiles + grid - 1) / grid) * nslab;
-    fprintf(stderr, "[tc prof CTA0, ~%u slabs] total %lld cyc (%.0f/slab)\n  tmaA wait aempty_s %lld | tmaB wait bempty %lld\n"
-            "  mma: wait bfull %lld, wait accempty %lld, wait afull %lld, total %lld\n"
-            "  split m0: wait afull_s %lld, wait aempty %lld, read+math %lld, st+arrive %lld, total %lld\n"
-            "  split m1: wait afull_s %lld, wait aempty %lld, read+math %lld, st+arrive %lld\n  epi: wait accfull %lld total %lld\n",
-            slabs, h[7], (double)h[7] / slabs, h[0], h[2], h[4], h[5], h[6], h[7], h[8], h[9], h[10], h[11], h[12], h[13], h[14], h[15], h[16], h[17], h[18]);
+    fprintf(stderr, "[tc prof CTA0, ~%u slabs] total %lld cyc (%.0f/slab)\n  tmaA wait aempty_s %lld (total %lld) | tmaB wait bempty %lld\n"
+            "  consumer warpgroup 0: wait afull_s %lld, wait bfull %lld\n",
+            slabs, h[6], (double)h[6] / slabs, h[0], h[1], h[2], h[4], h[5]);
 }
 
 // ---- the plan of one filter search: everything both the primary stage and the (possibly deferred) tail derive from
 // (device, args).  Deterministic, so the host-driven retry of nk_search can rebuild it after the fact.
 struct FilterPlan {
     uint32_t Qpad, QA, num_tiles, grid, k_emit, dimpad, sample;
-    bool pair;          // batches of >= 256 queries run on CTA pairs (scan_tensor_pair.cu)
     bool big;           // first stage = 16-bit pass (BF16 shadow of an fp32 shard, or an fp16 / bf16 corpus itself)
     bool stage2;        // the TF32 filter over the fp32 rows exists as the retry stage (fp32 shards with a shadow)
     bool can_exact_tc;  // exact stage = 3xTF32 kernel (else the CUDA-core scan)
@@ -1225,8 +1154,7 @@ static int make_filter_plan(const DeviceInfo &di, const ScanArgs &a, Workspace &
     const bool need_f32q = a.dtype == NK_DTYPE_F32;  // hi / lo arrays only serve passes over fp32 rows
     const size_t qaux_floats = (need_f32q ? (size_t)2 * f.Qpad * a.dim : 0) + (size_t)3 * f.QA;
     if (ws_reserve((void **)&ws.qaux, &ws.qaux_bytes, qaux_floats * 4 + (f.big ? (size_t)f.Qpad * f.dimpad * 2 : 0))) return -1;
-    f.pair = f.big && a.Q >= 256 && pair_pass_supported(di, a, f.grid);
-    if (ws_reserve((void **)&ws.cand, &ws.cand_bytes, (size_t)f.grid * (f.pair ? 256 : QT_MAX) * (f.big ? P_SHADOW : P) * 8)) return -1;
+    if (ws_reserve((void **)&ws.cand, &ws.cand_bytes, (size_t)f.grid * QT_MAX * (f.big ? P_SHADOW : P) * 8)) return -1;
     if (ws_reserve((void **)&ws.partial, &ws.partial_bytes, (size_t)a.Q * f.grid * f.k_emit * 8)) return -1;
     if (ws_reserve((void **)&ws.keys2, &ws.keys2_bytes, (size_t)f.QA * 8)) return -1;  // gtau[] + gcount[]
     f.qhi = need_f32q ? ws.qaux : nullptr;
@@ -1400,13 +1328,7 @@ int scan_tensor_filter(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, u
         ShadowPassArgs sp{};
         sp.grid = f.grid; sp.k_emit = f.k_emit; sp.dimpad = f.dimpad; sp.Qpad = f.Qpad; sp.q0 = q0;
         sp.qbf16 = f.qbf16; sp.qnorm = f.qnorm; sp.qa = f.qa; sp.qb = f.qb; sp.presampled = f.sample != 0;
-        if (left >= 256 && f.pair) {
-            // large batches: CTA pairs, 256 query columns per MMA, two query blocks per launch sharing tiles through L2
-            const uint32_t gmax = (uint32_t)tc_env_int("NK_PAIR_GROUPS", 4);
-            sp.qgroups = (left >= 1024 && f.grid >= 16 && gmax >= 4) ? 4u : (left >= 512 && f.grid >= 8 && gmax >= 2) ? 2u : 1u;
-            sp.nq = left < 256u * sp.qgroups ? left / 256u * 256u : 256u * sp.qgroups;
-            if (launch_pair_pass(di, a, ws, sp, launches)) return -1;
-        } else if (left > 64) {
+        if (left > 64) {
             uint32_t groups = 1;
             if (left > 3 * 128 && f.max_groups_shadow >= 4 && f.grid % 4 == 0 && f.grid >= 8) groups = 4;
             else if (left > 128 && f.max_groups_shadow >= 2 && f.grid % 2 == 0 && f.grid >= 4) groups = 2;

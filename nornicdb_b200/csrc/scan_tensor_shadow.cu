@@ -1,4 +1,4 @@
-// scan_tensor_shadow.cu — filter scan over the BF16 SHADOW of the corpus (tcgen05 / TMEM / TMA).
+// scan_tensor_shadow.cu — filter scan over the BF16 SHADOW of the corpus (wgmma / TMA / mbarrier).
 //
 // An fp32 shard optionally carries a bf16 copy of itself ("shadow", +50% HBM, built once at upload and kept in step by
 // append / update / remove) plus two floats per row: |x|^2 and |x - bf16(x)|^2.  The filter scan streams the SHADOW —
@@ -13,13 +13,13 @@
 // the worst case 2^-8), so the margin is as tight as Cauchy-Schwarz allows.  Rows whose upper bound reaches the running
 // k-th bound are kept; margin overflow raises the device flag and the TF32 filter, then the exact kernels, retry.
 //
-// Both operands are plain bf16 tiles in shared memory, so there is no conversion stage and TMEM holds only
-// accumulators — double-buffered: the epilogue of tile t overlaps the MMAs of tile t+1.
-//   warp 0      TMA: shadow slabs [256 rows x 64 bf16] (32 KB, 128B-swizzled), 4-stage ring;
+// Both operands are plain bf16 tiles in shared memory, so there is no conversion stage; the accumulators live in the
+// registers of the warpgroups that issue the MMAs and score them.
+//   warp 0      TMA: shadow slabs [256 rows x 64 bf16] (32 KB, 128B-swizzled), 5-stage ring;
 //   warp 3      TMA: query slabs [QT x 64 bf16] (8 / 16 KB), L2-resident;
-//   warp 1      MMA issuer: per slab 2 M-tiles x 4 tcgen05.mma.kind::f16 (M=128, N=QT, K=16), A and B from smem;
-//   warps 4-11  epilogue, one warpgroup per 128-row M-tile: row norms from global, tcgen05.ld 64 columns at a time,
-//               bound / compare / push, warp-level prunes.
+//   warps 4-11  two consumer warpgroups, one per 128-row M-tile: per slab 2 x 4 wgmma.m64nQTk16 (A and B from smem,
+//               fp32 accumulators in registers), then per tile: row norms from global, bound / compare / push straight
+//               from the accumulator registers, warp-level prunes.  The TMA rings run ahead during the epilogue.
 // Shared-memory traffic per [256 rows x 128 queries x 64 dims]: 112 KB (A 32 w + 32 r, B 16 w + 32 r) for twice the K
 // extent of a TF32 slab: half the bytes per product of the TF32 kernel, which is shared-memory-bandwidth bound at 128
 // query columns.  Algorithmic HBM bytes per launch: n * dimpad * 2 (shadow) + n * 8 (norms).
@@ -27,7 +27,7 @@
 #include <stdlib.h>
 
 #include "kernels.cuh"
-#include "ptx_sm100.cuh"
+#include "ptx_sm90.cuh"
 #include "scan_tensor_shared.cuh"
 
 namespace nk {
@@ -38,7 +38,7 @@ constexpr int NTHREADS = 384;
 constexpr int ROWS = 256;                 // corpus rows per tile (2 M-tiles of 128)
 constexpr int QT_MAX = 128;
 constexpr int BKB = 64;                   // bf16 per row per slab = one 128-byte swizzle row
-constexpr int ASTAGES = 4;
+constexpr int ASTAGES = 5;                // HBM look-ahead while the consumers run a tile's epilogue
 constexpr int A_BYTES = ROWS * 128;       // 32 KB
 constexpr int MAX_BSTAGES = 8;
 constexpr int EPI_WARP0 = 4, EPI_WARPS = 8, EPI_NT = EPI_WARPS * 32;
@@ -47,16 +47,13 @@ constexpr int PRUNE_LANE = PB / 32;       // keys per lane of a warp prune
 
 template <int QT> struct Cfg {
     static constexpr int B_BYTES = QT * 128;
-    static constexpr int BSTAGES = (80 * 1024) / B_BYTES > MAX_BSTAGES ? MAX_BSTAGES : (80 * 1024) / B_BYTES;
+    static constexpr int BSTAGES = (48 * 1024) / B_BYTES > MAX_BSTAGES ? MAX_BSTAGES : (48 * 1024) / B_BYTES;  // L2-resident: a short ring
     static constexpr int RING_BYTES = ASTAGES * A_BYTES + BSTAGES * B_BYTES;
-    static_assert(4 * QT <= TMEM_COLS, "two accumulator buffers of two M-tiles");
 };
 
 struct __align__(8) Shared {
     uint64_t afull[ASTAGES], aempty[ASTAGES];
     uint64_t bfull[MAX_BSTAGES], bempty[MAX_BSTAGES];
-    uint64_t accfull[2], accempty[2][2];          // per accumulator buffer (, M-tile)
-    uint32_t tmem_base;
     unsigned int maxxx, max_ra, max_rb;            // running maxima (float bits) of |x|^2 and the per-row bound factors
     float tau[QT_MAX];
     float qn[QT_MAX];                              // |q| (1 for cosine)
@@ -198,17 +195,12 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
     if (warp == 0 && lane == 0) {
         ptx::prefetch_tensormap(&map_rows);
         ptx::prefetch_tensormap(&map_q);
-        for (int i = 0; i < ASTAGES; ++i) { ptx::mbar_init(&sh.afull[i], 1); ptx::mbar_init(&sh.aempty[i], 1); }
-        for (int i = 0; i < C::BSTAGES; ++i) { ptx::mbar_init(&sh.bfull[i], 1); ptx::mbar_init(&sh.bempty[i], 1); }
-        for (int b = 0; b < 2; ++b) {
-            ptx::mbar_init(&sh.accfull[b], 1);
-            ptx::mbar_init(&sh.accempty[b][0], 4);
-            ptx::mbar_init(&sh.accempty[b][1], 4);
-        }
+        // a stage is free again once every consumer warp has seen its MMAs complete
+        for (int i = 0; i < ASTAGES; ++i) { ptx::mbar_init(&sh.afull[i], 1); ptx::mbar_init(&sh.aempty[i], EPI_WARPS); }
+        for (int i = 0; i < C::BSTAGES; ++i) { ptx::mbar_init(&sh.bfull[i], 1); ptx::mbar_init(&sh.bempty[i], EPI_WARPS); }
         sh.maxxx = 0u; sh.max_ra = 0u; sh.max_rb = 0u;
         ptx::fence_barrier_init();
     }
-    if (warp == 2) ptx::tmem_alloc(&sh.tmem_base, TMEM_COLS);
     if (tid < QT) {
         // start threshold: the caller's score floor and, when the prep kernel sampled the shard, a lower bound of the
         // query's k-th best score (no flood tiles then)
@@ -223,10 +215,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
         sh.qa[tid] = p.qa[qpad_off + tid];
         sh.qb[tid] = p.qb[qpad_off + tid];
     }
-    ptx::tc_fence_before();
     __syncthreads();
-    ptx::tc_fence_after();
-    const uint32_t tmem = sh.tmem_base;
     const bool flood = !p.presampled;  // first two tiles: every (row, query) pair is placed directly
     if (prof && tid == 0) g_sb_prof[blockIdx.x][1] = sb_now();
 
@@ -258,162 +247,142 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                 __syncwarp();
             }
         }
-    } else if (warp == 1) {
-        // ===================================== MMA issuer =========================================
-        const uint32_t idesc = p.op_f16 ? ptx::make_idesc_f16(128, QT) : ptx::make_idesc_bf16(128, QT);
+    } else if (warp >= EPI_WARP0) {
+        // ===================================== consumers: MMA + epilogue ===========================
+        // warpgroup m owns rows [128 m, 128 m + 128) of the tile as two m64 halves h; thread = 4 rows x QT/4 columns of
+        // the accumulator fragments: rows rbase + 64 h + 8 r, columns cbase + 8 (j / 2) + j % 2
+        const uint32_t ewarp = warp - EPI_WARP0, m = ewarp >> 2, wq = ewarp & 3;
+        const uint32_t rbase = m * 128 + wq * 16 + ((uint32_t)lane >> 2), cbase = 2u * ((uint32_t)lane & 3u);
+        uint64_t *my_cand = p.cand + (size_t)blockIdx.x * QT * PB;
+        // capacity rule: a buffer must be prunable below PB - ROWS, or the next tile could overflow it.  Prunes are TRIGGERED
+        // much earlier: an early, tight threshold keeps the buffers short, so the emission at the end of the launch needs no
+        // selection and the finish step reads short lists (small shards: 26 tiles per CTA at N = 1M would otherwise never
+        // prune at all).
+        const int prune_at = PB - ROWS;
+        const int prune_trigger = p.prune_trigger > 0 ? min(prune_at, p.prune_trigger) : min(prune_at, max(192, 4 * (int)p.k));
+        const bool cosine = p.metric == NK_METRIC_COSINE, euclid = p.metric == NK_METRIC_EUCLIDEAN;
+        const bool op_f16 = p.op_f16 != 0;
+        const bool eprof = prof && ewarp == 0 && lane == 0;
+        unsigned long long t_prune = 0, t_wait = 0, t_a = 0;
+        float acc[2][QT / 2];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int i = 0; i < QT / 2; ++i) acc[h][i] = 0.0f;
         uint32_t g = 0, it = 0;
         for (uint32_t tile = sub; tile < num_tiles; tile += sgrid, ++it) {
-            const uint32_t buf = it & 1;
-            ptx::mbar_wait(&sh.accempty[buf][0], ((it >> 1) & 1) ^ 1);  // the epilogue has drained this buffer (two tiles ago)
-            ptx::mbar_wait(&sh.accempty[buf][1], ((it >> 1) & 1) ^ 1);
+            if (eprof) t_a = sb_now();
+            uint32_t prev_sa = 0, prev_sb = 0;
             for (uint32_t j = 0; j < nslab; ++j, ++g) {
                 const uint32_t sa = g % ASTAGES, sbq = g % C::BSTAGES;
                 ptx::mbar_wait(&sh.bfull[sbq], (g / C::BSTAGES) & 1);
                 ptx::mbar_wait(&sh.afull[sa], (g / ASTAGES) & 1);
-                ptx::tc_fence_after();
-                if (ptx::elect_one_sync()) {
-                    const uint64_t bdesc = ptx::make_smem_desc_sw128(ptx::smem_u32(b_base + (size_t)sbq * C::B_BYTES));
-                    const uint32_t abase = ptx::smem_u32(a_base + (size_t)sa * A_BYTES);
-                    // K advance per MMA = 16 bf16 = 32 B = 2 descriptor units
+                const uint64_t bdesc = ptx::make_smem_desc_sw128(ptx::smem_u32(b_base + (size_t)sbq * C::B_BYTES));
+                const uint32_t abase = ptx::smem_u32(a_base + (size_t)sa * A_BYTES + (size_t)m * (A_BYTES / 2));
+                ptx::wgmma_fence();
+                // K advance per MMA = 16 bf16 = 32 B = 2 descriptor units
 #pragma unroll
-                    for (uint32_t m = 0; m < 2; ++m) {
-                        const uint64_t adesc = ptx::make_smem_desc_sw128(abase + m * (A_BYTES / 2));
-                        const uint32_t d = tmem + (buf * 2 + m) * QT;
+                for (uint32_t h = 0; h < 2; ++h) {
+                    const uint64_t adesc = ptx::make_smem_desc_sw128(abase + h * (A_BYTES / 4));
 #pragma unroll
-                        for (uint32_t kk = 0; kk < 4; ++kk) ptx::mma_bf16_ss(d, adesc + kk * 2, bdesc + kk * 2, idesc, (j | kk) != 0);
-                    }
-                    ptx::tc_commit(&sh.aempty[sa]);
-                    ptx::tc_commit(&sh.bempty[sbq]);
-                    if (j + 1 == nslab) ptx::tc_commit(&sh.accfull[buf]);
+                    for (uint32_t kk = 0; kk < 4; ++kk) ptx::wgmma_16bit<QT>(acc[h], adesc + kk * 2, bdesc + kk * 2, (j | kk) != 0, op_f16);
                 }
-                __syncwarp();
+                ptx::wgmma_commit();
+                if (j > 0) {  // the previous slab's MMAs are done while this slab's run: its stages go back to the producers
+                    ptx::wgmma_wait_one();
+                    __syncwarp();
+                    if (lane == 0) { ptx::mbar_arrive(&sh.aempty[prev_sa]); ptx::mbar_arrive(&sh.bempty[prev_sb]); }
+                }
+                prev_sa = sa;
+                prev_sb = sbq;
             }
-        }
-    } else if (warp >= EPI_WARP0) {
-        // ===================================== epilogue =========================================
-        const uint32_t m = (uint32_t)(warp - EPI_WARP0) >> 2, quad = warp & 3, ewarp = warp - EPI_WARP0;
-        const uint32_t lane_base = (quad * 32u) << 16;
-        const uint32_t rt = m * 128 + quad * 32 + lane;  // row within the tile
-        uint64_t *my_cand = p.cand + (size_t)blockIdx.x * QT * PB;
-        // capacity rule: a buffer must be prunable below PB - ROWS, or the next tile could overflow it.  Prunes are TRIGGERED
-        // much earlier (hidden behind the MMAs): an early, tight threshold keeps the buffers short, so the emission at the
-        // end of the launch needs no selection and the finish step reads short lists (small shards: 26 tiles per CTA at
-        // N = 1M would otherwise never prune at all).
-        const int prune_at = PB - ROWS;
-        const int prune_trigger = p.prune_trigger > 0 ? min(prune_at, p.prune_trigger) : min(prune_at, max(192, 4 * (int)p.k));  // (192 / 256 / 384 measured at k = 10: 0.445 / 0.448 / 0.476 ms per 1.25M-row search)
-        const bool cosine = p.metric == NK_METRIC_COSINE, euclid = p.metric == NK_METRIC_EUCLIDEAN;
-        const bool eprof = prof && ewarp == 0 && lane == 0;
-        unsigned long long t_prune = 0, t_wait = 0, t_a = 0;
-        uint32_t it = 0;
-        for (uint32_t tile = sub; tile < num_tiles; tile += sgrid, ++it) {
-            const uint32_t buf = it & 1;
-            const uint32_t row = tile * ROWS + rt;
-            const bool alive = row < p.n && (!p.mask || ((__ldg(p.mask + (row >> 5)) >> (row & 31)) & 1u));
-            // the buffered key is the UPPER bound of the score, bound(row, q) = ra qa[q] + rb qb[q]:
-            //   cosine     acc/|x|                        ra = |dx|/|x|   rb = 1
-            //   dot        acc                            ra = |dx|       rb = |x|
-            //   euclidean  -(|x|^2 + |q|^2 - 2 acc)        ra = 2|dx|      rb = 2|x|   (+ eps (|x|^2 + |q|^2))
-            const float x2 = row < p.n ? __ldg(p.xnorm2 + row) : 0.0f;
-            const float xn = sqrtf(x2);
-            const float dxn = sqrtf((row < p.n && p.dnorm2) ? __ldg(p.dnorm2 + row) : 0.0f) * 1.0001f;  // 16-bit corpus: no residue
-            float mul = 1.0f, ra = dxn, rb = xn;
-            if (cosine) {
-                mul = x2 > 0.0f ? 1.0f / xn : 0.0f;
-                ra = dxn * mul * 1.000001f;
-                rb = 1.0f;
-            } else if (euclid) {
-                mul = 2.0f; ra = 2.0f * dxn; rb = 2.0f * xn;
-            }
-            if (alive && ra < INFINITY && rb < INFINITY) {  // NaN / Inf rows are kept anyway (score NaN -> +inf below)
-                atomicMax(&sh.max_ra, __float_as_uint(ra));
-                if (!cosine) { atomicMax(&sh.max_rb, __float_as_uint(rb)); atomicMax(&sh.maxxx, __float_as_uint(x2)); }
-            }
-            if (eprof) t_a = sb_now();
-            ptx::mbar_wait(&sh.accfull[buf], (it >> 1) & 1);
-            ptx::tc_fence_after();
+            ptx::wgmma_wait_all();
+            ptx::fence_acc(acc[0]);
+            ptx::fence_acc(acc[1]);
+            __syncwarp();
+            if (lane == 0) { ptx::mbar_arrive(&sh.aempty[prev_sa]); ptx::mbar_arrive(&sh.bempty[prev_sb]); }
             if (eprof) {
                 const unsigned long long t = sb_now();
                 t_wait += t - t_a;
                 if (it == 0) g_sb_prof[blockIdx.x][2] = t;
             }
-#pragma unroll 1
-            for (uint32_t chunk = 0; chunk < QT / 64; ++chunk) {
-                const uint32_t cb = chunk * 64;
-                uint32_t v0[32], v1[32];
-                ptx::tmem_ld_32x32b_x32(tmem + lane_base + (buf * 2 + m) * QT + cb, v0);
-                ptx::tmem_ld_32x32b_x32(tmem + lane_base + (buf * 2 + m) * QT + cb + 32, v1);
-                ptx::tmem_wait_ld();
-                if (chunk + 1 == QT / 64) {  // this M-tile's accumulator is in registers / scored: hand it back
-                    ptx::tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) ptx::mbar_arrive(&sh.accempty[buf][m]);
-                }
-                if (DUMP && row < p.n) {  // tests only: score estimate and error bound per (row, query)
-                    for (uint32_t c = 0; c < 64 && cb + c < nq; ++c) {
-                        uint32_t bits = 0;
+            if (flood && it < 2 && ewarp == 0 && lane == 0)
+                for (uint32_t qi = 0; qi < nq; ++qi) sh.cnt[qi] = (int)((it + 1) * ROWS);
 #pragma unroll
-                        for (uint32_t i = 0; i < 32; ++i) {
-                            if (c == i) bits = v0[i];
-                            if (c == 32 + i) bits = v1[i];
-                        }
-                        const uint32_t qi = cb + c;
+            for (uint32_t ri = 0; ri < 4; ++ri) {
+                const uint32_t h = ri >> 1, r = ri & 1;
+                const uint32_t rt = rbase + 64 * h + 8 * r;  // row within the tile
+                const uint32_t row = tile * ROWS + rt;
+                const bool alive = row < p.n && (!p.mask || ((__ldg(p.mask + (row >> 5)) >> (row & 31)) & 1u));
+                // the buffered key is the UPPER bound of the score, bound(row, q) = ra qa[q] + rb qb[q]:
+                //   cosine     acc/|x|                        ra = |dx|/|x|   rb = 1
+                //   dot        acc                            ra = |dx|       rb = |x|
+                //   euclidean  -(|x|^2 + |q|^2 - 2 acc)        ra = 2|dx|      rb = 2|x|   (+ eps (|x|^2 + |q|^2))
+                const float x2 = row < p.n ? __ldg(p.xnorm2 + row) : 0.0f;
+                const float xn = sqrtf(x2);
+                const float dxn = sqrtf((row < p.n && p.dnorm2) ? __ldg(p.dnorm2 + row) : 0.0f) * 1.0001f;  // 16-bit corpus: no residue
+                float mul = 1.0f, ra = dxn, rb = xn;
+                if (cosine) {
+                    mul = x2 > 0.0f ? 1.0f / xn : 0.0f;
+                    ra = dxn * mul * 1.000001f;
+                    rb = 1.0f;
+                } else if (euclid) {
+                    mul = 2.0f; ra = 2.0f * dxn; rb = 2.0f * xn;
+                }
+                if ((lane & 3) == 0 && alive && ra < INFINITY && rb < INFINITY) {  // NaN / Inf rows are kept anyway (score NaN -> +inf below)
+                    atomicMax(&sh.max_ra, __float_as_uint(ra));
+                    if (!cosine) { atomicMax(&sh.max_rb, __float_as_uint(rb)); atomicMax(&sh.maxxx, __float_as_uint(x2)); }
+                }
+                float v[QT / 4];
+#pragma unroll
+                for (int jj = 0; jj < QT / 4; ++jj) v[jj] = acc[h][(jj >> 1) * 4 + r * 2 + (jj & 1)];
+                if (DUMP && row < p.n) {  // tests only: score estimate and error bound per (row, query)
+#pragma unroll
+                    for (int jj = 0; jj < QT / 4; ++jj) {
+                        const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
+                        if (qi >= nq) continue;
                         const float qn = sh.qn[qi];
-                        float est = __uint_as_float(bits) * mul, b = fmaf(ra, sh.qa[qi], rb * sh.qb[qi]);
+                        float est = v[jj] * mul, b = fmaf(ra, sh.qa[qi], rb * sh.qb[qi]);
                         if (euclid) { est -= fmaf(qn, qn, x2); b += EUC_EPS * fmaf(qn, qn, x2); }
                         p.dump_est[(size_t)row * p.dump_ld + q0 + qi] = est;
                         p.dump_bnd[(size_t)row * p.dump_ld + q0 + qi] = b;
                     }
                 }
-                if (flood && it < 2 && cb < nq) {
+                if (flood && it < 2) {
                     // Flood tiles: until the first prune every threshold is -inf and EVERY (row, query) pair is buffered:
                     // place them directly (slot = tile-local row), no atomics, no register select.
                     const uint32_t slot = it * ROWS + rt;
                     const uint32_t grow = (uint32_t)(p.row_base + row);
 #pragma unroll
-                    for (uint32_t c = 0; c < 64; ++c) {
-                        const uint32_t qi = cb + c;
+                    for (int jj = 0; jj < QT / 4; ++jj) {
+                        const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
                         if (qi < nq) {
-                            float sc = fmaf(__uint_as_float(c < 32 ? v0[c & 31] : v1[c & 31]), mul, fmaf(ra, sh.qa[qi], rb * sh.qb[qi]));
+                            float sc = fmaf(v[jj], mul, fmaf(ra, sh.qa[qi], rb * sh.qb[qi]));
                             if (euclid) { const float qn = sh.qn[qi]; sc -= EUC_KEEP * fmaf(qn, qn, x2); }
                             if (sc != sc) sc = INFINITY;
                             my_cand[(size_t)qi * PB + slot] = (alive && sc >= p.min_score) ? make_key(sc, grow) : 0ull;  // 0 = empty slot
                         }
                     }
-                    if (rt == 0 && chunk == 0)
-                        for (uint32_t qi = 0; qi < nq; ++qi) sh.cnt[qi] = (int)((it + 1) * ROWS);
-                } else if (alive && cb < nq) {
-                    // compact compare pass -> 64-bit mask of columns worth buffering (NaN passes); rare pushes out of line
-                    uint32_t pass0 = 0, pass1 = 0;
+                } else if (alive) {
+                    // compact compare pass -> mask of columns worth buffering (NaN passes); rare pushes out of line
+                    uint32_t pass = 0;
 #pragma unroll
-                    for (uint32_t c = 0; c < 32; ++c) {
-                        float s0 = fmaf(__uint_as_float(v0[c]), mul, fmaf(ra, sh.qa[cb + c], rb * sh.qb[cb + c]));
-                        float s1 = fmaf(__uint_as_float(v1[c]), mul, fmaf(ra, sh.qa[cb + 32 + c], rb * sh.qb[cb + 32 + c]));
-                        if (euclid) {
-                            const float q0n = sh.qn[cb + c], q1n = sh.qn[cb + 32 + c];
-                            s0 -= EUC_KEEP * fmaf(q0n, q0n, x2);
-                            s1 -= EUC_KEEP * fmaf(q1n, q1n, x2);
-                        }
-                        pass0 |= !(s0 < sh.tau[cb + c]) ? (1u << c) : 0u;
-                        pass1 |= !(s1 < sh.tau[cb + 32 + c]) ? (1u << c) : 0u;
+                    for (int jj = 0; jj < QT / 4; ++jj) {
+                        const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
+                        float s0 = fmaf(v[jj], mul, fmaf(ra, sh.qa[qi], rb * sh.qb[qi]));
+                        if (euclid) { const float qn = sh.qn[qi]; s0 -= EUC_KEEP * fmaf(qn, qn, x2); }
+                        pass |= (!(s0 < sh.tau[qi]) && qi < nq) ? (1u << jj) : 0u;
                     }
-                    uint64_t pass = (uint64_t)pass0 | ((uint64_t)pass1 << 32);
-                    if (nq - cb < 64) pass &= (1ull << (nq - cb)) - 1ull;
 #pragma unroll 1
                     while (pass) {
-                        const uint32_t c = (uint32_t)__ffsll((long long)pass) - 1u;
-                        pass &= pass - 1ull;
-                        // the register file is not indexable: a 6-level select tree (63 SEL) picks column c
-                        uint32_t t[32];
+                        const uint32_t c = (uint32_t)__ffs((int)pass) - 1u;
+                        pass &= pass - 1u;
+                        float val = 0.0f;
 #pragma unroll
-                        for (int i = 0; i < 32; ++i) t[i] = (c & 32u) ? v1[i] : v0[i];
-#pragma unroll
-                        for (int w = 16; w >= 1; w >>= 1) {
-#pragma unroll
-                            for (int i = 0; i < w; ++i) t[i] = (c & (uint32_t)w) ? t[i + w] : t[i];
-                        }
-                        const uint32_t bits = t[0];
-                        const uint32_t qi = cb + c;
-                        float sc = fmaf(__uint_as_float(bits), mul, fmaf(ra, sh.qa[qi], rb * sh.qb[qi]));
+                        for (uint32_t i = 0; i < (uint32_t)(QT / 4); ++i)  // the register file is not indexable: select by compare
+                            if (c == i) val = v[i];
+                        const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
+                        float sc = fmaf(val, mul, fmaf(ra, sh.qa[qi], rb * sh.qb[qi]));
                         if (euclid) { const float qn = sh.qn[qi]; sc -= EUC_KEEP * fmaf(qn, qn, x2); }
                         if (sc != sc) sc = INFINITY;  // undecidable here: keep it, the exact rescoring judges
                         if (sc >= sh.tau[qi]) {
@@ -600,9 +569,6 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             atomicMax(reinterpret_cast<unsigned int *>(p.flags + 6), cosine ? __float_as_uint(1.0f) : sh.max_rb);
         }
     }
-    ptx::tc_fence_before();
-    __syncthreads();
-    if (warp == 2) ptx::tmem_dealloc(tmem, TMEM_COLS);
     if (prof && tid == 0) g_sb_prof[blockIdx.x][4] = sb_now();
 }
 
@@ -639,7 +605,7 @@ static void sb_print_prof(cudaStream_t stream, uint32_t grid) {
 // The 16-bit pass needs a 16-bit image of the rows: the BF16 shadow of an fp32 shard, or — fp16 / bf16 corpora — the rows
 // themselves (a.shadow == a.rows, shadow_native: no rounding residue on the row side, only the per-row |x|^2 array).
 bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a) {
-    if (di.cc < 100 || a.shadow == nullptr || a.xnorm2 == nullptr || a.k > 192 || a.dim > 32768 || a.dim < 32 || a.n == 0) return false;
+    if (di.cc < 90 || a.shadow == nullptr || a.xnorm2 == nullptr || a.k > 192 || a.dim > 32768 || a.dim < 32 || a.n == 0) return false;
     if ((reinterpret_cast<uintptr_t>(a.rows) & 15) != 0 || (reinterpret_cast<uintptr_t>(a.shadow) & 15) != 0) return false;
     if (a.dtype == NK_DTYPE_F32) return a.dim % 4 == 0;
     return a.dim % 8 == 0;  // 16-bit rows: 16-byte TMA row stride and 128-bit exact re-scoring loads

@@ -25,11 +25,10 @@ enum {
     NK_FLAG_WORDS = 16
 };
 namespace tc {
-constexpr int THREADS = 512;
+constexpr int THREADS = 384;
 constexpr int BK = 32;           // floats per corpus K-slab = one 128-byte swizzle row
-constexpr int TMEM_COLS = 512;
-constexpr int EPI_THREADS = 128;
-constexpr int EPI_BAR = 1;
+constexpr int EPI_THREADS = 256; // the two consumer warpgroups
+constexpr int EPI_BAR = 1;       // named barrier of the consumers (2, 3: one per warpgroup)
 constexpr int P = 512;           // candidate buffer capacity per (CTA, query) of the TF32 kernels: warp_prune<16>
 constexpr int P_SHADOW = 1024;   // ... of the 16-bit kernel (wider margins, 4 query groups at k = 100): warp_prune<32>
 constexpr int QT_BIG = 256;      // padding of the per-query arrays (a CTA reads up to 128 entries past the last query)
@@ -65,8 +64,6 @@ struct Params {
     float *dump_est, *dump_bnd;  // DUMP kernels only (tests): per (row, query) score estimate and error bound, [n][dump_ld]
     uint32_t dump_ld;
     int op_f16;               // 16-bit kernel: operands are fp16 (an fp16 corpus scanned in place) instead of bf16
-    uint32_t *sync;           // pair kernel, optional sibling lockstep: one arrival counter per tile subset (zeroed per launch)
-    uint32_t sync_every;      // ... every this many slabs (0 = off)
 };
 
 
@@ -114,9 +111,6 @@ struct ShadowPassArgs {
 };
 int launch_shadow_pass(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches);
 bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a);
-// The same pass on CTA pairs (scan_tensor_pair.cu: tcgen05.mma.cta_group::2, 256 query columns): nq <= qgroups * 256
-bool pair_pass_supported(const DeviceInfo &di, const ScanArgs &a, uint32_t grid);
-int launch_pair_pass(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches);
 // stand-alone bf16 conversion of a query block (k-means assignment: centroids as "queries")
 int bf16_prep_queries(const ScanArgs &a, uint32_t Qpad, uint32_t dimpad, float acc_c, void *qbf16, float *qnorm, float *qa,
                       float *qb, uint64_t *launches);

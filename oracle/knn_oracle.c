@@ -13,7 +13,7 @@
  * fp64 scorer orc_knn_exact64() below.
  *
  * Third-party note: the arithmetic of pkg/simd lives in github.com/viterin/vek v0.4.3
- * (go.mod:17), which is NOT present under /root/reference and cannot be fetched (no Go
+ * (go.mod:17), which is NOT present in the reference repository and cannot be fetched (no Go
  * toolchain, no network).  Its published algorithm is restated here: vek32.Dot = sum a[i]*b[i];
  * vek32.CosineSimilarity = dot / sqrt(sum a^2 * sum b^2) in one pass (NaN for zero vectors,
  * which pkg/simd/simd_amd64.go:31-35 maps to 0); vek32.Distance = sqrt(sum (a-b)^2);

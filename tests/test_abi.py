@@ -1,4 +1,4 @@
-"""CPU-side checks of the drop-in boundary: the C-ABI library builds for sm_100a, loads, and exports every
+"""CPU-side checks of the drop-in boundary: the C-ABI library builds for sm_90a, loads, and exports every
 symbol include/nornic_knn.h declares, with the binding table in lock-step.  No compute calls (no GPU here)."""
 import os
 import re
@@ -41,10 +41,10 @@ def test_library_exports_every_declared_symbol(knn_lib):
     assert sorted(_lib.SIGNATURES) == syms
 
 
-def test_library_is_sm100a_and_self_contained(knn_lib):
+def test_library_is_sm90a_and_self_contained(knn_lib):
     from nornicdb_b200 import _lib
     out = subprocess.run(["cuobjdump", "-lelf", _lib.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out
     ldd = subprocess.run(["ldd", _lib.LIB_PATH], capture_output=True, text=True).stdout
     assert "cublas" not in ldd and "torch" not in ldd  # plain C ABI: cudart (static) only
 

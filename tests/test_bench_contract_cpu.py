@@ -1,6 +1,6 @@
 """bench.py's output contract, checked without a GPU: helpers import, every workload BASELINE.json names is defined, and
-the committed bench lines (profiles/bench_r1.jsonl, profiles/bench_r2.jsonl, produced by bench.py on B200 boxes) carry every
-key the driver reads — round 2 also the in-run parity check and the north_star grid."""
+the committed bench lines (profiles/bench_h100.jsonl: the default command and `--impl reference`, produced by bench.py on an
+H100) carry every key a reader of the results relies on, the in-run parity check and the north_star grid included."""
 import json
 import os
 
@@ -22,11 +22,10 @@ def test_bench_helpers_and_workloads():
     tf32, _ = bench.load_tensor_peak()
     bf16, _ = bench.load_tensor_peak(bf16=True)
     assert abs(bf16 - 2 * tf32) < 1e-6
-    assert bench.load_traffic("headline", "shadow") > 2.0e10 and bench.load_traffic("headline", "filter") > 4.0e10
 
 
 def test_committed_bench_lines_follow_the_contract():
-    lines = [json.loads(l) for l in open(os.path.join(ROOT, "profiles", "bench_r1.jsonl"))]
+    lines = [json.loads(l) for l in open(os.path.join(ROOT, "profiles", "bench_h100.jsonl"))]
     ours = [d for d in lines if d.get("impl") != "reference"]
     ref = [d for d in lines if d.get("impl") == "reference"]
     assert ours and ref
@@ -50,7 +49,7 @@ def test_committed_bench_lines_follow_the_contract():
 
 
 def test_round2_bench_lines_carry_parity_check_and_grid():
-    lines = [json.loads(l) for l in open(os.path.join(ROOT, "profiles", "bench_r2.jsonl"))]
+    lines = [json.loads(l) for l in open(os.path.join(ROOT, "profiles", "bench_h100.jsonl")) if json.loads(l).get("impl") != "reference"]
     by = {d["run"]: d for d in lines}
     for d in lines:
         for key in REQUIRED + ["scan", "timing"]:
@@ -75,9 +74,3 @@ def test_round2_bench_lines_carry_parity_check_and_grid():
     assert one["also"]["headline_clustered"]["filter_retries"]["exact_stage_rate"] <= 0.05
     st = one["cpu_baseline"]["single_thread"]
     assert st["cores"] == 1 and st["value"] > 0 and one["cpu_baseline"]["value"] >= st["value"] * 0.9
-    for name in ("headline_8gpu_peer", "c5_8gpu_peer"):
-        checks = " ".join(by[name]["parity_check"]["checks"])
-        assert "bit-identical to nk_index_create(devices=0..7) + nk_search" in checks, name
-    assert by["headline_8gpu_peer"]["exchange"].startswith("peer-memory")
-    c5 = by["default_8gpu"]["also"]["c5"]  # configs[4] rides on the default 8-GPU command
-    assert c5["parity_check"]["ok"] is True and c5["rows_per_gpu"] == 12_500_000 and c5["value"] > 0

@@ -3,8 +3,8 @@
 The BF16-shadow / FP16 / TF32 filter scans are sound iff, for every (row, query) pair, the score estimate the tensor
 cores produce is within the bound the kernel adds to it:   |est - exact| <= bnd,   where bnd is built from the kernel's
 own per-row and per-query factors (ra, rb, qa, qb / margin_c) and includes the allowance acc_c = d * 2^-22 + 4e-6 for
-tcgen05's fp32 accumulation — a constant round 1 only checked against a sequential numpy sum.  Here the DUMP
-instantiation of the scan kernels writes (est, bnd) for every pair straight from the TMEM accumulator, and the test
+the tensor cores' fp32 accumulation — a constant round 1 only checked against a sequential numpy sum.  Here the DUMP
+instantiation of the scan kernels writes (est, bnd) for every pair straight from the accumulator registers, and the test
 compares with the fp64 score on uniform, same-sign (no cancellation), huge / tiny scaled, sparse and heavy-cancellation
 data at d = 32 / 1024 / 4096: > 10^7 pairs per run.  The worst observed err / bnd is printed and must stay below 1 (it
 sits well below: the Cauchy-Schwarz bounds are loose by construction)."""

@@ -186,8 +186,8 @@ def _torch_fp64_topk(n, d, q, k, metric, slice_rows, rows_of_slice):
 
 
 def test_config3_full_size_all_queries_fp64(knn_lib, oracle_mod):
-    """BASELINE.json configs[2] at FULL size: N=10M d=1024 fp32, ALL 1024 queries, k=100, inner product (the CTA-pair
-    path), against an fp64 brute force over all 10^7 x 1024 (row, query) pairs computed slice by slice with torch on the
+    """BASELINE.json configs[2] at FULL size: N=10M d=1024 fp32, ALL 1024 queries, k=100, inner product (the 16-bit
+    pass with 4 query groups per launch), against an fp64 brute force over all 10^7 x 1024 (row, query) pairs computed slice by slice with torch on the
     same GPU (round-1 VERDICT: only 64 of these queries had ever been checked)."""
     import torch
     from nornicdb_b200.knn import KnnIndex, fill_uniform_device

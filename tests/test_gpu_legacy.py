@@ -14,10 +14,10 @@ def test_device_info(gpu_device):
     from nornicdb_b200 import cuda
     assert cuda.IsAvailable() and cuda.DeviceCount() >= 1
     assert gpu_device.ID() == 0
-    assert "B200" in gpu_device.Name() or gpu_device.Name()
+    assert "H100" in gpu_device.Name() or gpu_device.Name()
     assert gpu_device.MemoryBytes() > 0 and gpu_device.MemoryMB() > 0
     major, minor = gpu_device.ComputeCapability()
-    assert major == 10, f"this build targets sm_100a, device is {major}.{minor}"
+    assert (major, minor) == (9, 0), f"this build targets sm_90a, device is {major}.{minor}"
     assert cuda.HasGPUHardware() and cuda.IsCUDACapable()
     assert cuda.GPUName() == gpu_device.Name() and cuda.GPUMemoryMB() == gpu_device.MemoryMB()
 

@@ -368,8 +368,9 @@ def test_exchange_across_gpus_in_one_process(knn_lib, oracle_mod):
 @pytest.mark.parametrize("metric", ["cosine", "dot", "euclidean"])
 @pytest.mark.parametrize("Q,k", [(256, 10), (300, 10), (520, 100), (1024, 10)])
 def test_large_batches_on_cta_pairs(knn_lib, oracle_mod, metric, Q, k):
-    """Q >= 256: the 16-bit pass runs on CTA pairs (tcgen05.mma.cta_group::2, 256 query columns), the remainder on the
-    single-CTA kernels; results must match the fp64 oracle like every other path."""
+    """Q >= 256 (the name dates from the Blackwell CTA-pair kernel; the test ids are kept so that the large-batch cases
+    stay comparable across versions): the 16-bit pass runs in blocks of 128 query columns with 2 / 4 query groups per
+    launch, the remainder in a 64-column launch; results must match the fp64 oracle like every other path."""
     n, d = 70_000, 128
     rows = oracle_mod.fill_uniform(n, d, 101)
     q = oracle_mod.fill_uniform(Q, d, 102)
@@ -383,8 +384,9 @@ def test_large_batches_on_cta_pairs(knn_lib, oracle_mod, metric, Q, k):
 
 
 def test_cta_pairs_fp16_corpus_and_ragged_rows(knn_lib, oracle_mod):
+    """fp16 corpus, Q=512, a row count that is not a multiple of the 256-row tile, on the 16-bit pass (name: see above)."""
     from nornicdb_b200.knn import KnnIndex
-    n, d, Q, k = 33_333, 256, 512, 10  # n not a multiple of the 256-row pair tile
+    n, d, Q, k = 33_333, 256, 512, 10  # n not a multiple of the 256-row tile
     rows = oracle_mod.fill_uniform(n, d, 103).astype(np.float16)
     q = oracle_mod.fill_uniform(Q, d, 104)
     ix = KnnIndex(d, metric="cosine", dtype="f16")

@@ -1,4 +1,4 @@
-"""GPU parity tests of the tcgen05 / TMEM / TMA scan (path="tensor") against the fp64 oracle."""
+"""GPU parity tests of the wgmma / TMA scan (path="tensor") against the fp64 oracle."""
 import numpy as np
 import pytest
 
