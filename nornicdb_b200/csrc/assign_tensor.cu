@@ -1,9 +1,9 @@
 // assign_tensor.cu — k-means assignment step on the tensor cores (pkg/gpu/kmeans.go:458-546; SURVEY.md §8(f)4).
 //
 // nearest centroid of every corpus row = the Q x N^T contraction of the scan with Q = #centroids and an ARGMAX over the
-// centroid columns instead of a per-query top-k.  The kernel reuses the shadow scan's pipeline (scan_tensor_shadow.cu:
+// centroid columns instead of a per-query top-k.  The kernel reuses the shadow scan's pipeline (scan_tensor_shared.cuh:
 // TMA slabs of the BF16 shadow and of the bf16 centroids, wgmma from shared memory, accumulators in the registers of two
-// consumer warpgroups) with one more loop level — every corpus tile is multiplied with each block of 64 centroids in turn
+// consumer warpgroups; the centroids are prepared by filter_prep_kernel) with one more loop level — every corpus tile is multiplied with each block of 64 centroids in turn
 // (the tile is re-read from L2, it crossed HBM once) — and a register-only epilogue: each thread keeps, for each of its
 // four fragment rows, the four best UPPER bounds and the best LOWER bound over its columns of every centroid block; the
 // four lanes that share a row merge their lists at the end.
@@ -24,7 +24,6 @@ namespace nk {
 namespace asg {
 using namespace tc;
 constexpr int NTHREADS = 384;
-constexpr int ROWS = 256;
 constexpr int QT = 64;
 constexpr int BKB = 64;
 constexpr int ASTAGES = 4;
@@ -46,8 +45,7 @@ struct Params {
 };
 
 struct __align__(8) Shared {
-    uint64_t afull[ASTAGES], aempty[ASTAGES];
-    uint64_t bfull[BSTAGES], bempty[BSTAGES];
+    Rings<ASTAGES> ring;
 };
 }  // namespace asg
 
@@ -65,42 +63,23 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
     if (warp == 0 && lane == 0) {
         ptx::prefetch_tensormap(&map_rows);
         ptx::prefetch_tensormap(&map_q);
-        // a stage is free again once every consumer warp has seen its MMAs complete
-        for (int i = 0; i < ASTAGES; ++i) { ptx::mbar_init(&sh.afull[i], 1); ptx::mbar_init(&sh.aempty[i], 8); }
-        for (int i = 0; i < BSTAGES; ++i) { ptx::mbar_init(&sh.bfull[i], 1); ptx::mbar_init(&sh.bempty[i], 8); }
-        ptx::fence_barrier_init();
+        sh.ring.init(BSTAGES);
     }
     __syncthreads();
 
     if (warp == 0) {
         // TMA producer: shadow slabs; a tile is streamed once per centroid block (first from HBM, then from L2)
-        uint32_t g = 0;
-        for (uint32_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x)
-            for (uint32_t qbk = 0; qbk < nqb; ++qbk)
-                for (uint32_t j = 0; j < nslab; ++j, ++g) {
-                    const uint32_t s = g % ASTAGES;
-                    ptx::mbar_wait(&sh.aempty[s], ((g / ASTAGES) & 1) ^ 1);
-                    if (ptx::elect_one_sync()) {
-                        ptx::mbar_arrive_expect_tx(&sh.afull[s], A_BYTES);
-                        ptx::tma_load_2d(&map_rows, &sh.afull[s], a_base + (size_t)s * A_BYTES, (int32_t)(j * BKB), (int32_t)(tile * ROWS),
-                                         qbk + 1 == nqb ? ptx::CACHE_EVICT_FIRST : ptx::CACHE_EVICT_NORMAL);
-                    }
-                    __syncwarp();
-                }
+        tma_producer<ASTAGES>(sh.ring.aempty, blockIdx.x, num_tiles, gridDim.x, nqb, nslab, false, [&](uint32_t s, uint32_t tile, uint32_t qbk, uint32_t j) {
+            ptx::mbar_arrive_expect_tx(&sh.ring.afull[s], A_BYTES);
+            ptx::tma_load_2d(&map_rows, &sh.ring.afull[s], a_base + (size_t)s * A_BYTES, (int32_t)(j * BKB), (int32_t)(tile * ROWS),
+                             qbk + 1 == nqb ? ptx::CACHE_EVICT_FIRST : ptx::CACHE_EVICT_NORMAL);
+        });
     } else if (warp == 3) {
         // TMA producer: centroid slabs (L2-resident)
-        uint32_t g = 0;
-        for (uint32_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x)
-            for (uint32_t qbk = 0; qbk < nqb; ++qbk)
-                for (uint32_t j = 0; j < nslab; ++j, ++g) {
-                    const uint32_t s = g % BSTAGES;
-                    ptx::mbar_wait(&sh.bempty[s], ((g / BSTAGES) & 1) ^ 1);
-                    if (ptx::elect_one_sync()) {
-                        ptx::mbar_arrive_expect_tx(&sh.bfull[s], B_BYTES);
-                        ptx::tma_load_2d(&map_q, &sh.bfull[s], b_base + (size_t)s * B_BYTES, (int32_t)(j * BKB), (int32_t)(qbk * QT), ptx::CACHE_EVICT_LAST);
-                    }
-                    __syncwarp();
-                }
+        tma_producer<BSTAGES>(sh.ring.bempty, blockIdx.x, num_tiles, gridDim.x, nqb, nslab, false, [&](uint32_t s, uint32_t, uint32_t qbk, uint32_t j) {
+            ptx::mbar_arrive_expect_tx(&sh.ring.bfull[s], B_BYTES);
+            ptx::tma_load_2d(&map_q, &sh.ring.bfull[s], b_base + (size_t)s * B_BYTES, (int32_t)(j * BKB), (int32_t)(qbk * QT), ptx::CACHE_EVICT_LAST);
+        });
     } else if (warp >= EPI_WARP0) {
         // consumers: warpgroup m owns rows [128 m, 128 m + 128) of the tile as two m64 halves h; thread = 4 rows
         // (rbase + 64 h + 8 r) x QT/4 centroid columns (cbase + 8 (j / 2) + j % 2) of every centroid block
@@ -132,8 +111,8 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
             for (uint32_t qbk = 0; qbk < nqb; ++qbk) {
                 for (uint32_t j = 0; j < nslab; ++j, ++g) {
                     const uint32_t sa = g % ASTAGES, sbq = g % BSTAGES;
-                    ptx::mbar_wait(&sh.bfull[sbq], (g / BSTAGES) & 1);
-                    ptx::mbar_wait(&sh.afull[sa], (g / ASTAGES) & 1);
+                    ptx::mbar_wait(&sh.ring.bfull[sbq], (g / BSTAGES) & 1);
+                    ptx::mbar_wait(&sh.ring.afull[sa], (g / ASTAGES) & 1);
                     const uint64_t bdesc = ptx::make_smem_desc_sw128(ptx::smem_u32(b_base + (size_t)sbq * B_BYTES));
                     const uint32_t abase = ptx::smem_u32(a_base + (size_t)sa * A_BYTES + (size_t)m * (A_BYTES / 2));
                     ptx::wgmma_fence();
@@ -148,7 +127,7 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                     ptx::fence_acc(acc[0]);
                     ptx::fence_acc(acc[1]);
                     __syncwarp();
-                    if (lane == 0) { ptx::mbar_arrive(&sh.aempty[sa]); ptx::mbar_arrive(&sh.bempty[sbq]); }
+                    if (lane == 0) { ptx::mbar_arrive(&sh.ring.aempty[sa]); ptx::mbar_arrive(&sh.ring.bempty[sbq]); }
                 }
 #pragma unroll
                 for (int jj = 0; jj < QT / 4; ++jj) {
@@ -308,8 +287,10 @@ int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, u
     do {
         if (cudaMemsetAsync(amb_count, 0, 4, stream) != cudaSuccess) { rc = -1; break; }
         ScanArgs a;
-        a.queries = centroids_dev; a.Q = K; a.dim = dim; a.metric = metric; a.stream = stream;
-        if (bf16_prep_queries(a, Kpad, dimpad, acc_c, buf + off_q, qn, qa, qb, launches)) { rc = -1; break; }
+        a.queries = centroids_dev; a.Q = K; a.dim = dim; a.metric = metric;
+        PrepParams pp = prep_params(a, Kpad, dimpad);
+        pp.acc_c = acc_c; pp.qbf = reinterpret_cast<uint16_t *>(buf + off_q); pp.qnorm = qn; pp.qa = qa; pp.qb = qb;
+        if (launch_prep(di, pp, stream, launches)) { rc = -1; break; }
         CUtensorMap map_rows, map_q;
         if (tc_make_map(&map_rows, shadow, n, dimpad, 2, BKB, ROWS, (uint64_t)dimpad * 2)) { rc = -1; break; }
         if (tc_make_map(&map_q, buf + off_q, Kpad, dimpad, 2, BKB, QT, (uint64_t)dimpad * 2)) { rc = -1; break; }

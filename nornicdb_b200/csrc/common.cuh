@@ -169,43 +169,10 @@ __device__ __forceinline__ void block_prune(uint64_t *cand, int cap, int *cnt, f
     }
     __syncthreads();
 }
-// Same, for a sub-group of `nthreads` threads (a multiple of 32, all of whole warps) synchronising on
-// named barrier `bar_id` instead of the whole CTA: used by the epilogue warps of the tensor-core scan.
+// Barrier of a sub-group of `nthreads` threads (a multiple of 32, all of whole warps) on named barrier `bar_id` instead
+// of the whole CTA: used by the consumer warpgroups of the tensor-core scans.
 __device__ __forceinline__ void group_sync(int bar_id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(bar_id), "r"(nthreads) : "memory");
-}
-__device__ __forceinline__ void group_bitonic_sort_desc(uint64_t *s, int P, int gtid, int nthreads, int bar_id) {
-    for (int size = 2; size <= P; size <<= 1) {
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            group_sync(bar_id, nthreads);
-            for (int t = gtid; t < (P >> 1); t += nthreads) {
-                int lo = 2 * t - (t & (stride - 1));
-                int hi = lo + stride;
-                bool desc = (lo & size) == 0;
-                uint64_t a = s[lo], b = s[hi];
-                if ((a < b) == desc) {
-                    s[lo] = b;
-                    s[hi] = a;
-                }
-            }
-        }
-    }
-    group_sync(bar_id, nthreads);
-}
-__device__ __forceinline__ void group_prune(uint64_t *cand, int cap, int *cnt, float *tau, uint32_t k, uint64_t *sbuf,
-                                            int P, int gtid, int nthreads, int bar_id) {
-    group_sync(bar_id, nthreads);
-    int n = *cnt;
-    if (n > cap) n = cap;
-    for (int i = gtid; i < P; i += nthreads) sbuf[i] = i < n ? cand[i] : 0ull;
-    group_bitonic_sort_desc(sbuf, P, gtid, nthreads, bar_id);
-    int keep = n < (int)k ? n : (int)k;
-    for (int i = gtid; i < keep; i += nthreads) cand[i] = sbuf[i];
-    if (gtid == 0) {
-        *cnt = keep;
-        *tau = (n >= (int)k) ? key_score(sbuf[k - 1]) : -INFINITY;
-    }
-    group_sync(bar_id, nthreads);
 }
 // ---------------------------------------------------------------------------------------------
 // Warp-level prune: select the best k of n <= 32*PER_LANE buffered keys with the keys held in registers

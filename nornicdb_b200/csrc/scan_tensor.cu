@@ -29,6 +29,7 @@
 // Exact mode: per-CTA lists are folded by merge_keys().  Filter mode: CTAs share their thresholds through a per-query
 // atomic max, append their survivors to one list per query, and filter_finish_kernel (below) selects, re-scores and
 // sorts.  Large batches: 2 / 4 query groups per launch share every corpus tile through L2 (Params::qgroups).
+// The set-up, the producer loop and the filter epilogue are scan_tensor_shared.cuh's, shared with the 16-bit kernel.
 //
 // Algorithmic HBM traffic per launch: n*dim*4 (corpus, once); query re-reads are served from L2.
 #include <cuda.h>
@@ -46,12 +47,10 @@
 namespace nk {
 
 namespace tc {
-constexpr int ROWS = 256;        // corpus rows per tile (2 M-tiles of 128)
 constexpr int QT_MAX = 128;      // queries per launch (MMA N): 64, or 128 for large batches (filter mode)
 constexpr int ASTAGES = 4;       // corpus-slab smem ring
 constexpr int A_BYTES = ROWS * BK * 4;   // 32 KB
 constexpr int EPI_WARP0 = 4;     // consumer warpgroups: warps 4-7 (rows 0-127), 8-11 (rows 128-255)
-constexpr int MAX_BSTAGES = 8;
 
 template <int NT, int QT> struct Cfg {
     static constexpr int PARTS = NT == 3 ? 2 : 1;          // hi (+ lo)
@@ -65,9 +64,8 @@ template <int NT, int QT> struct Cfg {
 };
 
 struct __align__(8) Shared {
-    uint64_t afull_s[ASTAGES], aempty_s[ASTAGES];    // corpus slab in smem: TMA -> consumers -> TMA
-    uint64_t bfull[MAX_BSTAGES], bempty[MAX_BSTAGES];  // query slabs in smem: TMA -> consumers -> TMA
-    unsigned int maxxx;       // running max of |x|^2 (float bits) over the rows this CTA has scored
+    Rings<ASTAGES> ring;      // corpus and query slabs in smem: TMA -> consumers -> TMA
+    unsigned int maxxx;      // running max of |x|^2 (float bits) over the rows this CTA has scored
     float xx[ROWS];           // |x|^2 per row of the current tile (split step -> epilogue, same warpgroup)
     float tau[QT_MAX];
     float qn[QT_MAX];
@@ -153,26 +151,6 @@ __device__ __forceinline__ float warp_exact_score(const void *rows, int dtype, s
 //     tiles and pruning 64-128 full buffers per CTA (~25 us per launch, the largest fixed cost of a small-shard search).
 // ---------------------------------------------------------------------------------------------------
 constexpr int PREP_THREADS = 1024;  // 32 warps: the sample scoring is latency-bound (one 4 KB row per warp at a time)
-struct PrepParams {
-    const float *q;
-    uint32_t Q, dim, dimpad;
-    int normalise, metric;
-    float acc_c;
-    float *qhi, *qlo;      // [Qpad x dim] (nullable)
-    uint16_t *qbf;         // [Qpad x dimpad] (nullable); fp16 bits when qbf_f16
-    int qbf_f16;
-    float *qnorm, *qa, *qb;
-    uint32_t *state;       // gtau[QA] then gcount[QA]
-    uint32_t Qpad, QA;
-    int *flags;
-    // sampled initial threshold (sample == 0: none)
-    const void *rows;
-    int dtype;
-    uint32_t n, sample, k;
-    const uint32_t *mask;
-    float min_score;
-    const int *only_if;
-};
 
 __global__ void __launch_bounds__(PREP_THREADS) filter_prep_kernel(PrepParams p) {
     extern __shared__ __align__(16) unsigned char prep_smem[];
@@ -328,6 +306,27 @@ __global__ void __launch_bounds__(PREP_THREADS) filter_prep_kernel(PrepParams p)
     }
 }
 
+// Score estimate of one accumulator fragment row of the TF32 scan (keep_fragment_row):
+//   cosine     acc / |x|  (queries pre-normalised)       filter bound c
+//   dot        acc                                        filter bound c |x| |q|
+//   euclidean  -(|x|^2 + |q|^2 - 2 acc)   (filter only)   filter bound 2c |x| |q|
+// filter mode buffers the UPPER bound score + bound.
+template <bool FILTER> struct Tf32Est {
+    float mul, bnd, x2;
+    const float *qn;
+    bool euclid;
+    __device__ __forceinline__ float upper(float v, uint32_t qi) const {
+        float sc = v * mul;
+        if (FILTER) {
+            const float q = qn[qi];
+            if (euclid) sc -= tc::EUC_KEEP * fmaf(q, q, x2);
+            sc = fmaf(bnd, q, sc);
+        }
+        return sc;
+    }
+    __device__ __forceinline__ float bound(uint32_t qi) const { return bnd * qn[qi]; }
+};
+
 template <int NT, int QT, bool DUMP>
 __global__ void __launch_bounds__(tc::THREADS, 1)
 knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_qhi,
@@ -350,73 +349,48 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t num_tiles = (p.n + ROWS - 1) / ROWS;
-    // Query groups: CTA b serves query block (b % G) over the tile subset (b / G).  The G sibling CTAs stream the SAME
-    // corpus tiles at the same pace, so a tile crosses HBM once and its other G-1 readers hit the 50 MB L2: large
-    // batches (Q > 128) stop being bound by re-reading the corpus once per 128 queries.
-    const uint32_t grp = blockIdx.x % p.qgroups, sub = blockIdx.x / p.qgroups, sgrid = gridDim.x / p.qgroups;
-    const uint32_t q0 = p.q0 + grp * QT, qpad_off = p.qpad_off + grp * QT;
-    const uint32_t nq = p.nq - grp * QT < (uint32_t)QT ? p.nq - grp * QT : (uint32_t)QT;
-    const uint64_t a_policy = p.qgroups > 1 ? ptx::CACHE_EVICT_NORMAL : ptx::CACHE_EVICT_FIRST;
+    const QueryGroup<QT> qg(p);
+    const uint32_t sub = qg.sub, sgrid = qg.sgrid, q0 = qg.q0, qpad_off = qg.qpad_off, nq = qg.nq;
     const bool prof = (p.debug & 64) && blockIdx.x == 0;
-    long long acc_a = 0, acc_b = 0, acc_c = 0, acc_d = 0;
+    long long acc_a = 0, acc_b = 0;
     const long long t_start = prof ? clock64() : 0;
 
     if (warp == 0 && lane == 0) {
         ptx::prefetch_tensormap(&map_rows);
         ptx::prefetch_tensormap(&map_qhi);
         if (NT == 3) ptx::prefetch_tensormap(&map_qlo);
-        // a stage is free again once every consumer warp has seen its MMAs complete
-        for (int i = 0; i < ASTAGES; ++i) { ptx::mbar_init(&sh.afull_s[i], 1); ptx::mbar_init(&sh.aempty_s[i], 8); }
-        for (int i = 0; i < C::BSTAGES; ++i) { ptx::mbar_init(&sh.bfull[i], 1); ptx::mbar_init(&sh.bempty[i], 8); }
         sh.maxxx = 0u;
-        ptx::fence_barrier_init();
+        sh.ring.init(C::BSTAGES);
     }
     if (tid < QT) {
-        // start threshold: the caller's score floor and, when the prep kernel sampled the shard, a lower bound of the
-        // query's k-th best score (no flood tiles then)
-        float t0 = p.min_score;
-        if (FILTER && p.presampled && (uint32_t)tid < nq) {
-            const uint32_t g = __ldcg(p.gtau + q0 + tid);
-            if (g) t0 = fmaxf(t0, ord_to_float(g));
-        }
-        sh.tau[tid] = t0;
+        sh.tau[tid] = FILTER ? start_tau(p, q0, tid, nq) : p.min_score;
         sh.cnt[tid] = 0;
         sh.qn[tid] = (FILTER && p.qnorm) ? p.qnorm[qpad_off + tid] : 1.0f;
     }
     __syncthreads();
     const bool flood = !(FILTER && p.presampled);  // first two tiles: every (row, query) pair is placed directly
+    uint64_t *my_cand = p.cand + (size_t)blockIdx.x * QT * P;
+    auto prune = [&](uint32_t qi, uint64_t *out, int out_len, int max_keep, float floor_tau, int *gcount) {
+        const float margin2 = !FILTER ? 0.0f : filter_margin2(p.metric, p.margin_c, __uint_as_float(sh.maxxx), sh.qn[qi]);
+        warp_prune<16>(my_cand + (size_t)qi * P, &sh.cnt[qi], &sh.tau[qi], p.k, lane, out, out_len, FILTER, margin2, max_keep, floor_tau,
+                       gcount, p.flags + FLAG_OVERFLOW);
+    };
 
     if (warp == 0) {
         // ===================================== TMA producer: corpus slabs ========================
-        uint32_t g = 0;
-        for (uint32_t tile = sub; tile < num_tiles; tile += sgrid) {
-            for (uint32_t j = 0; j < p.nslab; ++j, ++g) {
-                const uint32_t s = g % ASTAGES;
-                { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.aempty_s[s], ((g / ASTAGES) & 1) ^ 1); TC_PROF_END(a); }
-                if (ptx::elect_one_sync()) {
-                    ptx::mbar_arrive_expect_tx(&sh.afull_s[s], A_BYTES);
-                    ptx::tma_load_2d(&map_rows, &sh.afull_s[s], a_base + (size_t)s * A_BYTES, (int32_t)(j * BK), (int32_t)(tile * ROWS), a_policy);
-                }
-                __syncwarp();
-            }
-        }
+        acc_a = tma_producer<ASTAGES>(sh.ring.aempty, sub, num_tiles, sgrid, 1, p.nslab, prof, [&](uint32_t s, uint32_t tile, uint32_t, uint32_t j) {
+            ptx::mbar_arrive_expect_tx(&sh.ring.afull[s], A_BYTES);
+            ptx::tma_load_2d(&map_rows, &sh.ring.afull[s], a_base + (size_t)s * A_BYTES, (int32_t)(j * BK), (int32_t)(tile * ROWS), qg.a_policy);
+        });
         if (prof && lane == 0) { g_tc_prof[0] = acc_a; g_tc_prof[1] = clock64() - t_start; }
     } else if (warp == 3) {
         // ===================================== TMA producer: query slabs (L2-resident) ===========
-        uint32_t g = 0;
-        for (uint32_t tile = sub; tile < num_tiles; tile += sgrid) {
-            for (uint32_t j = 0; j < p.nslab; ++j, ++g) {
-                const uint32_t s = g % C::BSTAGES;
-                { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.bempty[s], ((g / C::BSTAGES) & 1) ^ 1); TC_PROF_END(a); }
-                if (ptx::elect_one_sync()) {
-                    unsigned char *st = b_base + (size_t)s * C::BST_BYTES;
-                    ptx::mbar_arrive_expect_tx(&sh.bfull[s], C::BST_BYTES);
-                    ptx::tma_load_2d(&map_qhi, &sh.bfull[s], st, (int32_t)(j * BK), (int32_t)qpad_off, ptx::CACHE_EVICT_LAST);
-                    if (NT == 3) ptx::tma_load_2d(&map_qlo, &sh.bfull[s], st + B_BYTES, (int32_t)(j * BK), (int32_t)qpad_off, ptx::CACHE_EVICT_LAST);
-                }
-                __syncwarp();
-            }
-        }
+        acc_a = tma_producer<C::BSTAGES>(sh.ring.bempty, sub, num_tiles, sgrid, 1, p.nslab, prof, [&](uint32_t s, uint32_t, uint32_t, uint32_t j) {
+            unsigned char *st = b_base + (size_t)s * C::BST_BYTES;
+            ptx::mbar_arrive_expect_tx(&sh.ring.bfull[s], C::BST_BYTES);
+            ptx::tma_load_2d(&map_qhi, &sh.ring.bfull[s], st, (int32_t)(j * BK), (int32_t)qpad_off, ptx::CACHE_EVICT_LAST);
+            if (NT == 3) ptx::tma_load_2d(&map_qlo, &sh.ring.bfull[s], st + B_BYTES, (int32_t)(j * BK), (int32_t)qpad_off, ptx::CACHE_EVICT_LAST);
+        });
         if (prof && lane == 0) { g_tc_prof[2] = acc_a; }
     } else if (warp >= EPI_WARP0) {
         // ===================================== consumers: split + MMA + epilogue ===================
@@ -427,7 +401,6 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
         const uint32_t srow = m * 128 + ((uint32_t)tid & 127u);  // split row
         const uint32_t rbase = m * 128 + wq * 16 + ((uint32_t)lane >> 2), cbase = 2u * ((uint32_t)lane & 3u);
         unsigned char *xl_base = smem_raw + (size_t)ASTAGES * A_BYTES + (size_t)C::BSTAGES * C::BST_BYTES + (size_t)m * (A_BYTES / 2);
-        uint64_t *my_cand = p.cand + (size_t)blockIdx.x * QT * P;
         const int prune_at = P - ROWS;
         const bool cosine = p.metric == NK_METRIC_COSINE, euclid = p.metric == NK_METRIC_EUCLIDEAN;
         const float bfac = p.margin_c * (euclid ? 2.0f : 1.0f);  // bound on -dist^2 = -(|x|^2+|q|^2-2x.q) is 2c|x||q|
@@ -441,7 +414,7 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
             float xe = 0.0f, xo = 0.0f;  // |x|^2 of the split row: partial sums over even / odd elements
             for (uint32_t j = 0; j < p.nslab; ++j, ++g) {
                 const uint32_t s = g % ASTAGES, sb = g % C::BSTAGES;
-                { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.afull_s[s], (g / ASTAGES) & 1); TC_PROF_END(a); }
+                { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.ring.afull[s], (g / ASTAGES) & 1); TC_PROF_END(a); }
                 if (NT == 3 && j > 0) group_sync(2 + m, 128);  // the previous slab's MMAs no longer read the xl tile
                 // split: xh = rn_tf32(x) in place (the MMA's A operand), xl = x - xh (exact) into this warpgroup's xl tile,
                 // |x|^2 on the side
@@ -466,7 +439,7 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                 if (j + 1 == p.nslab) sh.xx[srow] = xe + xo;
                 ptx::fence_proxy_async_smem();
                 group_sync(2 + m, 128);  // every row of this warpgroup's half of the slab is rounded
-                { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.bfull[sb], (g / C::BSTAGES) & 1); TC_PROF_END(b); }
+                { TC_PROF_BEGIN(); ptx::mbar_wait(&sh.ring.bfull[sb], (g / C::BSTAGES) & 1); TC_PROF_END(b); }
                 const uint32_t bhi = ptx::smem_u32(b_base + (size_t)sb * C::BST_BYTES);
                 const uint64_t dhi = ptx::make_smem_desc_sw128(bhi), dlo = ptx::make_smem_desc_sw128(bhi + B_BYTES);
                 const uint32_t ahi = ptx::smem_u32(a_base + (size_t)s * A_BYTES + (size_t)m * (A_BYTES / 2)), alo = ptx::smem_u32(xl_base);
@@ -492,7 +465,7 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                 ptx::fence_acc(acc[0]);
                 ptx::fence_acc(acc[1]);
                 __syncwarp();
-                if (lane == 0) { ptx::mbar_arrive(&sh.aempty_s[s]); ptx::mbar_arrive(&sh.bempty[sb]); }
+                if (lane == 0) { ptx::mbar_arrive(&sh.ring.aempty[s]); ptx::mbar_arrive(&sh.ring.bempty[sb]); }
             }
             if (flood && it < 2 && ewarp == 0 && lane == 0)
                 for (uint32_t qi = 0; qi < nq; ++qi) sh.cnt[qi] = (int)((it + 1) * ROWS);
@@ -501,164 +474,42 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                 const uint32_t h = ri >> 1, r = ri & 1;
                 const uint32_t rt = rbase + 64 * h + 8 * r;  // row within the tile
                 const uint32_t row = tile * ROWS + rt;
-                const bool alive = row < p.n && (!p.mask || ((__ldg(p.mask + (row >> 5)) >> (row & 31)) & 1u));
-                // score(row, query c):
-                //   cosine     acc / |x|  (queries pre-normalised)       filter bound c
-                //   dot        acc                                        filter bound c |x| |q|
-                //   euclidean  -(|x|^2 + |q|^2 - 2 acc)   (filter only)   filter bound 2c |x| |q|
-                // filter mode buffers the UPPER bound score + bound.
-                const float x2 = sh.xx[rt];
-                const float xn = sqrtf(x2);
-                float mul = 1.0f, bnd = 0.0f;
-                if (cosine) mul = x2 > 0.0f ? 1.0f / xn : 0.0f;
+                const bool alive = row_alive(p, row);
+                Tf32Est<FILTER> est;
+                est.x2 = sh.xx[rt];
+                est.qn = sh.qn;
+                est.euclid = euclid;
+                const float xn = sqrtf(est.x2);
+                est.mul = 1.0f;
+                est.bnd = 0.0f;
+                if (cosine) est.mul = est.x2 > 0.0f ? 1.0f / xn : 0.0f;
                 if (FILTER) {
-                    bnd = cosine ? p.margin_c : bfac * xn;
-                    if (!cosine && alive && x2 < INFINITY && (lane & 3) == 0) atomicMax(&sh.maxxx, __float_as_uint(x2));  // NaN / Inf rows: kept, judged exactly
-                    if (euclid) mul = 2.0f;
+                    est.bnd = cosine ? p.margin_c : bfac * xn;
+                    if (!cosine && alive && est.x2 < INFINITY && (lane & 3) == 0) atomicMax(&sh.maxxx, __float_as_uint(est.x2));  // NaN / Inf rows: kept, judged exactly
+                    if (euclid) est.mul = 2.0f;
                 }
-                float v[QT / 4];
-#pragma unroll
-                for (int jj = 0; jj < QT / 4; ++jj) v[jj] = acc[h][(jj >> 1) * 4 + r * 2 + (jj & 1)];
-                if (DUMP && FILTER && row < p.n) {  // tests only: score estimate and error bound per (row, query)
-#pragma unroll
-                    for (int jj = 0; jj < QT / 4; ++jj) {
-                        const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
-                        if (qi >= nq) continue;
-                        const float qn = sh.qn[qi];
-                        float est = v[jj] * mul, b = bnd * qn;
-                        if (euclid) { est -= fmaf(qn, qn, x2); b += EUC_EPS * fmaf(qn, qn, x2); }
-                        p.dump_est[(size_t)row * p.dump_ld + q0 + qi] = est;
-                        p.dump_bnd[(size_t)row * p.dump_ld + q0 + qi] = b;
-                    }
-                }
-                if (flood && it < 2) {
-                    // Flood tiles: until the first prune (after this CTA's second tile) every threshold is -inf and
-                    // EVERY (row, query) pair is buffered.  Place them directly - slot = tile-local row, no atomics.
-                    const uint32_t slot = it * ROWS + rt;
-                    const uint32_t grow = (uint32_t)(p.row_base + row);
-#pragma unroll
-                    for (int jj = 0; jj < QT / 4; ++jj) {
-                        const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
-                        if (qi < nq) {
-                            float sc = v[jj] * mul;
-                            if (FILTER) {
-                                const float qn = sh.qn[qi];
-                                if (euclid) sc -= EUC_KEEP * fmaf(qn, qn, x2);
-                                sc = fmaf(bnd, qn, sc);
-                                if (sc != sc) sc = INFINITY;
-                            } else if (sc != sc) {
-                                sc = -INFINITY;
-                            }
-                            my_cand[(size_t)qi * P + slot] = (alive && sc >= p.min_score) ? make_key(sc, grow) : 0ull;  // 0 = empty slot
-                        }
-                    }
-                } else if (alive) {
-                    // Compact compare pass -> mask of columns worth buffering (NaN passes); the rare pushes run in a small
-                    // out-of-line loop so the hot code stays short.
-                    uint32_t pass = 0;
-#pragma unroll
-                    for (int jj = 0; jj < QT / 4; ++jj) {
-                        const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
-                        float s0 = v[jj] * mul;
-                        if (FILTER) {
-                            const float qn = sh.qn[qi];
-                            if (euclid) s0 -= EUC_KEEP * fmaf(qn, qn, x2);
-                            s0 = fmaf(bnd, qn, s0);
-                        }
-                        pass |= (!(s0 < sh.tau[qi]) && qi < nq) ? (1u << jj) : 0u;
-                    }
-#pragma unroll 1
-                    while (pass) {
-                        const uint32_t c = (uint32_t)__ffs((int)pass) - 1u;
-                        pass &= pass - 1u;
-                        float val = 0.0f;
-#pragma unroll
-                        for (uint32_t i = 0; i < (uint32_t)(QT / 4); ++i)  // register file is not indexable: select by compare
-                            if (c == i) val = v[i];
-                        const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
-                        float sc = val * mul;
-                        if (FILTER) {
-                            const float qn = sh.qn[qi];
-                            if (euclid) sc -= EUC_KEEP * fmaf(qn, qn, x2);
-                            sc = fmaf(bnd, qn, sc);
-                            if (sc != sc) sc = INFINITY;  // undecidable here: keep it, the exact rescoring judges
-                        } else if (sc != sc) {
-                            sc = -INFINITY;
-                        }
-                        if (sc >= sh.tau[qi]) {
-                            int pos = atomicAdd(&sh.cnt[qi], 1);
-                            if (pos < P) my_cand[(size_t)qi * P + pos] = make_key(sc, (uint32_t)(p.row_base + row));
-                            else atomicExch(p.flags, 1);
-                        }
-                    }
-                }
+                keep_fragment_row<QT, P, FILTER, DUMP && FILTER>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau, sh.qn,
+                                                                 sh.cnt, my_cand);
             }
             // prune any buffer that could overflow during the next tile; the 8 consumer warps prune different
             // queries concurrently with a register-resident warp selection
             group_sync(EPI_BAR, EPI_THREADS);  // every push of this tile is visible
-            for (uint32_t qi = ewarp; qi < nq; qi += EPI_THREADS / 32)
-                if (sh.cnt[qi] > prune_at) {
-                    const float margin2 = !FILTER ? 0.0f : filter_margin2(p.metric, p.margin_c, __uint_as_float(sh.maxxx), sh.qn[qi]);
-                    float floor_tau = p.min_score;
-                    if (FILTER) {
-                        const uint32_t g = __ldcg(p.gtau + q0 + qi);
-                        if (g) floor_tau = fmaxf(floor_tau, ord_to_float(g));
-                    }
-                    warp_prune<16>(my_cand + (size_t)qi * P, &sh.cnt[qi], &sh.tau[qi], p.k, lane, nullptr, 0, FILTER, margin2, prune_at, floor_tau,
-                                   nullptr, p.flags + FLAG_OVERFLOW);
-                    // everything inside the margin must fit below prune_at, or the next tile could overflow the buffer
-                    if (FILTER && lane == 0 && sh.cnt[qi] >= prune_at) atomicOr(p.flags + 1, 1);
-                    // publish: this CTA's threshold is a lower bound on the true global k-th best score, so every CTA
-                    // may filter with the largest one any CTA has found
-                    if (FILTER && lane == 0 && sh.tau[qi] > -INFINITY) atomicMax(p.gtau + q0 + qi, ord_bits(sh.tau[qi]));
-                }
+            prune_tile<FILTER>(p, q0, nq, ewarp, lane, sh.cnt, sh.tau, prune_at, prune_at, flood && it == 0, prune);
             group_sync(EPI_BAR, EPI_THREADS);
-            if (FILTER) {  // adopt the shared thresholds (one L2 read per query per tile)
-                for (uint32_t qi = tid - EPI_WARP0 * 32; qi < nq; qi += EPI_THREADS) {
-                    const uint32_t g = __ldcg(p.gtau + q0 + qi);
-                    if (g) sh.tau[qi] = fmaxf(sh.tau[qi], ord_to_float(g));
-                }
-            }
+            if (FILTER) adopt_shared_tau(p, q0, nq, tid - EPI_WARP0 * 32, sh.tau);
         }
     }
 
-    // ---- emit this CTA's list per query: best k (exact) or everything inside the margin (filter).  Every role has
-    // finished its tile loop here, so all 12 warps share the final prunes.
+    // ---- emit this CTA's list per query: everything inside the margin (filter) or the best k into fixed slots (exact).
+    // Every role has finished its tile loop here, so all 12 warps share the final prunes.
     __syncthreads();
-    {
-        const bool cosine = p.metric == NK_METRIC_COSINE;
-        uint64_t *my_cand = p.cand + (size_t)blockIdx.x * QT * P;
-        for (uint32_t qi = warp; qi < nq; qi += THREADS / 32) {
-            const float margin2 = !FILTER ? 0.0f : filter_margin2(p.metric, p.margin_c, __uint_as_float(sh.maxxx), sh.qn[qi]);
-            if (FILTER) {
-                // survivors (inside this CTA's margin AND above the shared threshold) go to the query's shared list
-                float floor_tau = p.min_score;
-                const uint32_t g = __ldcg(p.gtau + q0 + qi);
-                if (g) floor_tau = fmaxf(floor_tau, ord_to_float(g));
-                if (sh.cnt[qi] <= (int)p.k_emit) {
-                    // few entries: no local selection, the finish kernel selects globally — append what still reaches the
-                    // current threshold
-                    const float t = fmaxf(sh.tau[qi], floor_tau);
-                    uint64_t thr = t > -INFINITY ? (uint64_t)ord_bits(t) << 32 : 1ull;
-                    if (thr == 0ull) thr = 1ull;
-                    warp_emit_above(my_cand + (size_t)qi * P, sh.cnt[qi], thr, lane, p.partial + (size_t)(q0 + qi) * p.list_cap,
-                                    (int)p.list_cap, p.gcount + q0 + qi);
-                    continue;
-                }
-                warp_prune<16>(my_cand + (size_t)qi * P, &sh.cnt[qi], &sh.tau[qi], p.k, lane,
-                               p.partial + (size_t)(q0 + qi) * p.list_cap, (int)p.list_cap, true, margin2,
-                               (int)p.k_emit, floor_tau, p.gcount + q0 + qi, p.flags + FLAG_OVERFLOW);
-                // the list was cut at k_emit while rows inside the margin remained -> exact fallback
-                if (lane == 0 && sh.cnt[qi] >= (int)p.k_emit && (int)p.k_emit > (int)p.k) atomicOr(p.flags + FLAG_OVERFLOW, 2);
-                if (lane == 0 && sh.tau[qi] > -INFINITY) atomicMax(p.gtau + q0 + qi, ord_bits(sh.tau[qi]));
-            } else {
-                warp_prune<16>(my_cand + (size_t)qi * P, &sh.cnt[qi], &sh.tau[qi], p.k, lane,
-                               p.partial + ((size_t)(q0 + qi) * gridDim.x + blockIdx.x) * p.k_emit, (int)p.k_emit, false, 0.0f, (int)p.k_emit,
-                               p.min_score);
-            }
-        }
-        if (FILTER && !cosine && tid == 0) atomicMax(reinterpret_cast<unsigned int *>(p.flags + 2), sh.maxxx);
+    for (uint32_t qi = warp; qi < nq; qi += THREADS / 32) {
+        if (FILTER)
+            emit_query(p, q0, qi, lane, my_cand + (size_t)qi * P, sh.cnt, sh.tau, prune);
+        else
+            prune(qi, p.partial + ((size_t)(q0 + qi) * gridDim.x + blockIdx.x) * p.k_emit, (int)p.k_emit, (int)p.k_emit, p.min_score, nullptr);
     }
+    if (FILTER && p.metric != NK_METRIC_COSINE && tid == 0) atomicMax(reinterpret_cast<unsigned int *>(p.flags + FLAG_MAXXX), sh.maxxx);
 
     if (prof && tid == EPI_WARP0 * 32) { g_tc_prof[4] = acc_a; g_tc_prof[5] = acc_b; g_tc_prof[6] = clock64() - t_start; g_tc_prof[7] = (long long)num_tiles; }
 }
@@ -707,11 +558,6 @@ struct FinishParams {
 // Debug timeline of the finish kernel (NK_TC_DEBUG & 64), printed after the first-stage finish launch:
 //   [0] entry  [1] list cached  [2] k-th bound selected  [3] survivors gathered  [4] re-scored  [5] ranked  [6] exit  [7] list length
 __device__ unsigned long long g_fin_prof[256][8];
-__device__ __forceinline__ unsigned long long fin_now() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)::"memory");
-    return t;
-}
 
 __global__ void __launch_bounds__(FINISH_THREADS) filter_finish_kernel(FinishParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -727,7 +573,7 @@ __global__ void __launch_bounds__(FINISH_THREADS) filter_finish_kernel(FinishPar
     const uint32_t q = blockIdx.x;
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const bool prof = p.debug && q < 256 && tid == 0;
-    if (prof) g_fin_prof[q][0] = fin_now();
+    if (prof) g_fin_prof[q][0] = tc::globaltimer_ns();
     for (uint32_t j = tid; j < p.dim; j += FINISH_THREADS) qs[j] = p.queries[(size_t)q * p.dim + j];
     int n = p.gcount[q];
     if (tid == 0) atomicMax(p.flags + FLAG_LONGEST, n);  // diagnostics: longest shared list of this search
@@ -759,7 +605,7 @@ __global__ void __launch_bounds__(FINISH_THREADS) filter_finish_kernel(FinishPar
     }
     auto hi_at = [&](int i) -> uint32_t { return cached ? shi[i] : (uint32_t)(__ldcg(list + i) >> 32); };
     __syncthreads();
-    if (prof) { g_fin_prof[q][1] = fin_now(); g_fin_prof[q][7] = (unsigned long long)n; }
+    if (prof) { g_fin_prof[q][1] = tc::globaltimer_ns(); g_fin_prof[q][7] = (unsigned long long)n; }
     if (warp == 0) {
         float a = 0.0f;
         for (uint32_t j = lane; j < p.dim; j += 32) a = fmaf(qs[j], qs[j], a);
@@ -853,7 +699,7 @@ __global__ void __launch_bounds__(FINISH_THREADS) filter_finish_kernel(FinishPar
     // ---- how many rows are inside the margin?  Almost always a few dozen: ONE gather + re-score round.  Only adversarial
     // near-tie data (thousands of survivors) goes through the list in windows, the running best k carried over.
     const uint32_t thr_hi = (uint32_t)(thr_key >> 32);  // keys >= thr_key  <=>  score word >= thr_hi (thr_key's low word is 0 or 1)
-    if (prof) g_fin_prof[q][2] = fin_now();
+    if (prof) g_fin_prof[q][2] = tc::globaltimer_ns();
     int mine = 0;
     for (int i = tid; i < n; i += FINISH_THREADS) mine += hi_at(i) >= thr_hi ? 1 : 0;
     mine = __reduce_add_sync(0xffffffffu, mine);
@@ -874,7 +720,7 @@ __global__ void __launch_bounds__(FINISH_THREADS) filter_finish_kernel(FinishPar
             }
         }
         __syncthreads();
-        if (prof && w0 == 0) g_fin_prof[q][3] = fin_now();
+        if (prof && w0 == 0) g_fin_prof[q][3] = tc::globaltimer_ns();
         const int count = s_count;  // <= FINISH_WIN
         for (int i = warp; i < count; i += FINISH_THREADS / 32) {
             const uint32_t grow = key_row(sb[i]);
@@ -884,7 +730,7 @@ __global__ void __launch_bounds__(FINISH_THREADS) filter_finish_kernel(FinishPar
         }
         const int total = carry + count;
         __syncthreads();
-        if (prof && w0 == 0) g_fin_prof[q][4] = fin_now();
+        if (prof && w0 == 0) g_fin_prof[q][4] = tc::globaltimer_ns();
         if (total <= FINISH_THREADS) {
             // small sets (the common case): rank by counting — one barrier instead of a 15-45 stage bitonic network
             const uint64_t mykey = tid < total ? se[tid] : 0ull;
@@ -904,7 +750,7 @@ __global__ void __launch_bounds__(FINISH_THREADS) filter_finish_kernel(FinishPar
         }
         carry = total < (int)p.k ? total : (int)p.k;
     }
-    if (prof) g_fin_prof[q][5] = fin_now();
+    if (prof) g_fin_prof[q][5] = tc::globaltimer_ns();
     for (uint32_t i = tid; i < p.k; i += FINISH_THREADS) {
         const uint64_t key = (int)i < carry ? se[i] : 0ull;
         p.out[(size_t)q * p.k + i] = key;
@@ -922,7 +768,7 @@ __global__ void __launch_bounds__(FINISH_THREADS) filter_finish_kernel(FinishPar
         s_last = atomicAdd(p.flags + FLAG_FINISH_CTAS, 1) == (int)gridDim.x - 1;
     }
     __syncthreads();
-    if (prof) g_fin_prof[q][6] = fin_now();
+    if (prof) g_fin_prof[q][6] = tc::globaltimer_ns();
     if (!s_last) return;
     __threadfence();
     const int ovf = atomicOr(p.flags + FLAG_OVERFLOW, 0);
@@ -1044,16 +890,62 @@ bool scan_tensor_filter_supported(const DeviceInfo &di, const ScanArgs &a) {
 
 int tc_debug_flags() { return tc_env_int("NK_TC_DEBUG", 0); }
 
+tc::Params pass_params(const ScanArgs &a, Workspace &ws, const tc::PassArgs &t) {
+    tc::Params p{};
+    p.n = a.n; p.dim = a.dim; p.row_base = a.row_base;
+    p.q0 = t.q0; p.nq = t.nq; p.k = a.k; p.qpad_off = t.q0; p.qgroups = t.qgroups; p.list_cap = t.grid * t.k_emit;
+    p.metric = a.metric; p.k_emit = t.k_emit; p.qnorm = t.qnorm;
+    p.cand = ws.cand; p.partial = ws.partial; p.flags = ws.flags; p.debug = tc_debug_flags(); p.mask = a.row_mask;
+    p.gtau = reinterpret_cast<uint32_t *>(ws.keys2); p.gcount = reinterpret_cast<int *>(ws.keys2) + (t.Qpad + tc::QT_BIG);
+    p.presampled = t.presampled; p.min_score = a.min_score;
+    p.dump_est = t.dump_est; p.dump_bnd = t.dump_bnd; p.dump_ld = t.dump_ld;
+    return p;
+}
+
+// Splits queries [q0, q_end) into scan launches: 128 query columns per MMA while more than 64 queries remain (twice the
+// queries per corpus byte streamed), 64 for the tail.  4 query groups per launch while more than 384 queries remain and 2
+// while more than 128 remain (at most max_groups, grid % G == 0): the G sibling CTAs share every corpus tile through L2.
+// launch(qt, q0, nq, groups) returns nonzero on error.
+template <class Launch>
+static int plan_launches(uint32_t q0, uint32_t q_end, uint32_t grid, uint32_t max_groups, Launch launch) {
+    while (q0 < q_end) {
+        const uint32_t left = q_end - q0;
+        uint32_t qt = 64, groups = 1, nq = left;
+        if (left > 64) {
+            if (left > 3 * 128 && max_groups >= 4 && grid % 4 == 0 && grid >= 8) groups = 4;
+            else if (left > 128 && max_groups >= 2 && grid % 2 == 0 && grid >= 4) groups = 2;
+            qt = 128;
+            nq = left < 128u * groups ? left : 128u * groups;
+        }
+        if (launch(qt, q0, nq, groups)) return -1;
+        q0 += nq;
+    }
+    return 0;
+}
+
+PrepParams prep_params(const ScanArgs &a, uint32_t Qpad, uint32_t dimpad) {
+    PrepParams pp{};
+    pp.q = a.queries; pp.Q = a.Q; pp.dim = a.dim; pp.dimpad = dimpad; pp.Qpad = Qpad;
+    pp.normalise = a.metric == NK_METRIC_COSINE; pp.metric = a.metric;
+    pp.rows = a.rows; pp.dtype = a.dtype; pp.n = a.n; pp.k = a.k; pp.mask = a.row_mask; pp.min_score = a.min_score;
+    return pp;
+}
+
+int launch_prep(const DeviceInfo &di, const PrepParams &pp, cudaStream_t stream, uint64_t *launches) {
+    const size_t smem = (size_t)((pp.dim + 3) & ~3u) * 4 + (size_t)pp.sample * 8;
+    if (smem > 48 * 1024 && tc_ensure_smem(reinterpret_cast<const void *>(filter_prep_kernel), di.device_id, smem)) return -1;
+    filter_prep_kernel<<<pp.Qpad, PREP_THREADS, smem, stream>>>(pp);
+    NK_CUDA_OK(cudaGetLastError());
+    if (launches) ++*launches;
+    return 0;
+}
+
 // One launch: queries [q0, q0+nq) against the whole shard, QT = 64 or 128 query columns per MMA.
-struct TcPassArgs {
-    uint32_t grid, k_emit, Qpad, q0, nq, qgroups;
+struct TcPassArgs : tc::PassArgs {
     float margin_c;
-    const float *qhi, *qlo, *qnorm;
+    const float *qhi, *qlo;
     const int *only_if;
     bool count_main;
-    int presampled;
-    float *dump_est = nullptr, *dump_bnd = nullptr;
-    uint32_t dump_ld = 0;
 };
 template <int NT, int QT, bool DUMP = false>
 static int launch_pass(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const TcPassArgs &t, uint64_t *launches) {
@@ -1069,14 +961,8 @@ static int launch_pass(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, c
         return -1;
     }
     if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_tc_kernel<NT, QT, DUMP>), di.device_id, smem)) return -1;
-    Params p{};
-    p.n = a.n; p.dim = a.dim; p.nslab = (a.dim + BK - 1) / BK; p.row_base = a.row_base;
-    p.q0 = t.q0; p.nq = t.nq; p.k = a.k; p.qpad_off = t.q0; p.qgroups = t.qgroups; p.list_cap = t.grid * t.k_emit;
-    p.metric = a.metric; p.k_emit = t.k_emit; p.margin_c = t.margin_c; p.qnorm = t.qnorm;
-    p.cand = ws.cand; p.partial = ws.partial; p.flags = ws.flags; p.only_if = t.only_if; p.debug = tc_debug_flags(); p.mask = a.row_mask;
-    p.gtau = reinterpret_cast<uint32_t *>(ws.keys2); p.gcount = reinterpret_cast<int *>(ws.keys2) + (t.Qpad + QT_BIG);
-    p.presampled = t.presampled; p.min_score = a.min_score;
-    p.dump_est = t.dump_est; p.dump_bnd = t.dump_bnd; p.dump_ld = t.dump_ld;
+    Params p = pass_params(a, ws, t);
+    p.nslab = (a.dim + BK - 1) / BK; p.margin_c = t.margin_c; p.only_if = t.only_if;
     // (asynchronous API: the early-exit retry / exact stages are programmatic dependents — their launch overlaps the kernel
     // before them.  Not for the host-synchronous API: measured 5-15 us slower per nk_search, the copy-out behind it waits longer)
     NK_CUDA_OK(launch_pdl(knn_scan_tc_kernel<NT, QT, DUMP>, dim3(t.grid), dim3(THREADS), smem, a.stream, t.only_if != nullptr && !a.defer_tail, *map_rows, *map_qhi,
@@ -1125,8 +1011,8 @@ struct FilterPlan {
     float acc_c, margin_tf32;
     float *qhi, *qlo, *qnorm, *qa, *qb;
     void *qbf16;
-    uint32_t max_groups, max_groups_shadow;
-    size_t fsmem, psmem;
+    uint32_t max_groups_shadow;
+    size_t fsmem;
 };
 
 static int make_filter_plan(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, FilterPlan *fp) {
@@ -1163,11 +1049,9 @@ static int make_filter_plan(const DeviceInfo &di, const ScanArgs &a, Workspace &
     f.qa = f.qnorm + f.QA;
     f.qb = f.qa + f.QA;
     f.qbf16 = ws.qaux + qaux_floats;
-    f.max_groups = (uint32_t)tc_env_int("NK_TC_QGROUPS", 4);
     // G query groups leave each CTA 1/G of the grid for its queries, i.e. G times the rows — and G times the rows inside
     // the BF16 margin — per (CTA, query) buffer: large k keeps fewer groups so that k + margin rows stay inside k_emit
     f.max_groups_shadow = a.k <= 128 ? 4u : a.k <= 160 ? 2u : 1u;
-    if (f.max_groups_shadow > f.max_groups) f.max_groups_shadow = f.max_groups;
     // Sampled initial threshold: single-pass batches on shards with enough tiles per CTA for the flood tiles to matter.
     // (Large batches re-score the sample once per query — more L2 traffic than the flood tiles cost.)
     f.sample = 0;
@@ -1175,13 +1059,9 @@ static int make_filter_plan(const DeviceInfo &di, const ScanArgs &a, Workspace &
         f.sample = next_pow2(8 * a.k);  // k-th best of the sample = top k/S of the shard: ~8-12% of the rows pass at first
         if (f.sample < 128) f.sample = 128;
         if (f.sample > 2048) f.sample = 2048;
-        const int s_env = tc_env_int("NK_TAU_SAMPLE_S", 0);  // experiments: sample size override (power of two)
-        if (s_env >= 32 && s_env <= 2048) f.sample = next_pow2((uint32_t)s_env);
     }
     f.fsmem = (size_t)FINISH_HI * 4 + (size_t)FINISH_CAP * 16 + (size_t)a.dim * 4;
-    f.psmem = (size_t)((a.dim + 3) & ~3u) * 4 + (size_t)f.sample * 8;
     if (tc_ensure_smem(reinterpret_cast<const void *>(filter_finish_kernel), di.device_id, f.fsmem)) return -1;
-    if (f.psmem > 48 * 1024 && tc_ensure_smem(reinterpret_cast<const void *>(filter_prep_kernel), di.device_id, f.psmem)) return -1;
     return 0;
 }
 
@@ -1199,14 +1079,9 @@ static int scan_tensor_exact(const DeviceInfo &di, const ScanArgs &a, Workspace 
     if (ws_reserve((void **)&ws.partial, &ws.partial_bytes, (size_t)a.Q * grid * a.k * 8)) return -1;
     float *qhi = ws.qaux, *qlo = ws.qaux + (size_t)Qpad * a.dim;
     if (prep) {
-        PrepParams pp{};
-        pp.q = a.queries; pp.Q = a.Q; pp.dim = a.dim; pp.dimpad = a.dim; pp.normalise = a.metric == NK_METRIC_COSINE; pp.metric = a.metric;
-        pp.qhi = qhi; pp.qlo = qlo; pp.Qpad = Qpad; pp.only_if = only_if;
-        const size_t psmem = (size_t)((a.dim + 3) & ~3u) * 4;
-        if (psmem > 48 * 1024 && tc_ensure_smem(reinterpret_cast<const void *>(filter_prep_kernel), di.device_id, psmem)) return -1;
-        filter_prep_kernel<<<Qpad, PREP_THREADS, psmem, a.stream>>>(pp);
-        NK_CUDA_OK(cudaGetLastError());
-        if (launches) ++*launches;
+        PrepParams pp = prep_params(a, Qpad, a.dim);
+        pp.qhi = qhi; pp.qlo = qlo; pp.only_if = only_if;
+        if (launch_prep(di, pp, a.stream, launches)) return -1;
     }
     if (count_main && a.ev_begin) NK_CUDA_OK(cudaEventRecord(a.ev_begin, a.stream));
     for (uint32_t q0 = 0; q0 < a.Q; q0 += 64) {
@@ -1232,30 +1107,25 @@ int scan_tensor(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t
     return scan_tensor_exact(di, a, ws, out_keys, launches, nullptr, true, true);
 }
 
-// TF32 passes over queries [qfirst, Q): 128 query columns per MMA while more than 64 queries remain (twice the queries per
-// corpus byte streamed), a 64-column launch for the tail; 2 or 4 query blocks per launch share every corpus tile through
-// L2 (sibling CTAs).
-static int tf32_passes(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const FilterPlan &f, uint32_t qfirst, const int *only_if,
+// TF32 filter passes over all queries
+static int tf32_passes(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const FilterPlan &f, const int *only_if,
                        bool count_main, int presampled, uint64_t *launches) {
-    for (uint32_t q0 = qfirst; q0 < a.Q;) {
-        const uint32_t left = a.Q - q0;
+    return plan_launches(0, a.Q, f.grid, 4, [&](uint32_t qt, uint32_t q0, uint32_t nq, uint32_t groups) {
         TcPassArgs t{};
-        t.grid = f.grid; t.k_emit = f.k_emit; t.Qpad = f.Qpad; t.q0 = q0; t.margin_c = f.margin_tf32;
+        t.grid = f.grid; t.k_emit = f.k_emit; t.Qpad = f.Qpad; t.q0 = q0; t.nq = nq; t.qgroups = groups; t.margin_c = f.margin_tf32;
         t.qhi = f.qhi; t.qnorm = f.qnorm; t.only_if = only_if; t.count_main = count_main; t.presampled = presampled;
-        if (left > 64) {
-            uint32_t groups = 1;
-            if (left > 3 * 128 && f.max_groups >= 4 && f.grid % 4 == 0 && f.grid >= 8) groups = 4;
-            else if (left > 128 && f.max_groups >= 2 && f.grid % 2 == 0 && f.grid >= 4) groups = 2;
-            t.nq = left < 128u * groups ? left : 128u * groups;
-            t.qgroups = groups;
-            if (launch_pass<1, 128>(di, a, ws, t, launches)) return -1;
-        } else {
-            t.nq = left; t.qgroups = 1;
-            if (launch_pass<1, 64>(di, a, ws, t, launches)) return -1;
-        }
-        q0 += t.nq;
-    }
-    return 0;
+        return qt == 128 ? launch_pass<1, 128>(di, a, ws, t, launches) : launch_pass<1, 64>(di, a, ws, t, launches);
+    });
+}
+
+// The prep launch of a filter search: every query array the plan's passes read, the cleared search state, the sample.
+static PrepParams filter_prep_params(const ScanArgs &a, Workspace &ws, const FilterPlan &f) {
+    PrepParams pp = prep_params(a, f.Qpad, f.dimpad);
+    pp.acc_c = f.acc_c; pp.qhi = f.qhi;
+    pp.qbf = f.big ? static_cast<uint16_t *>(f.qbf16) : nullptr; pp.qbf_f16 = a.dtype == NK_DTYPE_F16;
+    pp.qnorm = f.qnorm; pp.qa = f.qa; pp.qb = f.qb;
+    pp.state = reinterpret_cast<uint32_t *>(ws.keys2); pp.QA = f.QA; pp.flags = ws.flags; pp.sample = f.sample;
+    return pp;
 }
 
 static void fill_finish(FinishParams &fp, const ScanArgs &a, Workspace &ws, const FilterPlan &f, uint64_t *out_keys) {
@@ -1278,7 +1148,7 @@ int scan_tensor_filter_tail(const DeviceInfo &di, const ScanArgs &a, Workspace &
         // the same search over the fp32 rows with the (much tighter) TF32 margins, if a 16-bit margin buffer overflowed.
         // Host-driven tail only: queued blindly (asynchronous API) the stage would cost two early-exit launches on EVERY
         // search to make the rare overflow cheaper — there an overflow goes straight to the exact stage.
-        if (tf32_passes(di, a, ws, f, 0, ws.flags + FLAG_RETRY, false, 0, launches)) return -1;
+        if (tf32_passes(di, a, ws, f, ws.flags + FLAG_RETRY, false, 0, launches)) return -1;
         FinishParams fp{};
         fill_finish(fp, a, ws, f, out_keys);
         fp.q_big = 0; fp.only_if = ws.flags + FLAG_RETRY; fp.mark_retry = 0;
@@ -1310,38 +1180,19 @@ int scan_tensor_filter(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, u
     if (make_filter_plan(di, a, ws, &f)) return -1;
     const uint32_t q_big = f.big ? a.Q : 0;  // queries served by the 16-bit kernel in the first stage (all or none)
 
-    PrepParams pp{};
-    pp.q = a.queries; pp.Q = a.Q; pp.dim = a.dim; pp.dimpad = f.dimpad; pp.normalise = a.metric == NK_METRIC_COSINE; pp.metric = a.metric;
-    pp.acc_c = f.acc_c;
-    pp.qhi = f.qhi; pp.qlo = f.can_exact_tc ? f.qlo : nullptr;
-    pp.qbf = f.big ? static_cast<uint16_t *>(f.qbf16) : nullptr; pp.qbf_f16 = a.dtype == NK_DTYPE_F16;
-    pp.qnorm = f.qnorm; pp.qa = f.qa; pp.qb = f.qb;
-    pp.state = reinterpret_cast<uint32_t *>(ws.keys2); pp.Qpad = f.Qpad; pp.QA = f.QA; pp.flags = ws.flags;
-    pp.rows = a.rows; pp.dtype = a.dtype; pp.n = a.n; pp.sample = f.sample; pp.k = a.k; pp.mask = a.row_mask; pp.min_score = a.min_score;
-    filter_prep_kernel<<<f.Qpad, PREP_THREADS, f.psmem, a.stream>>>(pp);
-    NK_CUDA_OK(cudaGetLastError());
-    if (launches) ++*launches;
+    PrepParams pp = filter_prep_params(a, ws, f);
+    pp.qlo = f.can_exact_tc ? f.qlo : nullptr;
+    if (launch_prep(di, pp, a.stream, launches)) return -1;
 
     if (a.ev_begin) NK_CUDA_OK(cudaEventRecord(a.ev_begin, a.stream));
-    for (uint32_t q0 = 0; q0 < q_big;) {  // 16-bit passes: 128 query columns (up to 4 query groups per launch), 64 for the tail
-        const uint32_t left = q_big - q0;
-        ShadowPassArgs sp{};
-        sp.grid = f.grid; sp.k_emit = f.k_emit; sp.dimpad = f.dimpad; sp.Qpad = f.Qpad; sp.q0 = q0;
-        sp.qbf16 = f.qbf16; sp.qnorm = f.qnorm; sp.qa = f.qa; sp.qb = f.qb; sp.presampled = f.sample != 0;
-        if (left > 64) {
-            uint32_t groups = 1;
-            if (left > 3 * 128 && f.max_groups_shadow >= 4 && f.grid % 4 == 0 && f.grid >= 8) groups = 4;
-            else if (left > 128 && f.max_groups_shadow >= 2 && f.grid % 2 == 0 && f.grid >= 4) groups = 2;
-            sp.nq = left < 128u * groups ? left : 128u * groups;
-            sp.qgroups = groups;
-            if (launch_shadow_pass(128, di, a, ws, sp, launches)) return -1;
-        } else {
-            sp.nq = left; sp.qgroups = 1;
-            if (launch_shadow_pass(64, di, a, ws, sp, launches)) return -1;
-        }
-        q0 += sp.nq;
-    }
-    if (!f.big && tf32_passes(di, a, ws, f, 0, nullptr, true, f.sample != 0, launches)) return -1;
+    if (plan_launches(0, q_big, f.grid, f.max_groups_shadow, [&](uint32_t qt, uint32_t q0, uint32_t nq, uint32_t groups) {
+            ShadowPassArgs sp{};
+            sp.grid = f.grid; sp.k_emit = f.k_emit; sp.dimpad = f.dimpad; sp.Qpad = f.Qpad; sp.q0 = q0; sp.nq = nq; sp.qgroups = groups;
+            sp.qbf16 = f.qbf16; sp.qnorm = f.qnorm; sp.qa = f.qa; sp.qb = f.qb; sp.presampled = f.sample != 0;
+            return launch_shadow_pass((int)qt, di, a, ws, sp, launches);
+        }))
+        return -1;
+    if (!f.big && tf32_passes(di, a, ws, f, nullptr, true, f.sample != 0, launches)) return -1;
     if (a.ev_end) NK_CUDA_OK(cudaEventRecord(a.ev_end, a.stream));
 
     FinishParams fp{};
@@ -1371,16 +1222,9 @@ int scan_filter_dump(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, int
     if (make_filter_plan(di, b, ws, &f)) return -1;
     if (which == NK_PATH_TENSOR_SHADOW && !f.big) { set_error("dump: no 16-bit pass for this shard"); return -1; }
     if (which == NK_PATH_TENSOR_FILTER && a.dtype != NK_DTYPE_F32) { set_error("dump: TF32 pass needs fp32 rows"); return -1; }
-    PrepParams pp{};
-    pp.q = b.queries; pp.Q = b.Q; pp.dim = b.dim; pp.dimpad = f.dimpad; pp.normalise = b.metric == NK_METRIC_COSINE; pp.metric = b.metric;
-    pp.acc_c = f.acc_c; pp.qhi = f.qhi; pp.qlo = nullptr;
-    pp.qbf = f.big ? static_cast<uint16_t *>(f.qbf16) : nullptr; pp.qbf_f16 = b.dtype == NK_DTYPE_F16;
-    pp.qnorm = f.qnorm; pp.qa = f.qa; pp.qb = f.qb;
-    pp.state = reinterpret_cast<uint32_t *>(ws.keys2); pp.Qpad = f.Qpad; pp.QA = f.QA; pp.flags = ws.flags;
-    pp.rows = b.rows; pp.dtype = b.dtype; pp.n = b.n; pp.sample = 0; pp.k = 1; pp.min_score = -INFINITY;
-    filter_prep_kernel<<<f.Qpad, PREP_THREADS, f.psmem, b.stream>>>(pp);
-    NK_CUDA_OK(cudaGetLastError());
-    if (launches) ++*launches;
+    PrepParams pp = filter_prep_params(b, ws, f);
+    pp.sample = 0;
+    if (launch_prep(di, pp, b.stream, launches)) return -1;
     if (which == NK_PATH_TENSOR_SHADOW) {
         ShadowPassArgs sp{};
         sp.grid = f.grid; sp.k_emit = f.k_emit; sp.dimpad = f.dimpad; sp.Qpad = f.Qpad; sp.q0 = 0; sp.nq = b.Q; sp.qgroups = 1;

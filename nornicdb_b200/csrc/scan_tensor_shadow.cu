@@ -19,7 +19,8 @@
 //   warp 3      TMA: query slabs [QT x 64 bf16] (8 / 16 KB), L2-resident;
 //   warps 4-11  two consumer warpgroups, one per 128-row M-tile: per slab 2 x 4 wgmma.m64nQTk16 (A and B from smem,
 //               fp32 accumulators in registers), then per tile: row norms from global, bound / compare / push straight
-//               from the accumulator registers, warp-level prunes.  The TMA rings run ahead during the epilogue.
+//               from the accumulator registers, warp-level prunes (scan_tensor_shared.cuh, shared with the TF32 kernel).
+//               The TMA rings run ahead during the epilogue.
 // Shared-memory traffic per [256 rows x 128 queries x 64 dims]: 112 KB (A 32 w + 32 r, B 16 w + 32 r) for twice the K
 // extent of a TF32 slab: half the bytes per product of the TF32 kernel, which is shared-memory-bandwidth bound at 128
 // query columns.  Algorithmic HBM bytes per launch: n * dimpad * 2 (shadow) + n * 8 (norms).
@@ -35,12 +36,10 @@ namespace nk {
 namespace sb {
 using namespace tc;
 constexpr int NTHREADS = 384;
-constexpr int ROWS = 256;                 // corpus rows per tile (2 M-tiles of 128)
 constexpr int QT_MAX = 128;
 constexpr int BKB = 64;                   // bf16 per row per slab = one 128-byte swizzle row
 constexpr int ASTAGES = 5;                // HBM look-ahead while the consumers run a tile's epilogue
 constexpr int A_BYTES = ROWS * 128;       // 32 KB
-constexpr int MAX_BSTAGES = 8;
 constexpr int EPI_WARP0 = 4, EPI_WARPS = 8, EPI_NT = EPI_WARPS * 32;
 constexpr int PB = tc::P_SHADOW;          // candidate buffer slots per (CTA, query)
 constexpr int PRUNE_LANE = PB / 32;       // keys per lane of a warp prune
@@ -52,8 +51,7 @@ template <int QT> struct Cfg {
 };
 
 struct __align__(8) Shared {
-    uint64_t afull[ASTAGES], aempty[ASTAGES];
-    uint64_t bfull[MAX_BSTAGES], bempty[MAX_BSTAGES];
+    Rings<ASTAGES> ring;
     unsigned int maxxx, max_ra, max_rb;            // running maxima (float bits) of |x|^2 and the per-row bound factors
     float tau[QT_MAX];
     float qn[QT_MAX];                              // |q| (1 for cosine)
@@ -63,52 +61,6 @@ struct __align__(8) Shared {
     int eoff[QT_MAX + 1];                          // emission: prefix of 32-entry chunk counts
 };
 }  // namespace sb
-
-// Queries -> bf16 [Qpad x dimpad] (zero padded), cosine normalises first.  Per query: qnorm = |q| (1 for cosine),
-// qa = |bf16(q)|, qb = |q - bf16(q)| + acc_c |q|  (both inflated by 1e-4 for the fp32 rounding of the sums).
-__global__ void bf16_prep_queries_kernel(const float *q, uint32_t Q, uint32_t dim, uint32_t dimpad, int normalise, float acc_c,
-                                         uint16_t *out, float *qnorm, float *qa, float *qb) {
-    const uint32_t row = blockIdx.x;
-    __shared__ float red[3][32];
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, nw = blockDim.x >> 5;
-    float t = 0.0f;
-    if (row < Q) {
-        float a = 0.0f;
-        for (uint32_t j = threadIdx.x; j < dim; j += blockDim.x) a = fmaf(q[(size_t)row * dim + j], q[(size_t)row * dim + j], a);
-#pragma unroll
-        for (int o = 16; o; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-        if (lane == 0) red[0][w] = a;
-        __syncthreads();
-        for (int i = 0; i < nw; ++i) t += red[0][i];
-        __syncthreads();
-    }
-    const float nrm = sqrtf(t);
-    const float inv = normalise ? (t > 0.0f ? 1.0f / nrm : 0.0f) : 1.0f;  // zero query -> all cosine scores 0
-    const float qn = normalise ? (t > 0.0f ? 1.0f : 0.0f) : nrm;
-    float hh = 0.0f, dd = 0.0f;
-    for (uint32_t j = threadIdx.x; j < dimpad; j += blockDim.x) {
-        const float v = (row < Q && j < dim) ? q[(size_t)row * dim + j] * inv : 0.0f;
-        const uint16_t b = ptx::f32_to_bf16_bits(v);
-        out[(size_t)row * dimpad + j] = b;
-        const float vb = __uint_as_float((uint32_t)b << 16);
-        hh = fmaf(vb, vb, hh);
-        dd = fmaf(v - vb, v - vb, dd);
-    }
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-        hh += __shfl_xor_sync(0xffffffffu, hh, o);
-        dd += __shfl_xor_sync(0xffffffffu, dd, o);
-    }
-    if (lane == 0) { red[1][w] = hh; red[2][w] = dd; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        hh = dd = 0.0f;
-        for (int i = 0; i < nw; ++i) { hh += red[1][i]; dd += red[2][i]; }
-        qnorm[row] = qn;
-        qa[row] = sqrtf(hh) * 1.0001f;
-        qb[row] = (sqrtf(dd) + acc_c * qn) * 1.0001f;
-    }
-}
 
 // fp32 rows -> bf16 shadow rows (row stride dimpad, zero padded) + |x|^2 and |x - bf16(x)|^2 per row.  One warp per row.
 __global__ void build_shadow_kernel(const float *rows, uint64_t n, uint32_t dim, uint32_t dimpad, uint16_t *shadow, float *xnorm2,
@@ -162,11 +114,23 @@ int build_shadow(const float *rows, uint64_t first, uint64_t count, uint32_t dim
 //   [0] entry  [1] set-up done  [2] first accumulator ready  [3] last tile's epilogue done  [4] exit
 //   [5] ns in the prune section (epilogue warp 0)  [6] tile index of the first prune  [7] ns waiting for accumulators
 __device__ unsigned long long g_sb_prof[256][16];  // [8] all warps past the tile loop  [9] warp 0 done emitting  [10] live chunks  [11] entries emitted by warp 0
-__device__ __forceinline__ unsigned long long sb_now() {
-    unsigned long long t;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)::"memory");
-    return t;
-}
+
+// Score estimate of one accumulator fragment row of the 16-bit scan (keep_fragment_row): the UPPER bound of the score,
+// bound(row, q) = ra qa[q] + rb qb[q]:
+//   cosine     acc/|x|                        ra = |dx|/|x|   rb = 1
+//   dot        acc                            ra = |dx|       rb = |x|
+//   euclidean  -(|x|^2 + |q|^2 - 2 acc)        ra = 2|dx|      rb = 2|x|   (+ eps (|x|^2 + |q|^2))
+struct Bf16Est {
+    float mul, ra, rb, x2;
+    const float *qa, *qb, *qn;
+    bool euclid;
+    __device__ __forceinline__ float upper(float v, uint32_t qi) const {
+        float sc = fmaf(v, mul, fmaf(ra, qa[qi], rb * qb[qi]));
+        if (euclid) { const float q = qn[qi]; sc -= tc::EUC_KEEP * fmaf(q, q, x2); }
+        return sc;
+    }
+    __device__ __forceinline__ float bound(uint32_t qi) const { return fmaf(ra, qa[qi], rb * qb[qi]); }
+};
 
 template <int QT, bool DUMP>
 __global__ void __launch_bounds__(sb::NTHREADS, 1)
@@ -183,33 +147,20 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const bool prof = (p.debug & 64) && blockIdx.x < 256;
-    if (prof && tid == 0) { g_sb_prof[blockIdx.x][0] = sb_now(); g_sb_prof[blockIdx.x][6] = ~0ull; }
+    if (prof && tid == 0) { g_sb_prof[blockIdx.x][0] = globaltimer_ns(); g_sb_prof[blockIdx.x][6] = ~0ull; }
     const uint32_t num_tiles = (p.n + ROWS - 1) / ROWS;
-    // query groups: CTA b serves query block (b % G) over the tile subset (b / G); siblings share tiles through L2
-    const uint32_t grp = blockIdx.x % p.qgroups, sub = blockIdx.x / p.qgroups, sgrid = gridDim.x / p.qgroups;
-    const uint32_t q0 = p.q0 + grp * QT, qpad_off = p.qpad_off + grp * QT;
-    const uint32_t nq = p.nq - grp * QT < (uint32_t)QT ? p.nq - grp * QT : (uint32_t)QT;
-    const uint64_t a_policy = p.qgroups > 1 ? ptx::CACHE_EVICT_NORMAL : ptx::CACHE_EVICT_FIRST;
+    const QueryGroup<QT> qg(p);
+    const uint32_t sub = qg.sub, sgrid = qg.sgrid, q0 = qg.q0, qpad_off = qg.qpad_off, nq = qg.nq;
     const uint32_t nslab = p.nslab;  // dimpad / 64
 
     if (warp == 0 && lane == 0) {
         ptx::prefetch_tensormap(&map_rows);
         ptx::prefetch_tensormap(&map_q);
-        // a stage is free again once every consumer warp has seen its MMAs complete
-        for (int i = 0; i < ASTAGES; ++i) { ptx::mbar_init(&sh.afull[i], 1); ptx::mbar_init(&sh.aempty[i], EPI_WARPS); }
-        for (int i = 0; i < C::BSTAGES; ++i) { ptx::mbar_init(&sh.bfull[i], 1); ptx::mbar_init(&sh.bempty[i], EPI_WARPS); }
         sh.maxxx = 0u; sh.max_ra = 0u; sh.max_rb = 0u;
-        ptx::fence_barrier_init();
+        sh.ring.init(C::BSTAGES);
     }
     if (tid < QT) {
-        // start threshold: the caller's score floor and, when the prep kernel sampled the shard, a lower bound of the
-        // query's k-th best score (no flood tiles then)
-        float t0 = p.min_score;
-        if (p.presampled && (uint32_t)tid < nq) {
-            const uint32_t g = __ldcg(p.gtau + q0 + tid);
-            if (g) t0 = fmaxf(t0, ord_to_float(g));
-        }
-        sh.tau[tid] = t0;
+        sh.tau[tid] = start_tau(p, q0, tid, nq);
         sh.cnt[tid] = 0;
         sh.qn[tid] = p.qnorm[qpad_off + tid];
         sh.qa[tid] = p.qa[qpad_off + tid];
@@ -217,50 +168,49 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
     }
     __syncthreads();
     const bool flood = !p.presampled;  // first two tiles: every (row, query) pair is placed directly
-    if (prof && tid == 0) g_sb_prof[blockIdx.x][1] = sb_now();
+    if (prof && tid == 0) g_sb_prof[blockIdx.x][1] = globaltimer_ns();
+    const bool cosine = p.metric == NK_METRIC_COSINE;
+    uint64_t *my_cand = p.cand + (size_t)blockIdx.x * QT * PB;
+    auto prune = [&](uint32_t qi, uint64_t *out, int out_len, int max_keep, float floor_tau, int *gcount) {
+        const float margin2 = bf16_margin2(p.metric, __uint_as_float(sh.max_ra), cosine ? 1.0f : __uint_as_float(sh.max_rb),
+                                           __uint_as_float(sh.maxxx), sh.qa[qi], sh.qb[qi], sh.qn[qi]);
+        // the select's cost is the register-resident key count: an early-trigger prune holds ~260-300 keys, not PB
+        uint64_t *c = my_cand + (size_t)qi * PB;
+        const int have = sh.cnt[qi];
+        if (have <= 320)
+            warp_prune<10>(c, &sh.cnt[qi], &sh.tau[qi], p.k, lane, out, out_len, true, margin2, max_keep, floor_tau, gcount, p.flags + FLAG_OVERFLOW);
+        else if (have <= 512)
+            warp_prune<16>(c, &sh.cnt[qi], &sh.tau[qi], p.k, lane, out, out_len, true, margin2, max_keep, floor_tau, gcount, p.flags + FLAG_OVERFLOW);
+        else
+            warp_prune<PRUNE_LANE>(c, &sh.cnt[qi], &sh.tau[qi], p.k, lane, out, out_len, true, margin2, max_keep, floor_tau, gcount,
+                                   p.flags + FLAG_OVERFLOW);
+    };
 
     if (warp == 0) {
         // ===================================== TMA producer: shadow slabs =========================
-        uint32_t g = 0;
-        for (uint32_t tile = sub; tile < num_tiles; tile += sgrid) {
-            for (uint32_t j = 0; j < nslab; ++j, ++g) {
-                const uint32_t s = g % ASTAGES;
-                ptx::mbar_wait(&sh.aempty[s], ((g / ASTAGES) & 1) ^ 1);
-                if (ptx::elect_one_sync()) {
-                    ptx::mbar_arrive_expect_tx(&sh.afull[s], A_BYTES);
-                    ptx::tma_load_2d(&map_rows, &sh.afull[s], a_base + (size_t)s * A_BYTES, (int32_t)(j * BKB), (int32_t)(tile * ROWS), a_policy);
-                }
-                __syncwarp();
-            }
-        }
+        tma_producer<ASTAGES>(sh.ring.aempty, sub, num_tiles, sgrid, 1, nslab, false, [&](uint32_t s, uint32_t tile, uint32_t, uint32_t j) {
+            ptx::mbar_arrive_expect_tx(&sh.ring.afull[s], A_BYTES);
+            ptx::tma_load_2d(&map_rows, &sh.ring.afull[s], a_base + (size_t)s * A_BYTES, (int32_t)(j * BKB), (int32_t)(tile * ROWS), qg.a_policy);
+        });
     } else if (warp == 3) {
         // ===================================== TMA producer: query slabs (L2-resident) ===========
-        uint32_t g = 0;
-        for (uint32_t tile = sub; tile < num_tiles; tile += sgrid) {
-            for (uint32_t j = 0; j < nslab; ++j, ++g) {
-                const uint32_t s = g % C::BSTAGES;
-                ptx::mbar_wait(&sh.bempty[s], ((g / C::BSTAGES) & 1) ^ 1);
-                if (ptx::elect_one_sync()) {
-                    ptx::mbar_arrive_expect_tx(&sh.bfull[s], C::B_BYTES);
-                    ptx::tma_load_2d(&map_q, &sh.bfull[s], b_base + (size_t)s * C::B_BYTES, (int32_t)(j * BKB), (int32_t)qpad_off, ptx::CACHE_EVICT_LAST);
-                }
-                __syncwarp();
-            }
-        }
+        tma_producer<C::BSTAGES>(sh.ring.bempty, sub, num_tiles, sgrid, 1, nslab, false, [&](uint32_t s, uint32_t, uint32_t, uint32_t j) {
+            ptx::mbar_arrive_expect_tx(&sh.ring.bfull[s], C::B_BYTES);
+            ptx::tma_load_2d(&map_q, &sh.ring.bfull[s], b_base + (size_t)s * C::B_BYTES, (int32_t)(j * BKB), (int32_t)qpad_off, ptx::CACHE_EVICT_LAST);
+        });
     } else if (warp >= EPI_WARP0) {
         // ===================================== consumers: MMA + epilogue ===========================
         // warpgroup m owns rows [128 m, 128 m + 128) of the tile as two m64 halves h; thread = 4 rows x QT/4 columns of
         // the accumulator fragments: rows rbase + 64 h + 8 r, columns cbase + 8 (j / 2) + j % 2
         const uint32_t ewarp = warp - EPI_WARP0, m = ewarp >> 2, wq = ewarp & 3;
         const uint32_t rbase = m * 128 + wq * 16 + ((uint32_t)lane >> 2), cbase = 2u * ((uint32_t)lane & 3u);
-        uint64_t *my_cand = p.cand + (size_t)blockIdx.x * QT * PB;
         // capacity rule: a buffer must be prunable below PB - ROWS, or the next tile could overflow it.  Prunes are TRIGGERED
         // much earlier: an early, tight threshold keeps the buffers short, so the emission at the end of the launch needs no
         // selection and the finish step reads short lists (small shards: 26 tiles per CTA at N = 1M would otherwise never
         // prune at all).
         const int prune_at = PB - ROWS;
-        const int prune_trigger = p.prune_trigger > 0 ? min(prune_at, p.prune_trigger) : min(prune_at, max(192, 4 * (int)p.k));
-        const bool cosine = p.metric == NK_METRIC_COSINE, euclid = p.metric == NK_METRIC_EUCLIDEAN;
+        const int prune_trigger = min(prune_at, max(192, 4 * (int)p.k));
+        const bool euclid = p.metric == NK_METRIC_EUCLIDEAN;
         const bool op_f16 = p.op_f16 != 0;
         const bool eprof = prof && ewarp == 0 && lane == 0;
         unsigned long long t_prune = 0, t_wait = 0, t_a = 0;
@@ -271,12 +221,12 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             for (int i = 0; i < QT / 2; ++i) acc[h][i] = 0.0f;
         uint32_t g = 0, it = 0;
         for (uint32_t tile = sub; tile < num_tiles; tile += sgrid, ++it) {
-            if (eprof) t_a = sb_now();
+            if (eprof) t_a = globaltimer_ns();
             uint32_t prev_sa = 0, prev_sb = 0;
             for (uint32_t j = 0; j < nslab; ++j, ++g) {
                 const uint32_t sa = g % ASTAGES, sbq = g % C::BSTAGES;
-                ptx::mbar_wait(&sh.bfull[sbq], (g / C::BSTAGES) & 1);
-                ptx::mbar_wait(&sh.afull[sa], (g / ASTAGES) & 1);
+                ptx::mbar_wait(&sh.ring.bfull[sbq], (g / C::BSTAGES) & 1);
+                ptx::mbar_wait(&sh.ring.afull[sa], (g / ASTAGES) & 1);
                 const uint64_t bdesc = ptx::make_smem_desc_sw128(ptx::smem_u32(b_base + (size_t)sbq * C::B_BYTES));
                 const uint32_t abase = ptx::smem_u32(a_base + (size_t)sa * A_BYTES + (size_t)m * (A_BYTES / 2));
                 ptx::wgmma_fence();
@@ -291,7 +241,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                 if (j > 0) {  // the previous slab's MMAs are done while this slab's run: its stages go back to the producers
                     ptx::wgmma_wait_one();
                     __syncwarp();
-                    if (lane == 0) { ptx::mbar_arrive(&sh.aempty[prev_sa]); ptx::mbar_arrive(&sh.bempty[prev_sb]); }
+                    if (lane == 0) { ptx::mbar_arrive(&sh.ring.aempty[prev_sa]); ptx::mbar_arrive(&sh.ring.bempty[prev_sb]); }
                 }
                 prev_sa = sa;
                 prev_sb = sbq;
@@ -300,9 +250,9 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             ptx::fence_acc(acc[0]);
             ptx::fence_acc(acc[1]);
             __syncwarp();
-            if (lane == 0) { ptx::mbar_arrive(&sh.aempty[prev_sa]); ptx::mbar_arrive(&sh.bempty[prev_sb]); }
+            if (lane == 0) { ptx::mbar_arrive(&sh.ring.aempty[prev_sa]); ptx::mbar_arrive(&sh.ring.bempty[prev_sb]); }
             if (eprof) {
-                const unsigned long long t = sb_now();
+                const unsigned long long t = globaltimer_ns();
                 t_wait += t - t_a;
                 if (it == 0) g_sb_prof[blockIdx.x][2] = t;
             }
@@ -313,128 +263,47 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                 const uint32_t h = ri >> 1, r = ri & 1;
                 const uint32_t rt = rbase + 64 * h + 8 * r;  // row within the tile
                 const uint32_t row = tile * ROWS + rt;
-                const bool alive = row < p.n && (!p.mask || ((__ldg(p.mask + (row >> 5)) >> (row & 31)) & 1u));
-                // the buffered key is the UPPER bound of the score, bound(row, q) = ra qa[q] + rb qb[q]:
-                //   cosine     acc/|x|                        ra = |dx|/|x|   rb = 1
-                //   dot        acc                            ra = |dx|       rb = |x|
-                //   euclidean  -(|x|^2 + |q|^2 - 2 acc)        ra = 2|dx|      rb = 2|x|   (+ eps (|x|^2 + |q|^2))
-                const float x2 = row < p.n ? __ldg(p.xnorm2 + row) : 0.0f;
-                const float xn = sqrtf(x2);
+                const bool alive = row_alive(p, row);
+                Bf16Est est;
+                est.x2 = row < p.n ? __ldg(p.xnorm2 + row) : 0.0f;
+                est.qa = sh.qa;
+                est.qb = sh.qb;
+                est.qn = sh.qn;
+                est.euclid = euclid;
+                const float xn = sqrtf(est.x2);
                 const float dxn = sqrtf((row < p.n && p.dnorm2) ? __ldg(p.dnorm2 + row) : 0.0f) * 1.0001f;  // 16-bit corpus: no residue
-                float mul = 1.0f, ra = dxn, rb = xn;
+                est.mul = 1.0f; est.ra = dxn; est.rb = xn;
                 if (cosine) {
-                    mul = x2 > 0.0f ? 1.0f / xn : 0.0f;
-                    ra = dxn * mul * 1.000001f;
-                    rb = 1.0f;
+                    est.mul = est.x2 > 0.0f ? 1.0f / xn : 0.0f;
+                    est.ra = dxn * est.mul * 1.000001f;
+                    est.rb = 1.0f;
                 } else if (euclid) {
-                    mul = 2.0f; ra = 2.0f * dxn; rb = 2.0f * xn;
+                    est.mul = 2.0f; est.ra = 2.0f * dxn; est.rb = 2.0f * xn;
                 }
-                if ((lane & 3) == 0 && alive && ra < INFINITY && rb < INFINITY) {  // NaN / Inf rows are kept anyway (score NaN -> +inf below)
-                    atomicMax(&sh.max_ra, __float_as_uint(ra));
-                    if (!cosine) { atomicMax(&sh.max_rb, __float_as_uint(rb)); atomicMax(&sh.maxxx, __float_as_uint(x2)); }
+                if ((lane & 3) == 0 && alive && est.ra < INFINITY && est.rb < INFINITY) {  // NaN / Inf rows are kept anyway (score NaN -> +inf)
+                    atomicMax(&sh.max_ra, __float_as_uint(est.ra));
+                    if (!cosine) { atomicMax(&sh.max_rb, __float_as_uint(est.rb)); atomicMax(&sh.maxxx, __float_as_uint(est.x2)); }
                 }
-                float v[QT / 4];
-#pragma unroll
-                for (int jj = 0; jj < QT / 4; ++jj) v[jj] = acc[h][(jj >> 1) * 4 + r * 2 + (jj & 1)];
-                if (DUMP && row < p.n) {  // tests only: score estimate and error bound per (row, query)
-#pragma unroll
-                    for (int jj = 0; jj < QT / 4; ++jj) {
-                        const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
-                        if (qi >= nq) continue;
-                        const float qn = sh.qn[qi];
-                        float est = v[jj] * mul, b = fmaf(ra, sh.qa[qi], rb * sh.qb[qi]);
-                        if (euclid) { est -= fmaf(qn, qn, x2); b += EUC_EPS * fmaf(qn, qn, x2); }
-                        p.dump_est[(size_t)row * p.dump_ld + q0 + qi] = est;
-                        p.dump_bnd[(size_t)row * p.dump_ld + q0 + qi] = b;
-                    }
-                }
-                if (flood && it < 2) {
-                    // Flood tiles: until the first prune every threshold is -inf and EVERY (row, query) pair is buffered:
-                    // place them directly (slot = tile-local row), no atomics, no register select.
-                    const uint32_t slot = it * ROWS + rt;
-                    const uint32_t grow = (uint32_t)(p.row_base + row);
-#pragma unroll
-                    for (int jj = 0; jj < QT / 4; ++jj) {
-                        const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
-                        if (qi < nq) {
-                            float sc = fmaf(v[jj], mul, fmaf(ra, sh.qa[qi], rb * sh.qb[qi]));
-                            if (euclid) { const float qn = sh.qn[qi]; sc -= EUC_KEEP * fmaf(qn, qn, x2); }
-                            if (sc != sc) sc = INFINITY;
-                            my_cand[(size_t)qi * PB + slot] = (alive && sc >= p.min_score) ? make_key(sc, grow) : 0ull;  // 0 = empty slot
-                        }
-                    }
-                } else if (alive) {
-                    // compact compare pass -> mask of columns worth buffering (NaN passes); rare pushes out of line
-                    uint32_t pass = 0;
-#pragma unroll
-                    for (int jj = 0; jj < QT / 4; ++jj) {
-                        const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
-                        float s0 = fmaf(v[jj], mul, fmaf(ra, sh.qa[qi], rb * sh.qb[qi]));
-                        if (euclid) { const float qn = sh.qn[qi]; s0 -= EUC_KEEP * fmaf(qn, qn, x2); }
-                        pass |= (!(s0 < sh.tau[qi]) && qi < nq) ? (1u << jj) : 0u;
-                    }
-#pragma unroll 1
-                    while (pass) {
-                        const uint32_t c = (uint32_t)__ffs((int)pass) - 1u;
-                        pass &= pass - 1u;
-                        float val = 0.0f;
-#pragma unroll
-                        for (uint32_t i = 0; i < (uint32_t)(QT / 4); ++i)  // the register file is not indexable: select by compare
-                            if (c == i) val = v[i];
-                        const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
-                        float sc = fmaf(val, mul, fmaf(ra, sh.qa[qi], rb * sh.qb[qi]));
-                        if (euclid) { const float qn = sh.qn[qi]; sc -= EUC_KEEP * fmaf(qn, qn, x2); }
-                        if (sc != sc) sc = INFINITY;  // undecidable here: keep it, the exact rescoring judges
-                        if (sc >= sh.tau[qi]) {
-                            int pos = atomicAdd(&sh.cnt[qi], 1);
-                            if (pos < PB) my_cand[(size_t)qi * PB + pos] = make_key(sc, (uint32_t)(p.row_base + row));
-                            else atomicExch(p.flags, 1);
-                        }
-                    }
-                }
+                keep_fragment_row<QT, PB, true, DUMP>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau, sh.qn, sh.cnt, my_cand);
             }
             // prune any buffer that could overflow during the next tile (8 warps, different queries concurrently)
             group_sync(EPI_BAR, EPI_NT);  // every push of this tile is visible
-            if (eprof) t_a = sb_now();
-            // (never between the two flood tiles: the second one is placed by slot, behind the first one's 256 entries)
-            for (uint32_t qi = ewarp; qi < nq; qi += EPI_WARPS)
-                if (sh.cnt[qi] > prune_trigger && !(flood && it == 0)) {
-                    if (eprof && g_sb_prof[blockIdx.x][6] == ~0ull) g_sb_prof[blockIdx.x][6] = it;
-                    const float margin2 = bf16_margin2(p.metric, __uint_as_float(sh.max_ra), cosine ? 1.0f : __uint_as_float(sh.max_rb),
-                                                       __uint_as_float(sh.maxxx), sh.qa[qi], sh.qb[qi], sh.qn[qi]);
-                    float floor_tau = p.min_score;
-                    const uint32_t gt = __ldcg(p.gtau + q0 + qi);
-                    if (gt) floor_tau = fmaxf(floor_tau, ord_to_float(gt));
-                    // the select's cost is the register-resident key count: an early-trigger prune holds ~260-300 keys, not PB
-                    const int have = sh.cnt[qi];
-                    if (have <= 320)
-                        warp_prune<10>(my_cand + (size_t)qi * PB, &sh.cnt[qi], &sh.tau[qi], p.k, lane, nullptr, 0, true, margin2, prune_at, floor_tau,
-                                       nullptr, p.flags + FLAG_OVERFLOW);
-                    else if (have <= 512)
-                        warp_prune<16>(my_cand + (size_t)qi * PB, &sh.cnt[qi], &sh.tau[qi], p.k, lane, nullptr, 0, true, margin2, prune_at, floor_tau,
-                                       nullptr, p.flags + FLAG_OVERFLOW);
-                    else
-                        warp_prune<PRUNE_LANE>(my_cand + (size_t)qi * PB, &sh.cnt[qi], &sh.tau[qi], p.k, lane, nullptr, 0, true, margin2, prune_at, floor_tau,
-                                               nullptr, p.flags + FLAG_OVERFLOW);
-                    // everything inside the margin must fit below prune_at, or the next tile could overflow the buffer
-                    if (lane == 0 && sh.cnt[qi] >= prune_at) atomicOr(p.flags + FLAG_OVERFLOW, 1);
-                    if (lane == 0 && sh.tau[qi] > -INFINITY) atomicMax(p.gtau + q0 + qi, ord_bits(sh.tau[qi]));
-                }
+            if (eprof) t_a = globaltimer_ns();
+            prune_tile<true>(p, q0, nq, ewarp, lane, sh.cnt, sh.tau, prune_trigger, prune_at, flood && it == 0,
+                             [&](uint32_t qi, uint64_t *out, int out_len, int max_keep, float floor_tau, int *gcount) {
+                                 if (eprof && g_sb_prof[blockIdx.x][6] == ~0ull) g_sb_prof[blockIdx.x][6] = it;
+                                 prune(qi, out, out_len, max_keep, floor_tau, gcount);
+                             });
             group_sync(EPI_BAR, EPI_NT);
-            if (eprof) t_prune += sb_now() - t_a;
-            for (uint32_t qi = tid - EPI_WARP0 * 32; qi < nq; qi += EPI_NT) {  // adopt the shared thresholds
-                const uint32_t gt = __ldcg(p.gtau + q0 + qi);
-                if (gt) sh.tau[qi] = fmaxf(sh.tau[qi], ord_to_float(gt));
-            }
+            if (eprof) t_prune += globaltimer_ns() - t_a;
+            adopt_shared_tau(p, q0, nq, tid - EPI_WARP0 * 32, sh.tau);
         }
-        if (eprof) { g_sb_prof[blockIdx.x][3] = sb_now(); g_sb_prof[blockIdx.x][5] = t_prune; g_sb_prof[blockIdx.x][7] = t_wait; }
+        if (eprof) { g_sb_prof[blockIdx.x][3] = globaltimer_ns(); g_sb_prof[blockIdx.x][5] = t_prune; g_sb_prof[blockIdx.x][7] = t_wait; }
     }
 
     // ---- emit: everything inside this CTA's margin AND above the shared threshold goes to the query's shared list.
     __syncthreads();
     {
-        const bool cosine = p.metric == NK_METRIC_COSINE;
-        uint64_t *my_cand = p.cand + (size_t)blockIdx.x * QT * PB;
         // Fast path (buffers with <= k_emit entries, i.e. almost always all of them): no selection, the finish kernel selects
         // globally — append what still reaches the current threshold.  The buffers live in global memory (L2); walking them
         // query by query was a chain of dependent round trips (~19 us at the end of every launch, measured).  Instead: the
@@ -442,7 +311,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
         // independent loads in flight per warp, then the list-fill atomics of the whole batch in one more round.
         constexpr int NW = NTHREADS / 32, JQ = (QT + NW - 1) / NW;
         constexpr int STAGE_CHUNKS = Cfg<QT>::RING_BYTES / 256;  // 32-key chunks the (contiguous) operand rings hold
-        if (prof && tid == 0) g_sb_prof[blockIdx.x][8] = sb_now();
+        if (prof && tid == 0) g_sb_prof[blockIdx.x][8] = globaltimer_ns();
         int n_emitted = 0;
         if (tid < QT) {
             // (the shared threshold is fetched asynchronously: its round trip — several microseconds while the other CTAs
@@ -477,7 +346,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             // The operand rings are idle now (every MMA has completed: the epilogue saw the last accumulator): stage the live
             // chunks there with asynchronous copies — every load of the warp in flight at once, no registers held.  Chunk
             // c of query q lands in stage slot eoff[q] + c; queries whose chunks do not fit the rings take the per-query path.
-            if (prof && tid == 0) g_sb_prof[blockIdx.x][12] = sb_now();  // prefix done
+            if (prof && tid == 0) g_sb_prof[blockIdx.x][12] = globaltimer_ns();  // prefix done
             uint64_t *stage = reinterpret_cast<uint64_t *>(a_base);
             for (uint32_t qi = warp; qi < nq; qi += NW) {
                 const int c0 = sh.eoff[qi], c1 = sh.eoff[qi + 1], n = sh.cnt[qi];
@@ -500,7 +369,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                 sh.ethr[tid] = t > -INFINITY ? ord_bits(t) : 0u;
             }
             __syncthreads();
-            if (prof && tid == 0) g_sb_prof[blockIdx.x][13] = sb_now();  // staged
+            if (prof && tid == 0) g_sb_prof[blockIdx.x][13] = globaltimer_ns();  // staged
             // survivors per query (pass A), ONE list-fill atomic per query — lane j owns the warp's j-th query, all of them
             // in one round trip — then the stores (pass B)
             int my = 0;
@@ -520,7 +389,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             }
             int off = 0;
             if (my > 0) off = atomicAdd(p.gcount + q0 + warp + lane * NW, my);
-            if (prof && tid == 0) g_sb_prof[blockIdx.x][14] = sb_now() + (off & 0);  // list-fill atomics answered
+            if (prof && tid == 0) g_sb_prof[blockIdx.x][14] = globaltimer_ns() + (off & 0);  // list-fill atomics answered
 #pragma unroll
             for (int j = 0; j < JQ; ++j) {
                 const uint32_t qi = warp + j * NW;
@@ -540,36 +409,19 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                     n_emitted += __popc(m);
                 }
             }
-            if (prof && tid == 0) { g_sb_prof[blockIdx.x][9] = sb_now(); g_sb_prof[blockIdx.x][10] = (unsigned long long)sh.eoff[QT]; g_sb_prof[blockIdx.x][11] = (unsigned long long)n_emitted; }
+            if (prof && tid == 0) { g_sb_prof[blockIdx.x][9] = globaltimer_ns(); g_sb_prof[blockIdx.x][10] = (unsigned long long)sh.eoff[QT]; g_sb_prof[blockIdx.x][11] = (unsigned long long)n_emitted; }
         }
         for (uint32_t qi = warp; qi < nq; qi += NW) {  // buffers beyond k_emit (near-tie data): select, then emit
             if (sh.cnt[qi] <= (int)p.k_emit && sh.eoff[qi + 1] <= STAGE_CHUNKS) continue;
-            const float margin2 = bf16_margin2(p.metric, __uint_as_float(sh.max_ra), cosine ? 1.0f : __uint_as_float(sh.max_rb),
-                                               __uint_as_float(sh.maxxx), sh.qa[qi], sh.qb[qi], sh.qn[qi]);
-            float floor_tau = p.min_score;
-            const uint32_t gt = __ldcg(p.gtau + q0 + qi);
-            if (gt) floor_tau = fmaxf(floor_tau, ord_to_float(gt));
-            if (sh.cnt[qi] <= (int)p.k_emit) {  // (did not fit the staging area)
-                const float t = fmaxf(sh.tau[qi], floor_tau);
-                uint64_t thr = t > -INFINITY ? (uint64_t)ord_bits(t) << 32 : 1ull;
-                if (thr == 0ull) thr = 1ull;
-                warp_emit_above(my_cand + (size_t)qi * PB, sh.cnt[qi], thr, lane, p.partial + (size_t)(q0 + qi) * p.list_cap,
-                                (int)p.list_cap, p.gcount + q0 + qi);
-                continue;
-            }
-            warp_prune<PRUNE_LANE>(my_cand + (size_t)qi * PB, &sh.cnt[qi], &sh.tau[qi], p.k, lane,
-                           p.partial + (size_t)(q0 + qi) * p.list_cap, (int)p.list_cap, true, margin2,
-                           (int)p.k_emit, floor_tau, p.gcount + q0 + qi, p.flags + FLAG_OVERFLOW);
-            if (lane == 0 && sh.cnt[qi] >= (int)p.k_emit && (int)p.k_emit > (int)p.k) atomicOr(p.flags + FLAG_OVERFLOW, 2);
-            if (lane == 0 && sh.tau[qi] > -INFINITY) atomicMax(p.gtau + q0 + qi, ord_bits(sh.tau[qi]));
+            emit_query(p, q0, qi, lane, my_cand + (size_t)qi * PB, sh.cnt, sh.tau, prune);  // (or did not fit the staging area)
         }
         if (tid == 0) {
-            atomicMax(reinterpret_cast<unsigned int *>(p.flags + 2), sh.maxxx);
-            atomicMax(reinterpret_cast<unsigned int *>(p.flags + 4), sh.max_ra);
-            atomicMax(reinterpret_cast<unsigned int *>(p.flags + 6), cosine ? __float_as_uint(1.0f) : sh.max_rb);
+            atomicMax(reinterpret_cast<unsigned int *>(p.flags + FLAG_MAXXX), sh.maxxx);
+            atomicMax(reinterpret_cast<unsigned int *>(p.flags + FLAG_MAX_RA), sh.max_ra);
+            atomicMax(reinterpret_cast<unsigned int *>(p.flags + FLAG_MAX_RB), cosine ? __float_as_uint(1.0f) : sh.max_rb);
         }
     }
-    if (prof && tid == 0) g_sb_prof[blockIdx.x][4] = sb_now();
+    if (prof && tid == 0) g_sb_prof[blockIdx.x][4] = globaltimer_ns();
 }
 
 static void sb_print_prof(cudaStream_t stream, uint32_t grid) {
@@ -611,16 +463,6 @@ bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a) {
     return a.dim % 8 == 0;  // 16-bit rows: 16-byte TMA row stride and 128-bit exact re-scoring loads
 }
 
-// Host: stand-alone bf16 conversion of a query block (assign_tensor.cu: the centroids).
-int bf16_prep_queries(const ScanArgs &a, uint32_t Qpad, uint32_t dimpad, float acc_c, void *qbf16, float *qnorm, float *qa,
-                      float *qb, uint64_t *launches) {
-    bf16_prep_queries_kernel<<<Qpad, 256, 0, a.stream>>>(a.queries, a.Q, a.dim, dimpad, a.metric == NK_METRIC_COSINE, acc_c,
-                                                         static_cast<uint16_t *>(qbf16), qnorm, qa, qb);
-    NK_CUDA_OK(cudaGetLastError());
-    if (launches) ++*launches;
-    return 0;
-}
-
 template <int QT, bool DUMP>
 static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
     using namespace sb;
@@ -636,16 +478,8 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
         return -1;
     }
     if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, DUMP>), di.device_id, smem)) return -1;
-    tc::Params p{};
-    p.n = a.n; p.dim = a.dim; p.nslab = sp.dimpad / BKB; p.row_base = a.row_base;
-    p.q0 = sp.q0; p.nq = sp.nq; p.k = a.k; p.qpad_off = sp.q0; p.qgroups = sp.qgroups; p.list_cap = sp.grid * sp.k_emit;
-    p.metric = a.metric; p.k_emit = sp.k_emit; p.margin_c = 0.0f; p.qnorm = sp.qnorm; p.qa = sp.qa; p.qb = sp.qb;
-    p.xnorm2 = a.xnorm2; p.dnorm2 = a.dnorm2;
-    p.cand = ws.cand; p.partial = ws.partial; p.flags = ws.flags; p.only_if = nullptr; p.debug = tc_debug_flags(); p.mask = a.row_mask;
-    p.gtau = reinterpret_cast<uint32_t *>(ws.keys2); p.gcount = reinterpret_cast<int *>(ws.keys2) + (sp.Qpad + QT_BIG);
-    p.presampled = sp.presampled; p.min_score = a.min_score; p.op_f16 = a.dtype == NK_DTYPE_F16;
-    p.prune_trigger = tc_env_int("NK_PRUNE_TRIGGER", 0);
-    p.dump_est = sp.dump_est; p.dump_bnd = sp.dump_bnd; p.dump_ld = sp.dump_ld;
+    tc::Params p = pass_params(a, ws, sp);
+    p.nslab = sp.dimpad / BKB; p.qa = sp.qa; p.qb = sp.qb; p.xnorm2 = a.xnorm2; p.dnorm2 = a.dnorm2; p.op_f16 = a.dtype == NK_DTYPE_F16;
     knn_scan_shadow_kernel<QT, DUMP><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
     NK_CUDA_OK(cudaGetLastError());
     if (launches) ++*launches;

@@ -1,9 +1,13 @@
-// scan_tensor_shared.cuh — declarations shared by the tensor-core scan kernels (scan_tensor.cu: TF32 exact / filter over
-// the fp32 rows, scan_tensor_shadow.cu: BF16 filter over the shadow corpus) and their common finish step.
+// scan_tensor_shared.cuh — what the tensor-core scan kernels (scan_tensor.cu: TF32 exact / filter over the fp32 rows,
+// scan_tensor_shadow.cu: BF16 filter over the shadow corpus; assign_tensor.cu: k-means assignment) share: parameters,
+// set-up, the TMA producer loop and the filter epilogue (keep rule, per-tile prune / publish / adopt, emission fallback).
 #pragma once
 #include <cuda.h>
 
 #include "kernels.cuh"
+#ifdef __CUDACC__
+#include "ptx_sm90.cuh"
+#endif
 
 namespace nk {
 
@@ -26,6 +30,8 @@ enum {
 };
 namespace tc {
 constexpr int THREADS = 384;
+constexpr int ROWS = 256;        // corpus rows per tile (2 M-tiles of 128)
+constexpr int MAX_BSTAGES = 8;   // deepest query-slab ring
 constexpr int BK = 32;           // floats per corpus K-slab = one 128-byte swizzle row
 constexpr int EPI_THREADS = 256; // the two consumer warpgroups
 constexpr int EPI_BAR = 1;       // named barrier of the consumers (2, 3: one per warpgroup)
@@ -56,7 +62,6 @@ struct Params {
     const int *only_if;       // exact fallback: run only if *only_if != 0
     const uint32_t *mask;     // row bitmask (bit set = row takes part) or nullptr
     int debug;                // NK_TC_DEBUG bit 64: clock64 wait-time instrumentation of CTA 0
-    int prune_trigger;        // 16-bit pass: early prune trigger override (NK_PRUNE_TRIGGER, 0 = default)
     int presampled;           // filter: gtau[] already holds a sampled lower bound of every query's k-th best score
                               // (filter_prep_kernel): no flood tiles, thresholds are adopted at kernel start
     float min_score;          // filter: caller's score floor (VectorIndex minSimilarity, vector_index.go:339-352): rows
@@ -66,6 +71,202 @@ struct Params {
     int op_f16;               // 16-bit kernel: operands are fp16 (an fp16 corpus scanned in place) instead of bf16
 };
 
+// What one scan launch covers: queries [q0, q0+nq) in `qgroups` query groups over a `grid`-CTA launch.  Both kernels'
+// launch arguments extend it; pass_params() turns it into the Params fields they share.
+struct PassArgs {
+    uint32_t grid, k_emit, Qpad, q0, nq, qgroups;
+    const float *qnorm;
+    int presampled;
+    float *dump_est = nullptr, *dump_bnd = nullptr;  // test-only DUMP instantiations
+    uint32_t dump_ld = 0;
+};
+
+#ifdef __CUDACC__
+// mbarriers of the two TMA rings (corpus slabs, query slabs) of a scan kernel; the first member of its shared state.
+template <int ASTAGES> struct Rings {
+    uint64_t afull[ASTAGES], aempty[ASTAGES];
+    uint64_t bfull[MAX_BSTAGES], bempty[MAX_BSTAGES];
+    // a stage is free again once every consumer warp has seen its MMAs complete
+    __device__ __forceinline__ void init(int bstages) {
+        for (int i = 0; i < ASTAGES; ++i) { ptx::mbar_init(&afull[i], 1); ptx::mbar_init(&aempty[i], 8); }
+        for (int i = 0; i < bstages; ++i) { ptx::mbar_init(&bfull[i], 1); ptx::mbar_init(&bempty[i], 8); }
+        ptx::fence_barrier_init();
+    }
+};
+
+// Query groups: CTA b serves query block (b % G) over the tile subset (b / G).  The G sibling CTAs stream the SAME
+// corpus tiles at the same pace, so a tile crosses HBM once and its other G-1 readers hit the 50 MB L2: large
+// batches (Q > 128) stop being bound by re-reading the corpus once per 128 queries.
+template <int QT> struct QueryGroup {
+    uint32_t sub, sgrid, q0, qpad_off, nq;
+    uint64_t a_policy;
+    __device__ __forceinline__ explicit QueryGroup(const Params &p) {
+        const uint32_t grp = blockIdx.x % p.qgroups;
+        sub = blockIdx.x / p.qgroups;
+        sgrid = gridDim.x / p.qgroups;
+        q0 = p.q0 + grp * QT;
+        qpad_off = p.qpad_off + grp * QT;
+        nq = p.nq - grp * QT < (uint32_t)QT ? p.nq - grp * QT : (uint32_t)QT;
+        a_policy = p.qgroups > 1 ? ptx::CACHE_EVICT_NORMAL : ptx::CACHE_EVICT_FIRST;
+    }
+};
+
+// One TMA producer warp: for every tile of this CTA (first, first + step, ..), `reps` passes over its nslab K-slabs
+// through a STAGES-deep ring.  issue(stage, tile, rep, slab) arms the stage's full barrier and starts the copies (one
+// elected lane).  Returns the cycles spent waiting for free stages when prof is set (NK_TC_DEBUG bit 64).
+template <int STAGES, class Issue>
+__device__ __forceinline__ long long tma_producer(uint64_t *empty, uint32_t first, uint32_t num_tiles, uint32_t step, uint32_t reps,
+                                                  uint32_t nslab, bool prof, Issue issue) {
+    long long waited = 0;
+    uint32_t g = 0;
+    for (uint32_t tile = first; tile < num_tiles; tile += step)
+        for (uint32_t rep = 0; rep < reps; ++rep)
+            for (uint32_t j = 0; j < nslab; ++j, ++g) {
+                const uint32_t s = g % STAGES;
+                const long long t0 = prof ? clock64() : 0;
+                ptx::mbar_wait(&empty[s], ((g / STAGES) & 1) ^ 1);
+                if (prof) waited += clock64() - t0;
+                if (ptx::elect_one_sync()) issue(s, tile, rep, j);
+                __syncwarp();
+            }
+    return waited;
+}
+
+// t raised to the query's cross-CTA shared threshold, if any CTA has published one
+__device__ __forceinline__ float with_shared_tau(const uint32_t *gtau_q, float t) {
+    const uint32_t g = __ldcg(gtau_q);
+    return g ? fmaxf(t, ord_to_float(g)) : t;
+}
+// Start threshold of a query: the caller's score floor and, when the prep kernel sampled the shard, a lower bound of the
+// query's k-th best score (no flood tiles then).
+__device__ __forceinline__ float start_tau(const Params &p, uint32_t q0, uint32_t qi, uint32_t nq) {
+    return p.presampled && qi < nq ? with_shared_tau(p.gtau + q0 + qi, p.min_score) : p.min_score;
+}
+__device__ __forceinline__ bool row_alive(const Params &p, uint32_t row) {
+    return row < p.n && (!p.mask || ((__ldg(p.mask + (row >> 5)) >> (row & 31)) & 1u));
+}
+
+// The filter's keep rule for one accumulator fragment row: thread = 1 row x QT/4 query columns cbase + 8 (j / 2) + j % 2
+// of acc (the row's 64-row half), r = which of the half's two fragment rows.  Buffers every (row, query) pair whose score
+// estimate can still reach the query's threshold.  The kernel supplies the estimate: est.upper(v, qi) is the UPPER bound
+// of the score from accumulator value v (exact mode: the score itself), est.bound(qi) its error bound before the
+// euclidean term (DUMP only), est.mul / est.x2 the row's scale and |x|^2.
+//   flood (first two tiles without a sampled threshold): every pair is placed directly at slot = tile-local row;
+//   otherwise a compact compare pass builds the mask of columns worth buffering (NaN passes) and the rare pushes run in a
+//   small out-of-line loop so the hot code stays short.
+// BOUNDED: a NaN estimate is undecidable here, so it is kept as +inf and the exact re-scoring judges; exact mode: -inf.
+template <int QT, int CAP, bool BOUNDED, bool DUMP, class Est>
+__device__ __forceinline__ void keep_fragment_row(const Params &p, const Est &est, const float (&acc)[QT / 2], uint32_t r,
+                                                  uint32_t row, uint32_t rt, bool alive, bool flood, uint32_t it, uint32_t cbase,
+                                                  uint32_t q0, uint32_t nq, const float *tau, const float *qn, int *cnt,
+                                                  uint64_t *cand) {
+    float v[QT / 4];
+#pragma unroll
+    for (int jj = 0; jj < QT / 4; ++jj) v[jj] = acc[(jj >> 1) * 4 + r * 2 + (jj & 1)];
+    if (DUMP && row < p.n) {  // tests only: score estimate and error bound per (row, query)
+#pragma unroll
+        for (int jj = 0; jj < QT / 4; ++jj) {
+            const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
+            if (qi >= nq) continue;
+            const float q = qn[qi];
+            float e = v[jj] * est.mul, b = est.bound(qi);
+            if (p.metric == NK_METRIC_EUCLIDEAN) { e -= fmaf(q, q, est.x2); b += EUC_EPS * fmaf(q, q, est.x2); }
+            p.dump_est[(size_t)row * p.dump_ld + q0 + qi] = e;
+            p.dump_bnd[(size_t)row * p.dump_ld + q0 + qi] = b;
+        }
+    }
+    if (flood && it < 2) {
+        // Until the first prune (after this CTA's second tile) every threshold is -inf and EVERY (row, query) pair is
+        // buffered: no atomics, no register select.
+        const uint32_t slot = it * ROWS + rt;
+        const uint32_t grow = (uint32_t)(p.row_base + row);
+#pragma unroll
+        for (int jj = 0; jj < QT / 4; ++jj) {
+            const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
+            if (qi < nq) {
+                float sc = est.upper(v[jj], qi);
+                if (sc != sc) sc = BOUNDED ? INFINITY : -INFINITY;
+                cand[(size_t)qi * CAP + slot] = (alive && sc >= p.min_score) ? make_key(sc, grow) : 0ull;  // 0 = empty slot
+            }
+        }
+    } else if (alive) {
+        uint32_t pass = 0;
+#pragma unroll
+        for (int jj = 0; jj < QT / 4; ++jj) {
+            const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
+            const float s0 = est.upper(v[jj], qi);
+            pass |= (!(s0 < tau[qi]) && qi < nq) ? (1u << jj) : 0u;
+        }
+#pragma unroll 1
+        while (pass) {
+            const uint32_t c = (uint32_t)__ffs((int)pass) - 1u;
+            pass &= pass - 1u;
+            float val = 0.0f;
+#pragma unroll
+            for (uint32_t i = 0; i < (uint32_t)(QT / 4); ++i)  // the register file is not indexable: select by compare
+                if (c == i) val = v[i];
+            const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
+            float sc = est.upper(val, qi);
+            if (sc != sc) sc = BOUNDED ? INFINITY : -INFINITY;
+            if (sc >= tau[qi]) {
+                int pos = atomicAdd(&cnt[qi], 1);
+                if (pos < CAP) cand[(size_t)qi * CAP + pos] = make_key(sc, (uint32_t)(p.row_base + row));
+                else atomicExch(p.flags + FLAG_FATAL, 1);
+            }
+        }
+    }
+}
+
+// End of a tile, after a barrier that makes every push visible: warp w of the consumers prunes queries w, w + 8, .. whose
+// buffer holds more than `trigger` entries (never between the two flood tiles: the second one is placed by slot, behind
+// the first one's 256 entries).  prune(qi, out, out_len, max_keep, floor_tau, gcount) runs the kernel's warp_prune.
+// Filter mode: everything inside the margin must then fit below prune_at, or the next tile could overflow the buffer; and
+// the new threshold is published: it is a lower bound on the true global k-th best score, so every CTA may filter with
+// the largest one any CTA has found.
+template <bool FILTER, class Prune>
+__device__ __forceinline__ void prune_tile(const Params &p, uint32_t q0, uint32_t nq, uint32_t ewarp, int lane, const int *cnt,
+                                           const float *tau, int trigger, int prune_at, bool between_floods, Prune prune) {
+    if (between_floods) return;
+    for (uint32_t qi = ewarp; qi < nq; qi += EPI_THREADS / 32)
+        if (cnt[qi] > trigger) {
+            prune(qi, nullptr, 0, prune_at, FILTER ? with_shared_tau(p.gtau + q0 + qi, p.min_score) : p.min_score, nullptr);
+            if (FILTER && lane == 0 && cnt[qi] >= prune_at) atomicOr(p.flags + FLAG_OVERFLOW, 1);
+            if (FILTER && lane == 0 && tau[qi] > -INFINITY) atomicMax(p.gtau + q0 + qi, ord_bits(tau[qi]));
+        }
+}
+// After the prunes: adopt the shared thresholds (one L2 read per query per tile), consumer thread etid of EPI_THREADS.
+__device__ __forceinline__ void adopt_shared_tau(const Params &p, uint32_t q0, uint32_t nq, uint32_t etid, float *tau) {
+    for (uint32_t qi = etid; qi < nq; qi += EPI_THREADS)
+        tau[qi] = with_shared_tau(p.gtau + q0 + qi, tau[qi]);
+}
+
+// Filter emission of one query by one warp: everything inside this CTA's margin AND above the shared threshold goes to the
+// query's shared list.  Few entries (<= k_emit): no local selection, the finish kernel selects globally — append what still
+// reaches the current threshold.  Otherwise select with the margin, and flag the exact fallback when the list was cut at
+// k_emit while rows inside the margin remained.
+template <class Prune>
+__device__ __forceinline__ void emit_query(const Params &p, uint32_t q0, uint32_t qi, int lane, const uint64_t *cand, const int *cnt,
+                                           const float *tau, Prune prune) {
+    const float floor_tau = with_shared_tau(p.gtau + q0 + qi, p.min_score);
+    uint64_t *list = p.partial + (size_t)(q0 + qi) * p.list_cap;
+    if (cnt[qi] <= (int)p.k_emit) {
+        const float t = fmaxf(tau[qi], floor_tau);
+        uint64_t thr = t > -INFINITY ? (uint64_t)ord_bits(t) << 32 : 1ull;
+        if (thr == 0ull) thr = 1ull;
+        warp_emit_above(cand, cnt[qi], thr, lane, list, (int)p.list_cap, p.gcount + q0 + qi);
+        return;
+    }
+    prune(qi, list, (int)p.list_cap, (int)p.k_emit, floor_tau, p.gcount + q0 + qi);
+    if (lane == 0 && cnt[qi] >= (int)p.k_emit && (int)p.k_emit > (int)p.k) atomicOr(p.flags + FLAG_OVERFLOW, 2);
+    if (lane == 0 && tau[qi] > -INFINITY) atomicMax(p.gtau + q0 + qi, ord_bits(tau[qi]));
+}
+
+__device__ __forceinline__ unsigned long long globaltimer_ns() {
+    unsigned long long t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)::"memory");
+    return t;
+}
+#endif
 
 }  // namespace tc
 
@@ -100,20 +301,42 @@ const CUtensorMap *tc_cached_map(Workspace &ws, int slot, const void *base, uint
                                  uint32_t box_cols, uint32_t box_rows, uint64_t row_stride_bytes, int map_dtype = 0);
 int tc_env_int(const char *name, int dflt);  // getenv once per name (read at first use)
 
+// The Params fields every scan launch fills the same way (scan_tensor.cu)
+tc::Params pass_params(const ScanArgs &a, Workspace &ws, const tc::PassArgs &t);
+
 // BF16 shadow filter pass (scan_tensor_shadow.cu): queries [q0, q0+nq), nq <= qgroups * qt, qt = 64 or 128.
-struct ShadowPassArgs {
-    uint32_t grid, k_emit, dimpad, Qpad, q0, nq, qgroups;
+struct ShadowPassArgs : tc::PassArgs {
+    uint32_t dimpad;
     const void *qbf16;
-    const float *qnorm, *qa, *qb;
-    int presampled;
-    float *dump_est = nullptr, *dump_bnd = nullptr;  // test-only DUMP instantiation
-    uint32_t dump_ld = 0;
+    const float *qa, *qb;
 };
 int launch_shadow_pass(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches);
 bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a);
-// stand-alone bf16 conversion of a query block (k-means assignment: centroids as "queries")
-int bf16_prep_queries(const ScanArgs &a, uint32_t Qpad, uint32_t dimpad, float acc_c, void *qbf16, float *qnorm, float *qa,
-                      float *qb, uint64_t *launches);
+
+// Query preparation (filter_prep_kernel, scan_tensor.cu), one CTA per padded query row.
+struct PrepParams {
+    const float *q;
+    uint32_t Q, dim, dimpad;
+    int normalise, metric;
+    float acc_c;
+    float *qhi, *qlo;      // [Qpad x dim] (nullable)
+    uint16_t *qbf;         // [Qpad x dimpad] (nullable); fp16 bits when qbf_f16
+    int qbf_f16;
+    float *qnorm, *qa, *qb;
+    uint32_t *state;       // gtau[QA] then gcount[QA] (nullable)
+    uint32_t Qpad, QA;
+    int *flags;
+    // sampled initial threshold (sample == 0: none)
+    const void *rows;
+    int dtype;
+    uint32_t n, sample, k;
+    const uint32_t *mask;
+    float min_score;
+    const int *only_if;
+};
+// The fields taken from the search arguments: the queries, the metric and the shard (for the sample).
+PrepParams prep_params(const ScanArgs &a, uint32_t Qpad, uint32_t dimpad);
+int launch_prep(const DeviceInfo &di, const PrepParams &pp, cudaStream_t stream, uint64_t *launches);
 // fp32 rows [first, first+count) -> bf16 shadow rows (stride dimpad) + |x|^2, |x - bf16(x)|^2
 int build_shadow(const float *rows, uint64_t first, uint64_t count, uint32_t dim, uint32_t dimpad, void *shadow, float *xnorm2,
                  float *dnorm2, cudaStream_t stream);
