@@ -226,6 +226,33 @@ int nk_search(NkIndex *ix, const float *queries_host, uint32_t Q, uint32_t k, ui
 int nk_search_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uint32_t k, uint32_t *out_idx_dev,
                      float *out_score_dev, void *stream);
 
+/* Per-query tag filters: one corpus pass for a batch whose queries carry different label filters (Qdrant SearchBatch with
+ * a Filter per request, search.Service Types, one queryNodes label per vector index).
+ * Every row carries a 64-bit tag word whose bits the caller assigns (labels, types, collection, keyword values); rows that
+ * were never tagged have tag 0.  Each query carries an NkFilter; row r is ADMISSIBLE for the query iff
+ *     (tag[r] & all_of) == all_of  &&  (tag[r] & none_of) == 0  &&  (any_of == 0 || (tag[r] & any_of) != 0)
+ * (Qdrant's must / must_not / should over bit conditions).  {0,0,0} admits every row, so filtered and unfiltered queries
+ * share a batch; all_of = none_of = ~0 admits no row.  The predicate is evaluated inside the scan kernels, before a pair can
+ * enter a candidate buffer: results are exact (every returned score re-scored in fp32), with nk_search's order and ties.
+ * The index-wide row mask and score floor still apply.  Returns min(k, rows passing the row mask), like nk_search; a query
+ * with fewer admissible rows gets 0xffffffff / 0 in its unused slots.  filters == NULL: no filter.
+ * Tags live per shard in device memory (8 B per row) and follow the rows: append gives new rows tag 0, update_row keeps the
+ * tag, remove_swap moves the last row's tag with its row; upload, upload_from_f32, fill_* and attach_device_rows reset every
+ * tag to 0.
+ * Not filtered: nk_search_groups, nk_score_subset, nk_search_keys_device, nk_search_sharded_device and the k-means calls. */
+typedef struct NkFilter {
+    uint64_t all_of, none_of, any_of;
+} NkFilter;
+/* Tags of rows [first_row, first_row + n_rows) (global, relative to the index's first row); may span shards. */
+int nk_index_set_row_tags(NkIndex *ix, uint64_t first_row, const uint64_t *tags_host, uint64_t n_rows);
+/* nk_search with one filter per query (filters_host [Q], NULL = none).  Synchronous, any number of devices. */
+int nk_search_filtered(NkIndex *ix, const float *queries_host, const NkFilter *filters_host, uint32_t Q, uint32_t k,
+                       uint32_t *out_idx, float *out_score);
+/* nk_search_device with one filter per query: filters_dev [Q] device memory (NULL = none) that must stay valid until `stream`
+ * has run the search. */
+int nk_search_filtered_device(NkIndex *ix, const float *queries_dev, const NkFilter *filters_dev, uint32_t Q, uint32_t k,
+                              uint32_t *out_idx_dev, float *out_score_dev, void *stream);
+
 /* Multi-process sharding (one rank per GPU): emit this shard's sorted candidate list as packed 64-bit
  * keys [Q x k] (order-preserving score bits << 32 | ~row index; larger key = better), to be exchanged
  * (e.g. ncclAllGather of Q*k*8 bytes per rank) and merged with nk_merge_keys_device. */

@@ -108,6 +108,17 @@ __host__ __device__ __forceinline__ uint64_t make_key(float s, uint32_t row) {
 __host__ __device__ __forceinline__ float key_score(uint64_t k) { return ord_to_float((uint32_t)(k >> 32)); }
 __host__ __device__ __forceinline__ uint32_t key_row(uint64_t k) { return 0xffffffffu - (uint32_t)k; }
 
+// Per-query tag filter (nk_search_filtered): may a row with tag word `tag` be returned for a query with filter f?
+__host__ __device__ __forceinline__ bool tag_admits(uint64_t tag, uint64_t all_of, uint64_t none_of, uint64_t any_of) {
+    return (tag & all_of) == all_of && (tag & none_of) == 0 && (any_of == 0 || (tag & any_of) != 0);
+}
+#ifdef __CUDACC__
+// The same against a device filter array [Q] (read through the read-only cache: 24 B per query, shared by every row).
+__device__ __forceinline__ bool tag_admits(uint64_t tag, const NkFilter *f) {
+    return tag_admits(tag, __ldg(&f->all_of), __ldg(&f->none_of), __ldg(&f->any_of));
+}
+#endif
+
 // Counter-based U[-1,1) generator, bit-identical to oracle/knn_oracle.c orc_uniform_at().
 __host__ __device__ __forceinline__ uint64_t mix64(uint64_t z) {
     z ^= z >> 30; z *= 0xBF58476D1CE4E5B9ULL;

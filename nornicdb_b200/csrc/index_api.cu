@@ -65,6 +65,10 @@ struct NkShard {
     uint32_t *mask = nullptr;  // optional row filter (nk_index_set_row_mask): bit = local row
     size_t mask_bytes = 0;
     bool mask_on = false;
+    // tag word per local row (nk_index_set_row_tags), grow-only; tags_on = false: every tag is 0 and the array may be stale
+    uint64_t *tags = nullptr;
+    uint64_t tags_cap = 0;
+    bool tags_on = false;
     size_t cvt_bytes = 0;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> timing;  // pending scan-kernel event pairs
     std::vector<uint64_t> timing_launches;
@@ -105,6 +109,32 @@ static void drop_row_mask(NkIndex *ix) {
     ix->mask_on = false;
     ix->n_groups = 0;
     for (auto &s : ix->shards) { s.mask_on = false; s.group_on = false; }
+}
+
+// ---- per-row tag words (nk_search_filtered) ---------------------------------------------------------------------------
+// The array follows the rows: rows [old_n, s.n) are new and get tag 0; the capacity follows the row capacity.  Synchronous,
+// so a search on any stream may read the array afterwards.
+static int shard_tags_grow(NkShard &s, uint64_t old_n) {
+    if (s.tags_cap < s.n) {
+        const uint64_t cap = std::max<uint64_t>(std::max(s.cap, s.n), 16);
+        uint64_t *p = nullptr;
+        NK_CUDA_OK(cudaMalloc((void **)&p, cap * 8));
+        if (s.tags && old_n) NK_CUDA_OK(cudaMemcpyAsync(p, s.tags, old_n * 8, cudaMemcpyDeviceToDevice, s.stream));
+        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+        if (s.tags) NK_CUDA_OK(cudaFree(s.tags));
+        s.tags = p;
+        s.tags_cap = cap;
+    }
+    if (s.n > old_n) NK_CUDA_OK(cudaMemsetAsync(s.tags + old_n, 0, (s.n - old_n) * 8, s.stream));
+    NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+    return 0;
+}
+// Make the shard's tag array real (all zero if the rows were never tagged since the last reset).
+static int shard_tags_on(NkShard &s) {
+    if (s.tags_on) return 0;
+    if (shard_tags_grow(s, 0)) return -1;
+    s.tags_on = true;
+    return 0;
 }
 
 static void shard_drop_shadow(NkShard &s) {
@@ -254,6 +284,7 @@ struct ScanOut {  // optional extras of run_scan
     uint32_t *out_idx = nullptr;   // fused decode (single-shard searches)
     float *out_score = nullptr;
     bool defer_tail = false;       // host-synchronous caller: retry stages are queued only if a flag was raised
+    const NkFilter *qfilter = nullptr;  // per-query tag filters [Q] (device; the shard's tag array must be on)
 };
 static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uint32_t k, uint64_t *out_keys,
                     cudaStream_t stream, const ScanOut &xo = ScanOut());
@@ -261,7 +292,8 @@ static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uin
 // k > NK_MAX_K (the reference accepts any k, cuda_bridge.go:327-375): ceil(k / NK_MAX_K) fused CUDA-core passes; pass p+1
 // only admits keys strictly below the last key pass p returned, so the passes tile the ranking exactly.
 static int run_scan_bigk(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uint32_t k, uint64_t *out_keys,
-                         cudaStream_t stream, const void *rows = nullptr, uint32_t n_rows = 0, bool custom_rows = false) {
+                         cudaStream_t stream, const void *rows = nullptr, uint32_t n_rows = 0, bool custom_rows = false,
+                         const NkFilter *qfilter = nullptr) {
     if (nk::ws_reserve((void **)&s.ws.below, &s.ws.below_bytes, (size_t)Q * 8)) return -1;
     if (nk::ws_reserve((void **)&s.ws.keys2, &s.ws.keys2_bytes, (size_t)Q * NK_MAX_K * 8)) return -1;
     NK_CUDA_OK(cudaMemsetAsync(s.ws.below, 0xff, (size_t)Q * 8, stream));
@@ -273,6 +305,7 @@ static int run_scan_bigk(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q
         a.queries = q_dev; a.Q = Q; a.k = kp; a.metric = ix->metric; a.stream = stream; a.below = s.ws.below;
         a.row_mask = (!custom_rows && s.mask_on) ? s.mask : nullptr;
         a.min_score = custom_rows ? -INFINITY : ix->key_floor();
+        if (qfilter && !custom_rows) { a.row_tags = s.tags; a.qfilter = qfilter; }
         if (nk::scan_simt(s.di, a, s.ws, s.ws.keys2, &ix->stats.kernel_launches)) return -1;
         NK_CUDA_OK(cudaMemcpy2DAsync(out_keys + done, (size_t)k * 8, s.ws.keys2, (size_t)kp * 8, (size_t)kp * 8, Q,
                                      cudaMemcpyDeviceToDevice, stream));
@@ -289,7 +322,7 @@ static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uin
                     cudaStream_t stream, const ScanOut &xo) {
     s.last_filter = false;
     if (k > NK_MAX_K) {
-        if (run_scan_bigk(ix, s, q_dev, Q, k, out_keys, stream)) return -1;
+        if (run_scan_bigk(ix, s, q_dev, Q, k, out_keys, stream, nullptr, 0, false, xo.qfilter)) return -1;
         if (xo.out_idx) {
             if (nk::decode_keys(out_keys, Q, k, ix->metric, xo.out_idx, xo.out_score, stream)) return -1;
             ix->stats.kernel_launches++;
@@ -301,6 +334,7 @@ static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uin
     a.queries = q_dev; a.Q = Q; a.k = k; a.metric = ix->metric; a.stream = stream;
     a.row_mask = s.mask_on ? s.mask : nullptr;
     a.out_idx = xo.out_idx; a.out_score = xo.out_score; a.min_score = ix->key_floor(); a.defer_tail = xo.defer_tail;
+    if (xo.qfilter) { a.row_tags = s.tags; a.qfilter = xo.qfilter; }
     // AUTO: CUDA cores keep Q <= 4 (the single-kernel scan already streams the fewest bytes), tensor cores from 5 queries
     // on.  With a BF16 shadow the filter streams half the bytes of the fp32 rows, so it serves every batch size once the
     // shard is large enough for bytes (not launches) to matter; small shards keep the CUDA-core scan at Q <= 4.  16-bit
@@ -456,6 +490,7 @@ void nk_index_release(NkIndex *ix) {
         }
         if (s.cvt) cudaFree(s.cvt);
         if (s.mask) cudaFree(s.mask);
+        if (s.tags) cudaFree(s.tags);
         if (s.group) cudaFree(s.group);
         s.ws.release();
     }
@@ -480,6 +515,7 @@ static int upload_impl(NkIndex *ix, const void *rows_host, uint64_t n_rows, bool
         NK_CUDA_OK(cudaSetDevice(s.device));
         if (!s.owns) { s.rows = nullptr; s.owns = true; s.cap = 0; s.shadow_attached = false; }
         s.n = 0;
+        s.tags_on = false;  // every tag back to 0
         if (shard_reserve_rows(ix, s, cnt, false)) return -1;
         if (stream_h2d(s, s.rows, static_cast<const char *>(rows_host) + off * src_rb, cnt * src_rb, cvt, ix->dtype)) return -1;
         s.n = cnt;
@@ -536,6 +572,7 @@ int nk_index_append(NkIndex *ix, const void *rows_host, uint64_t n_rows) {
     if (shard_reserve_rows(ix, s, s.n + n_rows, true)) return -1;
     if (stream_h2d(s, (char *)s.rows + s.n * rb, rows_host, n_rows * rb)) return -1;
     s.n += n_rows;
+    if (s.tags_on && shard_tags_grow(s, s.n - n_rows)) return -1;  // appended rows: tag 0
     if (shard_sync_shadow(ix, s)) return -1;  // converts only the appended rows (all of them if the shard was regrown)
     NK_CUDA_OK(cudaStreamSynchronize(s.stream));
     ix->stats.bytes_h2d += n_rows * rb;
@@ -588,6 +625,16 @@ int nk_index_remove_swap(NkIndex *ix, uint64_t row) {
         else NK_CUDA_OK(cudaMemcpyPeerAsync(dst, s->device, src, last->device, rb, s->stream));
         if (shard_shadow_row(ix, *s, local)) return -1;
         NK_CUDA_OK(cudaStreamSynchronize(s->stream));
+        if (last->tags_on || s->tags_on) {  // the last row's tag moves with its row
+            uint64_t tag = 0;
+            if (last->tags_on) {
+                NK_CUDA_OK(cudaSetDevice(last->device));
+                NK_CUDA_OK(cudaMemcpy(&tag, last->tags + (last->n - 1), 8, cudaMemcpyDeviceToHost));
+            }
+            NK_CUDA_OK(cudaSetDevice(s->device));
+            if (shard_tags_on(*s)) return -1;
+            NK_CUDA_OK(cudaMemcpy(s->tags + local, &tag, 8, cudaMemcpyHostToDevice));
+        }
     }
     last->n -= 1;
     if (last->shadow_n > last->n) last->shadow_n = last->n;
@@ -609,6 +656,7 @@ static int fill_impl(NkIndex *ix, uint64_t n_rows, uint64_t seed, uint32_t centr
         NK_CUDA_OK(cudaSetDevice(s.device));
         if (!s.owns) { s.rows = nullptr; s.owns = true; s.cap = 0; s.shadow_attached = false; }
         s.n = 0;
+        s.tags_on = false;  // every tag back to 0
         if (shard_reserve_rows(ix, s, cnt, false)) return -1;
         if (centres ? nk::fill_clustered(s.rows, ix->dtype, cnt, ix->dim, seed, ix->row_base + off, centres, sigma, unit, s.stream)
                     : nk::fill_uniform(s.rows, ix->dtype, cnt, ix->dim, seed, ix->row_base + off, s.stream))
@@ -658,6 +706,7 @@ int nk_index_attach_device_rows(NkIndex *ix, void *rows_dev, uint64_t n_rows) {
     shard_drop_shadow(s);
     drop_row_mask(ix);
     s.rows = rows_dev; s.owns = false; s.n = n_rows; s.cap = n_rows; s.shadow_attached = false;
+    s.tags_on = false;  // every tag back to 0
     rebase(ix);
     return 0;
 }
@@ -729,6 +778,32 @@ int nk_index_set_row_mask(NkIndex *ix, const uint32_t *mask_words, uint64_t n_bi
     }
     ix->mask_on = true;
     ix->mask_alive = alive;
+    return 0;
+}
+
+int nk_index_set_row_tags(NkIndex *ix, uint64_t first_row, const uint64_t *tags_host, uint64_t n_rows) {
+    nk::DeviceGuard _restore_device;
+    if (!ix) { nk::set_error("null index"); return -1; }
+    if (n_rows == 0) return 0;
+    if (!tags_host) { nk::set_error("null tags"); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
+    const uint64_t total = ix->rows();
+    if (first_row > total || n_rows > total - first_row) {
+        nk::set_error("row tags [%llu, %llu) out of range (index has %llu rows)", (unsigned long long)first_row,
+                      (unsigned long long)(first_row + n_rows), (unsigned long long)total);
+        return -1;
+    }
+    for (uint64_t i = 0; i < n_rows;) {
+        uint64_t local;
+        NkShard *s = find_shard(ix, first_row + i, &local);
+        const uint64_t cnt = std::min<uint64_t>(n_rows - i, s->n - local);
+        NK_CUDA_OK(cudaSetDevice(s->device));
+        if (shard_tags_on(*s)) return -1;
+        NK_CUDA_OK(cudaMemcpyAsync(s->tags + local, tags_host + i, cnt * 8, cudaMemcpyHostToDevice, s->stream));
+        NK_CUDA_OK(cudaStreamSynchronize(s->stream));
+        ix->stats.bytes_h2d += cnt * 8;
+        i += cnt;
+    }
     return 0;
 }
 
@@ -867,7 +942,9 @@ int nk_index_read_rows(NkIndex *ix, uint64_t row, uint64_t n_rows, void *rows_ho
     return 0;
 }
 
-int nk_search(NkIndex *ix, const float *queries_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
+// nk_search / nk_search_filtered: filters_host == nullptr is plain nk_search.
+static int search_host(NkIndex *ix, const float *queries_host, const NkFilter *filters_host, uint32_t Q, uint32_t k, uint32_t *out_idx,
+                       float *out_score) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
@@ -902,6 +979,15 @@ int nk_search(NkIndex *ix, const float *queries_host, uint32_t Q, uint32_t k, ui
         }
         NK_CUDA_OK(cudaMemcpyAsync(s->ws.queries, queries_host, qbytes, cudaMemcpyHostToDevice, s->stream));
         ix->stats.bytes_h2d += qbytes;
+        if (filters_host) {
+            // staged next to the queries, in the shard workspace: the deferred retry tail reads them after this call's first sync
+            const size_t fbytes = (size_t)Q * sizeof(NkFilter);
+            if (shard_tags_on(*s)) return -1;
+            if (nk::ws_reserve((void **)&s->ws.qfilter, &s->ws.qfilter_bytes, fbytes)) return -1;
+            NK_CUDA_OK(cudaMemcpyAsync(s->ws.qfilter, filters_host, fbytes, cudaMemcpyHostToDevice, s->stream));
+            ix->stats.bytes_h2d += fbytes;
+            xo.qfilter = s->ws.qfilter;
+        }
         if (run_scan(ix, *s, s->ws.queries, Q, ke, s->ws.keys, s->stream, xo)) return -1;
     }
 
@@ -1001,6 +1087,15 @@ int nk_search(NkIndex *ix, const float *queries_host, uint32_t Q, uint32_t k, ui
     return (int)ke;
 }
 
+int nk_search(NkIndex *ix, const float *queries_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
+    return search_host(ix, queries_host, nullptr, Q, k, out_idx, out_score);
+}
+
+int nk_search_filtered(NkIndex *ix, const float *queries_host, const NkFilter *filters_host, uint32_t Q, uint32_t k,
+                       uint32_t *out_idx, float *out_score) {
+    return search_host(ix, queries_host, filters_host, Q, k, out_idx, out_score);
+}
+
 static int single_shard(NkIndex *ix, NkShard **out) {
     if (!ix) { nk::set_error("null index"); return -1; }
     if (ix->shards.size() != 1) { nk::set_error("device-resident search needs a single-device index"); return -1; }
@@ -1029,8 +1124,9 @@ int nk_search_keys_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uin
     return (int)k;
 }
 
-int nk_search_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uint32_t k, uint32_t *out_idx_dev,
-                     float *out_score_dev, void *stream) {
+// nk_search_device / nk_search_filtered_device: filters_dev == nullptr is plain nk_search_device.
+static int search_device(NkIndex *ix, const float *queries_dev, const NkFilter *filters_dev, uint32_t Q, uint32_t k, uint32_t *out_idx_dev,
+                         float *out_score_dev, void *stream) {
     nk::DeviceGuard _restore_device;
     NkShard *s;
     if (single_shard(ix, &s)) return -1;
@@ -1048,8 +1144,22 @@ int nk_search_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uint32_t
     ix->stats.queries += Q;
     ScanOut xo;
     xo.out_idx = out_idx_dev; xo.out_score = out_score_dev;  // decoded by the last kernel of the path
+    if (filters_dev) {
+        if (shard_tags_on(*s)) return -1;
+        xo.qfilter = filters_dev;  // the caller keeps it valid until the stream has run (the blindly queued tail reads it too)
+    }
     if (run_scan(ix, *s, queries_dev, Q, k, s->ws.keys, st, xo)) return -1;
     return (int)k;
+}
+
+int nk_search_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uint32_t k, uint32_t *out_idx_dev,
+                     float *out_score_dev, void *stream) {
+    return search_device(ix, queries_dev, nullptr, Q, k, out_idx_dev, out_score_dev, stream);
+}
+
+int nk_search_filtered_device(NkIndex *ix, const float *queries_dev, const NkFilter *filters_dev, uint32_t Q, uint32_t k,
+                              uint32_t *out_idx_dev, float *out_score_dev, void *stream) {
+    return search_device(ix, queries_dev, filters_dev, Q, k, out_idx_dev, out_score_dev, stream);
 }
 
 // Device-resident searches cannot report a (never expected) candidate-buffer overflow when they return: this call waits

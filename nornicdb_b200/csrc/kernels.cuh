@@ -23,6 +23,7 @@ struct Workspace {
     float *queries = nullptr;     size_t queries_bytes = 0;  // staged queries (host API)
     uint32_t *out_idx = nullptr;  size_t out_idx_bytes = 0;
     float *out_score = nullptr;   size_t out_score_bytes = 0;
+    NkFilter *qfilter = nullptr;  size_t qfilter_bytes = 0;  // staged per-query tag filters (host API, next to the queries)
     float *qaux = nullptr;        size_t qaux_bytes = 0;     // tensor path: split / normalised queries
     float *rownorm = nullptr;     size_t rownorm_bytes = 0;  // tensor path: per-row inverse norms / sq norms
     int *flags = nullptr;   // NK_FLAG_WORDS ints of device status (layout: FLAG_* in scan_tensor_shared.cuh)
@@ -62,6 +63,11 @@ struct ScanArgs {
     // optional row filter (label / tombstone bitmask): bit r (LSB first in 32-bit words) set = local row r takes part;
     // nullptr = every row.  Honoured by every scan kernel.
     const uint32_t *row_mask = nullptr;
+    // optional per-query tag filters (nk_search_filtered): row_tags [n] (local rows) and qfilter [Q]; a (row, query) pair
+    // takes part only if tag_admits(row_tags[row], qfilter + q).  Both set or both nullptr; kernels that see them are the
+    // filtered (TAGS) instantiations, so unfiltered searches run unchanged code.
+    const uint64_t *row_tags = nullptr;
+    const NkFilter *qfilter = nullptr;
     // optional BF16 shadow of an fp32 shard (scan_tensor_shadow.cu): rows of `shadow_dimpad` bf16 + per-row |x|^2 and
     // |x - bf16(x)|^2; nullptr = none
     const void *shadow = nullptr;

@@ -44,6 +44,8 @@ struct SimtParams {
     const uint64_t *below;  // per-query exclusive key bound (k > NK_MAX_K passes) or nullptr
     const uint32_t *mask;   // row bitmask or nullptr
     float min_score;        // caller's score floor (key space); -inf = none
+    const uint64_t *row_tags;  // TAGS kernels only: tag word per local row
+    const NkFilter *qfilter;   // TAGS kernels only: filter per query [Q]
 };
 
 // ---- element loaders -------------------------------------------------------------------------
@@ -116,7 +118,8 @@ __device__ __forceinline__ void warp_reduce_scatter(float (&v)[V], int lane) {
     }
 }
 
-template <typename T, bool VEC, int QT, int R, bool EUCLID>
+// TAGS: filtered search — the owner lane also tests its (row, query) pair against the query's tag filter.
+template <typename T, bool VEC, int QT, int R, bool EUCLID, bool TAGS>
 __global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtParams p) {
     pdl_trigger();  // the merge launch behind this scan may begin (it waits for this grid before reading)
     pdl_wait();     // exact-stage twin of a filter search: programmatic dependent of the finish kernel
@@ -234,7 +237,8 @@ __global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtParams 
                 xr = __shfl_sync(0xffffffffu, xx[0], r * (32 / R));
             }
             const uint32_t row = row0 + r;
-            if ((lane % LPV) == 0 && row < n && (uint32_t)qi < p.nq && (!p.mask || ((p.mask[row >> 5] >> (row & 31)) & 1u))) {
+            if ((lane % LPV) == 0 && row < n && (uint32_t)qi < p.nq && (!p.mask || ((p.mask[row >> 5] >> (row & 31)) & 1u)) &&
+                (!TAGS || tag_admits(__ldg(p.row_tags + row), p.qfilter + p.q0 + qi))) {
                 if constexpr (EUCLID) {
                     s = -s;
                 } else if (p.metric == NK_METRIC_COSINE) {
@@ -295,34 +299,38 @@ __global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtParams 
 // ---------------------------------------------------------------------------------------------
 typedef void (*SimtKernel)(SimtParams);
 
-template <typename T, bool VEC, bool EUCLID>
+template <typename T, bool VEC, bool EUCLID, bool TAGS>
 static SimtKernel pick_qt(int qt) {
     if constexpr (VEC) {
         switch (qt) {
-            case 8: return knn_scan_simt_kernel<T, VEC, 8, 4, EUCLID>;
-            case 4: return knn_scan_simt_kernel<T, VEC, 4, 8, EUCLID>;
-            case 2: return knn_scan_simt_kernel<T, VEC, 2, 8, EUCLID>;
-            default: return knn_scan_simt_kernel<T, VEC, 1, 8, EUCLID>;
+            case 8: return knn_scan_simt_kernel<T, VEC, 8, 4, EUCLID, TAGS>;
+            case 4: return knn_scan_simt_kernel<T, VEC, 4, 8, EUCLID, TAGS>;
+            case 2: return knn_scan_simt_kernel<T, VEC, 2, 8, EUCLID, TAGS>;
+            default: return knn_scan_simt_kernel<T, VEC, 1, 8, EUCLID, TAGS>;
         }
     } else {
         switch (qt) {
-            case 4: return knn_scan_simt_kernel<T, VEC, 4, 8, EUCLID>;
-            default: return knn_scan_simt_kernel<T, VEC, 1, 8, EUCLID>;
+            case 4: return knn_scan_simt_kernel<T, VEC, 4, 8, EUCLID, TAGS>;
+            default: return knn_scan_simt_kernel<T, VEC, 1, 8, EUCLID, TAGS>;
         }
     }
 }
 
-static SimtKernel pick_kernel(int dtype, bool vec, bool euclid, int qt) {
+template <bool TAGS>
+static SimtKernel pick_kernel_t(int dtype, bool vec, bool euclid, int qt) {
     if (dtype == NK_DTYPE_F16) {
-        if (vec) return euclid ? pick_qt<__half, true, true>(qt) : pick_qt<__half, true, false>(qt);
-        return euclid ? pick_qt<__half, false, true>(qt) : pick_qt<__half, false, false>(qt);
+        if (vec) return euclid ? pick_qt<__half, true, true, TAGS>(qt) : pick_qt<__half, true, false, TAGS>(qt);
+        return euclid ? pick_qt<__half, false, true, TAGS>(qt) : pick_qt<__half, false, false, TAGS>(qt);
     }
     if (dtype == NK_DTYPE_BF16) {
-        if (vec) return euclid ? pick_qt<__nv_bfloat16, true, true>(qt) : pick_qt<__nv_bfloat16, true, false>(qt);
-        return euclid ? pick_qt<__nv_bfloat16, false, true>(qt) : pick_qt<__nv_bfloat16, false, false>(qt);
+        if (vec) return euclid ? pick_qt<__nv_bfloat16, true, true, TAGS>(qt) : pick_qt<__nv_bfloat16, true, false, TAGS>(qt);
+        return euclid ? pick_qt<__nv_bfloat16, false, true, TAGS>(qt) : pick_qt<__nv_bfloat16, false, false, TAGS>(qt);
     }
-    if (vec) return euclid ? pick_qt<float, true, true>(qt) : pick_qt<float, true, false>(qt);
-    return euclid ? pick_qt<float, false, true>(qt) : pick_qt<float, false, false>(qt);
+    if (vec) return euclid ? pick_qt<float, true, true, TAGS>(qt) : pick_qt<float, true, false, TAGS>(qt);
+    return euclid ? pick_qt<float, false, true, TAGS>(qt) : pick_qt<float, false, false, TAGS>(qt);
+}
+static SimtKernel pick_kernel(int dtype, bool vec, bool euclid, int qt, bool tags) {
+    return tags ? pick_kernel_t<true>(dtype, vec, euclid, qt) : pick_kernel_t<false>(dtype, vec, euclid, qt);
 }
 
 // cudaFuncSetAttribute + occupancy query once per (kernel, device, smem) instead of once per search
@@ -385,7 +393,7 @@ int scan_simt(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *
             set_error("dim=%u too large for the SIMT scan (needs %zu B shared memory)", a.dim, smem);
             return -1;
         }
-        SimtKernel kern = pick_kernel(a.dtype, vec, euclid, qt);
+        SimtKernel kern = pick_kernel(a.dtype, vec, euclid, qt, a.qfilter != nullptr);
         if (simt_ensure(reinterpret_cast<const void *>(kern), di.device_id, smem)) return -1;
         int occ = simt_occupancy(reinterpret_cast<const void *>(kern), di.device_id, smem);
         // One grid for every query group of this search so the per-CTA partial lists line up.
@@ -400,6 +408,7 @@ int scan_simt(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *
         p.rows = a.rows; p.n = a.n; p.dim = a.dim; p.row_base = a.row_base;
         p.queries = a.queries; p.q0 = q0; p.nq = left < (uint32_t)qt ? left : (uint32_t)qt; p.k = a.k;
         p.metric = a.metric; p.P = P; p.cand = ws.cand; p.partial = ws.partial; p.flags = ws.flags; p.only_if = a.only_if; p.below = a.below; p.mask = a.row_mask; p.min_score = a.min_score;
+        p.row_tags = a.row_tags; p.qfilter = a.qfilter;
         NK_CUDA_OK(launch_pdl(kern, dim3(grid_used), dim3(SIMT_THREADS), smem, a.stream, a.only_if != nullptr && !a.defer_tail, p));
         if (launches) ++*launches;
         if (a.main_launches) ++*a.main_launches;

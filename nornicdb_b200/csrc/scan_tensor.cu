@@ -152,6 +152,9 @@ __device__ __forceinline__ float warp_exact_score(const void *rows, int dtype, s
 // ---------------------------------------------------------------------------------------------------
 constexpr int PREP_THREADS = 1024;  // 32 warps: the sample scoring is latency-bound (one 4 KB row per warp at a time)
 
+// TAGS (filtered searches): the sample only counts rows the query admits, so a query with fewer than k admissible sample rows
+// starts at the score floor.
+template <bool TAGS>
 __global__ void __launch_bounds__(PREP_THREADS) filter_prep_kernel(PrepParams p) {
     extern __shared__ __align__(16) unsigned char prep_smem[];
     float *qs = reinterpret_cast<float *>(prep_smem);                                  // raw query [dim]
@@ -240,7 +243,9 @@ __global__ void __launch_bounds__(PREP_THREADS) filter_prep_kernel(PrepParams p)
         const float lo = sc - (p.metric == NK_METRIC_COSINE ? p.acc_c : p.metric == NK_METRIC_DOT ? p.acc_c * sqrtf(xx * t) : p.acc_c * -sc);
         return (lo == lo && lo > -INFINITY && lo < INFINITY) ? (uint64_t)ord_bits(lo) : 0ull;
     };
-    auto admissible = [&](uint64_t r) -> bool { return r < p.n && (!p.mask || ((__ldg(p.mask + (r >> 5)) >> (r & 31)) & 1u)); };
+    auto admissible = [&](uint64_t r) -> bool {
+        return r < p.n && (!p.mask || ((__ldg(p.mask + (r >> 5)) >> (r & 31)) & 1u)) && (!TAGS || tag_admits(__ldg(p.row_tags + r), p.qfilter + row));
+    };
     if (p.dtype == NK_DTYPE_F32 && p.metric != NK_METRIC_EUCLIDEAN) {
         // two rows per warp at a time: both rows' 128-bit loads are in flight together (the scoring is latency-bound:
         // one 4 KB row per warp per round trip)
@@ -327,7 +332,8 @@ template <bool FILTER> struct Tf32Est {
     __device__ __forceinline__ float bound(uint32_t qi) const { return bnd * qn[qi]; }
 };
 
-template <int NT, int QT, bool DUMP>
+// TAGS: filtered search (per-query tag filters in the keep rule); the unfiltered instantiations are TAGS = false.
+template <int NT, int QT, bool DUMP, bool TAGS>
 __global__ void __launch_bounds__(tc::THREADS, 1)
 knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_qhi,
                    const __grid_constant__ CUtensorMap map_qlo, tc::Params p) {
@@ -488,7 +494,7 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                     if (!cosine && alive && est.x2 < INFINITY && (lane & 3) == 0) atomicMax(&sh.maxxx, __float_as_uint(est.x2));  // NaN / Inf rows: kept, judged exactly
                     if (euclid) est.mul = 2.0f;
                 }
-                keep_fragment_row<QT, P, FILTER, DUMP && FILTER>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau, sh.qn,
+                keep_fragment_row<QT, P, FILTER, DUMP && FILTER, TAGS>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau, sh.qn,
                                                                  sh.cnt, my_cand);
             }
             // prune any buffer that could overflow during the next tile; the 8 consumer warps prune different
@@ -898,6 +904,7 @@ tc::Params pass_params(const ScanArgs &a, Workspace &ws, const tc::PassArgs &t) 
     p.cand = ws.cand; p.partial = ws.partial; p.flags = ws.flags; p.debug = tc_debug_flags(); p.mask = a.row_mask;
     p.gtau = reinterpret_cast<uint32_t *>(ws.keys2); p.gcount = reinterpret_cast<int *>(ws.keys2) + (t.Qpad + tc::QT_BIG);
     p.presampled = t.presampled; p.min_score = a.min_score;
+    p.row_tags = a.row_tags; p.qfilter = a.qfilter;
     p.dump_est = t.dump_est; p.dump_bnd = t.dump_bnd; p.dump_ld = t.dump_ld;
     return p;
 }
@@ -928,13 +935,17 @@ PrepParams prep_params(const ScanArgs &a, uint32_t Qpad, uint32_t dimpad) {
     pp.q = a.queries; pp.Q = a.Q; pp.dim = a.dim; pp.dimpad = dimpad; pp.Qpad = Qpad;
     pp.normalise = a.metric == NK_METRIC_COSINE; pp.metric = a.metric;
     pp.rows = a.rows; pp.dtype = a.dtype; pp.n = a.n; pp.k = a.k; pp.mask = a.row_mask; pp.min_score = a.min_score;
+    pp.row_tags = a.row_tags; pp.qfilter = a.qfilter;
     return pp;
 }
 
 int launch_prep(const DeviceInfo &di, const PrepParams &pp, cudaStream_t stream, uint64_t *launches) {
     const size_t smem = (size_t)((pp.dim + 3) & ~3u) * 4 + (size_t)pp.sample * 8;
-    if (smem > 48 * 1024 && tc_ensure_smem(reinterpret_cast<const void *>(filter_prep_kernel), di.device_id, smem)) return -1;
-    filter_prep_kernel<<<pp.Qpad, PREP_THREADS, smem, stream>>>(pp);
+    const bool tags = pp.qfilter != nullptr;
+    const void *kern = tags ? reinterpret_cast<const void *>(filter_prep_kernel<true>) : reinterpret_cast<const void *>(filter_prep_kernel<false>);
+    if (smem > 48 * 1024 && tc_ensure_smem(kern, di.device_id, smem)) return -1;
+    if (tags) filter_prep_kernel<true><<<pp.Qpad, PREP_THREADS, smem, stream>>>(pp);
+    else filter_prep_kernel<false><<<pp.Qpad, PREP_THREADS, smem, stream>>>(pp);
     NK_CUDA_OK(cudaGetLastError());
     if (launches) ++*launches;
     return 0;
@@ -947,8 +958,8 @@ struct TcPassArgs : tc::PassArgs {
     const int *only_if;
     bool count_main;
 };
-template <int NT, int QT, bool DUMP = false>
-static int launch_pass(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const TcPassArgs &t, uint64_t *launches) {
+template <int NT, int QT, bool DUMP = false, bool TAGS = false>
+static int launch_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const TcPassArgs &t, uint64_t *launches) {
     using namespace tc;
     const CUtensorMap *map_rows = tc_cached_map(ws, 0, a.rows, a.n, a.dim, 4, (uint32_t)BK, ROWS, (uint64_t)a.dim * 4);
     // query rows past Qpad are zero-filled by TMA
@@ -960,16 +971,22 @@ static int launch_pass(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, c
         set_error("tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;
     }
-    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_tc_kernel<NT, QT, DUMP>), di.device_id, smem)) return -1;
+    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_tc_kernel<NT, QT, DUMP, TAGS>), di.device_id, smem)) return -1;
     Params p = pass_params(a, ws, t);
     p.nslab = (a.dim + BK - 1) / BK; p.margin_c = t.margin_c; p.only_if = t.only_if;
     // (asynchronous API: the early-exit retry / exact stages are programmatic dependents — their launch overlaps the kernel
     // before them.  Not for the host-synchronous API: measured 5-15 us slower per nk_search, the copy-out behind it waits longer)
-    NK_CUDA_OK(launch_pdl(knn_scan_tc_kernel<NT, QT, DUMP>, dim3(t.grid), dim3(THREADS), smem, a.stream, t.only_if != nullptr && !a.defer_tail, *map_rows, *map_qhi,
+    NK_CUDA_OK(launch_pdl(knn_scan_tc_kernel<NT, QT, DUMP, TAGS>, dim3(t.grid), dim3(THREADS), smem, a.stream, t.only_if != nullptr && !a.defer_tail, *map_rows, *map_qhi,
                           *map_qlo, p));
     if (launches) ++*launches;
     if (t.count_main && a.main_launches) ++*a.main_launches;
     return 0;
+}
+// Filtered searches (per-query tag filters) run the TAGS instantiation of the same kernel.
+template <int NT, int QT, bool DUMP = false>
+static int launch_pass(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const TcPassArgs &t, uint64_t *launches) {
+    if (!DUMP && a.qfilter) return launch_pass_t<NT, QT, false, true>(di, a, ws, t, launches);
+    return launch_pass_t<NT, QT, DUMP, false>(di, a, ws, t, launches);
 }
 
 static void fin_print_prof(cudaStream_t stream, uint32_t Q) {

@@ -132,7 +132,9 @@ struct Bf16Est {
     __device__ __forceinline__ float bound(uint32_t qi) const { return fmaf(ra, qa[qi], rb * qb[qi]); }
 };
 
-template <int QT, bool DUMP>
+// TAGS: filtered search (per-query tag filters in the keep rule, read through the read-only cache: the shared-memory budget
+// is spent on the rings); the unfiltered instantiations are TAGS = false.
+template <int QT, bool DUMP, bool TAGS>
 __global__ void __launch_bounds__(sb::NTHREADS, 1)
 knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_q, tc::Params p) {
     using namespace sb;
@@ -284,7 +286,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                     atomicMax(&sh.max_ra, __float_as_uint(est.ra));
                     if (!cosine) { atomicMax(&sh.max_rb, __float_as_uint(est.rb)); atomicMax(&sh.maxxx, __float_as_uint(est.x2)); }
                 }
-                keep_fragment_row<QT, PB, true, DUMP>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau, sh.qn, sh.cnt, my_cand);
+                keep_fragment_row<QT, PB, true, DUMP, TAGS>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau, sh.qn, sh.cnt, my_cand);
             }
             // prune any buffer that could overflow during the next tile (8 warps, different queries concurrently)
             group_sync(EPI_BAR, EPI_NT);  // every push of this tile is visible
@@ -463,7 +465,7 @@ bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a) {
     return a.dim % 8 == 0;  // 16-bit rows: 16-byte TMA row stride and 128-bit exact re-scoring loads
 }
 
-template <int QT, bool DUMP>
+template <int QT, bool DUMP, bool TAGS = false>
 static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
     using namespace sb;
     const bool native = a.shadow_native;  // 16-bit corpus scanned in place: row stride dim * 2, columns past dim read as zero (TMA OOB fill)
@@ -477,10 +479,10 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
         set_error("shadow tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;
     }
-    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, DUMP>), di.device_id, smem)) return -1;
+    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, DUMP, TAGS>), di.device_id, smem)) return -1;
     tc::Params p = pass_params(a, ws, sp);
     p.nslab = sp.dimpad / BKB; p.qa = sp.qa; p.qb = sp.qb; p.xnorm2 = a.xnorm2; p.dnorm2 = a.dnorm2; p.op_f16 = a.dtype == NK_DTYPE_F16;
-    knn_scan_shadow_kernel<QT, DUMP><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
+    knn_scan_shadow_kernel<QT, DUMP, TAGS><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
     NK_CUDA_OK(cudaGetLastError());
     if (launches) ++*launches;
     if (a.main_launches) ++*a.main_launches;
@@ -490,6 +492,8 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
 
 int launch_shadow_pass(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
     if (sp.dump_est) return launch_shadow_pass_t<64, true>(di, a, ws, sp, launches);
+    if (a.qfilter)
+        return qt == 128 ? launch_shadow_pass_t<128, false, true>(di, a, ws, sp, launches) : launch_shadow_pass_t<64, false, true>(di, a, ws, sp, launches);
     return qt == 128 ? launch_shadow_pass_t<128, false>(di, a, ws, sp, launches) : launch_shadow_pass_t<64, false>(di, a, ws, sp, launches);
 }
 

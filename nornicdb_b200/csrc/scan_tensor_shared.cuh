@@ -69,6 +69,8 @@ struct Params {
     float *dump_est, *dump_bnd;  // DUMP kernels only (tests): per (row, query) score estimate and error bound, [n][dump_ld]
     uint32_t dump_ld;
     int op_f16;               // 16-bit kernel: operands are fp16 (an fp16 corpus scanned in place) instead of bf16
+    const uint64_t *row_tags; // TAGS kernels only: tag word per local row
+    const NkFilter *qfilter;  // TAGS kernels only: filter per query [Q], indexed like gtau (absolute query index)
 };
 
 // What one scan launch covers: queries [q0, q0+nq) in `qgroups` query groups over a `grid`-CTA launch.  Both kernels'
@@ -155,7 +157,10 @@ __device__ __forceinline__ bool row_alive(const Params &p, uint32_t row) {
 //   otherwise a compact compare pass builds the mask of columns worth buffering (NaN passes) and the rare pushes run in a
 //   small out-of-line loop so the hot code stays short.
 // BOUNDED: a NaN estimate is undecidable here, so it is kept as +inf and the exact re-scoring judges; exact mode: -inf.
-template <int QT, int CAP, bool BOUNDED, bool DUMP, class Est>
+// TAGS (filtered searches): a pair whose query does not admit the row's tag never enters a buffer — otherwise the pruned and
+// published thresholds would stop being lower bounds of the FILTERED k-th best score.  Flood tiles place it as key 0; the
+// compare pass loads the row's tag only when some column passed and clears the columns whose filter rejects it.
+template <int QT, int CAP, bool BOUNDED, bool DUMP, bool TAGS = false, class Est>
 __device__ __forceinline__ void keep_fragment_row(const Params &p, const Est &est, const float (&acc)[QT / 2], uint32_t r,
                                                   uint32_t row, uint32_t rt, bool alive, bool flood, uint32_t it, uint32_t cbase,
                                                   uint32_t q0, uint32_t nq, const float *tau, const float *qn, int *cnt,
@@ -180,13 +185,26 @@ __device__ __forceinline__ void keep_fragment_row(const Params &p, const Est &es
         // buffered: no atomics, no register select.
         const uint32_t slot = it * ROWS + rt;
         const uint32_t grow = (uint32_t)(p.row_base + row);
+        uint32_t admit = ~0u;  // columns whose filter admits the row (a compact loop: the unrolled one below stays as it is)
+        if (TAGS) {
+            admit = 0u;
+            if (alive) {
+                const uint64_t tag = __ldg(p.row_tags + row);
+#pragma unroll 1
+                for (uint32_t c = 0; c < (uint32_t)(QT / 4); ++c) {
+                    const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
+                    if (qi < nq && tag_admits(tag, p.qfilter + q0 + qi)) admit |= 1u << c;
+                }
+            }
+        }
 #pragma unroll
         for (int jj = 0; jj < QT / 4; ++jj) {
             const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
             if (qi < nq) {
                 float sc = est.upper(v[jj], qi);
                 if (sc != sc) sc = BOUNDED ? INFINITY : -INFINITY;
-                cand[(size_t)qi * CAP + slot] = (alive && sc >= p.min_score) ? make_key(sc, grow) : 0ull;  // 0 = empty slot
+                const bool keep = alive && sc >= p.min_score && ((admit >> jj) & 1u);
+                cand[(size_t)qi * CAP + slot] = keep ? make_key(sc, grow) : 0ull;  // 0 = empty slot
             }
         }
     } else if (alive) {
@@ -196,6 +214,16 @@ __device__ __forceinline__ void keep_fragment_row(const Params &p, const Est &es
             const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
             const float s0 = est.upper(v[jj], qi);
             pass |= (!(s0 < tau[qi]) && qi < nq) ? (1u << jj) : 0u;
+        }
+        if (TAGS && pass) {
+            const uint64_t tag = __ldg(p.row_tags + row);
+            uint32_t chk = pass;
+#pragma unroll 1
+            while (chk) {
+                const uint32_t c = (uint32_t)__ffs((int)chk) - 1u;
+                chk &= chk - 1u;
+                if (!tag_admits(tag, p.qfilter + q0 + cbase + 8 * (c >> 1) + (c & 1))) pass &= ~(1u << c);
+            }
         }
 #pragma unroll 1
         while (pass) {
@@ -333,6 +361,8 @@ struct PrepParams {
     const uint32_t *mask;
     float min_score;
     const int *only_if;
+    const uint64_t *row_tags;  // per-query tag filters (both set or both nullptr): the sample counts admissible rows only
+    const NkFilter *qfilter;
 };
 // The fields taken from the search arguments: the queries, the metric and the shard (for the sample).
 PrepParams prep_params(const ScanArgs &a, uint32_t Qpad, uint32_t dimpad);

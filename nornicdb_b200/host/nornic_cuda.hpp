@@ -266,6 +266,31 @@ public:
             }
         return out;
     }
+    // Per-query tag filters: tag words of rows [firstRow, firstRow + tags.size()) (row order of Add; 0 = untagged), then a
+    // batch whose queries each carry an NkFilter (Qdrant must / must_not / should over bit conditions) in one corpus pass.
+    void SetRowTags(uint64_t firstRow, const std::vector<uint64_t> &tags) {
+        std::lock_guard<std::mutex> lk(mu_);
+        check(nk_index_set_row_tags(ix_, firstRow, tags.data(), tags.size()));
+    }
+    std::vector<std::vector<SearchResult>> SearchBatchFiltered(const std::vector<float> &queries, const std::vector<NkFilter> &filters,
+                                                               uint32_t Q, int k) {
+        if (queries.size() != (size_t)Q * dims_) throw ErrInvalidDimensions();
+        if (filters.size() != Q) throw std::invalid_argument("gpu: one filter per query");
+        std::lock_guard<std::mutex> lk(mu_);
+        if (nodeIDs_.empty() || k <= 0) return std::vector<std::vector<SearchResult>>(Q);
+        std::vector<uint32_t> idx((size_t)Q * k);
+        std::vector<float> sc((size_t)Q * k);
+        int got = nk_search_filtered(ix_, queries.data(), filters.data(), Q, (uint32_t)k, idx.data(), sc.data());
+        if (got < 0) throw cuda::ErrKernelExecution(std::string("gpu: ") + nk_last_error());
+        std::vector<std::vector<SearchResult>> out(Q);
+        for (uint32_t q = 0; q < Q; ++q)
+            for (int i = 0; i < got; ++i) {
+                uint32_t r = idx[(size_t)q * k + i];
+                float s = sc[(size_t)q * k + i];
+                if (r < nodeIDs_.size()) out[q].push_back({nodeIDs_[r], s, 1.0f - s});  // 0xffffffff: fewer admissible rows than k
+            }
+        return out;
+    }
     std::vector<SearchResult> ScoreSubset(const std::vector<float> &query, const std::vector<std::string> &ids) {  // gpu.go:1552-1616
         if ((int)query.size() != dims_) throw ErrInvalidDimensions();
         std::lock_guard<std::mutex> lk(mu_);

@@ -227,6 +227,38 @@ class KnnIndex:
         return _check(self.lib.nk_search_device(self.ptr, q_ptr, Q, k, out_idx_ptr, out_score_ptr, stream),
                       "nk_search_device")
 
+    # -- per-query tag filters ---------------------------------------------------------------------
+    def set_row_tags(self, tags, first_row: int = 0) -> None:
+        """Tag words (uint64, one per row) of rows [first_row, first_row + len(tags)); untagged rows have tag 0."""
+        t = np.ascontiguousarray(np.asarray(tags, dtype=np.uint64).reshape(-1))
+        _check(self.lib.nk_index_set_row_tags(self.ptr, int(first_row), t.ctypes.data_as(C.c_void_p), int(t.size)),
+               "nk_index_set_row_tags")
+
+    def search_filtered(self, queries, k: int, filters) -> Tuple[np.ndarray, np.ndarray]:
+        """search() with one tag filter per query: filters [Q x 3] uint64 (all_of, none_of, any_of), None = no filter.
+        Slots beyond a query's admissible rows hold index 0xffffffff and score 0."""
+        q = np.ascontiguousarray(np.asarray(queries, dtype=np.float32))
+        if q.ndim == 1:
+            q = q.reshape(1, -1)
+        if q.shape[1] != self.dim:
+            raise KnnError(f"invalid dimensions: query has {q.shape[1]}, index has {self.dim}")
+        Q = q.shape[0]
+        f = None if filters is None else as_filters(filters, Q)
+        k = int(k)
+        if k <= 0 or Q == 0:
+            return np.empty((Q, 0), np.uint32), np.empty((Q, 0), np.float32)
+        idx = np.empty((Q, k), dtype=np.uint32)
+        sc = np.empty((Q, k), dtype=np.float32)
+        ke = _check(self.lib.nk_search_filtered(self.ptr, q.ctypes.data_as(C.c_void_p), None if f is None else f.ctypes.data_as(C.c_void_p),
+                                                Q, k, idx.ctypes.data_as(C.c_void_p), sc.ctypes.data_as(C.c_void_p)), "nk_search_filtered")
+        return idx[:, :ke], sc[:, :ke]
+
+    def search_filtered_device(self, q_ptr: int, filters_ptr: int, Q: int, k: int, out_idx_ptr: int, out_score_ptr: int,
+                               stream: int = 0) -> int:
+        """Device-resident filtered search: filters_ptr = device [Q x 3] uint64 (0 = no filter), valid until the stream ran."""
+        return _check(self.lib.nk_search_filtered_device(self.ptr, q_ptr, filters_ptr or None, Q, k, out_idx_ptr, out_score_ptr, stream),
+                      "nk_search_filtered_device")
+
     def search_keys_device(self, q_ptr: int, Q: int, k: int, out_keys_ptr: int, stream: int = 0) -> int:
         return _check(self.lib.nk_search_keys_device(self.ptr, q_ptr, Q, k, out_keys_ptr, stream),
                       "nk_search_keys_device")
@@ -270,6 +302,84 @@ class KnnIndex:
         _check(self.lib.nk_index_cluster_means(self.ptr, a.ctypes.data_as(C.c_void_p), c.shape[0], c.ctypes.data_as(C.c_void_p),
                                                counts.ctypes.data_as(C.c_void_p)), "nk_index_cluster_means")
         return c, counts
+
+
+ALL_BITS = 0xFFFFFFFFFFFFFFFF
+ADMIT_NONE = (ALL_BITS, ALL_BITS, 0)  # all_of = none_of = ~0: no row can meet it
+
+
+def as_filters(filters, Q: int) -> np.ndarray:
+    """[Q x 3] uint64 (all_of, none_of, any_of) rows, C-contiguous: the NkFilter array layout."""
+    f = np.ascontiguousarray(np.asarray(filters, dtype=np.uint64)).reshape(-1, 3)
+    if f.shape[0] != Q:
+        raise KnnError(f"filters: {f.shape[0]} rows for {Q} queries")
+    return f
+
+
+def admits(tags, all_of: int, none_of: int, any_of: int):
+    """The admissibility predicate of nk_search_filtered on host tag words (numpy; tests, callers' bookkeeping)."""
+    t = np.asarray(tags, dtype=np.uint64)
+    a, n, s = np.uint64(all_of), np.uint64(none_of), np.uint64(any_of)
+    return ((t & a) == a) & ((t & n) == 0) & ((s == 0) | ((t & s) != 0))
+
+
+def synthetic_tags(n_rows: int, seed: int, row_base: int = 0) -> np.ndarray:
+    """Synthetic tag words (bench.py, tests): splitmix64 of (seed, row), so every bit is set with probability 1/2 and a
+    row's tag depends only on (seed, row)."""
+    with np.errstate(over="ignore"):
+        z = (np.arange(row_base, row_base + n_rows, dtype=np.uint64) + np.uint64(seed) * np.uint64(0x9E3779B97F4A7C15))
+        z = z * np.uint64(0x9E3779B97F4A7C15)
+        z = (z ^ (z >> np.uint64(30))) * np.uint64(0xBF58476D1CE4E5B9)
+        z = (z ^ (z >> np.uint64(27))) * np.uint64(0x94D049BB133111EB)
+        return z ^ (z >> np.uint64(31))
+
+
+class Labels:
+    """Maps up to 64 label names (labels, types, collections, keyword values) to tag bits, in order of first use.
+
+        lab = Labels(); ix.set_row_tags(lab.row_tags([["Person"], ["Person", "Admin"], []]))
+        ix.search_filtered(q, 10, [lab.filter(must=["Person"], must_not=["Admin"])])
+    """
+
+    def __init__(self, names: Sequence[str] = ()):
+        self.bits = {}
+        for n in names:
+            self.bit(n)
+
+    def bit(self, name: str) -> int:
+        """The bit of `name`, assigned on first use; a 65th label raises."""
+        if name not in self.bits:
+            if len(self.bits) >= 64:
+                raise KnnError(f"label {name!r}: a tag word holds at most 64 labels")
+            self.bits[name] = 1 << len(self.bits)
+        return self.bits[name]
+
+    def row_tags(self, labels_per_row) -> np.ndarray:
+        """One uint64 tag word per row from an iterable of label collections."""
+        out = np.zeros(len(labels_per_row), dtype=np.uint64)
+        for r, names in enumerate(labels_per_row):
+            w = 0
+            for n in names:
+                w |= self.bit(n)
+            out[r] = w
+        return out
+
+    def filter(self, must=(), must_not=(), should=()) -> Tuple[int, int, int]:
+        """(all_of, none_of, any_of) of Qdrant-style conditions.  Names never seen: a `must` one admits no row; `must_not`
+        ones are ignored; `should` ones are ignored unless every `should` name is unknown (then no row matches)."""
+        if any(n not in self.bits for n in must):
+            return ADMIT_NONE
+        all_of = none_of = any_of = 0
+        for n in must:
+            all_of |= self.bits[n]
+        for n in must_not:
+            none_of |= self.bits.get(n, 0)
+        known = [n for n in should if n in self.bits]
+        if should and not known:
+            return ADMIT_NONE
+        for n in known:
+            any_of |= self.bits[n]
+        return all_of, none_of, any_of
 
 
 def to_bf16_bits(a) -> np.ndarray:
