@@ -186,12 +186,14 @@ __device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t a_desc,
         : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
 
-template <int N> __device__ __forceinline__ void wgmma_16bit(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc, bool f16);
-template <> __device__ __forceinline__ void wgmma_16bit<64>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc, bool f16) {
-    if (f16) wgmma_f16_n64(d, a, b, acc); else wgmma_bf16_n64(d, a, b, acc);
-}
-template <> __device__ __forceinline__ void wgmma_16bit<128>(float (&d)[64], uint64_t a, uint64_t b, uint32_t acc, bool f16) {
-    if (f16) wgmma_f16_n128(d, a, b, acc); else wgmma_bf16_n128(d, a, b, acc);
+// The wgmma form must be a compile-time choice (ptxas warning C7519 otherwise).
+template <int N, bool F16> __device__ __forceinline__ void wgmma_16bit(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc) {
+    static_assert(N == 64 || N == 128, "wgmma_16bit: N = 64 or 128");
+    if constexpr (N == 64) {
+        if constexpr (F16) wgmma_f16_n64(d, a, b, acc); else wgmma_bf16_n64(d, a, b, acc);
+    } else {
+        if constexpr (F16) wgmma_f16_n128(d, a, b, acc); else wgmma_bf16_n128(d, a, b, acc);
+    }
 }
 template <int N> __device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc);
 template <> __device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t a, uint64_t b, uint32_t acc) { wgmma_tf32_n64(d, a, b, acc); }
@@ -217,5 +219,15 @@ __device__ __forceinline__ uint32_t tf32_round_bits(uint32_t x) { return (x + 0x
 __device__ __forceinline__ void named_bar_sync(int id, int nthreads) {
     asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// Signal a named barrier without waiting on it (the threads that bar.sync on it wait for nthreads arrivals in all).
+__device__ __forceinline__ void named_bar_arrive(int id, int nthreads) {
+    asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
+}
+
+// Per-warp register budget of a warp-specialised kernel: every warp of a warpgroup executes the same call.  inc waits
+// until the CTA's pool holds the registers it asks for; the pool is only refilled by dec.  Every inc must therefore be
+// ordered after the dec that frees its registers: with several warps waiting, which one is served first is not defined.
+template <int REGS> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REGS)); }
+template <int REGS> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REGS)); }
 
 }}  // namespace nk::ptx

@@ -18,9 +18,12 @@
 //   warp 0      TMA: shadow slabs [256 rows x 64 bf16] (32 KB, 128B-swizzled), 5-stage ring;
 //   warp 3      TMA: query slabs [QT x 64 bf16] (8 / 16 KB), L2-resident;
 //   warps 4-11  two consumer warpgroups, one per 128-row M-tile: per slab 2 x 4 wgmma.m64nQTk16 (A and B from smem,
-//               fp32 accumulators in registers), then per tile: row norms from global, bound / compare / push straight
+//               fp32 accumulators in registers), then per tile: bound / compare / push straight
 //               from the accumulator registers, warp-level prunes (scan_tensor_shared.cuh, shared with the TF32 kernel).
-//               The TMA rings run ahead during the epilogue.
+//               The TMA rings run ahead during the epilogue.  The epilogue's global inputs (row norms, mask words, shared
+//               thresholds) are loaded at the top of the tile and have landed by the time the accumulators are ready.
+//   registers   setmaxnreg: TMA warpgroup 24, consumers 240 during the scan (no spills at QT = 128); all warps 160 for
+//               the end-of-launch emission, the producers' increase ordered after the consumers' decrease.
 // Shared-memory traffic per [256 rows x 128 queries x 64 dims]: 112 KB (A 32 w + 32 r, B 16 w + 32 r) for twice the K
 // extent of a TF32 slab: half the bytes per product of the TF32 kernel, which is shared-memory-bandwidth bound at 128
 // query columns.  Algorithmic HBM bytes per launch: n * dimpad * 2 (shadow) + n * 8 (norms).
@@ -41,6 +44,12 @@ constexpr int BKB = 64;                   // bf16 per row per slab = one 128-byt
 constexpr int ASTAGES = 5;                // HBM look-ahead while the consumers run a tile's epilogue
 constexpr int A_BYTES = ROWS * 128;       // 32 KB
 constexpr int EPI_WARP0 = 4, EPI_WARPS = 8, EPI_NT = EPI_WARPS * 32;
+// Registers (setmaxnreg): the TMA warpgroup gives its share to the consumers for the scan (128 x 24 + 256 x 240 = the
+// 384 x 168 of the launch); every warp has 160 for the end-of-launch emission.  The pool is handed over in two ordered
+// steps: the consumers' increase can only be served by the producers' decrease (nothing else asks for registers
+// then), and the producers increase again only after every consumer warp has decreased (named barrier REG_BAR).
+constexpr int PRODUCER_REGS = 24, CONSUMER_REGS = 240, EMIT_REGS = 160;
+constexpr int REG_BAR = 2;                // consumers arrive after releasing their scan registers, producers wait
 constexpr int PB = tc::P_SHADOW;          // candidate buffer slots per (CTA, query)
 constexpr int PRUNE_LANE = PB / 32;       // keys per lane of a warp prune
 
@@ -133,8 +142,9 @@ struct Bf16Est {
 };
 
 // TAGS: filtered search (per-query tag filters in the keep rule, read through the read-only cache: the shared-memory budget
-// is spent on the rings); the unfiltered instantiations are TAGS = false.
-template <int QT, bool DUMP, bool TAGS>
+// is spent on the rings); the unfiltered instantiations are TAGS = false.  F16: the operands are fp16 (an fp16 corpus
+// scanned in place) instead of bf16.
+template <int QT, bool F16, bool DUMP, bool TAGS>
 __global__ void __launch_bounds__(sb::NTHREADS, 1)
 knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_q, tc::Params p) {
     using namespace sb;
@@ -188,19 +198,25 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                                    p.flags + FLAG_OVERFLOW);
     };
 
-    if (warp == 0) {
-        // ===================================== TMA producer: shadow slabs =========================
-        tma_producer<ASTAGES>(sh.ring.aempty, sub, num_tiles, sgrid, 1, nslab, false, [&](uint32_t s, uint32_t tile, uint32_t, uint32_t j) {
-            ptx::mbar_arrive_expect_tx(&sh.ring.afull[s], A_BYTES);
-            ptx::tma_load_2d(&map_rows, &sh.ring.afull[s], a_base + (size_t)s * A_BYTES, (int32_t)(j * BKB), (int32_t)(tile * ROWS), qg.a_policy);
-        });
-    } else if (warp == 3) {
-        // ===================================== TMA producer: query slabs (L2-resident) ===========
-        tma_producer<C::BSTAGES>(sh.ring.bempty, sub, num_tiles, sgrid, 1, nslab, false, [&](uint32_t s, uint32_t, uint32_t, uint32_t j) {
-            ptx::mbar_arrive_expect_tx(&sh.ring.bfull[s], C::B_BYTES);
-            ptx::tma_load_2d(&map_q, &sh.ring.bfull[s], b_base + (size_t)s * C::B_BYTES, (int32_t)(j * BKB), (int32_t)qpad_off, ptx::CACHE_EVICT_LAST);
-        });
-    } else if (warp >= EPI_WARP0) {
+    if (warp < EPI_WARP0) {
+        ptx::setmaxnreg_dec<PRODUCER_REGS>();
+        if (warp == 0) {
+            // ===================================== TMA producer: shadow slabs =========================
+            tma_producer<ASTAGES>(sh.ring.aempty, sub, num_tiles, sgrid, 1, nslab, false, [&](uint32_t s, uint32_t tile, uint32_t, uint32_t j) {
+                ptx::mbar_arrive_expect_tx(&sh.ring.afull[s], A_BYTES);
+                ptx::tma_load_2d(&map_rows, &sh.ring.afull[s], a_base + (size_t)s * A_BYTES, (int32_t)(j * BKB), (int32_t)(tile * ROWS), qg.a_policy);
+            });
+        } else if (warp == 3) {
+            // ===================================== TMA producer: query slabs (L2-resident) ===========
+            tma_producer<C::BSTAGES>(sh.ring.bempty, sub, num_tiles, sgrid, 1, nslab, false, [&](uint32_t s, uint32_t, uint32_t, uint32_t j) {
+                ptx::mbar_arrive_expect_tx(&sh.ring.bfull[s], C::B_BYTES);
+                ptx::tma_load_2d(&map_q, &sh.ring.bfull[s], b_base + (size_t)s * C::B_BYTES, (int32_t)(j * BKB), (int32_t)qpad_off, ptx::CACHE_EVICT_LAST);
+            });
+        }
+        ptx::named_bar_sync(REG_BAR, NTHREADS);  // every consumer warp is back at EMIT_REGS: the pool holds what this asks for
+        ptx::setmaxnreg_inc<EMIT_REGS>();
+    } else {
+        ptx::setmaxnreg_inc<CONSUMER_REGS>();
         // ===================================== consumers: MMA + epilogue ===========================
         // warpgroup m owns rows [128 m, 128 m + 128) of the tile as two m64 halves h; thread = 4 rows x QT/4 columns of
         // the accumulator fragments: rows rbase + 64 h + 8 r, columns cbase + 8 (j / 2) + j % 2
@@ -213,7 +229,6 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
         const int prune_at = PB - ROWS;
         const int prune_trigger = min(prune_at, max(192, 4 * (int)p.k));
         const bool euclid = p.metric == NK_METRIC_EUCLIDEAN;
-        const bool op_f16 = p.op_f16 != 0;
         const bool eprof = prof && ewarp == 0 && lane == 0;
         unsigned long long t_prune = 0, t_wait = 0, t_a = 0;
         float acc[2][QT / 2];
@@ -224,6 +239,20 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
         uint32_t g = 0, it = 0;
         for (uint32_t tile = sub; tile < num_tiles; tile += sgrid, ++it) {
             if (eprof) t_a = globaltimer_ns();
+            // The epilogue's global inputs, loaded before the MMAs: |x|^2, |dx|^2 and the mask word of this thread's 4
+            // rows, and the shared threshold of query etid (it only grows: an earlier value is still a lower bound).
+            float x2[4], d2[4];
+            uint32_t mword[4];
+#pragma unroll
+            for (uint32_t ri = 0; ri < 4; ++ri) {
+                const uint32_t row = tile * ROWS + rbase + 64 * (ri >> 1) + 8 * (ri & 1);
+                const bool in = row < p.n;
+                x2[ri] = in ? __ldg(p.xnorm2 + row) : 0.0f;
+                d2[ri] = in && p.dnorm2 ? __ldg(p.dnorm2 + row) : 0.0f;  // 16-bit corpus: no residue
+                mword[ri] = in && p.mask ? __ldg(p.mask + (row >> 5)) : ~0u;
+            }
+            const uint32_t etid = tid - EPI_WARP0 * 32;  // consumer thread: one query each (QT <= EPI_NT)
+            const uint32_t gt_pre = etid < nq ? __ldcg(p.gtau + q0 + etid) : 0u;
             uint32_t prev_sa = 0, prev_sb = 0;
             for (uint32_t j = 0; j < nslab; ++j, ++g) {
                 const uint32_t sa = g % ASTAGES, sbq = g % C::BSTAGES;
@@ -237,7 +266,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                 for (uint32_t h = 0; h < 2; ++h) {
                     const uint64_t adesc = ptx::make_smem_desc_sw128(abase + h * (A_BYTES / 4));
 #pragma unroll
-                    for (uint32_t kk = 0; kk < 4; ++kk) ptx::wgmma_16bit<QT>(acc[h], adesc + kk * 2, bdesc + kk * 2, (j | kk) != 0, op_f16);
+                    for (uint32_t kk = 0; kk < 4; ++kk) ptx::wgmma_16bit<QT, F16>(acc[h], adesc + kk * 2, bdesc + kk * 2, (j | kk) != 0);
                 }
                 ptx::wgmma_commit();
                 if (j > 0) {  // the previous slab's MMAs are done while this slab's run: its stages go back to the producers
@@ -265,15 +294,15 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                 const uint32_t h = ri >> 1, r = ri & 1;
                 const uint32_t rt = rbase + 64 * h + 8 * r;  // row within the tile
                 const uint32_t row = tile * ROWS + rt;
-                const bool alive = row_alive(p, row);
+                const bool alive = row < p.n && ((mword[ri] >> (row & 31)) & 1u);
                 Bf16Est est;
-                est.x2 = row < p.n ? __ldg(p.xnorm2 + row) : 0.0f;
+                est.x2 = x2[ri];
                 est.qa = sh.qa;
                 est.qb = sh.qb;
                 est.qn = sh.qn;
                 est.euclid = euclid;
                 const float xn = sqrtf(est.x2);
-                const float dxn = sqrtf((row < p.n && p.dnorm2) ? __ldg(p.dnorm2 + row) : 0.0f) * 1.0001f;  // 16-bit corpus: no residue
+                const float dxn = sqrtf(d2[ri]) * 1.0001f;
                 est.mul = 1.0f; est.ra = dxn; est.rb = xn;
                 if (cosine) {
                     est.mul = est.x2 > 0.0f ? 1.0f / xn : 0.0f;
@@ -298,9 +327,11 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                              });
             group_sync(EPI_BAR, EPI_NT);
             if (eprof) t_prune += globaltimer_ns() - t_a;
-            adopt_shared_tau(p, q0, nq, tid - EPI_WARP0 * 32, sh.tau);
+            if (etid < nq) sh.tau[etid] = raise_to_shared_tau(gt_pre, sh.tau[etid]);  // adopt the shared threshold
         }
         if (eprof) { g_sb_prof[blockIdx.x][3] = globaltimer_ns(); g_sb_prof[blockIdx.x][5] = t_prune; g_sb_prof[blockIdx.x][7] = t_wait; }
+        ptx::setmaxnreg_dec<EMIT_REGS>();
+        ptx::named_bar_arrive(REG_BAR, NTHREADS);
     }
 
     // ---- emit: everything inside this CTA's margin AND above the shared threshold goes to the query's shared list.
@@ -465,7 +496,7 @@ bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a) {
     return a.dim % 8 == 0;  // 16-bit rows: 16-byte TMA row stride and 128-bit exact re-scoring loads
 }
 
-template <int QT, bool DUMP, bool TAGS = false>
+template <int QT, bool F16, bool DUMP, bool TAGS>
 static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
     using namespace sb;
     const bool native = a.shadow_native;  // 16-bit corpus scanned in place: row stride dim * 2, columns past dim read as zero (TMA OOB fill)
@@ -479,10 +510,10 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
         set_error("shadow tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;
     }
-    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, DUMP, TAGS>), di.device_id, smem)) return -1;
+    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, F16, DUMP, TAGS>), di.device_id, smem)) return -1;
     tc::Params p = pass_params(a, ws, sp);
-    p.nslab = sp.dimpad / BKB; p.qa = sp.qa; p.qb = sp.qb; p.xnorm2 = a.xnorm2; p.dnorm2 = a.dnorm2; p.op_f16 = a.dtype == NK_DTYPE_F16;
-    knn_scan_shadow_kernel<QT, DUMP, TAGS><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
+    p.nslab = sp.dimpad / BKB; p.qa = sp.qa; p.qb = sp.qb; p.xnorm2 = a.xnorm2; p.dnorm2 = a.dnorm2;
+    knn_scan_shadow_kernel<QT, F16, DUMP, TAGS><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
     NK_CUDA_OK(cudaGetLastError());
     if (launches) ++*launches;
     if (a.main_launches) ++*a.main_launches;
@@ -490,11 +521,19 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
     return 0;
 }
 
-int launch_shadow_pass(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
-    if (sp.dump_est) return launch_shadow_pass_t<64, true>(di, a, ws, sp, launches);
+template <bool F16>
+static int launch_shadow_pass_op(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
+    if (sp.dump_est) return launch_shadow_pass_t<64, F16, true, false>(di, a, ws, sp, launches);
     if (a.qfilter)
-        return qt == 128 ? launch_shadow_pass_t<128, false, true>(di, a, ws, sp, launches) : launch_shadow_pass_t<64, false, true>(di, a, ws, sp, launches);
-    return qt == 128 ? launch_shadow_pass_t<128, false>(di, a, ws, sp, launches) : launch_shadow_pass_t<64, false>(di, a, ws, sp, launches);
+        return qt == 128 ? launch_shadow_pass_t<128, F16, false, true>(di, a, ws, sp, launches)
+                         : launch_shadow_pass_t<64, F16, false, true>(di, a, ws, sp, launches);
+    return qt == 128 ? launch_shadow_pass_t<128, F16, false, false>(di, a, ws, sp, launches)
+                     : launch_shadow_pass_t<64, F16, false, false>(di, a, ws, sp, launches);
+}
+
+// fp16 corpora run the fp16 wgmma form; fp32 shards (BF16 shadow) and bf16 corpora the bf16 one
+int launch_shadow_pass(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
+    return a.dtype == NK_DTYPE_F16 ? launch_shadow_pass_op<true>(qt, di, a, ws, sp, launches) : launch_shadow_pass_op<false>(qt, di, a, ws, sp, launches);
 }
 
 }  // namespace nk

@@ -68,7 +68,6 @@ struct Params {
                               // whose upper bound is below it are never buffered (-inf = none)
     float *dump_est, *dump_bnd;  // DUMP kernels only (tests): per (row, query) score estimate and error bound, [n][dump_ld]
     uint32_t dump_ld;
-    int op_f16;               // 16-bit kernel: operands are fp16 (an fp16 corpus scanned in place) instead of bf16
     const uint64_t *row_tags; // TAGS kernels only: tag word per local row
     const NkFilter *qfilter;  // TAGS kernels only: filter per query [Q], indexed like gtau (absolute query index)
 };
@@ -134,11 +133,10 @@ __device__ __forceinline__ long long tma_producer(uint64_t *empty, uint32_t firs
     return waited;
 }
 
+// t raised to a shared threshold word g read earlier (0 = none published yet)
+__device__ __forceinline__ float raise_to_shared_tau(uint32_t g, float t) { return g ? fmaxf(t, ord_to_float(g)) : t; }
 // t raised to the query's cross-CTA shared threshold, if any CTA has published one
-__device__ __forceinline__ float with_shared_tau(const uint32_t *gtau_q, float t) {
-    const uint32_t g = __ldcg(gtau_q);
-    return g ? fmaxf(t, ord_to_float(g)) : t;
-}
+__device__ __forceinline__ float with_shared_tau(const uint32_t *gtau_q, float t) { return raise_to_shared_tau(__ldcg(gtau_q), t); }
 // Start threshold of a query: the caller's score floor and, when the prep kernel sampled the shard, a lower bound of the
 // query's k-th best score (no flood tiles then).
 __device__ __forceinline__ float start_tau(const Params &p, uint32_t q0, uint32_t qi, uint32_t nq) {
