@@ -253,6 +253,22 @@ int nk_search_filtered(NkIndex *ix, const float *queries_host, const NkFilter *f
 int nk_search_filtered_device(NkIndex *ix, const float *queries_dev, const NkFilter *filters_dev, uint32_t Q, uint32_t k,
                               uint32_t *out_idx_dev, float *out_score_dev, void *stream);
 
+/* ---- Range search ------------------------------------------------------------------------------------------------------
+ * Every admissible row whose score reaches the query's threshold (Cypher WHERE vector.similarity.* >= t, auto-links above a
+ * similarity threshold, near-duplicate checks): no k.  thresholds_host [Q]: cosine / dot a minimum score, euclidean a
+ * maximum distance (rows whose returned distance, sqrtf of the fp32 squared distance, is <= t; t < 0 admits none).  filters_host: NULL or [Q] NkFilters
+ * (nk_search_filtered).  The row mask and the score floor apply too; where floor and threshold disagree the stricter wins.
+ * Row r is returned for query q iff it is admissible and its exact fp32 score (the arithmetic of nk_search) meets the
+ * threshold; a NaN or -inf score (euclidean: NaN or infinite distance) never does.
+ * Results in CSR layout: query q's are [out_offsets[q], out_offsets[q+1]) of out_idx (global row ids) / out_score
+ * (euclidean: the distance), in nk_search's order (score desc / distance asc, ties by row asc).
+ * Size protocol (like snprintf): out_offsets [Q+1] and *out_total are always written and exact; if *out_total > capacity
+ * nothing else is written and the call returns 0 — allocate *out_total and call again.  Returns 0, or -1 with
+ * nk_last_error (NaN threshold, no device memory for the survivors, ...).  Synchronous, any number of devices. */
+int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresholds_host, const NkFilter *filters_host,
+                    uint32_t Q, uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx, float *out_score,
+                    uint64_t *out_total);
+
 /* Multi-process sharding (one rank per GPU): emit this shard's sorted candidate list as packed 64-bit
  * keys [Q x k] (order-preserving score bits << 32 | ~row index; larger key = better), to be exchanged
  * (e.g. ncclAllGather of Q*k*8 bytes per rank) and merged with nk_merge_keys_device. */

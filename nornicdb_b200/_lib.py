@@ -76,6 +76,7 @@ SIGNATURES = {
     "nk_index_set_row_tags": (_i, [_vp, _u64, _vp, _u64]),
     "nk_search_filtered": (_i, [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp]),
     "nk_search_filtered_device": (_i, [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp]),
+    "nk_search_range": (_i, [_vp, _vp, _vp, _vp, C.c_uint32, _u64, _vp, _vp, _vp, _vp]),
     "nk_search_keys_device":(_i, [_vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp]),
     "nk_merge_keys_device": (_i, [_i, _vp, C.c_uint32, C.c_uint32, C.c_uint32, _i, _vp, _vp, _vp]),
     "nk_score_subset": (_i, [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp]),

@@ -31,6 +31,10 @@ int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, u
                   uint64_t *launches, void **scratch, size_t *scratch_bytes);
 int build_shadow(const float *rows, uint64_t first, uint64_t count, uint32_t dim, uint32_t dimpad, void *shadow, float *xnorm2,
                  float *dnorm2, cudaStream_t stream);
+int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const uint32_t *thr_bits, Workspace &ws, uint64_t *launches,
+                     int *counts, uint32_t *list_cap, int *retried);
+int range_sorted_keys(const DeviceInfo &di, Workspace &ws, cudaStream_t stream, uint32_t Q, const int *counts, uint32_t list_cap,
+                      std::vector<uint64_t> *keys, uint64_t *launches);
 }
 
 struct NkShard {
@@ -318,6 +322,21 @@ static int run_scan_bigk(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q
     return 0;
 }
 
+// a with the shard's 16-bit image attached, if it has an up-to-date one: the BF16 shadow of an fp32 shard, or a 16-bit
+// shard's own rows
+static nk::ScanArgs with_16bit_image(const NkIndex *ix, const NkShard &s, const nk::ScanArgs &a) {
+    nk::ScanArgs as = a;
+    if (s.xnorm2 && s.shadow_n == s.n) {
+        if (ix->dtype == NK_DTYPE_F32) {
+            as.shadow = s.shadow; as.dnorm2 = s.dnorm2;
+        } else {
+            as.shadow = s.rows; as.shadow_native = true;
+        }
+        as.shadow_dimpad = ix->dimpad(); as.xnorm2 = s.xnorm2;
+    }
+    return as;
+}
+
 static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uint32_t k, uint64_t *out_keys,
                     cudaStream_t stream, const ScanOut &xo) {
     s.last_filter = false;
@@ -339,15 +358,7 @@ static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uin
     // on.  With a BF16 shadow the filter streams half the bytes of the fp32 rows, so it serves every batch size once the
     // shard is large enough for bytes (not launches) to matter; small shards keep the CUDA-core scan at Q <= 4.  16-bit
     // shards: the 16-bit tensor pass from 5 queries on.
-    nk::ScanArgs as = a;  // with the 16-bit image attached (if the shard has an up-to-date one)
-    if (s.xnorm2 && s.shadow_n == s.n) {
-        if (ix->dtype == NK_DTYPE_F32) {
-            as.shadow = s.shadow; as.dnorm2 = s.dnorm2;
-        } else {
-            as.shadow = s.rows; as.shadow_native = true;
-        }
-        as.shadow_dimpad = ix->dimpad(); as.xnorm2 = s.xnorm2;
-    }
+    const nk::ScanArgs as = with_16bit_image(ix, s, a);
     const bool tensor_ok = nk::scan_tensor_supported(s.di, a);
     const bool filter_ok = ix->dtype == NK_DTYPE_F32 && nk::scan_tensor_filter_supported(s.di, a);
     const bool shadow_ok = as.shadow != nullptr && nk::shadow_pass_supported(s.di, as) && nk::scan_tensor_filter_supported(s.di, as);
@@ -1094,6 +1105,157 @@ int nk_search(NkIndex *ix, const float *queries_host, uint32_t Q, uint32_t k, ui
 int nk_search_filtered(NkIndex *ix, const float *queries_host, const NkFilter *filters_host, uint32_t Q, uint32_t k,
                        uint32_t *out_idx, float *out_score) {
     return search_host(ix, queries_host, filters_host, Q, k, out_idx, out_score);
+}
+
+// ---- range search ---------------------------------------------------------------------------------------------------
+// Threshold of the API (cosine / dot: minimum score; euclidean: maximum distance) -> key space (score; -distance^2), the
+// index floor folded in: the stricter one wins.  Euclidean: a row qualifies iff the distance it is returned with,
+// sqrtf(d), is <= t, i.e. iff d <= the largest float whose sqrtf is <= t (sqrtf is correctly rounded, here as on the device),
+// so a threshold taken from a returned distance admits that row.  A negative maximum distance admits no row.
+static float range_key_threshold(const NkIndex *ix, float t) {
+    float key = t;
+    if (ix->metric == NK_METRIC_EUCLIDEAN) {
+        if (t < 0.0f) {
+            key = INFINITY;
+        } else if (t == INFINITY) {
+            key = -INFINITY;
+        } else {
+            float d = t * t;
+            while (d < INFINITY && sqrtf(nextafterf(d, INFINITY)) <= t) d = nextafterf(d, INFINITY);
+            while (d > 0.0f && sqrtf(d) > t) d = nextafterf(d, 0.0f);
+            key = -d;
+        }
+    }
+    return std::max(key, ix->key_floor());
+}
+
+int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresholds_host, const NkFilter *filters_host, uint32_t Q,
+                    uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total) {
+    nk::DeviceGuard _restore_device;
+    if (!ix) { nk::set_error("null index"); return -1; }
+    if (!out_offsets || !out_total) { nk::set_error("null argument"); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
+    out_offsets[0] = 0;
+    *out_total = 0;
+    if (Q == 0) return 0;
+    if (!queries_host || !thresholds_host) { nk::set_error("null argument"); return -1; }
+    std::vector<uint32_t> thr(Q);
+    for (uint32_t q = 0; q < Q; ++q) {
+        if (thresholds_host[q] != thresholds_host[q]) { nk::set_error("nk_search_range: threshold of query %u is NaN", q); return -1; }
+        thr[q] = nk::ord_bits(range_key_threshold(ix, thresholds_host[q]));
+    }
+    ix->stats.searches++;
+    ix->stats.queries += Q;
+    NK_RANGE_PUSH("nk_search_range");
+    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+    std::vector<NkShard *> live;
+    for (auto &s : ix->shards)
+        if (s.n) live.push_back(&s);
+    const size_t qbytes = (size_t)Q * ix->dim * sizeof(float);
+    std::vector<std::vector<int>> counts(live.size(), std::vector<int>(Q, 0));
+    std::vector<uint32_t> list_cap(live.size());
+    for (size_t i = 0; i < live.size(); ++i) {
+        NkShard &s = *live[i];
+        NK_CUDA_OK(cudaSetDevice(s.device));
+        if (nk::ws_reserve((void **)&s.ws.queries, &s.ws.queries_bytes, qbytes)) return -1;
+        NK_CUDA_OK(cudaMemcpyAsync(s.ws.queries, queries_host, qbytes, cudaMemcpyHostToDevice, s.stream));
+        ix->stats.bytes_h2d += qbytes;
+        nk::ScanArgs a;
+        a.rows = s.rows; a.dtype = ix->dtype; a.n = (uint32_t)s.n; a.dim = ix->dim; a.row_base = s.base;
+        a.queries = s.ws.queries; a.Q = Q; a.k = 1; a.metric = ix->metric; a.stream = s.stream;
+        a.row_mask = s.mask_on ? s.mask : nullptr; a.min_score = ix->key_floor();
+        if (filters_host) {
+            const size_t fbytes = (size_t)Q * sizeof(NkFilter);
+            if (shard_tags_on(s)) return -1;
+            if (nk::ws_reserve((void **)&s.ws.qfilter, &s.ws.qfilter_bytes, fbytes)) return -1;
+            NK_CUDA_OK(cudaMemcpyAsync(s.ws.qfilter, filters_host, fbytes, cudaMemcpyHostToDevice, s.stream));
+            ix->stats.bytes_h2d += fbytes;
+            a.row_tags = s.tags; a.qfilter = s.ws.qfilter;
+        }
+        // Paths: the 16-bit and TF32 filters with fixed thresholds, or the CUDA-core scan; AUTO picks as nk_search does (the
+        // exact 3xTF32 scan has no range mode).
+        const nk::ScanArgs as = with_16bit_image(ix, s, a);
+        const bool filter_ok = ix->dtype == NK_DTYPE_F32 && nk::scan_tensor_filter_supported(s.di, a);
+        const bool shadow_ok = as.shadow != nullptr && nk::shadow_pass_supported(s.di, as) && nk::scan_tensor_filter_supported(s.di, as);
+        int use = NK_PATH_SIMT;
+        if (ix->path == NK_PATH_TENSOR) {
+            nk::set_error("nk_search_range: the exact 3xTF32 path has no range mode (use AUTO, SIMT, TENSOR_FILTER or TENSOR_SHADOW)");
+            return -1;
+        } else if (ix->path == NK_PATH_TENSOR_FILTER || ix->path == NK_PATH_TENSOR_SHADOW) {
+            if (!(ix->path == NK_PATH_TENSOR_FILTER ? filter_ok : shadow_ok)) {
+                nk::set_error("tensor path %d does not support this shape (dim=%u dtype=%d metric=%d shadow=%d)", ix->path, ix->dim, ix->dtype,
+                              ix->metric, (int)(as.shadow != nullptr));
+                return -1;
+            }
+            use = ix->path;
+        } else if (ix->path == NK_PATH_AUTO) {
+            const bool big_shard = (uint64_t)s.n * ix->dim * 4 >= (64ull << 20);
+            if (Q >= 5) use = shadow_ok ? NK_PATH_TENSOR_SHADOW : filter_ok ? NK_PATH_TENSOR_FILTER : NK_PATH_SIMT;
+            else if (shadow_ok && big_shard && ix->dtype == NK_DTYPE_F32) use = NK_PATH_TENSOR_SHADOW;
+        }
+        cudaEvent_t e0 = nullptr, e1 = nullptr;
+        uint64_t main_launches = 0;
+        nk::ScanArgs b = use == NK_PATH_TENSOR_SHADOW ? as : a;
+        if (ix->timing_on) {
+            NK_CUDA_OK(cudaEventCreate(&e0));
+            NK_CUDA_OK(cudaEventCreate(&e1));
+            b.ev_begin = e0; b.ev_end = e1; b.main_launches = &main_launches;
+        }
+        int retried = 0;
+        const int rc = nk::range_scan_shard(s.di, b, use != NK_PATH_SIMT, thr.data(), s.ws, &ix->stats.kernel_launches, counts[i].data(),
+                                            &list_cap[i], &retried);
+        if (ix->timing_on) {
+            if (rc == 0 && main_launches) {
+                s.timing.emplace_back(e0, e1);
+                s.timing_launches.push_back(main_launches);
+            } else {
+                cudaEventDestroy(e0);
+                cudaEventDestroy(e1);
+            }
+        }
+        if (rc) return -1;
+        s.last_filter = false;
+        ix->last_path = use;
+        const uint64_t passes = (uint64_t)(retried ? 2 : 1) * (use == NK_PATH_SIMT ? (Q + 7) / 8 : (Q + 127) / 128);
+        ix->stats.bytes_scanned += passes * s.n * (use == NK_PATH_TENSOR_SHADOW ? (ix->dtype == NK_DTYPE_F32 ? ix->dimpad() : ix->dim) * 2
+                                                                                 : ix->dim * ix->esz());
+    }
+    // offsets: the shards' survivors of query q are merged into one run
+    for (uint32_t q = 0; q < Q; ++q) {
+        uint64_t c = 0;
+        for (size_t i = 0; i < live.size(); ++i) c += (uint64_t)counts[i][q];
+        out_offsets[q + 1] = out_offsets[q] + c;
+    }
+    *out_total = out_offsets[Q];
+    if (*out_total > capacity || *out_total == 0) return 0;
+    if (!out_idx || !out_score) { nk::set_error("null argument"); return -1; }
+    std::vector<std::vector<uint64_t>> keys(live.size());
+    std::vector<std::vector<uint64_t>> offs(live.size(), std::vector<uint64_t>(Q + 1, 0));
+    for (size_t i = 0; i < live.size(); ++i) {
+        NK_CUDA_OK(cudaSetDevice(live[i]->device));
+        if (nk::range_sorted_keys(live[i]->di, live[i]->ws, live[i]->stream, Q, counts[i].data(), list_cap[i], &keys[i], &ix->stats.kernel_launches))
+            return -1;
+        ix->stats.bytes_d2h += keys[i].size() * 8;
+        for (uint32_t q = 0; q < Q; ++q) offs[i][q + 1] = offs[i][q] + (uint64_t)counts[i][q];
+    }
+    std::vector<uint64_t> merged, tmp;
+    for (uint32_t q = 0; q < Q; ++q) {
+        merged.clear();
+        for (size_t i = 0; i < live.size(); ++i) {  // each shard's run is sorted: merge them (keys are unique across shards)
+            tmp.resize(merged.size() + (size_t)counts[i][q]);
+            std::merge(merged.begin(), merged.end(), keys[i].begin() + offs[i][q], keys[i].begin() + offs[i][q + 1], tmp.begin(),
+                       std::greater<uint64_t>());
+            merged.swap(tmp);
+        }
+        const uint64_t o = out_offsets[q];
+        for (size_t j = 0; j < merged.size(); ++j) {
+            float sc = nk::key_score(merged[j]);
+            if (ix->metric == NK_METRIC_EUCLIDEAN) sc = sqrtf(std::max(-sc, 0.0f));
+            out_idx[o + j] = nk::key_row(merged[j]);
+            out_score[o + j] = sc;
+        }
+    }
+    return 0;
 }
 
 static int single_shard(NkIndex *ix, NkShard **out) {

@@ -89,6 +89,16 @@ struct ScanArgs {
 // Writes per-query sorted candidate keys [Q][k] to out_keys (device).
 int scan_simt(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *out_keys, uint64_t *launches);
 
+// Range search (nk_search_range, range.cu).  State in the shard workspace: ws.keys2 = [range_qa(Q)] order-preserving bits of
+// every query's key-space threshold (score floor included), then [range_qa(Q)] list fills; ws.partial = the lists
+// [Q][list_cap].  A fill counts every survivor, also those past list_cap.  range_qa mirrors the filter's padded per-query
+// arrays (Qpad + tc::QT_BIG), whose shared thresholds and fills sit at the same places.
+inline uint32_t range_qa(uint32_t Q) { return (Q + 63) / 64 * 64 + 256; }
+// 16-bit (a.shadow set) or TF32 filter scan with fixed thresholds: lists hold every pair whose UPPER bound reaches the threshold.
+int scan_tensor_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint32_t list_cap, uint64_t *launches);
+// CUDA-core scan: lists hold every pair whose exact score reaches the threshold.
+int scan_simt_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint32_t list_cap, uint64_t *launches);
+
 // Merge n_lists sorted (or unsorted) key lists per query into the best k, sorted descending.
 // key(list l, query q, slot i) = keys[l*list_stride + q*q_stride + i], i < list_len (0 = k).
 // only_if != nullptr: the kernel returns at once unless *only_if != 0 (device-side conditional fallback).

@@ -20,6 +20,7 @@
 #include <map>
 #include <mutex>
 #include <tuple>
+#include <type_traits>
 
 #include "kernels.cuh"
 
@@ -47,6 +48,13 @@ struct SimtParams {
     const uint64_t *row_tags;  // TAGS kernels only: tag word per local row
     const NkFilter *qfilter;   // TAGS kernels only: filter per query [Q]
 };
+// RANGE kernels (nk_search_range) take these on top; the top-k kernels keep their parameter block as it is.
+struct SimtRangeParams : SimtParams {
+    const uint32_t *range_tau;  // order-preserving bits of each query's fixed threshold [Q] (floor included)
+    int *range_fill;            // list fill per query [Q], counts past list_cap
+    uint32_t list_cap;          // `partial` is [Q][list_cap]
+};
+template <bool RANGE> using SimtArgs = std::conditional_t<RANGE, SimtRangeParams, SimtParams>;
 
 // ---- element loaders -------------------------------------------------------------------------
 template <typename T, bool VEC> struct Lane;
@@ -119,8 +127,10 @@ __device__ __forceinline__ void warp_reduce_scatter(float (&v)[V], int lane) {
 }
 
 // TAGS: filtered search — the owner lane also tests its (row, query) pair against the query's tag filter.
-template <typename T, bool VEC, int QT, int R, bool EUCLID, bool TAGS>
-__global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtParams p) {
+// RANGE (nk_search_range): the owner lane appends every pair whose exact score reaches the query's fixed threshold straight to
+// the query's list — no buffer, no prune, no emission, and the scores need no re-scoring.
+template <typename T, bool VEC, int QT, int R, bool EUCLID, bool TAGS, bool RANGE>
+__global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtArgs<RANGE> p) {
     pdl_trigger();  // the merge launch behind this scan may begin (it waits for this grid before reading)
     pdl_wait();     // exact-stage twin of a filter search: programmatic dependent of the finish kernel
     if (p.only_if && *p.only_if == 0) return;
@@ -148,7 +158,8 @@ __global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtParams 
         qs[i] = qi < p.nq ? p.queries[(size_t)(p.q0 + qi) * dim + j] : 0.0f;
     }
     if (tid < QT) {
-        s_tau[tid] = p.min_score;
+        if constexpr (RANGE) s_tau[tid] = (uint32_t)tid < p.nq ? ord_to_float(p.range_tau[p.q0 + tid]) : INFINITY;
+        else s_tau[tid] = p.min_score;
         s_cnt[tid] = 0;
     }
     __syncthreads();
@@ -246,8 +257,15 @@ __global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtParams 
                     float den = sqrtf(xr * s_qq[qi]);
                     s = den > 0.0f ? s / den : 0.0f;
                 }
-                if (s != s) s = -INFINITY;
-                if (s >= s_tau[qi] && s >= p.min_score) {  // (a prune with fewer than k live keys resets tau to -inf)
+                if constexpr (RANGE) {
+                    if (s > -INFINITY && s >= s_tau[qi]) {  // NaN fails both compares
+                        const int pos = atomicAdd(p.range_fill + p.q0 + qi, 1);
+                        if (pos < (int)p.list_cap) p.partial[(size_t)(p.q0 + qi) * p.list_cap + pos] = make_key(s, (uint32_t)(p.row_base + row));
+                    }
+                } else if (s != s) {
+                    s = -INFINITY;
+                }
+                if (!RANGE && s >= s_tau[qi] && s >= p.min_score) {  // (a prune with fewer than k live keys resets tau to -inf)
                     const uint64_t key = make_key(s, (uint32_t)(p.row_base + row));
                     if (!p.below || key < p.below[p.q0 + qi]) {
                         int pos = atomicAdd(&s_cnt[qi], 1);
@@ -257,6 +275,7 @@ __global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtParams 
                 }
             }
         }
+        if constexpr (RANGE) continue;
         // ---- prune any buffer that could overflow during the next interval ---------------------
         __syncthreads();
         uint32_t need = 0;
@@ -275,6 +294,7 @@ __global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtParams 
         }
     }
 
+    if constexpr (RANGE) return;
     // ---- emit this CTA's best k per query --------------------------------------------------------
     if (p.P == 512) {
         // k <= 255: one warp per query selects the best k of the (<= 512) buffered keys with the register radix select
@@ -297,40 +317,44 @@ __global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtParams 
 }
 
 // ---------------------------------------------------------------------------------------------
-typedef void (*SimtKernel)(SimtParams);
+template <bool RANGE> using SimtKernelT = void (*)(SimtArgs<RANGE>);
+typedef SimtKernelT<false> SimtKernel;
 
-template <typename T, bool VEC, bool EUCLID, bool TAGS>
-static SimtKernel pick_qt(int qt) {
+template <typename T, bool VEC, bool EUCLID, bool TAGS, bool RANGE>
+static SimtKernelT<RANGE> pick_qt(int qt) {
     if constexpr (VEC) {
         switch (qt) {
-            case 8: return knn_scan_simt_kernel<T, VEC, 8, 4, EUCLID, TAGS>;
-            case 4: return knn_scan_simt_kernel<T, VEC, 4, 8, EUCLID, TAGS>;
-            case 2: return knn_scan_simt_kernel<T, VEC, 2, 8, EUCLID, TAGS>;
-            default: return knn_scan_simt_kernel<T, VEC, 1, 8, EUCLID, TAGS>;
+            case 8: return knn_scan_simt_kernel<T, VEC, 8, 4, EUCLID, TAGS, RANGE>;
+            case 4: return knn_scan_simt_kernel<T, VEC, 4, 8, EUCLID, TAGS, RANGE>;
+            case 2: return knn_scan_simt_kernel<T, VEC, 2, 8, EUCLID, TAGS, RANGE>;
+            default: return knn_scan_simt_kernel<T, VEC, 1, 8, EUCLID, TAGS, RANGE>;
         }
     } else {
         switch (qt) {
-            case 4: return knn_scan_simt_kernel<T, VEC, 4, 8, EUCLID, TAGS>;
-            default: return knn_scan_simt_kernel<T, VEC, 1, 8, EUCLID, TAGS>;
+            case 4: return knn_scan_simt_kernel<T, VEC, 4, 8, EUCLID, TAGS, RANGE>;
+            default: return knn_scan_simt_kernel<T, VEC, 1, 8, EUCLID, TAGS, RANGE>;
         }
     }
 }
 
-template <bool TAGS>
-static SimtKernel pick_kernel_t(int dtype, bool vec, bool euclid, int qt) {
+template <bool TAGS, bool RANGE>
+static SimtKernelT<RANGE> pick_kernel_t(int dtype, bool vec, bool euclid, int qt) {
     if (dtype == NK_DTYPE_F16) {
-        if (vec) return euclid ? pick_qt<__half, true, true, TAGS>(qt) : pick_qt<__half, true, false, TAGS>(qt);
-        return euclid ? pick_qt<__half, false, true, TAGS>(qt) : pick_qt<__half, false, false, TAGS>(qt);
+        if (vec) return euclid ? pick_qt<__half, true, true, TAGS, RANGE>(qt) : pick_qt<__half, true, false, TAGS, RANGE>(qt);
+        return euclid ? pick_qt<__half, false, true, TAGS, RANGE>(qt) : pick_qt<__half, false, false, TAGS, RANGE>(qt);
     }
     if (dtype == NK_DTYPE_BF16) {
-        if (vec) return euclid ? pick_qt<__nv_bfloat16, true, true, TAGS>(qt) : pick_qt<__nv_bfloat16, true, false, TAGS>(qt);
-        return euclid ? pick_qt<__nv_bfloat16, false, true, TAGS>(qt) : pick_qt<__nv_bfloat16, false, false, TAGS>(qt);
+        if (vec) return euclid ? pick_qt<__nv_bfloat16, true, true, TAGS, RANGE>(qt) : pick_qt<__nv_bfloat16, true, false, TAGS, RANGE>(qt);
+        return euclid ? pick_qt<__nv_bfloat16, false, true, TAGS, RANGE>(qt) : pick_qt<__nv_bfloat16, false, false, TAGS, RANGE>(qt);
     }
-    if (vec) return euclid ? pick_qt<float, true, true, TAGS>(qt) : pick_qt<float, true, false, TAGS>(qt);
-    return euclid ? pick_qt<float, false, true, TAGS>(qt) : pick_qt<float, false, false, TAGS>(qt);
+    if (vec) return euclid ? pick_qt<float, true, true, TAGS, RANGE>(qt) : pick_qt<float, true, false, TAGS, RANGE>(qt);
+    return euclid ? pick_qt<float, false, true, TAGS, RANGE>(qt) : pick_qt<float, false, false, TAGS, RANGE>(qt);
 }
 static SimtKernel pick_kernel(int dtype, bool vec, bool euclid, int qt, bool tags) {
-    return tags ? pick_kernel_t<true>(dtype, vec, euclid, qt) : pick_kernel_t<false>(dtype, vec, euclid, qt);
+    return tags ? pick_kernel_t<true, false>(dtype, vec, euclid, qt) : pick_kernel_t<false, false>(dtype, vec, euclid, qt);
+}
+static SimtKernelT<true> pick_range_kernel(int dtype, bool vec, bool euclid, int qt, bool tags) {
+    return tags ? pick_kernel_t<true, true>(dtype, vec, euclid, qt) : pick_kernel_t<false, true>(dtype, vec, euclid, qt);
 }
 
 // cudaFuncSetAttribute + occupancy query once per (kernel, device, smem) instead of once per search
@@ -421,6 +445,45 @@ int scan_simt(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *
                    a.metric))
         return -1;
     if (launches) ++*launches;
+    return 0;
+}
+
+// Range mode: one launch per query group of QT <= 8 (one corpus read each), the same grid for all.
+int scan_simt_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint32_t list_cap, uint64_t *launches) {
+    if (a.n == 0 || a.Q == 0) return 0;
+    const uint32_t vec_elems = a.dtype == NK_DTYPE_F32 ? 4 : 8;
+    const bool vec = (a.dim % vec_elems == 0) && ((reinterpret_cast<uintptr_t>(a.rows) & 15) == 0);
+    const size_t smem_budget = 96 * 1024;
+    const uint32_t num_iv = (a.n + SIMT_RT - 1) / SIMT_RT;
+    const uint32_t QA = range_qa(a.Q);
+    if (a.ev_begin) NK_CUDA_OK(cudaEventRecord(a.ev_begin, a.stream));
+    for (uint32_t q0 = 0; q0 < a.Q;) {
+        const uint32_t left = a.Q - q0;
+        int qt = left >= 5 ? 8 : left >= 3 ? 4 : left == 2 ? 2 : 1;
+        if (!vec) qt = left >= 3 ? 4 : 1;
+        while (qt > 1 && (size_t)qt * a.dim * 4 > smem_budget) qt = vec ? qt / 2 : 1;
+        const size_t smem = (size_t)qt * a.dim * 4;  // the queries only: no candidate buffer
+        if (smem > di.max_smem_optin) {
+            set_error("dim=%u too large for the SIMT scan (needs %zu B shared memory)", a.dim, smem);
+            return -1;
+        }
+        SimtKernelT<true> kern = pick_range_kernel(a.dtype, vec, a.metric == NK_METRIC_EUCLIDEAN, qt, a.qfilter != nullptr);
+        if (simt_ensure(reinterpret_cast<const void *>(kern), di.device_id, smem)) return -1;
+        const int occ = simt_occupancy(reinterpret_cast<const void *>(kern), di.device_id, smem);
+        uint32_t grid = (uint32_t)di.num_sms * (uint32_t)occ;
+        if (grid > num_iv) grid = num_iv;
+        SimtRangeParams p{};
+        p.rows = a.rows; p.n = a.n; p.dim = a.dim; p.row_base = a.row_base;
+        p.queries = a.queries; p.q0 = q0; p.nq = left < (uint32_t)qt ? left : (uint32_t)qt; p.k = 1;
+        p.metric = a.metric; p.P = 0; p.partial = ws.partial; p.flags = ws.flags; p.mask = a.row_mask; p.min_score = a.min_score;
+        p.row_tags = a.row_tags; p.qfilter = a.qfilter;
+        p.range_tau = reinterpret_cast<const uint32_t *>(ws.keys2); p.range_fill = reinterpret_cast<int *>(ws.keys2) + QA; p.list_cap = list_cap;
+        NK_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(SIMT_THREADS), smem, a.stream, false, p));
+        if (launches) ++*launches;
+        if (a.main_launches) ++*a.main_launches;
+        q0 += p.nq;
+    }
+    if (a.ev_end) NK_CUDA_OK(cudaEventRecord(a.ev_end, a.stream));
     return 0;
 }
 

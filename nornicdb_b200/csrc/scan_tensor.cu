@@ -78,67 +78,6 @@ __device__ long long g_tc_prof[32];
 #define TC_PROF_BEGIN() long long _t0 = prof ? clock64() : 0
 #define TC_PROF_END(slot) do { if (prof) { long long _t1 = clock64(); acc_##slot += _t1 - _t0; } } while (0)
 
-// Exact fp32 score of one corpus row against the query staged in shared memory, by one warp: the arithmetic every
-// filter path re-scores its survivors with (fp32 FMA, 128-bit loads; fp16 rows are widened exactly).  Returns the key
-// score: dot | dot / sqrt(|x|^2 |q|^2) (0 for zero vectors, simd_amd64.go:31-35) | -|x - q|^2; NaN -> -inf.  *xx_out = |x|^2.
-__device__ __forceinline__ float warp_exact_score(const void *rows, int dtype, size_t local, uint32_t dim, const float *qs, float qq,
-                                                  int metric, int lane, float *xx_out = nullptr) {
-    float d = 0.0f, xx = 0.0f;
-    const float4 *q4 = reinterpret_cast<const float4 *>(qs);
-    auto acc4 = [&](const float4 v, const float4 u) {
-        if (metric == NK_METRIC_EUCLIDEAN) {
-            float t;
-            t = v.x - u.x; d = fmaf(t, t, d);
-            t = v.y - u.y; d = fmaf(t, t, d);
-            t = v.z - u.z; d = fmaf(t, t, d);
-            t = v.w - u.w; d = fmaf(t, t, d);
-            xx = fmaf(v.x, v.x, xx); xx = fmaf(v.y, v.y, xx); xx = fmaf(v.z, v.z, xx); xx = fmaf(v.w, v.w, xx);
-        } else {
-            d = fmaf(v.x, u.x, d); xx = fmaf(v.x, v.x, xx);
-            d = fmaf(v.y, u.y, d); xx = fmaf(v.y, v.y, xx);
-            d = fmaf(v.z, u.z, d); xx = fmaf(v.z, v.z, xx);
-            d = fmaf(v.w, u.w, d); xx = fmaf(v.w, v.w, xx);
-        }
-    };
-    if (dtype == NK_DTYPE_F32) {
-        const float4 *x4 = reinterpret_cast<const float4 *>(static_cast<const float *>(rows) + local * dim);
-#pragma unroll 8
-        for (uint32_t j = lane; j < dim / 4; j += 32) acc4(__ldg(x4 + j), q4[j]);
-    } else if (dtype == NK_DTYPE_F16) {  // fp16 rows, dim % 8 == 0: 8 halves per 128-bit load
-        const uint4 *x8 = reinterpret_cast<const uint4 *>(static_cast<const __half *>(rows) + local * dim);
-#pragma unroll 4
-        for (uint32_t j = lane; j < dim / 8; j += 32) {
-            const uint4 w = __ldg(x8 + j);
-            const float2 f0 = __half22float2(*reinterpret_cast<const __half2 *>(&w.x)), f1 = __half22float2(*reinterpret_cast<const __half2 *>(&w.y));
-            const float2 f2 = __half22float2(*reinterpret_cast<const __half2 *>(&w.z)), f3 = __half22float2(*reinterpret_cast<const __half2 *>(&w.w));
-            acc4(make_float4(f0.x, f0.y, f1.x, f1.y), q4[2 * j]);
-            acc4(make_float4(f2.x, f2.y, f3.x, f3.y), q4[2 * j + 1]);
-        }
-    } else {  // bf16 rows: widening is a 16-bit shift
-        const uint4 *x8 = reinterpret_cast<const uint4 *>(static_cast<const uint16_t *>(rows) + local * dim);
-#pragma unroll 4
-        for (uint32_t j = lane; j < dim / 8; j += 32) {
-            const uint4 w = __ldg(x8 + j);
-            acc4(make_float4(__uint_as_float(w.x << 16), __uint_as_float(w.x & 0xffff0000u), __uint_as_float(w.y << 16), __uint_as_float(w.y & 0xffff0000u)), q4[2 * j]);
-            acc4(make_float4(__uint_as_float(w.z << 16), __uint_as_float(w.z & 0xffff0000u), __uint_as_float(w.w << 16), __uint_as_float(w.w & 0xffff0000u)), q4[2 * j + 1]);
-        }
-    }
-#pragma unroll
-    for (int o = 16; o; o >>= 1) {
-        d += __shfl_xor_sync(0xffffffffu, d, o);
-        xx += __shfl_xor_sync(0xffffffffu, xx, o);
-    }
-    float sc = d;
-    if (metric == NK_METRIC_EUCLIDEAN) sc = -d;
-    else if (metric == NK_METRIC_COSINE) {
-        const float den = sqrtf(xx * qq);
-        sc = den > 0.0f ? d / den : 0.0f;
-    }
-    if (sc != sc) sc = -INFINITY;
-    if (xx_out) *xx_out = xx;
-    return sc;
-}
-
 // ---------------------------------------------------------------------------------------------------
 // filter_prep_kernel — everything a filter search needs before its scan, in ONE launch (one CTA per padded query row):
 //   * |q|, cosine normalisation; TF32 hi / lo split (TF32 filter + exact 3xTF32 stages); BF16 copy with the measured
@@ -333,7 +272,8 @@ template <bool FILTER> struct Tf32Est {
 };
 
 // TAGS: filtered search (per-query tag filters in the keep rule); the unfiltered instantiations are TAGS = false.
-template <int NT, int QT, bool DUMP, bool TAGS>
+// RANGE (filter mode only, nk_search_range): fixed per-query thresholds; full buffers are flushed to the lists, never pruned.
+template <int NT, int QT, bool DUMP, bool TAGS, bool RANGE = false>
 __global__ void __launch_bounds__(tc::THREADS, 1)
 knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_qhi,
                    const __grid_constant__ CUtensorMap map_qlo, tc::Params p) {
@@ -500,9 +440,10 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
             // prune any buffer that could overflow during the next tile; the 8 consumer warps prune different
             // queries concurrently with a register-resident warp selection
             group_sync(EPI_BAR, EPI_THREADS);  // every push of this tile is visible
-            prune_tile<FILTER>(p, q0, nq, ewarp, lane, sh.cnt, sh.tau, prune_at, prune_at, flood && it == 0, prune);
+            if constexpr (RANGE) flush_tile<P>(p, q0, nq, ewarp, lane, my_cand, sh.cnt);
+            else prune_tile<FILTER>(p, q0, nq, ewarp, lane, sh.cnt, sh.tau, prune_at, prune_at, flood && it == 0, prune);
             group_sync(EPI_BAR, EPI_THREADS);
-            if (FILTER) adopt_shared_tau(p, q0, nq, tid - EPI_WARP0 * 32, sh.tau);
+            if (FILTER && !RANGE) adopt_shared_tau(p, q0, nq, tid - EPI_WARP0 * 32, sh.tau);
         }
     }
 
@@ -510,7 +451,9 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
     // Every role has finished its tile loop here, so all 12 warps share the final prunes.
     __syncthreads();
     for (uint32_t qi = warp; qi < nq; qi += THREADS / 32) {
-        if (FILTER)
+        if (RANGE)
+            flush_query(p, q0, qi, lane, my_cand + (size_t)qi * P, sh.cnt);
+        else if (FILTER)
             emit_query(p, q0, qi, lane, my_cand + (size_t)qi * P, sh.cnt, sh.tau, prune);
         else
             prune(qi, p.partial + ((size_t)(q0 + qi) * gridDim.x + blockIdx.x) * p.k_emit, (int)p.k_emit, (int)p.k_emit, p.min_score, nullptr);
@@ -899,7 +842,7 @@ int tc_debug_flags() { return tc_env_int("NK_TC_DEBUG", 0); }
 tc::Params pass_params(const ScanArgs &a, Workspace &ws, const tc::PassArgs &t) {
     tc::Params p{};
     p.n = a.n; p.dim = a.dim; p.row_base = a.row_base;
-    p.q0 = t.q0; p.nq = t.nq; p.k = a.k; p.qpad_off = t.q0; p.qgroups = t.qgroups; p.list_cap = t.grid * t.k_emit;
+    p.q0 = t.q0; p.nq = t.nq; p.k = a.k; p.qpad_off = t.q0; p.qgroups = t.qgroups; p.list_cap = t.range ? t.list_cap : t.grid * t.k_emit;
     p.metric = a.metric; p.k_emit = t.k_emit; p.qnorm = t.qnorm;
     p.cand = ws.cand; p.partial = ws.partial; p.flags = ws.flags; p.debug = tc_debug_flags(); p.mask = a.row_mask;
     p.gtau = reinterpret_cast<uint32_t *>(ws.keys2); p.gcount = reinterpret_cast<int *>(ws.keys2) + (t.Qpad + tc::QT_BIG);
@@ -958,7 +901,7 @@ struct TcPassArgs : tc::PassArgs {
     const int *only_if;
     bool count_main;
 };
-template <int NT, int QT, bool DUMP = false, bool TAGS = false>
+template <int NT, int QT, bool DUMP = false, bool TAGS = false, bool RANGE = false>
 static int launch_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const TcPassArgs &t, uint64_t *launches) {
     using namespace tc;
     const CUtensorMap *map_rows = tc_cached_map(ws, 0, a.rows, a.n, a.dim, 4, (uint32_t)BK, ROWS, (uint64_t)a.dim * 4);
@@ -971,20 +914,23 @@ static int launch_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws,
         set_error("tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;
     }
-    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_tc_kernel<NT, QT, DUMP, TAGS>), di.device_id, smem)) return -1;
+    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_tc_kernel<NT, QT, DUMP, TAGS, RANGE>), di.device_id, smem)) return -1;
     Params p = pass_params(a, ws, t);
     p.nslab = (a.dim + BK - 1) / BK; p.margin_c = t.margin_c; p.only_if = t.only_if;
     // (asynchronous API: the early-exit retry / exact stages are programmatic dependents — their launch overlaps the kernel
     // before them.  Not for the host-synchronous API: measured 5-15 us slower per nk_search, the copy-out behind it waits longer)
-    NK_CUDA_OK(launch_pdl(knn_scan_tc_kernel<NT, QT, DUMP, TAGS>, dim3(t.grid), dim3(THREADS), smem, a.stream, t.only_if != nullptr && !a.defer_tail, *map_rows, *map_qhi,
+    NK_CUDA_OK(launch_pdl(knn_scan_tc_kernel<NT, QT, DUMP, TAGS, RANGE>, dim3(t.grid), dim3(THREADS), smem, a.stream, t.only_if != nullptr && !a.defer_tail, *map_rows, *map_qhi,
                           *map_qlo, p));
     if (launches) ++*launches;
     if (t.count_main && a.main_launches) ++*a.main_launches;
     return 0;
 }
-// Filtered searches (per-query tag filters) run the TAGS instantiation of the same kernel.
+// Filtered searches (per-query tag filters) run the TAGS instantiation of the same kernel; range searches the RANGE one.
 template <int NT, int QT, bool DUMP = false>
 static int launch_pass(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const TcPassArgs &t, uint64_t *launches) {
+    if constexpr (NT == 1 && !DUMP)
+        if (t.range)
+            return a.qfilter ? launch_pass_t<NT, QT, false, true, true>(di, a, ws, t, launches) : launch_pass_t<NT, QT, false, false, true>(di, a, ws, t, launches);
     if (!DUMP && a.qfilter) return launch_pass_t<NT, QT, false, true>(di, a, ws, t, launches);
     return launch_pass_t<NT, QT, DUMP, false>(di, a, ws, t, launches);
 }
@@ -1222,6 +1168,45 @@ int scan_tensor_filter(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, u
     fin_print_prof(a.stream, a.Q);
     if (a.defer_tail) return 0;
     return scan_tensor_filter_tail(di, a, ws, out_keys, launches);
+}
+
+// Range mode (nk_search_range, range.cu): the query prep, then the 16-bit pass (shadow attached) or the TF32 filter over the
+// fp32 rows with FIXED thresholds: ws.keys2 holds the order-preserving bits of every query's key-space threshold where the
+// filter keeps its shared thresholds (presampled: no flood tiles, nothing is published), and every pair whose upper bound
+// reaches it lands in ws.partial [Q][list_cap], fill counted in the list fills next to them (range_qa).  The caller
+// re-scores the lists exactly.
+int scan_tensor_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint32_t list_cap, uint64_t *launches) {
+    using namespace tc;
+    static_assert(QT_BIG == 256, "range_qa() (kernels.cuh) mirrors the padded per-query arrays");
+    ScanArgs b = a;
+    b.k = 1;
+    FilterPlan f;
+    if (make_filter_plan(di, b, ws, &f)) return -1;
+    if (ws_reserve((void **)&ws.partial, &ws.partial_bytes, (size_t)a.Q * list_cap * 8)) return -1;
+    PrepParams pp = filter_prep_params(b, ws, f);
+    pp.state = nullptr;  // the thresholds and list fills are the caller's
+    pp.sample = 0;
+    if (launch_prep(di, pp, a.stream, launches)) return -1;
+    if (a.ev_begin) NK_CUDA_OK(cudaEventRecord(a.ev_begin, a.stream));
+    int rc;
+    if (f.big) {
+        rc = plan_launches(0, a.Q, f.grid, 4, [&](uint32_t qt, uint32_t q0, uint32_t nq, uint32_t groups) {
+            ShadowPassArgs sp{};
+            sp.grid = f.grid; sp.k_emit = f.k_emit; sp.dimpad = f.dimpad; sp.Qpad = f.Qpad; sp.q0 = q0; sp.nq = nq; sp.qgroups = groups;
+            sp.qbf16 = f.qbf16; sp.qnorm = f.qnorm; sp.qa = f.qa; sp.qb = f.qb; sp.presampled = 1; sp.range = true; sp.list_cap = list_cap;
+            return launch_shadow_pass((int)qt, di, b, ws, sp, launches);
+        });
+    } else {
+        rc = plan_launches(0, a.Q, f.grid, 4, [&](uint32_t qt, uint32_t q0, uint32_t nq, uint32_t groups) {
+            TcPassArgs t{};
+            t.grid = f.grid; t.k_emit = f.k_emit; t.Qpad = f.Qpad; t.q0 = q0; t.nq = nq; t.qgroups = groups; t.margin_c = f.margin_tf32;
+            t.qhi = f.qhi; t.qnorm = f.qnorm; t.count_main = true; t.presampled = 1; t.range = true; t.list_cap = list_cap;
+            return qt == 128 ? launch_pass<1, 128>(di, b, ws, t, launches) : launch_pass<1, 64>(di, b, ws, t, launches);
+        });
+    }
+    if (rc) return -1;
+    if (a.ev_end) NK_CUDA_OK(cudaEventRecord(a.ev_end, a.stream));
+    return 0;
 }
 
 // ---- tests only: the filters' raw score estimates and error bounds for every (row, query) pair --------------------

@@ -143,8 +143,9 @@ struct Bf16Est {
 
 // TAGS: filtered search (per-query tag filters in the keep rule, read through the read-only cache: the shared-memory budget
 // is spent on the rings); the unfiltered instantiations are TAGS = false.  F16: the operands are fp16 (an fp16 corpus
-// scanned in place) instead of bf16.
-template <int QT, bool F16, bool DUMP, bool TAGS>
+// scanned in place) instead of bf16.  RANGE (nk_search_range): fixed per-query thresholds; full buffers are flushed to the
+// lists, never pruned, and the end of the launch flushes what is left.
+template <int QT, bool F16, bool DUMP, bool TAGS, bool RANGE>
 __global__ void __launch_bounds__(sb::NTHREADS, 1)
 knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_q, tc::Params p) {
     using namespace sb;
@@ -252,7 +253,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                 mword[ri] = in && p.mask ? __ldg(p.mask + (row >> 5)) : ~0u;
             }
             const uint32_t etid = tid - EPI_WARP0 * 32;  // consumer thread: one query each (QT <= EPI_NT)
-            const uint32_t gt_pre = etid < nq ? __ldcg(p.gtau + q0 + etid) : 0u;
+            const uint32_t gt_pre = !RANGE && etid < nq ? __ldcg(p.gtau + q0 + etid) : 0u;
             uint32_t prev_sa = 0, prev_sb = 0;
             for (uint32_t j = 0; j < nslab; ++j, ++g) {
                 const uint32_t sa = g % ASTAGES, sbq = g % C::BSTAGES;
@@ -320,14 +321,17 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             // prune any buffer that could overflow during the next tile (8 warps, different queries concurrently)
             group_sync(EPI_BAR, EPI_NT);  // every push of this tile is visible
             if (eprof) t_a = globaltimer_ns();
-            prune_tile<true>(p, q0, nq, ewarp, lane, sh.cnt, sh.tau, prune_trigger, prune_at, flood && it == 0,
-                             [&](uint32_t qi, uint64_t *out, int out_len, int max_keep, float floor_tau, int *gcount) {
-                                 if (eprof && g_sb_prof[blockIdx.x][6] == ~0ull) g_sb_prof[blockIdx.x][6] = it;
-                                 prune(qi, out, out_len, max_keep, floor_tau, gcount);
-                             });
+            if constexpr (RANGE)
+                flush_tile<PB>(p, q0, nq, ewarp, lane, my_cand, sh.cnt);
+            else
+                prune_tile<true>(p, q0, nq, ewarp, lane, sh.cnt, sh.tau, prune_trigger, prune_at, flood && it == 0,
+                                 [&](uint32_t qi, uint64_t *out, int out_len, int max_keep, float floor_tau, int *gcount) {
+                                     if (eprof && g_sb_prof[blockIdx.x][6] == ~0ull) g_sb_prof[blockIdx.x][6] = it;
+                                     prune(qi, out, out_len, max_keep, floor_tau, gcount);
+                                 });
             group_sync(EPI_BAR, EPI_NT);
             if (eprof) t_prune += globaltimer_ns() - t_a;
-            if (etid < nq) sh.tau[etid] = raise_to_shared_tau(gt_pre, sh.tau[etid]);  // adopt the shared threshold
+            if (!RANGE && etid < nq) sh.tau[etid] = raise_to_shared_tau(gt_pre, sh.tau[etid]);  // adopt the shared threshold
         }
         if (eprof) { g_sb_prof[blockIdx.x][3] = globaltimer_ns(); g_sb_prof[blockIdx.x][5] = t_prune; g_sb_prof[blockIdx.x][7] = t_wait; }
         ptx::setmaxnreg_dec<EMIT_REGS>();
@@ -336,7 +340,9 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
 
     // ---- emit: everything inside this CTA's margin AND above the shared threshold goes to the query's shared list.
     __syncthreads();
-    {
+    if constexpr (RANGE) {  // range mode: what the last flushes left, whole (no staging: one buffer per warp at a time)
+        for (uint32_t qi = warp; qi < nq; qi += NTHREADS / 32) flush_query(p, q0, qi, lane, my_cand + (size_t)qi * PB, sh.cnt);
+    } else {
         // Fast path (buffers with <= k_emit entries, i.e. almost always all of them): no selection, the finish kernel selects
         // globally — append what still reaches the current threshold.  The buffers live in global memory (L2); walking them
         // query by query was a chain of dependent round trips (~19 us at the end of every launch, measured).  Instead: the
@@ -496,7 +502,7 @@ bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a) {
     return a.dim % 8 == 0;  // 16-bit rows: 16-byte TMA row stride and 128-bit exact re-scoring loads
 }
 
-template <int QT, bool F16, bool DUMP, bool TAGS>
+template <int QT, bool F16, bool DUMP, bool TAGS, bool RANGE = false>
 static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
     using namespace sb;
     const bool native = a.shadow_native;  // 16-bit corpus scanned in place: row stride dim * 2, columns past dim read as zero (TMA OOB fill)
@@ -510,10 +516,10 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
         set_error("shadow tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;
     }
-    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, F16, DUMP, TAGS>), di.device_id, smem)) return -1;
+    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, F16, DUMP, TAGS, RANGE>), di.device_id, smem)) return -1;
     tc::Params p = pass_params(a, ws, sp);
     p.nslab = sp.dimpad / BKB; p.qa = sp.qa; p.qb = sp.qb; p.xnorm2 = a.xnorm2; p.dnorm2 = a.dnorm2;
-    knn_scan_shadow_kernel<QT, F16, DUMP, TAGS><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
+    knn_scan_shadow_kernel<QT, F16, DUMP, TAGS, RANGE><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
     NK_CUDA_OK(cudaGetLastError());
     if (launches) ++*launches;
     if (a.main_launches) ++*a.main_launches;
@@ -524,6 +530,13 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
 template <bool F16>
 static int launch_shadow_pass_op(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
     if (sp.dump_est) return launch_shadow_pass_t<64, F16, true, false>(di, a, ws, sp, launches);
+    if (sp.range) {
+        if (a.qfilter)
+            return qt == 128 ? launch_shadow_pass_t<128, F16, false, true, true>(di, a, ws, sp, launches)
+                             : launch_shadow_pass_t<64, F16, false, true, true>(di, a, ws, sp, launches);
+        return qt == 128 ? launch_shadow_pass_t<128, F16, false, false, true>(di, a, ws, sp, launches)
+                         : launch_shadow_pass_t<64, F16, false, false, true>(di, a, ws, sp, launches);
+    }
     if (a.qfilter)
         return qt == 128 ? launch_shadow_pass_t<128, F16, false, true>(di, a, ws, sp, launches)
                          : launch_shadow_pass_t<64, F16, false, true>(di, a, ws, sp, launches);

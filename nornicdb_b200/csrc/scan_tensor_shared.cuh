@@ -80,6 +80,8 @@ struct PassArgs {
     int presampled;
     float *dump_est = nullptr, *dump_bnd = nullptr;  // test-only DUMP instantiations
     uint32_t dump_ld = 0;
+    bool range = false;       // range mode (nk_search_range): gtau[] holds fixed thresholds, survivors go to lists of list_cap
+    uint32_t list_cap = 0;
 };
 
 #ifdef __CUDACC__
@@ -287,6 +289,24 @@ __device__ __forceinline__ void emit_query(const Params &p, uint32_t q0, uint32_
     if (lane == 0 && tau[qi] > -INFINITY) atomicMax(p.gtau + q0 + qi, ord_bits(tau[qi]));
 }
 
+// Range mode (nk_search_range): the threshold is fixed (gtau[] holds it from the start, presampled), so a buffer is never
+// pruned: every key in it reached the threshold when it was pushed, and the buffer goes whole to the query's list and starts
+// over.  The list fill counts past list_cap, so a pass whose lists were too short still knows its exact survivor count.
+__device__ __forceinline__ void flush_query(const Params &p, uint32_t q0, uint32_t qi, int lane, const uint64_t *cand, int *cnt) {
+    warp_emit_above(cand, cnt[qi], 1ull, lane, p.partial + (size_t)(q0 + qi) * p.list_cap, (int)p.list_cap, p.gcount + q0 + qi);
+    __syncwarp();
+    if (lane == 0) cnt[qi] = 0;
+    __syncwarp();
+}
+// End of a tile in range mode (in place of prune_tile, after the same barrier): warp ewarp of the consumers flushes queries
+// ewarp, ewarp + 8, .. whose buffer could overflow during the next tile (a tile pushes at most ROWS keys per query).
+template <int CAP>
+__device__ __forceinline__ void flush_tile(const Params &p, uint32_t q0, uint32_t nq, uint32_t ewarp, int lane, const uint64_t *cand,
+                                           int *cnt) {
+    for (uint32_t qi = ewarp; qi < nq; qi += EPI_THREADS / 32)
+        if (cnt[qi] > CAP - ROWS) flush_query(p, q0, qi, lane, cand + (size_t)qi * CAP, cnt);
+}
+
 __device__ __forceinline__ unsigned long long globaltimer_ns() {
     unsigned long long t;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)::"memory");
@@ -297,6 +317,67 @@ __device__ __forceinline__ unsigned long long globaltimer_ns() {
 }  // namespace tc
 
 #ifdef __CUDACC__
+// Exact fp32 score of one corpus row against the query staged in shared memory, by one warp: the arithmetic every
+// filter path re-scores its survivors with (filter_finish_kernel, range_rescore_kernel) (fp32 FMA, 128-bit loads; fp16 rows are widened exactly).  Returns the key
+// score: dot | dot / sqrt(|x|^2 |q|^2) (0 for zero vectors, simd_amd64.go:31-35) | -|x - q|^2; NaN -> -inf.  *xx_out = |x|^2.
+__device__ __forceinline__ float warp_exact_score(const void *rows, int dtype, size_t local, uint32_t dim, const float *qs, float qq,
+                                                  int metric, int lane, float *xx_out = nullptr) {
+    float d = 0.0f, xx = 0.0f;
+    const float4 *q4 = reinterpret_cast<const float4 *>(qs);
+    auto acc4 = [&](const float4 v, const float4 u) {
+        if (metric == NK_METRIC_EUCLIDEAN) {
+            float t;
+            t = v.x - u.x; d = fmaf(t, t, d);
+            t = v.y - u.y; d = fmaf(t, t, d);
+            t = v.z - u.z; d = fmaf(t, t, d);
+            t = v.w - u.w; d = fmaf(t, t, d);
+            xx = fmaf(v.x, v.x, xx); xx = fmaf(v.y, v.y, xx); xx = fmaf(v.z, v.z, xx); xx = fmaf(v.w, v.w, xx);
+        } else {
+            d = fmaf(v.x, u.x, d); xx = fmaf(v.x, v.x, xx);
+            d = fmaf(v.y, u.y, d); xx = fmaf(v.y, v.y, xx);
+            d = fmaf(v.z, u.z, d); xx = fmaf(v.z, v.z, xx);
+            d = fmaf(v.w, u.w, d); xx = fmaf(v.w, v.w, xx);
+        }
+    };
+    if (dtype == NK_DTYPE_F32) {
+        const float4 *x4 = reinterpret_cast<const float4 *>(static_cast<const float *>(rows) + local * dim);
+#pragma unroll 8
+        for (uint32_t j = lane; j < dim / 4; j += 32) acc4(__ldg(x4 + j), q4[j]);
+    } else if (dtype == NK_DTYPE_F16) {  // fp16 rows, dim % 8 == 0: 8 halves per 128-bit load
+        const uint4 *x8 = reinterpret_cast<const uint4 *>(static_cast<const __half *>(rows) + local * dim);
+#pragma unroll 4
+        for (uint32_t j = lane; j < dim / 8; j += 32) {
+            const uint4 w = __ldg(x8 + j);
+            const float2 f0 = __half22float2(*reinterpret_cast<const __half2 *>(&w.x)), f1 = __half22float2(*reinterpret_cast<const __half2 *>(&w.y));
+            const float2 f2 = __half22float2(*reinterpret_cast<const __half2 *>(&w.z)), f3 = __half22float2(*reinterpret_cast<const __half2 *>(&w.w));
+            acc4(make_float4(f0.x, f0.y, f1.x, f1.y), q4[2 * j]);
+            acc4(make_float4(f2.x, f2.y, f3.x, f3.y), q4[2 * j + 1]);
+        }
+    } else {  // bf16 rows: widening is a 16-bit shift
+        const uint4 *x8 = reinterpret_cast<const uint4 *>(static_cast<const uint16_t *>(rows) + local * dim);
+#pragma unroll 4
+        for (uint32_t j = lane; j < dim / 8; j += 32) {
+            const uint4 w = __ldg(x8 + j);
+            acc4(make_float4(__uint_as_float(w.x << 16), __uint_as_float(w.x & 0xffff0000u), __uint_as_float(w.y << 16), __uint_as_float(w.y & 0xffff0000u)), q4[2 * j]);
+            acc4(make_float4(__uint_as_float(w.z << 16), __uint_as_float(w.z & 0xffff0000u), __uint_as_float(w.w << 16), __uint_as_float(w.w & 0xffff0000u)), q4[2 * j + 1]);
+        }
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        d += __shfl_xor_sync(0xffffffffu, d, o);
+        xx += __shfl_xor_sync(0xffffffffu, xx, o);
+    }
+    float sc = d;
+    if (metric == NK_METRIC_EUCLIDEAN) sc = -d;
+    else if (metric == NK_METRIC_COSINE) {
+        const float den = sqrtf(xx * qq);
+        sc = den > 0.0f ? d / den : 0.0f;
+    }
+    if (sc != sc) sc = -INFINITY;
+    if (xx_out) *xx_out = xx;
+    return sc;
+}
+
 // Filter mode: 2 x (largest possible gap between an upper bound and the true score) for rows with |x|^2 <= maxxx.
 //   cosine 2c | dot 2c|x||q| | euclidean (on -dist^2) 2(2c|x||q| + eps(|x|^2+|q|^2))
 __device__ __forceinline__ float filter_margin2(int metric, float c, float maxxx, float qn) {

@@ -291,6 +291,33 @@ public:
             }
         return out;
     }
+    // Every node whose similarity reaches the query's threshold (cosine / dot: minimum score; euclidean: maximum distance),
+    // best first; filters empty = none, else one per query.  Sizes its buffers from the library's exact total.
+    std::vector<std::vector<SearchResult>> SearchRange(const std::vector<float> &queries, const std::vector<float> &thresholds,
+                                                       const std::vector<NkFilter> &filters, uint32_t Q) {
+        if (queries.size() != (size_t)Q * dims_) throw ErrInvalidDimensions();
+        if (thresholds.size() != Q) throw std::invalid_argument("gpu: one threshold per query");
+        if (!filters.empty() && filters.size() != Q) throw std::invalid_argument("gpu: one filter per query");
+        std::lock_guard<std::mutex> lk(mu_);
+        std::vector<std::vector<SearchResult>> out(Q);
+        if (nodeIDs_.empty() || Q == 0) return out;
+        std::vector<uint64_t> off((size_t)Q + 1);
+        std::vector<uint32_t> idx;
+        std::vector<float> sc;
+        uint64_t total = 0;
+        for (int pass = 0; pass < 2; ++pass) {
+            if (nk_search_range(ix_, queries.data(), thresholds.data(), filters.empty() ? nullptr : filters.data(), Q, idx.size(), off.data(),
+                                idx.data(), sc.data(), &total) < 0)
+                throw cuda::ErrKernelExecution(std::string("gpu: ") + nk_last_error());
+            if (total <= idx.size()) break;
+            idx.resize(total);
+            sc.resize(total);
+        }
+        for (uint32_t q = 0; q < Q; ++q)
+            for (uint64_t i = off[q]; i < off[q + 1]; ++i)
+                if (idx[i] < nodeIDs_.size()) out[q].push_back({nodeIDs_[idx[i]], sc[i], 1.0f - sc[i]});
+        return out;
+    }
     std::vector<SearchResult> ScoreSubset(const std::vector<float> &query, const std::vector<std::string> &ids) {  // gpu.go:1552-1616
         if ((int)query.size() != dims_) throw ErrInvalidDimensions();
         std::lock_guard<std::mutex> lk(mu_);

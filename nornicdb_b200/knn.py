@@ -6,7 +6,7 @@ time by one fused distance + top-k kernel per shard."""
 from __future__ import annotations
 
 import ctypes as C
-from typing import Optional, Sequence, Tuple
+from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -252,6 +252,35 @@ class KnnIndex:
         ke = _check(self.lib.nk_search_filtered(self.ptr, q.ctypes.data_as(C.c_void_p), None if f is None else f.ctypes.data_as(C.c_void_p),
                                                 Q, k, idx.ctypes.data_as(C.c_void_p), sc.ctypes.data_as(C.c_void_p)), "nk_search_filtered")
         return idx[:, :ke], sc[:, :ke]
+
+    def search_range(self, queries, thresholds, filters=None) -> List[Tuple[np.ndarray, np.ndarray]]:
+        """Every admissible row whose score reaches the query's threshold (cosine / dot: minimum score; euclidean: maximum
+        distance), one threshold per query (a scalar applies to all).  Returns one (idx uint32, score float32) pair per query,
+        in search()'s order.  The result buffer grows to the size the library reports (nk_search_range's size protocol)."""
+        q = np.ascontiguousarray(np.asarray(queries, dtype=np.float32))
+        if q.ndim == 1:
+            q = q.reshape(1, -1)
+        if q.shape[1] != self.dim:
+            raise KnnError(f"invalid dimensions: query has {q.shape[1]}, index has {self.dim}")
+        Q = q.shape[0]
+        t = np.ascontiguousarray(np.broadcast_to(np.asarray(thresholds, dtype=np.float32), (Q,)))
+        f = None if filters is None else as_filters(filters, Q)
+        off = np.zeros(Q + 1, dtype=np.uint64)
+        total = C.c_uint64(0)
+        cap = getattr(self, "_range_cap", 0)
+        while True:
+            idx = np.empty(max(cap, 1), dtype=np.uint32)
+            sc = np.empty(max(cap, 1), dtype=np.float32)
+            _check(self.lib.nk_search_range(self.ptr, q.ctypes.data_as(C.c_void_p), t.ctypes.data_as(C.c_void_p),
+                                            None if f is None else f.ctypes.data_as(C.c_void_p), Q, cap,
+                                            off.ctypes.data_as(C.c_void_p), idx.ctypes.data_as(C.c_void_p),
+                                            sc.ctypes.data_as(C.c_void_p), C.byref(total)), "nk_search_range")
+            if total.value <= cap:
+                break
+            cap = int(total.value)
+            self._range_cap = cap
+        o = off.astype(np.int64)
+        return [(idx[o[i]:o[i + 1]].copy(), sc[o[i]:o[i + 1]].copy()) for i in range(Q)]
 
     def search_filtered_device(self, q_ptr: int, filters_ptr: int, Q: int, k: int, out_idx_ptr: int, out_score_ptr: int,
                                stream: int = 0) -> int:
