@@ -253,6 +253,22 @@ int nk_search_filtered(NkIndex *ix, const float *queries_host, const NkFilter *f
 int nk_search_filtered_device(NkIndex *ix, const float *queries_dev, const NkFilter *filters_dev, uint32_t Q, uint32_t k,
                               uint32_t *out_idx_dev, float *out_score_dev, void *stream);
 
+/* ---- Search by stored row ----------------------------------------------------------------------------------------------
+ * The k nearest OTHER rows of stored rows ("which nodes are like this node?", FindSimilar, OnStore's related-node search, the
+ * k-NN graph of the whole index).  rows_host [Q]: row ids relative to the index's first row (< nk_index_rows; duplicates
+ * allowed).  Query q is row rows_host[q] as stored NOW, widened exactly to fp32 for fp16 / bf16 indexes, read on the device
+ * that holds it (on a single device only the ids cross PCIe).  Result: the top k, in nk_search's order and ties, of the
+ * admissible rows other than rows_host[q] itself: row mask and score floor apply as in nk_search, and a masked-out row may
+ * still be a query.  out_idx / out_score: [Q x k] (row stride k), global row ids.  Returns min(k, rows passing the row mask);
+ * a query with fewer admissible other rows gets 0xffffffff / 0 in its unused slots.  Any Q, including every row of the index
+ * (the k-NN graph): queries run in blocks of 1024, so the device workspace stays bounded; any number of devices.
+ * k <= NK_MAX_K_TOTAL - 1.  Out-of-range ids, a null pointer with Q > 0, or a larger k return -1; k == 0, Q == 0 or no
+ * admissible row return 0.  Synchronous, and it holds the index lock throughout: a whole-index graph call blocks every
+ * other call on the index for its duration.
+ * Equals nk_search(the rows read back and widened, k + 1) with the query's own row removed from each list (or, where it is
+ * not in the list, the last entry), bit for bit, for the same blocks of 1024 queries. */
+int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score);
+
 /* ---- Range search ------------------------------------------------------------------------------------------------------
  * Every admissible row whose score reaches the query's threshold (Cypher WHERE vector.similarity.* >= t, auto-links above a
  * similarity threshold, near-duplicate checks): no k.  thresholds_host [Q]: cosine / dot a minimum score, euclidean a

@@ -7,6 +7,7 @@
 // fused scan per shard + a candidate merge; nothing is allocated per query and only Q*k results leave
 // the device.
 #include <algorithm>
+#include <functional>
 #include <map>
 #include <mutex>
 #include <stdlib.h>
@@ -92,6 +93,8 @@ struct NkIndex {
     bool mask_on = false;
     float min_score = -INFINITY;  // score floor of subsequent searches, in the API's score domain (nk_index_set_min_score)
     uint32_t n_groups = 0;        // nk_index_set_row_groups
+    float *h_qrows = nullptr;     // pinned: a block of nk_search_rows queries assembled from several shards, + gather staging
+    size_t h_qrows_bytes = 0;
     NkStats stats{};
     std::mutex mu;
     size_t esz() const { return dtype == NK_DTYPE_F32 ? 4 : 2; }
@@ -505,6 +508,7 @@ void nk_index_release(NkIndex *ix) {
         if (s.group) cudaFree(s.group);
         s.ws.release();
     }
+    if (ix->h_qrows) cudaFreeHost(ix->h_qrows);
     delete ix;
 }
 
@@ -953,26 +957,14 @@ int nk_index_read_rows(NkIndex *ix, uint64_t row, uint64_t n_rows, void *rows_ho
     return 0;
 }
 
-// nk_search / nk_search_filtered: filters_host == nullptr is plain nk_search.
-static int search_host(NkIndex *ix, const float *queries_host, const NkFilter *filters_host, uint32_t Q, uint32_t k, uint32_t *out_idx,
-                       float *out_score) {
-    nk::DeviceGuard _restore_device;
-    if (!ix) { nk::set_error("null index"); return -1; }
-    std::lock_guard<std::mutex> lk(ix->mu);
-    const uint64_t N = ix->mask_on ? ix->mask_alive : ix->rows();  // rows that can be returned
-    if (k == 0 || N == 0 || Q == 0) return 0;  // cuda_bridge.go:644-646, gpu.go:1540-1542
-    if (!queries_host || !out_idx || !out_score) { nk::set_error("null argument"); return -1; }
-    const uint32_t ke = k > N ? (uint32_t)N : k;  // cuda_bridge.go:647-649
-    if (ke > NK_MAX_K_TOTAL) { nk::set_error("k=%u exceeds NK_MAX_K_TOTAL=%u", ke, NK_MAX_K_TOTAL); return -1; }
-    const size_t qbytes = (size_t)Q * ix->dim * sizeof(float);
-    ix->stats.searches++;
-    ix->stats.queries += Q;
-    NK_RANGE_PUSH("nk_search");
-    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+// Writes the Q fp32 queries of a search into s.ws.queries (already reserved) on s.stream; the device is s's.
+using StageQueries = std::function<int(NkShard &)>;
 
-    std::vector<NkShard *> live;
-    for (auto &s : ix->shards)
-        if (s.n) live.push_back(&s);
+// One synchronous search of Q staged queries over the live (non-empty) shards, the index lock held: scan, deferred retry
+// tail, merge; writes ke results per query into out_idx / out_score [Q x k] (row stride k) and returns ke.
+static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const StageQueries &stage, const NkFilter *filters_host,
+                       uint32_t Q, uint32_t ke, uint32_t k, uint32_t *out_idx, float *out_score) {
+    const size_t qbytes = (size_t)Q * ix->dim * sizeof(float);
     const bool single = live.size() == 1;
 
     // Launch every shard asynchronously, then collect.  A single shard writes the decoded (index, score) arrays from
@@ -988,8 +980,7 @@ static int search_host(NkIndex *ix, const float *queries_host, const NkFilter *f
             if (nk::ws_reserve((void **)&s->ws.out_score, &s->ws.out_score_bytes, (size_t)Q * ke * 4)) return -1;
             xo.out_idx = s->ws.out_idx; xo.out_score = s->ws.out_score;
         }
-        NK_CUDA_OK(cudaMemcpyAsync(s->ws.queries, queries_host, qbytes, cudaMemcpyHostToDevice, s->stream));
-        ix->stats.bytes_h2d += qbytes;
+        if (stage(*s)) return -1;
         if (filters_host) {
             // staged next to the queries, in the shard workspace: the deferred retry tail reads them after this call's first sync
             const size_t fbytes = (size_t)Q * sizeof(NkFilter);
@@ -1098,6 +1089,34 @@ static int search_host(NkIndex *ix, const float *queries_host, const NkFilter *f
     return (int)ke;
 }
 
+// nk_search / nk_search_filtered: filters_host == nullptr is plain nk_search.
+static int search_host(NkIndex *ix, const float *queries_host, const NkFilter *filters_host, uint32_t Q, uint32_t k, uint32_t *out_idx,
+                       float *out_score) {
+    nk::DeviceGuard _restore_device;
+    if (!ix) { nk::set_error("null index"); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
+    const uint64_t N = ix->mask_on ? ix->mask_alive : ix->rows();  // rows that can be returned
+    if (k == 0 || N == 0 || Q == 0) return 0;  // cuda_bridge.go:644-646, gpu.go:1540-1542
+    if (!queries_host || !out_idx || !out_score) { nk::set_error("null argument"); return -1; }
+    const uint32_t ke = k > N ? (uint32_t)N : k;  // cuda_bridge.go:647-649
+    if (ke > NK_MAX_K_TOTAL) { nk::set_error("k=%u exceeds NK_MAX_K_TOTAL=%u", ke, NK_MAX_K_TOTAL); return -1; }
+    const size_t qbytes = (size_t)Q * ix->dim * sizeof(float);
+    ix->stats.searches++;
+    ix->stats.queries += Q;
+    NK_RANGE_PUSH("nk_search");
+    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+
+    std::vector<NkShard *> live;
+    for (auto &s : ix->shards)
+        if (s.n) live.push_back(&s);
+    const StageQueries upload = [&](NkShard &s) {
+        NK_CUDA_OK(cudaMemcpyAsync(s.ws.queries, queries_host, qbytes, cudaMemcpyHostToDevice, s.stream));
+        ix->stats.bytes_h2d += qbytes;
+        return 0;
+    };
+    return search_live(ix, live, upload, filters_host, Q, ke, k, out_idx, out_score);
+}
+
 int nk_search(NkIndex *ix, const float *queries_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
     return search_host(ix, queries_host, nullptr, Q, k, out_idx, out_score);
 }
@@ -1105,6 +1124,108 @@ int nk_search(NkIndex *ix, const float *queries_host, uint32_t Q, uint32_t k, ui
 int nk_search_filtered(NkIndex *ix, const float *queries_host, const NkFilter *filters_host, uint32_t Q, uint32_t k,
                        uint32_t *out_idx, float *out_score) {
     return search_host(ix, queries_host, filters_host, Q, k, out_idx, out_score);
+}
+
+// ---- search by stored row (DESIGN.md §3.5c) ---------------------------------------------------------------------------
+// Each query is a stored row, gathered (and widened to fp32) on the device that owns it.  The scan asks for k' = min(k+1, N)
+// and the host drops the query's own row from the decoded list, or the last slot if its row is not in it: the k'-list is a
+// prefix of the (score desc, row asc) order over the admissible rows, so either way the rest is the top of the other rows.
+// Queries run in blocks of SEARCH_ROWS_BLOCK, which bounds the workspace (the 16-bit scan's survivor lists grow with Q)
+// whatever Q is, the whole index included; one host synchronisation per block.
+constexpr uint32_t SEARCH_ROWS_BLOCK = 1024;
+
+int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
+    nk::DeviceGuard _restore_device;
+    if (!ix) { nk::set_error("null index"); return -1; }
+    if (Q && (!rows_host || !out_idx || !out_score)) { nk::set_error("null argument"); return -1; }
+    if (k > NK_MAX_K_TOTAL - 1) { nk::set_error("nk_search_rows: k=%u exceeds NK_MAX_K_TOTAL - 1 = %u", k, NK_MAX_K_TOTAL - 1); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
+    const uint64_t total = ix->rows();
+    const uint64_t N = ix->mask_on ? ix->mask_alive : total;  // rows that can be returned
+    if (k == 0 || N == 0 || Q == 0) return 0;
+    for (uint32_t q = 0; q < Q; ++q)
+        if (rows_host[q] >= total) {
+            nk::set_error("nk_search_rows: row %u (query %u) out of range, index has %llu rows", rows_host[q], q, (unsigned long long)total);
+            return -1;
+        }
+    const uint32_t kk = (uint32_t)std::min<uint64_t>((uint64_t)k + 1, N);  // asked of the scan
+    const uint32_t ke = (uint32_t)std::min<uint64_t>(k, N);                // returned
+    ix->stats.searches++;
+    ix->stats.queries += Q;
+    NK_RANGE_PUSH("nk_search_rows");
+    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+
+    std::vector<NkShard *> live;
+    for (auto &s : ix->shards)
+        if (s.n) live.push_back(&s);
+    const size_t rb = (size_t)ix->dim * sizeof(float);
+    const uint32_t QB = std::min(Q, SEARCH_ROWS_BLOCK);
+    std::vector<uint32_t> bidx((size_t)QB * kk), local(QB), pos(QB);
+    std::vector<float> bsc((size_t)QB * kk);
+    if (live.size() > 1 && ix->h_qrows_bytes < 2 * QB * rb) {
+        if (ix->h_qrows) cudaFreeHost(ix->h_qrows);
+        ix->h_qrows = nullptr; ix->h_qrows_bytes = 0;
+        NK_CUDA_OK(cudaMallocHost((void **)&ix->h_qrows, 2 * QB * rb));
+        ix->h_qrows_bytes = 2 * QB * rb;
+    }
+    for (uint32_t b = 0; b < Q; b += QB) {
+        const uint32_t nb = std::min(QB, Q - b);
+        const uint32_t *ids = rows_host + b;
+        StageQueries stage;
+        if (live.size() == 1) {  // only the ids cross PCIe; the rows are gathered straight into the query block
+            stage = [&](NkShard &s) {
+                for (uint32_t q = 0; q < nb; ++q) local[q] = ids[q] - (uint32_t)(s.base - ix->row_base);
+                if (nk::ws_reserve((void **)&s.ws.sub_rows, &s.ws.sub_rows_bytes, (size_t)nb * 4)) return -1;
+                NK_CUDA_OK(cudaMemcpyAsync(s.ws.sub_rows, local.data(), (size_t)nb * 4, cudaMemcpyHostToDevice, s.stream));
+                if (nk::gather_rows(s.rows, ix->dtype, ix->dim, s.ws.sub_rows, nb, s.ws.queries, true, s.stream)) return -1;
+                ix->stats.bytes_h2d += (uint64_t)nb * 4;
+                ix->stats.kernel_launches++;
+                return 0;
+            };
+        } else {  // the block may straddle shards: gather on each owner, assemble in pinned host memory, send to every shard
+            float *blk = ix->h_qrows, *part = ix->h_qrows + (size_t)QB * ix->dim;
+            for (NkShard *o : live) {
+                uint32_t m = 0;
+                for (uint32_t q = 0; q < nb; ++q) {
+                    uint64_t l;
+                    if (find_shard(ix, ids[q], &l) == o) { pos[m] = q; local[m++] = (uint32_t)l; }
+                }
+                if (m == 0) continue;
+                NK_CUDA_OK(cudaSetDevice(o->device));
+                if (nk::ws_reserve((void **)&o->ws.sub_rows, &o->ws.sub_rows_bytes, (size_t)m * 4)) return -1;
+                if (nk::ws_reserve(&o->ws.sub_gather, &o->ws.sub_gather_bytes, (size_t)m * rb)) return -1;
+                NK_CUDA_OK(cudaMemcpyAsync(o->ws.sub_rows, local.data(), (size_t)m * 4, cudaMemcpyHostToDevice, o->stream));
+                if (nk::gather_rows(o->rows, ix->dtype, ix->dim, o->ws.sub_rows, m, o->ws.sub_gather, true, o->stream)) return -1;
+                NK_CUDA_OK(cudaMemcpyAsync(part, o->ws.sub_gather, (size_t)m * rb, cudaMemcpyDeviceToHost, o->stream));
+                NK_CUDA_OK(cudaStreamSynchronize(o->stream));
+                ix->stats.bytes_h2d += (uint64_t)m * 4;
+                ix->stats.bytes_d2h += (uint64_t)m * rb;
+                ix->stats.kernel_launches++;
+                for (uint32_t i = 0; i < m; ++i) memcpy(blk + (size_t)pos[i] * ix->dim, part + (size_t)i * ix->dim, rb);
+            }
+            stage = [&](NkShard &s) {
+                NK_CUDA_OK(cudaMemcpyAsync(s.ws.queries, blk, (size_t)nb * rb, cudaMemcpyHostToDevice, s.stream));
+                ix->stats.bytes_h2d += (uint64_t)nb * rb;
+                return 0;
+            };
+        }
+        if (search_live(ix, live, stage, nullptr, nb, kk, kk, bidx.data(), bsc.data()) < 0) return -1;
+        for (uint32_t q = 0; q < nb; ++q) {
+            const uint32_t self = (uint32_t)(ix->row_base + ids[q]);
+            const uint32_t *ri = bidx.data() + (size_t)q * kk;
+            const float *rs = bsc.data() + (size_t)q * kk;
+            uint32_t drop = kk - 1;
+            for (uint32_t j = 0; j < kk; ++j)
+                if (ri[j] == self) { drop = j; break; }
+            uint32_t *oi = out_idx + (size_t)(b + q) * k;
+            float *os = out_score + (size_t)(b + q) * k;
+            uint32_t w = 0;
+            for (uint32_t j = 0; j < kk && w < ke; ++j)
+                if (j != drop) { oi[w] = ri[j]; os[w] = rs[j]; ++w; }
+            for (; w < ke; ++w) { oi[w] = 0xffffffffu; os[w] = 0.0f; }  // k >= N: one admissible row fewer than k'
+        }
+    }
+    return (int)ke;
 }
 
 // ---- range search ---------------------------------------------------------------------------------------------------
@@ -1395,7 +1516,7 @@ int nk_score_subset(NkIndex *ix, const float *query_host, const uint32_t *rows_h
     std::vector<uint32_t> pos((size_t)ke);
     do {
         if (cudaMemcpyAsync(d_rows, local.data(), (size_t)n_subset * 4, cudaMemcpyHostToDevice, s->stream) != cudaSuccess) { rc = -1; break; }
-        if (nk::gather_rows(s->rows, ix->dtype, ix->dim, d_rows, n_subset, d_gather, s->stream)) { rc = -1; break; }
+        if (nk::gather_rows(s->rows, ix->dtype, ix->dim, d_rows, n_subset, d_gather, false, s->stream)) { rc = -1; break; }
         if (nk::ws_reserve((void **)&s->ws.queries, &s->ws.queries_bytes, (size_t)ix->dim * 4)) { rc = -1; break; }
         if (nk::ws_reserve((void **)&s->ws.keys, &s->ws.keys_bytes, (size_t)ke * 8)) { rc = -1; break; }
         if (nk::ws_reserve((void **)&s->ws.out_idx, &s->ws.out_idx_bytes, (size_t)ke * 4)) { rc = -1; break; }

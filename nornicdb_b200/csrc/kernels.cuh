@@ -138,7 +138,8 @@ int cluster_sums(const float *rows, uint64_t n, uint32_t dim, const int32_t *ass
                  unsigned long long *counts, cudaStream_t s);
 int count_changed(const int32_t *a, const uint32_t *b, uint64_t n, unsigned long long *changed, cudaStream_t s);
 int convert_f32_to_16(const float *src, void *dst, int dtype, size_t n, cudaStream_t s);  // fp16 / bf16, round to nearest even like the host's astype
-int gather_rows(const void *rows, int dtype, uint32_t dim, const uint32_t *idx, uint32_t n_idx, void *out,
+// out[r] = rows[idx[r]]: in the rows' dtype, or (out_f32) widened exactly to fp32
+int gather_rows(const void *rows, int dtype, uint32_t dim, const uint32_t *idx, uint32_t n_idx, void *out, bool out_f32,
                 cudaStream_t s);
 
 }  // namespace nk

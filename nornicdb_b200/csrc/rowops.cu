@@ -199,14 +199,19 @@ __global__ void fill_clustered_kernel(T *out, uint64_t n_rows, uint32_t dim, uin
     }
 }
 
-template <typename T>
-__global__ void gather_rows_kernel(const T *rows, uint32_t dim, const uint32_t *idx, uint32_t n_idx, T *out) {
+// O == T: a copy; O == float with 16-bit rows: the exact widening (every fp16 / bf16 value is an fp32 value)
+template <typename T, typename O>
+__global__ void gather_rows_kernel(const T *rows, uint32_t dim, const uint32_t *idx, uint32_t n_idx, O *out) {
     uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
     uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
     for (uint32_t r = warp; r < n_idx; r += nwarps) {
         const T *src = rows + (size_t)idx[r] * dim;
-        T *dst = out + (size_t)r * dim;
-        for (uint32_t j = lane; j < dim; j += 32) dst[j] = src[j];
+        O *dst = out + (size_t)r * dim;
+        for (uint32_t j = lane; j < dim; j += 32) {
+            if constexpr (std::is_same<T, O>::value) dst[j] = src[j];
+            else if constexpr (std::is_same<T, __half>::value) dst[j] = __half2float(src[j]);
+            else dst[j] = __bfloat162float(src[j]);
+        }
     }
 }
 
@@ -380,13 +385,17 @@ int count_changed(const int32_t *a, const uint32_t *b, uint64_t n, unsigned long
     NK_CUDA_OK(cudaGetLastError());
     return 0;
 }
-int gather_rows(const void *rows, int dtype, uint32_t dim, const uint32_t *idx, uint32_t n_idx, void *out,
+int gather_rows(const void *rows, int dtype, uint32_t dim, const uint32_t *idx, uint32_t n_idx, void *out, bool out_f32,
                 cudaStream_t s) {
     if (n_idx == 0) return 0;
-    if (dtype != NK_DTYPE_F32)  // fp16 / bf16: a 2-byte copy either way
-        gather_rows_kernel<__half><<<warp_grid(n_idx), 256, 0, s>>>((const __half *)rows, dim, idx, n_idx, (__half *)out);
+    if (dtype == NK_DTYPE_F32)
+        gather_rows_kernel<float, float><<<warp_grid(n_idx), 256, 0, s>>>((const float *)rows, dim, idx, n_idx, (float *)out);
+    else if (!out_f32)  // fp16 / bf16: a 2-byte copy either way
+        gather_rows_kernel<__half, __half><<<warp_grid(n_idx), 256, 0, s>>>((const __half *)rows, dim, idx, n_idx, (__half *)out);
+    else if (dtype == NK_DTYPE_F16)
+        gather_rows_kernel<__half, float><<<warp_grid(n_idx), 256, 0, s>>>((const __half *)rows, dim, idx, n_idx, (float *)out);
     else
-        gather_rows_kernel<float><<<warp_grid(n_idx), 256, 0, s>>>((const float *)rows, dim, idx, n_idx, (float *)out);
+        gather_rows_kernel<__nv_bfloat16, float><<<warp_grid(n_idx), 256, 0, s>>>((const __nv_bfloat16 *)rows, dim, idx, n_idx, (float *)out);
     NK_CUDA_OK(cudaGetLastError());
     return 0;
 }

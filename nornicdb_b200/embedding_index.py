@@ -175,6 +175,21 @@ class EmbeddingIndex:
             idx, sc = self._ix.score_subset(q, rows)
             return self._results(idx, sc)
 
+    def SearchSimilar(self, ids: Sequence[str], k: int) -> List[List[SearchResult]]:
+        """The k most similar OTHER nodes of each stored node (FindSimilar, GraphQL `similar`, OnStore's related nodes), best
+        first, searched with the node's embedding as stored.  One list per id; an id the index does not hold gets an empty
+        list (missing ids are ignored, as in ScoreSubset)."""
+        with self.mu:
+            out: List[List[SearchResult]] = [[] for _ in ids]
+            at = [(i, self.idToIndex[n]) for i, n in enumerate(ids) if n in self.idToIndex]
+            if not at or k <= 0:
+                return out
+            self.searchesGPU += 1
+            idx, sc = self._ix.search_rows([r for _, r in at], k)
+            for j, (i, _) in enumerate(at):
+                out[i] = self._results(idx[j], sc[j])
+            return out
+
     # -- bookkeeping ---------------------------------------------------------------------------------
     def SyncToGPU(self) -> None:  # gpu.go:2025 — nothing to copy: the device rows are always current
         with self.mu:

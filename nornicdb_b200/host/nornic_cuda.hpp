@@ -318,6 +318,31 @@ public:
                 if (idx[i] < nodeIDs_.size()) out[q].push_back({nodeIDs_[idx[i]], sc[i], 1.0f - sc[i]});
         return out;
     }
+    // The k most similar OTHER nodes of each stored node (FindSimilar, GraphQL similar, OnStore's related nodes), best first,
+    // searched with the node's embedding as stored.  One list per id; an id the index does not hold gets an empty list
+    // (missing ids are ignored, as in ScoreSubset).
+    std::vector<std::vector<SearchResult>> SearchSimilar(const std::vector<std::string> &ids, int k) {
+        std::lock_guard<std::mutex> lk(mu_);
+        std::vector<std::vector<SearchResult>> out(ids.size());
+        std::vector<uint32_t> rows;
+        std::vector<size_t> at;
+        for (size_t i = 0; i < ids.size(); ++i) {
+            auto it = idToIndex_.find(ids[i]);
+            if (it != idToIndex_.end()) { rows.push_back((uint32_t)it->second); at.push_back(i); }
+        }
+        if (rows.empty() || k <= 0) return out;
+        std::vector<uint32_t> idx(rows.size() * (size_t)k);
+        std::vector<float> sc(rows.size() * (size_t)k);
+        int got = nk_search_rows(ix_, rows.data(), (uint32_t)rows.size(), (uint32_t)k, idx.data(), sc.data());
+        if (got < 0) throw cuda::ErrKernelExecution(std::string("gpu: ") + nk_last_error());
+        for (size_t j = 0; j < rows.size(); ++j)
+            for (int i = 0; i < got; ++i) {
+                uint32_t r = idx[j * k + i];
+                float s = sc[j * k + i];
+                if (r < nodeIDs_.size()) out[at[j]].push_back({nodeIDs_[r], s, 1.0f - s});  // 0xffffffff: fewer other nodes than k
+            }
+        return out;
+    }
     std::vector<SearchResult> ScoreSubset(const std::vector<float> &query, const std::vector<std::string> &ids) {  // gpu.go:1552-1616
         if ((int)query.size() != dims_) throw ErrInvalidDimensions();
         std::lock_guard<std::mutex> lk(mu_);

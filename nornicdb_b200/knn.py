@@ -223,6 +223,25 @@ class KnnIndex:
                                        sc.ctypes.data_as(C.c_void_p)), "nk_search")
         return idx[:, :ke], sc[:, :ke]
 
+    def search_rows(self, rows, k: int) -> Tuple[np.ndarray, np.ndarray]:
+        """The k nearest OTHER rows of stored rows: rows = row ids (< len(self), repeats allowed), each searched as stored now
+        -> (idx [Q x k'] uint32, score [Q x k'] fp32), k' = min(k, admissible rows), with search()'s conventions.  A query
+        with fewer admissible other rows gets index 0xffffffff and score 0 in its unused slots.  rows = every row id gives
+        the k-NN graph of the index in one call (served in blocks of 1024 queries)."""
+        r = np.asarray(rows, dtype=np.int64).reshape(-1)
+        if r.size and (r.min() < 0 or r.max() > 0xFFFFFFFF):
+            raise KnnError("search_rows: row ids must be in [0, 2^32)")
+        r = np.ascontiguousarray(r.astype(np.uint32))
+        Q = r.size
+        k = int(k)
+        if k <= 0 or Q == 0:
+            return np.empty((Q, 0), np.uint32), np.empty((Q, 0), np.float32)
+        idx = np.empty((Q, k), dtype=np.uint32)
+        sc = np.empty((Q, k), dtype=np.float32)
+        ke = _check(self.lib.nk_search_rows(self.ptr, r.ctypes.data_as(C.c_void_p), Q, k, idx.ctypes.data_as(C.c_void_p),
+                                            sc.ctypes.data_as(C.c_void_p)), "nk_search_rows")
+        return idx[:, :ke], sc[:, :ke]
+
     def search_device(self, q_ptr: int, Q: int, k: int, out_idx_ptr: int, out_score_ptr: int, stream: int = 0) -> int:
         return _check(self.lib.nk_search_device(self.ptr, q_ptr, Q, k, out_idx_ptr, out_score_ptr, stream),
                       "nk_search_device")
