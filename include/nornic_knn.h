@@ -222,7 +222,12 @@ int nk_index_read_rows(NkIndex *ix, uint64_t row, uint64_t n_rows, void *rows_ho
 int nk_search(NkIndex *ix, const float *queries_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score);
 
 /* Same, single-device index, everything device-resident and asynchronous on `stream` (a cudaStream_t,
- * NULL = the index's own stream).  queries_dev [Q x dim] fp32; out_idx_dev/out_score_dev [Q x k]. */
+ * NULL = the index's own stream).  queries_dev [Q x dim] fp32; out_idx_dev/out_score_dev [Q x k].
+ * Call order: the calls on one index take effect in the order they are made, on any mix of streams and threads.  A device
+ * search still queued on a busy stream sees the rows, mask and tags as they were when it was called, not a later
+ * nk_index_update_row / remove_swap / set_row_mask; two device searches on two streams, or a device search and a host
+ * search, run one after the other on the device (they share the shard's workspace).  Each shard keeps one event for this:
+ * every call makes its stream wait on it and records it again afterwards.  Nothing waits on the host. */
 int nk_search_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uint32_t k, uint32_t *out_idx_dev,
                      float *out_score_dev, void *stream);
 

@@ -42,6 +42,7 @@ struct NkShard {
     int device = 0;
     nk::DeviceInfo di;
     cudaStream_t stream = nullptr;
+    cudaEvent_t last = nullptr;  // the end of the last work any call queued on this shard, on whichever stream (ShardOrder)
     void *rows = nullptr;
     bool owns = true;
     uint64_t n = 0, cap = 0, base = 0;
@@ -111,6 +112,51 @@ struct NkIndex {
     }
 };
 
+// ---- call order (include/nornic_knn.h, "Call order") ------------------------------------------------------------------
+// The calls on one index take effect in call order, whatever streams they run on: the device searches run on the caller's
+// stream, everything else on the shard's own non-blocking stream, and all of them share the shard's rows, masks, tags and
+// workspace.  A call holds a ShardOrder, under the index lock, for every shard it queues work on: its stream first waits on
+// the shard's event, which marks the end of the last call's work, and when the call is done the event is recorded on its
+// stream.  One wait and one record per shard and call; no host synchronisation.
+class ShardOrder {
+  public:
+    explicit ShardOrder(NkIndex *ix) {  // every shard, each on its own stream
+        for (auto &s : ix->shards) enter(s, s.stream);
+    }
+    ShardOrder(NkShard &s, cudaStream_t st) { enter(s, st); }
+    ~ShardOrder() {
+        for (auto &h : held_) {
+            cudaSetDevice(h.first->device);
+            cudaEventRecord(h.first->last, h.second);
+        }
+    }
+    ShardOrder(const ShardOrder &) = delete;
+    ShardOrder &operator=(const ShardOrder &) = delete;
+    bool failed() const { return failed_; }
+
+  private:
+    void enter(NkShard &s, cudaStream_t st) {
+        cudaError_t e = cudaSetDevice(s.device);
+        if (e == cudaSuccess) e = cudaStreamWaitEvent(st, s.last, 0);
+        if (e != cudaSuccess) {
+            nk::set_error("cannot order the call after earlier work on device %d: %s", s.device, cudaGetErrorString(e));
+            failed_ = true;
+            return;
+        }
+        held_.emplace_back(&s, st);
+    }
+    std::vector<std::pair<NkShard *, cudaStream_t>> held_;
+    bool failed_ = false;
+};
+
+// Block until every call queued on the shard so far has run, and this call's work on the shard's own stream too: before a
+// buffer that earlier work, on any stream, may still read is freed or replaced.
+static int shard_drain(NkShard &s) {
+    NK_CUDA_OK(cudaEventSynchronize(s.last));
+    NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+    return 0;
+}
+
 // Row-count changing mutations invalidate the row mask (its bits are positions).
 static void drop_row_mask(NkIndex *ix) {
     ix->mask_on = false;
@@ -127,7 +173,7 @@ static int shard_tags_grow(NkShard &s, uint64_t old_n) {
         uint64_t *p = nullptr;
         NK_CUDA_OK(cudaMalloc((void **)&p, cap * 8));
         if (s.tags && old_n) NK_CUDA_OK(cudaMemcpyAsync(p, s.tags, old_n * 8, cudaMemcpyDeviceToDevice, s.stream));
-        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+        if (shard_drain(s)) return -1;
         if (s.tags) NK_CUDA_OK(cudaFree(s.tags));
         s.tags = p;
         s.tags_cap = cap;
@@ -164,7 +210,7 @@ static int shard_sync_shadow(NkIndex *ix, NkShard &s) {
     }
     const uint32_t dimpad = ix->dimpad();
     if (s.shadow_cap < s.n) {
-        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+        if (shard_drain(s)) return -1;
         shard_drop_shadow(s);
         const uint64_t cap = s.cap > s.n ? s.cap : s.n;
         cudaError_t e = f32 ? cudaMalloc(&s.shadow, cap * dimpad * 2) : cudaSuccess;
@@ -260,7 +306,7 @@ static int shard_reserve_rows(NkIndex *ix, NkShard &s, uint64_t need_rows, bool 
     NK_CUDA_OK(cudaMalloc(&p, cap * rb));
     if (s.rows) {
         if (keep && s.n) NK_CUDA_OK(cudaMemcpyAsync(p, s.rows, s.n * rb, cudaMemcpyDeviceToDevice, s.stream));
-        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+        if (shard_drain(s)) return -1;
         NK_CUDA_OK(cudaFree(s.rows));
     }
     s.rows = p;
@@ -473,6 +519,7 @@ NkIndex *nk_index_create(const int *device_ids, int n_devices, uint32_t dim, int
         cudaError_t e = cudaSetDevice(s.device);
         if (e == cudaSuccess && nk::query_device_info(s.device, &s.di) != 0) e = cudaErrorUnknown;
         if (e == cudaSuccess) e = cudaStreamCreateWithFlags(&s.stream, cudaStreamNonBlocking);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s.last, cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaMalloc((void **)&s.ws.flags, sizeof(int) * nk::NK_FLAG_WORDS);
         if (e == cudaSuccess) e = cudaMemset(s.ws.flags, 0, sizeof(int) * nk::NK_FLAG_WORDS);
         if (e != cudaSuccess) {
@@ -490,6 +537,10 @@ void nk_index_release(NkIndex *ix) {
     if (!ix) return;
     for (auto &s : ix->shards) {
         cudaSetDevice(s.device);
+        if (s.last) {  // work queued on any stream, a device search on the caller's included, may still read the buffers
+            cudaEventSynchronize(s.last);
+            cudaEventDestroy(s.last);
+        }
         if (s.stream) {
             cudaStreamSynchronize(s.stream);
             cudaStreamDestroy(s.stream);
@@ -517,6 +568,8 @@ static int upload_impl(NkIndex *ix, const void *rows_host, uint64_t n_rows, bool
     if (!ix) { nk::set_error("null index"); return -1; }
     if (n_rows && !rows_host) { nk::set_error("null rows"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
     drop_row_mask(ix);
     const bool cvt = src_is_f32 && ix->dtype != NK_DTYPE_F32;
     const size_t rb = (size_t)ix->dim * ix->esz(), src_rb = (size_t)ix->dim * (cvt ? 4 : ix->esz());
@@ -579,8 +632,10 @@ int nk_index_append(NkIndex *ix, const void *rows_host, uint64_t n_rows) {
     if (n_rows == 0) return 0;
     if (!rows_host) { nk::set_error("null rows"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
-    drop_row_mask(ix);
     NkShard &s = ix->shards.back();
+    ShardOrder order(s, s.stream);
+    if (order.failed()) return -1;
+    drop_row_mask(ix);
     const size_t rb = (size_t)ix->dim * ix->esz();
     if (ix->row_base + ix->rows() + n_rows > 0xfffffff0ull) { nk::set_error("index exceeds 2^32 rows (row ids are uint32)"); return -1; }
     NK_CUDA_OK(cudaSetDevice(s.device));
@@ -602,6 +657,8 @@ int nk_index_update_row(NkIndex *ix, uint64_t row, const void *row_host) {
     uint64_t local;
     NkShard *s = find_shard(ix, row, &local);
     if (!s) { nk::set_error("row %llu out of range", (unsigned long long)row); return -1; }
+    ShardOrder order(*s, s->stream);
+    if (order.failed()) return -1;
     const size_t rb = (size_t)ix->dim * ix->esz();
     NK_CUDA_OK(cudaSetDevice(s->device));
     NK_CUDA_OK(cudaMemcpyAsync((char *)s->rows + local * rb, row_host, rb, cudaMemcpyHostToDevice, s->stream));
@@ -617,6 +674,8 @@ int nk_index_remove_swap(NkIndex *ix, uint64_t row) {
     std::lock_guard<std::mutex> lk(ix->mu);
     uint64_t total = ix->rows();
     if (row >= total) { nk::set_error("row %llu out of range", (unsigned long long)row); return -1; }
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
     drop_row_mask(ix);
     // last non-empty shard holds the last row
     NkShard *last = nullptr;
@@ -661,6 +720,8 @@ static int fill_impl(NkIndex *ix, uint64_t n_rows, uint64_t seed, uint32_t centr
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
     drop_row_mask(ix);
     const uint64_t G = ix->shards.size();
     if (ix->row_base + n_rows > 0xfffffff0ull) { nk::set_error("index exceeds 2^32 rows (row ids are uint32)"); return -1; }
@@ -713,11 +774,13 @@ int nk_index_attach_device_rows(NkIndex *ix, void *rows_dev, uint64_t n_rows) {
     if (ix->row_base + n_rows > 0xfffffff0ull) { nk::set_error("index exceeds 2^32 rows (row ids are uint32)"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
     NkShard &s = ix->shards[0];
+    ShardOrder order(s, s.stream);
+    if (order.failed()) return -1;
     NK_CUDA_OK(cudaSetDevice(s.device));
+    if (shard_drain(s)) return -1;
     if (s.rows && s.owns) NK_CUDA_OK(cudaFree(s.rows));
     // caller-owned rows may change behind the library's back (cuda_normalize_vectors runs right after NewBuffer,
     // gpu.go:2100-2106): no shadow until the caller says the rows are final (nk_index_refresh_shadow)
-    NK_CUDA_OK(cudaStreamSynchronize(s.stream));
     shard_drop_shadow(s);
     drop_row_mask(ix);
     s.rows = rows_dev; s.owns = false; s.n = n_rows; s.cap = n_rows; s.shadow_attached = false;
@@ -733,6 +796,8 @@ int nk_index_refresh_shadow(NkIndex *ix) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
     for (auto &s : ix->shards) {
         NK_CUDA_OK(cudaSetDevice(s.device));
         if (!s.owns) s.shadow_attached = true;
@@ -772,6 +837,8 @@ int nk_index_set_row_mask(NkIndex *ix, const uint32_t *mask_words, uint64_t n_bi
         return 0;
     }
     if (n_bits != ix->rows()) { nk::set_error("row mask has %llu bits, index has %llu rows", (unsigned long long)n_bits, (unsigned long long)ix->rows()); return -1; }
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
     uint64_t off = 0, alive = 0;
     std::vector<uint32_t> local;
     for (auto &s : ix->shards) {
@@ -808,6 +875,8 @@ int nk_index_set_row_tags(NkIndex *ix, uint64_t first_row, const uint64_t *tags_
                       (unsigned long long)(first_row + n_rows), (unsigned long long)total);
         return -1;
     }
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
     for (uint64_t i = 0; i < n_rows;) {
         uint64_t local;
         NkShard *s = find_shard(ix, first_row + i, &local);
@@ -874,6 +943,8 @@ int nk_debug_filter_dump(NkIndex *ix, const float *queries_host, uint32_t Q, int
     s = &ix->shards[0];
     if (!queries_host || !est_host || !bnd_host || Q == 0 || Q > 64 || s->n == 0) { nk::set_error("bad argument (1 <= Q <= 64, non-empty index)"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
+    ShardOrder order(*s, s->stream);
+    if (order.failed()) return -1;
     NK_CUDA_OK(cudaSetDevice(s->device));
     const size_t cells = (size_t)s->n * Q;
     float *d = nullptr;
@@ -943,6 +1014,8 @@ int nk_index_read_rows(NkIndex *ix, uint64_t row, uint64_t n_rows, void *rows_ho
     nk::DeviceGuard _restore_device;
     if (!ix || (!rows_host && n_rows)) { nk::set_error("null argument"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
     const size_t rb = (size_t)ix->dim * ix->esz();
     for (uint64_t i = 0; i < n_rows;) {
         uint64_t local;
@@ -950,7 +1023,8 @@ int nk_index_read_rows(NkIndex *ix, uint64_t row, uint64_t n_rows, void *rows_ho
         if (!s) { nk::set_error("row %llu out of range", (unsigned long long)(row + i)); return -1; }
         uint64_t cnt = std::min<uint64_t>(n_rows - i, s->n - local);
         NK_CUDA_OK(cudaSetDevice(s->device));
-        NK_CUDA_OK(cudaMemcpy((char *)rows_host + i * rb, (const char *)s->rows + local * rb, cnt * rb, cudaMemcpyDeviceToHost));
+        NK_CUDA_OK(cudaMemcpyAsync((char *)rows_host + i * rb, (const char *)s->rows + local * rb, cnt * rb, cudaMemcpyDeviceToHost, s->stream));
+        NK_CUDA_OK(cudaStreamSynchronize(s->stream));
         ix->stats.bytes_d2h += cnt * rb;
         i += cnt;
     }
@@ -1105,6 +1179,8 @@ static int search_host(NkIndex *ix, const float *queries_host, const NkFilter *f
     ix->stats.queries += Q;
     NK_RANGE_PUSH("nk_search");
     struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
 
     std::vector<NkShard *> live;
     for (auto &s : ix->shards)
@@ -1154,6 +1230,8 @@ int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t 
     ix->stats.queries += Q;
     NK_RANGE_PUSH("nk_search_rows");
     struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
 
     std::vector<NkShard *> live;
     for (auto &s : ix->shards)
@@ -1269,6 +1347,8 @@ int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresho
     ix->stats.queries += Q;
     NK_RANGE_PUSH("nk_search_range");
     struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
     std::vector<NkShard *> live;
     for (auto &s : ix->shards)
         if (s.n) live.push_back(&s);
@@ -1386,17 +1466,12 @@ static int single_shard(NkIndex *ix, NkShard **out) {
     return 0;
 }
 
-int nk_search_keys_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uint32_t k, uint64_t *out_keys_dev,
-                          void *stream) {
-    nk::DeviceGuard _restore_device;
-    NkShard *s;
-    if (single_shard(ix, &s)) return -1;
-    if (k == 0 || Q == 0) return 0;
+// nk_search_keys_device with the index lock and the shard's call order held by the caller (Q, k > 0)
+static int search_keys_locked(NkIndex *ix, NkShard *s, const float *queries_dev, uint32_t Q, uint32_t k, uint64_t *out_keys_dev,
+                              cudaStream_t st) {
     if (!queries_dev || !out_keys_dev) { nk::set_error("null argument"); return -1; }
     if (k > NK_MAX_K_TOTAL) { nk::set_error("k=%u exceeds NK_MAX_K_TOTAL=%u", k, NK_MAX_K_TOTAL); return -1; }
-    std::lock_guard<std::mutex> lk(ix->mu);
     NK_CUDA_OK(cudaSetDevice(s->device));
-    cudaStream_t st = stream ? (cudaStream_t)stream : s->stream;
     ix->stats.searches++;
     ix->stats.queries += Q;
     if (s->n == 0) {
@@ -1405,6 +1480,19 @@ int nk_search_keys_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uin
     }
     if (run_scan(ix, *s, queries_dev, Q, k, out_keys_dev, st)) return -1;
     return (int)k;
+}
+
+int nk_search_keys_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uint32_t k, uint64_t *out_keys_dev,
+                          void *stream) {
+    nk::DeviceGuard _restore_device;
+    NkShard *s;
+    if (single_shard(ix, &s)) return -1;
+    if (k == 0 || Q == 0) return 0;
+    std::lock_guard<std::mutex> lk(ix->mu);
+    const cudaStream_t st = stream ? (cudaStream_t)stream : s->stream;
+    ShardOrder order(*s, st);
+    if (order.failed()) return -1;
+    return search_keys_locked(ix, s, queries_dev, Q, k, out_keys_dev, st);
 }
 
 // nk_search_device / nk_search_filtered_device: filters_dev == nullptr is plain nk_search_device.
@@ -1420,8 +1508,10 @@ static int search_device(NkIndex *ix, const float *queries_dev, const NkFilter *
     const uint64_t N = s->n;
     if (N == 0) return 0;
     if (k > N) { nk::set_error("nk_search_device: k=%u > rows=%llu (clamp on the host side)", k, (unsigned long long)N); return -1; }
+    const cudaStream_t st = stream ? (cudaStream_t)stream : s->stream;
+    ShardOrder order(*s, st);
+    if (order.failed()) return -1;
     NK_CUDA_OK(cudaSetDevice(s->device));
-    cudaStream_t st = stream ? (cudaStream_t)stream : s->stream;
     if (nk::ws_reserve((void **)&s->ws.keys, &s->ws.keys_bytes, (size_t)Q * k * 8)) return -1;
     ix->stats.searches++;
     ix->stats.queries += Q;
@@ -1456,7 +1546,7 @@ int nk_index_status(NkIndex *ix, void *stream) {
     for (auto &s : ix->shards) {
         NK_CUDA_OK(cudaSetDevice(s.device));
         if (stream) NK_CUDA_OK(cudaStreamSynchronize((cudaStream_t)stream));
-        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+        if (shard_drain(s)) return -1;
         int h = 0;
         NK_CUDA_OK(cudaMemcpy(&h, s.ws.flags, sizeof(int), cudaMemcpyDeviceToHost));
         if (h) {
@@ -1502,6 +1592,8 @@ int nk_score_subset(NkIndex *ix, const float *query_host, const uint32_t *rows_h
             nk::set_error("subset row %u out of range", rows_host[i]);
             return -1;
         }
+    ShardOrder order(*s, s->stream);
+    if (order.failed()) return -1;
     NK_CUDA_OK(cudaSetDevice(s->device));
     const size_t rb = (size_t)ix->dim * ix->esz();
     // grow-only workspace of the shard: no allocation per call (cuda.Device.Search allocates two buffers per query,
@@ -1560,6 +1652,8 @@ int nk_index_assign_nearest(NkIndex *ix, const float *centroids_host, uint32_t K
     if (K == 0) { nk::set_error("nk_index_assign_nearest: K must be >= 1"); return -1; }
     if (metric < NK_METRIC_COSINE || metric > NK_METRIC_EUCLIDEAN) { nk::set_error("unknown metric %d", metric); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
     uint64_t total_changed = 0, off = 0;
     for (auto &s : ix->shards) {
         if (s.n == 0) continue;
@@ -1623,6 +1717,8 @@ int nk_index_cluster_means(NkIndex *ix, const int32_t *assign_host, uint32_t K, 
     if (ix->dtype != NK_DTYPE_F32) { nk::set_error("nk_index_cluster_means: fp32 index required"); return -1; }
     if (K == 0) return 0;
     std::lock_guard<std::mutex> lk(ix->mu);
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
     const size_t KD = (size_t)K * ix->dim;
     std::vector<double> sums(KD, 0.0), part(KD);
     std::vector<unsigned long long> counts(K, 0ull), cpart(K);
@@ -1679,6 +1775,8 @@ int nk_index_set_row_groups(NkIndex *ix, const uint32_t *group_of_row, uint64_t 
     for (uint64_t r = 0; r < n_rows; ++r)
         if (group_of_row[r] >= n_groups) { nk::set_error("row groups: group id %u of row %llu out of range", group_of_row[r], (unsigned long long)r); return -1; }
     NkShard &s = ix->shards[0];
+    ShardOrder order(s, s.stream);
+    if (order.failed()) return -1;
     NK_CUDA_OK(cudaSetDevice(s.device));
     if (nk::ws_reserve((void **)&s.group, &s.group_bytes, (size_t)(n_rows ? n_rows : 1) * 4)) return -1;
     NK_CUDA_OK(cudaMemcpyAsync(s.group, group_of_row, n_rows * 4, cudaMemcpyHostToDevice, s.stream));
@@ -1702,6 +1800,8 @@ int nk_search_groups(NkIndex *ix, const float *query_host, uint32_t k, uint32_t 
     if (!s->group_on || ix->n_groups == 0) { nk::set_error("nk_search_groups: no row groups set (nk_index_set_row_groups)"); return -1; }
     const uint32_t G = ix->n_groups, ke = k < G ? k : G;
     if (ke > NK_MAX_K) { nk::set_error("nk_search_groups: k=%u exceeds NK_MAX_K=%u", ke, NK_MAX_K); return -1; }
+    ShardOrder order(*s, s->stream);
+    if (order.failed()) return -1;
     NK_CUDA_OK(cudaSetDevice(s->device));
     NK_RANGE_PUSH("nk_search_groups");
     struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
@@ -1742,13 +1842,14 @@ int nk_search_sharded_device(NkIndex *ix, NkComm *comm, const float *queries_dev
     if (single_shard(ix, &s)) return -1;
     if (!comm) { nk::set_error("null communicator"); return -1; }
     if (k == 0 || Q == 0) return 0;
-    cudaStream_t st = stream ? (cudaStream_t)stream : s->stream;
-    {
-        std::lock_guard<std::mutex> lk(ix->mu);
-        NK_CUDA_OK(cudaSetDevice(s->device));
-        if (nk::ws_reserve((void **)&s->ws.keys, &s->ws.keys_bytes, (size_t)Q * k * 8)) return -1;
-    }
-    if (nk_search_keys_device(ix, queries_dev, Q, k, s->ws.keys, st) < 0) return -1;
+    const cudaStream_t st = stream ? (cudaStream_t)stream : s->stream;
+    // one call in the shard's order: the exchange reads the keys from the shard's workspace, which the next call may reuse
+    std::lock_guard<std::mutex> lk(ix->mu);
+    ShardOrder order(*s, st);
+    if (order.failed()) return -1;
+    NK_CUDA_OK(cudaSetDevice(s->device));
+    if (nk::ws_reserve((void **)&s->ws.keys, &s->ws.keys_bytes, (size_t)Q * k * 8)) return -1;
+    if (search_keys_locked(ix, s, queries_dev, Q, k, s->ws.keys, st) < 0) return -1;
     if (nk_comm_exchange_merge(comm, s->ws.keys, Q, k, ix->metric, out_idx_dev, out_score_dev, st) < 0) return -1;
     ix->stats.kernel_launches += 2;
     return (int)k;

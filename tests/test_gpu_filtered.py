@@ -207,14 +207,16 @@ def _near_tie_corpus(oracle, n, noise, seed):
 
 
 @pytest.mark.parametrize("api", ["host", "device"])
-@pytest.mark.parametrize("path,n,noise", [("filter", 20_000, 1e-5), ("shadow", 160_000, 1e-4)])
-def test_retry_and_exact_tail_honour_the_filters(knn_lib, oracle_mod, api, path, n, noise):
+@pytest.mark.parametrize("path,n,noise,metric", [
+    pytest.param(path, n, noise, metric, id=f"{path}-{n}-{noise}" + ("" if metric == "cosine" else f"-{metric}"))
+    for path, n, noise in [("filter", 20_000, 1e-5), ("shadow", 160_000, 1e-4)] for metric in ("cosine", "dot", "euclidean")])
+def test_retry_and_exact_tail_honour_the_filters(knn_lib, oracle_mod, api, path, n, noise, metric):
     """The near-tie corpora of test_gpu_tensor.py overflow the filter stages; the retry / exact kernels (deferred by the
-    host API, queued blindly by the device API) must apply the same filters."""
+    host API, queued blindly by the device API: 3xTF32, or the CUDA-core scan for euclidean) must apply the same filters."""
     import torch
     from nornicdb_b200.knn import KnnIndex
     rows, q = _near_tie_corpus(oracle_mod, n, noise, 1 if path == "shadow" else 0)
-    Q, k, metric = q.shape[0], 10, "cosine"
+    Q, k = q.shape[0], 10
     tags = make_tags(n, 8)
     filters = mixed_filters(Q)
     filters[::2] = 0  # unfiltered queries keep the margin buffers overflowing

@@ -337,16 +337,23 @@ def _sharded_search(world, devices, rows, q, k, metric):
     return results
 
 
-@pytest.mark.parametrize("metric", ["cosine", "euclidean"])
-def test_exchange_two_ranks_on_one_device(knn_lib, oracle_mod, metric):
-    """The exchange kernels (peer push + fused wait/merge/decode) with both ranks living on cuda:0."""
-    n, d, Q, k = 50_000, 128, 16, 10
-    rows = oracle_mod.fill_uniform(n, d, 91)
-    q = oracle_mod.fill_uniform(Q, d, 92)
+@pytest.mark.parametrize("metric,near_tie", [
+    pytest.param(metric, near_tie, id=metric + ("-near-tie" if near_tie else ""))
+    for near_tie in (False, True) for metric in ("cosine", "dot", "euclidean") if near_tie or metric != "dot"])
+def test_exchange_two_ranks_on_one_device(knn_lib, oracle_mod, metric, near_tie):
+    """The exchange kernels (peer push + fused wait/merge/decode) with both ranks living on cuda:0, also on the near-tie
+    corpus of test_gpu_tensor.py, where each rank's filter meets thousands of rows inside its margins."""
+    if near_tie:
+        from test_gpu_filtered import _near_tie_corpus
+        rows, q = _near_tie_corpus(oracle_mod, 20_000, 1e-5, 0)
+    else:
+        rows = oracle_mod.fill_uniform(50_000, 128, 91)
+        q = oracle_mod.fill_uniform(16, 128, 92)
+    k = 10
     res = _sharded_search(2, (0, 0), rows, q, k, metric)
     oi, os_ = oracle_mod.knn_exact64(rows, q, k, metric)
     for gi, gs in res:
-        check_parity(rows, q, k, metric, gi, gs, oi, os_)
+        check_parity(rows, q, k, metric, gi, gs, oi, os_, swap_eps=5e-6 if near_tie else 2e-6)
     assert (res[0][0] == res[1][0]).all()
 
 
