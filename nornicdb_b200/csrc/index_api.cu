@@ -18,26 +18,6 @@
 #include "kernels.cuh"
 #include "scan_tensor_shared.cuh"
 
-namespace nk {
-int scan_tensor(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *out_keys, uint64_t *launches);
-bool scan_tensor_supported(const DeviceInfo &di, const ScanArgs &a);
-int scan_tensor_filter(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *out_keys, uint64_t *launches);
-int scan_tensor_filter_tail(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *out_keys, uint64_t *launches);
-int scan_filter_dump(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, int which, float *est, float *bnd, uint32_t ld, uint64_t *launches);
-bool scan_tensor_filter_supported(const DeviceInfo &di, const ScanArgs &a);
-bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a);
-bool assign_tensor_supported(const DeviceInfo &di, uint32_t dim, uint32_t K, int metric);
-int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, uint32_t dimpad, const float *xnorm2, const float *dnorm2,
-                  uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric, uint32_t *assign_dev, cudaStream_t stream,
-                  uint64_t *launches, void **scratch, size_t *scratch_bytes);
-int build_shadow(const float *rows, uint64_t first, uint64_t count, uint32_t dim, uint32_t dimpad, void *shadow, float *xnorm2,
-                 float *dnorm2, cudaStream_t stream);
-int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const uint32_t *thr_bits, Workspace &ws, uint64_t *launches,
-                     int *counts, uint32_t *list_cap, int *retried);
-int range_sorted_keys(const DeviceInfo &di, Workspace &ws, cudaStream_t stream, uint32_t Q, const int *counts, uint32_t list_cap,
-                      std::vector<uint64_t> *keys, uint64_t *launches);
-}
-
 struct NkShard {
     int device = 0;
     nk::DeviceInfo di;
@@ -162,6 +142,36 @@ static void drop_row_mask(NkIndex *ix) {
     ix->mask_on = false;
     ix->n_groups = 0;
     for (auto &s : ix->shards) { s.mask_on = false; s.group_on = false; }
+}
+
+// Global row ids are 32-bit on this boundary (SearchResult.Index uint32, cuda_bridge.go:425-428): may the index hold `rows`?
+static int check_row_limit(const NkIndex *ix, uint64_t rows) {
+    if (ix->row_base + rows > 0xfffffff0ull) { nk::set_error("index exceeds 2^32 rows (row ids are uint32)"); return -1; }
+    return 0;
+}
+
+static std::vector<NkShard *> live_shards(NkIndex *ix) {  // the non-empty shards
+    std::vector<NkShard *> live;
+    for (auto &s : ix->shards)
+        if (s.n) live.push_back(&s);
+    return live;
+}
+
+// Grow-only pinned host staging (25% headroom, like the device workspace).
+static int pinned_reserve(void **p, size_t *cur, size_t need) {
+    if (*cur >= need) return 0;
+    if (*p) cudaFreeHost(*p);
+    *p = nullptr; *cur = 0;
+    NK_CUDA_OK(cudaMallocHost(p, need + need / 4));
+    *cur = need + need / 4;
+    return 0;
+}
+
+// A result key -> (global row, score in the API's domain: euclidean keys are -distance^2).
+static void decode_key(int metric, uint64_t key, uint32_t *row, float *score) {
+    const float sc = nk::key_score(key);
+    *row = nk::key_row(key);
+    *score = metric == NK_METRIC_EUCLIDEAN ? sqrtf(std::max(-sc, 0.0f)) : sc;
 }
 
 // ---- per-row tag words (nk_search_filtered) ---------------------------------------------------------------------------
@@ -333,42 +343,16 @@ static NkShard *find_shard(NkIndex *ix, uint64_t row, uint64_t *local) {
     return nullptr;
 }
 
-struct ScanOut {  // optional extras of run_scan
-    uint32_t *out_idx = nullptr;   // fused decode (single-shard searches)
-    float *out_score = nullptr;
-    bool defer_tail = false;       // host-synchronous caller: retry stages are queued only if a flag was raised
-    const NkFilter *qfilter = nullptr;  // per-query tag filters [Q] (device; the shard's tag array must be on)
-};
-static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uint32_t k, uint64_t *out_keys,
-                    cudaStream_t stream, const ScanOut &xo = ScanOut());
-
-// k > NK_MAX_K (the reference accepts any k, cuda_bridge.go:327-375): ceil(k / NK_MAX_K) fused CUDA-core passes; pass p+1
-// only admits keys strictly below the last key pass p returned, so the passes tile the ranking exactly.
-static int run_scan_bigk(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uint32_t k, uint64_t *out_keys,
-                         cudaStream_t stream, const void *rows = nullptr, uint32_t n_rows = 0, bool custom_rows = false,
-                         const NkFilter *qfilter = nullptr) {
-    if (nk::ws_reserve((void **)&s.ws.below, &s.ws.below_bytes, (size_t)Q * 8)) return -1;
-    if (nk::ws_reserve((void **)&s.ws.keys2, &s.ws.keys2_bytes, (size_t)Q * NK_MAX_K * 8)) return -1;
-    NK_CUDA_OK(cudaMemsetAsync(s.ws.below, 0xff, (size_t)Q * 8, stream));
-    for (uint32_t done = 0; done < k;) {
-        const uint32_t kp = k - done < NK_MAX_K ? k - done : NK_MAX_K;
-        nk::ScanArgs a;
-        a.rows = custom_rows ? rows : s.rows; a.dtype = ix->dtype; a.n = custom_rows ? n_rows : (uint32_t)s.n; a.dim = ix->dim;
-        a.row_base = custom_rows ? 0 : s.base;
-        a.queries = q_dev; a.Q = Q; a.k = kp; a.metric = ix->metric; a.stream = stream; a.below = s.ws.below;
-        a.row_mask = (!custom_rows && s.mask_on) ? s.mask : nullptr;
-        a.min_score = custom_rows ? -INFINITY : ix->key_floor();
-        if (qfilter && !custom_rows) { a.row_tags = s.tags; a.qfilter = qfilter; }
-        if (nk::scan_simt(s.di, a, s.ws, s.ws.keys2, &ix->stats.kernel_launches)) return -1;
-        NK_CUDA_OK(cudaMemcpy2DAsync(out_keys + done, (size_t)k * 8, s.ws.keys2, (size_t)kp * 8, (size_t)kp * 8, Q,
-                                     cudaMemcpyDeviceToDevice, stream));
-        if (nk::update_below(s.ws.keys2, Q, kp, s.ws.below, stream)) return -1;
-        ix->stats.kernel_launches++;
-        ix->stats.bytes_scanned += (uint64_t)s.n * ix->dim * ix->esz() * ((Q + 7) / 8);
-        done += kp;
-    }
-    ix->last_path = NK_PATH_SIMT;
-    return 0;
+// The scan of Q device queries over shard s as it stands: its rows, the row mask and the score floor; qfilter (per-query tag
+// filters [Q] on the device, nullptr = none) needs the shard's tag array on.
+static nk::ScanArgs shard_scan_args(const NkIndex *ix, const NkShard &s, const float *q_dev, uint32_t Q, uint32_t k,
+                                    cudaStream_t stream, const NkFilter *qfilter = nullptr) {
+    nk::ScanArgs a;
+    a.rows = s.rows; a.dtype = ix->dtype; a.n = (uint32_t)s.n; a.dim = ix->dim; a.row_base = s.base;
+    a.queries = q_dev; a.Q = Q; a.k = k; a.metric = ix->metric; a.stream = stream;
+    a.row_mask = s.mask_on ? s.mask : nullptr; a.min_score = ix->key_floor();
+    if (qfilter) { a.row_tags = s.tags; a.qfilter = qfilter; }
+    return a;
 }
 
 // a with the shard's 16-bit image attached, if it has an up-to-date one: the BF16 shadow of an fp32 shard, or a 16-bit
@@ -386,53 +370,125 @@ static nk::ScanArgs with_16bit_image(const NkIndex *ix, const NkShard &s, const 
     return as;
 }
 
+// The path a scan of *a over shard s takes: the forced one (an error if it cannot serve the shape), or AUTO's pick.  *a gets
+// the shard's 16-bit image attached if the path is the 16-bit pass.  Range searches have no exact 3xTF32 mode.
+// AUTO: CUDA cores keep Q <= 4 (the single-kernel scan already streams the fewest bytes), tensor cores from 5 queries on.
+// With a BF16 shadow the filter streams half the bytes of the fp32 rows, so it serves every batch size once the shard is
+// large enough for bytes (not launches) to matter; small shards keep the CUDA-core scan at Q <= 4.  16-bit shards: the
+// 16-bit tensor pass from 5 queries on.
+static int plan_path(const NkIndex *ix, const NkShard &s, bool range, nk::ScanArgs *a) {
+    if (range && ix->path == NK_PATH_TENSOR) {
+        nk::set_error("nk_search_range: the exact 3xTF32 path has no range mode (use AUTO, SIMT, TENSOR_FILTER or TENSOR_SHADOW)");
+        return -1;
+    }
+    const nk::ScanArgs as = with_16bit_image(ix, s, *a);
+    const bool tensor_ok = !range && nk::scan_tensor_supported(s.di, *a);
+    const bool filter_ok = ix->dtype == NK_DTYPE_F32 && nk::scan_tensor_filter_supported(s.di, *a);
+    const bool shadow_ok = as.shadow != nullptr && nk::shadow_pass_supported(s.di, as) && nk::scan_tensor_filter_supported(s.di, as);
+    int use = NK_PATH_SIMT;
+    if (ix->path == NK_PATH_TENSOR || ix->path == NK_PATH_TENSOR_FILTER || ix->path == NK_PATH_TENSOR_SHADOW) {
+        if (!(ix->path == NK_PATH_TENSOR ? tensor_ok : ix->path == NK_PATH_TENSOR_FILTER ? filter_ok : shadow_ok)) {
+            nk::set_error("tensor path %d does not support this shape (dim=%u dtype=%d metric=%d Q=%u k=%u shadow=%d)", ix->path, ix->dim,
+                          ix->dtype, ix->metric, a->Q, a->k, (int)(as.shadow != nullptr));
+            return -1;
+        }
+        use = ix->path;
+    } else if (ix->path == NK_PATH_AUTO) {
+        const bool big_shard = (uint64_t)s.n * ix->dim * 4 >= (64ull << 20);
+        if (a->Q >= 5) use = shadow_ok ? NK_PATH_TENSOR_SHADOW : filter_ok ? NK_PATH_TENSOR_FILTER : tensor_ok ? NK_PATH_TENSOR : NK_PATH_SIMT;
+        else if (shadow_ok && big_shard && ix->dtype == NK_DTYPE_F32) use = NK_PATH_TENSOR_SHADOW;
+    }
+    if (use == NK_PATH_TENSOR_SHADOW) *a = as;
+    return use;
+}
+
+// Times the main kernels of one scan (nk_index_enable_timing): attach() gives the scan an event pair, keep() hands it to the
+// shard for nk_index_scan_time_ms if the scan launched a main kernel.  Every pair not kept is destroyed.
+class ScanTimer {
+  public:
+    explicit ScanTimer(NkShard &s) : s_(s) {}
+    ~ScanTimer() {
+        for (cudaEvent_t e : ev_)
+            if (e) cudaEventDestroy(e);
+    }
+    ScanTimer(const ScanTimer &) = delete;
+    ScanTimer &operator=(const ScanTimer &) = delete;
+    int attach(const NkIndex *ix, nk::ScanArgs *a) {
+        if (!ix->timing_on) return 0;
+        for (cudaEvent_t &e : ev_) NK_CUDA_OK(cudaEventCreate(&e));
+        a->ev_begin = ev_[0]; a->ev_end = ev_[1]; a->main_launches = &launches_;
+        return 0;
+    }
+    void keep() {  // the scan succeeded
+        if (!launches_) return;
+        s_.timing.emplace_back(ev_[0], ev_[1]);
+        s_.timing_launches.push_back(launches_);
+        ev_[0] = ev_[1] = nullptr;
+    }
+
+  private:
+    NkShard &s_;
+    cudaEvent_t ev_[2] = {nullptr, nullptr};
+    uint64_t launches_ = 0;
+};
+
+// NkStats::bytes_scanned of `passes` scans of a on path `use`: every pass streams the a.n rows once per block of queries
+// (8 on CUDA cores, 64 in the exact 3xTF32 scan, 128 in the filters); the 16-bit pass streams the 16-bit image, dimpad bf16
+// per fp32 row.
+static uint64_t scan_bytes(const NkIndex *ix, int use, const nk::ScanArgs &a, uint64_t passes) {
+    const uint32_t width = use == NK_PATH_SIMT ? 8 : use == NK_PATH_TENSOR ? 64 : 128;
+    const uint64_t row_bytes = use == NK_PATH_TENSOR_SHADOW ? (uint64_t)(ix->dtype == NK_DTYPE_F32 ? ix->dimpad() : ix->dim) * 2
+                                                            : (uint64_t)ix->dim * ix->esz();
+    return (uint64_t)a.n * row_bytes * ((a.Q + width - 1) / width) * passes;
+}
+
+// a.k > NK_MAX_K (the reference accepts any k, cuda_bridge.go:327-375): ceil(a.k / NK_MAX_K) fused CUDA-core passes; pass p+1
+// only admits keys strictly below the last key pass p returned, so the passes tile the ranking exactly.
+static int run_scan_bigk(NkIndex *ix, NkShard &s, nk::ScanArgs a, uint64_t *out_keys) {
+    const uint32_t Q = a.Q, k = a.k;
+    if (nk::ws_reserve((void **)&s.ws.below, &s.ws.below_bytes, (size_t)Q * 8)) return -1;
+    if (nk::ws_reserve((void **)&s.ws.keys2, &s.ws.keys2_bytes, (size_t)Q * NK_MAX_K * 8)) return -1;
+    NK_CUDA_OK(cudaMemsetAsync(s.ws.below, 0xff, (size_t)Q * 8, a.stream));
+    a.below = s.ws.below;
+    for (uint32_t done = 0; done < k;) {
+        const uint32_t kp = k - done < NK_MAX_K ? k - done : NK_MAX_K;
+        a.k = kp;
+        if (nk::scan_simt(s.di, a, s.ws, s.ws.keys2, &ix->stats.kernel_launches)) return -1;
+        NK_CUDA_OK(cudaMemcpy2DAsync(out_keys + done, (size_t)k * 8, s.ws.keys2, (size_t)kp * 8, (size_t)kp * 8, Q,
+                                     cudaMemcpyDeviceToDevice, a.stream));
+        if (nk::update_below(s.ws.keys2, Q, kp, s.ws.below, a.stream)) return -1;
+        ix->stats.kernel_launches++;
+        ix->stats.bytes_scanned += scan_bytes(ix, NK_PATH_SIMT, a, 1);
+        done += kp;
+    }
+    ix->last_path = NK_PATH_SIMT;
+    return 0;
+}
+
+struct ScanOut {  // optional extras of run_scan
+    uint32_t *out_idx = nullptr;   // fused decode (single-shard searches)
+    float *out_score = nullptr;
+    bool defer_tail = false;       // host-synchronous caller: retry stages are queued only if a flag was raised
+    const NkFilter *qfilter = nullptr;  // per-query tag filters [Q] (device; the shard's tag array must be on)
+};
+
 static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uint32_t k, uint64_t *out_keys,
-                    cudaStream_t stream, const ScanOut &xo) {
+                    cudaStream_t stream, const ScanOut &xo = ScanOut()) {
     s.last_filter = false;
+    nk::ScanArgs a = shard_scan_args(ix, s, q_dev, Q, k, stream, xo.qfilter);
     if (k > NK_MAX_K) {
-        if (run_scan_bigk(ix, s, q_dev, Q, k, out_keys, stream, nullptr, 0, false, xo.qfilter)) return -1;
+        if (run_scan_bigk(ix, s, a, out_keys)) return -1;
         if (xo.out_idx) {
             if (nk::decode_keys(out_keys, Q, k, ix->metric, xo.out_idx, xo.out_score, stream)) return -1;
             ix->stats.kernel_launches++;
         }
         return 0;
     }
-    nk::ScanArgs a;
-    a.rows = s.rows; a.dtype = ix->dtype; a.n = (uint32_t)s.n; a.dim = ix->dim; a.row_base = s.base;
-    a.queries = q_dev; a.Q = Q; a.k = k; a.metric = ix->metric; a.stream = stream;
-    a.row_mask = s.mask_on ? s.mask : nullptr;
-    a.out_idx = xo.out_idx; a.out_score = xo.out_score; a.min_score = ix->key_floor(); a.defer_tail = xo.defer_tail;
-    if (xo.qfilter) { a.row_tags = s.tags; a.qfilter = xo.qfilter; }
-    // AUTO: CUDA cores keep Q <= 4 (the single-kernel scan already streams the fewest bytes), tensor cores from 5 queries
-    // on.  With a BF16 shadow the filter streams half the bytes of the fp32 rows, so it serves every batch size once the
-    // shard is large enough for bytes (not launches) to matter; small shards keep the CUDA-core scan at Q <= 4.  16-bit
-    // shards: the 16-bit tensor pass from 5 queries on.
-    const nk::ScanArgs as = with_16bit_image(ix, s, a);
-    const bool tensor_ok = nk::scan_tensor_supported(s.di, a);
-    const bool filter_ok = ix->dtype == NK_DTYPE_F32 && nk::scan_tensor_filter_supported(s.di, a);
-    const bool shadow_ok = as.shadow != nullptr && nk::shadow_pass_supported(s.di, as) && nk::scan_tensor_filter_supported(s.di, as);
-    int use = NK_PATH_SIMT;
-    if (ix->path == NK_PATH_TENSOR || ix->path == NK_PATH_TENSOR_FILTER || ix->path == NK_PATH_TENSOR_SHADOW) {
-        if (!(ix->path == NK_PATH_TENSOR ? tensor_ok : ix->path == NK_PATH_TENSOR_FILTER ? filter_ok : shadow_ok)) {
-            nk::set_error("tensor path %d does not support this shape (dim=%u dtype=%d metric=%d Q=%u k=%u shadow=%d)", ix->path, ix->dim,
-                          ix->dtype, ix->metric, Q, k, (int)(as.shadow != nullptr));
-            return -1;
-        }
-        use = ix->path;
-    } else if (ix->path == NK_PATH_AUTO) {
-        const bool big_shard = (uint64_t)s.n * ix->dim * 4 >= (64ull << 20);
-        if (Q >= 5) use = shadow_ok ? NK_PATH_TENSOR_SHADOW : filter_ok ? NK_PATH_TENSOR_FILTER : tensor_ok ? NK_PATH_TENSOR : NK_PATH_SIMT;
-        else if (shadow_ok && big_shard && ix->dtype == NK_DTYPE_F32) use = NK_PATH_TENSOR_SHADOW;
-    }
-    if (use == NK_PATH_TENSOR_SHADOW) a = as;
-    const bool use_tensor = use != NK_PATH_SIMT;
-    cudaEvent_t e0 = nullptr, e1 = nullptr;
-    uint64_t main_launches = 0;
-    if (ix->timing_on) {
-        NK_CUDA_OK(cudaEventCreate(&e0));
-        NK_CUDA_OK(cudaEventCreate(&e1));
-        a.ev_begin = e0; a.ev_end = e1; a.main_launches = &main_launches;
-    }
+    a.out_idx = xo.out_idx; a.out_score = xo.out_score; a.defer_tail = xo.defer_tail;
+    const int use = plan_path(ix, s, false, &a);
+    if (use < 0) return -1;
+    ScanTimer timer(s);
+    if (timer.attach(ix, &a)) return -1;
     const bool is_filter = use == NK_PATH_TENSOR_FILTER || use == NK_PATH_TENSOR_SHADOW;
     NK_RANGE_PUSH(use == NK_PATH_TENSOR_SHADOW ? "nk:scan:shadow" : use == NK_PATH_TENSOR_FILTER ? "nk:scan:tf32-filter"
                   : use == NK_PATH_TENSOR ? "nk:scan:3xtf32" : "nk:scan:simt");
@@ -440,53 +496,44 @@ static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uin
              : use == NK_PATH_TENSOR ? nk::scan_tensor(s.di, a, s.ws, out_keys, &ix->stats.kernel_launches)
                                      : nk::scan_simt(s.di, a, s.ws, out_keys, &ix->stats.kernel_launches);
     NK_RANGE_POP();
-    if (ix->timing_on) {
-        if (rc == 0 && main_launches) {
-            s.timing.emplace_back(e0, e1);
-            s.timing_launches.push_back(main_launches);
-        } else {
-            cudaEventDestroy(e0);
-            cudaEventDestroy(e1);
-        }
-    }
     ix->last_path = use;
-    if (rc == 0 && is_filter) {
+    if (rc) return rc;
+    timer.keep();
+    if (is_filter) {
         s.last_filter = true;
         s.last_args = a;
         s.last_args.ev_begin = s.last_args.ev_end = nullptr;
         s.last_args.main_launches = nullptr;
         s.last_out_keys = out_keys;
     }
-    if (rc == 0)
-        ix->stats.bytes_scanned += use == NK_PATH_TENSOR_SHADOW ? (uint64_t)s.n * (ix->dtype == NK_DTYPE_F32 ? ix->dimpad() : ix->dim) * 2 * ((Q + 127) / 128)
-                                   : (uint64_t)s.n * ix->dim * ix->esz() * (use == NK_PATH_TENSOR_FILTER ? ((Q + 127) / 128) : use_tensor ? ((Q + 63) / 64) : ((Q + 7) / 8));
-    return rc;
+    ix->stats.bytes_scanned += scan_bytes(ix, use, a, 1);
+    return 0;
 }
 
-// Host-synchronous searches defer the retry / exact stages of the filter paths: after the stream has drained, look at the
-// status words; only if a stage overflowed (adversarial near-ties, NaN rows) queue the tail, wait again and let the caller
-// re-read the results.  Returns 1 if a retry ran, 0 if not, -1 on error (a fatal candidate-buffer overflow included).
-static int finish_deferred(NkIndex *ix, NkShard &s) {
-    int h[nk::NK_FLAG_WORDS];
-    NK_CUDA_OK(cudaMemcpyAsync(h, s.ws.flags, sizeof(h), cudaMemcpyDeviceToHost, s.stream));
-    NK_CUDA_OK(cudaStreamSynchronize(s.stream));
-    int retried = 0;
-    if (s.last_filter && s.last_args.defer_tail && (h[nk::FLAG_RETRY] || h[nk::FLAG_OVERFLOW])) {
-        NK_RANGE_PUSH("nk:retry-tail");
-        const int rc = nk::scan_tensor_filter_tail(s.di, s.last_args, s.ws, s.last_out_keys, &ix->stats.kernel_launches);
-        NK_RANGE_POP();
-        if (rc) return -1;
-        NK_CUDA_OK(cudaMemcpyAsync(h, s.ws.flags, sizeof(int), cudaMemcpyDeviceToHost, s.stream));
-        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
-        retried = 1;
-    }
+// Host-synchronous searches defer the retry / exact stages of the filter paths.  h is the shard's status words, read after
+// the stream has drained: the fatal word set -> clear it and fail (-1); a deferred filter stage overflowed (adversarial
+// near-ties, NaN rows) -> queue the tail, and the caller waits and reads again (1); else the results stand (0).  The tail is
+// queued at most once per search.
+static int shard_status(NkIndex *ix, NkShard &s, const int *h) {
+    const bool tail = s.last_filter && s.last_args.defer_tail && (h[nk::FLAG_RETRY] || h[nk::FLAG_OVERFLOW]);
     s.last_filter = false;
-    if (h[nk::FLAG_FATAL]) {
-        cudaMemsetAsync(s.ws.flags, 0, sizeof(int), s.stream);
-        nk::set_error("internal: candidate buffer overflow (flag=%d)", h[nk::FLAG_FATAL]);
-        return -1;
+    if (h[nk::FLAG_FATAL]) return nk::fatal_overflow(h[nk::FLAG_FATAL], s.ws.flags, s.stream);
+    if (!tail) return 0;
+    NK_RANGE_PUSH("nk:retry-tail");
+    const int rc = nk::scan_tensor_filter_tail(s.di, s.last_args, s.ws, s.last_out_keys, &ix->stats.kernel_launches);
+    NK_RANGE_POP();
+    return rc ? -1 : 1;
+}
+
+// shard_status on the status words alone, the retry tail included: 0 or -1.
+static int finish_deferred(NkIndex *ix, NkShard &s) {
+    for (;;) {
+        int h[nk::NK_FLAG_WORDS];
+        NK_CUDA_OK(cudaMemcpyAsync(h, s.ws.flags, sizeof(h), cudaMemcpyDeviceToHost, s.stream));
+        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+        const int st = shard_status(ix, s, h);
+        if (st <= 0) return st;
     }
-    return retried;
 }
 
 extern "C" {
@@ -563,42 +610,50 @@ void nk_index_release(NkIndex *ix) {
     delete ix;
 }
 
-static int upload_impl(NkIndex *ix, const void *rows_host, uint64_t n_rows, bool src_is_f32) {
-    nk::DeviceGuard _restore_device;
-    if (!ix) { nk::set_error("null index"); return -1; }
-    if (n_rows && !rows_host) { nk::set_error("null rows"); return -1; }
+// Replace the whole corpus by n_rows new rows, shard g taking the contiguous range [g*N/G, (g+1)*N/G): write(s, first, cnt)
+// queues the write of rows [first, first+cnt) into the shard's reserved rows on its stream.
+using WriteRows = std::function<int(NkShard &, uint64_t first, uint64_t cnt)>;
+static int repartition(NkIndex *ix, uint64_t n_rows, const WriteRows &write) {
     std::lock_guard<std::mutex> lk(ix->mu);
     ShardOrder order(ix);
     if (order.failed()) return -1;
     drop_row_mask(ix);
-    const bool cvt = src_is_f32 && ix->dtype != NK_DTYPE_F32;
-    const size_t rb = (size_t)ix->dim * ix->esz(), src_rb = (size_t)ix->dim * (cvt ? 4 : ix->esz());
+    if (check_row_limit(ix, n_rows)) return -1;
     const uint64_t G = ix->shards.size();
-    // global row ids are 32-bit on this boundary (SearchResult.Index uint32, cuda_bridge.go:425-428)
-    if (ix->row_base + n_rows > 0xfffffff0ull) { nk::set_error("index exceeds 2^32 rows (row ids are uint32)"); return -1; }
     uint64_t off = 0;
     for (uint64_t g = 0; g < G; ++g) {
         NkShard &s = ix->shards[g];
-        uint64_t cnt = n_rows * (g + 1) / G - n_rows * g / G;  // contiguous range [g*N/G, (g+1)*N/G)
+        const uint64_t cnt = n_rows * (g + 1) / G - n_rows * g / G;
         NK_CUDA_OK(cudaSetDevice(s.device));
         if (!s.owns) { s.rows = nullptr; s.owns = true; s.cap = 0; s.shadow_attached = false; }
         s.n = 0;
         s.tags_on = false;  // every tag back to 0
         if (shard_reserve_rows(ix, s, cnt, false)) return -1;
-        if (stream_h2d(s, s.rows, static_cast<const char *>(rows_host) + off * src_rb, cnt * src_rb, cvt, ix->dtype)) return -1;
+        if (write(s, off, cnt)) return -1;
         s.n = cnt;
         s.shadow_n = 0;
         if (shard_sync_shadow(ix, s)) return -1;
         off += cnt;
-        ix->stats.bytes_h2d += cnt * src_rb;
     }
     for (auto &s : ix->shards) {
         NK_CUDA_OK(cudaSetDevice(s.device));
         NK_CUDA_OK(cudaStreamSynchronize(s.stream));
     }
     rebase(ix);
-    (void)rb;
     return 0;
+}
+
+static int upload_impl(NkIndex *ix, const void *rows_host, uint64_t n_rows, bool src_is_f32) {
+    nk::DeviceGuard _restore_device;
+    if (!ix) { nk::set_error("null index"); return -1; }
+    if (n_rows && !rows_host) { nk::set_error("null rows"); return -1; }
+    const bool cvt = src_is_f32 && ix->dtype != NK_DTYPE_F32;
+    const size_t src_rb = (size_t)ix->dim * (cvt ? 4 : ix->esz());
+    return repartition(ix, n_rows, [&](NkShard &s, uint64_t first, uint64_t cnt) {
+        if (stream_h2d(s, s.rows, static_cast<const char *>(rows_host) + first * src_rb, cnt * src_rb, cvt, ix->dtype)) return -1;
+        ix->stats.bytes_h2d += cnt * src_rb;
+        return 0;
+    });
 }
 
 int nk_index_upload(NkIndex *ix, const void *rows_host, uint64_t n_rows) { return upload_impl(ix, rows_host, n_rows, false); }
@@ -637,7 +692,7 @@ int nk_index_append(NkIndex *ix, const void *rows_host, uint64_t n_rows) {
     if (order.failed()) return -1;
     drop_row_mask(ix);
     const size_t rb = (size_t)ix->dim * ix->esz();
-    if (ix->row_base + ix->rows() + n_rows > 0xfffffff0ull) { nk::set_error("index exceeds 2^32 rows (row ids are uint32)"); return -1; }
+    if (check_row_limit(ix, ix->rows() + n_rows)) return -1;
     NK_CUDA_OK(cudaSetDevice(s.device));
     if (shard_reserve_rows(ix, s, s.n + n_rows, true)) return -1;
     if (stream_h2d(s, (char *)s.rows + s.n * rb, rows_host, n_rows * rb)) return -1;
@@ -719,36 +774,14 @@ int nk_index_remove_swap(NkIndex *ix, uint64_t row) {
 static int fill_impl(NkIndex *ix, uint64_t n_rows, uint64_t seed, uint32_t centres, float sigma, int unit) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
-    std::lock_guard<std::mutex> lk(ix->mu);
-    ShardOrder order(ix);
-    if (order.failed()) return -1;
-    drop_row_mask(ix);
-    const uint64_t G = ix->shards.size();
-    if (ix->row_base + n_rows > 0xfffffff0ull) { nk::set_error("index exceeds 2^32 rows (row ids are uint32)"); return -1; }
-    uint64_t off = 0;
-    for (uint64_t g = 0; g < G; ++g) {
-        NkShard &s = ix->shards[g];
-        uint64_t cnt = n_rows * (g + 1) / G - n_rows * g / G;
-        NK_CUDA_OK(cudaSetDevice(s.device));
-        if (!s.owns) { s.rows = nullptr; s.owns = true; s.cap = 0; s.shadow_attached = false; }
-        s.n = 0;
-        s.tags_on = false;  // every tag back to 0
-        if (shard_reserve_rows(ix, s, cnt, false)) return -1;
-        if (centres ? nk::fill_clustered(s.rows, ix->dtype, cnt, ix->dim, seed, ix->row_base + off, centres, sigma, unit, s.stream)
-                    : nk::fill_uniform(s.rows, ix->dtype, cnt, ix->dim, seed, ix->row_base + off, s.stream))
+    return repartition(ix, n_rows, [&](NkShard &s, uint64_t first, uint64_t cnt) {
+        const uint64_t row0 = ix->row_base + first;
+        if (centres ? nk::fill_clustered(s.rows, ix->dtype, cnt, ix->dim, seed, row0, centres, sigma, unit, s.stream)
+                    : nk::fill_uniform(s.rows, ix->dtype, cnt, ix->dim, seed, row0, s.stream))
             return -1;
         ix->stats.kernel_launches++;
-        s.n = cnt;
-        s.shadow_n = 0;
-        if (shard_sync_shadow(ix, s)) return -1;
-        off += cnt;
-    }
-    for (auto &s : ix->shards) {
-        NK_CUDA_OK(cudaSetDevice(s.device));
-        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
-    }
-    rebase(ix);
-    return 0;
+        return 0;
+    });
 }
 
 int nk_index_fill_uniform(NkIndex *ix, uint64_t n_rows, uint64_t seed) { return fill_impl(ix, n_rows, seed, 0, 0.0f, 0); }
@@ -771,7 +804,7 @@ int nk_index_attach_device_rows(NkIndex *ix, void *rows_dev, uint64_t n_rows) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
     if (ix->shards.size() != 1) { nk::set_error("attach applies to single-device indexes"); return -1; }
-    if (ix->row_base + n_rows > 0xfffffff0ull) { nk::set_error("index exceeds 2^32 rows (row ids are uint32)"); return -1; }
+    if (check_row_limit(ix, n_rows)) return -1;
     std::lock_guard<std::mutex> lk(ix->mu);
     NkShard &s = ix->shards[0];
     ShardOrder order(s, s.stream);
@@ -893,6 +926,7 @@ int nk_index_set_row_tags(NkIndex *ix, uint64_t first_row, const uint64_t *tags_
 
 int nk_index_set_path(NkIndex *ix, int path) {
     if (!ix || path < NK_PATH_AUTO || path > NK_PATH_TENSOR_SHADOW) { nk::set_error("bad path"); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
     ix->path = path;
     return 0;
 }
@@ -906,14 +940,20 @@ int nk_index_stats(const NkIndex *ix, NkStats *out) {
     return 0;
 }
 
-int nk_index_debug_flags(NkIndex *ix, int out[4]) {
-    nk::DeviceGuard _restore_device;
+// Shard 0's status words once its device has drained (diagnostics); out is the caller's output, checked for null here.
+static int shard0_status_words(NkIndex *ix, const void *out, int h[nk::NK_FLAG_WORDS]) {
     if (!ix || !out || ix->shards.empty()) { nk::set_error("null argument"); return -1; }
     NkShard &s = ix->shards[0];
     NK_CUDA_OK(cudaSetDevice(s.device));
     NK_CUDA_OK(cudaDeviceSynchronize());
+    NK_CUDA_OK(cudaMemcpy(h, s.ws.flags, sizeof(int) * nk::NK_FLAG_WORDS, cudaMemcpyDeviceToHost));
+    return 0;
+}
+
+int nk_index_debug_flags(NkIndex *ix, int out[4]) {
+    nk::DeviceGuard _restore_device;
     int h[nk::NK_FLAG_WORDS];
-    NK_CUDA_OK(cudaMemcpy(h, s.ws.flags, sizeof(h), cudaMemcpyDeviceToHost));
+    if (shard0_status_words(ix, out, h)) return -1;
     out[0] = h[nk::FLAG_FATAL]; out[1] = h[nk::FLAG_OVERFLOW]; out[2] = h[nk::FLAG_MAXXX]; out[3] = h[nk::FLAG_RETRY];
     return 0;
 }
@@ -923,12 +963,8 @@ int nk_index_debug_flags(NkIndex *ix, int out[4]) {
 // survivor list of the last filter search.  bench.py reports out[0..1] / searches as the retry rate of a corpus.
 int nk_index_debug_counters(NkIndex *ix, uint64_t out[4]) {
     nk::DeviceGuard _restore_device;
-    if (!ix || !out || ix->shards.empty()) { nk::set_error("null argument"); return -1; }
-    NkShard &s = ix->shards[0];
-    NK_CUDA_OK(cudaSetDevice(s.device));
-    NK_CUDA_OK(cudaDeviceSynchronize());
     int h[nk::NK_FLAG_WORDS];
-    NK_CUDA_OK(cudaMemcpy(h, s.ws.flags, sizeof(h), cudaMemcpyDeviceToHost));
+    if (shard0_status_words(ix, out, h)) return -1;
     out[0] = (uint64_t)h[nk::FLAG_N_RETRY]; out[1] = (uint64_t)h[nk::FLAG_N_EXACT]; out[2] = (uint64_t)h[nk::FLAG_LONGEST]; out[3] = (uint64_t)h[nk::FLAG_OVF_BITS];
     return 0;
 }
@@ -941,8 +977,8 @@ int nk_debug_filter_dump(NkIndex *ix, const float *queries_host, uint32_t Q, int
     NkShard *s;
     if (!ix || ix->shards.size() != 1) { nk::set_error("single-device index required"); return -1; }
     s = &ix->shards[0];
-    if (!queries_host || !est_host || !bnd_host || Q == 0 || Q > 64 || s->n == 0) { nk::set_error("bad argument (1 <= Q <= 64, non-empty index)"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
+    if (!queries_host || !est_host || !bnd_host || Q == 0 || Q > 64 || s->n == 0) { nk::set_error("bad argument (1 <= Q <= 64, non-empty index)"); return -1; }
     ShardOrder order(*s, s->stream);
     if (order.failed()) return -1;
     NK_CUDA_OK(cudaSetDevice(s->device));
@@ -954,14 +990,8 @@ int nk_debug_filter_dump(NkIndex *ix, const float *queries_host, uint32_t Q, int
         if (nk::ws_reserve((void **)&s->ws.queries, &s->ws.queries_bytes, (size_t)Q * ix->dim * 4)) break;
         if (cudaMemcpyAsync(s->ws.queries, queries_host, (size_t)Q * ix->dim * 4, cudaMemcpyHostToDevice, s->stream) != cudaSuccess) break;
         if (cudaMemsetAsync(d, 0, cells * 8, s->stream) != cudaSuccess) break;
-        nk::ScanArgs a;
-        a.rows = s->rows; a.dtype = ix->dtype; a.n = (uint32_t)s->n; a.dim = ix->dim; a.row_base = s->base;
-        a.queries = s->ws.queries; a.Q = Q; a.k = 1; a.metric = ix->metric; a.stream = s->stream;
-        if (s->xnorm2 && s->shadow_n == s->n) {
-            if (ix->dtype == NK_DTYPE_F32) { a.shadow = s->shadow; a.dnorm2 = s->dnorm2; }
-            else { a.shadow = s->rows; a.shadow_native = true; }
-            a.shadow_dimpad = ix->dimpad(); a.xnorm2 = s->xnorm2;
-        }
+        nk::ScanArgs a = with_16bit_image(ix, *s, shard_scan_args(ix, *s, s->ws.queries, Q, 1, s->stream));
+        a.row_mask = nullptr;  // every pair (the dump ignores the score floor itself)
         if (nk::scan_filter_dump(s->di, a, s->ws, which, d, d + cells, Q, &ix->stats.kernel_launches)) break;
         if (cudaMemcpyAsync(est_host, d, cells * 4, cudaMemcpyDeviceToHost, s->stream) != cudaSuccess) break;
         if (cudaMemcpyAsync(bnd_host, d + cells, cells * 4, cudaMemcpyDeviceToHost, s->stream) != cudaSuccess) break;
@@ -981,6 +1011,7 @@ int nk_index_last_path(const NkIndex *ix) { return ix ? ix->last_path : -1; }
 
 int nk_index_enable_timing(NkIndex *ix, int enabled) {
     if (!ix) { nk::set_error("null index"); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
     ix->timing_on = enabled != 0;
     return 0;
 }
@@ -1034,6 +1065,17 @@ int nk_index_read_rows(NkIndex *ix, uint64_t row, uint64_t n_rows, void *rows_ho
 // Writes the Q fp32 queries of a search into s.ws.queries (already reserved) on s.stream; the device is s's.
 using StageQueries = std::function<int(NkShard &)>;
 
+// Per-query tag filters of a host search -> the shard workspace, next to the queries (the deferred retry tail reads them
+// after the call's first synchronisation), with the shard's tag array on.  The device copy, or nullptr on error.
+static const NkFilter *stage_filters(NkIndex *ix, NkShard &s, const NkFilter *filters_host, uint32_t Q) {
+    const size_t fbytes = (size_t)Q * sizeof(NkFilter);
+    if (shard_tags_on(s)) return nullptr;
+    if (nk::ws_reserve((void **)&s.ws.qfilter, &s.ws.qfilter_bytes, fbytes)) return nullptr;
+    NK_CUDA_OK_PTR(cudaMemcpyAsync(s.ws.qfilter, filters_host, fbytes, cudaMemcpyHostToDevice, s.stream));
+    ix->stats.bytes_h2d += fbytes;
+    return s.ws.qfilter;
+}
+
 // One synchronous search of Q staged queries over the live (non-empty) shards, the index lock held: scan, deferred retry
 // tail, merge; writes ke results per query into out_idx / out_score [Q x k] (row stride k) and returns ke.
 static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const StageQueries &stage, const NkFilter *filters_host,
@@ -1055,15 +1097,7 @@ static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const St
             xo.out_idx = s->ws.out_idx; xo.out_score = s->ws.out_score;
         }
         if (stage(*s)) return -1;
-        if (filters_host) {
-            // staged next to the queries, in the shard workspace: the deferred retry tail reads them after this call's first sync
-            const size_t fbytes = (size_t)Q * sizeof(NkFilter);
-            if (shard_tags_on(*s)) return -1;
-            if (nk::ws_reserve((void **)&s->ws.qfilter, &s->ws.qfilter_bytes, fbytes)) return -1;
-            NK_CUDA_OK(cudaMemcpyAsync(s->ws.qfilter, filters_host, fbytes, cudaMemcpyHostToDevice, s->stream));
-            ix->stats.bytes_h2d += fbytes;
-            xo.qfilter = s->ws.qfilter;
-        }
+        if (filters_host && !(xo.qfilter = stage_filters(ix, *s, filters_host, Q))) return -1;
         if (run_scan(ix, *s, s->ws.queries, Q, ke, s->ws.keys, s->stream, xo)) return -1;
     }
 
@@ -1072,36 +1106,17 @@ static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const St
         // synchronisation (pageable cudaMemcpyAsync targets cost a driver-side staging round trip each).
         NkShard *s = live[0];
         NK_CUDA_OK(cudaSetDevice(s->device));
-        const size_t rbytes = (size_t)Q * ke * 4, need = 2 * rbytes + sizeof(int) * nk::NK_FLAG_WORDS;
-        if (s->h_res_bytes < need) {
-            if (s->h_res) cudaFreeHost(s->h_res);
-            s->h_res = nullptr; s->h_res_bytes = 0;
-            NK_CUDA_OK(cudaMallocHost((void **)&s->h_res, need + need / 4));
-            s->h_res_bytes = need + need / 4;
-        }
+        const size_t rbytes = (size_t)Q * ke * 4;
+        if (pinned_reserve((void **)&s->h_res, &s->h_res_bytes, 2 * rbytes + sizeof(int) * nk::NK_FLAG_WORDS)) return -1;
         int *hflags = reinterpret_cast<int *>(s->h_res + 2 * rbytes);
-        for (int pass = 0; pass < 2; ++pass) {
+        for (int st = 1; st;) {  // read, and once more after a retry tail
             NK_CUDA_OK(cudaMemcpyAsync(s->h_res, s->ws.out_idx, rbytes, cudaMemcpyDeviceToHost, s->stream));
             NK_CUDA_OK(cudaMemcpyAsync(s->h_res + rbytes, s->ws.out_score, rbytes, cudaMemcpyDeviceToHost, s->stream));
             NK_CUDA_OK(cudaMemcpyAsync(hflags, s->ws.flags, sizeof(int) * nk::NK_FLAG_WORDS, cudaMemcpyDeviceToHost, s->stream));
             NK_CUDA_OK(cudaStreamSynchronize(s->stream));
             ix->stats.bytes_d2h += (uint64_t)Q * ke * 8;
-            if (hflags[nk::FLAG_FATAL]) {
-                cudaMemsetAsync(s->ws.flags, 0, sizeof(int), s->stream);
-                nk::set_error("internal: candidate buffer overflow (flag=%d)", hflags[nk::FLAG_FATAL]);
-                return -1;
-            }
-            if (pass == 0 && s->last_filter && s->last_args.defer_tail && (hflags[nk::FLAG_RETRY] || hflags[nk::FLAG_OVERFLOW])) {
-                // a filter stage overflowed (near-ties, NaN rows): queue the retry / exact stages now and read again
-                NK_RANGE_PUSH("nk:retry-tail");
-                const int rc = nk::scan_tensor_filter_tail(s->di, s->last_args, s->ws, s->last_out_keys, &ix->stats.kernel_launches);
-                NK_RANGE_POP();
-                if (rc) return -1;
-                continue;
-            }
-            break;
+            if ((st = shard_status(ix, *s, hflags)) < 0) return -1;
         }
-        s->last_filter = false;
         const uint32_t *hi = reinterpret_cast<const uint32_t *>(s->h_res);
         const float *hs = reinterpret_cast<const float *>(s->h_res + rbytes);
         if (ke == k) {
@@ -1121,12 +1136,7 @@ static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const St
     const size_t kbytes = (size_t)Q * ke * 8;
     for (NkShard *s : live) {
         NK_CUDA_OK(cudaSetDevice(s->device));
-        if (s->h_keys_bytes < kbytes) {
-            if (s->h_keys) cudaFreeHost(s->h_keys);
-            s->h_keys = nullptr; s->h_keys_bytes = 0;
-            NK_CUDA_OK(cudaMallocHost((void **)&s->h_keys, kbytes + kbytes / 4));
-            s->h_keys_bytes = kbytes + kbytes / 4;
-        }
+        if (pinned_reserve((void **)&s->h_keys, &s->h_keys_bytes, kbytes)) return -1;
     }
     for (NkShard *s : live) {
         NK_CUDA_OK(cudaSetDevice(s->device));
@@ -1150,10 +1160,7 @@ static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const St
         std::partial_sort(tmp.begin(), tmp.begin() + take, tmp.begin() + m, std::greater<uint64_t>());
         for (uint32_t i = 0; i < ke; ++i) {
             if (i < take) {
-                float sc = nk::key_score(tmp[i]);
-                if (ix->metric == NK_METRIC_EUCLIDEAN) sc = sqrtf(std::max(-sc, 0.0f));
-                out_idx[(size_t)q * k + i] = nk::key_row(tmp[i]);
-                out_score[(size_t)q * k + i] = sc;
+                decode_key(ix->metric, tmp[i], out_idx + (size_t)q * k + i, out_score + (size_t)q * k + i);
             } else {
                 out_idx[(size_t)q * k + i] = 0xffffffffu;
                 out_score[(size_t)q * k + i] = 0.0f;
@@ -1182,9 +1189,7 @@ static int search_host(NkIndex *ix, const float *queries_host, const NkFilter *f
     ShardOrder order(ix);
     if (order.failed()) return -1;
 
-    std::vector<NkShard *> live;
-    for (auto &s : ix->shards)
-        if (s.n) live.push_back(&s);
+    const std::vector<NkShard *> live = live_shards(ix);
     const StageQueries upload = [&](NkShard &s) {
         NK_CUDA_OK(cudaMemcpyAsync(s.ws.queries, queries_host, qbytes, cudaMemcpyHostToDevice, s.stream));
         ix->stats.bytes_h2d += qbytes;
@@ -1233,19 +1238,12 @@ int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t 
     ShardOrder order(ix);
     if (order.failed()) return -1;
 
-    std::vector<NkShard *> live;
-    for (auto &s : ix->shards)
-        if (s.n) live.push_back(&s);
+    const std::vector<NkShard *> live = live_shards(ix);
     const size_t rb = (size_t)ix->dim * sizeof(float);
     const uint32_t QB = std::min(Q, SEARCH_ROWS_BLOCK);
     std::vector<uint32_t> bidx((size_t)QB * kk), local(QB), pos(QB);
     std::vector<float> bsc((size_t)QB * kk);
-    if (live.size() > 1 && ix->h_qrows_bytes < 2 * QB * rb) {
-        if (ix->h_qrows) cudaFreeHost(ix->h_qrows);
-        ix->h_qrows = nullptr; ix->h_qrows_bytes = 0;
-        NK_CUDA_OK(cudaMallocHost((void **)&ix->h_qrows, 2 * QB * rb));
-        ix->h_qrows_bytes = 2 * QB * rb;
-    }
+    if (live.size() > 1 && pinned_reserve((void **)&ix->h_qrows, &ix->h_qrows_bytes, 2 * QB * rb)) return -1;
     for (uint32_t b = 0; b < Q; b += QB) {
         const uint32_t nb = std::min(QB, Q - b);
         const uint32_t *ids = rows_host + b;
@@ -1349,9 +1347,7 @@ int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresho
     struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
     ShardOrder order(ix);
     if (order.failed()) return -1;
-    std::vector<NkShard *> live;
-    for (auto &s : ix->shards)
-        if (s.n) live.push_back(&s);
+    const std::vector<NkShard *> live = live_shards(ix);
     const size_t qbytes = (size_t)Q * ix->dim * sizeof(float);
     std::vector<std::vector<int>> counts(live.size(), std::vector<int>(Q, 0));
     std::vector<uint32_t> list_cap(live.size());
@@ -1361,65 +1357,22 @@ int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresho
         if (nk::ws_reserve((void **)&s.ws.queries, &s.ws.queries_bytes, qbytes)) return -1;
         NK_CUDA_OK(cudaMemcpyAsync(s.ws.queries, queries_host, qbytes, cudaMemcpyHostToDevice, s.stream));
         ix->stats.bytes_h2d += qbytes;
-        nk::ScanArgs a;
-        a.rows = s.rows; a.dtype = ix->dtype; a.n = (uint32_t)s.n; a.dim = ix->dim; a.row_base = s.base;
-        a.queries = s.ws.queries; a.Q = Q; a.k = 1; a.metric = ix->metric; a.stream = s.stream;
-        a.row_mask = s.mask_on ? s.mask : nullptr; a.min_score = ix->key_floor();
-        if (filters_host) {
-            const size_t fbytes = (size_t)Q * sizeof(NkFilter);
-            if (shard_tags_on(s)) return -1;
-            if (nk::ws_reserve((void **)&s.ws.qfilter, &s.ws.qfilter_bytes, fbytes)) return -1;
-            NK_CUDA_OK(cudaMemcpyAsync(s.ws.qfilter, filters_host, fbytes, cudaMemcpyHostToDevice, s.stream));
-            ix->stats.bytes_h2d += fbytes;
-            a.row_tags = s.tags; a.qfilter = s.ws.qfilter;
-        }
-        // Paths: the 16-bit and TF32 filters with fixed thresholds, or the CUDA-core scan; AUTO picks as nk_search does (the
-        // exact 3xTF32 scan has no range mode).
-        const nk::ScanArgs as = with_16bit_image(ix, s, a);
-        const bool filter_ok = ix->dtype == NK_DTYPE_F32 && nk::scan_tensor_filter_supported(s.di, a);
-        const bool shadow_ok = as.shadow != nullptr && nk::shadow_pass_supported(s.di, as) && nk::scan_tensor_filter_supported(s.di, as);
-        int use = NK_PATH_SIMT;
-        if (ix->path == NK_PATH_TENSOR) {
-            nk::set_error("nk_search_range: the exact 3xTF32 path has no range mode (use AUTO, SIMT, TENSOR_FILTER or TENSOR_SHADOW)");
-            return -1;
-        } else if (ix->path == NK_PATH_TENSOR_FILTER || ix->path == NK_PATH_TENSOR_SHADOW) {
-            if (!(ix->path == NK_PATH_TENSOR_FILTER ? filter_ok : shadow_ok)) {
-                nk::set_error("tensor path %d does not support this shape (dim=%u dtype=%d metric=%d shadow=%d)", ix->path, ix->dim, ix->dtype,
-                              ix->metric, (int)(as.shadow != nullptr));
-                return -1;
-            }
-            use = ix->path;
-        } else if (ix->path == NK_PATH_AUTO) {
-            const bool big_shard = (uint64_t)s.n * ix->dim * 4 >= (64ull << 20);
-            if (Q >= 5) use = shadow_ok ? NK_PATH_TENSOR_SHADOW : filter_ok ? NK_PATH_TENSOR_FILTER : NK_PATH_SIMT;
-            else if (shadow_ok && big_shard && ix->dtype == NK_DTYPE_F32) use = NK_PATH_TENSOR_SHADOW;
-        }
-        cudaEvent_t e0 = nullptr, e1 = nullptr;
-        uint64_t main_launches = 0;
-        nk::ScanArgs b = use == NK_PATH_TENSOR_SHADOW ? as : a;
-        if (ix->timing_on) {
-            NK_CUDA_OK(cudaEventCreate(&e0));
-            NK_CUDA_OK(cudaEventCreate(&e1));
-            b.ev_begin = e0; b.ev_end = e1; b.main_launches = &main_launches;
-        }
+        const NkFilter *qfilter = nullptr;
+        if (filters_host && !(qfilter = stage_filters(ix, s, filters_host, Q))) return -1;
+        // Paths: the 16-bit and TF32 filters with fixed thresholds, or the CUDA-core scan.
+        nk::ScanArgs a = shard_scan_args(ix, s, s.ws.queries, Q, 1, s.stream, qfilter);
+        const int use = plan_path(ix, s, true, &a);
+        if (use < 0) return -1;
+        ScanTimer timer(s);
+        if (timer.attach(ix, &a)) return -1;
         int retried = 0;
-        const int rc = nk::range_scan_shard(s.di, b, use != NK_PATH_SIMT, thr.data(), s.ws, &ix->stats.kernel_launches, counts[i].data(),
-                                            &list_cap[i], &retried);
-        if (ix->timing_on) {
-            if (rc == 0 && main_launches) {
-                s.timing.emplace_back(e0, e1);
-                s.timing_launches.push_back(main_launches);
-            } else {
-                cudaEventDestroy(e0);
-                cudaEventDestroy(e1);
-            }
-        }
-        if (rc) return -1;
+        if (nk::range_scan_shard(s.di, a, use != NK_PATH_SIMT, thr.data(), s.ws, &ix->stats.kernel_launches, counts[i].data(), &list_cap[i],
+                                 &retried))
+            return -1;
+        timer.keep();
         s.last_filter = false;
         ix->last_path = use;
-        const uint64_t passes = (uint64_t)(retried ? 2 : 1) * (use == NK_PATH_SIMT ? (Q + 7) / 8 : (Q + 127) / 128);
-        ix->stats.bytes_scanned += passes * s.n * (use == NK_PATH_TENSOR_SHADOW ? (ix->dtype == NK_DTYPE_F32 ? ix->dimpad() : ix->dim) * 2
-                                                                                 : ix->dim * ix->esz());
+        ix->stats.bytes_scanned += scan_bytes(ix, use, a, retried ? 2 : 1);
     }
     // offsets: the shards' survivors of query q are merged into one run
     for (uint32_t q = 0; q < Q; ++q) {
@@ -1449,12 +1402,7 @@ int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresho
             merged.swap(tmp);
         }
         const uint64_t o = out_offsets[q];
-        for (size_t j = 0; j < merged.size(); ++j) {
-            float sc = nk::key_score(merged[j]);
-            if (ix->metric == NK_METRIC_EUCLIDEAN) sc = sqrtf(std::max(-sc, 0.0f));
-            out_idx[o + j] = nk::key_row(merged[j]);
-            out_score[o + j] = sc;
-        }
+        for (size_t j = 0; j < merged.size(); ++j) decode_key(ix->metric, merged[j], out_idx + o + j, out_score + o + j);
     }
     return 0;
 }
@@ -1550,12 +1498,13 @@ int nk_index_status(NkIndex *ix, void *stream) {
         int h = 0;
         NK_CUDA_OK(cudaMemcpy(&h, s.ws.flags, sizeof(int), cudaMemcpyDeviceToHost));
         if (h) {
+            // cleared synchronously: this call holds no ShardOrder, so a clear queued on a stream would not be ordered
+            // before the index's next call
             NK_CUDA_OK(cudaMemset(s.ws.flags, 0, sizeof(int)));
             bad = h;
         }
     }
-    if (bad) { nk::set_error("internal: candidate buffer overflow (flag=%d)", bad); return -1; }
-    return 0;
+    return bad ? nk::fatal_overflow(bad, nullptr, nullptr) : 0;
 }
 
 // (No scratch buffer: the merge kernel writes the decoded arrays itself, so concurrent merges on different streams share
@@ -1614,15 +1563,17 @@ int nk_score_subset(NkIndex *ix, const float *query_host, const uint32_t *rows_h
         if (nk::ws_reserve((void **)&s->ws.out_idx, &s->ws.out_idx_bytes, (size_t)ke * 4)) { rc = -1; break; }
         if (nk::ws_reserve((void **)&s->ws.out_score, &s->ws.out_score_bytes, (size_t)ke * 4)) { rc = -1; break; }
         if (cudaMemcpyAsync(s->ws.queries, query_host, (size_t)ix->dim * 4, cudaMemcpyHostToDevice, s->stream) != cudaSuccess) { rc = -1; break; }
+        // the gathered rows, positions 0..n_subset-1: no row mask, score floor or tags
         nk::ScanArgs a;
         a.rows = d_gather; a.dtype = ix->dtype; a.n = n_subset; a.dim = ix->dim; a.row_base = 0;
         a.queries = s->ws.queries; a.Q = 1; a.k = ke; a.metric = ix->metric; a.stream = s->stream;
         if (ke > NK_MAX_K) {  // ScoreSubset ranks every candidate (up to MaxCandidates = 5000, vector_pipeline.go:24-31)
-            if (run_scan_bigk(ix, *s, s->ws.queries, 1, ke, s->ws.keys, s->stream, d_gather, n_subset, true)) { rc = -1; break; }
+            if (run_scan_bigk(ix, *s, a, s->ws.keys)) { rc = -1; break; }
             if (nk::decode_keys(s->ws.keys, 1, ke, ix->metric, s->ws.out_idx, s->ws.out_score, s->stream)) { rc = -1; break; }
         } else {
             a.out_idx = s->ws.out_idx; a.out_score = s->ws.out_score;  // decoded by the merge launch
             if (nk::scan_simt(s->di, a, s->ws, s->ws.keys, &ix->stats.kernel_launches)) { rc = -1; break; }
+            ix->stats.bytes_scanned += scan_bytes(ix, NK_PATH_SIMT, a, 1);
         }
         if (cudaMemcpyAsync(pos.data(), s->ws.out_idx, (size_t)ke * 4, cudaMemcpyDeviceToHost, s->stream) != cudaSuccess) { rc = -1; break; }
         if (cudaMemcpyAsync(out_score, s->ws.out_score, (size_t)ke * 4, cudaMemcpyDeviceToHost, s->stream) != cudaSuccess) { rc = -1; break; }
@@ -1794,9 +1745,9 @@ int nk_search_groups(NkIndex *ix, const float *query_host, uint32_t k, uint32_t 
     nk::DeviceGuard _restore_device;
     NkShard *s;
     if (single_shard(ix, &s)) return -1;
+    std::lock_guard<std::mutex> lk(ix->mu);
     if (k == 0 || s->n == 0) return 0;
     if (!query_host || !out_group || !out_row || !out_score) { nk::set_error("null argument"); return -1; }
-    std::lock_guard<std::mutex> lk(ix->mu);
     if (!s->group_on || ix->n_groups == 0) { nk::set_error("nk_search_groups: no row groups set (nk_index_set_row_groups)"); return -1; }
     const uint32_t G = ix->n_groups, ke = k < G ? k : G;
     if (ke > NK_MAX_K) { nk::set_error("nk_search_groups: k=%u exceeds NK_MAX_K=%u", ke, NK_MAX_K); return -1; }

@@ -1,5 +1,7 @@
 // kernels.cuh — internal launcher interface between the C-ABI host code and the kernels.
 #pragma once
+#include <vector>
+
 #include "common.cuh"
 
 namespace nk {
@@ -89,6 +91,30 @@ struct ScanArgs {
 // Writes per-query sorted candidate keys [Q][k] to out_keys (device).
 int scan_simt(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *out_keys, uint64_t *launches);
 
+// Tensor-core scans (scan_tensor.cu, scan_tensor_shadow.cu): the exact 3xTF32 scan, and the filter (TF32 over fp32 rows, or
+// the 16-bit pass over a.shadow) with exact re-scoring.  scan_tensor_filter_tail queues the retry / exact stages a deferred
+// (a.defer_tail) filter search skipped.
+int scan_tensor(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *out_keys, uint64_t *launches);
+bool scan_tensor_supported(const DeviceInfo &di, const ScanArgs &a);
+int scan_tensor_filter(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *out_keys, uint64_t *launches);
+int scan_tensor_filter_tail(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *out_keys, uint64_t *launches);
+bool scan_tensor_filter_supported(const DeviceInfo &di, const ScanArgs &a);
+bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a);
+// Tests only: the filters' score estimates and error bounds for every (row, query) pair (nk_debug_filter_dump).
+int scan_filter_dump(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, int which, float *est, float *bnd, uint32_t ld, uint64_t *launches);
+// fp32 rows [first, first+count) -> bf16 shadow rows (stride dimpad) + |x|^2, |x - bf16(x)|^2
+int build_shadow(const float *rows, uint64_t first, uint64_t count, uint32_t dim, uint32_t dimpad, void *shadow, float *xnorm2,
+                 float *dnorm2, cudaStream_t stream);
+// k-means assignment as one pass of the 16-bit scan with an argmax epilogue (assign_tensor.cu).
+bool assign_tensor_supported(const DeviceInfo &di, uint32_t dim, uint32_t K, int metric);
+int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, uint32_t dimpad, const float *xnorm2, const float *dnorm2,
+                  uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric, uint32_t *assign_dev, cudaStream_t stream,
+                  uint64_t *launches, void **scratch, size_t *scratch_bytes);
+
+// A shard's fatal status word (FLAG_FATAL) held `flag`: clear the word on `stream` (flags == nullptr: the caller has cleared
+// it), set the error message and return -1.
+int fatal_overflow(int flag, int *flags, cudaStream_t stream);
+
 // Range search (nk_search_range, range.cu).  State in the shard workspace: ws.keys2 = [range_qa(Q)] order-preserving bits of
 // every query's key-space threshold (score floor included), then [range_qa(Q)] list fills; ws.partial = the lists
 // [Q][list_cap].  A fill counts every survivor, also those past list_cap.  range_qa mirrors the filter's padded per-query
@@ -98,6 +124,13 @@ inline uint32_t range_qa(uint32_t Q) { return (Q + 63) / 64 * 64 + 256; }
 int scan_tensor_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint32_t list_cap, uint64_t *launches);
 // CUDA-core scan: lists hold every pair whose exact score reaches the threshold.
 int scan_simt_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint32_t list_cap, uint64_t *launches);
+// One shard's scan (tensor: the filter, else the CUDA-core scan) and exact re-scoring: survivors per query -> counts[Q] (host);
+// *list_cap = the list capacity the lists were filled with; *retried = 1 if the scan ran twice.
+int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const uint32_t *thr_bits, Workspace &ws, uint64_t *launches,
+                     int *counts, uint32_t *list_cap, int *retried);
+// After range_scan_shard: the shard's survivors, CSR by counts[Q], each query's run sorted -> *keys (host).
+int range_sorted_keys(const DeviceInfo &di, Workspace &ws, cudaStream_t stream, uint32_t Q, const int *counts, uint32_t list_cap,
+                      std::vector<uint64_t> *keys, uint64_t *launches);
 
 // Merge n_lists sorted (or unsorted) key lists per query into the best k, sorted descending.
 // key(list l, query q, slot i) = keys[l*list_stride + q*q_stride + i], i < list_len (0 = k).

@@ -178,11 +178,7 @@ int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const
         NK_CUDA_OK(cudaMemcpyAsync(fill.data(), ws_fill(ws, Q), (size_t)Q * 4, cudaMemcpyDeviceToHost, a.stream));
         NK_CUDA_OK(cudaMemcpyAsync(&fatal, ws.flags + FLAG_FATAL, 4, cudaMemcpyDeviceToHost, a.stream));
         NK_CUDA_OK(cudaStreamSynchronize(a.stream));
-        if (fatal) {
-            cudaMemsetAsync(ws.flags, 0, sizeof(int), a.stream);
-            set_error("internal: candidate buffer overflow (flag=%d)", fatal);
-            return -1;
-        }
+        if (fatal) return fatal_overflow(fatal, ws.flags, a.stream);
         int longest = 0;
         for (int f : fill) {
             if (f < 0) { set_error("nk_search_range: more than 2^31 survivors for one query"); return -1; }

@@ -44,6 +44,12 @@ void clear_error() {
     g_last[0] = 0;
 }
 
+int fatal_overflow(int flag, int *flags, cudaStream_t stream) {
+    if (flags) cudaMemsetAsync(flags, 0, sizeof(int), stream);
+    set_error("internal: candidate buffer overflow (flag=%d)", flag);
+    return -1;
+}
+
 int query_device_info(int device_id, DeviceInfo *out) {
     cudaDeviceProp prop;
     NK_CUDA_OK(cudaGetDeviceProperties(&prop, device_id));

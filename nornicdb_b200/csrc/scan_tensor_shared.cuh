@@ -418,7 +418,6 @@ struct ShadowPassArgs : tc::PassArgs {
     const float *qa, *qb;
 };
 int launch_shadow_pass(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches);
-bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a);
 
 // Query preparation (filter_prep_kernel, scan_tensor.cu), one CTA per padded query row.
 struct PrepParams {
@@ -446,8 +445,5 @@ struct PrepParams {
 // The fields taken from the search arguments: the queries, the metric and the shard (for the sample).
 PrepParams prep_params(const ScanArgs &a, uint32_t Qpad, uint32_t dimpad);
 int launch_prep(const DeviceInfo &di, const PrepParams &pp, cudaStream_t stream, uint64_t *launches);
-// fp32 rows [first, first+count) -> bf16 shadow rows (stride dimpad) + |x|^2, |x - bf16(x)|^2
-int build_shadow(const float *rows, uint64_t first, uint64_t count, uint32_t dim, uint32_t dimpad, void *shadow, float *xnorm2,
-                 float *dnorm2, cudaStream_t stream);
 
 }  // namespace nk

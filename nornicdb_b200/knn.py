@@ -205,14 +205,19 @@ class KnnIndex:
         return {name: int(getattr(st, name)) for name, _ in st._fields_}
 
     # -- search ------------------------------------------------------------------------------------
-    def search(self, queries, k: int) -> Tuple[np.ndarray, np.ndarray]:
-        """queries [Q x dim] fp32 host -> (idx [Q x k'] uint32, score [Q x k'] fp32), k' = min(k, N).
-        Euclidean scores are distances (ascending); cosine / dot are similarities (descending)."""
+    def _queries(self, queries) -> np.ndarray:
+        """queries [Q x dim] (or one [dim] vector) -> contiguous fp32 [Q x dim]."""
         q = np.ascontiguousarray(np.asarray(queries, dtype=np.float32))
         if q.ndim == 1:
             q = q.reshape(1, -1)
         if q.shape[1] != self.dim:
             raise KnnError(f"invalid dimensions: query has {q.shape[1]}, index has {self.dim}")  # gpu.go:1533-1535
+        return q
+
+    def search(self, queries, k: int) -> Tuple[np.ndarray, np.ndarray]:
+        """queries [Q x dim] fp32 host -> (idx [Q x k'] uint32, score [Q x k'] fp32), k' = min(k, N).
+        Euclidean scores are distances (ascending); cosine / dot are similarities (descending)."""
+        q = self._queries(queries)
         Q = q.shape[0]
         k = int(k)
         if k <= 0 or Q == 0:
@@ -256,11 +261,7 @@ class KnnIndex:
     def search_filtered(self, queries, k: int, filters) -> Tuple[np.ndarray, np.ndarray]:
         """search() with one tag filter per query: filters [Q x 3] uint64 (all_of, none_of, any_of), None = no filter.
         Slots beyond a query's admissible rows hold index 0xffffffff and score 0."""
-        q = np.ascontiguousarray(np.asarray(queries, dtype=np.float32))
-        if q.ndim == 1:
-            q = q.reshape(1, -1)
-        if q.shape[1] != self.dim:
-            raise KnnError(f"invalid dimensions: query has {q.shape[1]}, index has {self.dim}")
+        q = self._queries(queries)
         Q = q.shape[0]
         f = None if filters is None else as_filters(filters, Q)
         k = int(k)
@@ -276,11 +277,7 @@ class KnnIndex:
         """Every admissible row whose score reaches the query's threshold (cosine / dot: minimum score; euclidean: maximum
         distance), one threshold per query (a scalar applies to all).  Returns one (idx uint32, score float32) pair per query,
         in search()'s order.  The result buffer grows to the size the library reports (nk_search_range's size protocol)."""
-        q = np.ascontiguousarray(np.asarray(queries, dtype=np.float32))
-        if q.ndim == 1:
-            q = q.reshape(1, -1)
-        if q.shape[1] != self.dim:
-            raise KnnError(f"invalid dimensions: query has {q.shape[1]}, index has {self.dim}")
+        q = self._queries(queries)
         Q = q.shape[0]
         t = np.ascontiguousarray(np.broadcast_to(np.asarray(thresholds, dtype=np.float32), (Q,)))
         f = None if filters is None else as_filters(filters, Q)

@@ -194,7 +194,9 @@ def test_score_subset(knn_lib, kats, oracle_mod):
     subset = np.random.default_rng(3).choice(5000, 700, replace=False).astype(np.uint32)
     ix = KnnIndex(96)
     ix.upload(rows)
+    before = ix.stats()["bytes_scanned"]
     gi, gs = ix.score_subset(q, subset)
+    assert ix.stats()["bytes_scanned"] - before == 700 * 96 * 4  # the subset rows, one CUDA-core pass
     ix.release()
     ex = oracle_mod.scores_exact64(rows[subset], q, "cosine")
     order = np.argsort(-ex, kind="stable")
@@ -283,7 +285,9 @@ def test_score_subset_large(knn_lib, oracle_mod):
     subset = np.random.default_rng(4).choice(8000, 3000, replace=False).astype(np.uint32)
     ix = KnnIndex(64)
     ix.upload(rows)
+    before = ix.stats()["bytes_scanned"]
     gi, gs = ix.score_subset(q, subset)  # ranks all 3000 candidates (> NK_MAX_K)
+    assert ix.stats()["bytes_scanned"] - before == 3 * 3000 * 64 * 4  # the subset rows, once per NK_MAX_K pass
     ix.release()
     ex = oracle_mod.scores_exact64(rows[subset], q, "cosine")
     order = np.argsort(-ex, kind="stable")
