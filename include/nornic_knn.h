@@ -97,7 +97,8 @@ enum { NK_DTYPE_F32 = 0, NK_DTYPE_F16 = 1, NK_DTYPE_BF16 = 2 };
 enum { NK_PATH_AUTO = 0, NK_PATH_SIMT = 1, NK_PATH_TENSOR = 2, NK_PATH_TENSOR_FILTER = 3, NK_PATH_TENSOR_SHADOW = 4 };
 
 /* k up to NK_MAX_K is one fused pass; larger k (the reference accepts any k) is served by ceil(k/NK_MAX_K) passes
- * of the CUDA-core scan, up to NK_MAX_K_TOTAL results per query. */
+ * of the CUDA-core scan, up to NK_MAX_K_TOTAL results per query.  Merging candidate lists (nk_merge_keys_device,
+ * nk_comm_exchange_merge, nk_search_sharded_device) is limited to k <= NK_MAX_K. */
 #define NK_MAX_K 1024u
 #define NK_MAX_K_TOTAL 65536u
 
@@ -292,13 +293,15 @@ int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresho
 
 /* Multi-process sharding (one rank per GPU): emit this shard's sorted candidate list as packed 64-bit
  * keys [Q x k] (order-preserving score bits << 32 | ~row index; larger key = better), to be exchanged
- * (e.g. ncclAllGather of Q*k*8 bytes per rank) and merged with nk_merge_keys_device. */
+ * (e.g. ncclAllGather of Q*k*8 bytes per rank) and merged with nk_merge_keys_device.  k <= NK_MAX_K_TOTAL: one shard's
+ * keys are useful on their own, but only lists of k <= NK_MAX_K can be merged. */
 int nk_search_keys_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uint32_t k, uint64_t *out_keys_dev,
                           void *stream);
 /* Merge n_lists candidate lists laid out [n_lists][Q][k] into final [Q x k] idx/score on the current
  * device of `device_id`.  metric selects the score decoding (euclidean: distance).  With a stream the call is
  * asynchronous on it (the searches that produced the keys must be ordered before it on that stream); with
- * stream == NULL it synchronises the device first and returns after the merge has completed. */
+ * stream == NULL it synchronises the device first and returns after the merge has completed.  k > NK_MAX_K (the merge
+ * width) returns -1 before any work. */
 int nk_merge_keys_device(int device_id, const uint64_t *keys_dev, uint32_t n_lists, uint32_t Q, uint32_t k,
                          int metric, uint32_t *out_idx_dev, float *out_score_dev, void *stream);
 
@@ -320,7 +323,9 @@ int nk_search_groups(NkIndex *ix, const float *query_host, uint32_t k, uint32_t 
  *   (the host exchanges the world handles by any transport);  nk_comm_connect(c, all_handles = world x 64 B in rank order);
  *   nk_search_sharded_device(ix, c, queries_dev, Q, k, out_idx_dev, out_score_dev, stream)  on every rank, same sequence.
  * Ranks living in ONE process (several single-device indexes) use nk_comm_connect_local instead of export / connect.
- * nk_comm_status synchronises the stream and reports a peer that never arrived (the device-side wait is bounded: 2 s). */
+ * nk_comm_status synchronises the stream and reports a peer that never arrived (the device-side wait is bounded: 2 s).
+ * k <= NK_MAX_K (the merge width): a larger k returns -1 before the scan, before the exchange epoch advances and before
+ * anything is written to a peer, so every rank's next call works as if the failed one had never been made. */
 NkComm *nk_comm_create(int device_id, int rank, int world, size_t slot_bytes);
 int nk_comm_export(NkComm *c, void *handle_out);
 int nk_comm_connect(NkComm *c, const void *handles);

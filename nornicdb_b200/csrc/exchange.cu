@@ -174,6 +174,8 @@ int nk_comm_exchange_merge(NkComm *c, const uint64_t *keys_dev, uint32_t Q, uint
     if (!c || !keys_dev || !out_idx_dev || !out_score_dev) { nk::set_error("null argument"); return -1; }
     if (!c->connected) { nk::set_error("exchange: communicator is not connected"); return -1; }
     if (Q == 0 || k == 0) return 0;
+    // refused before the epoch advances and anything reaches a peer: a failed call leaves every rank's buffers untouched
+    if (k > NK_MAX_K) { nk::set_error("exchange: k=%u exceeds NK_MAX_K=%u (the merge width)", k, NK_MAX_K); return -1; }
     const size_t bytes = (size_t)Q * k * 8;
     if (bytes > c->slot_bytes) { nk::set_error("exchange: Q*k*8 = %zu bytes exceeds the slot size %zu", bytes, c->slot_bytes); return -1; }
     NK_CUDA_OK(cudaSetDevice(c->device));

@@ -1513,6 +1513,7 @@ int nk_merge_keys_device(int device_id, const uint64_t *keys_dev, uint32_t n_lis
                          uint32_t *out_idx_dev, float *out_score_dev, void *stream) {
     nk::DeviceGuard _restore_device;
     if (k == 0 || Q == 0 || n_lists == 0) return 0;
+    if (k > NK_MAX_K) { nk::set_error("nk_merge_keys_device: k=%u exceeds NK_MAX_K=%u (the merge width)", k, NK_MAX_K); return -1; }
     if (!keys_dev || !out_idx_dev || !out_score_dev) { nk::set_error("null argument"); return -1; }
     if (device_id < 0 || device_id >= 64) { nk::set_error("bad device id %d", device_id); return -1; }
     NK_CUDA_OK(cudaSetDevice(device_id));
@@ -1793,6 +1794,8 @@ int nk_search_sharded_device(NkIndex *ix, NkComm *comm, const float *queries_dev
     if (single_shard(ix, &s)) return -1;
     if (!comm) { nk::set_error("null communicator"); return -1; }
     if (k == 0 || Q == 0) return 0;
+    // refused before the scan: the exchange could not merge the lists
+    if (k > NK_MAX_K) { nk::set_error("nk_search_sharded_device: k=%u exceeds NK_MAX_K=%u (the merge width)", k, NK_MAX_K); return -1; }
     const cudaStream_t st = stream ? (cudaStream_t)stream : s->stream;
     // one call in the shard's order: the exchange reads the keys from the shard's workspace, which the next call may reuse
     std::lock_guard<std::mutex> lk(ix->mu);

@@ -228,12 +228,16 @@ def test_shadow_follows_incremental_updates(knn_lib, oracle_mod):
 
 def test_auto_dispatch(knn_lib, oracle_mod):
     from nornicdb_b200.knn import KnnIndex
+    rows = oracle_mod.fill_uniform(2000, 128, 1)
     ix = KnnIndex(128, metric="cosine")
-    ix.upload(oracle_mod.fill_uniform(2000, 128, 1))
+    ix.upload(rows)
     ix.search(oracle_mod.fill_uniform(4, 128, 2), 5)
     assert ix.last_path() == "simt"       # Q <= 4: CUDA-core scan
     ix.search(oracle_mod.fill_uniform(40, 128, 2), 5)
     assert ix.last_path() == "shadow"     # Q >= 5: tensor cores over the BF16 shadow
-    ix.search(oracle_mod.fill_uniform(40, 128, 2), 500)
+    q = oracle_mod.fill_uniform(40, 128, 2)
+    gi, gs = ix.search(q, 500)
     assert ix.last_path() == "simt"       # k beyond the tensor paths
     ix.release()
+    oi, os_ = oracle_mod.knn_exact64(rows, q, 500, "cosine")
+    check_parity(rows, q, 500, "cosine", gi, gs, oi, os_)
