@@ -15,7 +15,7 @@
 //
 // Both operands are plain bf16 tiles in shared memory, so there is no conversion stage; the accumulators live in the
 // registers of the warpgroups that issue the MMAs and score them.
-//   warp 0      TMA: shadow slabs [256 rows x 64 bf16] (32 KB, 128B-swizzled), 5-stage ring;
+//   warp 0      TMA: shadow slabs [256 rows x 64 bf16] (32 KB, 128B-swizzled), 6-stage ring at QT = 64, 5 at QT = 128;
 //   warp 3      TMA: query slabs [QT x 64 bf16] (8 / 16 KB), L2-resident;
 //   warps 4-11  two consumer warpgroups, one per 128-row M-tile: per slab 2 x 4 wgmma.m64nQTk16 (A and B from smem,
 //               fp32 accumulators in registers), then per tile: bound / compare / push straight
@@ -41,7 +41,7 @@ using namespace tc;
 constexpr int NTHREADS = 384;
 constexpr int QT_MAX = 128;
 constexpr int BKB = 64;                   // bf16 per row per slab = one 128-byte swizzle row
-constexpr int ASTAGES = 5;                // HBM look-ahead while the consumers run a tile's epilogue
+constexpr int ASTAGES_MAX = 6;            // deepest shadow-slab ring (Cfg<QT>::ASTAGES)
 constexpr int A_BYTES = ROWS * 128;       // 32 KB
 constexpr int EPI_WARP0 = 4, EPI_WARPS = 8, EPI_NT = EPI_WARPS * 32;
 // Registers (setmaxnreg): the TMA warpgroup gives its share to the consumers for the scan (128 x 24 + 256 x 240 = the
@@ -53,14 +53,21 @@ constexpr int REG_BAR = 2;                // consumers arrive after releasing th
 constexpr int PB = tc::P_SHADOW;          // candidate buffer slots per (CTA, query)
 constexpr int PRUNE_LANE = PB / 32;       // keys per lane of a warp prune
 
+// The shadow-slab ring is the HBM look-ahead that keeps loads in flight while the consumers run a tile's epilogue (every
+// stage it holds is ~1.3 us of one SM's share of HBM time at the headline shape; the epilogue takes longer than the ring
+// covers).  The query-slab ring reads L2-resident data and only has to stay ahead of the consumers' pace: at QT = 64 three
+// stages suffice, and the 24 KB this frees from six buys a sixth shadow stage.  QT = 128 (16 KB query slabs) has no room
+// for one: 5 x 32 KB + 3 x 16 KB is already the shared-memory budget.
 template <int QT> struct Cfg {
     static constexpr int B_BYTES = QT * 128;
-    static constexpr int BSTAGES = (48 * 1024) / B_BYTES > MAX_BSTAGES ? MAX_BSTAGES : (48 * 1024) / B_BYTES;  // L2-resident: a short ring
+    static constexpr int ASTAGES = QT == 64 ? 6 : 5;
+    static constexpr int BSTAGES = QT == 64 ? 3 : (48 * 1024) / B_BYTES;
     static constexpr int RING_BYTES = ASTAGES * A_BYTES + BSTAGES * B_BYTES;
+    static_assert(ASTAGES <= ASTAGES_MAX && BSTAGES <= MAX_BSTAGES, "ring deeper than its barriers");
 };
 
 struct __align__(8) Shared {
-    Rings<ASTAGES> ring;
+    Rings<ASTAGES_MAX> ring;                       // (QT = 128 leaves the last stage's barriers unused)
     unsigned int maxxx, max_ra, max_rb;            // running maxima (float bits) of |x|^2 and the per-row bound factors
     float tau[QT_MAX];
     float qn[QT_MAX];                              // |q| (1 for cosine)
@@ -155,7 +162,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
     extern __shared__ unsigned char smem_dyn[];
     unsigned char *smem_raw = smem_dyn + ((1024u - (ptx::smem_u32(smem_dyn) & 1023u)) & 1023u);
     unsigned char *a_base = smem_raw;
-    unsigned char *b_base = smem_raw + (size_t)ASTAGES * A_BYTES;
+    unsigned char *b_base = smem_raw + (size_t)C::ASTAGES * A_BYTES;
     Shared &sh = *reinterpret_cast<Shared *>(smem_raw + (size_t)C::RING_BYTES);
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -203,7 +210,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
         ptx::setmaxnreg_dec<PRODUCER_REGS>();
         if (warp == 0) {
             // ===================================== TMA producer: shadow slabs =========================
-            tma_producer<ASTAGES>(sh.ring.aempty, sub, num_tiles, sgrid, 1, nslab, false, [&](uint32_t s, uint32_t tile, uint32_t, uint32_t j) {
+            tma_producer<C::ASTAGES>(sh.ring.aempty, sub, num_tiles, sgrid, 1, nslab, false, [&](uint32_t s, uint32_t tile, uint32_t, uint32_t j) {
                 ptx::mbar_arrive_expect_tx(&sh.ring.afull[s], A_BYTES);
                 ptx::tma_load_2d(&map_rows, &sh.ring.afull[s], a_base + (size_t)s * A_BYTES, (int32_t)(j * BKB), (int32_t)(tile * ROWS), qg.a_policy);
             });
@@ -256,9 +263,9 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             const uint32_t gt_pre = !RANGE && etid < nq ? __ldcg(p.gtau + q0 + etid) : 0u;
             uint32_t prev_sa = 0, prev_sb = 0;
             for (uint32_t j = 0; j < nslab; ++j, ++g) {
-                const uint32_t sa = g % ASTAGES, sbq = g % C::BSTAGES;
+                const uint32_t sa = g % C::ASTAGES, sbq = g % C::BSTAGES;
                 ptx::mbar_wait(&sh.ring.bfull[sbq], (g / C::BSTAGES) & 1);
-                ptx::mbar_wait(&sh.ring.afull[sa], (g / ASTAGES) & 1);
+                ptx::mbar_wait(&sh.ring.afull[sa], (g / C::ASTAGES) & 1);
                 const uint64_t bdesc = ptx::make_smem_desc_sw128(ptx::smem_u32(b_base + (size_t)sbq * C::B_BYTES));
                 const uint32_t abase = ptx::smem_u32(a_base + (size_t)sa * A_BYTES + (size_t)m * (A_BYTES / 2));
                 ptx::wgmma_fence();
