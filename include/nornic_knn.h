@@ -291,6 +291,32 @@ int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresho
                     uint32_t Q, uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx, float *out_score,
                     uint64_t *out_total);
 
+/* ---- Similarity self-join ----------------------------------------------------------------------------------------------
+ * Every pair of stored rows whose similarity reaches one threshold (near-duplicate detection, threshold auto-linking of a
+ * graph, MATCH (a),(b) WHERE vector.similarity.cosine(a.e, b.e) >= t), each unordered pair scanned and returned once.
+ * Left rows: the stripe i in [first_row, first_row + n_rows), ids relative to the index's first row as in nk_search_rows;
+ * first_row = 0, n_rows = nk_index_rows(ix) is the whole index.  Left row i gets every row j with a higher global id such that
+ *   - j is admissible: it passes the row mask and `filter` (one NkFilter, NULL = none, the predicate of nk_search_filtered);
+ *   - i itself passes the row mask and `filter` (otherwise i's list is empty);
+ *   - the exact fp32 score of row j against the query "row i as stored, widened to fp32" meets `threshold` with the score
+ *     floor folded in: the arithmetic and threshold of nk_search_range (cosine / dot a minimum score, euclidean a maximum
+ *     distance; a NaN score never qualifies).
+ * So every unordered pair {i, j} appears exactly once when the stripe covers both rows: under the lower id, scored with the
+ * lower row as the query.
+ * Results in CSR layout over the stripe: left row first_row + r owns [out_offsets[r], out_offsets[r+1]) of out_idx (global
+ * row ids) / out_score (euclidean: the distance), out_offsets [n_rows + 1], each list in nk_search's order (score desc /
+ * distance asc, ties by row asc).
+ * Size protocol (nk_search_range's): out_offsets and *out_total are always written and exact; if *out_total > capacity
+ * nothing else is written and the call returns 0.  Returns 0, or -1 with nk_last_error for a NaN threshold, a stripe past
+ * the end, a null pointer with n_rows > 0 or the exact 3xTF32 path forced.  Any number of devices.  Synchronous, and it holds
+ * the index lock throughout, like nk_search_rows.
+ * Costs: the result is staged in host memory during the call, 8 B per pair.  A call that overflows `capacity` has done the
+ * whole join, and the retry does it again: callers of a whole-index job should work in stripes.
+ * Equals, bit for bit, nk_search_range(queries = the stripe's rows read back and widened, thresholds = threshold, filters =
+ * filter for every query) with each list cut to the rows above its own query row, and emptied for inadmissible left rows. */
+int nk_search_pairs(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float threshold, const NkFilter *filter, uint64_t capacity,
+                    uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total);
+
 /* Multi-process sharding (one rank per GPU): emit this shard's sorted candidate list as packed 64-bit
  * keys [Q x k] (order-preserving score bits << 32 | ~row index; larger key = better), to be exchanged
  * (e.g. ncclAllGather of Q*k*8 bytes per rank) and merged with nk_merge_keys_device.  k <= NK_MAX_K_TOTAL: one shard's

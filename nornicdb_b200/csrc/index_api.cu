@@ -1215,6 +1215,81 @@ int nk_search_filtered(NkIndex *ix, const float *queries_host, const NkFilter *f
 // whatever Q is, the whole index included; one host synchronisation per block.
 constexpr uint32_t SEARCH_ROWS_BLOCK = 1024;
 
+// The queries of a block of stored rows ids[nb] (relative to the index's first row), each read and widened to fp32 on the
+// device that holds it.  *stage then writes the block into s.ws.queries (reserved by the caller) of any shard the search runs
+// on.  With one live shard only the ids cross PCIe and the rows are gathered straight into the query block; otherwise each
+// owner gathers its rows now, the block is assembled in pinned host memory and *stage sends it.  admit (nk_search_pairs):
+// *stage also writes the per-query filters into s.ws.qfilter, with the shard's tag array on: *admit for a row that passes the
+// row mask and *admit, the filter that admits no row otherwise, decided on the row's own device.
+static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, const uint32_t *ids, uint32_t nb, const NkFilter *admit,
+                           StageQueries *stage) {
+    const size_t rb = (size_t)ix->dim * sizeof(float);
+    std::vector<uint32_t> local(nb);
+    if (live.size() == 1) {
+        const bool filt = admit != nullptr;
+        const NkFilter f = filt ? *admit : NkFilter{0, 0, 0};
+        *stage = [ix, ids, nb, local, filt, f](NkShard &s) mutable {
+            for (uint32_t q = 0; q < nb; ++q) local[q] = ids[q] - (uint32_t)(s.base - ix->row_base);
+            if (nk::ws_reserve((void **)&s.ws.sub_rows, &s.ws.sub_rows_bytes, (size_t)nb * 4)) return -1;
+            NK_CUDA_OK(cudaMemcpyAsync(s.ws.sub_rows, local.data(), (size_t)nb * 4, cudaMemcpyHostToDevice, s.stream));
+            if (nk::gather_rows(s.rows, ix->dtype, ix->dim, s.ws.sub_rows, nb, s.ws.queries, true, s.stream)) return -1;
+            ix->stats.bytes_h2d += (uint64_t)nb * 4;
+            ix->stats.kernel_launches++;
+            if (filt) {
+                if (shard_tags_on(s)) return -1;
+                if (nk::ws_reserve((void **)&s.ws.qfilter, &s.ws.qfilter_bytes, (size_t)nb * sizeof(NkFilter))) return -1;
+                if (nk::row_filters(s.ws.sub_rows, nb, s.mask_on ? s.mask : nullptr, s.tags, f, s.ws.qfilter, s.stream)) return -1;
+                ix->stats.kernel_launches++;
+            }
+            return 0;
+        };
+        return 0;
+    }
+    // the block may straddle shards: gather on each owner, assemble in pinned host memory, send to every shard
+    if (pinned_reserve((void **)&ix->h_qrows, &ix->h_qrows_bytes, 2 * nb * rb)) return -1;
+    float *blk = ix->h_qrows, *part = ix->h_qrows + (size_t)nb * ix->dim;
+    std::vector<uint32_t> pos(nb);
+    std::vector<NkFilter> filters(admit ? nb : 0), part_f(admit ? nb : 0);
+    for (NkShard *o : live) {
+        uint32_t m = 0;
+        for (uint32_t q = 0; q < nb; ++q) {
+            uint64_t l;
+            if (find_shard(ix, ids[q], &l) == o) { pos[m] = q; local[m++] = (uint32_t)l; }
+        }
+        if (m == 0) continue;
+        NK_CUDA_OK(cudaSetDevice(o->device));
+        if (nk::ws_reserve((void **)&o->ws.sub_rows, &o->ws.sub_rows_bytes, (size_t)m * 4)) return -1;
+        if (nk::ws_reserve(&o->ws.sub_gather, &o->ws.sub_gather_bytes, (size_t)m * rb)) return -1;
+        NK_CUDA_OK(cudaMemcpyAsync(o->ws.sub_rows, local.data(), (size_t)m * 4, cudaMemcpyHostToDevice, o->stream));
+        if (nk::gather_rows(o->rows, ix->dtype, ix->dim, o->ws.sub_rows, m, o->ws.sub_gather, true, o->stream)) return -1;
+        NK_CUDA_OK(cudaMemcpyAsync(part, o->ws.sub_gather, (size_t)m * rb, cudaMemcpyDeviceToHost, o->stream));
+        if (admit) {  // the owner's qfilter slot is free until the scan stages its own filters
+            if (nk::ws_reserve((void **)&o->ws.qfilter, &o->ws.qfilter_bytes, (size_t)m * sizeof(NkFilter))) return -1;
+            if (nk::row_filters(o->ws.sub_rows, m, o->mask_on ? o->mask : nullptr, o->tags_on ? o->tags : nullptr, *admit, o->ws.qfilter,
+                                o->stream))
+                return -1;
+            NK_CUDA_OK(cudaMemcpyAsync(part_f.data(), o->ws.qfilter, (size_t)m * sizeof(NkFilter), cudaMemcpyDeviceToHost, o->stream));
+            ix->stats.kernel_launches++;
+            ix->stats.bytes_d2h += (uint64_t)m * sizeof(NkFilter);
+        }
+        NK_CUDA_OK(cudaStreamSynchronize(o->stream));
+        ix->stats.bytes_h2d += (uint64_t)m * 4;
+        ix->stats.bytes_d2h += (uint64_t)m * rb;
+        ix->stats.kernel_launches++;
+        for (uint32_t i = 0; i < m; ++i) {
+            memcpy(blk + (size_t)pos[i] * ix->dim, part + (size_t)i * ix->dim, rb);
+            if (admit) filters[pos[i]] = part_f[i];
+        }
+    }
+    *stage = [ix, blk, nb, rb, filters](NkShard &s) {
+        NK_CUDA_OK(cudaMemcpyAsync(s.ws.queries, blk, (size_t)nb * rb, cudaMemcpyHostToDevice, s.stream));
+        ix->stats.bytes_h2d += (uint64_t)nb * rb;
+        if (!filters.empty() && !stage_filters(ix, s, filters.data(), nb)) return -1;
+        return 0;
+    };
+    return 0;
+}
+
 int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
@@ -1239,52 +1314,14 @@ int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t 
     if (order.failed()) return -1;
 
     const std::vector<NkShard *> live = live_shards(ix);
-    const size_t rb = (size_t)ix->dim * sizeof(float);
     const uint32_t QB = std::min(Q, SEARCH_ROWS_BLOCK);
-    std::vector<uint32_t> bidx((size_t)QB * kk), local(QB), pos(QB);
+    std::vector<uint32_t> bidx((size_t)QB * kk);
     std::vector<float> bsc((size_t)QB * kk);
-    if (live.size() > 1 && pinned_reserve((void **)&ix->h_qrows, &ix->h_qrows_bytes, 2 * QB * rb)) return -1;
     for (uint32_t b = 0; b < Q; b += QB) {
         const uint32_t nb = std::min(QB, Q - b);
         const uint32_t *ids = rows_host + b;
         StageQueries stage;
-        if (live.size() == 1) {  // only the ids cross PCIe; the rows are gathered straight into the query block
-            stage = [&](NkShard &s) {
-                for (uint32_t q = 0; q < nb; ++q) local[q] = ids[q] - (uint32_t)(s.base - ix->row_base);
-                if (nk::ws_reserve((void **)&s.ws.sub_rows, &s.ws.sub_rows_bytes, (size_t)nb * 4)) return -1;
-                NK_CUDA_OK(cudaMemcpyAsync(s.ws.sub_rows, local.data(), (size_t)nb * 4, cudaMemcpyHostToDevice, s.stream));
-                if (nk::gather_rows(s.rows, ix->dtype, ix->dim, s.ws.sub_rows, nb, s.ws.queries, true, s.stream)) return -1;
-                ix->stats.bytes_h2d += (uint64_t)nb * 4;
-                ix->stats.kernel_launches++;
-                return 0;
-            };
-        } else {  // the block may straddle shards: gather on each owner, assemble in pinned host memory, send to every shard
-            float *blk = ix->h_qrows, *part = ix->h_qrows + (size_t)QB * ix->dim;
-            for (NkShard *o : live) {
-                uint32_t m = 0;
-                for (uint32_t q = 0; q < nb; ++q) {
-                    uint64_t l;
-                    if (find_shard(ix, ids[q], &l) == o) { pos[m] = q; local[m++] = (uint32_t)l; }
-                }
-                if (m == 0) continue;
-                NK_CUDA_OK(cudaSetDevice(o->device));
-                if (nk::ws_reserve((void **)&o->ws.sub_rows, &o->ws.sub_rows_bytes, (size_t)m * 4)) return -1;
-                if (nk::ws_reserve(&o->ws.sub_gather, &o->ws.sub_gather_bytes, (size_t)m * rb)) return -1;
-                NK_CUDA_OK(cudaMemcpyAsync(o->ws.sub_rows, local.data(), (size_t)m * 4, cudaMemcpyHostToDevice, o->stream));
-                if (nk::gather_rows(o->rows, ix->dtype, ix->dim, o->ws.sub_rows, m, o->ws.sub_gather, true, o->stream)) return -1;
-                NK_CUDA_OK(cudaMemcpyAsync(part, o->ws.sub_gather, (size_t)m * rb, cudaMemcpyDeviceToHost, o->stream));
-                NK_CUDA_OK(cudaStreamSynchronize(o->stream));
-                ix->stats.bytes_h2d += (uint64_t)m * 4;
-                ix->stats.bytes_d2h += (uint64_t)m * rb;
-                ix->stats.kernel_launches++;
-                for (uint32_t i = 0; i < m; ++i) memcpy(blk + (size_t)pos[i] * ix->dim, part + (size_t)i * ix->dim, rb);
-            }
-            stage = [&](NkShard &s) {
-                NK_CUDA_OK(cudaMemcpyAsync(s.ws.queries, blk, (size_t)nb * rb, cudaMemcpyHostToDevice, s.stream));
-                ix->stats.bytes_h2d += (uint64_t)nb * rb;
-                return 0;
-            };
-        }
+        if (stage_row_block(ix, live, ids, nb, nullptr, &stage)) return -1;
         if (search_live(ix, live, stage, nullptr, nb, kk, kk, bidx.data(), bsc.data()) < 0) return -1;
         for (uint32_t q = 0; q < nb; ++q) {
             const uint32_t self = (uint32_t)(ix->row_base + ids[q]);
@@ -1326,6 +1363,69 @@ static float range_key_threshold(const NkIndex *ix, float t) {
     return std::max(key, ix->key_floor());
 }
 
+// One shard's range scan of the Q queries staged in s.ws.queries (qfilter: their per-query filters, on the device): path,
+// scan and exact re-scoring -> counts[Q] (host), *list_cap (range_scan_shard).  from > 0 (the self-join's triangular window):
+// only rows [from, s.n) are scanned, from a multiple of the 256-row scan tile, so the window's row-mask words, TMA base and
+// 16-byte alignment are those of the shard; the window gets its own TMA maps (tc_cached_map keys on the base).  pair_first:
+// see range_scan_shard.
+static int range_shard(NkIndex *ix, NkShard &s, uint32_t Q, const NkFilter *qfilter, const uint32_t *thr, uint64_t from,
+                       const uint64_t *pair_first, int *counts, uint32_t *list_cap) {
+    // Paths: the 16-bit and TF32 filters with fixed thresholds, or the CUDA-core scan.
+    nk::ScanArgs a = shard_scan_args(ix, s, s.ws.queries, Q, 1, s.stream, qfilter);
+    const int use = plan_path(ix, s, true, &a);
+    if (use < 0) return -1;
+    if (from) {
+        a.rows = static_cast<const char *>(a.rows) + from * ix->dim * ix->esz();
+        a.n = (uint32_t)(s.n - from);
+        a.row_base = s.base + from;
+        if (a.row_mask) a.row_mask += from / 32;
+        if (a.row_tags) a.row_tags += from;
+        if (a.shadow) {
+            a.shadow = static_cast<const char *>(a.shadow) + from * (a.shadow_native ? ix->dim : a.shadow_dimpad) * 2;
+            a.xnorm2 += from;
+            if (a.dnorm2) a.dnorm2 += from;
+        }
+    }
+    ScanTimer timer(s);
+    if (timer.attach(ix, &a)) return -1;
+    int retried = 0;
+    if (nk::range_scan_shard(s.di, a, use != NK_PATH_SIMT, thr, s.ws, &ix->stats.kernel_launches, counts, list_cap, &retried, pair_first))
+        return -1;
+    timer.keep();
+    s.last_filter = false;
+    ix->last_path = use;
+    ix->stats.bytes_scanned += scan_bytes(ix, use, a, retried ? 2 : 1);
+    return 0;
+}
+
+// After range_shard on every shard of `shards`: each query's survivors, the shards' sorted runs merged into nk_search's order
+// (keys are unique across shards), appended to *out query after query.
+static int range_collect(NkIndex *ix, const std::vector<NkShard *> &shards, uint32_t Q, const std::vector<std::vector<int>> &counts,
+                         const std::vector<uint32_t> &list_cap, std::vector<uint64_t> *out) {
+    std::vector<std::vector<uint64_t>> keys(shards.size());
+    std::vector<std::vector<uint64_t>> offs(shards.size(), std::vector<uint64_t>(Q + 1, 0));
+    for (size_t i = 0; i < shards.size(); ++i) {
+        NK_CUDA_OK(cudaSetDevice(shards[i]->device));
+        if (nk::range_sorted_keys(shards[i]->di, shards[i]->ws, shards[i]->stream, Q, counts[i].data(), list_cap[i], &keys[i],
+                                  &ix->stats.kernel_launches))
+            return -1;
+        ix->stats.bytes_d2h += keys[i].size() * 8;
+        for (uint32_t q = 0; q < Q; ++q) offs[i][q + 1] = offs[i][q] + (uint64_t)counts[i][q];
+    }
+    std::vector<uint64_t> merged, tmp;
+    for (uint32_t q = 0; q < Q; ++q) {
+        merged.clear();
+        for (size_t i = 0; i < shards.size(); ++i) {
+            tmp.resize(merged.size() + (size_t)counts[i][q]);
+            std::merge(merged.begin(), merged.end(), keys[i].begin() + offs[i][q], keys[i].begin() + offs[i][q + 1], tmp.begin(),
+                       std::greater<uint64_t>());
+            merged.swap(tmp);
+        }
+        out->insert(out->end(), merged.begin(), merged.end());
+    }
+    return 0;
+}
+
 int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresholds_host, const NkFilter *filters_host, uint32_t Q,
                     uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total) {
     nk::DeviceGuard _restore_device;
@@ -1359,20 +1459,7 @@ int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresho
         ix->stats.bytes_h2d += qbytes;
         const NkFilter *qfilter = nullptr;
         if (filters_host && !(qfilter = stage_filters(ix, s, filters_host, Q))) return -1;
-        // Paths: the 16-bit and TF32 filters with fixed thresholds, or the CUDA-core scan.
-        nk::ScanArgs a = shard_scan_args(ix, s, s.ws.queries, Q, 1, s.stream, qfilter);
-        const int use = plan_path(ix, s, true, &a);
-        if (use < 0) return -1;
-        ScanTimer timer(s);
-        if (timer.attach(ix, &a)) return -1;
-        int retried = 0;
-        if (nk::range_scan_shard(s.di, a, use != NK_PATH_SIMT, thr.data(), s.ws, &ix->stats.kernel_launches, counts[i].data(), &list_cap[i],
-                                 &retried))
-            return -1;
-        timer.keep();
-        s.last_filter = false;
-        ix->last_path = use;
-        ix->stats.bytes_scanned += scan_bytes(ix, use, a, retried ? 2 : 1);
+        if (range_shard(ix, s, Q, qfilter, thr.data(), 0, nullptr, counts[i].data(), &list_cap[i])) return -1;
     }
     // offsets: the shards' survivors of query q are merged into one run
     for (uint32_t q = 0; q < Q; ++q) {
@@ -1383,27 +1470,94 @@ int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresho
     *out_total = out_offsets[Q];
     if (*out_total > capacity || *out_total == 0) return 0;
     if (!out_idx || !out_score) { nk::set_error("null argument"); return -1; }
-    std::vector<std::vector<uint64_t>> keys(live.size());
-    std::vector<std::vector<uint64_t>> offs(live.size(), std::vector<uint64_t>(Q + 1, 0));
-    for (size_t i = 0; i < live.size(); ++i) {
-        NK_CUDA_OK(cudaSetDevice(live[i]->device));
-        if (nk::range_sorted_keys(live[i]->di, live[i]->ws, live[i]->stream, Q, counts[i].data(), list_cap[i], &keys[i], &ix->stats.kernel_launches))
-            return -1;
-        ix->stats.bytes_d2h += keys[i].size() * 8;
-        for (uint32_t q = 0; q < Q; ++q) offs[i][q + 1] = offs[i][q] + (uint64_t)counts[i][q];
+    std::vector<uint64_t> keys;
+    keys.reserve(*out_total);
+    if (range_collect(ix, live, Q, counts, list_cap, &keys)) return -1;
+    for (size_t j = 0; j < keys.size(); ++j) decode_key(ix->metric, keys[j], out_idx + j, out_score + j);
+    return 0;
+}
+
+// ---- similarity self-join (DESIGN.md §3.5d) ---------------------------------------------------------------------------
+// The stripe's rows are range queries, one threshold for all, in blocks of SEARCH_ROWS_BLOCK consecutive rows gathered on the
+// device as nk_search_rows gathers them.  For a block starting at row s0 the scan skips every shard whose rows all lie at or
+// below s0, and in the shard holding s0 covers only the window from s0 rounded down to the 256-row scan tile; the re-scoring
+// kernel keeps row j for the block's query q only if j > s0 + q.  Left rows that fail the row mask or the filter get the filter
+// that admits no row, on the device that holds them.  Each block's merged survivors are staged in host memory (8 B per pair)
+// until the whole stripe is done, so the offsets and the total are exact before anything is written.
+constexpr uint64_t SCAN_TILE_ROWS = 256;
+
+int nk_search_pairs(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float threshold, const NkFilter *filter, uint64_t capacity,
+                    uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total) {
+    nk::DeviceGuard _restore_device;
+    if (!ix) { nk::set_error("null index"); return -1; }
+    if (n_rows && (!out_offsets || !out_total)) { nk::set_error("null argument"); return -1; }
+    if (threshold != threshold) { nk::set_error("nk_search_pairs: threshold is NaN"); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
+    if (ix->path == NK_PATH_TENSOR) {
+        nk::set_error("nk_search_pairs: the exact 3xTF32 path has no range mode (use AUTO, SIMT, TENSOR_FILTER or TENSOR_SHADOW)");
+        return -1;
     }
-    std::vector<uint64_t> merged, tmp;
-    for (uint32_t q = 0; q < Q; ++q) {
-        merged.clear();
-        for (size_t i = 0; i < live.size(); ++i) {  // each shard's run is sorted: merge them (keys are unique across shards)
-            tmp.resize(merged.size() + (size_t)counts[i][q]);
-            std::merge(merged.begin(), merged.end(), keys[i].begin() + offs[i][q], keys[i].begin() + offs[i][q + 1], tmp.begin(),
-                       std::greater<uint64_t>());
-            merged.swap(tmp);
+    const uint64_t total_rows = ix->rows();
+    if (first_row > total_rows || n_rows > total_rows - first_row) {
+        nk::set_error("nk_search_pairs: rows [%llu, %llu) past the end of the index (%llu rows)", (unsigned long long)first_row,
+                      (unsigned long long)(first_row + n_rows), (unsigned long long)total_rows);
+        return -1;
+    }
+    if (out_offsets) out_offsets[0] = 0;
+    if (out_total) *out_total = 0;
+    if (n_rows == 0) return 0;
+    ix->stats.searches++;
+    ix->stats.queries += n_rows;
+    NK_RANGE_PUSH("nk_search_pairs");
+    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
+
+    const std::vector<NkShard *> live = live_shards(ix);
+    const bool admit = filter || ix->mask_on;  // some left rows may be inadmissible: per-query filters
+    const NkFilter f = filter ? *filter : NkFilter{0, 0, 0};
+    const uint32_t QB = (uint32_t)std::min<uint64_t>(n_rows, SEARCH_ROWS_BLOCK);
+    const std::vector<uint32_t> thr(QB, nk::ord_bits(range_key_threshold(ix, threshold)));
+    std::vector<uint32_t> ids(QB);
+    std::vector<uint64_t> keys;  // the result so far, [out_offsets[0], out_offsets[b])
+    for (uint64_t b = 0; b < n_rows; b += QB) {
+        const uint32_t nb = (uint32_t)std::min<uint64_t>(QB, n_rows - b);
+        const uint64_t s0 = first_row + b;  // the block's first row, relative to the index's first row
+        for (uint32_t q = 0; q < nb; ++q) ids[q] = (uint32_t)(s0 + q);
+        std::vector<NkShard *> scan;
+        std::vector<uint64_t> from;
+        for (NkShard *s : live) {
+            const uint64_t lo = s->base - ix->row_base;
+            if (lo + s->n <= s0 + 1) continue;  // every row at or below s0
+            scan.push_back(s);
+            from.push_back(lo <= s0 ? (s0 - lo) / SCAN_TILE_ROWS * SCAN_TILE_ROWS : 0);
         }
-        const uint64_t o = out_offsets[q];
-        for (size_t j = 0; j < merged.size(); ++j) decode_key(ix->metric, merged[j], out_idx + o + j, out_score + o + j);
+        std::vector<std::vector<int>> counts(scan.size(), std::vector<int>(nb, 0));
+        std::vector<uint32_t> list_cap(scan.size());
+        if (!scan.empty()) {
+            StageQueries stage;
+            if (stage_row_block(ix, live, ids.data(), nb, admit ? &f : nullptr, &stage)) return -1;
+            const uint64_t pair_first = ix->row_base + s0;
+            for (size_t i = 0; i < scan.size(); ++i) {
+                NkShard &s = *scan[i];
+                NK_CUDA_OK(cudaSetDevice(s.device));
+                if (nk::ws_reserve((void **)&s.ws.queries, &s.ws.queries_bytes, (size_t)nb * ix->dim * sizeof(float))) return -1;
+                if (stage(s)) return -1;
+                if (range_shard(ix, s, nb, admit ? s.ws.qfilter : nullptr, thr.data(), from[i], &pair_first, counts[i].data(), &list_cap[i]))
+                    return -1;
+            }
+        }
+        for (uint32_t q = 0; q < nb; ++q) {
+            uint64_t c = 0;
+            for (size_t i = 0; i < scan.size(); ++i) c += (uint64_t)counts[i][q];
+            out_offsets[b + q + 1] = out_offsets[b + q] + c;
+        }
+        if (out_offsets[b + nb] > keys.size() && range_collect(ix, scan, nb, counts, list_cap, &keys)) return -1;
     }
+    *out_total = out_offsets[n_rows];
+    if (*out_total > capacity || *out_total == 0) return 0;
+    if (!out_idx || !out_score) { nk::set_error("null argument"); return -1; }
+    for (size_t j = 0; j < keys.size(); ++j) decode_key(ix->metric, keys[j], out_idx + j, out_score + j);
     return 0;
 }
 

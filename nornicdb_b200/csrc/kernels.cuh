@@ -125,9 +125,10 @@ int scan_tensor_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, ui
 // CUDA-core scan: lists hold every pair whose exact score reaches the threshold.
 int scan_simt_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint32_t list_cap, uint64_t *launches);
 // One shard's scan (tensor: the filter, else the CUDA-core scan) and exact re-scoring: survivors per query -> counts[Q] (host);
-// *list_cap = the list capacity the lists were filled with; *retried = 1 if the scan ran twice.
+// *list_cap = the list capacity the lists were filled with; *retried = 1 if the scan ran twice.  pair_first (the self-join,
+// nk_search_pairs): query q is stored row *pair_first + q (global id) and keeps only rows above it; nullptr = range search.
 int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const uint32_t *thr_bits, Workspace &ws, uint64_t *launches,
-                     int *counts, uint32_t *list_cap, int *retried);
+                     int *counts, uint32_t *list_cap, int *retried, const uint64_t *pair_first = nullptr);
 // After range_scan_shard: the shard's survivors, CSR by counts[Q], each query's run sorted -> *keys (host).
 int range_sorted_keys(const DeviceInfo &di, Workspace &ws, cudaStream_t stream, uint32_t Q, const int *counts, uint32_t list_cap,
                       std::vector<uint64_t> *keys, uint64_t *launches);
@@ -173,6 +174,10 @@ int count_changed(const int32_t *a, const uint32_t *b, uint64_t n, unsigned long
 int convert_f32_to_16(const float *src, void *dst, int dtype, size_t n, cudaStream_t s);  // fp16 / bf16, round to nearest even like the host's astype
 // out[r] = rows[idx[r]]: in the rows' dtype, or (out_f32) widened exactly to fp32
 int gather_rows(const void *rows, int dtype, uint32_t dim, const uint32_t *idx, uint32_t n_idx, void *out, bool out_f32,
+                cudaStream_t s);
+// Left-row admission of a self-join (nk_search_pairs): out[r] = f if local row idx[r] passes the row mask (nullptr = every
+// row) and f admits its tag (tags nullptr = tag 0), else the filter that admits no row (all_of = none_of = ~0).
+int row_filters(const uint32_t *idx, uint32_t n_idx, const uint32_t *mask, const uint64_t *tags, NkFilter f, NkFilter *out,
                 cudaStream_t s);
 
 }  // namespace nk

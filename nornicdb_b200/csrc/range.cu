@@ -5,7 +5,9 @@
 //   1. the list fills come back to the host; a pass whose lists were too short is re-run ONCE with lists of the exact size
 //      (the fills count past the capacity, and the scan is deterministic);
 //   2. range_rescore_kernel re-scores every listed pair exactly in fp32 (warp_exact_score, the arithmetic of every filter
-//      path's finish) and keeps those that meet the threshold; the survivor counts come back to the host (size protocol);
+//      path's finish) and keeps those that meet the threshold; the survivor counts come back to the host (size protocol).
+//      The self-join (nk_search_pairs) runs its twin range_rescore_pairs_kernel, which also drops every row at or below the
+//      query's own row;
 //   3. range_compact_kernel packs the survivors of every query into one CSR array, range_sort_runs_kernel sorts runs of
 //      RUN keys per query in shared memory, range_merge_kernel merges sorted runs pairwise until each query's segment is
 //      one run: (score desc, row asc), the order of nk_search.
@@ -40,9 +42,13 @@ struct RescoreParams {
     int rescore;           // 0: CUDA-core lists (already exact): count only
 };
 
-// One CTA per (RS_ENTRIES-entry chunk, query): each listed key becomes the exact key if that meets the threshold, else 0.
-// A NaN score (-inf after warp_exact_score) or -inf never qualifies.
-__global__ void __launch_bounds__(RS_THREADS) range_rescore_kernel(RescoreParams p) {
+// The body of range_rescore_kernel: one CTA per (RS_ENTRIES-entry chunk, query); each listed key becomes the exact key if
+// that meets the threshold, else 0.  A NaN score (-inf after warp_exact_score) or -inf never qualifies.
+// PAIRS (nk_search_pairs): query q is stored row pair_first + q (global id), and only rows above it are kept, so each
+// unordered pair of a self-join survives once, under its lower row.  Compiled in only for the pairs kernel: range searches
+// run the code they always ran.
+template <bool PAIRS>
+__device__ __forceinline__ void rescore_lists(const RescoreParams &p, uint64_t pair_first) {
     extern __shared__ __align__(16) float qs[];  // the query, [dim]
     __shared__ float s_qq;
     __shared__ int s_cnt;
@@ -54,6 +60,7 @@ __global__ void __launch_bounds__(RS_THREADS) range_rescore_kernel(RescoreParams
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint64_t *list = p.lists + (size_t)q * p.list_cap;
     const float thr = ord_to_float(p.thr[q]);
+    const uint64_t self = pair_first + q;  // PAIRS: keep rows > self
     if (tid == 0) s_cnt = 0;
     int mine = 0;
     if (p.rescore) {
@@ -69,6 +76,10 @@ __global__ void __launch_bounds__(RS_THREADS) range_rescore_kernel(RescoreParams
         __syncthreads();
         for (int i = i0 + warp; i < i1; i += RS_THREADS / 32) {
             const uint32_t grow = key_row(list[i]);
+            if (PAIRS && grow <= self) {  // the pair belongs to the lower row's list: not scored here
+                if (lane == 0) list[i] = 0ull;
+                continue;
+            }
             const float sc = warp_exact_score(p.rows, p.dtype, (size_t)(grow - (uint32_t)p.row_base), p.dim, qs, s_qq, p.metric, lane);
             const bool keep = sc > -INFINITY && sc >= thr;
             if (lane == 0) {
@@ -78,12 +89,21 @@ __global__ void __launch_bounds__(RS_THREADS) range_rescore_kernel(RescoreParams
         }
     } else {
         __syncthreads();
-        for (int i = i0 + tid; i < i1; i += RS_THREADS) mine += list[i] != 0ull ? 1 : 0;
+        for (int i = i0 + tid; i < i1; i += RS_THREADS) {
+            uint64_t key = list[i];
+            if (PAIRS && key != 0ull && key_row(key) <= self) list[i] = key = 0ull;
+            mine += key != 0ull ? 1 : 0;
+        }
     }
     mine = __reduce_add_sync(0xffffffffu, mine);
     if (lane == 0 && mine) atomicAdd(&s_cnt, mine);
     __syncthreads();
     if (tid == 0 && s_cnt) atomicAdd(p.count + q, s_cnt);
+}
+
+__global__ void __launch_bounds__(RS_THREADS) range_rescore_kernel(RescoreParams p) { rescore_lists<false>(p, 0); }
+__global__ void __launch_bounds__(RS_THREADS) range_rescore_pairs_kernel(RescoreParams p, uint64_t pair_first) {
+    rescore_lists<true>(p, pair_first);
 }
 
 // Survivors (non-zero keys) of query q's list -> out[off[q] ..), in list order.
@@ -160,7 +180,7 @@ constexpr uint32_t LIST0 = 1024;  // first list capacity per query (the workspac
 // Steps 1 and 2 on one shard: survivors per query -> counts[Q] (host); *list_cap = the list capacity the lists were filled
 // with (range_sorted_keys reads them); *retried = 1 if the scan ran twice.
 int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const uint32_t *thr_bits, Workspace &ws, uint64_t *launches,
-                     int *counts, uint32_t *list_cap_out, int *retried) {
+                     int *counts, uint32_t *list_cap_out, int *retried, const uint64_t *pair_first) {
     const uint32_t Q = a.Q, QA = range_qa(Q);
     *retried = 0;
     if (ws_reserve((void **)&ws.keys2, &ws.keys2_bytes, (size_t)(2 * QA + 2 * Q) * 4 + (size_t)(Q + 1) * 8)) return -1;
@@ -196,11 +216,14 @@ int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const
     rp.lists = ws.partial; rp.list_cap = list_cap; rp.fill = ws_fill(ws, Q); rp.thr = ws_thr(ws); rp.count = ws_count(ws, Q);
     rp.rescore = tensor ? 1 : 0;
     const size_t smem = tensor ? (size_t)a.dim * 4 : 0;
-    if (smem > 48 * 1024 && tc_ensure_smem(reinterpret_cast<const void *>(range_rescore_kernel), di.device_id, smem)) return -1;
+    const void *kern = pair_first ? reinterpret_cast<const void *>(range_rescore_pairs_kernel) : reinterpret_cast<const void *>(range_rescore_kernel);
+    if (smem > 48 * 1024 && tc_ensure_smem(kern, di.device_id, smem)) return -1;
     if (longest > 0)
         for (uint32_t q0 = 0; q0 < Q; q0 += MAX_GRID_Y) {
             rp.q_base = q0;
-            range_rescore_kernel<<<dim3((longest + RS_ENTRIES - 1) / RS_ENTRIES, std::min(MAX_GRID_Y, Q - q0)), RS_THREADS, smem, a.stream>>>(rp);
+            const dim3 grid((longest + RS_ENTRIES - 1) / RS_ENTRIES, std::min(MAX_GRID_Y, Q - q0));
+            if (pair_first) range_rescore_pairs_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp, *pair_first);
+            else range_rescore_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp);
             NK_CUDA_OK(cudaGetLastError());
             if (launches) ++*launches;
         }

@@ -6,6 +6,7 @@
 //   fill_uniform / fill_clustered   synthetic corpora generated in HBM (bench / tests); the uniform one is bit-identical
 //                   to the oracle's, the Gaussian mixture is SURVEY.md §8(d)'s near-tie corpus
 //   gather_rows     row gather for ScoreSubset (gpu.go:1578-1589 does this on the host + re-upload)
+//   row_filters     left-row admission of the self-join (nk_search_pairs): one thread per row, not warp-per-row
 //   row_sqnorms16   |x|^2 per row of an fp16 / bf16 corpus (the 16-bit tensor pass scans such a corpus in place)
 //   group_best      best-of-chunks per node for db.index.vector.queryNodes (call_vector.go:217-240)
 // All are warp-per-row, lanes striding the row in 16-byte vectors where the layout allows (one 512 B coalesced segment per
@@ -215,6 +216,16 @@ __global__ void gather_rows_kernel(const T *rows, uint32_t dim, const uint32_t *
     }
 }
 
+__global__ void row_filters_kernel(const uint32_t *idx, uint32_t n_idx, const uint32_t *mask, const uint64_t *tags, NkFilter f,
+                                   NkFilter *out) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_idx) return;
+    const uint32_t row = idx[r];
+    const bool in_mask = !mask || ((mask[row >> 5] >> (row & 31)) & 1u);
+    const uint64_t tag = tags ? tags[row] : 0ull;
+    out[r] = in_mask && tag_admits(tag, f.all_of, f.none_of, f.any_of) ? f : NkFilter{~0ull, ~0ull, 0ull};
+}
+
 // |x|^2 per row of a 16-bit corpus (fp32 accumulation of the exactly widened elements)
 template <typename T>
 __global__ void row_sqnorms16_kernel(const T *rows, uint64_t n, uint32_t dim, float *out) {
@@ -396,6 +407,13 @@ int gather_rows(const void *rows, int dtype, uint32_t dim, const uint32_t *idx, 
         gather_rows_kernel<__half, float><<<warp_grid(n_idx), 256, 0, s>>>((const __half *)rows, dim, idx, n_idx, (float *)out);
     else
         gather_rows_kernel<__nv_bfloat16, float><<<warp_grid(n_idx), 256, 0, s>>>((const __nv_bfloat16 *)rows, dim, idx, n_idx, (float *)out);
+    NK_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+int row_filters(const uint32_t *idx, uint32_t n_idx, const uint32_t *mask, const uint64_t *tags, NkFilter f, NkFilter *out,
+                cudaStream_t s) {
+    if (n_idx == 0) return 0;
+    row_filters_kernel<<<(n_idx + 255) / 256, 256, 0, s>>>(idx, n_idx, mask, tags, f, out);
     NK_CUDA_OK(cudaGetLastError());
     return 0;
 }

@@ -11,6 +11,7 @@
 //   namespace nornic::gpu    EmbeddingIndex (Add / AddBatch / Remove / Search / SearchBatch / ScoreSubset /
 //                            Count / Has / Get / Serialize / Deserialize), device corpus kept in step incrementally
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <cstring>
 #include <memory>
@@ -200,6 +201,11 @@ struct SearchResult {  // gpu.go SearchResult{ID, Score, Distance}
     float Distance;
 };
 
+struct SimilarPair {  // one pair of a self-join: A is the node at the lower row
+    std::string A, B;
+    float Score;
+};
+
 // gpu.EmbeddingIndex (gpu.go:1224-2454) with the device corpus kept in step incrementally (no re-upload on Add/Remove,
 // rows stay raw, cosine computed in-kernel).  Node-id strings live on the host only (gpu.go:1228-1231).
 class EmbeddingIndex {
@@ -316,6 +322,34 @@ public:
         for (uint32_t q = 0; q < Q; ++q)
             for (uint64_t i = off[q]; i < off[q + 1]; ++i)
                 if (idx[i] < nodeIDs_.size()) out[q].push_back({nodeIDs_[idx[i]], sc[i], 1.0f - sc[i]});
+        return out;
+    }
+    // Every pair of stored nodes whose similarity reaches the threshold (cosine / dot: minimum score; euclidean: maximum
+    // distance), each pair once, grouped by its lower row and best first within a group; filter = nullptr or one tag filter
+    // both nodes must pass.  The join runs in stripes of at most stripeRows left rows, so the staging (8 B per pair) and the
+    // cost of a call that outgrows its buffer stay bounded.  Sizes its buffers from the library's exact total.
+    std::vector<SimilarPair> SearchPairs(float threshold, const NkFilter *filter = nullptr, uint64_t stripeRows = 1u << 16) {
+        std::lock_guard<std::mutex> lk(mu_);
+        std::vector<SimilarPair> out;
+        const uint64_t n = nk_index_rows(ix_);
+        if (stripeRows == 0) stripeRows = 1;
+        std::vector<uint32_t> idx;
+        std::vector<float> sc;
+        for (uint64_t first = 0; first < n; first += stripeRows) {
+            const uint64_t rows = std::min<uint64_t>(stripeRows, n - first);
+            std::vector<uint64_t> off(rows + 1);
+            uint64_t total = 0;
+            for (int pass = 0; pass < 2; ++pass) {
+                if (nk_search_pairs(ix_, first, rows, threshold, filter, idx.size(), off.data(), idx.data(), sc.data(), &total) < 0)
+                    throw cuda::ErrKernelExecution(std::string("gpu: ") + nk_last_error());
+                if (total <= idx.size()) break;
+                idx.resize(total);
+                sc.resize(total);
+            }
+            for (uint64_t r = 0; r < rows; ++r)
+                for (uint64_t i = off[r]; i < off[r + 1]; ++i)
+                    if (first + r < nodeIDs_.size() && idx[i] < nodeIDs_.size()) out.push_back({nodeIDs_[first + r], nodeIDs_[idx[i]], sc[i]});
+        }
         return out;
     }
     // The k most similar OTHER nodes of each stored node (FindSimilar, GraphQL similar, OnStore's related nodes), best first,

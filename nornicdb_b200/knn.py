@@ -298,6 +298,35 @@ class KnnIndex:
         o = off.astype(np.int64)
         return [(idx[o[i]:o[i + 1]].copy(), sc[o[i]:o[i + 1]].copy()) for i in range(Q)]
 
+    def search_pairs(self, threshold: float, first_row: int = 0, n_rows: Optional[int] = None,
+                     filter=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """Similarity self-join: for each left row i of the stripe [first_row, first_row + n_rows) (default: to the end of the
+        index), every admissible row j > i whose score against row i reaches `threshold` (cosine / dot: minimum score;
+        euclidean: maximum distance), so each pair of the stripe appears once, under its lower row.  filter = one
+        (all_of, none_of, any_of) tag filter for both sides, None = none.  Returns CSR arrays (offsets uint64 [n_rows + 1],
+        idx uint32, score float32): row first_row + r's list is [offsets[r], offsets[r + 1]), in search()'s order.  The result
+        buffer grows to the size the library reports (nk_search_pairs' size protocol); a call that outgrows it joins twice."""
+        first_row = int(first_row)
+        n_rows = max(len(self) - first_row, 0) if n_rows is None else int(n_rows)
+        if first_row < 0 or n_rows < 0:
+            raise KnnError("search_pairs: first_row and n_rows must be >= 0")
+        f = None if filter is None else as_filters(filter, 1)
+        off = np.zeros(n_rows + 1, dtype=np.uint64)
+        total = C.c_uint64(0)
+        cap = getattr(self, "_pairs_cap", 0)
+        while True:
+            idx = np.empty(max(cap, 1), dtype=np.uint32)
+            sc = np.empty(max(cap, 1), dtype=np.float32)
+            _check(self.lib.nk_search_pairs(self.ptr, first_row, n_rows, float(threshold), None if f is None else f.ctypes.data_as(C.c_void_p),
+                                            cap, off.ctypes.data_as(C.c_void_p), idx.ctypes.data_as(C.c_void_p),
+                                            sc.ctypes.data_as(C.c_void_p), C.byref(total)), "nk_search_pairs")
+            if total.value <= cap:
+                break
+            cap = int(total.value)
+            self._pairs_cap = cap
+        t = int(total.value)
+        return off, idx[:t].copy(), sc[:t].copy()
+
     def search_filtered_device(self, q_ptr: int, filters_ptr: int, Q: int, k: int, out_idx_ptr: int, out_score_ptr: int,
                                stream: int = 0) -> int:
         """Device-resident filtered search: filters_ptr = device [Q x 3] uint64 (0 = no filter), valid until the stream ran."""
