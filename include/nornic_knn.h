@@ -317,6 +317,32 @@ int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresho
 int nk_search_pairs(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float threshold, const NkFilter *filter, uint64_t capacity,
                     uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total);
 
+/* ---- k-NN graph update -------------------------------------------------------------------------------------------------
+ * Keeps the k-NN graph of nk_search_rows exact across nk_index_append and nk_index_update_row without an O(N^2) rebuild.
+ * graph_idx / graph_score: host arrays [nk_index_rows(ix) x k], row stride k.  On entry rows [0, n_old) hold what
+ * nk_search_rows(rows 0 .. n_old-1, k) returned before the changes, unused slots 0xffffffff / 0.  Rows [n_old, N) are the
+ * rows appended since; changed_rows [n_changed] the old rows rewritten since (ids < n_old, repeats allowed).  On return every
+ * row holds, bit for bit, what nk_search_rows(rows 0 .. N-1, k) returns now (order, ties, scores), slots past a list 0xffffffff
+ * / 0; *n_lists_changed (nullable) = how many old rows' lists changed.  Ids are global (row_base included), as returned.
+ * New and rewritten rows, and the old rows that list a rewritten row, are searched again; every other old row's list only
+ * takes in new or rewritten rows that beat its k-th entry, found by one scan of those rows with per-row thresholds.
+ * Preconditions (not checked): the metric and the score floor are unchanged since the graph was built, every old row keeps
+ * its row-mask bit (nk_index_append clears the mask: set it again), and the graph was built on the graph path — TENSOR_SHADOW
+ * or TENSOR_FILTER forced, or under AUTO the 16-bit pass where every live shard has a 16-bit image and the TF32 filter
+ * otherwise.  (AUTO runs blocks of <= 4 rows on a shard under 64 MB on the CUDA cores, whose arithmetic differs: build a graph
+ * that will be updated with the path set.)  This call runs on that path whatever AUTO would pick.
+ * Returns min(k, admissible rows), the entries a list can hold (nk_search_rows' return value), or -1 with nk_last_error,
+ * before the arrays are touched, for: the SIMT or 3xTF32 path forced, k == 0 or
+ * k > NK_GRAPH_MAX_K, a shape without a filter path, n_old > N, a changed id >= n_old, a graph entry of rows [0, n_old) that is
+ * neither an old row nor 0xffffffff, or a null pointer.  nk_index_remove_swap renumbers rows: rebuild after it.
+ * NaN rows: a search block with a NaN query falls through to the exact stage, whose cosine / dot arithmetic differs, so
+ * nk_search_rows itself depends on the block there; the guarantee covers the rows of rebuild blocks without a NaN query, and
+ * a NaN row's own list holds the right rows with its stage's scores.
+ * Synchronous, and it holds the index lock throughout, like nk_search_rows. */
+#define NK_GRAPH_MAX_K 191u /* nk_search_rows asks the scan for k + 1; the filter paths stop at 192 */
+int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
+                        uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed);
+
 /* Multi-process sharding (one rank per GPU): emit this shard's sorted candidate list as packed 64-bit
  * keys [Q x k] (order-preserving score bits << 32 | ~row index; larger key = better), to be exchanged
  * (e.g. ncclAllGather of Q*k*8 bytes per rank) and merged with nk_merge_keys_device.  k <= NK_MAX_K_TOTAL: one shard's

@@ -1290,30 +1290,13 @@ static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, cons
     return 0;
 }
 
-int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
-    nk::DeviceGuard _restore_device;
-    if (!ix) { nk::set_error("null index"); return -1; }
-    if (Q && (!rows_host || !out_idx || !out_score)) { nk::set_error("null argument"); return -1; }
-    if (k > NK_MAX_K_TOTAL - 1) { nk::set_error("nk_search_rows: k=%u exceeds NK_MAX_K_TOTAL - 1 = %u", k, NK_MAX_K_TOTAL - 1); return -1; }
-    std::lock_guard<std::mutex> lk(ix->mu);
-    const uint64_t total = ix->rows();
-    const uint64_t N = ix->mask_on ? ix->mask_alive : total;  // rows that can be returned
-    if (k == 0 || N == 0 || Q == 0) return 0;
-    for (uint32_t q = 0; q < Q; ++q)
-        if (rows_host[q] >= total) {
-            nk::set_error("nk_search_rows: row %u (query %u) out of range, index has %llu rows", rows_host[q], q, (unsigned long long)total);
-            return -1;
-        }
+// The body of nk_search_rows, the index lock held and the ids checked: returns ke, the entries written per query (the rest of
+// each k-wide output row is left as it is).
+static int search_rows_locked(NkIndex *ix, const std::vector<NkShard *> &live, const uint32_t *rows_host, uint32_t Q, uint32_t k,
+                              uint32_t *out_idx, float *out_score) {
+    const uint64_t N = ix->mask_on ? ix->mask_alive : ix->rows();  // rows that can be returned
     const uint32_t kk = (uint32_t)std::min<uint64_t>((uint64_t)k + 1, N);  // asked of the scan
     const uint32_t ke = (uint32_t)std::min<uint64_t>(k, N);                // returned
-    ix->stats.searches++;
-    ix->stats.queries += Q;
-    NK_RANGE_PUSH("nk_search_rows");
-    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
-    ShardOrder order(ix);
-    if (order.failed()) return -1;
-
-    const std::vector<NkShard *> live = live_shards(ix);
     const uint32_t QB = std::min(Q, SEARCH_ROWS_BLOCK);
     std::vector<uint32_t> bidx((size_t)QB * kk);
     std::vector<float> bsc((size_t)QB * kk);
@@ -1339,6 +1322,29 @@ int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t 
         }
     }
     return (int)ke;
+}
+
+int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
+    nk::DeviceGuard _restore_device;
+    if (!ix) { nk::set_error("null index"); return -1; }
+    if (Q && (!rows_host || !out_idx || !out_score)) { nk::set_error("null argument"); return -1; }
+    if (k > NK_MAX_K_TOTAL - 1) { nk::set_error("nk_search_rows: k=%u exceeds NK_MAX_K_TOTAL - 1 = %u", k, NK_MAX_K_TOTAL - 1); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
+    const uint64_t total = ix->rows();
+    const uint64_t N = ix->mask_on ? ix->mask_alive : total;  // rows that can be returned
+    if (k == 0 || N == 0 || Q == 0) return 0;
+    for (uint32_t q = 0; q < Q; ++q)
+        if (rows_host[q] >= total) {
+            nk::set_error("nk_search_rows: row %u (query %u) out of range, index has %llu rows", rows_host[q], q, (unsigned long long)total);
+            return -1;
+        }
+    ix->stats.searches++;
+    ix->stats.queries += Q;
+    NK_RANGE_PUSH("nk_search_rows");
+    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
+    return search_rows_locked(ix, live_shards(ix), rows_host, Q, k, out_idx, out_score);
 }
 
 // ---- range search ---------------------------------------------------------------------------------------------------
@@ -1368,12 +1374,16 @@ static float range_key_threshold(const NkIndex *ix, float t) {
 // only rows [from, s.n) are scanned, from a multiple of the 256-row scan tile, so the window's row-mask words, TMA base and
 // 16-byte alignment are those of the shard; the window gets its own TMA maps (tc_cached_map keys on the base).  pair_first:
 // see range_scan_shard.
+// row_thr (nk_knn_graph_update's reverse scan, device [s.n]): per-row thresholds, and row_keep (device mask words) takes the
+// place of the row mask: it selects the rows whose lists are updated, not the rows that may be returned.
 static int range_shard(NkIndex *ix, NkShard &s, uint32_t Q, const NkFilter *qfilter, const uint32_t *thr, uint64_t from,
-                       const uint64_t *pair_first, int *counts, uint32_t *list_cap) {
+                       const uint64_t *pair_first, int *counts, uint32_t *list_cap, const float *row_thr = nullptr,
+                       const uint32_t *row_keep = nullptr) {
     // Paths: the 16-bit and TF32 filters with fixed thresholds, or the CUDA-core scan.
     nk::ScanArgs a = shard_scan_args(ix, s, s.ws.queries, Q, 1, s.stream, qfilter);
     const int use = plan_path(ix, s, true, &a);
     if (use < 0) return -1;
+    if (row_thr) { a.row_thr = row_thr; a.row_mask = row_keep; }
     if (from) {
         a.rows = static_cast<const char *>(a.rows) + from * ix->dim * ix->esz();
         a.n = (uint32_t)(s.n - from);
@@ -1559,6 +1569,300 @@ int nk_search_pairs(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float thre
     if (!out_idx || !out_score) { nk::set_error("null argument"); return -1; }
     for (size_t j = 0; j < keys.size(); ++j) decode_key(ix->metric, keys[j], out_idx + j, out_score + j);
     return 0;
+}
+
+// ---- k-NN graph update (DESIGN.md §3.5e) -------------------------------------------------------------------------------
+// Rows whose list may have changed in more than one place (the new and rewritten rows, and every old row that lists a
+// rewritten one) are searched again, as nk_search_rows searches them.  For every other old row r only the rows C that are new
+// or rewritten can enter its list: they are scanned as queries over the index with the row's own threshold (the k-th entry's
+// score, or the floor if the list is not full) and the rows searched again masked out, re-scored as r's list scores them
+// (K(r, q), warp_pair_score), and merged with the old entries, whose keys are recomputed the same way.  The graph path
+// (16-bit pass or TF32 filter) is forced for the whole call: every score it makes is warp_exact_score's, whichever block of
+// queries it is computed in.
+constexpr uint32_t GRAPH_PAD = 0xffffffffu;
+
+// Rows among the first n (relative ids) that pass the row mask.
+static int admissible_below(NkIndex *ix, uint64_t n, uint64_t *out) {
+    uint64_t c = 0;
+    for (auto &s : ix->shards) {
+        const uint64_t lo = s.base - ix->row_base;
+        if (s.n == 0 || lo >= n) continue;
+        const uint64_t m = std::min<uint64_t>(s.n, n - lo);
+        if (!ix->mask_on || !s.mask_on) { c += m; continue; }
+        std::vector<uint32_t> w((m + 31) / 32);
+        NK_CUDA_OK(cudaSetDevice(s.device));
+        NK_CUDA_OK(cudaMemcpyAsync(w.data(), s.mask, w.size() * 4, cudaMemcpyDeviceToHost, s.stream));
+        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+        for (uint64_t i = 0; i < m; ++i) c += (w[i >> 5] >> (i & 31)) & 1u;
+    }
+    *out = c;
+    return 0;
+}
+
+// Searches that fell through to the exact stage so far, all shards (cumulative status word FLAG_N_EXACT).
+static int exact_stage_runs(NkIndex *ix, uint64_t *out) {
+    uint64_t c = 0;
+    for (auto &s : ix->shards) {
+        if (!s.ws.flags) continue;
+        int h = 0;
+        NK_CUDA_OK(cudaSetDevice(s.device));
+        NK_CUDA_OK(cudaMemcpyAsync(&h, s.ws.flags + nk::FLAG_N_EXACT, 4, cudaMemcpyDeviceToHost, s.stream));
+        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+        c += (uint64_t)h;
+    }
+    *out = c;
+    return 0;
+}
+
+// The keys K(r, j) of pairs (r, j) (relative ids), r all on shard s -> keys[i].
+static int graph_pair_keys_on(NkIndex *ix, const std::vector<NkShard *> &live, NkShard &s, const std::vector<uint32_t> &pr,
+                              const std::vector<uint32_t> &pj, std::vector<uint64_t> *keys) {
+    keys->assign(pr.size(), 0ull);
+    std::vector<uint32_t> js(pj);  // distinct j, staged in blocks of SEARCH_ROWS_BLOCK
+    std::sort(js.begin(), js.end());
+    js.erase(std::unique(js.begin(), js.end()), js.end());
+    std::vector<uint32_t> order(pr.size());
+    for (size_t i = 0; i < order.size(); ++i) order[i] = (uint32_t)i;
+    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return pj[a] < pj[b]; });
+    size_t at = 0;
+    for (size_t b = 0; b < js.size(); b += SEARCH_ROWS_BLOCK) {
+        const uint32_t nb = (uint32_t)std::min<size_t>(SEARCH_ROWS_BLOCK, js.size() - b);
+        StageQueries stage;
+        if (stage_row_block(ix, live, js.data() + b, nb, nullptr, &stage)) return -1;
+        NK_CUDA_OK(cudaSetDevice(s.device));
+        if (nk::ws_reserve((void **)&s.ws.queries, &s.ws.queries_bytes, (size_t)nb * ix->dim * sizeof(float))) return -1;
+        if (stage(s)) return -1;
+        const uint32_t last = js[b + nb - 1];
+        std::vector<uint32_t> arg;  // [r local | slot of j | global j]
+        std::vector<uint32_t> idx;
+        for (; at < order.size() && pj[order[at]] <= last; ++at) idx.push_back(order[at]);
+        const size_t n = idx.size();
+        if (n == 0) continue;
+        arg.resize(3 * n);
+        for (size_t i = 0; i < n; ++i) {
+            arg[i] = pr[idx[i]] - (uint32_t)(s.base - ix->row_base);
+            arg[n + i] = (uint32_t)(std::lower_bound(js.begin() + b, js.begin() + b + nb, pj[idx[i]]) - (js.begin() + b));
+            arg[2 * n + i] = (uint32_t)(ix->row_base + pj[idx[i]]);
+        }
+        if (nk::ws_reserve(&s.ws.scratch, &s.ws.scratch_bytes, n * 12 + n * 8 + 8)) return -1;
+        uint32_t *d_arg = static_cast<uint32_t *>(s.ws.scratch);
+        uint64_t *d_out = reinterpret_cast<uint64_t *>(static_cast<char *>(s.ws.scratch) + (n * 12 + 7) / 8 * 8);
+        std::vector<uint64_t> out(n);
+        NK_CUDA_OK(cudaMemcpyAsync(d_arg, arg.data(), n * 12, cudaMemcpyHostToDevice, s.stream));
+        if (nk::graph_pair_keys(s.rows, ix->dtype, ix->dim, ix->metric, s.ws.queries, d_arg, d_arg + n, d_arg + 2 * n, (uint32_t)n, d_out,
+                                s.stream))
+            return -1;
+        NK_CUDA_OK(cudaMemcpyAsync(out.data(), d_out, n * 8, cudaMemcpyDeviceToHost, s.stream));
+        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+        ix->stats.kernel_launches++;
+        ix->stats.bytes_h2d += n * 12;
+        ix->stats.bytes_d2h += n * 8;
+        for (size_t i = 0; i < n; ++i) (*keys)[idx[i]] = out[i];
+    }
+    return 0;
+}
+
+int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
+                        uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed) {
+    nk::DeviceGuard _restore_device;
+    if (!ix) { nk::set_error("null index"); return -1; }
+    if (!graph_idx || !graph_score || (n_changed && !changed_rows)) { nk::set_error("null argument"); return -1; }
+    if (k == 0 || k > NK_GRAPH_MAX_K) { nk::set_error("nk_knn_graph_update: k=%u outside [1, %u]", k, NK_GRAPH_MAX_K); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
+    if (ix->path == NK_PATH_SIMT || ix->path == NK_PATH_TENSOR) {
+        nk::set_error("nk_knn_graph_update: the graph is kept on the filter paths (AUTO, TENSOR_FILTER or TENSOR_SHADOW), not path %d", ix->path);
+        return -1;
+    }
+    const uint64_t N = ix->rows();
+    if (n_old > N) { nk::set_error("nk_knn_graph_update: n_old=%llu exceeds the index's %llu rows", (unsigned long long)n_old, (unsigned long long)N); return -1; }
+    for (uint32_t i = 0; i < n_changed; ++i)
+        if (changed_rows[i] >= n_old) { nk::set_error("nk_knn_graph_update: changed row %u is not an old row (n_old=%llu)", changed_rows[i], (unsigned long long)n_old); return -1; }
+    for (uint64_t i = 0; i < n_old * k; ++i)
+        if (graph_idx[i] != GRAPH_PAD && (graph_idx[i] < ix->row_base || graph_idx[i] - ix->row_base >= n_old)) {
+            nk::set_error("nk_knn_graph_update: entry %llu of the graph (row %u) is not an old row", (unsigned long long)i, graph_idx[i]);
+            return -1;
+        }
+    const std::vector<NkShard *> live = live_shards(ix);
+    // the graph path: the forced one, or under AUTO the 16-bit pass where every live shard has a 16-bit image, else the TF32 filter
+    int gpath = ix->path;
+    if (gpath == NK_PATH_AUTO) {
+        gpath = NK_PATH_TENSOR_SHADOW;
+        for (NkShard *s : live)
+            if (!(s->xnorm2 && s->shadow_n == s->n)) gpath = NK_PATH_TENSOR_FILTER;
+    }
+    struct PathGuard {
+        NkIndex *ix; int saved;
+        ~PathGuard() { ix->path = saved; }
+    } path_guard{ix, ix->path};
+    ix->path = gpath;
+    for (NkShard *s : live) {
+        nk::ScanArgs a = shard_scan_args(ix, *s, nullptr, SEARCH_ROWS_BLOCK, k + 1, s->stream);
+        if (plan_path(ix, *s, false, &a) < 0) return -1;  // the error names the path and the shape
+    }
+    if (n_lists_changed) *n_lists_changed = 0;
+    ix->stats.searches++;
+    NK_RANGE_PUSH("nk_knn_graph_update");
+    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
+
+    // the rows to search again (R) and the queries of the reverse scan (C: new and rewritten rows)
+    std::vector<uint8_t> in_r(N, 0), changed(n_old, 0);
+    std::vector<uint32_t> C;
+    for (uint32_t i = 0; i < n_changed; ++i)
+        if (!changed[changed_rows[i]]) { changed[changed_rows[i]] = 1; in_r[changed_rows[i]] = 1; C.push_back(changed_rows[i]); }
+    for (uint64_t r = n_old; r < N; ++r) { in_r[r] = 1; C.push_back((uint32_t)r); }
+    const uint64_t adm = ix->mask_on ? ix->mask_alive : N;
+    const int ke = (int)std::min<uint64_t>(k, adm);
+    if (C.empty()) return ke;
+    // nk_search_rows treats a row specially while no more than k rows are admissible (its list drops one of them when the row
+    // itself is not admissible): then every row is searched again
+    uint64_t old_adm = 0;
+    if (admissible_below(ix, n_old, &old_adm)) return -1;
+    const bool all = old_adm <= k || adm <= k;
+    // A NaN row's list (every score -inf, decoded) comes from the exact stage its search block falls through to: its keys are
+    // that stage's, not warp_exact_score's, so such a row is searched again rather than merged.
+    const float nan_score = ix->metric == NK_METRIC_EUCLIDEAN ? INFINITY : -INFINITY;
+    for (uint64_t r = 0; r < n_old; ++r) {
+        if (in_r[r]) continue;
+        if (all || (graph_idx[r * k] != GRAPH_PAD && graph_score[r * k] == nan_score)) { in_r[r] = 1; continue; }
+        for (uint32_t j = 0; j < k; ++j) {
+            const uint32_t e = graph_idx[r * k + j];
+            if (e != GRAPH_PAD && changed[e - ix->row_base]) { in_r[r] = 1; break; }
+        }
+    }
+    uint64_t n_changed_lists = 0;
+    auto write_list = [&](uint64_t r, const uint32_t *li, const float *ls) {
+        if (r < n_old && (memcmp(graph_idx + r * k, li, (size_t)k * 4) || memcmp(graph_score + r * k, ls, (size_t)k * 4))) ++n_changed_lists;
+        memcpy(graph_idx + r * k, li, (size_t)k * 4);
+        memcpy(graph_score + r * k, ls, (size_t)k * 4);
+    };
+
+    // reverse scan + merge for the old rows outside R
+    bool reverse = false;
+    for (uint64_t r = 0; r < n_old && !reverse; ++r) reverse = !in_r[r];
+    if (reverse) {
+        for (NkShard *s : live) {  // per-row thresholds and the mask of rows outside R
+            const uint64_t lo = s->base - ix->row_base, words = (s->n + 31) / 32;
+            std::vector<float> thr(s->n + words);
+            uint32_t *keep = reinterpret_cast<uint32_t *>(thr.data() + s->n);
+            for (uint64_t w = 0; w < words; ++w) keep[w] = 0u;
+            for (uint64_t l = 0; l < s->n; ++l) {
+                const uint64_t r = lo + l;
+                thr[l] = INFINITY;
+                if (in_r[r]) continue;
+                keep[l >> 5] |= 1u << (l & 31);
+                thr[l] = graph_idx[r * k + k - 1] != GRAPH_PAD ? range_key_threshold(ix, graph_score[r * k + k - 1]) : ix->key_floor();
+            }
+            NK_CUDA_OK(cudaSetDevice(s->device));
+            if (nk::ws_reserve((void **)&s->ws.row_thr, &s->ws.row_thr_bytes, thr.size() * 4)) return -1;
+            NK_CUDA_OK(cudaMemcpyAsync(s->ws.row_thr, thr.data(), thr.size() * 4, cudaMemcpyHostToDevice, s->stream));
+            NK_CUDA_OK(cudaStreamSynchronize(s->stream));  // thr is pageable and goes out of scope
+            ix->stats.bytes_h2d += thr.size() * 4;
+        }
+        const NkFilter all_rows{0, 0, 0};  // masked-out queries get the filter that admits no row (stage_row_block)
+        const uint32_t QB = (uint32_t)std::min<size_t>(C.size(), SEARCH_ROWS_BLOCK);
+        const std::vector<uint32_t> floor_thr(QB, nk::ord_bits(ix->key_floor()));
+        std::vector<std::pair<uint32_t, uint64_t>> entrants;  // (old row r, key of the new or rewritten row in r's list)
+        std::vector<uint64_t> keys;
+        for (size_t b = 0; b < C.size(); b += QB) {
+            const uint32_t nb = (uint32_t)std::min<size_t>(QB, C.size() - b);
+            StageQueries stage;
+            if (stage_row_block(ix, live, C.data() + b, nb, ix->mask_on ? &all_rows : nullptr, &stage)) return -1;
+            std::vector<std::vector<int>> counts(live.size(), std::vector<int>(nb, 0));
+            std::vector<uint32_t> list_cap(live.size());
+            for (size_t i = 0; i < live.size(); ++i) {
+                NkShard &s = *live[i];
+                NK_CUDA_OK(cudaSetDevice(s.device));
+                if (nk::ws_reserve((void **)&s.ws.queries, &s.ws.queries_bytes, (size_t)nb * ix->dim * sizeof(float))) return -1;
+                if (stage(s)) return -1;
+                if (range_shard(ix, s, nb, ix->mask_on ? s.ws.qfilter : nullptr, floor_thr.data(), 0, nullptr, counts[i].data(), &list_cap[i],
+                                s.ws.row_thr, reinterpret_cast<const uint32_t *>(s.ws.row_thr + s.n)))
+                    return -1;
+            }
+            keys.clear();
+            if (range_collect(ix, live, nb, counts, list_cap, &keys)) return -1;
+            size_t at = 0;
+            for (uint32_t q = 0; q < nb; ++q) {
+                uint64_t c = 0;
+                for (size_t i = 0; i < live.size(); ++i) c += (uint64_t)counts[i][q];
+                const uint64_t qrow = 0xffffffffull - (ix->row_base + C[b + q]);
+                for (uint64_t j = 0; j < c; ++j, ++at)
+                    entrants.emplace_back((uint32_t)(nk::key_row(keys[at]) - ix->row_base), (keys[at] & 0xffffffff00000000ull) | qrow);
+            }
+        }
+        std::sort(entrants.begin(), entrants.end());
+        // keys of the touched rows' old entries, per shard of the row
+        std::vector<std::vector<uint64_t>> okeys(live.size());
+        std::vector<std::vector<uint32_t>> opr(live.size()), opj(live.size());
+        std::vector<uint32_t> touched;
+        for (size_t i = 0; i < entrants.size(); ++i)
+            if (i == 0 || entrants[i].first != entrants[i - 1].first) touched.push_back(entrants[i].first);
+        std::vector<size_t> shard_of(touched.size());
+        for (size_t t = 0; t < touched.size(); ++t) {
+            const uint32_t r = touched[t];
+            for (size_t i = 0; i < live.size(); ++i)
+                if (r >= live[i]->base - ix->row_base && r < live[i]->base - ix->row_base + live[i]->n) shard_of[t] = i;
+            for (uint32_t j = 0; j < k; ++j) {
+                const uint32_t e = graph_idx[(uint64_t)r * k + j];
+                if (e == GRAPH_PAD) break;
+                opr[shard_of[t]].push_back(r);
+                opj[shard_of[t]].push_back((uint32_t)(e - ix->row_base));
+            }
+        }
+        for (size_t i = 0; i < live.size(); ++i)
+            if (!opr[i].empty() && graph_pair_keys_on(ix, live, *live[i], opr[i], opj[i], &okeys[i])) return -1;
+        // merge: each touched row's old entries and entrants in key space, the best k kept
+        std::vector<size_t> opos(live.size(), 0);
+        std::vector<uint64_t> cand;
+        std::vector<uint32_t> li(k);
+        std::vector<float> ls(k);
+        size_t e0 = 0;
+        for (size_t t = 0; t < touched.size(); ++t) {
+            const uint32_t r = touched[t];
+            cand.clear();
+            const size_t si = shard_of[t];
+            while (opos[si] < opr[si].size() && opr[si][opos[si]] == r) cand.push_back(okeys[si][opos[si]++]);
+            for (; e0 < entrants.size() && entrants[e0].first == r; ++e0) cand.push_back(entrants[e0].second);
+            const size_t take = std::min<size_t>(k, cand.size());
+            std::partial_sort(cand.begin(), cand.begin() + take, cand.end(), std::greater<uint64_t>());
+            for (uint32_t j = 0; j < k; ++j) {
+                if (j < take) decode_key(ix->metric, cand[j], &li[j], &ls[j]);
+                else { li[j] = GRAPH_PAD; ls[j] = 0.0f; }
+            }
+            write_list(r, li.data(), ls.data());
+        }
+    }
+
+    // the rows of R, searched again.  A block with a NaN row among its queries overflows the filter and falls through to the
+    // exact stage, whose arithmetic differs: such a block is searched once more without its NaN rows (lists of -inf scores,
+    // the same on every path), so the other rows get the lists a rebuild gives them in blocks without a NaN query.
+    std::vector<uint32_t> rows;
+    for (uint64_t r = 0; r < N; ++r)
+        if (in_r[r]) rows.push_back((uint32_t)r);
+    std::vector<uint32_t> ri((size_t)std::min<size_t>(rows.size(), SEARCH_ROWS_BLOCK) * k), sub;
+    std::vector<float> rs(ri.size());
+    for (size_t b = 0; b < rows.size(); b += SEARCH_ROWS_BLOCK) {
+        uint32_t nb = (uint32_t)std::min<size_t>(SEARCH_ROWS_BLOCK, rows.size() - b);
+        std::fill(ri.begin(), ri.end(), GRAPH_PAD);
+        std::fill(rs.begin(), rs.end(), 0.0f);
+        uint64_t exact0 = 0, exact1 = 0;
+        if (exact_stage_runs(ix, &exact0) || search_rows_locked(ix, live, rows.data() + b, nb, k, ri.data(), rs.data()) < 0 ||
+            exact_stage_runs(ix, &exact1))
+            return -1;
+        sub.clear();
+        for (uint32_t q = 0; q < nb; ++q) {
+            const bool nan_row = ri[(size_t)q * k] != GRAPH_PAD && rs[(size_t)q * k] == nan_score;
+            if (exact1 == exact0 || nan_row) write_list(rows[b + q], ri.data() + (size_t)q * k, rs.data() + (size_t)q * k);
+            else sub.push_back(rows[b + q]);
+        }
+        if (sub.empty()) continue;
+        nb = (uint32_t)sub.size();
+        if (search_rows_locked(ix, live, sub.data(), nb, k, ri.data(), rs.data()) < 0) return -1;
+        for (uint32_t q = 0; q < nb; ++q) write_list(sub[q], ri.data() + (size_t)q * k, rs.data() + (size_t)q * k);
+    }
+    if (n_lists_changed) *n_lists_changed = n_changed_lists;
+    return ke;
 }
 
 static int single_shard(NkIndex *ix, NkShard **out) {

@@ -32,6 +32,7 @@ struct Workspace {
     uint32_t *sub_rows = nullptr; size_t sub_rows_bytes = 0;  // nk_score_subset: row ids + gathered rows (no per-call alloc)
     void *sub_gather = nullptr;   size_t sub_gather_bytes = 0;
     void *scratch = nullptr;      size_t scratch_bytes = 0;    // k-means routing / group search scratch
+    float *row_thr = nullptr;     size_t row_thr_bytes = 0;    // nk_knn_graph_update: per-row thresholds [n], then keep-mask words
     // cached TMA descriptors (tc_cached_map): re-encoded only when the base pointer or shape changes
     struct MapSlot {
         alignas(64) unsigned char bytes[128];
@@ -85,6 +86,9 @@ struct ScanArgs {
     // filter paths: do not queue the retry / exact stages; the (host-synchronous) caller inspects the status words and
     // calls scan_tensor_filter_tail only when a stage overflowed
     bool defer_tail = false;
+    // range mode only, the reverse scan of nk_knn_graph_update: key-space threshold per local row [n]; a (row, query) pair is
+    // listed only if it reaches both the query's threshold and the row's (tensor-core filters, ROWTHR instantiations)
+    const float *row_thr = nullptr;
 };
 
 // Fused distance + top-k scan on CUDA cores (small Q, any dim / dtype / alignment).
@@ -132,6 +136,11 @@ int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const
 // After range_scan_shard: the shard's survivors, CSR by counts[Q], each query's run sorted -> *keys (host).
 int range_sorted_keys(const DeviceInfo &di, Workspace &ws, cudaStream_t stream, uint32_t Q, const int *counts, uint32_t list_cap,
                       std::vector<uint64_t> *keys, uint64_t *launches);
+
+// nk_knn_graph_update's merge: out[i] = the key K(r, j) under which row j ranks in the k-NN list of local row rl[i] of `rows`,
+// j = row js_row[i] of the widened fp32 block js (device, [.. x dim]), global id jid[i] (warp_pair_score).
+int graph_pair_keys(const void *rows, int dtype, uint32_t dim, int metric, const float *js, const uint32_t *rl, const uint32_t *js_row,
+                    const uint32_t *jid, uint32_t n_pairs, uint64_t *out, cudaStream_t stream);
 
 // Merge n_lists sorted (or unsorted) key lists per query into the best k, sorted descending.
 // key(list l, query q, slot i) = keys[l*list_stride + q*q_stride + i], i < list_len (0 = k).

@@ -7,7 +7,8 @@
 //   2. range_rescore_kernel re-scores every listed pair exactly in fp32 (warp_exact_score, the arithmetic of every filter
 //      path's finish) and keeps those that meet the threshold; the survivor counts come back to the host (size protocol).
 //      The self-join (nk_search_pairs) runs its twin range_rescore_pairs_kernel, which also drops every row at or below the
-//      query's own row;
+//      query's own row; the reverse scan of nk_knn_graph_update runs range_rescore_reverse_kernel, which scores each pair as
+//      the listed row's k-NN list ranks the query (warp_pair_score) and also holds it to the row's threshold;
 //   3. range_compact_kernel packs the survivors of every query into one CSR array, range_sort_runs_kernel sorts runs of
 //      RUN keys per query in shared memory, range_merge_kernel merges sorted runs pairwise until each query's segment is
 //      one run: (score desc, row asc), the order of nk_search.
@@ -40,6 +41,7 @@ struct RescoreParams {
     int *count;            // [Q] survivors (zeroed by the caller)
     uint32_t q_base;       // first query of this launch (grid.y covers at most MAX_GRID_Y queries)
     int rescore;           // 0: CUDA-core lists (already exact): count only
+    const float *row_thr;  // REVERSE: key-space threshold per local row
 };
 
 // The body of range_rescore_kernel: one CTA per (RS_ENTRIES-entry chunk, query); each listed key becomes the exact key if
@@ -47,7 +49,10 @@ struct RescoreParams {
 // PAIRS (nk_search_pairs): query q is stored row pair_first + q (global id), and only rows above it are kept, so each
 // unordered pair of a self-join survives once, under its lower row.  Compiled in only for the pairs kernel: range searches
 // run the code they always ran.
-template <bool PAIRS>
+// REVERSE (nk_knn_graph_update): query q is a new or rewritten stored row and each listed row r an old row whose k-NN list q
+// may enter.  The score is K(r, q), q's score in r's list (warp_pair_score: |q|^2 as a stored row's), and it must reach both
+// the query's threshold (the score floor) and r's own (the score of r's k-th entry).  Tensor-core lists only.
+template <bool PAIRS, bool REVERSE = false>
 __device__ __forceinline__ void rescore_lists(const RescoreParams &p, uint64_t pair_first) {
     extern __shared__ __align__(16) float qs[];  // the query, [dim]
     __shared__ float s_qq;
@@ -66,7 +71,12 @@ __device__ __forceinline__ void rescore_lists(const RescoreParams &p, uint64_t p
     if (p.rescore) {
         for (uint32_t j = tid; j < p.dim; j += RS_THREADS) qs[j] = p.queries[(size_t)q * p.dim + j];
         __syncthreads();
-        if (warp == 0) {  // |q|^2 as filter_finish_kernel computes it
+        if (REVERSE) {
+            if (warp == 0) {
+                const float a = warp_stored_sqnorm(qs, p.dtype, p.dim, lane);
+                if (lane == 0) s_qq = a;
+            }
+        } else if (warp == 0) {  // |q|^2 as filter_finish_kernel computes it
             float a = 0.0f;
             for (uint32_t j = lane; j < p.dim; j += 32) a = fmaf(qs[j], qs[j], a);
 #pragma unroll
@@ -80,8 +90,11 @@ __device__ __forceinline__ void rescore_lists(const RescoreParams &p, uint64_t p
                 if (lane == 0) list[i] = 0ull;
                 continue;
             }
-            const float sc = warp_exact_score(p.rows, p.dtype, (size_t)(grow - (uint32_t)p.row_base), p.dim, qs, s_qq, p.metric, lane);
-            const bool keep = sc > -INFINITY && sc >= thr;
+            const size_t local = (size_t)(grow - (uint32_t)p.row_base);
+            const float sc = REVERSE ? warp_pair_score(p.rows, p.dtype, local, p.dim, qs, s_qq, p.metric, lane)
+                                     : warp_exact_score(p.rows, p.dtype, local, p.dim, qs, s_qq, p.metric, lane);
+            // (the graph keeps -inf scores, as filter_finish_kernel does under no floor)
+            const bool keep = REVERSE ? sc >= thr && sc >= __ldg(p.row_thr + local) : sc > -INFINITY && sc >= thr;
             if (lane == 0) {
                 list[i] = keep ? make_key(sc, grow) : 0ull;
                 mine += keep ? 1 : 0;
@@ -104,6 +117,21 @@ __device__ __forceinline__ void rescore_lists(const RescoreParams &p, uint64_t p
 __global__ void __launch_bounds__(RS_THREADS) range_rescore_kernel(RescoreParams p) { rescore_lists<false>(p, 0); }
 __global__ void __launch_bounds__(RS_THREADS) range_rescore_pairs_kernel(RescoreParams p, uint64_t pair_first) {
     rescore_lists<true>(p, pair_first);
+}
+__global__ void __launch_bounds__(RS_THREADS) range_rescore_reverse_kernel(RescoreParams p) { rescore_lists<false, true>(p, 0); }
+
+// The keys K(r, j) of given pairs (nk_knn_graph_update's merge), one warp per pair: r = local row rl[i] of `rows`, j = row
+// js_row[i] of the widened block js [.. x dim] (global id jid[i]).
+__global__ void __launch_bounds__(RS_THREADS) graph_pair_keys_kernel(const void *rows, int dtype, uint32_t dim, int metric, const float *js,
+                                                                     const uint32_t *rl, const uint32_t *js_row, const uint32_t *jid,
+                                                                     uint32_t n_pairs, uint64_t *out) {
+    const int lane = threadIdx.x & 31;
+    const uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    if (i >= n_pairs) return;  // uniform over the warp
+    const float *j = js + (size_t)js_row[i] * dim;
+    const float jj = warp_stored_sqnorm(j, dtype, dim, lane);
+    const float sc = warp_pair_score(rows, dtype, rl[i], dim, j, jj, metric, lane);
+    if (lane == 0) out[i] = make_key(sc, jid[i]);
 }
 
 // Survivors (non-zero keys) of query q's list -> out[off[q] ..), in list order.
@@ -214,15 +242,18 @@ int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const
     RescoreParams rp{};
     rp.rows = a.rows; rp.dtype = a.dtype; rp.dim = a.dim; rp.row_base = a.row_base; rp.metric = a.metric; rp.queries = a.queries;
     rp.lists = ws.partial; rp.list_cap = list_cap; rp.fill = ws_fill(ws, Q); rp.thr = ws_thr(ws); rp.count = ws_count(ws, Q);
-    rp.rescore = tensor ? 1 : 0;
+    rp.rescore = tensor ? 1 : 0; rp.row_thr = a.row_thr;
+    if (a.row_thr && !tensor) { set_error("internal: the per-row threshold scan runs on the tensor-core filters only"); return -1; }
     const size_t smem = tensor ? (size_t)a.dim * 4 : 0;
-    const void *kern = pair_first ? reinterpret_cast<const void *>(range_rescore_pairs_kernel) : reinterpret_cast<const void *>(range_rescore_kernel);
+    const void *kern = a.row_thr ? reinterpret_cast<const void *>(range_rescore_reverse_kernel)
+                       : pair_first ? reinterpret_cast<const void *>(range_rescore_pairs_kernel) : reinterpret_cast<const void *>(range_rescore_kernel);
     if (smem > 48 * 1024 && tc_ensure_smem(kern, di.device_id, smem)) return -1;
     if (longest > 0)
         for (uint32_t q0 = 0; q0 < Q; q0 += MAX_GRID_Y) {
             rp.q_base = q0;
             const dim3 grid((longest + RS_ENTRIES - 1) / RS_ENTRIES, std::min(MAX_GRID_Y, Q - q0));
-            if (pair_first) range_rescore_pairs_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp, *pair_first);
+            if (a.row_thr) range_rescore_reverse_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp);
+            else if (pair_first) range_rescore_pairs_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp, *pair_first);
             else range_rescore_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp);
             NK_CUDA_OK(cudaGetLastError());
             if (launches) ++*launches;
@@ -275,6 +306,15 @@ int range_sorted_keys(const DeviceInfo &di, Workspace &ws, cudaStream_t stream, 
     }
     NK_CUDA_OK(cudaMemcpyAsync(keys->data(), a, total * 8, cudaMemcpyDeviceToHost, stream));
     NK_CUDA_OK(cudaStreamSynchronize(stream));
+    return 0;
+}
+
+int graph_pair_keys(const void *rows, int dtype, uint32_t dim, int metric, const float *js, const uint32_t *rl, const uint32_t *js_row,
+                    const uint32_t *jid, uint32_t n_pairs, uint64_t *out, cudaStream_t stream) {
+    if (n_pairs == 0) return 0;
+    const uint64_t blocks = ((uint64_t)n_pairs * 32 + RS_THREADS - 1) / RS_THREADS;
+    graph_pair_keys_kernel<<<(unsigned)blocks, RS_THREADS, 0, stream>>>(rows, dtype, dim, metric, js, rl, js_row, jid, n_pairs, out);
+    NK_CUDA_OK(cudaGetLastError());
     return 0;
 }
 

@@ -273,7 +273,8 @@ template <bool FILTER> struct Tf32Est {
 
 // TAGS: filtered search (per-query tag filters in the keep rule); the unfiltered instantiations are TAGS = false.
 // RANGE (filter mode only, nk_search_range): fixed per-query thresholds; full buffers are flushed to the lists, never pruned.
-template <int NT, int QT, bool DUMP, bool TAGS, bool RANGE = false>
+// ROWTHR (with RANGE, the reverse scan of nk_knn_graph_update): a pair must also reach its row's threshold p.row_thr[row].
+template <int NT, int QT, bool DUMP, bool TAGS, bool RANGE = false, bool ROWTHR = false>
 __global__ void __launch_bounds__(tc::THREADS, 1)
 knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_qhi,
                    const __grid_constant__ CUtensorMap map_qlo, tc::Params p) {
@@ -434,8 +435,9 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                     if (!cosine && alive && est.x2 < INFINITY && (lane & 3) == 0) atomicMax(&sh.maxxx, __float_as_uint(est.x2));  // NaN / Inf rows: kept, judged exactly
                     if (euclid) est.mul = 2.0f;
                 }
-                keep_fragment_row<QT, P, FILTER, DUMP && FILTER, TAGS>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau, sh.qn,
-                                                                 sh.cnt, my_cand);
+                keep_fragment_row<QT, P, FILTER, DUMP && FILTER, TAGS, ROWTHR>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau,
+                                                                         sh.qn, sh.cnt, my_cand,
+                                                                         ROWTHR && row < p.n ? __ldg(p.row_thr + row) : -INFINITY);
             }
             // prune any buffer that could overflow during the next tile; the 8 consumer warps prune different
             // queries concurrently with a register-resident warp selection
@@ -847,7 +849,7 @@ tc::Params pass_params(const ScanArgs &a, Workspace &ws, const tc::PassArgs &t) 
     p.cand = ws.cand; p.partial = ws.partial; p.flags = ws.flags; p.debug = tc_debug_flags(); p.mask = a.row_mask;
     p.gtau = reinterpret_cast<uint32_t *>(ws.keys2); p.gcount = reinterpret_cast<int *>(ws.keys2) + (t.Qpad + tc::QT_BIG);
     p.presampled = t.presampled; p.min_score = a.min_score;
-    p.row_tags = a.row_tags; p.qfilter = a.qfilter;
+    p.row_tags = a.row_tags; p.qfilter = a.qfilter; p.row_thr = a.row_thr;
     p.dump_est = t.dump_est; p.dump_bnd = t.dump_bnd; p.dump_ld = t.dump_ld;
     return p;
 }
@@ -901,7 +903,7 @@ struct TcPassArgs : tc::PassArgs {
     const int *only_if;
     bool count_main;
 };
-template <int NT, int QT, bool DUMP = false, bool TAGS = false, bool RANGE = false>
+template <int NT, int QT, bool DUMP = false, bool TAGS = false, bool RANGE = false, bool ROWTHR = false>
 static int launch_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const TcPassArgs &t, uint64_t *launches) {
     using namespace tc;
     const CUtensorMap *map_rows = tc_cached_map(ws, 0, a.rows, a.n, a.dim, 4, (uint32_t)BK, ROWS, (uint64_t)a.dim * 4);
@@ -914,20 +916,25 @@ static int launch_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws,
         set_error("tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;
     }
-    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_tc_kernel<NT, QT, DUMP, TAGS, RANGE>), di.device_id, smem)) return -1;
+    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_tc_kernel<NT, QT, DUMP, TAGS, RANGE, ROWTHR>), di.device_id, smem)) return -1;
     Params p = pass_params(a, ws, t);
     p.nslab = (a.dim + BK - 1) / BK; p.margin_c = t.margin_c; p.only_if = t.only_if;
     // (asynchronous API: the early-exit retry / exact stages are programmatic dependents — their launch overlaps the kernel
     // before them.  Not for the host-synchronous API: measured 5-15 us slower per nk_search, the copy-out behind it waits longer)
-    NK_CUDA_OK(launch_pdl(knn_scan_tc_kernel<NT, QT, DUMP, TAGS, RANGE>, dim3(t.grid), dim3(THREADS), smem, a.stream, t.only_if != nullptr && !a.defer_tail, *map_rows, *map_qhi,
+    NK_CUDA_OK(launch_pdl(knn_scan_tc_kernel<NT, QT, DUMP, TAGS, RANGE, ROWTHR>, dim3(t.grid), dim3(THREADS), smem, a.stream, t.only_if != nullptr && !a.defer_tail, *map_rows, *map_qhi,
                           *map_qlo, p));
     if (launches) ++*launches;
     if (t.count_main && a.main_launches) ++*a.main_launches;
     return 0;
 }
-// Filtered searches (per-query tag filters) run the TAGS instantiation of the same kernel; range searches the RANGE one.
+// Filtered searches (per-query tag filters) run the TAGS instantiation of the same kernel; range searches the RANGE one, and
+// the reverse scan of nk_knn_graph_update (per-row thresholds) the ROWTHR one.
 template <int NT, int QT, bool DUMP = false>
 static int launch_pass(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const TcPassArgs &t, uint64_t *launches) {
+    if constexpr (NT == 1 && !DUMP)
+        if (t.range && a.row_thr)
+            return a.qfilter ? launch_pass_t<NT, QT, false, true, true, true>(di, a, ws, t, launches)
+                             : launch_pass_t<NT, QT, false, false, true, true>(di, a, ws, t, launches);
     if constexpr (NT == 1 && !DUMP)
         if (t.range)
             return a.qfilter ? launch_pass_t<NT, QT, false, true, true>(di, a, ws, t, launches) : launch_pass_t<NT, QT, false, false, true>(di, a, ws, t, launches);

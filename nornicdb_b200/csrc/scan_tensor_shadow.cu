@@ -151,8 +151,9 @@ struct Bf16Est {
 // TAGS: filtered search (per-query tag filters in the keep rule, read through the read-only cache: the shared-memory budget
 // is spent on the rings); the unfiltered instantiations are TAGS = false.  F16: the operands are fp16 (an fp16 corpus
 // scanned in place) instead of bf16.  RANGE (nk_search_range): fixed per-query thresholds; full buffers are flushed to the
-// lists, never pruned, and the end of the launch flushes what is left.
-template <int QT, bool F16, bool DUMP, bool TAGS, bool RANGE>
+// lists, never pruned, and the end of the launch flushes what is left.  ROWTHR (with RANGE, the reverse scan of
+// nk_knn_graph_update): a pair must also reach its row's threshold p.row_thr[row], loaded with the row's norms.
+template <int QT, bool F16, bool DUMP, bool TAGS, bool RANGE, bool ROWTHR = false>
 __global__ void __launch_bounds__(sb::NTHREADS, 1)
 knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_q, tc::Params p) {
     using namespace sb;
@@ -249,7 +250,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             if (eprof) t_a = globaltimer_ns();
             // The epilogue's global inputs, loaded before the MMAs: |x|^2, |dx|^2 and the mask word of this thread's 4
             // rows, and the shared threshold of query etid (it only grows: an earlier value is still a lower bound).
-            float x2[4], d2[4];
+            float x2[4], d2[4], rthr[4];
             uint32_t mword[4];
 #pragma unroll
             for (uint32_t ri = 0; ri < 4; ++ri) {
@@ -258,6 +259,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                 x2[ri] = in ? __ldg(p.xnorm2 + row) : 0.0f;
                 d2[ri] = in && p.dnorm2 ? __ldg(p.dnorm2 + row) : 0.0f;  // 16-bit corpus: no residue
                 mword[ri] = in && p.mask ? __ldg(p.mask + (row >> 5)) : ~0u;
+                rthr[ri] = ROWTHR && in ? __ldg(p.row_thr + row) : -INFINITY;
             }
             const uint32_t etid = tid - EPI_WARP0 * 32;  // consumer thread: one query each (QT <= EPI_NT)
             const uint32_t gt_pre = !RANGE && etid < nq ? __ldcg(p.gtau + q0 + etid) : 0u;
@@ -323,7 +325,8 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                     atomicMax(&sh.max_ra, __float_as_uint(est.ra));
                     if (!cosine) { atomicMax(&sh.max_rb, __float_as_uint(est.rb)); atomicMax(&sh.maxxx, __float_as_uint(est.x2)); }
                 }
-                keep_fragment_row<QT, PB, true, DUMP, TAGS>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau, sh.qn, sh.cnt, my_cand);
+                keep_fragment_row<QT, PB, true, DUMP, TAGS, ROWTHR>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau, sh.qn, sh.cnt,
+                                                                    my_cand, rthr[ri]);
             }
             // prune any buffer that could overflow during the next tile (8 warps, different queries concurrently)
             group_sync(EPI_BAR, EPI_NT);  // every push of this tile is visible
@@ -509,7 +512,7 @@ bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a) {
     return a.dim % 8 == 0;  // 16-bit rows: 16-byte TMA row stride and 128-bit exact re-scoring loads
 }
 
-template <int QT, bool F16, bool DUMP, bool TAGS, bool RANGE = false>
+template <int QT, bool F16, bool DUMP, bool TAGS, bool RANGE = false, bool ROWTHR = false>
 static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
     using namespace sb;
     const bool native = a.shadow_native;  // 16-bit corpus scanned in place: row stride dim * 2, columns past dim read as zero (TMA OOB fill)
@@ -523,10 +526,10 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
         set_error("shadow tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;
     }
-    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, F16, DUMP, TAGS, RANGE>), di.device_id, smem)) return -1;
+    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, F16, DUMP, TAGS, RANGE, ROWTHR>), di.device_id, smem)) return -1;
     tc::Params p = pass_params(a, ws, sp);
     p.nslab = sp.dimpad / BKB; p.qa = sp.qa; p.qb = sp.qb; p.xnorm2 = a.xnorm2; p.dnorm2 = a.dnorm2;
-    knn_scan_shadow_kernel<QT, F16, DUMP, TAGS, RANGE><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
+    knn_scan_shadow_kernel<QT, F16, DUMP, TAGS, RANGE, ROWTHR><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
     NK_CUDA_OK(cudaGetLastError());
     if (launches) ++*launches;
     if (a.main_launches) ++*a.main_launches;
@@ -537,6 +540,13 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
 template <bool F16>
 static int launch_shadow_pass_op(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
     if (sp.dump_est) return launch_shadow_pass_t<64, F16, true, false>(di, a, ws, sp, launches);
+    if (sp.range && a.row_thr) {  // the reverse scan of nk_knn_graph_update
+        if (a.qfilter)
+            return qt == 128 ? launch_shadow_pass_t<128, F16, false, true, true, true>(di, a, ws, sp, launches)
+                             : launch_shadow_pass_t<64, F16, false, true, true, true>(di, a, ws, sp, launches);
+        return qt == 128 ? launch_shadow_pass_t<128, F16, false, false, true, true>(di, a, ws, sp, launches)
+                         : launch_shadow_pass_t<64, F16, false, false, true, true>(di, a, ws, sp, launches);
+    }
     if (sp.range) {
         if (a.qfilter)
             return qt == 128 ? launch_shadow_pass_t<128, F16, false, true, true>(di, a, ws, sp, launches)

@@ -70,6 +70,7 @@ struct Params {
     uint32_t dump_ld;
     const uint64_t *row_tags; // TAGS kernels only: tag word per local row
     const NkFilter *qfilter;  // TAGS kernels only: filter per query [Q], indexed like gtau (absolute query index)
+    const float *row_thr;     // ROWTHR kernels only: key-space threshold per local row (the reverse scan of nk_knn_graph_update)
 };
 
 // What one scan launch covers: queries [q0, q0+nq) in `qgroups` query groups over a `grid`-CTA launch.  Both kernels'
@@ -160,11 +161,12 @@ __device__ __forceinline__ bool row_alive(const Params &p, uint32_t row) {
 // TAGS (filtered searches): a pair whose query does not admit the row's tag never enters a buffer — otherwise the pruned and
 // published thresholds would stop being lower bounds of the FILTERED k-th best score.  Flood tiles place it as key 0; the
 // compare pass loads the row's tag only when some column passed and clears the columns whose filter rejects it.
-template <int QT, int CAP, bool BOUNDED, bool DUMP, bool TAGS = false, class Est>
+// ROWTHR (the reverse scan of nk_knn_graph_update, range mode): a pair must also reach the ROW's threshold rthr.
+template <int QT, int CAP, bool BOUNDED, bool DUMP, bool TAGS = false, bool ROWTHR = false, class Est>
 __device__ __forceinline__ void keep_fragment_row(const Params &p, const Est &est, const float (&acc)[QT / 2], uint32_t r,
                                                   uint32_t row, uint32_t rt, bool alive, bool flood, uint32_t it, uint32_t cbase,
                                                   uint32_t q0, uint32_t nq, const float *tau, const float *qn, int *cnt,
-                                                  uint64_t *cand) {
+                                                  uint64_t *cand, float rthr = -INFINITY) {
     float v[QT / 4];
 #pragma unroll
     for (int jj = 0; jj < QT / 4; ++jj) v[jj] = acc[(jj >> 1) * 4 + r * 2 + (jj & 1)];
@@ -213,7 +215,8 @@ __device__ __forceinline__ void keep_fragment_row(const Params &p, const Est &es
         for (int jj = 0; jj < QT / 4; ++jj) {
             const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
             const float s0 = est.upper(v[jj], qi);
-            pass |= (!(s0 < tau[qi]) && qi < nq) ? (1u << jj) : 0u;
+            const float t = ROWTHR ? fmaxf(tau[qi], rthr) : tau[qi];
+            pass |= (!(s0 < t) && qi < nq) ? (1u << jj) : 0u;
         }
         if (TAGS && pass) {
             const uint64_t tag = __ldg(p.row_tags + row);
@@ -236,7 +239,7 @@ __device__ __forceinline__ void keep_fragment_row(const Params &p, const Est &es
             const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
             float sc = est.upper(val, qi);
             if (sc != sc) sc = BOUNDED ? INFINITY : -INFINITY;
-            if (sc >= tau[qi]) {
+            if (sc >= (ROWTHR ? fmaxf(tau[qi], rthr) : tau[qi])) {
                 int pos = atomicAdd(&cnt[qi], 1);
                 if (pos < CAP) cand[(size_t)qi * CAP + pos] = make_key(sc, (uint32_t)(p.row_base + row));
                 else atomicExch(p.flags + FLAG_FATAL, 1);
@@ -375,6 +378,45 @@ __device__ __forceinline__ float warp_exact_score(const void *rows, int dtype, s
     }
     if (sc != sc) sc = -INFINITY;
     if (xx_out) *xx_out = xx;
+    return sc;
+}
+
+// |x|^2 of a row of `dtype` held widened in fp32 (xs), accumulated as warp_exact_score accumulates a STORED row's: per lane in
+// chunks of 4 (fp32) or 8 (16-bit) elements, then the same butterfly.
+__device__ __forceinline__ float warp_stored_sqnorm(const float *xs, int dtype, uint32_t dim, int lane) {
+    const uint32_t w = dtype == NK_DTYPE_F32 ? 4 : 8;
+    float xx = 0.0f;
+    for (uint32_t c = lane; c < dim / w; c += 32)
+        for (uint32_t e = 0; e < w; ++e) xx = fmaf(xs[c * w + e], xs[c * w + e], xx);
+#pragma unroll
+    for (int o = 16; o; o >>= 1) xx += __shfl_xor_sync(0xffffffffu, xx, o);
+    return xx;
+}
+
+// Key score K(r, j) of the k-NN graph, by one warp: the score nk_search_rows gives stored row j in the list of query = stored
+// row r, whichever of the two is at hand as the widened fp32 copy.  js = row j widened (any memory), jj = its
+// warp_stored_sqnorm; r = local row of `rows`, read here.  The dot product or squared difference accumulates the same
+// products in the same order whichever row warp_exact_score stages as the query (fmaf is commutative in its factors); for
+// cosine the norms are not symmetric: |j|^2 is a stored row's (jj) and |r|^2 a query's, lane-strided as filter_finish_kernel
+// accumulates it.  (warp_exact_score in dot mode returns the raw product with NaN -> -inf, which leaves the cosine quotient's
+// result unchanged: NaN / den and -inf / den both end at -inf.)
+__device__ __forceinline__ float warp_pair_score(const void *rows, int dtype, size_t r, uint32_t dim, const float *js, float jj,
+                                                 int metric, int lane) {
+    const float d = warp_exact_score(rows, dtype, r, dim, js, 1.0f, metric == NK_METRIC_EUCLIDEAN ? metric : NK_METRIC_DOT, lane);
+    if (metric != NK_METRIC_COSINE) return d;
+    float rr = 0.0f;
+    for (uint32_t j = lane; j < dim; j += 32) {
+        float x;
+        if (dtype == NK_DTYPE_F32) x = __ldg(static_cast<const float *>(rows) + r * dim + j);
+        else if (dtype == NK_DTYPE_F16) x = __half2float(static_cast<const __half *>(rows)[r * dim + j]);
+        else x = __uint_as_float((uint32_t)static_cast<const uint16_t *>(rows)[r * dim + j] << 16);
+        rr = fmaf(x, x, rr);
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) rr += __shfl_xor_sync(0xffffffffu, rr, o);
+    const float den = sqrtf(jj * rr);
+    float sc = den > 0.0f ? d / den : 0.0f;
+    if (sc != sc) sc = -INFINITY;
     return sc;
 }
 

@@ -224,8 +224,10 @@ public:
         std::lock_guard<std::mutex> lk(mu_);
         gpuSynced_ = false;
         auto it = idToIndex_.find(nodeID);
-        if (it != idToIndex_.end()) check(nk_index_update_row(ix_, it->second, embedding.data()));
-        else {
+        if (it != idToIndex_.end()) {
+            check(nk_index_update_row(ix_, it->second, embedding.data()));
+            if (it->second < graphRows_) graphChanged_.push_back((uint32_t)it->second);  // SimilarGraph's next update
+        } else {
             check(nk_index_append(ix_, embedding.data(), 1));
             idToIndex_[nodeID] = nodeIDs_.size();
             nodeIDs_.push_back(nodeID);
@@ -241,6 +243,7 @@ public:
         if (it == idToIndex_.end()) return false;
         const uint64_t idx = it->second, last = nodeIDs_.size() - 1;
         gpuSynced_ = false;
+        graphK_ = 0;  // rows renumbered: the next SimilarGraph rebuilds
         check(nk_index_remove_swap(ix_, idx));
         if (idx != last) {
             nodeIDs_[idx] = nodeIDs_[last];
@@ -377,6 +380,46 @@ public:
             }
         return out;
     }
+    // The k-NN graph of every node (SearchSimilar over all ids), kept current across Add / AddBatch: the rows they append or
+    // rewrite go to nk_knn_graph_update instead of a rebuild; the first call, a new k, or any Remove / Deserialize since the
+    // last call rebuild it with nk_search_rows.  Lists in row order (the order of insertion, as swapped by Remove).  The graph
+    // is built and updated on the 16-bit filter path (the TF32 filter if the shape has no 16-bit image), which the update
+    // requires; other searches keep the automatic choice.
+    std::vector<std::vector<SearchResult>> SimilarGraph(int k) {
+        std::lock_guard<std::mutex> lk(mu_);
+        const uint64_t n = nodeIDs_.size();
+        if (n == 0 || k <= 0) return std::vector<std::vector<SearchResult>>(n);
+        int got = -1;
+        for (int path : {NK_PATH_TENSOR_SHADOW, NK_PATH_TENSOR_FILTER}) {
+            check(nk_index_set_path(ix_, path));
+            if (graphK_ == (uint32_t)k) {
+                graphIdx_.resize(n * k, 0xffffffffu);
+                graphScore_.resize(n * k, 0.0f);
+                got = nk_knn_graph_update(ix_, (uint32_t)k, graphRows_, graphChanged_.data(), (uint32_t)graphChanged_.size(),
+                                          graphIdx_.data(), graphScore_.data(), nullptr);
+            } else {
+                std::vector<uint32_t> rows(n);
+                for (uint64_t r = 0; r < n; ++r) rows[r] = (uint32_t)r;
+                graphIdx_.assign(n * k, 0xffffffffu);
+                graphScore_.assign(n * k, 0.0f);
+                got = nk_search_rows(ix_, rows.data(), (uint32_t)n, (uint32_t)k, graphIdx_.data(), graphScore_.data());
+            }
+            if (got >= 0) break;
+        }
+        check(nk_index_set_path(ix_, NK_PATH_AUTO));
+        if (got < 0) { graphK_ = 0; throw cuda::ErrKernelExecution(std::string("gpu: ") + nk_last_error()); }
+        graphK_ = (uint32_t)k;
+        graphRows_ = n;
+        graphChanged_.clear();
+        std::vector<std::vector<SearchResult>> out(n);
+        for (uint64_t r = 0; r < n; ++r)
+            for (int i = 0; i < got; ++i) {
+                const uint32_t j = graphIdx_[r * k + i];
+                const float s = graphScore_[r * k + i];
+                if (j < n) out[r].push_back({nodeIDs_[j], s, 1.0f - s});  // 0xffffffff: fewer other nodes than k
+            }
+        return out;
+    }
     std::vector<SearchResult> ScoreSubset(const std::vector<float> &query, const std::vector<std::string> &ids) {  // gpu.go:1552-1616
         if ((int)query.size() != dims_) throw ErrInvalidDimensions();
         std::lock_guard<std::mutex> lk(mu_);
@@ -437,6 +480,7 @@ public:
         std::lock_guard<std::mutex> lk(mu_);
         check(nk_index_upload(ix_, data.data() + off, count));  // the blob streams straight into device memory
         gpuSynced_ = false;
+        graphK_ = 0;
         nodeIDs_ = ids;
         idToIndex_.clear();
         for (uint32_t i = 0; i < count; ++i) idToIndex_[nodeIDs_[i]] = i;
@@ -449,6 +493,12 @@ private:
     std::vector<std::string> nodeIDs_;
     std::unordered_map<std::string, uint64_t> idToIndex_;
     bool gpuSynced_ = false;
+    // SimilarGraph: the graph of rows [0, graphRows_) for k = graphK_ (0: none), and the old rows rewritten since
+    uint32_t graphK_ = 0;
+    uint64_t graphRows_ = 0;
+    std::vector<uint32_t> graphIdx_;
+    std::vector<float> graphScore_;
+    std::vector<uint32_t> graphChanged_;
     std::mutex mu_;
 };
 

@@ -247,6 +247,41 @@ class KnnIndex:
                                             sc.ctypes.data_as(C.c_void_p)), "nk_search_rows")
         return idx[:, :ke], sc[:, :ke]
 
+    def update_knn_graph(self, idx, score, n_old: int, changed=None, k: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray, int]:
+        """Bring the k-NN graph search_rows(range(n_old), k) returned up to date after rows were appended (rows n_old ..
+        len(self) - 1) and old rows rewritten (`changed`: their ids, repeats allowed) -> (idx, score, lists_changed): what
+        search_rows(every row, k) returns now, k' = min(k, admissible rows) columns, and how many old rows' lists changed.
+        idx / score: [n_old x w]; k defaults to w, and a narrower graph (search_rows returns fewer than k columns while fewer
+        rows are admissible) is padded with 0xffffffff / 0.  Build the graph with the path set (set_path("shadow") or
+        "filter"), keep the metric, the score floor and the old rows' mask bits (set the mask again after append), and rebuild
+        after remove_swap (nk_knn_graph_update)."""
+        idx = np.asarray(idx, dtype=np.uint32)
+        score = np.asarray(score, dtype=np.float32)
+        n_old = int(n_old)
+        if idx.ndim != 2 or score.shape != idx.shape or idx.shape[0] != n_old:
+            raise KnnError("update_knn_graph: idx and score must both be [n_old x w]")
+        k = idx.shape[1] if k is None else int(k)
+        if k < idx.shape[1]:
+            raise KnnError(f"update_knn_graph: k={k} is narrower than the graph ({idx.shape[1]} columns)")
+        n = len(self)
+        if n_old > n:
+            raise KnnError(f"update_knn_graph: n_old={n_old} exceeds the index's {n} rows")
+        ch = np.ascontiguousarray(np.asarray([] if changed is None else changed, dtype=np.int64).reshape(-1))
+        if ch.size and ch.min() < 0:
+            raise KnnError("update_knn_graph: changed row ids must be >= 0")
+        ch = np.ascontiguousarray(ch.astype(np.uint32))
+        if k <= 0 or n == 0:
+            return np.empty((n, 0), np.uint32), np.empty((n, 0), np.float32), 0
+        gi = np.full((n, k), 0xFFFFFFFF, dtype=np.uint32)
+        gs = np.zeros((n, k), dtype=np.float32)
+        gi[:n_old, :idx.shape[1]] = idx
+        gs[:n_old, :idx.shape[1]] = score
+        changed_lists = C.c_uint64(0)
+        ke = _check(self.lib.nk_knn_graph_update(self.ptr, k, n_old, ch.ctypes.data_as(C.c_void_p) if ch.size else None, int(ch.size),
+                                                 gi.ctypes.data_as(C.c_void_p), gs.ctypes.data_as(C.c_void_p), C.byref(changed_lists)),
+                    "nk_knn_graph_update")
+        return gi[:, :ke], gs[:, :ke], int(changed_lists.value)
+
     def search_device(self, q_ptr: int, Q: int, k: int, out_idx_ptr: int, out_score_ptr: int, stream: int = 0) -> int:
         return _check(self.lib.nk_search_device(self.ptr, q_ptr, Q, k, out_idx_ptr, out_score_ptr, stream),
                       "nk_search_device")
