@@ -334,14 +334,36 @@ int nk_search_pairs(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float thre
  * Returns min(k, admissible rows), the entries a list can hold (nk_search_rows' return value), or -1 with nk_last_error,
  * before the arrays are touched, for: the SIMT or 3xTF32 path forced, k == 0 or
  * k > NK_GRAPH_MAX_K, a shape without a filter path, n_old > N, a changed id >= n_old, a graph entry of rows [0, n_old) that is
- * neither an old row nor 0xffffffff, or a null pointer.  nk_index_remove_swap renumbers rows: rebuild after it.
+ * neither an old row nor 0xffffffff, or a null pointer.  nk_index_remove_swap renumbers rows: use nk_knn_graph_remap below.
  * NaN rows: a search block with a NaN query falls through to the exact stage, whose cosine / dot arithmetic differs, so
  * nk_search_rows itself depends on the block there; the guarantee covers the rows of rebuild blocks without a NaN query, and
  * a NaN row's own list holds the right rows with its stage's scores.
- * Synchronous, and it holds the index lock throughout, like nk_search_rows. */
+ * Synchronous, and it holds the index lock throughout, like nk_search_rows.  It is nk_knn_graph_remap with old rows kept at
+ * their ids, changed_rows and rows >= n_old NK_ROW_NEW, done in place. */
 #define NK_GRAPH_MAX_K 191u /* nk_search_rows asks the scan for k + 1; the filter paths stop at 192 */
 int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
                         uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed);
+
+/* Keeps the same graph exact across any mix of nk_index_append, nk_index_update_row and nk_index_remove_swap (which moves the
+ * last row into the removed row's id), given where each current row's contents came from.
+ * src_of_row [N], N = nk_index_rows(ix) now: the old row (relative id < n_old) whose contents current row f holds unchanged
+ * since the graph was built, or NK_ROW_NEW if f holds contents the old graph never saw (appended, rewritten).  Non-NEW values
+ * must be distinct.  Old rows named by no entry are gone (removed, or overwritten by a move or a rewrite).
+ * graph_idx_in / graph_score_in [n_old x k]: what nk_search_rows(rows 0 .. n_old-1, k) returned when the graph was built,
+ * unused slots 0xffffffff / 0.  graph_idx_out / graph_score_out [N x k], which must not overlap the input: on return,
+ * bit for bit, what nk_search_rows(rows 0 .. N-1, k) returns now (order, ties, scores), slots past a list 0xffffffff / 0.
+ * *n_lists_changed (nullable) = how many rows f with src_of_row[f] == f got a list that differs from their old one.
+ * New and moved rows, and the rows at unchanged ids whose old list holds a gone or moved row (a moved row's tie-break key
+ * changes with its id), are searched again; every other row only takes in new or moved rows that beat its k-th entry, found
+ * by one scan of those rows with per-row thresholds.
+ * Preconditions, return value, NaN caveat and refusals: those of nk_knn_graph_update, with "old rows keep their mask bit"
+ * read as "every kept old row has, at its new id, the mask bit it had when the graph was built".  Also refused, before any
+ * output is written: a src_of_row value >= n_old other than NK_ROW_NEW, a repeated non-NEW value, a null src_of_row with
+ * N > 0, and output arrays that overlap the input.  (n_old may exceed N: rows were removed.) */
+#define NK_ROW_NEW 0xffffffffu
+int nk_knn_graph_remap(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row,
+                       const uint32_t *graph_idx_in, const float *graph_score_in,
+                       uint32_t *graph_idx_out, float *graph_score_out, uint64_t *n_lists_changed);
 
 /* Multi-process sharding (one rank per GPU): emit this shard's sorted candidate list as packed 64-bit
  * keys [Q x k] (order-preserving score bits << 32 | ~row index; larger key = better), to be exchanged

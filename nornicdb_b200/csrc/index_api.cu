@@ -1571,31 +1571,31 @@ int nk_search_pairs(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float thre
     return 0;
 }
 
-// ---- k-NN graph update (DESIGN.md §3.5e) -------------------------------------------------------------------------------
-// Rows whose list may have changed in more than one place (the new and rewritten rows, and every old row that lists a
-// rewritten one) are searched again, as nk_search_rows searches them.  For every other old row r only the rows C that are new
-// or rewritten can enter its list: they are scanned as queries over the index with the row's own threshold (the k-th entry's
-// score, or the floor if the list is not full) and the rows searched again masked out, re-scored as r's list scores them
-// (K(r, q), warp_pair_score), and merged with the old entries, whose keys are recomputed the same way.  The graph path
-// (16-bit pass or TF32 filter) is forced for the whole call: every score it makes is warp_exact_score's, whichever block of
-// queries it is computed in.
+// ---- k-NN graph update and remap (DESIGN.md §3.5e) ----------------------------------------------------------------------
+// Current row f holds the contents old row src[f] had when the graph was built (kept: src[f] == f; moved: src[f] != f), or
+// contents the graph never saw (NK_ROW_NEW: appended or rewritten).  Rows whose list may have changed in more than one place
+// are searched again, as nk_search_rows searches them: the new and moved rows, and every kept row whose list holds an old row
+// that no longer sits at its id (gone, moved or rewritten: a moved row's key changes with its id).  Every other kept row r
+// lists only kept rows, so only the rows C that are new or moved can enter its list (a moved row when its new id wins a tie):
+// they are scanned as queries over the index with the row's own threshold (the k-th entry's score, or the floor if the list
+// is not full) and the rows searched again masked out, re-scored as r's list scores them (K(r, q), warp_pair_score), and
+// merged with the old entries, whose keys are recomputed the same way.  The graph path (16-bit pass or TF32 filter) is
+// forced for the whole call: every score it makes is warp_exact_score's, whichever block of queries it is computed in.
 constexpr uint32_t GRAPH_PAD = 0xffffffffu;
 
-// Rows among the first n (relative ids) that pass the row mask.
-static int admissible_below(NkIndex *ix, uint64_t n, uint64_t *out) {
-    uint64_t c = 0;
+// Whether each current row (relative id) passes the row mask -> ok[rows()].
+static int admissible_rows(NkIndex *ix, std::vector<uint8_t> *ok) {
+    ok->assign(ix->rows(), 1);
+    if (!ix->mask_on) return 0;
     for (auto &s : ix->shards) {
+        if (s.n == 0 || !s.mask_on) continue;
         const uint64_t lo = s.base - ix->row_base;
-        if (s.n == 0 || lo >= n) continue;
-        const uint64_t m = std::min<uint64_t>(s.n, n - lo);
-        if (!ix->mask_on || !s.mask_on) { c += m; continue; }
-        std::vector<uint32_t> w((m + 31) / 32);
+        std::vector<uint32_t> w((s.n + 31) / 32);
         NK_CUDA_OK(cudaSetDevice(s.device));
         NK_CUDA_OK(cudaMemcpyAsync(w.data(), s.mask, w.size() * 4, cudaMemcpyDeviceToHost, s.stream));
         NK_CUDA_OK(cudaStreamSynchronize(s.stream));
-        for (uint64_t i = 0; i < m; ++i) c += (w[i >> 5] >> (i & 31)) & 1u;
+        for (uint64_t i = 0; i < s.n; ++i) (*ok)[lo + i] = (w[i >> 5] >> (i & 31)) & 1u;
     }
-    *out = c;
     return 0;
 }
 
@@ -1662,24 +1662,37 @@ static int graph_pair_keys_on(NkIndex *ix, const std::vector<NkShard *> &live, N
     return 0;
 }
 
-int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
-                        uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed) {
-    nk::DeviceGuard _restore_device;
-    if (!ix) { nk::set_error("null index"); return -1; }
-    if (!graph_idx || !graph_score || (n_changed && !changed_rows)) { nk::set_error("null argument"); return -1; }
-    if (k == 0 || k > NK_GRAPH_MAX_K) { nk::set_error("nk_knn_graph_update: k=%u outside [1, %u]", k, NK_GRAPH_MAX_K); return -1; }
-    std::lock_guard<std::mutex> lk(ix->mu);
+// The body of nk_knn_graph_remap and nk_knn_graph_update, the index lock held and the caller's own arguments checked (src
+// is non-null if the index has rows).  gi_in / gs_in [n_old x k] is the old graph, gi / gs [N x k] the output; they are one
+// array only when every old row that is still named keeps its id (nk_knn_graph_update): each row's old list is read before
+// that row is written.  by_id: *n_lists_changed counts every row f < n_old whose list differs from old row f's, else only the
+// kept rows'.  Returns ke, or -1 with nothing written.
+static int knn_graph_remap_locked(NkIndex *ix, const char *what, uint32_t k, uint64_t n_old, const uint32_t *src,
+                                  const uint32_t *gi_in, const float *gs_in, uint32_t *gi, float *gs, bool by_id,
+                                  uint64_t *n_lists_changed) {
+    if (k == 0 || k > NK_GRAPH_MAX_K) { nk::set_error("%s: k=%u outside [1, %u]", what, k, NK_GRAPH_MAX_K); return -1; }
     if (ix->path == NK_PATH_SIMT || ix->path == NK_PATH_TENSOR) {
-        nk::set_error("nk_knn_graph_update: the graph is kept on the filter paths (AUTO, TENSOR_FILTER or TENSOR_SHADOW), not path %d", ix->path);
+        nk::set_error("%s: the graph is kept on the filter paths (AUTO, TENSOR_FILTER or TENSOR_SHADOW), not path %d", what, ix->path);
         return -1;
     }
     const uint64_t N = ix->rows();
-    if (n_old > N) { nk::set_error("nk_knn_graph_update: n_old=%llu exceeds the index's %llu rows", (unsigned long long)n_old, (unsigned long long)N); return -1; }
-    for (uint32_t i = 0; i < n_changed; ++i)
-        if (changed_rows[i] >= n_old) { nk::set_error("nk_knn_graph_update: changed row %u is not an old row (n_old=%llu)", changed_rows[i], (unsigned long long)n_old); return -1; }
+    std::vector<uint32_t> now_at(n_old, NK_ROW_NEW);  // the current id of old row o, NK_ROW_NEW once it is gone
+    for (uint64_t f = 0; f < N; ++f) {
+        const uint32_t o = src[f];
+        if (o == NK_ROW_NEW) continue;
+        if (o >= n_old) {
+            nk::set_error("%s: src_of_row[%llu] = %u is not an old row (n_old=%llu)", what, (unsigned long long)f, o, (unsigned long long)n_old);
+            return -1;
+        }
+        if (now_at[o] != NK_ROW_NEW) {
+            nk::set_error("%s: old row %u is the source of rows %u and %llu", what, o, now_at[o], (unsigned long long)f);
+            return -1;
+        }
+        now_at[o] = (uint32_t)f;
+    }
     for (uint64_t i = 0; i < n_old * k; ++i)
-        if (graph_idx[i] != GRAPH_PAD && (graph_idx[i] < ix->row_base || graph_idx[i] - ix->row_base >= n_old)) {
-            nk::set_error("nk_knn_graph_update: entry %llu of the graph (row %u) is not an old row", (unsigned long long)i, graph_idx[i]);
+        if (gi_in[i] != GRAPH_PAD && (gi_in[i] < ix->row_base || gi_in[i] - ix->row_base >= n_old)) {
+            nk::set_error("%s: entry %llu of the graph (row %u) is not an old row", what, (unsigned long long)i, gi_in[i]);
             return -1;
         }
     const std::vector<NkShard *> live = live_shards(ix);
@@ -1701,46 +1714,63 @@ int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t 
     }
     if (n_lists_changed) *n_lists_changed = 0;
     ix->stats.searches++;
-    NK_RANGE_PUSH("nk_knn_graph_update");
+    NK_RANGE_PUSH(what);
     struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
     ShardOrder order(ix);
     if (order.failed()) return -1;
+    if (gi != gi_in)  // kept rows start from their old lists
+        for (uint64_t f = 0; f < N; ++f)
+            if (src[f] == f) {
+                memcpy(gi + f * k, gi_in + f * k, (size_t)k * 4);
+                memcpy(gs + f * k, gs_in + f * k, (size_t)k * 4);
+            }
 
-    // the rows to search again (R) and the queries of the reverse scan (C: new and rewritten rows)
-    std::vector<uint8_t> in_r(N, 0), changed(n_old, 0);
+    // the rows to search again (R) and the queries of the reverse scan (C: new and moved rows)
+    std::vector<uint8_t> in_r(N, 0);
     std::vector<uint32_t> C;
-    for (uint32_t i = 0; i < n_changed; ++i)
-        if (!changed[changed_rows[i]]) { changed[changed_rows[i]] = 1; in_r[changed_rows[i]] = 1; C.push_back(changed_rows[i]); }
-    for (uint64_t r = n_old; r < N; ++r) { in_r[r] = 1; C.push_back((uint32_t)r); }
+    for (uint64_t f = 0; f < N; ++f)
+        if (src[f] != f) { in_r[f] = 1; C.push_back((uint32_t)f); }
     const uint64_t adm = ix->mask_on ? ix->mask_alive : N;
     const int ke = (int)std::min<uint64_t>(k, adm);
-    if (C.empty()) return ke;
+    if (C.empty() && N == n_old) return ke;  // every row kept at its id
     // nk_search_rows treats a row specially while no more than k rows are admissible (its list drops one of them when the row
-    // itself is not admissible): then every row is searched again
-    uint64_t old_adm = 0;
-    if (admissible_below(ix, n_old, &old_adm)) return -1;
-    const bool all = old_adm <= k || adm <= k;
+    // itself is not admissible): then every row is searched again.  Gone rows have no mask bit any more, so whether that held
+    // when the graph was built is bounded: then every old list was short, and no more than k of the old rows still present
+    // are admissible.  With no row gone this is exactly "no more than k old rows are admissible".
+    bool all = adm <= k;
+    if (!all) {
+        bool full = false;
+        for (uint64_t o = 0; o < n_old && !full; ++o) full = gi_in[o * k + k - 1] != GRAPH_PAD;
+        if (!full) {
+            std::vector<uint8_t> ok;
+            if (admissible_rows(ix, &ok)) return -1;
+            uint64_t still = 0;
+            for (uint64_t f = 0; f < N; ++f) still += src[f] != NK_ROW_NEW && ok[f];
+            all = still <= k;
+        }
+    }
     // A NaN row's list (every score -inf, decoded) comes from the exact stage its search block falls through to: its keys are
     // that stage's, not warp_exact_score's, so such a row is searched again rather than merged.
     const float nan_score = ix->metric == NK_METRIC_EUCLIDEAN ? INFINITY : -INFINITY;
-    for (uint64_t r = 0; r < n_old; ++r) {
-        if (in_r[r]) continue;
-        if (all || (graph_idx[r * k] != GRAPH_PAD && graph_score[r * k] == nan_score)) { in_r[r] = 1; continue; }
+    for (uint64_t r = 0; r < N; ++r) {
+        if (in_r[r]) continue;  // r is kept from here on: r < n_old
+        if (all || (gi_in[r * k] != GRAPH_PAD && gs_in[r * k] == nan_score)) { in_r[r] = 1; continue; }
         for (uint32_t j = 0; j < k; ++j) {
-            const uint32_t e = graph_idx[r * k + j];
-            if (e != GRAPH_PAD && changed[e - ix->row_base]) { in_r[r] = 1; break; }
+            const uint32_t e = gi_in[r * k + j];
+            if (e != GRAPH_PAD && now_at[e - ix->row_base] != e - ix->row_base) { in_r[r] = 1; break; }
         }
     }
     uint64_t n_changed_lists = 0;
     auto write_list = [&](uint64_t r, const uint32_t *li, const float *ls) {
-        if (r < n_old && (memcmp(graph_idx + r * k, li, (size_t)k * 4) || memcmp(graph_score + r * k, ls, (size_t)k * 4))) ++n_changed_lists;
-        memcpy(graph_idx + r * k, li, (size_t)k * 4);
-        memcpy(graph_score + r * k, ls, (size_t)k * 4);
+        if (r < n_old && (by_id || src[r] == r) && (memcmp(gi_in + r * k, li, (size_t)k * 4) || memcmp(gs_in + r * k, ls, (size_t)k * 4)))
+            ++n_changed_lists;
+        memcpy(gi + r * k, li, (size_t)k * 4);
+        memcpy(gs + r * k, ls, (size_t)k * 4);
     };
 
-    // reverse scan + merge for the old rows outside R
+    // reverse scan + merge for the kept rows outside R
     bool reverse = false;
-    for (uint64_t r = 0; r < n_old && !reverse; ++r) reverse = !in_r[r];
+    for (uint64_t r = 0; r < N && !reverse; ++r) reverse = !in_r[r];
     if (reverse) {
         for (NkShard *s : live) {  // per-row thresholds and the mask of rows outside R
             const uint64_t lo = s->base - ix->row_base, words = (s->n + 31) / 32;
@@ -1752,7 +1782,7 @@ int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t 
                 thr[l] = INFINITY;
                 if (in_r[r]) continue;
                 keep[l >> 5] |= 1u << (l & 31);
-                thr[l] = graph_idx[r * k + k - 1] != GRAPH_PAD ? range_key_threshold(ix, graph_score[r * k + k - 1]) : ix->key_floor();
+                thr[l] = gi_in[r * k + k - 1] != GRAPH_PAD ? range_key_threshold(ix, gs_in[r * k + k - 1]) : ix->key_floor();
             }
             NK_CUDA_OK(cudaSetDevice(s->device));
             if (nk::ws_reserve((void **)&s->ws.row_thr, &s->ws.row_thr_bytes, thr.size() * 4)) return -1;
@@ -1763,7 +1793,7 @@ int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t 
         const NkFilter all_rows{0, 0, 0};  // masked-out queries get the filter that admits no row (stage_row_block)
         const uint32_t QB = (uint32_t)std::min<size_t>(C.size(), SEARCH_ROWS_BLOCK);
         const std::vector<uint32_t> floor_thr(QB, nk::ord_bits(ix->key_floor()));
-        std::vector<std::pair<uint32_t, uint64_t>> entrants;  // (old row r, key of the new or rewritten row in r's list)
+        std::vector<std::pair<uint32_t, uint64_t>> entrants;  // (kept row r, key of the new or moved row in r's list)
         std::vector<uint64_t> keys;
         for (size_t b = 0; b < C.size(); b += QB) {
             const uint32_t nb = (uint32_t)std::min<size_t>(QB, C.size() - b);
@@ -1804,7 +1834,7 @@ int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t 
             for (size_t i = 0; i < live.size(); ++i)
                 if (r >= live[i]->base - ix->row_base && r < live[i]->base - ix->row_base + live[i]->n) shard_of[t] = i;
             for (uint32_t j = 0; j < k; ++j) {
-                const uint32_t e = graph_idx[(uint64_t)r * k + j];
+                const uint32_t e = gi_in[(uint64_t)r * k + j];
                 if (e == GRAPH_PAD) break;
                 opr[shard_of[t]].push_back(r);
                 opj[shard_of[t]].push_back((uint32_t)(e - ix->row_base));
@@ -1863,6 +1893,49 @@ int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t 
     }
     if (n_lists_changed) *n_lists_changed = n_changed_lists;
     return ke;
+}
+
+int nk_knn_graph_remap(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row, const uint32_t *graph_idx_in,
+                       const float *graph_score_in, uint32_t *graph_idx_out, float *graph_score_out, uint64_t *n_lists_changed) {
+    nk::DeviceGuard _restore_device;
+    if (!ix) { nk::set_error("null index"); return -1; }
+    if (!graph_idx_out || !graph_score_out || (n_old && (!graph_idx_in || !graph_score_in))) { nk::set_error("null argument"); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
+    const uint64_t N = ix->rows();
+    if (N && !src_of_row) { nk::set_error("null argument"); return -1; }
+    // the output is written while the input is still read: overlapping arrays are refused
+    auto overlap = [](const void *a, size_t na, const void *b, size_t nb) {
+        const uintptr_t pa = (uintptr_t)a, pb = (uintptr_t)b;
+        return na && nb && pa < pb + nb && pb < pa + na;
+    };
+    const size_t in_bytes = (size_t)(n_old * k) * 4, out_bytes = (size_t)(N * k) * 4;
+    for (const void *in : {(const void *)graph_idx_in, (const void *)graph_score_in})
+        for (const void *out : {(const void *)graph_idx_out, (const void *)graph_score_out})
+            if (overlap(in, in_bytes, out, out_bytes)) {
+                nk::set_error("nk_knn_graph_remap: the output arrays overlap the input graph");
+                return -1;
+            }
+    return knn_graph_remap_locked(ix, "nk_knn_graph_remap", k, n_old, src_of_row, graph_idx_in, graph_score_in, graph_idx_out,
+                                  graph_score_out, false, n_lists_changed);
+}
+
+// An old row keeps its id; a rewritten row and every row from n_old on hold contents the graph never saw.  In place.
+int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
+                        uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed) {
+    nk::DeviceGuard _restore_device;
+    if (!ix) { nk::set_error("null index"); return -1; }
+    if (!graph_idx || !graph_score || (n_changed && !changed_rows)) { nk::set_error("null argument"); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
+    const uint64_t N = ix->rows();
+    if (n_old > N) { nk::set_error("nk_knn_graph_update: n_old=%llu exceeds the index's %llu rows", (unsigned long long)n_old, (unsigned long long)N); return -1; }
+    std::vector<uint32_t> src(N, NK_ROW_NEW);
+    for (uint64_t f = 0; f < n_old; ++f) src[f] = (uint32_t)f;
+    for (uint32_t i = 0; i < n_changed; ++i) {
+        if (changed_rows[i] >= n_old) { nk::set_error("nk_knn_graph_update: changed row %u is not an old row (n_old=%llu)", changed_rows[i], (unsigned long long)n_old); return -1; }
+        src[changed_rows[i]] = NK_ROW_NEW;
+    }
+    return knn_graph_remap_locked(ix, "nk_knn_graph_update", k, n_old, src.data(), graph_idx, graph_score, graph_idx, graph_score, true,
+                                  n_lists_changed);
 }
 
 static int single_shard(NkIndex *ix, NkShard **out) {

@@ -226,9 +226,10 @@ public:
         auto it = idToIndex_.find(nodeID);
         if (it != idToIndex_.end()) {
             check(nk_index_update_row(ix_, it->second, embedding.data()));
-            if (it->second < graphRows_) graphChanged_.push_back((uint32_t)it->second);  // SimilarGraph's next update
+            if (graphK_) graphSrc_[it->second] = NK_ROW_NEW;  // contents SimilarGraph's graph never saw
         } else {
             check(nk_index_append(ix_, embedding.data(), 1));
+            if (graphK_) graphSrc_.push_back(NK_ROW_NEW);
             idToIndex_[nodeID] = nodeIDs_.size();
             nodeIDs_.push_back(nodeID);
         }
@@ -243,8 +244,11 @@ public:
         if (it == idToIndex_.end()) return false;
         const uint64_t idx = it->second, last = nodeIDs_.size() - 1;
         gpuSynced_ = false;
-        graphK_ = 0;  // rows renumbered: the next SimilarGraph rebuilds
         check(nk_index_remove_swap(ix_, idx));
+        if (graphK_) {  // the last row's contents move to idx, as on the device
+            graphSrc_[idx] = graphSrc_[last];
+            graphSrc_.pop_back();
+        }
         if (idx != last) {
             nodeIDs_[idx] = nodeIDs_[last];
             idToIndex_[nodeIDs_[idx]] = idx;
@@ -380,29 +384,29 @@ public:
             }
         return out;
     }
-    // The k-NN graph of every node (SearchSimilar over all ids), kept current across Add / AddBatch: the rows they append or
-    // rewrite go to nk_knn_graph_update instead of a rebuild; the first call, a new k, or any Remove / Deserialize since the
-    // last call rebuild it with nk_search_rows.  Lists in row order (the order of insertion, as swapped by Remove).  The graph
-    // is built and updated on the 16-bit filter path (the TF32 filter if the shape has no 16-bit image), which the update
-    // requires; other searches keep the automatic choice.
+    // The k-NN graph of every node (SearchSimilar over all ids), kept current across Add / AddBatch / Remove: the index keeps,
+    // for each row, which row of the last graph its contents came from (swapped by Remove as the device swaps rows), and the
+    // next call hands that map to nk_knn_graph_remap instead of rebuilding.  The first call, a new k, or a Deserialize since
+    // the last call rebuild it with nk_search_rows.  Lists in row order (the order of insertion, as swapped by Remove).  The
+    // graph is built and updated on the 16-bit filter path (the TF32 filter if the shape has no 16-bit image), which the
+    // update requires; other searches keep the automatic choice.
     std::vector<std::vector<SearchResult>> SimilarGraph(int k) {
         std::lock_guard<std::mutex> lk(mu_);
         const uint64_t n = nodeIDs_.size();
         if (n == 0 || k <= 0) return std::vector<std::vector<SearchResult>>(n);
         int got = -1;
+        std::vector<uint32_t> gi(n * k, 0xffffffffu);
+        std::vector<float> gs(n * k, 0.0f);
         for (int path : {NK_PATH_TENSOR_SHADOW, NK_PATH_TENSOR_FILTER}) {
             check(nk_index_set_path(ix_, path));
             if (graphK_ == (uint32_t)k) {
-                graphIdx_.resize(n * k, 0xffffffffu);
-                graphScore_.resize(n * k, 0.0f);
-                got = nk_knn_graph_update(ix_, (uint32_t)k, graphRows_, graphChanged_.data(), (uint32_t)graphChanged_.size(),
-                                          graphIdx_.data(), graphScore_.data(), nullptr);
+                got = nk_knn_graph_remap(ix_, (uint32_t)k, graphRows_, graphSrc_.data(), graphIdx_.data(), graphScore_.data(), gi.data(),
+                                         gs.data(), nullptr);
             } else {
                 std::vector<uint32_t> rows(n);
                 for (uint64_t r = 0; r < n; ++r) rows[r] = (uint32_t)r;
-                graphIdx_.assign(n * k, 0xffffffffu);
-                graphScore_.assign(n * k, 0.0f);
-                got = nk_search_rows(ix_, rows.data(), (uint32_t)n, (uint32_t)k, graphIdx_.data(), graphScore_.data());
+                got = nk_search_rows(ix_, rows.data(), (uint32_t)n, (uint32_t)k, gi.data(), gs.data());
+                if (got >= 0) ++graphRebuilds_;
             }
             if (got >= 0) break;
         }
@@ -410,7 +414,10 @@ public:
         if (got < 0) { graphK_ = 0; throw cuda::ErrKernelExecution(std::string("gpu: ") + nk_last_error()); }
         graphK_ = (uint32_t)k;
         graphRows_ = n;
-        graphChanged_.clear();
+        graphIdx_.swap(gi);
+        graphScore_.swap(gs);
+        graphSrc_.resize(n);
+        for (uint64_t r = 0; r < n; ++r) graphSrc_[r] = (uint32_t)r;
         std::vector<std::vector<SearchResult>> out(n);
         for (uint64_t r = 0; r < n; ++r)
             for (int i = 0; i < got; ++i) {
@@ -441,6 +448,7 @@ public:
     // kept: false after Add / Remove / Deserialize, true after SyncToGPU
     void SyncToGPU() { std::lock_guard<std::mutex> lk(mu_); gpuSynced_ = true; }
     bool IsGPUSynced() const { return gpuSynced_; }
+    uint64_t GraphRebuilds() const { return graphRebuilds_; }  // SimilarGraph calls that searched every row
     int Count() const { return (int)nodeIDs_.size(); }                                   // gpu.go:2225
     bool Has(const std::string &id) const { return idToIndex_.count(id) != 0; }          // gpu.go:2279
     bool Get(const std::string &id, std::vector<float> *out) {                           // gpu.go:2287
@@ -493,12 +501,14 @@ private:
     std::vector<std::string> nodeIDs_;
     std::unordered_map<std::string, uint64_t> idToIndex_;
     bool gpuSynced_ = false;
-    // SimilarGraph: the graph of rows [0, graphRows_) for k = graphK_ (0: none), and the old rows rewritten since
+    // SimilarGraph: the graph of rows [0, graphRows_) for k = graphK_ (0: none), and for each current row the graph row its
+    // contents came from (NK_ROW_NEW: appended or rewritten since); how many times the graph was built from scratch
     uint32_t graphK_ = 0;
     uint64_t graphRows_ = 0;
     std::vector<uint32_t> graphIdx_;
     std::vector<float> graphScore_;
-    std::vector<uint32_t> graphChanged_;
+    std::vector<uint32_t> graphSrc_;
+    uint64_t graphRebuilds_ = 0;
     std::mutex mu_;
 };
 

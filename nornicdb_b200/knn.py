@@ -253,8 +253,8 @@ class KnnIndex:
         search_rows(every row, k) returns now, k' = min(k, admissible rows) columns, and how many old rows' lists changed.
         idx / score: [n_old x w]; k defaults to w, and a narrower graph (search_rows returns fewer than k columns while fewer
         rows are admissible) is padded with 0xffffffff / 0.  Build the graph with the path set (set_path("shadow") or
-        "filter"), keep the metric, the score floor and the old rows' mask bits (set the mask again after append), and rebuild
-        after remove_swap (nk_knn_graph_update)."""
+        "filter"), and keep the metric, the score floor and the old rows' mask bits (set the mask again after append).  After
+        remove_swap, use remap_knn_graph (nk_knn_graph_update)."""
         idx = np.asarray(idx, dtype=np.uint32)
         score = np.asarray(score, dtype=np.float32)
         n_old = int(n_old)
@@ -280,6 +280,43 @@ class KnnIndex:
         ke = _check(self.lib.nk_knn_graph_update(self.ptr, k, n_old, ch.ctypes.data_as(C.c_void_p) if ch.size else None, int(ch.size),
                                                  gi.ctypes.data_as(C.c_void_p), gs.ctypes.data_as(C.c_void_p), C.byref(changed_lists)),
                     "nk_knn_graph_update")
+        return gi[:, :ke], gs[:, :ke], int(changed_lists.value)
+
+    def remap_knn_graph(self, idx, score, n_old: int, src, k: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray, int]:
+        """Bring the k-NN graph search_rows(range(n_old), k) returned up to date after any mix of append, update_row and
+        remove_swap -> (idx, score, lists_changed): what search_rows(every row, k) returns now, k' = min(k, admissible rows)
+        columns, and how many rows that hold their old contents at their old id got a different list.  src: a GraphRowMap
+        that followed the changes, or its src_of_row (one entry per current row: the old row whose contents it holds, or
+        ROW_NEW).  idx / score / k and the preconditions are those of update_knn_graph, the mask bit of a moved row included
+        (nk_knn_graph_remap)."""
+        idx = np.asarray(idx, dtype=np.uint32)
+        score = np.asarray(score, dtype=np.float32)
+        n_old = int(n_old)
+        if idx.ndim != 2 or score.shape != idx.shape or idx.shape[0] != n_old:
+            raise KnnError("remap_knn_graph: idx and score must both be [n_old x w]")
+        k = idx.shape[1] if k is None else int(k)
+        if k < idx.shape[1]:
+            raise KnnError(f"remap_knn_graph: k={k} is narrower than the graph ({idx.shape[1]} columns)")
+        s = np.asarray(src.src_of_row if isinstance(src, GraphRowMap) else src, dtype=np.int64).reshape(-1)
+        n = len(self)
+        if s.size != n:
+            raise KnnError(f"remap_knn_graph: src_of_row has {s.size} entries, the index {n} rows")
+        if s.size and (s.min() < 0 or s.max() > ROW_NEW):
+            raise KnnError("remap_knn_graph: src_of_row entries must be old row ids or ROW_NEW")
+        s = np.ascontiguousarray(s.astype(np.uint32))
+        if k <= 0 or n == 0:
+            return np.empty((n, 0), np.uint32), np.empty((n, 0), np.float32), 0
+        oi = np.full((n_old, k), 0xFFFFFFFF, dtype=np.uint32)
+        osc = np.zeros((n_old, k), dtype=np.float32)
+        oi[:, :idx.shape[1]] = idx
+        osc[:, :idx.shape[1]] = score
+        gi = np.full((n, k), 0xFFFFFFFF, dtype=np.uint32)
+        gs = np.zeros((n, k), dtype=np.float32)
+        changed_lists = C.c_uint64(0)
+        ke = _check(self.lib.nk_knn_graph_remap(self.ptr, k, n_old, s.ctypes.data_as(C.c_void_p), oi.ctypes.data_as(C.c_void_p),
+                                                osc.ctypes.data_as(C.c_void_p), gi.ctypes.data_as(C.c_void_p),
+                                                gs.ctypes.data_as(C.c_void_p), C.byref(changed_lists)),
+                    "nk_knn_graph_remap")
         return gi[:, :ke], gs[:, :ke], int(changed_lists.value)
 
     def search_device(self, q_ptr: int, Q: int, k: int, out_idx_ptr: int, out_score_ptr: int, stream: int = 0) -> int:
@@ -415,6 +452,49 @@ class KnnIndex:
 
 ALL_BITS = 0xFFFFFFFFFFFFFFFF
 ADMIT_NONE = (ALL_BITS, ALL_BITS, 0)  # all_of = none_of = ~0: no row can meet it
+ROW_NEW = 0xFFFFFFFF  # NK_ROW_NEW: a row whose contents a k-NN graph never saw
+
+
+class GraphRowMap:
+    """Where each row of an index came from since a k-NN graph of its first n_old rows was built: follow the index's own
+    append / update_row / remove_swap on it, then hand it (or src_of_row) to KnnIndex.remap_knn_graph.  src_of_row[f] is
+    the old row whose contents row f holds unchanged, or ROW_NEW for appended or rewritten contents."""
+
+    def __init__(self, n_old: int):
+        self.n_old = int(n_old)
+        self._src = np.arange(self.n_old, dtype=np.uint32)
+        self._n = self.n_old
+
+    def __len__(self) -> int:
+        return self._n
+
+    @property
+    def src_of_row(self) -> np.ndarray:
+        return self._src[:self._n].copy()
+
+    def append(self, n_rows: int = 1) -> None:
+        n_rows = int(n_rows)
+        if self._n + n_rows > self._src.size:
+            grown = np.empty(max(self._n + n_rows, 2 * self._src.size), dtype=np.uint32)
+            grown[:self._n] = self._src[:self._n]
+            self._src = grown
+        self._src[self._n:self._n + n_rows] = ROW_NEW
+        self._n += n_rows
+
+    def _row(self, row: int) -> int:
+        row = int(row)
+        if not 0 <= row < self._n:
+            raise KnnError(f"GraphRowMap: row {row} out of range ({self._n} rows)")
+        return row
+
+    def update_row(self, row: int) -> None:
+        self._src[self._row(row)] = ROW_NEW
+
+    def remove_swap(self, row: int) -> None:
+        """nk_index_remove_swap: the last row moves into `row`, and the index shrinks by one"""
+        row = self._row(row)
+        self._src[row] = self._src[self._n - 1]
+        self._n -= 1
 
 
 def as_filters(filters, Q: int) -> np.ndarray:

@@ -1,0 +1,30 @@
+"""The C++ host mirror's k-NN graph (gpu::EmbeddingIndex::SimilarGraph) compiles against the C ABI, and keeps the graph of a
+small index current across Remove, Add and AddBatch on the GPU without rebuilding it."""
+import os
+import subprocess
+
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+@pytest.fixture(scope="module")
+def graph_remove_binary(knn_lib, tmp_path_factory):
+    src = os.path.join(ROOT, "tests", "cpp", "graph_remove_mirror_test.cpp")
+    lib = os.path.join(ROOT, "nornicdb_b200", "libnornic_knn.so")
+    out = str(tmp_path_factory.mktemp("cpp") / "graph_remove_mirror_test")
+    subprocess.run(["/usr/bin/g++", "-std=c++17", "-O1", "-Wall", "-I", ROOT, src, "-L", os.path.dirname(lib), "-lnornic_knn",
+                    f"-Wl,-rpath,{os.path.dirname(lib)}", "-lpthread", "-o", out], check=True, cwd=ROOT)
+    return out
+
+
+def test_graph_remove_mirror_compiles(graph_remove_binary):
+    out = subprocess.run([graph_remove_binary, "--no-gpu"], capture_output=True, text=True)
+    assert out.returncode == 0 and "graph remove mirror ok" in out.stdout
+
+
+@pytest.mark.gpu
+def test_graph_remove_mirror_on_gpu(graph_remove_binary):
+    out = subprocess.run([graph_remove_binary], capture_output=True, text=True, timeout=120)
+    assert out.returncode == 0, out.stdout + out.stderr
+    assert "graph remove mirror ok" in out.stdout
