@@ -274,6 +274,16 @@ int nk_search_filtered_device(NkIndex *ix, const float *queries_dev, const NkFil
  * Equals nk_search(the rows read back and widened, k + 1) with the query's own row removed from each list (or, where it is
  * not in the list, the last entry), bit for bit, for the same blocks of 1024 queries. */
 int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score);
+/* nk_search_rows with one tag filter per query (filters_host [Q], NULL = none: then nk_search_rows bit for bit), e.g. "the k
+ * nearest rows of the same collection".  Query q gets the top k of the rows other than rows_host[q] that filters_host[q]
+ * admits (nk_search_filtered's predicate), with the row mask and the score floor as in nk_search_rows.  The query row itself
+ * may be inadmissible (masked out, or refused by its own filter).  Return value, padding, blocks of 1024, devices, k limit,
+ * locking and refusals: those of nk_search_rows.
+ * Equals nk_search_filtered(the rows read back and widened, filters_host, k' = min(k + 1, rows passing the row mask)) with the
+ * query's own row removed from each list (or, where it is not in the list, the last entry), bit for bit, for the same blocks
+ * of 1024 queries. */
+int nk_search_rows_filtered(NkIndex *ix, const uint32_t *rows_host, const NkFilter *filters_host, uint32_t Q, uint32_t k,
+                            uint32_t *out_idx, float *out_score);
 
 /* ---- Range search ------------------------------------------------------------------------------------------------------
  * Every admissible row whose score reaches the query's threshold (Cypher WHERE vector.similarity.* >= t, auto-links above a
@@ -364,6 +374,23 @@ int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t 
 int nk_knn_graph_remap(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row,
                        const uint32_t *graph_idx_in, const float *graph_score_in,
                        uint32_t *graph_idx_out, float *graph_score_out, uint64_t *n_lists_changed);
+
+/* Filtered k-NN graphs: one graph per collection (or any tag predicate) of a shared index.  filters_host [N], N =
+ * nk_index_rows(ix) now: the filter of each current row's list (NULL = none: then nk_knn_graph_update / nk_knn_graph_remap bit
+ * for bit).  The graph is what nk_search_rows_filtered(rows 0 .. N-1, filters_host, k) returns: row r's list holds only rows
+ * r's filter admits.  On entry the old graph is what nk_search_rows_filtered(rows 0 .. n_old-1, the filters of that time, k)
+ * returned.  Arguments, return value, refusals and every other precondition: those of the unfiltered call.
+ * One more precondition (not checked): every kept row (nk_knn_graph_update_filtered: an old row not in changed_rows;
+ * nk_knn_graph_remap_filtered: src_of_row[f] != NK_ROW_NEW) has the tag and the filter its contents had when the graph was
+ * built.  Report a row whose tag or filter changed as new contents, exactly like a rewritten row (a changed row, or
+ * NK_ROW_NEW): lists that held it are searched again and every other list is offered it.
+ * Each list holds only rows its own filter admits: rows searched again are searched with their own filter, and the scan of
+ * new and moved rows also holds each pair (row r, new row c) to r's filter admitting c's tag, inside the scan kernel. */
+int nk_knn_graph_update_filtered(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
+                                 const NkFilter *filters_host, uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed);
+int nk_knn_graph_remap_filtered(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row, const NkFilter *filters_host,
+                                const uint32_t *graph_idx_in, const float *graph_score_in, uint32_t *graph_idx_out,
+                                float *graph_score_out, uint64_t *n_lists_changed);
 
 /* Multi-process sharding (one rank per GPU): emit this shard's sorted candidate list as packed 64-bit
  * keys [Q x k] (order-preserving score bits << 32 | ~row index; larger key = better), to be exchanged

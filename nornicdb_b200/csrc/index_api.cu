@@ -1290,10 +1290,10 @@ static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, cons
     return 0;
 }
 
-// The body of nk_search_rows, the index lock held and the ids checked: returns ke, the entries written per query (the rest of
-// each k-wide output row is left as it is).
-static int search_rows_locked(NkIndex *ix, const std::vector<NkShard *> &live, const uint32_t *rows_host, uint32_t Q, uint32_t k,
-                              uint32_t *out_idx, float *out_score) {
+// The body of nk_search_rows and nk_search_rows_filtered (filters_host [Q] or nullptr), the index lock held and the ids
+// checked: returns ke, the entries written per query (the rest of each k-wide output row is left as it is).
+static int search_rows_locked(NkIndex *ix, const std::vector<NkShard *> &live, const uint32_t *rows_host, const NkFilter *filters_host,
+                              uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
     const uint64_t N = ix->mask_on ? ix->mask_alive : ix->rows();  // rows that can be returned
     const uint32_t kk = (uint32_t)std::min<uint64_t>((uint64_t)k + 1, N);  // asked of the scan
     const uint32_t ke = (uint32_t)std::min<uint64_t>(k, N);                // returned
@@ -1305,7 +1305,7 @@ static int search_rows_locked(NkIndex *ix, const std::vector<NkShard *> &live, c
         const uint32_t *ids = rows_host + b;
         StageQueries stage;
         if (stage_row_block(ix, live, ids, nb, nullptr, &stage)) return -1;
-        if (search_live(ix, live, stage, nullptr, nb, kk, kk, bidx.data(), bsc.data()) < 0) return -1;
+        if (search_live(ix, live, stage, filters_host ? filters_host + b : nullptr, nb, kk, kk, bidx.data(), bsc.data()) < 0) return -1;
         for (uint32_t q = 0; q < nb; ++q) {
             const uint32_t self = (uint32_t)(ix->row_base + ids[q]);
             const uint32_t *ri = bidx.data() + (size_t)q * kk;
@@ -1324,27 +1324,38 @@ static int search_rows_locked(NkIndex *ix, const std::vector<NkShard *> &live, c
     return (int)ke;
 }
 
-int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
+// nk_search_rows / nk_search_rows_filtered: filters_host == nullptr is plain nk_search_rows.
+static int search_rows_host(NkIndex *ix, const char *what, const uint32_t *rows_host, const NkFilter *filters_host, uint32_t Q, uint32_t k,
+                            uint32_t *out_idx, float *out_score) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
     if (Q && (!rows_host || !out_idx || !out_score)) { nk::set_error("null argument"); return -1; }
-    if (k > NK_MAX_K_TOTAL - 1) { nk::set_error("nk_search_rows: k=%u exceeds NK_MAX_K_TOTAL - 1 = %u", k, NK_MAX_K_TOTAL - 1); return -1; }
+    if (k > NK_MAX_K_TOTAL - 1) { nk::set_error("%s: k=%u exceeds NK_MAX_K_TOTAL - 1 = %u", what, k, NK_MAX_K_TOTAL - 1); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
     const uint64_t total = ix->rows();
     const uint64_t N = ix->mask_on ? ix->mask_alive : total;  // rows that can be returned
     if (k == 0 || N == 0 || Q == 0) return 0;
     for (uint32_t q = 0; q < Q; ++q)
         if (rows_host[q] >= total) {
-            nk::set_error("nk_search_rows: row %u (query %u) out of range, index has %llu rows", rows_host[q], q, (unsigned long long)total);
+            nk::set_error("%s: row %u (query %u) out of range, index has %llu rows", what, rows_host[q], q, (unsigned long long)total);
             return -1;
         }
     ix->stats.searches++;
     ix->stats.queries += Q;
-    NK_RANGE_PUSH("nk_search_rows");
+    NK_RANGE_PUSH(what);
     struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
     ShardOrder order(ix);
     if (order.failed()) return -1;
-    return search_rows_locked(ix, live_shards(ix), rows_host, Q, k, out_idx, out_score);
+    return search_rows_locked(ix, live_shards(ix), rows_host, filters_host, Q, k, out_idx, out_score);
+}
+
+int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
+    return search_rows_host(ix, "nk_search_rows", rows_host, nullptr, Q, k, out_idx, out_score);
+}
+
+int nk_search_rows_filtered(NkIndex *ix, const uint32_t *rows_host, const NkFilter *filters_host, uint32_t Q, uint32_t k,
+                            uint32_t *out_idx, float *out_score) {
+    return search_rows_host(ix, "nk_search_rows_filtered", rows_host, filters_host, Q, k, out_idx, out_score);
 }
 
 // ---- range search ---------------------------------------------------------------------------------------------------
@@ -1375,15 +1386,17 @@ static float range_key_threshold(const NkIndex *ix, float t) {
 // 16-byte alignment are those of the shard; the window gets its own TMA maps (tc_cached_map keys on the base).  pair_first:
 // see range_scan_shard.
 // row_thr (nk_knn_graph_update's reverse scan, device [s.n]): per-row thresholds, and row_keep (device mask words) takes the
-// place of the row mask: it selects the rows whose lists are updated, not the rows that may be returned.
+// place of the row mask: it selects the rows whose lists are updated, not the rows that may be returned.  row_filter (a
+// filtered graph, device [s.n]) and qtags (device [Q]): a pair (row, query) is listed only if the row's filter admits the
+// query's tag; qfilter must be set then.
 static int range_shard(NkIndex *ix, NkShard &s, uint32_t Q, const NkFilter *qfilter, const uint32_t *thr, uint64_t from,
                        const uint64_t *pair_first, int *counts, uint32_t *list_cap, const float *row_thr = nullptr,
-                       const uint32_t *row_keep = nullptr) {
+                       const uint32_t *row_keep = nullptr, const NkFilter *row_filter = nullptr, const uint64_t *qtags = nullptr) {
     // Paths: the 16-bit and TF32 filters with fixed thresholds, or the CUDA-core scan.
     nk::ScanArgs a = shard_scan_args(ix, s, s.ws.queries, Q, 1, s.stream, qfilter);
     const int use = plan_path(ix, s, true, &a);
     if (use < 0) return -1;
-    if (row_thr) { a.row_thr = row_thr; a.row_mask = row_keep; }
+    if (row_thr) { a.row_thr = row_thr; a.row_mask = row_keep; a.row_filter = row_filter; a.qtags = qtags; }
     if (from) {
         a.rows = static_cast<const char *>(a.rows) + from * ix->dim * ix->esz();
         a.n = (uint32_t)(s.n - from);
@@ -1599,6 +1612,19 @@ static int admissible_rows(NkIndex *ix, std::vector<uint8_t> *ok) {
     return 0;
 }
 
+// The tag word of each current row (relative id) -> tags[rows()]; 0 where a shard has no tags.
+static int host_row_tags(NkIndex *ix, std::vector<uint64_t> *tags) {
+    tags->assign(ix->rows(), 0ull);
+    for (auto &s : ix->shards) {
+        if (s.n == 0 || !s.tags_on) continue;
+        NK_CUDA_OK(cudaSetDevice(s.device));
+        NK_CUDA_OK(cudaMemcpyAsync(tags->data() + (s.base - ix->row_base), s.tags, s.n * 8, cudaMemcpyDeviceToHost, s.stream));
+        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+        ix->stats.bytes_d2h += s.n * 8;
+    }
+    return 0;
+}
+
 // Searches that fell through to the exact stage so far, all shards (cumulative status word FLAG_N_EXACT).
 static int exact_stage_runs(NkIndex *ix, uint64_t *out) {
     uint64_t c = 0;
@@ -1666,8 +1692,11 @@ static int graph_pair_keys_on(NkIndex *ix, const std::vector<NkShard *> &live, N
 // is non-null if the index has rows).  gi_in / gs_in [n_old x k] is the old graph, gi / gs [N x k] the output; they are one
 // array only when every old row that is still named keeps its id (nk_knn_graph_update): each row's old list is read before
 // that row is written.  by_id: *n_lists_changed counts every row f < n_old whose list differs from old row f's, else only the
-// kept rows'.  Returns ke, or -1 with nothing written.
-static int knn_graph_remap_locked(NkIndex *ix, const char *what, uint32_t k, uint64_t n_old, const uint32_t *src,
+// kept rows'.  filters [N] (nullptr: none): the graph of nk_search_rows_filtered, each row's list bounded by its own filter.
+// A kept row has the tag and the filter it had when the graph was built (the caller reports any other row as new), so the
+// rows searched again are the same; they are searched with their own filters, and the reverse scan also holds each pair
+// (r, c) to r's filter admitting c's tag.  Returns ke, or -1 with nothing written.
+static int knn_graph_remap_locked(NkIndex *ix, const char *what, uint32_t k, uint64_t n_old, const uint32_t *src, const NkFilter *filters,
                                   const uint32_t *gi_in, const float *gs_in, uint32_t *gi, float *gs, bool by_id,
                                   uint64_t *n_lists_changed) {
     if (k == 0 || k > NK_GRAPH_MAX_K) { nk::set_error("%s: k=%u outside [1, %u]", what, k, NK_GRAPH_MAX_K); return -1; }
@@ -1737,6 +1766,10 @@ static int knn_graph_remap_locked(NkIndex *ix, const char *what, uint32_t k, uin
     // itself is not admissible): then every row is searched again.  Gone rows have no mask bit any more, so whether that held
     // when the graph was built is bounded: then every old list was short, and no more than k of the old rows still present
     // are admissible.  With no row gone this is exactly "no more than k old rows are admissible".
+    // Filters leave this rule as it is: the scan still asks for k' = min(k + 1, rows passing the mask), so with more than k
+    // such rows the last slot a row drops is the (k+1)-th of its filtered order, and a list shorter than k holds every other
+    // row its filter and the floor admit — its threshold is the floor, as for an unfiltered short list.  A list that is
+    // full implies more than k rows passing the mask, filtered or not.
     bool all = adm <= k;
     if (!all) {
         bool full = false;
@@ -1787,9 +1820,19 @@ static int knn_graph_remap_locked(NkIndex *ix, const char *what, uint32_t k, uin
             NK_CUDA_OK(cudaSetDevice(s->device));
             if (nk::ws_reserve((void **)&s->ws.row_thr, &s->ws.row_thr_bytes, thr.size() * 4)) return -1;
             NK_CUDA_OK(cudaMemcpyAsync(s->ws.row_thr, thr.data(), thr.size() * 4, cudaMemcpyHostToDevice, s->stream));
+            if (filters) {  // each row's own filter, for the row side of the scan
+                if (nk::ws_reserve((void **)&s->ws.row_filter, &s->ws.row_filter_bytes, s->n * sizeof(NkFilter))) return -1;
+                NK_CUDA_OK(cudaMemcpyAsync(s->ws.row_filter, filters + lo, s->n * sizeof(NkFilter), cudaMemcpyHostToDevice, s->stream));
+                ix->stats.bytes_h2d += s->n * sizeof(NkFilter);
+            }
             NK_CUDA_OK(cudaStreamSynchronize(s->stream));  // thr is pageable and goes out of scope
             ix->stats.bytes_h2d += thr.size() * 4;
         }
+        // a filtered graph's queries also carry their tags, and always a per-query filter (the row-filtered scan is a mode
+        // of the tag-filtered one)
+        std::vector<uint64_t> tags, qtags;
+        if (filters && host_row_tags(ix, &tags)) return -1;
+        const bool qfilt = ix->mask_on || filters;
         const NkFilter all_rows{0, 0, 0};  // masked-out queries get the filter that admits no row (stage_row_block)
         const uint32_t QB = (uint32_t)std::min<size_t>(C.size(), SEARCH_ROWS_BLOCK);
         const std::vector<uint32_t> floor_thr(QB, nk::ord_bits(ix->key_floor()));
@@ -1798,7 +1841,11 @@ static int knn_graph_remap_locked(NkIndex *ix, const char *what, uint32_t k, uin
         for (size_t b = 0; b < C.size(); b += QB) {
             const uint32_t nb = (uint32_t)std::min<size_t>(QB, C.size() - b);
             StageQueries stage;
-            if (stage_row_block(ix, live, C.data() + b, nb, ix->mask_on ? &all_rows : nullptr, &stage)) return -1;
+            if (stage_row_block(ix, live, C.data() + b, nb, qfilt ? &all_rows : nullptr, &stage)) return -1;
+            if (filters) {
+                qtags.resize(nb);
+                for (uint32_t q = 0; q < nb; ++q) qtags[q] = tags[C[b + q]];
+            }
             std::vector<std::vector<int>> counts(live.size(), std::vector<int>(nb, 0));
             std::vector<uint32_t> list_cap(live.size());
             for (size_t i = 0; i < live.size(); ++i) {
@@ -1806,8 +1853,14 @@ static int knn_graph_remap_locked(NkIndex *ix, const char *what, uint32_t k, uin
                 NK_CUDA_OK(cudaSetDevice(s.device));
                 if (nk::ws_reserve((void **)&s.ws.queries, &s.ws.queries_bytes, (size_t)nb * ix->dim * sizeof(float))) return -1;
                 if (stage(s)) return -1;
-                if (range_shard(ix, s, nb, ix->mask_on ? s.ws.qfilter : nullptr, floor_thr.data(), 0, nullptr, counts[i].data(), &list_cap[i],
-                                s.ws.row_thr, reinterpret_cast<const uint32_t *>(s.ws.row_thr + s.n)))
+                if (filters) {  // read by the scan before range_shard's first synchronisation
+                    if (nk::ws_reserve((void **)&s.ws.qtags, &s.ws.qtags_bytes, (size_t)nb * 8)) return -1;
+                    NK_CUDA_OK(cudaMemcpyAsync(s.ws.qtags, qtags.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, s.stream));
+                    ix->stats.bytes_h2d += (uint64_t)nb * 8;
+                }
+                if (range_shard(ix, s, nb, qfilt ? s.ws.qfilter : nullptr, floor_thr.data(), 0, nullptr, counts[i].data(), &list_cap[i],
+                                s.ws.row_thr, reinterpret_cast<const uint32_t *>(s.ws.row_thr + s.n), filters ? s.ws.row_filter : nullptr,
+                                filters ? s.ws.qtags : nullptr))
                     return -1;
             }
             keys.clear();
@@ -1872,12 +1925,20 @@ static int knn_graph_remap_locked(NkIndex *ix, const char *what, uint32_t k, uin
         if (in_r[r]) rows.push_back((uint32_t)r);
     std::vector<uint32_t> ri((size_t)std::min<size_t>(rows.size(), SEARCH_ROWS_BLOCK) * k), sub;
     std::vector<float> rs(ri.size());
+    std::vector<NkFilter> rf;  // filters: the block's rows' own
+    auto row_filters = [&](const uint32_t *ids, uint32_t nb) -> const NkFilter * {
+        if (!filters) return nullptr;
+        rf.resize(nb);
+        for (uint32_t q = 0; q < nb; ++q) rf[q] = filters[ids[q]];
+        return rf.data();
+    };
     for (size_t b = 0; b < rows.size(); b += SEARCH_ROWS_BLOCK) {
         uint32_t nb = (uint32_t)std::min<size_t>(SEARCH_ROWS_BLOCK, rows.size() - b);
         std::fill(ri.begin(), ri.end(), GRAPH_PAD);
         std::fill(rs.begin(), rs.end(), 0.0f);
         uint64_t exact0 = 0, exact1 = 0;
-        if (exact_stage_runs(ix, &exact0) || search_rows_locked(ix, live, rows.data() + b, nb, k, ri.data(), rs.data()) < 0 ||
+        if (exact_stage_runs(ix, &exact0) ||
+            search_rows_locked(ix, live, rows.data() + b, row_filters(rows.data() + b, nb), nb, k, ri.data(), rs.data()) < 0 ||
             exact_stage_runs(ix, &exact1))
             return -1;
         sub.clear();
@@ -1888,15 +1949,16 @@ static int knn_graph_remap_locked(NkIndex *ix, const char *what, uint32_t k, uin
         }
         if (sub.empty()) continue;
         nb = (uint32_t)sub.size();
-        if (search_rows_locked(ix, live, sub.data(), nb, k, ri.data(), rs.data()) < 0) return -1;
+        if (search_rows_locked(ix, live, sub.data(), row_filters(sub.data(), nb), nb, k, ri.data(), rs.data()) < 0) return -1;
         for (uint32_t q = 0; q < nb; ++q) write_list(sub[q], ri.data() + (size_t)q * k, rs.data() + (size_t)q * k);
     }
     if (n_lists_changed) *n_lists_changed = n_changed_lists;
     return ke;
 }
 
-int nk_knn_graph_remap(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row, const uint32_t *graph_idx_in,
-                       const float *graph_score_in, uint32_t *graph_idx_out, float *graph_score_out, uint64_t *n_lists_changed) {
+static int knn_graph_remap_host(NkIndex *ix, const char *what, uint32_t k, uint64_t n_old, const uint32_t *src_of_row,
+                                const NkFilter *filters, const uint32_t *graph_idx_in, const float *graph_score_in,
+                                uint32_t *graph_idx_out, float *graph_score_out, uint64_t *n_lists_changed) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
     if (!graph_idx_out || !graph_score_out || (n_old && (!graph_idx_in || !graph_score_in))) { nk::set_error("null argument"); return -1; }
@@ -1912,30 +1974,55 @@ int nk_knn_graph_remap(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *
     for (const void *in : {(const void *)graph_idx_in, (const void *)graph_score_in})
         for (const void *out : {(const void *)graph_idx_out, (const void *)graph_score_out})
             if (overlap(in, in_bytes, out, out_bytes)) {
-                nk::set_error("nk_knn_graph_remap: the output arrays overlap the input graph");
+                nk::set_error("%s: the output arrays overlap the input graph", what);
                 return -1;
             }
-    return knn_graph_remap_locked(ix, "nk_knn_graph_remap", k, n_old, src_of_row, graph_idx_in, graph_score_in, graph_idx_out,
-                                  graph_score_out, false, n_lists_changed);
+    return knn_graph_remap_locked(ix, what, k, n_old, src_of_row, filters, graph_idx_in, graph_score_in, graph_idx_out, graph_score_out,
+                                  false, n_lists_changed);
+}
+
+int nk_knn_graph_remap(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row, const uint32_t *graph_idx_in,
+                       const float *graph_score_in, uint32_t *graph_idx_out, float *graph_score_out, uint64_t *n_lists_changed) {
+    return knn_graph_remap_host(ix, "nk_knn_graph_remap", k, n_old, src_of_row, nullptr, graph_idx_in, graph_score_in, graph_idx_out,
+                                graph_score_out, n_lists_changed);
+}
+
+int nk_knn_graph_remap_filtered(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row, const NkFilter *filters_host,
+                                const uint32_t *graph_idx_in, const float *graph_score_in, uint32_t *graph_idx_out,
+                                float *graph_score_out, uint64_t *n_lists_changed) {
+    return knn_graph_remap_host(ix, "nk_knn_graph_remap_filtered", k, n_old, src_of_row, filters_host, graph_idx_in, graph_score_in,
+                                graph_idx_out, graph_score_out, n_lists_changed);
 }
 
 // An old row keeps its id; a rewritten row and every row from n_old on hold contents the graph never saw.  In place.
-int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
-                        uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed) {
+static int knn_graph_update_host(NkIndex *ix, const char *what, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
+                                 const NkFilter *filters, uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
     if (!graph_idx || !graph_score || (n_changed && !changed_rows)) { nk::set_error("null argument"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
     const uint64_t N = ix->rows();
-    if (n_old > N) { nk::set_error("nk_knn_graph_update: n_old=%llu exceeds the index's %llu rows", (unsigned long long)n_old, (unsigned long long)N); return -1; }
+    if (n_old > N) { nk::set_error("%s: n_old=%llu exceeds the index's %llu rows", what, (unsigned long long)n_old, (unsigned long long)N); return -1; }
     std::vector<uint32_t> src(N, NK_ROW_NEW);
     for (uint64_t f = 0; f < n_old; ++f) src[f] = (uint32_t)f;
     for (uint32_t i = 0; i < n_changed; ++i) {
-        if (changed_rows[i] >= n_old) { nk::set_error("nk_knn_graph_update: changed row %u is not an old row (n_old=%llu)", changed_rows[i], (unsigned long long)n_old); return -1; }
+        if (changed_rows[i] >= n_old) { nk::set_error("%s: changed row %u is not an old row (n_old=%llu)", what, changed_rows[i], (unsigned long long)n_old); return -1; }
         src[changed_rows[i]] = NK_ROW_NEW;
     }
-    return knn_graph_remap_locked(ix, "nk_knn_graph_update", k, n_old, src.data(), graph_idx, graph_score, graph_idx, graph_score, true,
+    return knn_graph_remap_locked(ix, what, k, n_old, src.data(), filters, graph_idx, graph_score, graph_idx, graph_score, true,
                                   n_lists_changed);
+}
+
+int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
+                        uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed) {
+    return knn_graph_update_host(ix, "nk_knn_graph_update", k, n_old, changed_rows, n_changed, nullptr, graph_idx, graph_score,
+                                 n_lists_changed);
+}
+
+int nk_knn_graph_update_filtered(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
+                                 const NkFilter *filters_host, uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed) {
+    return knn_graph_update_host(ix, "nk_knn_graph_update_filtered", k, n_old, changed_rows, n_changed, filters_host, graph_idx,
+                                 graph_score, n_lists_changed);
 }
 
 static int single_shard(NkIndex *ix, NkShard **out) {

@@ -33,6 +33,8 @@ struct Workspace {
     void *sub_gather = nullptr;   size_t sub_gather_bytes = 0;
     void *scratch = nullptr;      size_t scratch_bytes = 0;    // k-means routing / group search scratch
     float *row_thr = nullptr;     size_t row_thr_bytes = 0;    // nk_knn_graph_update: per-row thresholds [n], then keep-mask words
+    NkFilter *row_filter = nullptr; size_t row_filter_bytes = 0;  // filtered graph update: each row's own filter [n]
+    uint64_t *qtags = nullptr;    size_t qtags_bytes = 0;      // ... and the tags of the reverse scan's queries [Q]
     // cached TMA descriptors (tc_cached_map): re-encoded only when the base pointer or shape changes
     struct MapSlot {
         alignas(64) unsigned char bytes[128];
@@ -89,6 +91,11 @@ struct ScanArgs {
     // range mode only, the reverse scan of nk_knn_graph_update: key-space threshold per local row [n]; a (row, query) pair is
     // listed only if it reaches both the query's threshold and the row's (tensor-core filters, ROWTHR instantiations)
     const float *row_thr = nullptr;
+    // with row_thr, a filtered graph's reverse scan: row_filter [n] (local rows) and qtags [Q]; a (row, query) pair is also
+    // listed only if tag_admits(qtags[q], row_filter + row), the mirror image of row_tags / qfilter.  Needs qfilter as well
+    // (the ROWTHR + TAGS + RFILT instantiations).
+    const NkFilter *row_filter = nullptr;
+    const uint64_t *qtags = nullptr;
 };
 
 // Fused distance + top-k scan on CUDA cores (small Q, any dim / dtype / alignment).

@@ -274,7 +274,9 @@ template <bool FILTER> struct Tf32Est {
 // TAGS: filtered search (per-query tag filters in the keep rule); the unfiltered instantiations are TAGS = false.
 // RANGE (filter mode only, nk_search_range): fixed per-query thresholds; full buffers are flushed to the lists, never pruned.
 // ROWTHR (with RANGE, the reverse scan of nk_knn_graph_update): a pair must also reach its row's threshold p.row_thr[row].
-template <int NT, int QT, bool DUMP, bool TAGS, bool RANGE = false, bool ROWTHR = false>
+// RFILT (with ROWTHR and TAGS, a filtered graph): the row's own filter must also admit the query's tag (keep_fragment_row);
+// the launch's query tags are staged in shared memory past Shared.
+template <int NT, int QT, bool DUMP, bool TAGS, bool RANGE = false, bool ROWTHR = false, bool RFILT = false>
 __global__ void __launch_bounds__(tc::THREADS, 1)
 knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_qhi,
                    const __grid_constant__ CUtensorMap map_qlo, tc::Params p) {
@@ -314,6 +316,8 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
         sh.cnt[tid] = 0;
         sh.qn[tid] = (FILTER && p.qnorm) ? p.qnorm[qpad_off + tid] : 1.0f;
     }
+    uint64_t *qtag = reinterpret_cast<uint64_t *>(smem_raw + (size_t)C::RING_BYTES + sizeof(Shared));  // RFILT only
+    if (RFILT && tid < QT) qtag[tid] = (uint32_t)tid < nq ? p.qtags[q0 + tid] : 0ull;
     __syncthreads();
     const bool flood = !(FILTER && p.presampled);  // first two tiles: every (row, query) pair is placed directly
     uint64_t *my_cand = p.cand + (size_t)blockIdx.x * QT * P;
@@ -435,9 +439,9 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                     if (!cosine && alive && est.x2 < INFINITY && (lane & 3) == 0) atomicMax(&sh.maxxx, __float_as_uint(est.x2));  // NaN / Inf rows: kept, judged exactly
                     if (euclid) est.mul = 2.0f;
                 }
-                keep_fragment_row<QT, P, FILTER, DUMP && FILTER, TAGS, ROWTHR>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau,
-                                                                         sh.qn, sh.cnt, my_cand,
-                                                                         ROWTHR && row < p.n ? __ldg(p.row_thr + row) : -INFINITY);
+                keep_fragment_row<QT, P, FILTER, DUMP && FILTER, TAGS, ROWTHR, RFILT>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq,
+                                                                                sh.tau, sh.qn, sh.cnt, my_cand,
+                                                                                ROWTHR && row < p.n ? __ldg(p.row_thr + row) : -INFINITY, qtag);
             }
             // prune any buffer that could overflow during the next tile; the 8 consumer warps prune different
             // queries concurrently with a register-resident warp selection
@@ -849,7 +853,7 @@ tc::Params pass_params(const ScanArgs &a, Workspace &ws, const tc::PassArgs &t) 
     p.cand = ws.cand; p.partial = ws.partial; p.flags = ws.flags; p.debug = tc_debug_flags(); p.mask = a.row_mask;
     p.gtau = reinterpret_cast<uint32_t *>(ws.keys2); p.gcount = reinterpret_cast<int *>(ws.keys2) + (t.Qpad + tc::QT_BIG);
     p.presampled = t.presampled; p.min_score = a.min_score;
-    p.row_tags = a.row_tags; p.qfilter = a.qfilter; p.row_thr = a.row_thr;
+    p.row_tags = a.row_tags; p.qfilter = a.qfilter; p.row_thr = a.row_thr; p.row_filter = a.row_filter; p.qtags = a.qtags;
     p.dump_est = t.dump_est; p.dump_bnd = t.dump_bnd; p.dump_ld = t.dump_ld;
     return p;
 }
@@ -903,7 +907,7 @@ struct TcPassArgs : tc::PassArgs {
     const int *only_if;
     bool count_main;
 };
-template <int NT, int QT, bool DUMP = false, bool TAGS = false, bool RANGE = false, bool ROWTHR = false>
+template <int NT, int QT, bool DUMP = false, bool TAGS = false, bool RANGE = false, bool ROWTHR = false, bool RFILT = false>
 static int launch_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const TcPassArgs &t, uint64_t *launches) {
     using namespace tc;
     const CUtensorMap *map_rows = tc_cached_map(ws, 0, a.rows, a.n, a.dim, 4, (uint32_t)BK, ROWS, (uint64_t)a.dim * 4);
@@ -911,26 +915,33 @@ static int launch_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws,
     const CUtensorMap *map_qhi = tc_cached_map(ws, QT == 64 ? 1 : 2, t.qhi, t.Qpad, a.dim, 4, (uint32_t)BK, QT, (uint64_t)a.dim * 4);
     const CUtensorMap *map_qlo = NT == 3 ? tc_cached_map(ws, 3, t.qlo, t.Qpad, a.dim, 4, (uint32_t)BK, QT, (uint64_t)a.dim * 4) : map_qhi;
     if (!map_rows || !map_qhi || !map_qlo) return -1;
-    const size_t smem = (size_t)Cfg<NT, QT>::RING_BYTES + sizeof(Shared) + 1024;
+    const size_t smem = (size_t)Cfg<NT, QT>::RING_BYTES + sizeof(Shared) + (RFILT ? QT * sizeof(uint64_t) : 0) + 1024;
     if (smem > di.max_smem_optin) {
         set_error("tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;
     }
-    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_tc_kernel<NT, QT, DUMP, TAGS, RANGE, ROWTHR>), di.device_id, smem)) return -1;
+    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_tc_kernel<NT, QT, DUMP, TAGS, RANGE, ROWTHR, RFILT>), di.device_id, smem))
+        return -1;
     Params p = pass_params(a, ws, t);
     p.nslab = (a.dim + BK - 1) / BK; p.margin_c = t.margin_c; p.only_if = t.only_if;
     // (asynchronous API: the early-exit retry / exact stages are programmatic dependents — their launch overlaps the kernel
     // before them.  Not for the host-synchronous API: measured 5-15 us slower per nk_search, the copy-out behind it waits longer)
-    NK_CUDA_OK(launch_pdl(knn_scan_tc_kernel<NT, QT, DUMP, TAGS, RANGE, ROWTHR>, dim3(t.grid), dim3(THREADS), smem, a.stream, t.only_if != nullptr && !a.defer_tail, *map_rows, *map_qhi,
+    NK_CUDA_OK(launch_pdl(knn_scan_tc_kernel<NT, QT, DUMP, TAGS, RANGE, ROWTHR, RFILT>, dim3(t.grid), dim3(THREADS), smem, a.stream, t.only_if != nullptr && !a.defer_tail, *map_rows, *map_qhi,
                           *map_qlo, p));
     if (launches) ++*launches;
     if (t.count_main && a.main_launches) ++*a.main_launches;
     return 0;
 }
 // Filtered searches (per-query tag filters) run the TAGS instantiation of the same kernel; range searches the RANGE one, and
-// the reverse scan of nk_knn_graph_update (per-row thresholds) the ROWTHR one.
+// the reverse scan of nk_knn_graph_update (per-row thresholds) the ROWTHR one, and that of a filtered graph (each row's own
+// filter, which needs the per-query filters too) the ROWTHR + RFILT one.
 template <int NT, int QT, bool DUMP = false>
 static int launch_pass(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const TcPassArgs &t, uint64_t *launches) {
+    if constexpr (NT == 1 && !DUMP)
+        if (t.range && a.row_thr && a.row_filter) {
+            if (!a.qfilter || !a.qtags) { set_error("internal: the row-filtered reverse scan needs per-query filters and tags"); return -1; }
+            return launch_pass_t<NT, QT, false, true, true, true, true>(di, a, ws, t, launches);
+        }
     if constexpr (NT == 1 && !DUMP)
         if (t.range && a.row_thr)
             return a.qfilter ? launch_pass_t<NT, QT, false, true, true, true>(di, a, ws, t, launches)

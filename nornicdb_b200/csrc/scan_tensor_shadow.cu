@@ -152,8 +152,10 @@ struct Bf16Est {
 // is spent on the rings); the unfiltered instantiations are TAGS = false.  F16: the operands are fp16 (an fp16 corpus
 // scanned in place) instead of bf16.  RANGE (nk_search_range): fixed per-query thresholds; full buffers are flushed to the
 // lists, never pruned, and the end of the launch flushes what is left.  ROWTHR (with RANGE, the reverse scan of
-// nk_knn_graph_update): a pair must also reach its row's threshold p.row_thr[row], loaded with the row's norms.
-template <int QT, bool F16, bool DUMP, bool TAGS, bool RANGE, bool ROWTHR = false>
+// nk_knn_graph_update): a pair must also reach its row's threshold p.row_thr[row], loaded with the row's norms.  RFILT (with
+// ROWTHR and TAGS, a filtered graph): the row's own filter must also admit the query's tag (keep_fragment_row); the launch's
+// query tags are staged in shared memory past Shared.
+template <int QT, bool F16, bool DUMP, bool TAGS, bool RANGE, bool ROWTHR = false, bool RFILT = false>
 __global__ void __launch_bounds__(sb::NTHREADS, 1)
 knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_q, tc::Params p) {
     using namespace sb;
@@ -187,6 +189,8 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
         sh.qa[tid] = p.qa[qpad_off + tid];
         sh.qb[tid] = p.qb[qpad_off + tid];
     }
+    uint64_t *qtag = reinterpret_cast<uint64_t *>(smem_raw + (size_t)C::RING_BYTES + sizeof(Shared));  // RFILT only
+    if (RFILT && tid < QT) qtag[tid] = (uint32_t)tid < nq ? p.qtags[q0 + tid] : 0ull;
     __syncthreads();
     const bool flood = !p.presampled;  // first two tiles: every (row, query) pair is placed directly
     if (prof && tid == 0) g_sb_prof[blockIdx.x][1] = globaltimer_ns();
@@ -325,8 +329,8 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                     atomicMax(&sh.max_ra, __float_as_uint(est.ra));
                     if (!cosine) { atomicMax(&sh.max_rb, __float_as_uint(est.rb)); atomicMax(&sh.maxxx, __float_as_uint(est.x2)); }
                 }
-                keep_fragment_row<QT, PB, true, DUMP, TAGS, ROWTHR>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau, sh.qn, sh.cnt,
-                                                                    my_cand, rthr[ri]);
+                keep_fragment_row<QT, PB, true, DUMP, TAGS, ROWTHR, RFILT>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau, sh.qn,
+                                                                           sh.cnt, my_cand, rthr[ri], qtag);
             }
             // prune any buffer that could overflow during the next tile (8 warps, different queries concurrently)
             group_sync(EPI_BAR, EPI_NT);  // every push of this tile is visible
@@ -512,7 +516,7 @@ bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a) {
     return a.dim % 8 == 0;  // 16-bit rows: 16-byte TMA row stride and 128-bit exact re-scoring loads
 }
 
-template <int QT, bool F16, bool DUMP, bool TAGS, bool RANGE = false, bool ROWTHR = false>
+template <int QT, bool F16, bool DUMP, bool TAGS, bool RANGE = false, bool ROWTHR = false, bool RFILT = false>
 static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
     using namespace sb;
     const bool native = a.shadow_native;  // 16-bit corpus scanned in place: row stride dim * 2, columns past dim read as zero (TMA OOB fill)
@@ -521,15 +525,16 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
     const CUtensorMap *map_q = tc_cached_map(ws, QT == 64 ? 5 : 6, sp.qbf16, sp.Qpad, sp.dimpad, 2, BKB, QT, (uint64_t)sp.dimpad * 2,
                                              a.dtype);  // rows past Qpad: zero
     if (!map_rows || !map_q) return -1;
-    const size_t smem = (size_t)Cfg<QT>::RING_BYTES + sizeof(Shared) + 1024;
+    const size_t smem = (size_t)Cfg<QT>::RING_BYTES + sizeof(Shared) + (RFILT ? QT * sizeof(uint64_t) : 0) + 1024;
     if (smem > di.max_smem_optin) {
         set_error("shadow tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;
     }
-    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, F16, DUMP, TAGS, RANGE, ROWTHR>), di.device_id, smem)) return -1;
+    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, F16, DUMP, TAGS, RANGE, ROWTHR, RFILT>), di.device_id, smem))
+        return -1;
     tc::Params p = pass_params(a, ws, sp);
     p.nslab = sp.dimpad / BKB; p.qa = sp.qa; p.qb = sp.qb; p.xnorm2 = a.xnorm2; p.dnorm2 = a.dnorm2;
-    knn_scan_shadow_kernel<QT, F16, DUMP, TAGS, RANGE, ROWTHR><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
+    knn_scan_shadow_kernel<QT, F16, DUMP, TAGS, RANGE, ROWTHR, RFILT><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
     NK_CUDA_OK(cudaGetLastError());
     if (launches) ++*launches;
     if (a.main_launches) ++*a.main_launches;
@@ -540,6 +545,11 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
 template <bool F16>
 static int launch_shadow_pass_op(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
     if (sp.dump_est) return launch_shadow_pass_t<64, F16, true, false>(di, a, ws, sp, launches);
+    if (sp.range && a.row_thr && a.row_filter) {  // the reverse scan of a filtered graph: each row's own filter
+        if (!a.qfilter || !a.qtags) { set_error("internal: the row-filtered reverse scan needs per-query filters and tags"); return -1; }
+        return qt == 128 ? launch_shadow_pass_t<128, F16, false, true, true, true, true>(di, a, ws, sp, launches)
+                         : launch_shadow_pass_t<64, F16, false, true, true, true, true>(di, a, ws, sp, launches);
+    }
     if (sp.range && a.row_thr) {  // the reverse scan of nk_knn_graph_update
         if (a.qfilter)
             return qt == 128 ? launch_shadow_pass_t<128, F16, false, true, true, true>(di, a, ws, sp, launches)

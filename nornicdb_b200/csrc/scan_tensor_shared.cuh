@@ -71,6 +71,8 @@ struct Params {
     const uint64_t *row_tags; // TAGS kernels only: tag word per local row
     const NkFilter *qfilter;  // TAGS kernels only: filter per query [Q], indexed like gtau (absolute query index)
     const float *row_thr;     // ROWTHR kernels only: key-space threshold per local row (the reverse scan of nk_knn_graph_update)
+    const NkFilter *row_filter;  // RFILT kernels only: the filter of each local row's own k-NN list (filtered graphs)
+    const uint64_t *qtags;    // RFILT kernels only: tag word per query [Q], indexed like gtau; staged in shared memory per CTA
 };
 
 // What one scan launch covers: queries [q0, q0+nq) in `qgroups` query groups over a `grid`-CTA launch.  Both kernels'
@@ -162,11 +164,15 @@ __device__ __forceinline__ bool row_alive(const Params &p, uint32_t row) {
 // published thresholds would stop being lower bounds of the FILTERED k-th best score.  Flood tiles place it as key 0; the
 // compare pass loads the row's tag only when some column passed and clears the columns whose filter rejects it.
 // ROWTHR (the reverse scan of nk_knn_graph_update, range mode): a pair must also reach the ROW's threshold rthr.
-template <int QT, int CAP, bool BOUNDED, bool DUMP, bool TAGS = false, bool ROWTHR = false, class Est>
+// RFILT (with ROWTHR and TAGS, the reverse scan of a filtered graph): the row's own filter p.row_filter[row] must also admit
+// the query's tag qtag[qi] (the CTA's query tags, in shared memory) — the mirror image of TAGS.  The row's filter is loaded
+// only for a fragment row with a pair that already reached both thresholds.
+template <int QT, int CAP, bool BOUNDED, bool DUMP, bool TAGS = false, bool ROWTHR = false, bool RFILT = false, class Est>
 __device__ __forceinline__ void keep_fragment_row(const Params &p, const Est &est, const float (&acc)[QT / 2], uint32_t r,
                                                   uint32_t row, uint32_t rt, bool alive, bool flood, uint32_t it, uint32_t cbase,
                                                   uint32_t q0, uint32_t nq, const float *tau, const float *qn, int *cnt,
-                                                  uint64_t *cand, float rthr = -INFINITY) {
+                                                  uint64_t *cand, float rthr = -INFINITY, const uint64_t *qtag = nullptr) {
+    static_assert(!RFILT || (TAGS && ROWTHR), "the row-side filter is a mode of the filtered reverse scan");
     float v[QT / 4];
 #pragma unroll
     for (int jj = 0; jj < QT / 4; ++jj) v[jj] = acc[(jj >> 1) * 4 + r * 2 + (jj & 1)];
@@ -195,7 +201,8 @@ __device__ __forceinline__ void keep_fragment_row(const Params &p, const Est &es
 #pragma unroll 1
                 for (uint32_t c = 0; c < (uint32_t)(QT / 4); ++c) {
                     const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
-                    if (qi < nq && tag_admits(tag, p.qfilter + q0 + qi)) admit |= 1u << c;
+                    if (qi < nq && tag_admits(tag, p.qfilter + q0 + qi) && (!RFILT || tag_admits(qtag[qi], p.row_filter + row)))
+                        admit |= 1u << c;
                 }
             }
         }
@@ -226,6 +233,17 @@ __device__ __forceinline__ void keep_fragment_row(const Params &p, const Est &es
                 const uint32_t c = (uint32_t)__ffs((int)chk) - 1u;
                 chk &= chk - 1u;
                 if (!tag_admits(tag, p.qfilter + q0 + cbase + 8 * (c >> 1) + (c & 1))) pass &= ~(1u << c);
+            }
+        }
+        if (RFILT && pass) {
+            const NkFilter *rf = p.row_filter + row;
+            const uint64_t all_of = __ldg(&rf->all_of), none_of = __ldg(&rf->none_of), any_of = __ldg(&rf->any_of);
+            uint32_t chk = pass;
+#pragma unroll 1
+            while (chk) {
+                const uint32_t c = (uint32_t)__ffs((int)chk) - 1u;
+                chk &= chk - 1u;
+                if (!tag_admits(qtag[cbase + 8 * (c >> 1) + (c & 1)], all_of, none_of, any_of)) pass &= ~(1u << c);
             }
         }
 #pragma unroll 1

@@ -230,6 +230,7 @@ public:
         } else {
             check(nk_index_append(ix_, embedding.data(), 1));
             if (graphK_) graphSrc_.push_back(NK_ROW_NEW);
+            tags_.push_back(0);  // nk_index_append: tag 0
             idToIndex_[nodeID] = nodeIDs_.size();
             nodeIDs_.push_back(nodeID);
         }
@@ -249,6 +250,8 @@ public:
             graphSrc_[idx] = graphSrc_[last];
             graphSrc_.pop_back();
         }
+        tags_[idx] = tags_[last];  // the tag moves with its row
+        tags_.pop_back();
         if (idx != last) {
             nodeIDs_[idx] = nodeIDs_[last];
             idToIndex_[nodeIDs_[idx]] = idx;
@@ -281,9 +284,14 @@ public:
     }
     // Per-query tag filters: tag words of rows [firstRow, firstRow + tags.size()) (row order of Add; 0 = untagged), then a
     // batch whose queries each carry an NkFilter (Qdrant must / must_not / should over bit conditions) in one corpus pass.
+    // A row whose tag changes is new contents to SimilarGraph's graph.
     void SetRowTags(uint64_t firstRow, const std::vector<uint64_t> &tags) {
         std::lock_guard<std::mutex> lk(mu_);
         check(nk_index_set_row_tags(ix_, firstRow, tags.data(), tags.size()));
+        for (size_t i = 0; i < tags.size(); ++i) {
+            if (graphK_ && tags_[firstRow + i] != tags[i]) graphSrc_[firstRow + i] = NK_ROW_NEW;
+            tags_[firstRow + i] = tags[i];
+        }
     }
     std::vector<std::vector<SearchResult>> SearchBatchFiltered(const std::vector<float> &queries, const std::vector<NkFilter> &filters,
                                                                uint32_t Q, int k) {
@@ -361,20 +369,28 @@ public:
     }
     // The k most similar OTHER nodes of each stored node (FindSimilar, GraphQL similar, OnStore's related nodes), best first,
     // searched with the node's embedding as stored.  One list per id; an id the index does not hold gets an empty list
-    // (missing ids are ignored, as in ScoreSubset).
-    std::vector<std::vector<SearchResult>> SearchSimilar(const std::vector<std::string> &ids, int k) {
+    // (missing ids are ignored, as in ScoreSubset).  filters empty = none, else one tag filter per id (e.g. "same collection"):
+    // each list then holds only nodes its filter admits.
+    std::vector<std::vector<SearchResult>> SearchSimilar(const std::vector<std::string> &ids, int k, const std::vector<NkFilter> &filters = {}) {
+        if (!filters.empty() && filters.size() != ids.size()) throw std::invalid_argument("gpu: one filter per id");
         std::lock_guard<std::mutex> lk(mu_);
         std::vector<std::vector<SearchResult>> out(ids.size());
         std::vector<uint32_t> rows;
+        std::vector<NkFilter> f;
         std::vector<size_t> at;
         for (size_t i = 0; i < ids.size(); ++i) {
             auto it = idToIndex_.find(ids[i]);
-            if (it != idToIndex_.end()) { rows.push_back((uint32_t)it->second); at.push_back(i); }
+            if (it != idToIndex_.end()) {
+                rows.push_back((uint32_t)it->second);
+                at.push_back(i);
+                if (!filters.empty()) f.push_back(filters[i]);
+            }
         }
         if (rows.empty() || k <= 0) return out;
         std::vector<uint32_t> idx(rows.size() * (size_t)k);
         std::vector<float> sc(rows.size() * (size_t)k);
-        int got = nk_search_rows(ix_, rows.data(), (uint32_t)rows.size(), (uint32_t)k, idx.data(), sc.data());
+        int got = nk_search_rows_filtered(ix_, rows.data(), f.empty() ? nullptr : f.data(), (uint32_t)rows.size(), (uint32_t)k, idx.data(),
+                                          sc.data());
         if (got < 0) throw cuda::ErrKernelExecution(std::string("gpu: ") + nk_last_error());
         for (size_t j = 0; j < rows.size(); ++j)
             for (int i = 0; i < got; ++i) {
@@ -389,23 +405,35 @@ public:
     // next call hands that map to nk_knn_graph_remap instead of rebuilding.  The first call, a new k, or a Deserialize since
     // the last call rebuild it with nk_search_rows.  Lists in row order (the order of insertion, as swapped by Remove).  The
     // graph is built and updated on the 16-bit filter path (the TF32 filter if the shape has no 16-bit image), which the
-    // update requires; other searches keep the automatic choice.
-    std::vector<std::vector<SearchResult>> SimilarGraph(int k) {
+    // update requires; other searches keep the automatic choice.  filters empty = none, else one tag filter per row (row
+    // order): each node's list holds only nodes its filter admits, e.g. one graph per collection of the shared index.  A node
+    // whose filter or tag (SetRowTags) changed since the last call is handed to the update as new contents.
+    std::vector<std::vector<SearchResult>> SimilarGraph(int k, const std::vector<NkFilter> &filters = {}) {
         std::lock_guard<std::mutex> lk(mu_);
         const uint64_t n = nodeIDs_.size();
+        if (!filters.empty() && filters.size() != n) throw std::invalid_argument("gpu: one filter per node");
         if (n == 0 || k <= 0) return std::vector<std::vector<SearchResult>>(n);
+        auto filter_of = [&](uint64_t r) { return filters.empty() ? NkFilter{0, 0, 0} : filters[r]; };
+        auto same_filter = [](const NkFilter &a, const NkFilter &b) { return a.all_of == b.all_of && a.none_of == b.none_of && a.any_of == b.any_of; };
+        const NkFilter *fp = filters.empty() ? nullptr : filters.data();
         int got = -1;
         std::vector<uint32_t> gi(n * k, 0xffffffffu);
         std::vector<float> gs(n * k, 0.0f);
+        std::vector<uint32_t> src;  // graphSrc_ with the rows whose filter changed as new contents
+        if (graphK_ == (uint32_t)k) {
+            src = graphSrc_;
+            for (uint64_t f = 0; f < n; ++f)
+                if (src[f] != NK_ROW_NEW && !same_filter(filter_of(f), graphFilter_[src[f]])) src[f] = NK_ROW_NEW;
+        }
         for (int path : {NK_PATH_TENSOR_SHADOW, NK_PATH_TENSOR_FILTER}) {
             check(nk_index_set_path(ix_, path));
             if (graphK_ == (uint32_t)k) {
-                got = nk_knn_graph_remap(ix_, (uint32_t)k, graphRows_, graphSrc_.data(), graphIdx_.data(), graphScore_.data(), gi.data(),
-                                         gs.data(), nullptr);
+                got = nk_knn_graph_remap_filtered(ix_, (uint32_t)k, graphRows_, src.data(), fp, graphIdx_.data(), graphScore_.data(), gi.data(),
+                                                  gs.data(), nullptr);
             } else {
                 std::vector<uint32_t> rows(n);
                 for (uint64_t r = 0; r < n; ++r) rows[r] = (uint32_t)r;
-                got = nk_search_rows(ix_, rows.data(), (uint32_t)n, (uint32_t)k, gi.data(), gs.data());
+                got = nk_search_rows_filtered(ix_, rows.data(), fp, (uint32_t)n, (uint32_t)k, gi.data(), gs.data());
                 if (got >= 0) ++graphRebuilds_;
             }
             if (got >= 0) break;
@@ -417,7 +445,8 @@ public:
         graphIdx_.swap(gi);
         graphScore_.swap(gs);
         graphSrc_.resize(n);
-        for (uint64_t r = 0; r < n; ++r) graphSrc_[r] = (uint32_t)r;
+        graphFilter_.resize(n);
+        for (uint64_t r = 0; r < n; ++r) { graphSrc_[r] = (uint32_t)r; graphFilter_[r] = filter_of(r); }
         std::vector<std::vector<SearchResult>> out(n);
         for (uint64_t r = 0; r < n; ++r)
             for (int i = 0; i < got; ++i) {
@@ -449,6 +478,7 @@ public:
     void SyncToGPU() { std::lock_guard<std::mutex> lk(mu_); gpuSynced_ = true; }
     bool IsGPUSynced() const { return gpuSynced_; }
     uint64_t GraphRebuilds() const { return graphRebuilds_; }  // SimilarGraph calls that searched every row
+    std::vector<uint64_t> RowTags() { std::lock_guard<std::mutex> lk(mu_); return tags_; }  // the tag of each row, row order
     int Count() const { return (int)nodeIDs_.size(); }                                   // gpu.go:2225
     bool Has(const std::string &id) const { return idToIndex_.count(id) != 0; }          // gpu.go:2279
     bool Get(const std::string &id, std::vector<float> *out) {                           // gpu.go:2287
@@ -489,6 +519,7 @@ public:
         check(nk_index_upload(ix_, data.data() + off, count));  // the blob streams straight into device memory
         gpuSynced_ = false;
         graphK_ = 0;
+        tags_.assign(count, 0);  // nk_index_upload: every tag 0
         nodeIDs_ = ids;
         idToIndex_.clear();
         for (uint32_t i = 0; i < count; ++i) idToIndex_[nodeIDs_[i]] = i;
@@ -508,6 +539,8 @@ private:
     std::vector<uint32_t> graphIdx_;
     std::vector<float> graphScore_;
     std::vector<uint32_t> graphSrc_;
+    std::vector<NkFilter> graphFilter_;  // the filter of each graph row's list when it was made ({0,0,0}: none)
+    std::vector<uint64_t> tags_;         // the tag of each row, as on the device
     uint64_t graphRebuilds_ = 0;
     std::mutex mu_;
 };

@@ -228,33 +228,55 @@ class KnnIndex:
                                        sc.ctypes.data_as(C.c_void_p)), "nk_search")
         return idx[:, :ke], sc[:, :ke]
 
-    def search_rows(self, rows, k: int) -> Tuple[np.ndarray, np.ndarray]:
+    def search_rows(self, rows, k: int, filters=None) -> Tuple[np.ndarray, np.ndarray]:
         """The k nearest OTHER rows of stored rows: rows = row ids (< len(self), repeats allowed), each searched as stored now
         -> (idx [Q x k'] uint32, score [Q x k'] fp32), k' = min(k, admissible rows), with search()'s conventions.  A query
         with fewer admissible other rows gets index 0xffffffff and score 0 in its unused slots.  rows = every row id gives
-        the k-NN graph of the index in one call (served in blocks of 1024 queries)."""
+        the k-NN graph of the index in one call (served in blocks of 1024 queries).  filters: None, or one tag filter per
+        query ([Q x 3] uint64, as in search_filtered): query q then lists only rows its filter admits (its own row may be
+        refused by it) (nk_search_rows_filtered)."""
         r = np.asarray(rows, dtype=np.int64).reshape(-1)
         if r.size and (r.min() < 0 or r.max() > 0xFFFFFFFF):
             raise KnnError("search_rows: row ids must be in [0, 2^32)")
         r = np.ascontiguousarray(r.astype(np.uint32))
         Q = r.size
+        f = None if filters is None else as_filters(filters, Q)
         k = int(k)
         if k <= 0 or Q == 0:
             return np.empty((Q, 0), np.uint32), np.empty((Q, 0), np.float32)
         idx = np.empty((Q, k), dtype=np.uint32)
         sc = np.empty((Q, k), dtype=np.float32)
-        ke = _check(self.lib.nk_search_rows(self.ptr, r.ctypes.data_as(C.c_void_p), Q, k, idx.ctypes.data_as(C.c_void_p),
-                                            sc.ctypes.data_as(C.c_void_p)), "nk_search_rows")
+        if f is None:
+            ke = _check(self.lib.nk_search_rows(self.ptr, r.ctypes.data_as(C.c_void_p), Q, k, idx.ctypes.data_as(C.c_void_p),
+                                                sc.ctypes.data_as(C.c_void_p)), "nk_search_rows")
+        else:
+            ke = _check(self.lib.nk_search_rows_filtered(self.ptr, r.ctypes.data_as(C.c_void_p), f.ctypes.data_as(C.c_void_p), Q, k,
+                                                         idx.ctypes.data_as(C.c_void_p), sc.ctypes.data_as(C.c_void_p)),
+                        "nk_search_rows_filtered")
         return idx[:, :ke], sc[:, :ke]
 
-    def update_knn_graph(self, idx, score, n_old: int, changed=None, k: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray, int]:
+    def _graph_filters(self, filters, what: str):
+        """filters of a graph call: None, or one [n x 3] uint64 filter per current row"""
+        if filters is None:
+            return None
+        n = len(self)
+        f = np.ascontiguousarray(np.asarray(filters, dtype=np.uint64))
+        if f.shape != (n, 3):
+            raise KnnError(f"{what}: filters must be [{n} x 3] (one per current row), not {list(f.shape)}")
+        return f
+
+    def update_knn_graph(self, idx, score, n_old: int, changed=None, k: Optional[int] = None,
+                         filters=None) -> Tuple[np.ndarray, np.ndarray, int]:
         """Bring the k-NN graph search_rows(range(n_old), k) returned up to date after rows were appended (rows n_old ..
         len(self) - 1) and old rows rewritten (`changed`: their ids, repeats allowed) -> (idx, score, lists_changed): what
         search_rows(every row, k) returns now, k' = min(k, admissible rows) columns, and how many old rows' lists changed.
         idx / score: [n_old x w]; k defaults to w, and a narrower graph (search_rows returns fewer than k columns while fewer
         rows are admissible) is padded with 0xffffffff / 0.  Build the graph with the path set (set_path("shadow") or
         "filter"), and keep the metric, the score floor and the old rows' mask bits (set the mask again after append).  After
-        remove_swap, use remap_knn_graph (nk_knn_graph_update)."""
+        remove_swap, use remap_knn_graph (nk_knn_graph_update).
+        filters: None, or one tag filter per current row ([len(self) x 3] uint64): the graph of search_rows(every row, k,
+        filters), each list bounded by its row's own filter.  An old row whose tag or filter changed since the graph was built
+        must be listed in `changed`, like a rewritten row (nk_knn_graph_update_filtered)."""
         idx = np.asarray(idx, dtype=np.uint32)
         score = np.asarray(score, dtype=np.float32)
         n_old = int(n_old)
@@ -270,6 +292,7 @@ class KnnIndex:
         if ch.size and ch.min() < 0:
             raise KnnError("update_knn_graph: changed row ids must be >= 0")
         ch = np.ascontiguousarray(ch.astype(np.uint32))
+        f = self._graph_filters(filters, "update_knn_graph")
         if k <= 0 or n == 0:
             return np.empty((n, 0), np.uint32), np.empty((n, 0), np.float32), 0
         gi = np.full((n, k), 0xFFFFFFFF, dtype=np.uint32)
@@ -277,18 +300,27 @@ class KnnIndex:
         gi[:n_old, :idx.shape[1]] = idx
         gs[:n_old, :idx.shape[1]] = score
         changed_lists = C.c_uint64(0)
-        ke = _check(self.lib.nk_knn_graph_update(self.ptr, k, n_old, ch.ctypes.data_as(C.c_void_p) if ch.size else None, int(ch.size),
-                                                 gi.ctypes.data_as(C.c_void_p), gs.ctypes.data_as(C.c_void_p), C.byref(changed_lists)),
-                    "nk_knn_graph_update")
+        chp = ch.ctypes.data_as(C.c_void_p) if ch.size else None
+        if f is None:
+            ke = _check(self.lib.nk_knn_graph_update(self.ptr, k, n_old, chp, int(ch.size), gi.ctypes.data_as(C.c_void_p),
+                                                     gs.ctypes.data_as(C.c_void_p), C.byref(changed_lists)), "nk_knn_graph_update")
+        else:
+            ke = _check(self.lib.nk_knn_graph_update_filtered(self.ptr, k, n_old, chp, int(ch.size), f.ctypes.data_as(C.c_void_p),
+                                                              gi.ctypes.data_as(C.c_void_p), gs.ctypes.data_as(C.c_void_p),
+                                                              C.byref(changed_lists)), "nk_knn_graph_update_filtered")
         return gi[:, :ke], gs[:, :ke], int(changed_lists.value)
 
-    def remap_knn_graph(self, idx, score, n_old: int, src, k: Optional[int] = None) -> Tuple[np.ndarray, np.ndarray, int]:
+    def remap_knn_graph(self, idx, score, n_old: int, src, k: Optional[int] = None,
+                        filters=None) -> Tuple[np.ndarray, np.ndarray, int]:
         """Bring the k-NN graph search_rows(range(n_old), k) returned up to date after any mix of append, update_row and
         remove_swap -> (idx, score, lists_changed): what search_rows(every row, k) returns now, k' = min(k, admissible rows)
         columns, and how many rows that hold their old contents at their old id got a different list.  src: a GraphRowMap
         that followed the changes, or its src_of_row (one entry per current row: the old row whose contents it holds, or
         ROW_NEW).  idx / score / k and the preconditions are those of update_knn_graph, the mask bit of a moved row included
-        (nk_knn_graph_remap)."""
+        (nk_knn_graph_remap).
+        filters: None, or one tag filter per current row ([len(self) x 3] uint64, in current row order): the graph of
+        search_rows(every row, k, filters).  A row whose tag or filter changed since the graph was built must be ROW_NEW in
+        src: record it with GraphRowMap.update_row, like a rewrite (nk_knn_graph_remap_filtered)."""
         idx = np.asarray(idx, dtype=np.uint32)
         score = np.asarray(score, dtype=np.float32)
         n_old = int(n_old)
@@ -304,6 +336,7 @@ class KnnIndex:
         if s.size and (s.min() < 0 or s.max() > ROW_NEW):
             raise KnnError("remap_knn_graph: src_of_row entries must be old row ids or ROW_NEW")
         s = np.ascontiguousarray(s.astype(np.uint32))
+        f = self._graph_filters(filters, "remap_knn_graph")
         if k <= 0 or n == 0:
             return np.empty((n, 0), np.uint32), np.empty((n, 0), np.float32), 0
         oi = np.full((n_old, k), 0xFFFFFFFF, dtype=np.uint32)
@@ -313,10 +346,13 @@ class KnnIndex:
         gi = np.full((n, k), 0xFFFFFFFF, dtype=np.uint32)
         gs = np.zeros((n, k), dtype=np.float32)
         changed_lists = C.c_uint64(0)
-        ke = _check(self.lib.nk_knn_graph_remap(self.ptr, k, n_old, s.ctypes.data_as(C.c_void_p), oi.ctypes.data_as(C.c_void_p),
-                                                osc.ctypes.data_as(C.c_void_p), gi.ctypes.data_as(C.c_void_p),
-                                                gs.ctypes.data_as(C.c_void_p), C.byref(changed_lists)),
-                    "nk_knn_graph_remap")
+        graph = (oi.ctypes.data_as(C.c_void_p), osc.ctypes.data_as(C.c_void_p), gi.ctypes.data_as(C.c_void_p),
+                 gs.ctypes.data_as(C.c_void_p), C.byref(changed_lists))
+        if f is None:
+            ke = _check(self.lib.nk_knn_graph_remap(self.ptr, k, n_old, s.ctypes.data_as(C.c_void_p), *graph), "nk_knn_graph_remap")
+        else:
+            ke = _check(self.lib.nk_knn_graph_remap_filtered(self.ptr, k, n_old, s.ctypes.data_as(C.c_void_p),
+                                                             f.ctypes.data_as(C.c_void_p), *graph), "nk_knn_graph_remap_filtered")
         return gi[:, :ke], gs[:, :ke], int(changed_lists.value)
 
     def search_device(self, q_ptr: int, Q: int, k: int, out_idx_ptr: int, out_score_ptr: int, stream: int = 0) -> int:
@@ -325,7 +361,9 @@ class KnnIndex:
 
     # -- per-query tag filters ---------------------------------------------------------------------
     def set_row_tags(self, tags, first_row: int = 0) -> None:
-        """Tag words (uint64, one per row) of rows [first_row, first_row + len(tags)); untagged rows have tag 0."""
+        """Tag words (uint64, one per row) of rows [first_row, first_row + len(tags)); untagged rows have tag 0.  A filtered
+        k-NN graph is not told: the caller reports each row whose tag changed as rewritten (GraphRowMap.update_row, or
+        update_knn_graph's `changed`)."""
         t = np.ascontiguousarray(np.asarray(tags, dtype=np.uint64).reshape(-1))
         _check(self.lib.nk_index_set_row_tags(self.ptr, int(first_row), t.ctypes.data_as(C.c_void_p), int(t.size)),
                "nk_index_set_row_tags")
@@ -488,6 +526,8 @@ class GraphRowMap:
         return row
 
     def update_row(self, row: int) -> None:
+        """The row's contents changed (update_row).  For a filtered graph, also call it for a row whose tag or filter
+        changed: the graph treats such a row as rewritten."""
         self._src[self._row(row)] = ROW_NEW
 
     def remove_swap(self, row: int) -> None:
