@@ -200,6 +200,12 @@ int nk_index_debug_counters(NkIndex *ix, uint64_t out[4]);
  * (1xTF32 pass over fp32 rows) or NK_PATH_TENSOR_SHADOW (16-bit pass).  The filters are sound iff |est - exact| <= bnd;
  * tests/test_gpu_error_model.py measures the worst err / bnd ratio against fp64 on adversarial data. */
 int nk_debug_filter_dump(NkIndex *ix, const float *queries_host, uint32_t Q, int which, float *est_host, float *bnd_host);
+/* Tests only: run nk_index_assign_nearest on a single-device index (from a zero assignment, result discarded) and return
+ * how many rows it listed as near-ties, i.e. rows whose centroid the exact fix-up decided rather than the assignment's error
+ * bound.  The first min(count, cap) such rows go to rows_out and their 4 candidate ids each to cand_out ([cap x 4]; 0xfffffffe
+ * = every centroid, 0xffffffff = no candidate).  Rows not listed were decided by the bound. */
+int nk_debug_assign_ties(NkIndex *ix, const float *centroids_host, uint32_t K, int metric, uint32_t *rows_out, uint32_t *cand_out,
+                         uint32_t cap);
 /* Device-resident searches return before the device has run: this waits for `stream` (and the index's own streams), reads
  * and clears the sticky internal-overflow word nk_search checks on every call, and returns 0 / -1 with that message. */
 int nk_index_status(NkIndex *ix, void *stream);
@@ -451,7 +457,12 @@ int nk_score_subset(NkIndex *ix, const float *query_host, const uint32_t *rows_h
  * distance) / assignToCentroidsGPU (kmeans.go:491-546, NK_METRIC_COSINE: highest cosine): the fused scan with the roles
  * swapped — the K centroids (host, [K x dim]) are the corpus, the index's rows are the queries, read in place.
  * assign_io (host, [rows], int32) holds the previous assignment on entry (any value, e.g. 0 as in Go) and the new one
- * on return; *changed (nullable) = how many differ.  Ties go to the lowest centroid index.
+ * on return; *changed (nullable) = how many differ.  The result is exact, on every path (DESIGN §7 item 3):
+ *   euclidean: kmeans.go's assignment row for row (squaredEuclidean: fp32 differences, fp64 sums; lowest index on ties);
+ *   cosine: the argmax of the fp64 cosine of the fp32 inputs, lowest index among equal scores; a zero row or a zero
+ *   centroid scores 0 and NaN never wins.  This equals cosineSimilarityFlat's choice wherever its own fp32 rounding cannot
+ *   flip the order, and departs from it where its sqrt32 has not converged (|c|^2 far outside about [1e-4, 1e5]).
+ * A row no centroid scores (all NaN) goes to centroid 0.
  * nk_index_cluster_means = updateCentroidsWithBuffer (kmeans.go:585-618): centroids_io (host, [K x dim]) <- float32 of the
  * float64 mean of each cluster's rows; clusters without members keep their value; counts_out (nullable, [K]). */
 int nk_index_assign_nearest(NkIndex *ix, const float *centroids_host, uint32_t K, int metric, int32_t *assign_io,

@@ -99,6 +99,7 @@ SIGNATURES = {
     "nk_index_set_min_score": (_i, [_vp, C.c_float]),
     "nk_index_debug_counters": (_i, [_vp, C.POINTER(C.c_uint64)]),
     "nk_debug_filter_dump": (_i, [_vp, _vp, C.c_uint32, _i, _vp, _vp]),
+    "nk_debug_assign_ties": (_i, [_vp, _vp, C.c_uint32, _i, _vp, _vp, C.c_uint32]),
     "nk_index_status": (_i, [_vp, _vp]),
     "nk_index_set_row_groups": (_i, [_vp, _vp, _u64, C.c_uint32]),
     "nk_search_groups": (_i, [_vp, _vp, C.c_uint32, _vp, _vp, _vp]),

@@ -9,10 +9,13 @@
 // four lanes that share a row merge their lists at the end.
 //   cosine    (assignToCentroidsGPU, kmeans.go:491-546)  score = x.c/|c|            (|x| > 0 does not change the argmax)
 //   euclidean (assignToCentroids,    kmeans.go:458-489)  score = 2 x.c - |c|^2      (argmin |x-c|^2)
-// with the rigorous BF16 bound of scan_tensor_shadow.cu.  A row whose runner-up cannot reach the winner's lower bound is
-// decided; the others (near-ties) are listed with their <= 4 candidates and assign_fixup_kernel re-scores those candidates
-// exactly in fp32 (strict comparison in ascending centroid order = lowest index wins ties, kmeans.go:470-476,529-534).
+// with the rigorous BF16 bound of scan_tensor_shadow.cu, widened under euclidean by the rounding of kmeans.go's own
+// arithmetic (fp32 differences: 2^-22 (|x|^2 - lo), DESIGN §7 item 3).  A row whose runner-up cannot reach the winner's
+// lower bound is decided; the others (near-ties) are listed with their <= 3 candidates (or ALL) and assign_fixup_kernel
+// decides them with the contract's arithmetic: squaredEuclidean bit for bit, or the fp64 cosine (strict comparison in
+// ascending centroid order = lowest index wins ties, kmeans.go:470-476,529-534).
 #include <cuda.h>
+#include <float.h>
 #include <stdlib.h>
 
 #include "kernels.cuh"
@@ -86,7 +89,7 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
         const uint32_t ewarp = warp - EPI_WARP0, m = ewarp >> 2, wq = ewarp & 3;
         const uint32_t rbase = m * 128 + wq * 16 + ((uint32_t)lane >> 2), cbase = 2u * ((uint32_t)lane & 3u);
         const bool euclid = p.metric == NK_METRIC_EUCLIDEAN;
-        // score = mul * acc - (euclid ? |c|^2 : 0);  bound = ra qa[c] + rb qb[c] (+ 1e-6 |c|^2)
+        // score = mul * acc - (euclid ? |c|^2 : 0);  bound = ra qa[c] + rb qb[c] (+ 1e-6 |c|^2 + 2^-22 (xhi - (score - bound)))
         const float mul = euclid ? 2.0f : 1.0f;
         float acc[2][QT / 2];
 #pragma unroll
@@ -138,7 +141,10 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
 #pragma unroll
                     for (int ri = 0; ri < 4; ++ri) {
                         const float s = fmaf(acc[ri >> 1][(jj >> 1) * 4 + (ri & 1) * 2 + (jj & 1)], mul, -cc);
-                        const float bnd = fmaf(ra[ri], qa, rb[ri] * qb) + 1e-6f * cc;
+                        float bnd = fmaf(ra[ri], qa, rb[ri] * qb) + 1e-6f * cc;
+                        // kmeans.go rounds every difference x_j - c_j to fp32: its squared distance is within 2^-23 (1 + 2^-15) of
+                        // the exact one, which is at most |x|^2 - lo <= 1.001 xx - lo (xx: the fp32 |x|^2, relative error < 6.3e-5)
+                        if (euclid) bnd = fmaf(fmaxf(fmaf(x2[ri], 1.001f, bnd - s), 0.0f), 2.384185791015625e-7f, bnd);
                         const float up = s + bnd, lo = s - bnd;
                         maxlo[ri] = fmaxf(maxlo[ri], lo);  // NaN scores never enter: such rows end up in the exact fix-up
                         if (up > u[ri][3]) {  // strict: among equal bounds the lower centroid index stays ahead
@@ -188,7 +194,7 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                 if (decided) {
                     p.assign[row] = i0;
                 } else {
-                    // near-tie (or a zero / non-finite row): exact fp32 re-scoring of the candidates decides
+                    // near-tie (or a zero / non-finite row): the fix-up re-scores the candidates with the contract's arithmetic
                     const uint32_t pos = atomicAdd(p.amb_count, 1u);
                     if (pos < p.amb_cap) {
                         p.amb_rows[pos] = row;
@@ -205,8 +211,39 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
     }
 }
 
-// Exact fp32 decision for the listed rows: one warp per row, candidates in ascending centroid order, strict comparison
-// (kmeans.go:470-476: dist < minDist; :529-534: sim > maxSim), so the lowest index wins ties.
+// squaredEuclidean (kmeans.go:430-454, oracle orc_sq_euclid64) bit for bit: fp32 differences, fp64 squares in four
+// interleaved sums, the tail into s0, then s0 + s1 + s2 + s3.  Explicit round-to-nearest intrinsics: nvcc would contract
+// a * b + c into an fma and change the rounding.
+__device__ __forceinline__ double sq_euclid64(const float *x, const float *c, uint32_t dim) {
+    double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
+    uint32_t j = 0;
+    for (; j + 4 <= dim; j += 4) {
+        const double d0 = (double)__fsub_rn(x[j], c[j]), d1 = (double)__fsub_rn(x[j + 1], c[j + 1]);
+        const double d2 = (double)__fsub_rn(x[j + 2], c[j + 2]), d3 = (double)__fsub_rn(x[j + 3], c[j + 3]);
+        s0 = __dadd_rn(s0, __dmul_rn(d0, d0)); s1 = __dadd_rn(s1, __dmul_rn(d1, d1));
+        s2 = __dadd_rn(s2, __dmul_rn(d2, d2)); s3 = __dadd_rn(s3, __dmul_rn(d3, d3));
+    }
+    for (; j < dim; ++j) {
+        const double d = (double)__fsub_rn(x[j], c[j]);
+        s0 = __dadd_rn(s0, __dmul_rn(d, d));
+    }
+    return __dadd_rn(__dadd_rn(__dadd_rn(s0, s1), s2), s3);
+}
+
+// fp64 cosine of the fp32 inputs: 0 for a zero row or centroid, NaN for non-finite inputs (never wins)
+__device__ __forceinline__ double cosine64(const float *x, const float *c, uint32_t dim) {
+    double xc = 0.0, xx = 0.0, cc = 0.0;
+    for (uint32_t j = 0; j < dim; ++j) {
+        const double a = x[j], b = c[j];
+        xc = fma(a, b, xc); xx = fma(a, a, xx); cc = fma(b, b, cc);
+    }
+    return (xx == 0.0 || cc == 0.0) ? 0.0 : xc / (sqrt(xx) * sqrt(cc));
+}
+
+// The contract's decision for the listed rows: one warp per row, lane t scores candidates t, t + 32, ... sequentially (the
+// near-tie rows are few), then the warp keeps the best (score, lowest index): the strict comparison in ascending centroid
+// order of kmeans.go:470-476 (dist < minDist from math.MaxFloat64) and :529-534 (sim > maxSim); NaN never wins, and a
+// row no candidate beats the initial value of goes to centroid 0.
 __global__ void assign_fixup_kernel(const float *rows, uint32_t dim, const float *centroids, uint32_t K, int metric,
                                     const uint32_t *amb_count, uint32_t amb_cap, const uint32_t *amb_rows, const uint32_t *amb_cand,
                                     uint32_t *assign) {
@@ -214,50 +251,42 @@ __global__ void assign_fixup_kernel(const float *rows, uint32_t dim, const float
     uint32_t total = *amb_count;
     if (total > amb_cap) total = amb_cap;
     const uint32_t warps = gridDim.x * (blockDim.x >> 5);
+    const bool euclid = metric == NK_METRIC_EUCLIDEAN;
     for (uint32_t e = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); e < total; e += warps) {
         const uint32_t row = amb_rows[e];
         const float *x = rows + (size_t)row * dim;
-        uint32_t cand[3] = {amb_cand[4 * e], amb_cand[4 * e + 1], amb_cand[4 * e + 2]};
-        const bool all = cand[0] == asg::ALL;
-        if (!all) {  // ascending order (3-element sorting network; NONE = 0xffffffff sorts last)
-            if (cand[0] > cand[1]) { uint32_t t = cand[0]; cand[0] = cand[1]; cand[1] = t; }
-            if (cand[1] > cand[2]) { uint32_t t = cand[1]; cand[1] = cand[2]; cand[2] = t; }
-            if (cand[0] > cand[1]) { uint32_t t = cand[0]; cand[0] = cand[1]; cand[1] = t; }
-        }
-        float xx = 0.0f;
-        if (metric != NK_METRIC_EUCLIDEAN) {
-            for (uint32_t j = lane; j < dim; j += 32) xx = fmaf(x[j], x[j], xx);
-#pragma unroll
-            for (int o = 16; o; o >>= 1) xx += __shfl_xor_sync(0xffffffffu, xx, o);
-        }
-        float best = metric == NK_METRIC_EUCLIDEAN ? INFINITY : -INFINITY;
-        uint32_t nearest = 0;
+        const bool all = amb_cand[4 * e] == asg::ALL;
         const uint32_t count = all ? K : 3u;
-        for (uint32_t t = 0; t < count; ++t) {
-            const uint32_t ci = all ? t : cand[t];
+        // euclidean: minimise d, kept as -d so both metrics maximise; ties -> lower index
+        double best = euclid ? -DBL_MAX : -INFINITY;
+        uint32_t nearest = asg::NONE;
+        for (uint32_t t = lane; t < count; t += 32) {
+            const uint32_t ci = all ? t : amb_cand[4 * e + t];
             if (ci >= K) continue;
             const float *c = centroids + (size_t)ci * dim;
-            float a = 0.0f, cc = 0.0f;
-            if (metric == NK_METRIC_EUCLIDEAN) {
-                for (uint32_t j = lane; j < dim; j += 32) { const float d = x[j] - c[j]; a = fmaf(d, d, a); }
-            } else {
-                for (uint32_t j = lane; j < dim; j += 32) { a = fmaf(x[j], c[j], a); cc = fmaf(c[j], c[j], cc); }
-            }
-#pragma unroll
-            for (int o = 16; o; o >>= 1) {
-                a += __shfl_xor_sync(0xffffffffu, a, o);
-                cc += __shfl_xor_sync(0xffffffffu, cc, o);
-            }
-            if (metric == NK_METRIC_EUCLIDEAN) {
-                if (a < best) { best = a; nearest = ci; }
-            } else {
-                const float den = sqrtf(xx * cc);
-                const float sim = den > 0.0f ? a / den : 0.0f;  // cosineSimilarityFlat: 0 for zero vectors (gpu.go:2467-2484)
-                if (sim > best) { best = sim; nearest = ci; }
-            }
+            const double sc = euclid ? -sq_euclid64(x, c, dim) : cosine64(x, c, dim);
+            if (sc > best || (sc == best && ci < nearest)) { best = sc; nearest = ci; }
         }
-        if (lane == 0) assign[row] = nearest;
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+            const double ob = __shfl_xor_sync(0xffffffffu, best, o);
+            const uint32_t on = __shfl_xor_sync(0xffffffffu, nearest, o);
+            if (ob > best || (ob == best && on < nearest)) { best = ob; nearest = on; }
+        }
+        if (lane == 0) assign[row] = nearest == asg::NONE ? 0u : nearest;
     }
+}
+
+// A centroid with a NaN or infinite element scores NaN under the contract (never wins), but filter_prep_kernel scales it to
+// a zero vector under cosine (t = |c|^2 is not > 0 or 1/|c| = 0), which would score an exact 0 with a zero bound.  A NaN
+// bound factor keeps such a centroid out of every row's candidates (its upper and lower bounds are NaN).
+__global__ void assign_mark_nonfinite_kernel(const float *centroids, uint32_t K, uint32_t dim, float *qb) {
+    const uint32_t c = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (c >= K) return;
+    bool bad = false;
+    for (uint32_t j = lane; j < dim; j += 32) bad |= !isfinite(centroids[(size_t)c * dim + j]);
+    if (__any_sync(0xffffffffu, bad) && lane == 0) qb[c] = __int_as_float(0x7fc00000);
 }
 
 bool assign_tensor_supported(const DeviceInfo &di, uint32_t dim, uint32_t K, int metric) {
@@ -268,21 +297,20 @@ bool assign_tensor_supported(const DeviceInfo &di, uint32_t dim, uint32_t K, int
 
 // rows / shadow / norms: one shard (device pointers); centroids_dev: [K x dim] fp32 on the same device; assign_dev: [n].
 int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, uint32_t dimpad, const float *xnorm2, const float *dnorm2,
-                  uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric, uint32_t *assign_dev, cudaStream_t stream,
-                  uint64_t *launches, void **scratch, size_t *scratch_bytes) {
+                  uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric, AssignTies ties, uint32_t *assign_dev,
+                  cudaStream_t stream, uint64_t *launches, void **scratch, size_t *scratch_bytes) {
     using namespace asg;
     if (n == 0) return 0;
+    if (ties.cap < n) { set_error("assign_tensor: near-tie list shorter than the shard"); return -1; }
     const uint32_t nqb = (K + QT - 1) / QT, Kpad = nqb * QT;
     const float acc_c = (float)dim * 2.384185791015625e-7f + 4e-6f;
-    // scratch: bf16 centroids [Kpad x dimpad], qn / qa / qb [Kpad], near-tie list (every row could be one)
-    const size_t off_q = 0, off_f = ((size_t)Kpad * dimpad * 2 + 255) & ~(size_t)255, off_amb = off_f + (((size_t)3 * Kpad * 4 + 255) & ~(size_t)255);
-    const size_t total = off_amb + 4 + (size_t)n * 4 + (size_t)n * 16 + 64;
+    // scratch: bf16 centroids [Kpad x dimpad], qn / qa / qb [Kpad]
+    const size_t off_q = 0, off_f = ((size_t)Kpad * dimpad * 2 + 255) & ~(size_t)255;
+    const size_t total = off_f + (size_t)3 * Kpad * 4;
     if (ws_reserve(scratch, scratch_bytes, total)) return -1;  // grow-only, reused across calls
     unsigned char *buf = static_cast<unsigned char *>(*scratch);
     float *qn = reinterpret_cast<float *>(buf + off_f), *qa = qn + Kpad, *qb = qa + Kpad;
-    uint32_t *amb_count = reinterpret_cast<uint32_t *>(buf + off_amb);
-    uint32_t *amb_rows = amb_count + 1;
-    uint32_t *amb_cand = amb_rows + n;
+    uint32_t *amb_count = ties.count, *amb_rows = ties.rows, *amb_cand = ties.cand;
     int rc = 0;
     do {
         if (cudaMemsetAsync(amb_count, 0, 4, stream) != cudaSuccess) { rc = -1; break; }
@@ -291,6 +319,7 @@ int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, u
         PrepParams pp = prep_params(a, Kpad, dimpad);
         pp.acc_c = acc_c; pp.qbf = reinterpret_cast<uint16_t *>(buf + off_q); pp.qnorm = qn; pp.qa = qa; pp.qb = qb;
         if (launch_prep(di, pp, stream, launches)) { rc = -1; break; }
+        assign_mark_nonfinite_kernel<<<(K + 7) / 8, 256, 0, stream>>>(centroids_dev, K, dim, qb);
         CUtensorMap map_rows, map_q;
         if (tc_make_map(&map_rows, shadow, n, dimpad, 2, BKB, ROWS, (uint64_t)dimpad * 2)) { rc = -1; break; }
         if (tc_make_map(&map_q, buf + off_q, Kpad, dimpad, 2, BKB, QT, (uint64_t)dimpad * 2)) { rc = -1; break; }
@@ -305,7 +334,7 @@ int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, u
         assign_scan_kernel<<<grid, NTHREADS, smem, stream>>>(map_rows, map_q, p);
         assign_fixup_kernel<<<di.num_sms * 4, 256, 0, stream>>>(rows, dim, centroids_dev, K, metric, amb_count, n, amb_rows, amb_cand, assign_dev);
         if (cudaGetLastError() != cudaSuccess) { rc = -1; break; }
-        if (launches) *launches += 2;
+        if (launches) *launches += 3;
     } while (0);
     if (rc != 0) {
         cudaError_t e = cudaGetLastError();
@@ -313,6 +342,48 @@ int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, u
     }
     cudaStreamSynchronize(stream);
     return rc;
+}
+
+// The search path's near-ties.  idx / sc: [n x k] results of a k = min(2, K) search of the rows against the centroids
+// (warp_exact_score's fp32 scores, euclidean as the distance).  Each such score is within acc_c of the real cosine, or within
+// acc_c d^2 of the real squared distance d^2, and kmeans.go's own arithmetic is within 2^-22 d^2 of it, so a row whose top
+// two are further apart than 3 acc_c (d1^2 under euclidean) has the search's winner as the contract's; the others, and
+// every row with a non-finite score or a missing result, are listed as ALL (DESIGN §7 item 3).
+__global__ void assign_search_ties_kernel(const uint32_t *idx, const float *sc, uint32_t n, uint32_t k, uint32_t K, int metric,
+                                          float acc_c, uint32_t *assign, uint32_t *amb_count, uint32_t *amb_rows, uint32_t *amb_cand) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n) return;
+    const uint32_t i0 = idx[(size_t)r * k];
+    assign[r] = i0 < K ? i0 : 0u;
+    if (K < 2) return;  // one centroid: it is every row's
+    const uint32_t i1 = idx[(size_t)r * k + 1];
+    const double s0 = sc[(size_t)r * k], s1 = sc[(size_t)r * k + 1];
+    bool tie = !(i0 < K && i1 < K && isfinite(s0) && isfinite(s1));
+    if (!tie) {
+        if (metric == NK_METRIC_EUCLIDEAN) tie = s1 * s1 - s0 * s0 <= 3.0 * acc_c * (s1 * s1);
+        else tie = s0 - s1 <= 3.0 * acc_c;
+    }
+    if (tie) {
+        const uint32_t pos = atomicAdd(amb_count, 1u);
+        amb_rows[pos] = r;
+        amb_cand[4 * pos] = asg::ALL;
+        amb_cand[4 * pos + 1] = amb_cand[4 * pos + 2] = amb_cand[4 * pos + 3] = asg::NONE;
+    }
+}
+
+int assign_from_search(const DeviceInfo &di, const float *rows, uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric,
+                       const uint32_t *idx, const float *sc, uint32_t k, AssignTies ties, uint32_t *assign_dev, cudaStream_t stream,
+                       uint64_t *launches) {
+    if (n == 0) return 0;
+    if (ties.cap < n) { set_error("assign_from_search: near-tie list shorter than the shard"); return -1; }
+    const float acc_c = (float)dim * 2.384185791015625e-7f + 4e-6f;
+    if (cudaMemsetAsync(ties.count, 0, 4, stream) != cudaSuccess) return -1;
+    assign_search_ties_kernel<<<(n + 255) / 256, 256, 0, stream>>>(idx, sc, n, k, K, metric, acc_c, assign_dev, ties.count, ties.rows, ties.cand);
+    assign_fixup_kernel<<<di.num_sms * 4, 256, 0, stream>>>(rows, dim, centroids_dev, K, metric, ties.count, n, ties.rows, ties.cand, assign_dev);
+    if (launches) *launches += 2;
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) { set_error("assign_from_search: %s", cudaGetErrorString(e)); return -1; }
+    return 0;
 }
 
 }  // namespace nk

@@ -2212,10 +2212,13 @@ int nk_score_subset(NkIndex *ix, const float *query_host, const uint32_t *rows_h
 }
 
 // ---- k-means routing on device (pkg/gpu/kmeans.go; SURVEY.md §8(f)4) -----------------------------------------------
-// Assignment is the fused scan with the roles swapped: the K centroids are the indexed corpus, the shard's rows are the
-// queries — read in place from HBM, 8192 at a time — and k = 1.  Ties go to the lowest centroid index (strict < / >
-// in kmeans.go:470-476,529-534).
-int nk_index_assign_nearest(NkIndex *ix, const float *centroids_host, uint32_t K, int metric, int32_t *assign_io, uint64_t *changed) {
+// Assignment (DESIGN §7 item 3).  With a usable BF16 shadow it is ONE pass of the tensor-core scan with an argmax
+// epilogue (assign_tensor.cu); otherwise the fused kNN scan with the roles swapped: the K centroids are the indexed corpus,
+// the shard's rows are the queries — read in place from HBM, 8192 at a time — and k = min(2, K).  Either way the rows a
+// rigorous bound cannot decide are listed and assign_fixup_kernel decides them with the contract's arithmetic, so both
+// paths return the same assignment.  ties_* (tests, single-device index): the near-tie list of that call.
+static int assign_nearest(NkIndex *ix, const float *centroids_host, uint32_t K, int metric, int32_t *assign_io, uint64_t *changed,
+                          uint32_t *ties_rows, uint32_t *ties_cand, uint32_t ties_cap, uint32_t *ties_count) {
     nk::DeviceGuard _restore_device;
     if (!ix || !centroids_host || !assign_io) { nk::set_error("null argument"); return -1; }
     if (ix->dtype != NK_DTYPE_F32) { nk::set_error("nk_index_assign_nearest: fp32 index required"); return -1; }
@@ -2225,45 +2228,64 @@ int nk_index_assign_nearest(NkIndex *ix, const float *centroids_host, uint32_t K
     ShardOrder order(ix);
     if (order.failed()) return -1;
     uint64_t total_changed = 0, off = 0;
+    if (ties_count) *ties_count = 0;
     for (auto &s : ix->shards) {
         if (s.n == 0) continue;
         NK_CUDA_OK(cudaSetDevice(s.device));
-        // With a BF16 shadow the assignment is ONE pass of the tensor-core scan with an argmax epilogue (assign_tensor.cu);
-        // otherwise the fused kNN scan with the roles swapped: centroids as the corpus, rows as the queries, k = 1.
         const bool tensor = s.shadow && s.shadow_n == s.n && nk::assign_tensor_supported(s.di, ix->dim, K, metric);
+        const uint32_t k = K < 2 ? K : 2u;
         NkIndex *cx = tensor ? nullptr : nk_index_create(&s.device, 1, ix->dim, NK_DTYPE_F32, metric);
         if (!tensor && !cx) return -1;
-        // one grow-only scratch buffer per shard, carved up (no cudaMalloc / cudaFree per call)
-        const size_t n4 = (s.n * 4 + 255) & ~(size_t)255, cen_b = tensor ? (((size_t)K * ix->dim * 4 + 255) & ~(size_t)255) : 0;
+        // one grow-only scratch buffer per shard, carved up (no cudaMalloc / cudaFree per call): search results [n x k]
+        // (indices, scores), the assignment, the previous one, the changed count, the near-tie list, the centroids
+        const size_t n4 = (s.n * 4 + 255) & ~(size_t)255, cen_b = ((size_t)K * ix->dim * 4 + 255) & ~(size_t)255;
+        const size_t o_sc = 2 * n4, o_asg = 4 * n4, o_prev = 5 * n4, o_chg = 6 * n4, o_tc = o_chg + 256, o_tr = o_tc + 256, o_tcand = o_tr + n4,
+                     o_cen = o_tcand + 4 * n4;
         unsigned long long h_changed = 0;
         int rc = tensor ? 0 : nk_index_upload(cx, centroids_host, K);
-        if (rc == 0 && nk::ws_reserve(&s.ws.scratch, &s.ws.scratch_bytes, 3 * n4 + 256 + cen_b)) rc = -1;
+        if (rc == 0 && nk::ws_reserve(&s.ws.scratch, &s.ws.scratch_bytes, o_cen + cen_b)) rc = -1;
         unsigned char *base = static_cast<unsigned char *>(s.ws.scratch);
         uint32_t *d_idx = reinterpret_cast<uint32_t *>(base);
-        float *d_sc = reinterpret_cast<float *>(base + n4);
-        int32_t *d_prev = reinterpret_cast<int32_t *>(base + 2 * n4);
-        unsigned long long *d_changed = reinterpret_cast<unsigned long long *>(base + 3 * n4);
-        float *d_cen = reinterpret_cast<float *>(base + 3 * n4 + 256);
+        float *d_sc = reinterpret_cast<float *>(base + o_sc);
+        uint32_t *d_asg = reinterpret_cast<uint32_t *>(base + o_asg);
+        int32_t *d_prev = reinterpret_cast<int32_t *>(base + o_prev);
+        unsigned long long *d_changed = reinterpret_cast<unsigned long long *>(base + o_chg);
+        nk::AssignTies ties;
+        ties.count = reinterpret_cast<uint32_t *>(base + o_tc);
+        ties.rows = reinterpret_cast<uint32_t *>(base + o_tr);
+        ties.cand = reinterpret_cast<uint32_t *>(base + o_tcand);
+        ties.cap = (uint32_t)s.n;
+        float *d_cen = reinterpret_cast<float *>(base + o_cen);
         cudaError_t e = cudaSuccess;
         if (rc == 0) {
-            if (tensor) e = cudaMemcpyAsync(d_cen, centroids_host, (size_t)K * ix->dim * 4, cudaMemcpyHostToDevice, s.stream);
+            e = cudaMemcpyAsync(d_cen, centroids_host, (size_t)K * ix->dim * 4, cudaMemcpyHostToDevice, s.stream);
             if (e == cudaSuccess) e = cudaMemsetAsync(d_changed, 0, 8, s.stream);
             if (e == cudaSuccess) e = cudaMemcpyAsync(d_prev, assign_io + off, s.n * 4, cudaMemcpyHostToDevice, s.stream);
             if (e != cudaSuccess) rc = -1;
         }
+        const float *rows = static_cast<const float *>(s.rows);
         if (rc == 0 && tensor) {
-            rc = nk::assign_tensor(s.di, static_cast<const float *>(s.rows), s.shadow, ix->dimpad(), s.xnorm2, s.dnorm2, (uint32_t)s.n, ix->dim,
-                                   d_cen, K, metric, d_idx, s.stream, &ix->stats.kernel_launches, &s.ws.sub_gather, &s.ws.sub_gather_bytes);
+            rc = nk::assign_tensor(s.di, rows, s.shadow, ix->dimpad(), s.xnorm2, s.dnorm2, (uint32_t)s.n, ix->dim, d_cen, K, metric, ties, d_asg,
+                                   s.stream, &ix->stats.kernel_launches, &s.ws.sub_gather, &s.ws.sub_gather_bytes);
         }
         const uint64_t B = 8192;  // rows per fused search: amortises the ~12 fixed launches of a search over 8 scan launches
         for (uint64_t b = 0; rc == 0 && !tensor && b < s.n; b += B) {
             const uint32_t nb = (uint32_t)std::min<uint64_t>(B, s.n - b);
-            if (nk_search_device(cx, static_cast<const float *>(s.rows) + b * ix->dim, nb, 1, d_idx + b, d_sc + b, s.stream) < 0) rc = -1;
+            if (nk_search_device(cx, rows + b * ix->dim, nb, k, d_idx + b * k, d_sc + b * k, s.stream) < 0) rc = -1;
         }
-        if (rc == 0 && nk::count_changed(d_prev, d_idx, s.n, d_changed, s.stream)) rc = -1;
+        if (rc == 0 && !tensor)
+            rc = nk::assign_from_search(s.di, rows, (uint32_t)s.n, ix->dim, d_cen, K, metric, d_idx, d_sc, k, ties, d_asg, s.stream,
+                                        &ix->stats.kernel_launches);
+        if (rc == 0 && nk::count_changed(d_prev, d_asg, s.n, d_changed, s.stream)) rc = -1;
+        uint32_t h_ties = 0;
         if (rc == 0) {
-            e = cudaMemcpyAsync(assign_io + off, d_idx, s.n * 4, cudaMemcpyDeviceToHost, s.stream);
+            e = cudaMemcpyAsync(assign_io + off, d_asg, s.n * 4, cudaMemcpyDeviceToHost, s.stream);
             if (e == cudaSuccess) e = cudaMemcpyAsync(&h_changed, d_changed, 8, cudaMemcpyDeviceToHost, s.stream);
+            if (e == cudaSuccess && ties_count) e = cudaMemcpyAsync(&h_ties, ties.count, 4, cudaMemcpyDeviceToHost, s.stream);
+            if (e == cudaSuccess) e = cudaStreamSynchronize(s.stream);
+            const uint32_t m = std::min(h_ties, ties_cap);
+            if (e == cudaSuccess && m) e = cudaMemcpyAsync(ties_rows, ties.rows, (size_t)m * 4, cudaMemcpyDeviceToHost, s.stream);
+            if (e == cudaSuccess && m) e = cudaMemcpyAsync(ties_cand, ties.cand, (size_t)m * 16, cudaMemcpyDeviceToHost, s.stream);
             if (e == cudaSuccess) e = cudaStreamSynchronize(s.stream);
             if (e != cudaSuccess) rc = -1;
         }
@@ -2272,11 +2294,29 @@ int nk_index_assign_nearest(NkIndex *ix, const float *centroids_host, uint32_t K
         ix->stats.kernel_launches += (cx ? cx->stats.kernel_launches : 0) + 1;
         if (cx) nk_index_release(cx);
         if (rc != 0) return -1;
+        if (ties_count) *ties_count = h_ties;
         total_changed += h_changed;
         off += s.n;
     }
     if (changed) *changed = total_changed;
     return 0;
+}
+
+int nk_index_assign_nearest(NkIndex *ix, const float *centroids_host, uint32_t K, int metric, int32_t *assign_io, uint64_t *changed) {
+    return assign_nearest(ix, centroids_host, K, metric, assign_io, changed, nullptr, nullptr, 0, nullptr);
+}
+
+// Tests only: run the assignment of every row (from a zero assignment; the result is discarded) and return the number of
+// rows it listed as near-ties; the first min(count, cap) rows and their 4 candidate ids are copied to rows_out / cand_out.
+int nk_debug_assign_ties(NkIndex *ix, const float *centroids_host, uint32_t K, int metric, uint32_t *rows_out, uint32_t *cand_out,
+                         uint32_t cap) {
+    if (!ix || ix->shards.size() != 1) { nk::set_error("single-device index required"); return -1; }
+    if (cap && (!rows_out || !cand_out)) { nk::set_error("null argument"); return -1; }
+    if (ix->shards[0].n == 0) return 0;
+    std::vector<int32_t> assign(ix->shards[0].n, 0);
+    uint32_t count = 0;
+    if (assign_nearest(ix, centroids_host, K, metric, assign.data(), nullptr, rows_out, cand_out, cap, &count)) return -1;
+    return (int)count;
 }
 
 // Update step (kmeans.go:585-618): centroid c <- float32(mean in float64 of the rows assigned to c); clusters without

@@ -116,11 +116,22 @@ int scan_filter_dump(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, int
 // fp32 rows [first, first+count) -> bf16 shadow rows (stride dimpad) + |x|^2, |x - bf16(x)|^2
 int build_shadow(const float *rows, uint64_t first, uint64_t count, uint32_t dim, uint32_t dimpad, void *shadow, float *xnorm2,
                  float *dnorm2, cudaStream_t stream);
-// k-means assignment as one pass of the 16-bit scan with an argmax epilogue (assign_tensor.cu).
+// k-means assignment (assign_tensor.cu).  Both paths list their near-tie rows (device buffers: count, rows [cap], 4
+// candidate ids per row, 0xfffffffe = every centroid) and decide them with assign_fixup_kernel's contract arithmetic; the
+// list stays readable after the call (nk_debug_assign_ties).  cap >= n.
+struct AssignTies {
+    uint32_t *count = nullptr, *rows = nullptr, *cand = nullptr;
+    uint32_t cap = 0;
+};
+// One pass of the 16-bit scan with an argmax epilogue.
 bool assign_tensor_supported(const DeviceInfo &di, uint32_t dim, uint32_t K, int metric);
 int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, uint32_t dimpad, const float *xnorm2, const float *dnorm2,
-                  uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric, uint32_t *assign_dev, cudaStream_t stream,
-                  uint64_t *launches, void **scratch, size_t *scratch_bytes);
+                  uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric, AssignTies ties, uint32_t *assign_dev,
+                  cudaStream_t stream, uint64_t *launches, void **scratch, size_t *scratch_bytes);
+// From a k = min(2, K) search of the rows against the centroids (idx / sc: [n x k], euclidean scores as distances).
+int assign_from_search(const DeviceInfo &di, const float *rows, uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric,
+                       const uint32_t *idx, const float *sc, uint32_t k, AssignTies ties, uint32_t *assign_dev, cudaStream_t stream,
+                       uint64_t *launches);
 
 // A shard's fatal status word (FLAG_FATAL) held `flag`: clear the word on `stream` (flags == nullptr: the caller has cleared
 // it), set the error message and return -1.

@@ -161,6 +161,20 @@ class KnnIndex:
                                              est.ctypes.data_as(C.c_void_p), bnd.ctypes.data_as(C.c_void_p)), "nk_debug_filter_dump")
         return est, bnd
 
+    def assign_ties(self, centroids, metric: str = "euclidean") -> Tuple[np.ndarray, np.ndarray]:
+        """Tests only: (rows, candidates [rows x 4]) that assign_nearest listed as near-ties and decided exactly;
+        candidate 0xfffffffe = every centroid, 0xffffffff = none.  Every other row was decided by the error bound."""
+        c = np.ascontiguousarray(np.asarray(centroids, dtype=np.float32))
+        if c.ndim != 2 or c.shape[1] != self.dim:
+            raise KnnError(f"invalid dimensions: centroids {c.shape}, index has {self.dim}")
+        n = len(self)
+        rows = np.empty(max(n, 1), dtype=np.uint32)
+        cand = np.empty((max(n, 1), 4), dtype=np.uint32)
+        m = _check(self.lib.nk_debug_assign_ties(self.ptr, c.ctypes.data_as(C.c_void_p), c.shape[0], METRICS[metric],
+                                                 rows.ctypes.data_as(C.c_void_p), cand.ctypes.data_as(C.c_void_p), n),
+                   "nk_debug_assign_ties")
+        return rows[:m].copy(), cand[:m].copy()
+
     def status(self, stream: int = 0) -> None:
         _check(self.lib.nk_index_status(self.ptr, stream), "nk_index_status")
 
