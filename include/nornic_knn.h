@@ -92,7 +92,8 @@ enum { NK_DTYPE_F32 = 0, NK_DTYPE_F16 = 1, NK_DTYPE_BF16 = 2 };
 /* TENSOR = exact 3xTF32 tensor-core scan; TENSOR_FILTER = 1xTF32 prefilter over the fp32 rows with rigorous margins +
  * exact fp32 rescoring (device-side fallback to the exact scan on margin overflow); TENSOR_SHADOW = the same filter
  * streaming a BF16 shadow copy of the shard (half the HBM bytes; built at upload for library-owned fp32 shards unless
- * NK_SHADOW=0, +50% device memory), exact fp32 rescoring from the fp32 rows, device-side retry through TENSOR_FILTER
+ * NK_SHADOW=0, +50% device memory; plus an int8 copy with one scale per row, +25%, a quarter of the fp32 bytes, which
+ * serves k <= 16 on large shards), exact fp32 rescoring from the fp32 rows, device-side retry through TENSOR_FILTER
  * and then the exact scan.  All paths return identical index sets. */
 enum { NK_PATH_AUTO = 0, NK_PATH_SIMT = 1, NK_PATH_TENSOR = 2, NK_PATH_TENSOR_FILTER = 3, NK_PATH_TENSOR_SHADOW = 4 };
 

@@ -9,7 +9,8 @@
 // four lanes that share a row merge their lists at the end.
 //   cosine    (assignToCentroidsGPU, kmeans.go:491-546)  score = x.c/|c|            (|x| > 0 does not change the argmax)
 //   euclidean (assignToCentroids,    kmeans.go:458-489)  score = 2 x.c - |c|^2      (argmin |x-c|^2)
-// with the rigorous BF16 bound of scan_tensor_shadow.cu, widened under euclidean by the rounding of kmeans.go's own
+// with the rigorous bound of scan_tensor_shadow.cu (over the BF16 shadow, or the int8 image: s8 MMAs, 128-byte slabs of
+// 128 elements, the estimate scaled by the row's and the centroid's scales), widened under euclidean by the rounding of kmeans.go's own
 // arithmetic (fp32 differences: 2^-22 (|x|^2 - lo), DESIGN §7 item 3).  A row whose runner-up cannot reach the winner's
 // lower bound is decided; the others (near-ties) are listed with their <= 3 candidates (or ALL) and assign_fixup_kernel
 // decides them with the contract's arithmetic: squaredEuclidean bit for bit, or the fp64 cosine (strict comparison in
@@ -38,10 +39,11 @@ constexpr int EPI_WARP0 = 4;
 constexpr uint32_t NONE = 0xffffffffu, ALL = 0xfffffffeu;
 
 struct Params {
-    uint32_t n, nslab, K, nqb;   // rows, 64-element slabs per row, centroids, blocks of 128 centroids
+    uint32_t n, nslab, K, nqb;   // rows, 128-byte slabs per row, centroids, blocks of 64 centroids
     int metric;
     const float *qn, *qa, *qb;   // per centroid (padded): |c| (1 for cosine), bound factors
     const float *xnorm2, *dnorm2;
+    const float *xscale, *qscale;  // int8 image: per row, per centroid (padded)
     uint32_t *assign;            // [n] out
     uint32_t *amb_count, *amb_rows, *amb_cand;  // near-ties: count, rows, 4 candidates each (ALL = every centroid)
     uint32_t amb_cap;
@@ -52,6 +54,7 @@ struct __align__(8) Shared {
 };
 }  // namespace asg
 
+template <ptx::Opnd OP>
 __global__ void __launch_bounds__(asg::NTHREADS, 1)
 assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_q, asg::Params p) {
     using namespace asg;
@@ -62,6 +65,8 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
     Shared &sh = *reinterpret_cast<Shared *>(smem_raw + (size_t)RING_BYTES);
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const uint32_t num_tiles = (p.n + ROWS - 1) / ROWS, nslab = p.nslab, nqb = p.nqb;
+    constexpr bool S8 = OP == ptx::Opnd::S8;
+    constexpr uint32_t KCOLS = S8 ? 128 : BKB;  // elements per 128-byte slab row
 
     if (warp == 0 && lane == 0) {
         ptx::prefetch_tensormap(&map_rows);
@@ -74,14 +79,14 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
         // TMA producer: shadow slabs; a tile is streamed once per centroid block (first from HBM, then from L2)
         tma_producer<ASTAGES>(sh.ring.aempty, blockIdx.x, num_tiles, gridDim.x, nqb, nslab, false, [&](uint32_t s, uint32_t tile, uint32_t qbk, uint32_t j) {
             ptx::mbar_arrive_expect_tx(&sh.ring.afull[s], A_BYTES);
-            ptx::tma_load_2d(&map_rows, &sh.ring.afull[s], a_base + (size_t)s * A_BYTES, (int32_t)(j * BKB), (int32_t)(tile * ROWS),
+            ptx::tma_load_2d(&map_rows, &sh.ring.afull[s], a_base + (size_t)s * A_BYTES, (int32_t)(j * KCOLS), (int32_t)(tile * ROWS),
                              qbk + 1 == nqb ? ptx::CACHE_EVICT_FIRST : ptx::CACHE_EVICT_NORMAL);
         });
     } else if (warp == 3) {
         // TMA producer: centroid slabs (L2-resident)
         tma_producer<BSTAGES>(sh.ring.bempty, blockIdx.x, num_tiles, gridDim.x, nqb, nslab, false, [&](uint32_t s, uint32_t, uint32_t qbk, uint32_t j) {
             ptx::mbar_arrive_expect_tx(&sh.ring.bfull[s], B_BYTES);
-            ptx::tma_load_2d(&map_q, &sh.ring.bfull[s], b_base + (size_t)s * B_BYTES, (int32_t)(j * BKB), (int32_t)(qbk * QT), ptx::CACHE_EVICT_LAST);
+            ptx::tma_load_2d(&map_q, &sh.ring.bfull[s], b_base + (size_t)s * B_BYTES, (int32_t)(j * KCOLS), (int32_t)(qbk * QT), ptx::CACHE_EVICT_LAST);
         });
     } else if (warp >= EPI_WARP0) {
         // consumers: warpgroup m owns rows [128 m, 128 m + 128) of the tile as two m64 halves h; thread = 4 rows
@@ -98,7 +103,7 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
             for (int i = 0; i < QT / 2; ++i) acc[h][i] = 0.0f;
         uint32_t g = 0;
         for (uint32_t tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-            float x2[4], ra[4], rb[4], maxlo[4], u[4][4];
+            float x2[4], ra[4], rb[4], xs[4], maxlo[4], u[4][4];
             uint32_t id[4][4];
 #pragma unroll
             for (int ri = 0; ri < 4; ++ri) {
@@ -107,6 +112,7 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                 const float dxn = sqrtf(row < p.n ? __ldg(p.dnorm2 + row) : 0.0f) * 1.0001f;
                 ra[ri] = mul * dxn;
                 rb[ri] = mul * sqrtf(x2[ri]);
+                xs[ri] = S8 ? mul * (row < p.n ? __ldg(p.xscale + row) : 0.0f) : mul;  // the estimate's multiplier
                 maxlo[ri] = -INFINITY;
 #pragma unroll
                 for (int e = 0; e < 4; ++e) { u[ri][e] = -INFINITY; id[ri][e] = NONE; }
@@ -123,7 +129,7 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                     for (uint32_t h = 0; h < 2; ++h) {
                         const uint64_t adesc = ptx::make_smem_desc_sw128(abase + h * (A_BYTES / 4));
 #pragma unroll
-                        for (uint32_t kk = 0; kk < 4; ++kk) ptx::wgmma_bf16_n64(acc[h], adesc + kk * 2, bdesc + kk * 2, (j | kk) != 0);
+                        for (uint32_t kk = 0; kk < 4; ++kk) ptx::wgmma_op<QT, OP>(acc[h], adesc + kk * 2, bdesc + kk * 2, (j | kk) != 0);
                     }
                     ptx::wgmma_commit();
                     ptx::wgmma_wait_all();
@@ -138,9 +144,11 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                     if (ci >= p.K) continue;
                     const float qn = __ldg(p.qn + ci), qa = __ldg(p.qa + ci), qb = __ldg(p.qb + ci);
                     const float cc = euclid ? qn * qn : 0.0f;
+                    const float qs = S8 ? __ldg(p.qscale + ci) : 1.0f;
 #pragma unroll
                     for (int ri = 0; ri < 4; ++ri) {
-                        const float s = fmaf(acc[ri >> 1][(jj >> 1) * 4 + (ri & 1) * 2 + (jj & 1)], mul, -cc);
+                        const float av = acc[ri >> 1][(jj >> 1) * 4 + (ri & 1) * 2 + (jj & 1)];
+                        const float s = fmaf(S8 ? __int2float_rn(__float_as_int(av)) * qs : av, xs[ri], -cc);
                         float bnd = fmaf(ra[ri], qa, rb[ri] * qb) + 1e-6f * cc;
                         // kmeans.go rounds every difference x_j - c_j to fp32: its squared distance is within 2^-23 (1 + 2^-15) of
                         // the exact one, which is at most |x|^2 - lo <= 1.001 xx - lo (xx: the fp32 |x|^2, relative error < 6.3e-5)
@@ -296,20 +304,22 @@ bool assign_tensor_supported(const DeviceInfo &di, uint32_t dim, uint32_t K, int
 }
 
 // rows / shadow / norms: one shard (device pointers); centroids_dev: [K x dim] fp32 on the same device; assign_dev: [n].
-int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, uint32_t dimpad, const float *xnorm2, const float *dnorm2,
-                  uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric, AssignTies ties, uint32_t *assign_dev,
+int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, uint32_t dimpad, const float *xscale, const float *xnorm2,
+                  const float *dnorm2, uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric, AssignTies ties, uint32_t *assign_dev,
                   cudaStream_t stream, uint64_t *launches, void **scratch, size_t *scratch_bytes) {
     using namespace asg;
     if (n == 0) return 0;
     if (ties.cap < n) { set_error("assign_tensor: near-tie list shorter than the shard"); return -1; }
     const uint32_t nqb = (K + QT - 1) / QT, Kpad = nqb * QT;
     const float acc_c = (float)dim * 2.384185791015625e-7f + 4e-6f;
-    // scratch: bf16 centroids [Kpad x dimpad], qn / qa / qb [Kpad]
-    const size_t off_q = 0, off_f = ((size_t)Kpad * dimpad * 2 + 255) & ~(size_t)255;
-    const size_t total = off_f + (size_t)3 * Kpad * 4;
+    // scratch: bf16 (int8 image: int8) centroids [Kpad x dimpad], qn / qa / qb (/ scales) [Kpad]
+    const bool s8 = xscale != nullptr;
+    const uint32_t esz = s8 ? 1 : 2;
+    const size_t off_q = 0, off_f = ((size_t)Kpad * dimpad * esz + 255) & ~(size_t)255;
+    const size_t total = off_f + (size_t)4 * Kpad * 4;
     if (ws_reserve(scratch, scratch_bytes, total)) return -1;  // grow-only, reused across calls
     unsigned char *buf = static_cast<unsigned char *>(*scratch);
-    float *qn = reinterpret_cast<float *>(buf + off_f), *qa = qn + Kpad, *qb = qa + Kpad;
+    float *qn = reinterpret_cast<float *>(buf + off_f), *qa = qn + Kpad, *qb = qa + Kpad, *qsc = qb + Kpad;
     uint32_t *amb_count = ties.count, *amb_rows = ties.rows, *amb_cand = ties.cand;
     int rc = 0;
     do {
@@ -317,21 +327,26 @@ int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, u
         ScanArgs a;
         a.queries = centroids_dev; a.Q = K; a.dim = dim; a.metric = metric;
         PrepParams pp = prep_params(a, Kpad, dimpad);
-        pp.acc_c = acc_c; pp.qbf = reinterpret_cast<uint16_t *>(buf + off_q); pp.qnorm = qn; pp.qa = qa; pp.qb = qb;
+        pp.acc_c = acc_c; pp.qnorm = qn; pp.qa = qa; pp.qb = qb;
+        if (s8) { pp.qs8 = reinterpret_cast<int8_t *>(buf + off_q); pp.qscale = qsc; }
+        else pp.qbf = reinterpret_cast<uint16_t *>(buf + off_q);
         if (launch_prep(di, pp, stream, launches)) { rc = -1; break; }
         assign_mark_nonfinite_kernel<<<(K + 7) / 8, 256, 0, stream>>>(centroids_dev, K, dim, qb);
         CUtensorMap map_rows, map_q;
-        if (tc_make_map(&map_rows, shadow, n, dimpad, 2, BKB, ROWS, (uint64_t)dimpad * 2)) { rc = -1; break; }
-        if (tc_make_map(&map_q, buf + off_q, Kpad, dimpad, 2, BKB, QT, (uint64_t)dimpad * 2)) { rc = -1; break; }
+        if (tc_make_map(&map_rows, shadow, n, dimpad, esz, 128 / esz, ROWS, (uint64_t)dimpad * esz)) { rc = -1; break; }
+        if (tc_make_map(&map_q, buf + off_q, Kpad, dimpad, esz, 128 / esz, QT, (uint64_t)dimpad * esz)) { rc = -1; break; }
         const size_t smem = (size_t)RING_BYTES + sizeof(Shared) + 1024;
-        if (cudaFuncSetAttribute(assign_scan_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { rc = -1; break; }
+        const void *kern = s8 ? reinterpret_cast<const void *>(assign_scan_kernel<ptx::Opnd::S8>)
+                              : reinterpret_cast<const void *>(assign_scan_kernel<ptx::Opnd::BF16>);
+        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { rc = -1; break; }
         asg::Params p;
-        p.n = n; p.nslab = dimpad / BKB; p.K = K; p.nqb = nqb; p.metric = metric;
-        p.qn = qn; p.qa = qa; p.qb = qb; p.xnorm2 = xnorm2; p.dnorm2 = dnorm2;
+        p.n = n; p.nslab = dimpad * esz / 128; p.K = K; p.nqb = nqb; p.metric = metric;
+        p.qn = qn; p.qa = qa; p.qb = qb; p.xnorm2 = xnorm2; p.dnorm2 = dnorm2; p.xscale = xscale; p.qscale = qsc;
         p.assign = assign_dev; p.amb_count = amb_count; p.amb_rows = amb_rows; p.amb_cand = amb_cand; p.amb_cap = n;
         const uint32_t num_tiles = (n + ROWS - 1) / ROWS;
         const uint32_t grid = num_tiles < (uint32_t)di.num_sms ? num_tiles : (uint32_t)di.num_sms;
-        assign_scan_kernel<<<grid, NTHREADS, smem, stream>>>(map_rows, map_q, p);
+        if (s8) assign_scan_kernel<ptx::Opnd::S8><<<grid, NTHREADS, smem, stream>>>(map_rows, map_q, p);
+        else assign_scan_kernel<ptx::Opnd::BF16><<<grid, NTHREADS, smem, stream>>>(map_rows, map_q, p);
         assign_fixup_kernel<<<di.num_sms * 4, 256, 0, stream>>>(rows, dim, centroids_dev, K, metric, amb_count, n, amb_rows, amb_cand, assign_dev);
         if (cudaGetLastError() != cudaSuccess) { rc = -1; break; }
         if (launches) *launches += 3;

@@ -26,10 +26,19 @@ struct NkShard {
     void *rows = nullptr;
     bool owns = true;
     uint64_t n = 0, cap = 0, base = 0;
-    // BF16 shadow of an owned fp32 shard (scan_tensor_shadow.cu): rows [0, shadow_n) are converted; capacity in rows
+    // Images of an owned fp32 shard that the filter scans (scan_tensor_shadow.cu): the BF16 shadow (+ |x - bf16(x)|^2 per
+    // row) and the int8 image img8 (+ per-row scale xscale and |x - s_x xq|^2), either or both; |x|^2 is shared.  Rows
+    // [0, shadow_n) are converted; capacity in rows.
     // 16-bit shards (fp16 / bf16) are scanned in place by the same kernel: they only carry xnorm2 (shadow stays null).
-    void *shadow = nullptr;
-    float *xnorm2 = nullptr, *dnorm2 = nullptr;
+    void *shadow = nullptr, *img8 = nullptr;
+    float *xnorm2 = nullptr, *dnorm2 = nullptr, *xscale = nullptr, *d8norm2 = nullptr;
+    // The int8 image is dropped from the kNN filter of this shard once a search on it overflowed its margin buffers (a
+    // near-tie-heavy corpus: its ~3x wider margins send such searches to the slower retry stages).  The overflow counters
+    // are copied to pinned memory behind every int8 search and read, without waiting, when the next search is planned.
+    mutable bool s8_off = false;
+    mutable cudaEvent_t s8_ev = nullptr;
+    mutable int *s8_h = nullptr;      // pinned: FLAG_N_RETRY, FLAG_N_EXACT after the last int8 search
+    mutable int64_t s8_seen = 0;      // their sum when last read
     uint64_t shadow_cap = 0, shadow_n = 0;
     bool shadow_attached = false;  // caller-owned rows: shadow built on request (nk_index_refresh_shadow)
     // last filter search (host-synchronous API): what the deferred retry tail needs
@@ -65,7 +74,11 @@ struct NkIndex {
     int dtype = NK_DTYPE_F32;
     int metric = NK_METRIC_COSINE;
     int path = NK_PATH_AUTO;
-    bool shadow_on = true;  // NK_SHADOW=0 at creation: never build the BF16 shadow (saves 50% HBM, halves filter speed)
+    // Images of fp32 shards, NK_SHADOW at creation: unset / 1 both the BF16 shadow (+50% HBM) and the int8 image (+25%;
+    // the int8 image alone is dropped when its memory cannot be had), bf16 the BF16 shadow only, int8 the int8 image only,
+    // 0 none
+    bool shadow_on = true;
+    bool image_bf16 = true, image_s8 = true;
     bool timing_on = false;
     int last_path = NK_PATH_SIMT;
     uint64_t row_base = 0;
@@ -85,6 +98,9 @@ struct NkIndex {
         return min_score > -INFINITY ? min_score : -INFINITY;
     }
     uint32_t dimpad() const { return (dim + 63) / 64 * 64; }
+    uint32_t dimpad8() const { return (dim + 127) / 128 * 128; }  // row stride (bytes) of the int8 image
+    bool s8() const { return image_s8 && dtype == NK_DTYPE_F32; }     // fp32 shards carry the int8 image
+    bool bf16() const { return image_bf16 || dtype != NK_DTYPE_F32; }  // ... the BF16 shadow (16-bit shards: their |x|^2)
     uint64_t rows() const {
         uint64_t t = 0;
         for (auto &s : shards) t += s.n;
@@ -204,12 +220,15 @@ static void shard_drop_shadow(NkShard &s) {
     if (s.shadow) cudaFree(s.shadow);
     if (s.xnorm2) cudaFree(s.xnorm2);
     if (s.dnorm2) cudaFree(s.dnorm2);
-    s.shadow = nullptr; s.xnorm2 = s.dnorm2 = nullptr;
+    if (s.img8) cudaFree(s.img8);
+    if (s.xscale) cudaFree(s.xscale);
+    if (s.d8norm2) cudaFree(s.d8norm2);
+    s.shadow = s.img8 = nullptr; s.xnorm2 = s.dnorm2 = s.xscale = s.d8norm2 = nullptr;
     s.shadow_cap = s.shadow_n = 0;
 }
 
-// Bring the 16-bit image of a shard up to date with rows [0, s.n) (converting only what is missing): the BF16 shadow + norms
-// of an fp32 shard, or just the |x|^2 array of an fp16 / bf16 shard (scanned in place).  It is an optimisation: if its memory
+// Bring the image of a shard up to date with rows [0, s.n) (converting only what is missing): the int8 image or the BF16
+// shadow + norms of an fp32 shard, or just the |x|^2 array of an fp16 / bf16 shard (scanned in place).  It is an optimisation: if its memory
 // cannot be had the shard simply goes without (TF32 filter / CUDA-core scan over the rows).
 static int shard_sync_shadow(NkIndex *ix, NkShard &s) {
     const bool f32 = ix->dtype == NK_DTYPE_F32;
@@ -218,14 +237,28 @@ static int shard_sync_shadow(NkIndex *ix, NkShard &s) {
         s.shadow_n = 0;
         return 0;
     }
-    const uint32_t dimpad = ix->dimpad();
+    const uint32_t dimpad = ix->dimpad(), dimpad8 = ix->dimpad8();
+    const bool bf = f32 && ix->bf16(), s8 = ix->s8();
     if (s.shadow_cap < s.n) {
         if (shard_drain(s)) return -1;
         shard_drop_shadow(s);
         const uint64_t cap = s.cap > s.n ? s.cap : s.n;
-        cudaError_t e = f32 ? cudaMalloc(&s.shadow, cap * dimpad * 2) : cudaSuccess;
-        if (e == cudaSuccess) e = cudaMalloc((void **)&s.xnorm2, cap * 4);
-        if (e == cudaSuccess && f32) e = cudaMalloc((void **)&s.dnorm2, cap * 4);
+        cudaError_t e = cudaMalloc((void **)&s.xnorm2, cap * 4);
+        if (e == cudaSuccess && bf) e = cudaMalloc(&s.shadow, cap * dimpad * 2);
+        if (e == cudaSuccess && bf) e = cudaMalloc((void **)&s.dnorm2, cap * 4);
+        if (e == cudaSuccess && s8) {
+            e = cudaMalloc(&s.img8, cap * dimpad8);
+            if (e == cudaSuccess) e = cudaMalloc((void **)&s.xscale, cap * 4);
+            if (e == cudaSuccess) e = cudaMalloc((void **)&s.d8norm2, cap * 4);
+            if (e != cudaSuccess && bf) {  // the shard keeps its BF16 shadow and goes without the int8 image
+                cudaGetLastError();
+                if (s.img8) cudaFree(s.img8);
+                if (s.xscale) cudaFree(s.xscale);
+                if (s.d8norm2) cudaFree(s.d8norm2);
+                s.img8 = nullptr; s.xscale = s.d8norm2 = nullptr;
+                e = cudaSuccess;
+            }
+        }
         if (e != cudaSuccess) {
             cudaGetLastError();
             shard_drop_shadow(s);
@@ -234,9 +267,12 @@ static int shard_sync_shadow(NkIndex *ix, NkShard &s) {
         s.shadow_cap = cap;
     }
     if (s.shadow_n < s.n) {
+        const float *rows = static_cast<const float *>(s.rows);
         if (f32) {
-            if (nk::build_shadow(static_cast<const float *>(s.rows), s.shadow_n, s.n - s.shadow_n, ix->dim, dimpad, s.shadow, s.xnorm2,
-                                 s.dnorm2, s.stream))
+            if (s.img8 && nk::build_image_s8(rows, s.shadow_n, s.n - s.shadow_n, ix->dim, dimpad8, s.img8, s.xscale, s.xnorm2, s.d8norm2,
+                                             s.stream))
+                return -1;
+            if (s.shadow && nk::build_shadow(rows, s.shadow_n, s.n - s.shadow_n, ix->dim, dimpad, s.shadow, s.xnorm2, s.dnorm2, s.stream))
                 return -1;
         } else if (nk::row_sqnorms16(s.rows, ix->dtype, s.shadow_n, s.n - s.shadow_n, ix->dim, s.xnorm2, s.stream)) {
             return -1;
@@ -250,7 +286,9 @@ static int shard_shadow_row(NkIndex *ix, NkShard &s, uint64_t local) {  // one r
     if (!s.xnorm2 || local >= s.shadow_n) return 0;
     ix->stats.kernel_launches++;
     if (ix->dtype != NK_DTYPE_F32) return nk::row_sqnorms16(s.rows, ix->dtype, local, 1, ix->dim, s.xnorm2, s.stream);
-    return nk::build_shadow(static_cast<const float *>(s.rows), local, 1, ix->dim, ix->dimpad(), s.shadow, s.xnorm2, s.dnorm2, s.stream);
+    const float *rows = static_cast<const float *>(s.rows);
+    if (s.img8 && nk::build_image_s8(rows, local, 1, ix->dim, ix->dimpad8(), s.img8, s.xscale, s.xnorm2, s.d8norm2, s.stream)) return -1;
+    return s.shadow ? nk::build_shadow(rows, local, 1, ix->dim, ix->dimpad(), s.shadow, s.xnorm2, s.dnorm2, s.stream) : 0;
 }
 
 // ---- cold-start feed (SURVEY.md §8(f)3) ---------------------------------------------------------------------------
@@ -355,19 +393,57 @@ static nk::ScanArgs shard_scan_args(const NkIndex *ix, const NkShard &s, const f
     return a;
 }
 
-// a with the shard's 16-bit image attached, if it has an up-to-date one: the BF16 shadow of an fp32 shard, or a 16-bit
-// shard's own rows
-static nk::ScanArgs with_16bit_image(const NkIndex *ix, const NkShard &s, const nk::ScanArgs &a) {
+// Has a search on the shard's int8 image overflowed its margin buffers since the last look?  Reads the counters copied
+// behind the last int8 search if they have landed (never waits); once true, the shard's kNN filter keeps to the BF16 shadow.
+static bool shard_s8_off(const NkShard &s) {
+    if (!s.s8_off && s.s8_ev && cudaEventQuery(s.s8_ev) == cudaSuccess) {
+        const int64_t seen = (int64_t)s.s8_h[0] + s.s8_h[1];
+        if (seen > s.s8_seen) s.s8_off = true;
+        s.s8_seen = seen;
+    }
+    return s.s8_off;
+}
+
+// The int8 image serves the kNN filter where it wins: a shard large enough for the scan to be bound by HBM bytes (the same
+// 64 MB as AUTO's), k <= S8_MAX_K, and no earlier overflow on it.  Its margins are ~3x the BF16 shadow's, so at larger k
+// every CTA emits several times more rows for exact re-scoring (Q = 1024, k = 100: 5.6x slower, DESIGN §3.3), and range
+// searches would list more rows; those keep to the BF16 shadow where the shard has one.
+constexpr uint32_t S8_MAX_K = 16;
+static bool use_s8(const NkIndex *ix, const NkShard &s, const nk::ScanArgs &a, bool range) {
+    if (!s.img8) return false;
+    if (!s.shadow) return true;
+    return !range && a.k <= S8_MAX_K && (uint64_t)s.n * ix->dim * 4 >= (64ull << 20) && !shard_s8_off(s);
+}
+
+// a with the shard's image attached, if it has an up-to-date one: the int8 image or the BF16 shadow of an fp32 shard
+// (use_s8), or a 16-bit shard's own rows
+static nk::ScanArgs with_16bit_image(const NkIndex *ix, const NkShard &s, const nk::ScanArgs &a, bool range = false) {
     nk::ScanArgs as = a;
     if (s.xnorm2 && s.shadow_n == s.n) {
-        if (ix->dtype == NK_DTYPE_F32) {
-            as.shadow = s.shadow; as.dnorm2 = s.dnorm2;
+        if (ix->dtype != NK_DTYPE_F32) {
+            as.shadow = s.rows; as.shadow_native = true; as.shadow_dimpad = ix->dimpad();
+        } else if (use_s8(ix, s, a, range)) {
+            as.shadow = s.img8; as.dnorm2 = s.d8norm2; as.xscale = s.xscale; as.shadow_dimpad = ix->dimpad8();
         } else {
-            as.shadow = s.rows; as.shadow_native = true;
+            as.shadow = s.shadow; as.dnorm2 = s.dnorm2; as.shadow_dimpad = ix->dimpad();
         }
-        as.shadow_dimpad = ix->dimpad(); as.xnorm2 = s.xnorm2;
+        as.xnorm2 = s.xnorm2;
     }
     return as;
+}
+
+// Behind a search on the int8 image: copy the shard's overflow counters to pinned memory (read by shard_s8_off).
+static int shard_s8_watch(NkShard &s, cudaStream_t stream) {
+    if (!s.s8_ev) {
+        if (cudaEventCreateWithFlags(&s.s8_ev, cudaEventDisableTiming) != cudaSuccess ||
+            cudaMallocHost((void **)&s.s8_h, 2 * sizeof(int)) != cudaSuccess) {
+            nk::set_error("int8 image: event / pinned counters unavailable");
+            return -1;
+        }
+    }
+    NK_CUDA_OK(cudaMemcpyAsync(s.s8_h, s.ws.flags + nk::FLAG_N_RETRY, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+    NK_CUDA_OK(cudaEventRecord(s.s8_ev, stream));
+    return 0;
 }
 
 // The path a scan of *a over shard s takes: the forced one (an error if it cannot serve the shape), or AUTO's pick.  *a gets
@@ -381,7 +457,7 @@ static int plan_path(const NkIndex *ix, const NkShard &s, bool range, nk::ScanAr
         nk::set_error("nk_search_range: the exact 3xTF32 path has no range mode (use AUTO, SIMT, TENSOR_FILTER or TENSOR_SHADOW)");
         return -1;
     }
-    const nk::ScanArgs as = with_16bit_image(ix, s, *a);
+    const nk::ScanArgs as = with_16bit_image(ix, s, *a, range);
     const bool tensor_ok = !range && nk::scan_tensor_supported(s.di, *a);
     const bool filter_ok = ix->dtype == NK_DTYPE_F32 && nk::scan_tensor_filter_supported(s.di, *a);
     const bool shadow_ok = as.shadow != nullptr && nk::shadow_pass_supported(s.di, as) && nk::scan_tensor_filter_supported(s.di, as);
@@ -433,12 +509,14 @@ class ScanTimer {
 };
 
 // NkStats::bytes_scanned of `passes` scans of a on path `use`: every pass streams the a.n rows once per block of queries
-// (8 on CUDA cores, 64 in the exact 3xTF32 scan, 128 in the filters); the 16-bit pass streams the 16-bit image, dimpad bf16
-// per fp32 row.
+// (8 on CUDA cores, 64 in the exact 3xTF32 scan, 128 in the filters); the image pass streams the image, dimpad8 bytes (int8)
+// or dimpad bf16 per fp32 row.
 static uint64_t scan_bytes(const NkIndex *ix, int use, const nk::ScanArgs &a, uint64_t passes) {
     const uint32_t width = use == NK_PATH_SIMT ? 8 : use == NK_PATH_TENSOR ? 64 : 128;
-    const uint64_t row_bytes = use == NK_PATH_TENSOR_SHADOW ? (uint64_t)(ix->dtype == NK_DTYPE_F32 ? ix->dimpad() : ix->dim) * 2
-                                                            : (uint64_t)ix->dim * ix->esz();
+    const uint64_t row_bytes = use != NK_PATH_TENSOR_SHADOW ? (uint64_t)ix->dim * ix->esz()
+                               : ix->dtype != NK_DTYPE_F32  ? (uint64_t)ix->dim * 2
+                               : a.xscale                   ? (uint64_t)ix->dimpad8()
+                                                            : (uint64_t)ix->dimpad() * 2;
     return (uint64_t)a.n * row_bytes * ((a.Q + width - 1) / width) * passes;
 }
 
@@ -507,6 +585,7 @@ static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uin
         s.last_out_keys = out_keys;
     }
     ix->stats.bytes_scanned += scan_bytes(ix, use, a, 1);
+    if (use == NK_PATH_TENSOR_SHADOW && a.xscale && shard_s8_watch(s, stream)) return -1;
     return 0;
 }
 
@@ -557,7 +636,11 @@ NkIndex *nk_index_create(const int *device_ids, int n_devices, uint32_t dim, int
     }
     NkIndex *ix = new NkIndex();
     ix->dim = dim; ix->dtype = dtype; ix->metric = metric;
-    if (const char *e = getenv("NK_SHADOW")) ix->shadow_on = atoi(e) != 0;  // read once, at creation
+    if (const char *e = getenv("NK_SHADOW")) {  // read once, at creation: unset / 1 both images, bf16 / int8 one of them, 0 none
+        if (strcmp(e, "int8") == 0) ix->image_bf16 = false;
+        else if (strcmp(e, "bf16") == 0) ix->image_s8 = false;
+        else ix->shadow_on = atoi(e) != 0;
+    }
     ix->stats.dim = dim; ix->stats.n_devices = (uint32_t)n_devices;
     ix->shards.resize(n_devices);
     for (int i = 0; i < n_devices; ++i) {
@@ -596,6 +679,8 @@ void nk_index_release(NkIndex *ix) {
         shard_drop_shadow(s);
         if (s.h_keys) cudaFreeHost(s.h_keys);
         if (s.h_res) cudaFreeHost(s.h_res);
+        if (s.s8_h) cudaFreeHost(s.s8_h);
+        if (s.s8_ev) cudaEventDestroy(s.s8_ev);
         for (int i = 0; i < 2; ++i) {
             if (s.stage[i]) cudaFreeHost(s.stage[i]);
             if (s.stage_ev[i]) cudaEventDestroy(s.stage_ev[i]);
@@ -1404,9 +1489,10 @@ static int range_shard(NkIndex *ix, NkShard &s, uint32_t Q, const NkFilter *qfil
         if (a.row_mask) a.row_mask += from / 32;
         if (a.row_tags) a.row_tags += from;
         if (a.shadow) {
-            a.shadow = static_cast<const char *>(a.shadow) + from * (a.shadow_native ? ix->dim : a.shadow_dimpad) * 2;
+            a.shadow = static_cast<const char *>(a.shadow) + from * (a.shadow_native ? ix->dim * 2 : a.xscale ? a.shadow_dimpad : a.shadow_dimpad * 2);
             a.xnorm2 += from;
             if (a.dnorm2) a.dnorm2 += from;
+            if (a.xscale) a.xscale += from;
         }
     }
     ScanTimer timer(s);
@@ -2232,7 +2318,7 @@ static int assign_nearest(NkIndex *ix, const float *centroids_host, uint32_t K, 
     for (auto &s : ix->shards) {
         if (s.n == 0) continue;
         NK_CUDA_OK(cudaSetDevice(s.device));
-        const bool tensor = s.shadow && s.shadow_n == s.n && nk::assign_tensor_supported(s.di, ix->dim, K, metric);
+        const bool tensor = (s.shadow || s.img8) && s.shadow_n == s.n && nk::assign_tensor_supported(s.di, ix->dim, K, metric);
         const uint32_t k = K < 2 ? K : 2u;
         NkIndex *cx = tensor ? nullptr : nk_index_create(&s.device, 1, ix->dim, NK_DTYPE_F32, metric);
         if (!tensor && !cx) return -1;
@@ -2265,7 +2351,11 @@ static int assign_nearest(NkIndex *ix, const float *centroids_host, uint32_t K, 
         }
         const float *rows = static_cast<const float *>(s.rows);
         if (rc == 0 && tensor) {
-            rc = nk::assign_tensor(s.di, rows, s.shadow, ix->dimpad(), s.xnorm2, s.dnorm2, (uint32_t)s.n, ix->dim, d_cen, K, metric, ties, d_asg,
+            // (the BF16 shadow where the shard has one: the int8 image's wider margins leave more near-ties to the fix-up)
+            rc = s.shadow ? nk::assign_tensor(s.di, rows, s.shadow, ix->dimpad(), nullptr, s.xnorm2, s.dnorm2, (uint32_t)s.n,
+                                              ix->dim, d_cen, K, metric, ties, d_asg, s.stream, &ix->stats.kernel_launches,
+                                              &s.ws.sub_gather, &s.ws.sub_gather_bytes)
+                          : nk::assign_tensor(s.di, rows, s.img8, ix->dimpad8(), s.xscale, s.xnorm2, s.d8norm2, (uint32_t)s.n, ix->dim, d_cen, K, metric, ties, d_asg,
                                    s.stream, &ix->stats.kernel_launches, &s.ws.sub_gather, &s.ws.sub_gather_bytes);
         }
         const uint64_t B = 8192;  // rows per fused search: amortises the ~12 fixed launches of a search over 8 scan launches

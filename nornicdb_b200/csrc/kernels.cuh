@@ -73,12 +73,14 @@ struct ScanArgs {
     // filtered (TAGS) instantiations, so unfiltered searches run unchanged code.
     const uint64_t *row_tags = nullptr;
     const NkFilter *qfilter = nullptr;
-    // optional BF16 shadow of an fp32 shard (scan_tensor_shadow.cu): rows of `shadow_dimpad` bf16 + per-row |x|^2 and
-    // |x - bf16(x)|^2; nullptr = none
+    // optional image of an fp32 shard (scan_tensor_shadow.cu): rows of `shadow_dimpad` elements + per-row |x|^2 and
+    // |x - image(x)|^2; nullptr = none.  xscale != nullptr: the int8 image (x ~ xscale[row] * int8 row, stride shadow_dimpad
+    // bytes); otherwise the BF16 shadow (stride shadow_dimpad * 2 bytes)
     const void *shadow = nullptr;
     uint32_t shadow_dimpad = 0;
     bool shadow_native = false;  // 16-bit corpus: shadow == rows (row stride dim * 2 bytes), dnorm2 == nullptr
     const float *xnorm2 = nullptr, *dnorm2 = nullptr;
+    const float *xscale = nullptr;
     // optional fused decode: the final (index, score) arrays [Q x k] are written by the last kernel of the path
     uint32_t *out_idx = nullptr;
     float *out_score = nullptr;
@@ -116,6 +118,10 @@ int scan_filter_dump(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, int
 // fp32 rows [first, first+count) -> bf16 shadow rows (stride dimpad) + |x|^2, |x - bf16(x)|^2
 int build_shadow(const float *rows, uint64_t first, uint64_t count, uint32_t dim, uint32_t dimpad, void *shadow, float *xnorm2,
                  float *dnorm2, cudaStream_t stream);
+// fp32 rows [first, first+count) -> int8 image rows (stride dimpad bytes, a multiple of 128) + per-row scale s = max|x_i| / 127
+// (NaN for a row with a non-finite element), |x|^2 and |x - s q|^2
+int build_image_s8(const float *rows, uint64_t first, uint64_t count, uint32_t dim, uint32_t dimpad, void *image, float *xscale,
+                   float *xnorm2, float *dnorm2, cudaStream_t stream);
 // k-means assignment (assign_tensor.cu).  Both paths list their near-tie rows (device buffers: count, rows [cap], 4
 // candidate ids per row, 0xfffffffe = every centroid) and decide them with assign_fixup_kernel's contract arithmetic; the
 // list stays readable after the call (nk_debug_assign_ties).  cap >= n.
@@ -125,8 +131,8 @@ struct AssignTies {
 };
 // One pass of the 16-bit scan with an argmax epilogue.
 bool assign_tensor_supported(const DeviceInfo &di, uint32_t dim, uint32_t K, int metric);
-int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, uint32_t dimpad, const float *xnorm2, const float *dnorm2,
-                  uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric, AssignTies ties, uint32_t *assign_dev,
+int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, uint32_t dimpad, const float *xscale, const float *xnorm2,
+                  const float *dnorm2, uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric, AssignTies ties, uint32_t *assign_dev,
                   cudaStream_t stream, uint64_t *launches, void **scratch, size_t *scratch_bytes);
 // From a k = min(2, K) search of the rows against the centroids (idx / sc: [n x k], euclidean scores as distances).
 int assign_from_search(const DeviceInfo &di, const float *rows, uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric,

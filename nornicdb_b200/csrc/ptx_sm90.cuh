@@ -186,13 +186,66 @@ __device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t a_desc,
         : "l"(a_desc), "l"(b_desc), "r"(accumulate));
 }
 
+// Integer forms: s8 x s8 -> exact s32 accumulators, K = 32 bytes per MMA (the same 32 B of a swizzle row as one k16 MMA of
+// a 16-bit form), both operands K-major (no transpose or scale operands).  The accumulators live in the registers of the
+// caller's float array (bit patterns, same layout as the fp32 forms); the kernel converts them in place once they are done.
+__device__ __forceinline__ void wgmma_s8_n64(float (&f)[32], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    uint32_t d[32];
+#pragma unroll
+    for (int i = 0; i < 32; ++i) d[i] = __float_as_uint(f[i]);
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %34, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n64k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+#pragma unroll
+    for (int i = 0; i < 32; ++i) f[i] = __uint_as_float(d[i]);
+}
+
+__device__ __forceinline__ void wgmma_s8_n128(float (&f)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+    uint32_t d[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) d[i] = __float_as_uint(f[i]);
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k32.s32.s8.s8 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p;\n\t}"
+        : "+r"(d[0]), "+r"(d[1]), "+r"(d[2]), "+r"(d[3]), "+r"(d[4]), "+r"(d[5]), "+r"(d[6]), "+r"(d[7]),
+          "+r"(d[8]), "+r"(d[9]), "+r"(d[10]), "+r"(d[11]), "+r"(d[12]), "+r"(d[13]), "+r"(d[14]), "+r"(d[15]),
+          "+r"(d[16]), "+r"(d[17]), "+r"(d[18]), "+r"(d[19]), "+r"(d[20]), "+r"(d[21]), "+r"(d[22]), "+r"(d[23]),
+          "+r"(d[24]), "+r"(d[25]), "+r"(d[26]), "+r"(d[27]), "+r"(d[28]), "+r"(d[29]), "+r"(d[30]), "+r"(d[31]),
+          "+r"(d[32]), "+r"(d[33]), "+r"(d[34]), "+r"(d[35]), "+r"(d[36]), "+r"(d[37]), "+r"(d[38]), "+r"(d[39]),
+          "+r"(d[40]), "+r"(d[41]), "+r"(d[42]), "+r"(d[43]), "+r"(d[44]), "+r"(d[45]), "+r"(d[46]), "+r"(d[47]),
+          "+r"(d[48]), "+r"(d[49]), "+r"(d[50]), "+r"(d[51]), "+r"(d[52]), "+r"(d[53]), "+r"(d[54]), "+r"(d[55]),
+          "+r"(d[56]), "+r"(d[57]), "+r"(d[58]), "+r"(d[59]), "+r"(d[60]), "+r"(d[61]), "+r"(d[62]), "+r"(d[63])
+        : "l"(a_desc), "l"(b_desc), "r"(accumulate));
+#pragma unroll
+    for (int i = 0; i < 64; ++i) f[i] = __uint_as_float(d[i]);
+}
+
+// Operand type of the filter scan over a row image: bf16 (BF16 shadow, bf16 corpora), fp16 (fp16 corpora) or int8 (the
+// per-row-scaled int8 image of fp32 shards; s32 accumulators).
+enum class Opnd { BF16, F16, S8 };
+
 // The wgmma form must be a compile-time choice (ptxas warning C7519 otherwise).
-template <int N, bool F16> __device__ __forceinline__ void wgmma_16bit(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc) {
-    static_assert(N == 64 || N == 128, "wgmma_16bit: N = 64 or 128");
+template <int N, Opnd OP> __device__ __forceinline__ void wgmma_op(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc) {
+    static_assert(N == 64 || N == 128, "wgmma_op: N = 64 or 128");
     if constexpr (N == 64) {
-        if constexpr (F16) wgmma_f16_n64(d, a, b, acc); else wgmma_bf16_n64(d, a, b, acc);
+        if constexpr (OP == Opnd::S8) wgmma_s8_n64(d, a, b, acc);
+        else if constexpr (OP == Opnd::F16) wgmma_f16_n64(d, a, b, acc);
+        else wgmma_bf16_n64(d, a, b, acc);
     } else {
-        if constexpr (F16) wgmma_f16_n128(d, a, b, acc); else wgmma_bf16_n128(d, a, b, acc);
+        if constexpr (OP == Opnd::S8) wgmma_s8_n128(d, a, b, acc);
+        else if constexpr (OP == Opnd::F16) wgmma_f16_n128(d, a, b, acc);
+        else wgmma_bf16_n128(d, a, b, acc);
     }
 }
 template <int N> __device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t acc);

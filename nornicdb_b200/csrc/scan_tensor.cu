@@ -162,11 +162,44 @@ __global__ void __launch_bounds__(PREP_THREADS) filter_prep_kernel(PrepParams p)
             dd += __shfl_xor_sync(0xffffffffu, dd, o);
         }
         if (lane == 0) { red[1][w] = hh; red[2][w] = dd; }
+    } else if (p.qs8) {
+        // int8 image q ~ s qq, s = max|q_i| / 127 (NaN if an element is not finite: every estimate of the query is then NaN
+        // and kept as +inf); qa / qb below measure |s qq| and |q - s qq| as the BF16 copy's residues are measured
+        float mx = 0.0f;
+        bool bad = false;
+        for (uint32_t j = tid; j < p.dim; j += PREP_THREADS) {
+            const float v = row < p.Q ? qs[j] * inv : 0.0f;
+            mx = fmaxf(mx, fabsf(v));
+            bad |= (v - v) != 0.0f;
+        }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        bad = __any_sync(0xffffffffu, bad);
+        if (lane == 0) red[1][w] = bad ? NAN : mx;
+        __syncthreads();
+        for (int i = 0; i < NW; ++i) { const float r = red[1][i]; mx = (mx != mx || r != r) ? NAN : fmaxf(mx, r); }  // NaN sticks
+        __syncthreads();  // red[1] is reused below
+        const float s = mx / 127.0f, sinv = mx > 0.0f ? 127.0f / mx : 0.0f;  // (mx NaN: s NaN, sinv 0)
+        for (uint32_t j = tid; j < p.dimpad; j += PREP_THREADS) {
+            const float v = (row < p.Q && j < p.dim) ? qs[j] * inv : 0.0f;
+            const int iq = max(-127, min(127, __float2int_rn(v * sinv)));
+            p.qs8[(size_t)row * p.dimpad + j] = (int8_t)iq;
+            const float vb = s * (float)iq, e = fmaf(-s, (float)iq, v);
+            hh = fmaf(vb, vb, hh);
+            dd = fmaf(e, e, dd);
+        }
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+            hh += __shfl_xor_sync(0xffffffffu, hh, o);
+            dd += __shfl_xor_sync(0xffffffffu, dd, o);
+        }
+        if (lane == 0) { red[1][w] = hh; red[2][w] = dd; }
+        if (tid == 0) p.qscale[row] = s;
     }
     __syncthreads();
     if (tid == 0) {
         if (p.qnorm) p.qnorm[row] = qn;
-        if (p.qbf) {
+        if (p.qbf || p.qs8) {
             hh = dd = 0.0f;
             for (int i = 0; i < NW; ++i) { hh += red[1][i]; dd += red[2][i]; }
             p.qa[row] = sqrtf(hh) * 1.0001f;
@@ -772,6 +805,7 @@ int tc_make_map(CUtensorMap *m, const void *base, uint64_t rows, uint32_t cols, 
     cuuint32_t box[2] = {box_cols, box_rows};
     cuuint32_t estr[2] = {1, 1};
     const CUtensorMapDataType dt = elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                   : elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
                                    : map_dtype == NK_DTYPE_F16 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
     CUresult r = enc(m, dt, 2,
                      const_cast<void *>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
@@ -990,8 +1024,8 @@ struct FilterPlan {
     bool stage2;        // the TF32 filter over the fp32 rows exists as the retry stage (fp32 shards with a shadow)
     bool can_exact_tc;  // exact stage = 3xTF32 kernel (else the CUDA-core scan)
     float acc_c, margin_tf32;
-    float *qhi, *qlo, *qnorm, *qa, *qb;
-    void *qbf16;
+    float *qhi, *qlo, *qnorm, *qa, *qb, *qscale;
+    void *qbf16;        // the queries in the image's element type: bf16 / fp16, or int8 (with qscale) for an int8 image
     uint32_t max_groups_shadow;
     size_t fsmem;
 };
@@ -1015,11 +1049,13 @@ static int make_filter_plan(const DeviceInfo &di, const ScanArgs &a, Workspace &
     f.stage2 = f.big && a.dtype == NK_DTYPE_F32 && tc_common_ok(di, a);
     f.can_exact_tc = scan_tensor_supported(di, a);  // euclidean / 16-bit rows have no 3xTF32 twin: overflow -> CUDA-core scan
     // 16-bit margins are ~6x wider than TF32's and clustered corpora put hundreds of rows per CTA inside them: the 16-bit
-    // kernel has 1024-slot buffers and emits up to 512 entries per (CTA, query) (the finish step re-scores in rounds)
-    if (f.big) f.k_emit = a.k <= 160 ? 512u : (uint32_t)(P_SHADOW - ROWS);
+    // kernel has 1024-slot buffers and emits up to 512 entries per (CTA, query) (the finish step re-scores in rounds).  The
+    // int8 image's margins are ~3x the BF16 shadow's: a CTA's local top 100 of 300k uniform rows already has ~550 rows inside
+    // them, so it emits up to the whole prunable buffer at every k.
+    if (f.big) f.k_emit = a.k <= 160 && !a.xscale ? 512u : (uint32_t)(P_SHADOW - ROWS);
     f.dimpad = f.big ? a.shadow_dimpad : (a.dim + 63) / 64 * 64;
     const bool need_f32q = a.dtype == NK_DTYPE_F32;  // hi / lo arrays only serve passes over fp32 rows
-    const size_t qaux_floats = (need_f32q ? (size_t)2 * f.Qpad * a.dim : 0) + (size_t)3 * f.QA;
+    const size_t qaux_floats = (need_f32q ? (size_t)2 * f.Qpad * a.dim : 0) + (size_t)4 * f.QA;
     if (ws_reserve((void **)&ws.qaux, &ws.qaux_bytes, qaux_floats * 4 + (f.big ? (size_t)f.Qpad * f.dimpad * 2 : 0))) return -1;
     if (ws_reserve((void **)&ws.cand, &ws.cand_bytes, (size_t)f.grid * QT_MAX * (f.big ? P_SHADOW : P) * 8)) return -1;
     if (ws_reserve((void **)&ws.partial, &ws.partial_bytes, (size_t)a.Q * f.grid * f.k_emit * 8)) return -1;
@@ -1029,6 +1065,7 @@ static int make_filter_plan(const DeviceInfo &di, const ScanArgs &a, Workspace &
     f.qnorm = ws.qaux + (need_f32q ? (size_t)2 * f.Qpad * a.dim : 0);
     f.qa = f.qnorm + f.QA;
     f.qb = f.qa + f.QA;
+    f.qscale = a.xscale ? f.qb + f.QA : nullptr;
     f.qbf16 = ws.qaux + qaux_floats;
     // G query groups leave each CTA 1/G of the grid for its queries, i.e. G times the rows — and G times the rows inside
     // the BF16 margin — per (CTA, query) buffer: large k keeps fewer groups so that k + margin rows stay inside k_emit
@@ -1103,7 +1140,8 @@ static int tf32_passes(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, c
 static PrepParams filter_prep_params(const ScanArgs &a, Workspace &ws, const FilterPlan &f) {
     PrepParams pp = prep_params(a, f.Qpad, f.dimpad);
     pp.acc_c = f.acc_c; pp.qhi = f.qhi;
-    pp.qbf = f.big ? static_cast<uint16_t *>(f.qbf16) : nullptr; pp.qbf_f16 = a.dtype == NK_DTYPE_F16;
+    pp.qbf = f.big && !a.xscale ? static_cast<uint16_t *>(f.qbf16) : nullptr; pp.qbf_f16 = a.dtype == NK_DTYPE_F16;
+    pp.qs8 = f.big && a.xscale ? static_cast<int8_t *>(f.qbf16) : nullptr; pp.qscale = f.qscale;
     pp.qnorm = f.qnorm; pp.qa = f.qa; pp.qb = f.qb;
     pp.state = reinterpret_cast<uint32_t *>(ws.keys2); pp.QA = f.QA; pp.flags = ws.flags; pp.sample = f.sample;
     return pp;
@@ -1169,7 +1207,7 @@ int scan_tensor_filter(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, u
     if (plan_launches(0, q_big, f.grid, f.max_groups_shadow, [&](uint32_t qt, uint32_t q0, uint32_t nq, uint32_t groups) {
             ShadowPassArgs sp{};
             sp.grid = f.grid; sp.k_emit = f.k_emit; sp.dimpad = f.dimpad; sp.Qpad = f.Qpad; sp.q0 = q0; sp.nq = nq; sp.qgroups = groups;
-            sp.qbf16 = f.qbf16; sp.qnorm = f.qnorm; sp.qa = f.qa; sp.qb = f.qb; sp.presampled = f.sample != 0;
+            sp.qbf16 = f.qbf16; sp.qnorm = f.qnorm; sp.qa = f.qa; sp.qb = f.qb; sp.qscale = f.qscale; sp.presampled = f.sample != 0;
             return launch_shadow_pass((int)qt, di, a, ws, sp, launches);
         }))
         return -1;
@@ -1211,7 +1249,7 @@ int scan_tensor_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, ui
         rc = plan_launches(0, a.Q, f.grid, 4, [&](uint32_t qt, uint32_t q0, uint32_t nq, uint32_t groups) {
             ShadowPassArgs sp{};
             sp.grid = f.grid; sp.k_emit = f.k_emit; sp.dimpad = f.dimpad; sp.Qpad = f.Qpad; sp.q0 = q0; sp.nq = nq; sp.qgroups = groups;
-            sp.qbf16 = f.qbf16; sp.qnorm = f.qnorm; sp.qa = f.qa; sp.qb = f.qb; sp.presampled = 1; sp.range = true; sp.list_cap = list_cap;
+            sp.qbf16 = f.qbf16; sp.qnorm = f.qnorm; sp.qa = f.qa; sp.qb = f.qb; sp.qscale = f.qscale; sp.presampled = 1; sp.range = true; sp.list_cap = list_cap;
             return launch_shadow_pass((int)qt, di, b, ws, sp, launches);
         });
     } else {
@@ -1248,7 +1286,7 @@ int scan_filter_dump(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, int
     if (which == NK_PATH_TENSOR_SHADOW) {
         ShadowPassArgs sp{};
         sp.grid = f.grid; sp.k_emit = f.k_emit; sp.dimpad = f.dimpad; sp.Qpad = f.Qpad; sp.q0 = 0; sp.nq = b.Q; sp.qgroups = 1;
-        sp.qbf16 = f.qbf16; sp.qnorm = f.qnorm; sp.qa = f.qa; sp.qb = f.qb; sp.presampled = 0;
+        sp.qbf16 = f.qbf16; sp.qnorm = f.qnorm; sp.qa = f.qa; sp.qb = f.qb; sp.qscale = f.qscale; sp.presampled = 0;
         sp.dump_est = est; sp.dump_bnd = bnd; sp.dump_ld = ld;
         if (launch_shadow_pass(64, di, b, ws, sp, launches)) return -1;
     } else {

@@ -27,6 +27,12 @@
 // Shared-memory traffic per [256 rows x 128 queries x 64 dims]: 112 KB (A 32 w + 32 r, B 16 w + 32 r) for twice the K
 // extent of a TF32 slab: half the bytes per product of the TF32 kernel, which is shared-memory-bandwidth bound at 128
 // query columns.  Algorithmic HBM bytes per launch: n * dimpad * 2 (shadow) + n * 8 (norms).
+//
+// Int8 image (Opnd::S8; the kNN filter picks it per search, index_api.cu use_s8): rows of dimpad8 = ceil(d / 128) * 128 int8 with one fp32 scale per row, x ~ s_x xq,
+// and int8 queries with one scale each.  The shared-memory layout is the same byte for byte (a 128-byte swizzle row holds 128
+// int8, one m64nQTk32 s8 MMA consumes the 32 B of one bf16 k16 MMA), the slab count halves, the exact s32 accumulators are
+// converted in place to float(acc) s_q and s_x joins the row's multiplier.  The bound above holds for any image xb, qb, with
+// the measured int8 residues; integer accumulation adds no error.  Bytes per launch: n * dimpad8 + n * 12.
 #include <cuda.h>
 #include <stdlib.h>
 
@@ -40,7 +46,7 @@ namespace sb {
 using namespace tc;
 constexpr int NTHREADS = 384;
 constexpr int QT_MAX = 128;
-constexpr int BKB = 64;                   // bf16 per row per slab = one 128-byte swizzle row
+constexpr int BKB = 64;                   // bf16 per row per slab = one 128-byte swizzle row (int8 images: 128 elements)
 constexpr int ASTAGES_MAX = 6;            // deepest shadow-slab ring (Cfg<QT>::ASTAGES)
 constexpr int A_BYTES = ROWS * 128;       // 32 KB
 constexpr int EPI_WARP0 = 4, EPI_WARPS = 8, EPI_NT = EPI_WARPS * 32;
@@ -72,6 +78,7 @@ struct __align__(8) Shared {
     float tau[QT_MAX];
     float qn[QT_MAX];                              // |q| (1 for cosine)
     float qa[QT_MAX], qb[QT_MAX];                  // bound(row, q) = ra(row) qa[q] + rb(row) qb[q]
+    float qs[QT_MAX];                              // int8 image: scale of the query's int8 copy
     int cnt[QT_MAX];
     uint32_t ethr[QT_MAX];                         // emission: score-word threshold per query
     int eoff[QT_MAX + 1];                          // emission: prefix of 32-entry chunk counts
@@ -126,6 +133,67 @@ int build_shadow(const float *rows, uint64_t first, uint64_t count, uint32_t dim
     return 0;
 }
 
+// fp32 rows -> int8 image rows (row stride dimpad bytes, zero padded) + per row s = max|x_i| / 127, |x|^2 and |x - s q|^2.
+// One warp per row, two passes over the row (the second from L1): the maximum, then the rounding.  A row with a non-finite
+// element gets s = NaN (and q = 0): its estimates are NaN and it is kept with bound +inf, as a NaN row of the BF16 shadow is.
+// A zero row has s = 0, q = 0 and a zero residue.
+__global__ void build_image_s8_kernel(const float *rows, uint64_t n, uint32_t dim, uint32_t dimpad, int8_t *image, float *xscale,
+                                      float *xnorm2, float *dnorm2) {
+    const uint64_t row = (uint64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (row >= n) return;
+    const float *x = rows + row * dim;
+    const bool vec = (dim & 3u) == 0 && ((reinterpret_cast<uintptr_t>(rows) & 15) == 0);
+    auto load4 = [&](uint32_t j) {
+        if (j >= dim) return make_float4(0.f, 0.f, 0.f, 0.f);
+        if (vec) return __ldg(reinterpret_cast<const float4 *>(x + j));
+        return make_float4(__ldg(x + j), j + 1 < dim ? __ldg(x + j + 1) : 0.f, j + 2 < dim ? __ldg(x + j + 2) : 0.f, j + 3 < dim ? __ldg(x + j + 3) : 0.f);
+    };
+    float mx = 0.0f, xx = 0.0f;
+    bool bad = false;
+    for (uint32_t j = lane * 4; j < dim; j += 128) {
+        const float4 v = load4(j);
+        mx = fmaxf(fmaxf(mx, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
+        bad |= (v.x - v.x) != 0.0f || (v.y - v.y) != 0.0f || (v.z - v.z) != 0.0f || (v.w - v.w) != 0.0f;
+        xx = fmaf(v.x, v.x, xx); xx = fmaf(v.y, v.y, xx); xx = fmaf(v.z, v.z, xx); xx = fmaf(v.w, v.w, xx);
+    }
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+        mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
+        xx += __shfl_xor_sync(0xffffffffu, xx, o);
+    }
+    bad = __any_sync(0xffffffffu, bad);
+    const float sc = bad ? NAN : mx / 127.0f, sinv = !bad && mx > 0.0f ? 127.0f / mx : 0.0f;
+    int8_t *o = image + row * dimpad;
+    float dd = 0.0f;
+    for (uint32_t j = lane * 4; j < dimpad; j += 128) {
+        const float4 v = load4(j);
+        const float f[4] = {v.x, v.y, v.z, v.w};
+        uint32_t packed = 0;
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+            const int iq = max(-127, min(127, __float2int_rn(f[e] * sinv)));
+            const float r = fmaf(-sc, (float)iq, f[e]);
+            dd = fmaf(r, r, dd);
+            packed |= ((uint32_t)iq & 0xffu) << (8 * e);
+        }
+        *reinterpret_cast<uint32_t *>(o + j) = packed;
+    }
+#pragma unroll
+    for (int s = 16; s; s >>= 1) dd += __shfl_xor_sync(0xffffffffu, dd, s);
+    if (lane == 0) { xscale[row] = sc; xnorm2[row] = xx; dnorm2[row] = dd; }
+}
+
+int build_image_s8(const float *rows, uint64_t first, uint64_t count, uint32_t dim, uint32_t dimpad, void *image, float *xscale,
+                   float *xnorm2, float *dnorm2, cudaStream_t stream) {
+    if (count == 0) return 0;
+    const unsigned int blocks = (unsigned int)((count + 7) / 8);
+    build_image_s8_kernel<<<blocks, 256, 0, stream>>>(rows + first * dim, count, dim, dimpad, static_cast<int8_t *>(image) + first * dimpad,
+                                                      xscale + first, xnorm2 + first, dnorm2 + first);
+    NK_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+
 // Debug timeline (NK_TC_DEBUG & 64): per-CTA globaltimer stamps, printed by launch_shadow_pass_t after a synchronize.
 //   [0] entry  [1] set-up done  [2] first accumulator ready  [3] last tile's epilogue done  [4] exit
 //   [5] ns in the prune section (epilogue warp 0)  [6] tile index of the first prune  [7] ns waiting for accumulators
@@ -149,13 +217,13 @@ struct Bf16Est {
 };
 
 // TAGS: filtered search (per-query tag filters in the keep rule, read through the read-only cache: the shared-memory budget
-// is spent on the rings); the unfiltered instantiations are TAGS = false.  F16: the operands are fp16 (an fp16 corpus
-// scanned in place) instead of bf16.  RANGE (nk_search_range): fixed per-query thresholds; full buffers are flushed to the
+// is spent on the rings); the unfiltered instantiations are TAGS = false.  OP: the operand type, bf16 (BF16 shadow, bf16
+// corpora), fp16 (an fp16 corpus scanned in place) or int8 (the int8 image of an fp32 shard).  RANGE (nk_search_range): fixed per-query thresholds; full buffers are flushed to the
 // lists, never pruned, and the end of the launch flushes what is left.  ROWTHR (with RANGE, the reverse scan of
 // nk_knn_graph_update): a pair must also reach its row's threshold p.row_thr[row], loaded with the row's norms.  RFILT (with
 // ROWTHR and TAGS, a filtered graph): the row's own filter must also admit the query's tag (keep_fragment_row); the launch's
 // query tags are staged in shared memory past Shared.
-template <int QT, bool F16, bool DUMP, bool TAGS, bool RANGE, bool ROWTHR = false, bool RFILT = false>
+template <int QT, ptx::Opnd OP, bool DUMP, bool TAGS, bool RANGE, bool ROWTHR = false, bool RFILT = false>
 __global__ void __launch_bounds__(sb::NTHREADS, 1)
 knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_q, tc::Params p) {
     using namespace sb;
@@ -174,7 +242,9 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
     const uint32_t num_tiles = (p.n + ROWS - 1) / ROWS;
     const QueryGroup<QT> qg(p);
     const uint32_t sub = qg.sub, sgrid = qg.sgrid, q0 = qg.q0, qpad_off = qg.qpad_off, nq = qg.nq;
-    const uint32_t nslab = p.nslab;  // dimpad / 64
+    const uint32_t nslab = p.nslab;  // dimpad / 64 (int8 image: dimpad / 128)
+    constexpr bool S8 = OP == ptx::Opnd::S8;
+    constexpr uint32_t KCOLS = S8 ? 128 : BKB;  // elements per row of a slab: 128 bytes either way
 
     if (warp == 0 && lane == 0) {
         ptx::prefetch_tensormap(&map_rows);
@@ -188,6 +258,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
         sh.qn[tid] = p.qnorm[qpad_off + tid];
         sh.qa[tid] = p.qa[qpad_off + tid];
         sh.qb[tid] = p.qb[qpad_off + tid];
+        if (S8) sh.qs[tid] = p.qscale[qpad_off + tid];
     }
     uint64_t *qtag = reinterpret_cast<uint64_t *>(smem_raw + (size_t)C::RING_BYTES + sizeof(Shared));  // RFILT only
     if (RFILT && tid < QT) qtag[tid] = (uint32_t)tid < nq ? p.qtags[q0 + tid] : 0ull;
@@ -217,13 +288,13 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             // ===================================== TMA producer: shadow slabs =========================
             tma_producer<C::ASTAGES>(sh.ring.aempty, sub, num_tiles, sgrid, 1, nslab, false, [&](uint32_t s, uint32_t tile, uint32_t, uint32_t j) {
                 ptx::mbar_arrive_expect_tx(&sh.ring.afull[s], A_BYTES);
-                ptx::tma_load_2d(&map_rows, &sh.ring.afull[s], a_base + (size_t)s * A_BYTES, (int32_t)(j * BKB), (int32_t)(tile * ROWS), qg.a_policy);
+                ptx::tma_load_2d(&map_rows, &sh.ring.afull[s], a_base + (size_t)s * A_BYTES, (int32_t)(j * KCOLS), (int32_t)(tile * ROWS), qg.a_policy);
             });
         } else if (warp == 3) {
             // ===================================== TMA producer: query slabs (L2-resident) ===========
             tma_producer<C::BSTAGES>(sh.ring.bempty, sub, num_tiles, sgrid, 1, nslab, false, [&](uint32_t s, uint32_t, uint32_t, uint32_t j) {
                 ptx::mbar_arrive_expect_tx(&sh.ring.bfull[s], C::B_BYTES);
-                ptx::tma_load_2d(&map_q, &sh.ring.bfull[s], b_base + (size_t)s * C::B_BYTES, (int32_t)(j * BKB), (int32_t)qpad_off, ptx::CACHE_EVICT_LAST);
+                ptx::tma_load_2d(&map_q, &sh.ring.bfull[s], b_base + (size_t)s * C::B_BYTES, (int32_t)(j * KCOLS), (int32_t)qpad_off, ptx::CACHE_EVICT_LAST);
             });
         }
         ptx::named_bar_sync(REG_BAR, NTHREADS);  // every consumer warp is back at EMIT_REGS: the pool holds what this asks for
@@ -252,9 +323,10 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
         uint32_t g = 0, it = 0;
         for (uint32_t tile = sub; tile < num_tiles; tile += sgrid, ++it) {
             if (eprof) t_a = globaltimer_ns();
-            // The epilogue's global inputs, loaded before the MMAs: |x|^2, |dx|^2 and the mask word of this thread's 4
-            // rows, and the shared threshold of query etid (it only grows: an earlier value is still a lower bound).
-            float x2[4], d2[4], rthr[4];
+            // The epilogue's global inputs, loaded before the MMAs: |x|^2, |dx|^2 (int8 image: and the row's scale) and the
+            // mask word of this thread's 4 rows, and the shared threshold of query etid (it only grows: an earlier value is
+            // still a lower bound).
+            float x2[4], d2[4], rthr[4], xs[4];
             uint32_t mword[4];
 #pragma unroll
             for (uint32_t ri = 0; ri < 4; ++ri) {
@@ -264,6 +336,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                 d2[ri] = in && p.dnorm2 ? __ldg(p.dnorm2 + row) : 0.0f;  // 16-bit corpus: no residue
                 mword[ri] = in && p.mask ? __ldg(p.mask + (row >> 5)) : ~0u;
                 rthr[ri] = ROWTHR && in ? __ldg(p.row_thr + row) : -INFINITY;
+                xs[ri] = S8 && in ? __ldg(p.xscale + row) : 1.0f;
             }
             const uint32_t etid = tid - EPI_WARP0 * 32;  // consumer thread: one query each (QT <= EPI_NT)
             const uint32_t gt_pre = !RANGE && etid < nq ? __ldcg(p.gtau + q0 + etid) : 0u;
@@ -275,12 +348,12 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                 const uint64_t bdesc = ptx::make_smem_desc_sw128(ptx::smem_u32(b_base + (size_t)sbq * C::B_BYTES));
                 const uint32_t abase = ptx::smem_u32(a_base + (size_t)sa * A_BYTES + (size_t)m * (A_BYTES / 2));
                 ptx::wgmma_fence();
-                // K advance per MMA = 16 bf16 = 32 B = 2 descriptor units
+                // K advance per MMA = 16 bf16 (32 int8) = 32 B = 2 descriptor units
 #pragma unroll
                 for (uint32_t h = 0; h < 2; ++h) {
                     const uint64_t adesc = ptx::make_smem_desc_sw128(abase + h * (A_BYTES / 4));
 #pragma unroll
-                    for (uint32_t kk = 0; kk < 4; ++kk) ptx::wgmma_16bit<QT, F16>(acc[h], adesc + kk * 2, bdesc + kk * 2, (j | kk) != 0);
+                    for (uint32_t kk = 0; kk < 4; ++kk) ptx::wgmma_op<QT, OP>(acc[h], adesc + kk * 2, bdesc + kk * 2, (j | kk) != 0);
                 }
                 ptx::wgmma_commit();
                 if (j > 0) {  // the previous slab's MMAs are done while this slab's run: its stages go back to the producers
@@ -294,6 +367,15 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             ptx::wgmma_wait_all();
             ptx::fence_acc(acc[0]);
             ptx::fence_acc(acc[1]);
+            if constexpr (S8) {
+                // exact int32 dot products of the int8 rows -> fp32 in the same registers, times the query's scale (the
+                // row's scale is part of the estimate's multiplier): acc = xq.qq s_q, the estimate (s_x xq).(s_q qq)
+#pragma unroll
+                for (int h = 0; h < 2; ++h)
+#pragma unroll
+                    for (int i = 0; i < QT / 2; ++i)
+                        acc[h][i] = __int2float_rn(__float_as_int(acc[h][i])) * sh.qs[cbase + 8 * (i >> 2) + (i & 1)];
+            }
             __syncwarp();
             if (lane == 0) { ptx::mbar_arrive(&sh.ring.aempty[prev_sa]); ptx::mbar_arrive(&sh.ring.bempty[prev_sb]); }
             if (eprof) {
@@ -325,6 +407,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                 } else if (euclid) {
                     est.mul = 2.0f; est.ra = 2.0f * dxn; est.rb = 2.0f * xn;
                 }
+                if (S8) est.mul *= xs[ri];  // (a NaN scale: a non-finite row, every estimate NaN -> kept)
                 if ((lane & 3) == 0 && alive && est.ra < INFINITY && est.rb < INFINITY) {  // NaN / Inf rows are kept anyway (score NaN -> +inf)
                     atomicMax(&sh.max_ra, __float_as_uint(est.ra));
                     if (!cosine) { atomicMax(&sh.max_rb, __float_as_uint(est.rb)); atomicMax(&sh.maxxx, __float_as_uint(est.x2)); }
@@ -516,13 +599,14 @@ bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a) {
     return a.dim % 8 == 0;  // 16-bit rows: 16-byte TMA row stride and 128-bit exact re-scoring loads
 }
 
-template <int QT, bool F16, bool DUMP, bool TAGS, bool RANGE = false, bool ROWTHR = false, bool RFILT = false>
+template <int QT, ptx::Opnd OP, bool DUMP, bool TAGS, bool RANGE = false, bool ROWTHR = false, bool RFILT = false>
 static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
     using namespace sb;
     const bool native = a.shadow_native;  // 16-bit corpus scanned in place: row stride dim * 2, columns past dim read as zero (TMA OOB fill)
-    const CUtensorMap *map_rows = tc_cached_map(ws, 4, a.shadow, a.n, native ? a.dim : sp.dimpad, 2, BKB, ROWS,
-                                                (uint64_t)(native ? a.dim : sp.dimpad) * 2, a.dtype);
-    const CUtensorMap *map_q = tc_cached_map(ws, QT == 64 ? 5 : 6, sp.qbf16, sp.Qpad, sp.dimpad, 2, BKB, QT, (uint64_t)sp.dimpad * 2,
+    const uint32_t esz = OP == ptx::Opnd::S8 ? 1 : 2, kcols = 128 / esz;  // int8 image: 1-byte elements, 128 per swizzle row
+    const CUtensorMap *map_rows = tc_cached_map(ws, 4, a.shadow, a.n, native ? a.dim : sp.dimpad, esz, kcols, ROWS,
+                                                (uint64_t)(native ? a.dim : sp.dimpad) * esz, a.dtype);
+    const CUtensorMap *map_q = tc_cached_map(ws, QT == 64 ? 5 : 6, sp.qbf16, sp.Qpad, sp.dimpad, esz, kcols, QT, (uint64_t)sp.dimpad * esz,
                                              a.dtype);  // rows past Qpad: zero
     if (!map_rows || !map_q) return -1;
     const size_t smem = (size_t)Cfg<QT>::RING_BYTES + sizeof(Shared) + (RFILT ? QT * sizeof(uint64_t) : 0) + 1024;
@@ -530,11 +614,12 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
         set_error("shadow tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;
     }
-    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, F16, DUMP, TAGS, RANGE, ROWTHR, RFILT>), di.device_id, smem))
+    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, OP, DUMP, TAGS, RANGE, ROWTHR, RFILT>), di.device_id, smem))
         return -1;
     tc::Params p = pass_params(a, ws, sp);
-    p.nslab = sp.dimpad / BKB; p.qa = sp.qa; p.qb = sp.qb; p.xnorm2 = a.xnorm2; p.dnorm2 = a.dnorm2;
-    knn_scan_shadow_kernel<QT, F16, DUMP, TAGS, RANGE, ROWTHR, RFILT><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
+    p.nslab = sp.dimpad / kcols; p.qa = sp.qa; p.qb = sp.qb; p.xnorm2 = a.xnorm2; p.dnorm2 = a.dnorm2;
+    p.xscale = a.xscale; p.qscale = sp.qscale;
+    knn_scan_shadow_kernel<QT, OP, DUMP, TAGS, RANGE, ROWTHR, RFILT><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
     NK_CUDA_OK(cudaGetLastError());
     if (launches) ++*launches;
     if (a.main_launches) ++*a.main_launches;
@@ -542,38 +627,41 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
     return 0;
 }
 
-template <bool F16>
+template <ptx::Opnd OP>
 static int launch_shadow_pass_op(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
-    if (sp.dump_est) return launch_shadow_pass_t<64, F16, true, false>(di, a, ws, sp, launches);
+    if (sp.dump_est) return launch_shadow_pass_t<64, OP, true, false>(di, a, ws, sp, launches);
     if (sp.range && a.row_thr && a.row_filter) {  // the reverse scan of a filtered graph: each row's own filter
         if (!a.qfilter || !a.qtags) { set_error("internal: the row-filtered reverse scan needs per-query filters and tags"); return -1; }
-        return qt == 128 ? launch_shadow_pass_t<128, F16, false, true, true, true, true>(di, a, ws, sp, launches)
-                         : launch_shadow_pass_t<64, F16, false, true, true, true, true>(di, a, ws, sp, launches);
+        return qt == 128 ? launch_shadow_pass_t<128, OP, false, true, true, true, true>(di, a, ws, sp, launches)
+                         : launch_shadow_pass_t<64, OP, false, true, true, true, true>(di, a, ws, sp, launches);
     }
     if (sp.range && a.row_thr) {  // the reverse scan of nk_knn_graph_update
         if (a.qfilter)
-            return qt == 128 ? launch_shadow_pass_t<128, F16, false, true, true, true>(di, a, ws, sp, launches)
-                             : launch_shadow_pass_t<64, F16, false, true, true, true>(di, a, ws, sp, launches);
-        return qt == 128 ? launch_shadow_pass_t<128, F16, false, false, true, true>(di, a, ws, sp, launches)
-                         : launch_shadow_pass_t<64, F16, false, false, true, true>(di, a, ws, sp, launches);
+            return qt == 128 ? launch_shadow_pass_t<128, OP, false, true, true, true>(di, a, ws, sp, launches)
+                             : launch_shadow_pass_t<64, OP, false, true, true, true>(di, a, ws, sp, launches);
+        return qt == 128 ? launch_shadow_pass_t<128, OP, false, false, true, true>(di, a, ws, sp, launches)
+                         : launch_shadow_pass_t<64, OP, false, false, true, true>(di, a, ws, sp, launches);
     }
     if (sp.range) {
         if (a.qfilter)
-            return qt == 128 ? launch_shadow_pass_t<128, F16, false, true, true>(di, a, ws, sp, launches)
-                             : launch_shadow_pass_t<64, F16, false, true, true>(di, a, ws, sp, launches);
-        return qt == 128 ? launch_shadow_pass_t<128, F16, false, false, true>(di, a, ws, sp, launches)
-                         : launch_shadow_pass_t<64, F16, false, false, true>(di, a, ws, sp, launches);
+            return qt == 128 ? launch_shadow_pass_t<128, OP, false, true, true>(di, a, ws, sp, launches)
+                             : launch_shadow_pass_t<64, OP, false, true, true>(di, a, ws, sp, launches);
+        return qt == 128 ? launch_shadow_pass_t<128, OP, false, false, true>(di, a, ws, sp, launches)
+                         : launch_shadow_pass_t<64, OP, false, false, true>(di, a, ws, sp, launches);
     }
     if (a.qfilter)
-        return qt == 128 ? launch_shadow_pass_t<128, F16, false, true>(di, a, ws, sp, launches)
-                         : launch_shadow_pass_t<64, F16, false, true>(di, a, ws, sp, launches);
-    return qt == 128 ? launch_shadow_pass_t<128, F16, false, false>(di, a, ws, sp, launches)
-                     : launch_shadow_pass_t<64, F16, false, false>(di, a, ws, sp, launches);
+        return qt == 128 ? launch_shadow_pass_t<128, OP, false, true>(di, a, ws, sp, launches)
+                         : launch_shadow_pass_t<64, OP, false, true>(di, a, ws, sp, launches);
+    return qt == 128 ? launch_shadow_pass_t<128, OP, false, false>(di, a, ws, sp, launches)
+                     : launch_shadow_pass_t<64, OP, false, false>(di, a, ws, sp, launches);
 }
 
-// fp16 corpora run the fp16 wgmma form; fp32 shards (BF16 shadow) and bf16 corpora the bf16 one
+// fp32 shards with the int8 image run the s8 wgmma form, fp16 corpora the fp16 one, fp32 shards with the BF16 shadow and
+// bf16 corpora the bf16 one
 int launch_shadow_pass(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
-    return a.dtype == NK_DTYPE_F16 ? launch_shadow_pass_op<true>(qt, di, a, ws, sp, launches) : launch_shadow_pass_op<false>(qt, di, a, ws, sp, launches);
+    if (a.xscale) return launch_shadow_pass_op<ptx::Opnd::S8>(qt, di, a, ws, sp, launches);
+    return a.dtype == NK_DTYPE_F16 ? launch_shadow_pass_op<ptx::Opnd::F16>(qt, di, a, ws, sp, launches)
+                                   : launch_shadow_pass_op<ptx::Opnd::BF16>(qt, di, a, ws, sp, launches);
 }
 
 }  // namespace nk

@@ -52,7 +52,8 @@ struct Params {
     float margin_c;           // filter mode: c in |s_hat - s| <= c |x| |q|
     const float *qnorm;       // filter mode: |q| per query (1 for cosine), padded
     const float *qa, *qb;     // shadow kernel: per-query bound factors |bf16(q)| and |q - bf16(q)| + acc_c |q|
-    const float *xnorm2, *dnorm2;  // shadow kernel: per-row |x|^2 and |x - bf16(x)|^2
+    const float *xnorm2, *dnorm2;  // shadow kernel: per-row |x|^2 and |x - image(x)|^2
+    const float *xscale, *qscale;  // shadow kernel over an int8 image: per-row and per-query scales (image = scale * int8)
     uint64_t *cand;           // [grid][QT][P]
     uint32_t qpad_off;        // row of this launch's first query inside the padded query arrays
     uint64_t *partial;        // exact: [Q][grid][k_emit] fixed slots; filter: [Q][grid*k_emit] shared append lists
@@ -455,8 +456,8 @@ __device__ __forceinline__ float bf16_margin2(int metric, float max_ra, float ma
 }
 #endif
 
-// 2-D row-major [rows x cols] tensor of 4-byte (fp32) or 2-byte (bf16) elements, box = [box_rows x box_cols] with
-// box_cols * elem_bytes == 128 (one swizzle row), 128-byte swizzle, OOB -> 0.
+// 2-D row-major [rows x cols] tensor of 4-byte (fp32), 2-byte (bf16) or 1-byte (int8) elements, box = [box_rows x box_cols]
+// with box_cols * elem_bytes == 128 (one swizzle row), 128-byte swizzle, OOB -> 0.
 // map_dtype (2-byte elements only): NK_DTYPE_F16 -> fp16 tensor, anything else -> bf16.
 int tc_make_map(CUtensorMap *m, const void *base, uint64_t rows, uint32_t cols, uint32_t elem_bytes, uint32_t box_cols,
                 uint32_t box_rows, uint64_t row_stride_bytes, int map_dtype = 0);
@@ -471,11 +472,12 @@ int tc_env_int(const char *name, int dflt);  // getenv once per name (read at fi
 // The Params fields every scan launch fills the same way (scan_tensor.cu)
 tc::Params pass_params(const ScanArgs &a, Workspace &ws, const tc::PassArgs &t);
 
-// BF16 shadow filter pass (scan_tensor_shadow.cu): queries [q0, q0+nq), nq <= qgroups * qt, qt = 64 or 128.
+// Filter pass over a row image (scan_tensor_shadow.cu): queries [q0, q0+nq), nq <= qgroups * qt, qt = 64 or 128.  qbf16:
+// the queries in the image's element type (int8 images: int8, with the per-query scales qscale).
 struct ShadowPassArgs : tc::PassArgs {
     uint32_t dimpad;
     const void *qbf16;
-    const float *qa, *qb;
+    const float *qa, *qb, *qscale;
 };
 int launch_shadow_pass(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches);
 
@@ -488,6 +490,8 @@ struct PrepParams {
     float *qhi, *qlo;      // [Qpad x dim] (nullable)
     uint16_t *qbf;         // [Qpad x dimpad] (nullable); fp16 bits when qbf_f16
     int qbf_f16;
+    int8_t *qs8;           // [Qpad x dimpad] int8 image q = qscale * qs8 (nullable; exclusive with qbf)
+    float *qscale;         // [Qpad] with qs8
     float *qnorm, *qa, *qb;
     uint32_t *state;       // gtau[QA] then gcount[QA] (nullable)
     uint32_t Qpad, QA;
