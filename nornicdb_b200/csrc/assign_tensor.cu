@@ -303,18 +303,18 @@ bool assign_tensor_supported(const DeviceInfo &di, uint32_t dim, uint32_t K, int
     return di.cc >= 90 && dim % 4 == 0 && dim >= 32 && dim <= 32768 && K >= 1 && (metric == NK_METRIC_COSINE || metric == NK_METRIC_EUCLIDEAN);
 }
 
-// rows / shadow / norms: one shard (device pointers); centroids_dev: [K x dim] fp32 on the same device; assign_dev: [n].
-int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, uint32_t dimpad, const float *xscale, const float *xnorm2,
-                  const float *dnorm2, uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric, AssignTies ties, uint32_t *assign_dev,
-                  cudaStream_t stream, uint64_t *launches, void **scratch, size_t *scratch_bytes) {
+// rows / img: one fp32 shard and its BF16 shadow or int8 image (device pointers); centroids_dev: [K x dim] fp32 on the same
+// device; assign_dev: [n].
+int assign_tensor(const DeviceInfo &di, const float *rows, const RowImage &img, uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K,
+                  int metric, AssignTies ties, uint32_t *assign_dev, cudaStream_t stream, uint64_t *launches, void **scratch, size_t *scratch_bytes) {
     using namespace asg;
     if (n == 0) return 0;
     if (ties.cap < n) { set_error("assign_tensor: near-tie list shorter than the shard"); return -1; }
     const uint32_t nqb = (K + QT - 1) / QT, Kpad = nqb * QT;
     const float acc_c = (float)dim * 2.384185791015625e-7f + 4e-6f;
     // scratch: bf16 (int8 image: int8) centroids [Kpad x dimpad], qn / qa / qb (/ scales) [Kpad]
-    const bool s8 = xscale != nullptr;
-    const uint32_t esz = s8 ? 1 : 2;
+    const bool s8 = img.kind == RowImage::S8;
+    const uint32_t esz = img.esz(), dimpad = img.dimpad;
     const size_t off_q = 0, off_f = ((size_t)Kpad * dimpad * esz + 255) & ~(size_t)255;
     const size_t total = off_f + (size_t)4 * Kpad * 4;
     if (ws_reserve(scratch, scratch_bytes, total)) return -1;  // grow-only, reused across calls
@@ -333,7 +333,7 @@ int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, u
         if (launch_prep(di, pp, stream, launches)) { rc = -1; break; }
         assign_mark_nonfinite_kernel<<<(K + 7) / 8, 256, 0, stream>>>(centroids_dev, K, dim, qb);
         CUtensorMap map_rows, map_q;
-        if (tc_make_map(&map_rows, shadow, n, dimpad, esz, 128 / esz, ROWS, (uint64_t)dimpad * esz)) { rc = -1; break; }
+        if (tc_make_map(&map_rows, img.data, n, img.stride, esz, 128 / esz, ROWS, img.row_bytes())) { rc = -1; break; }
         if (tc_make_map(&map_q, buf + off_q, Kpad, dimpad, esz, 128 / esz, QT, (uint64_t)dimpad * esz)) { rc = -1; break; }
         const size_t smem = (size_t)RING_BYTES + sizeof(Shared) + 1024;
         const void *kern = s8 ? reinterpret_cast<const void *>(assign_scan_kernel<ptx::Opnd::S8>)
@@ -341,7 +341,7 @@ int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, u
         if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) { rc = -1; break; }
         asg::Params p;
         p.n = n; p.nslab = dimpad * esz / 128; p.K = K; p.nqb = nqb; p.metric = metric;
-        p.qn = qn; p.qa = qa; p.qb = qb; p.xnorm2 = xnorm2; p.dnorm2 = dnorm2; p.xscale = xscale; p.qscale = qsc;
+        p.qn = qn; p.qa = qa; p.qb = qb; p.xnorm2 = img.xnorm2; p.dnorm2 = img.dnorm2; p.xscale = img.xscale; p.qscale = qsc;
         p.assign = assign_dev; p.amb_count = amb_count; p.amb_rows = amb_rows; p.amb_cand = amb_cand; p.amb_cap = n;
         const uint32_t num_tiles = (n + ROWS - 1) / ROWS;
         const uint32_t grid = num_tiles < (uint32_t)di.num_sms ? num_tiles : (uint32_t)di.num_sms;

@@ -18,6 +18,36 @@
 #include "kernels.cuh"
 #include "scan_tensor_shared.cuh"
 
+// The images of a shard that the filter scans instead of its rows (nk::RowImage, shard_image): the BF16 shadow (+ |x -
+// bf16(x)|^2 per row) and the int8 image (+ per-row scale s and |x - s xq|^2) of an owned fp32 shard, either or both; a
+// 16-bit shard (fp16 / bf16) is scanned in place and only carries |x|^2, which all images share.  Rows [0, n) are
+// converted; capacity in rows.
+struct ShardImages {
+    void *bf16 = nullptr, *s8 = nullptr;
+    float *xnorm2 = nullptr, *bf16_dnorm2 = nullptr, *s8_dnorm2 = nullptr, *s8_scale = nullptr;
+    uint64_t cap = 0, n = 0;
+    bool attached = false;  // caller-owned rows: images built on request (nk_index_refresh_shadow)
+    // The int8 image is dropped from the kNN filter of this shard once a search on it overflowed its margin buffers (a
+    // near-tie-heavy corpus: its ~3x wider margins send such searches to the slower retry stages).  The overflow counters
+    // are copied to pinned memory behind every int8 search and read, without waiting, when the next search is planned.
+    mutable bool s8_off = false;
+    mutable cudaEvent_t s8_ev = nullptr;
+    mutable int *s8_h = nullptr;      // pinned: FLAG_N_RETRY, FLAG_N_EXACT after the last int8 search
+    mutable int64_t s8_seen = 0;      // their sum when last read
+    nk::RowImage bf16_image(uint32_t dim) const { return nk::RowImage(nk::RowImage::BF16, bf16, dim, xnorm2, bf16_dnorm2); }
+    nk::RowImage s8_image(uint32_t dim) const { return nk::RowImage(nk::RowImage::S8, s8, dim, xnorm2, s8_dnorm2, s8_scale); }
+    bool current(uint64_t rows) const { return xnorm2 && n == rows; }  // are all `rows` rows converted?
+    // Free the int8 image alone (s8_only) or every buffer.  The overflow watch stays: a shard that left the int8 image stays off it.
+    void release(bool s8_only = false) {
+        cudaFree(s8); cudaFree(s8_scale); cudaFree(s8_dnorm2);
+        s8 = nullptr; s8_scale = s8_dnorm2 = nullptr;
+        if (s8_only) return;
+        cudaFree(bf16); cudaFree(bf16_dnorm2); cudaFree(xnorm2);
+        bf16 = nullptr; bf16_dnorm2 = xnorm2 = nullptr;
+        cap = n = 0;
+    }
+};
+
 struct NkShard {
     int device = 0;
     nk::DeviceInfo di;
@@ -26,21 +56,7 @@ struct NkShard {
     void *rows = nullptr;
     bool owns = true;
     uint64_t n = 0, cap = 0, base = 0;
-    // Images of an owned fp32 shard that the filter scans (scan_tensor_shadow.cu): the BF16 shadow (+ |x - bf16(x)|^2 per
-    // row) and the int8 image img8 (+ per-row scale xscale and |x - s_x xq|^2), either or both; |x|^2 is shared.  Rows
-    // [0, shadow_n) are converted; capacity in rows.
-    // 16-bit shards (fp16 / bf16) are scanned in place by the same kernel: they only carry xnorm2 (shadow stays null).
-    void *shadow = nullptr, *img8 = nullptr;
-    float *xnorm2 = nullptr, *dnorm2 = nullptr, *xscale = nullptr, *d8norm2 = nullptr;
-    // The int8 image is dropped from the kNN filter of this shard once a search on it overflowed its margin buffers (a
-    // near-tie-heavy corpus: its ~3x wider margins send such searches to the slower retry stages).  The overflow counters
-    // are copied to pinned memory behind every int8 search and read, without waiting, when the next search is planned.
-    mutable bool s8_off = false;
-    mutable cudaEvent_t s8_ev = nullptr;
-    mutable int *s8_h = nullptr;      // pinned: FLAG_N_RETRY, FLAG_N_EXACT after the last int8 search
-    mutable int64_t s8_seen = 0;      // their sum when last read
-    uint64_t shadow_cap = 0, shadow_n = 0;
-    bool shadow_attached = false;  // caller-owned rows: shadow built on request (nk_index_refresh_shadow)
+    ShardImages img;
     // last filter search (host-synchronous API): what the deferred retry tail needs
     nk::ScanArgs last_args;
     uint64_t *last_out_keys = nullptr;
@@ -74,11 +90,11 @@ struct NkIndex {
     int dtype = NK_DTYPE_F32;
     int metric = NK_METRIC_COSINE;
     int path = NK_PATH_AUTO;
-    // Images of fp32 shards, NK_SHADOW at creation: unset / 1 both the BF16 shadow (+50% HBM) and the int8 image (+25%;
-    // the int8 image alone is dropped when its memory cannot be had), bf16 the BF16 shadow only, int8 the int8 image only,
-    // 0 none
-    bool shadow_on = true;
-    bool image_bf16 = true, image_s8 = true;
+    // The image kinds shards keep (bit 1 << nk::RowImage::Kind), NK_SHADOW at creation: unset / 1 both the BF16 shadow (+50%
+    // HBM) and the int8 image (+25%; the int8 image alone is dropped when its memory cannot be had) of fp32 shards, bf16 the
+    // BF16 shadow only, int8 the int8 image only; 16-bit shards are scanned in place unless NK_SHADOW is 0, which keeps none
+    unsigned images = 1u << nk::RowImage::BF16 | 1u << nk::RowImage::S8 | 1u << nk::RowImage::NATIVE;
+    bool keeps(nk::RowImage::Kind k) const { return images >> k & 1u; }
     bool timing_on = false;
     int last_path = NK_PATH_SIMT;
     uint64_t row_base = 0;
@@ -97,10 +113,6 @@ struct NkIndex {
         if (metric == NK_METRIC_EUCLIDEAN) return (min_score >= 0.0f && min_score < INFINITY) ? -(min_score * min_score) : -INFINITY;
         return min_score > -INFINITY ? min_score : -INFINITY;
     }
-    uint32_t dimpad() const { return (dim + 63) / 64 * 64; }
-    uint32_t dimpad8() const { return (dim + 127) / 128 * 128; }  // row stride (bytes) of the int8 image
-    bool s8() const { return image_s8 && dtype == NK_DTYPE_F32; }     // fp32 shards carry the int8 image
-    bool bf16() const { return image_bf16 || dtype != NK_DTYPE_F32; }  // ... the BF16 shadow (16-bit shards: their |x|^2)
     uint64_t rows() const {
         uint64_t t = 0;
         for (auto &s : shards) t += s.n;
@@ -216,79 +228,57 @@ static int shard_tags_on(NkShard &s) {
     return 0;
 }
 
-static void shard_drop_shadow(NkShard &s) {
-    if (s.shadow) cudaFree(s.shadow);
-    if (s.xnorm2) cudaFree(s.xnorm2);
-    if (s.dnorm2) cudaFree(s.dnorm2);
-    if (s.img8) cudaFree(s.img8);
-    if (s.xscale) cudaFree(s.xscale);
-    if (s.d8norm2) cudaFree(s.d8norm2);
-    s.shadow = s.img8 = nullptr; s.xnorm2 = s.dnorm2 = s.xscale = s.d8norm2 = nullptr;
-    s.shadow_cap = s.shadow_n = 0;
+// Convert rows [first, first+count) into every image the shard has (one launch counted): the int8 image and / or the BF16
+// shadow with their norms (fp32 shards), or the |x|^2 array (16-bit shards).
+static int shard_image_build(NkIndex *ix, NkShard &s, uint64_t first, uint64_t count) {
+    const ShardImages &m = s.img;
+    ix->stats.kernel_launches++;
+    if (ix->dtype != NK_DTYPE_F32) return nk::row_sqnorms16(s.rows, ix->dtype, first, count, ix->dim, m.xnorm2, s.stream);
+    const float *rows = static_cast<const float *>(s.rows);
+    if (m.s8 && nk::build_image_s8(rows, first, count, ix->dim, m.s8_image(ix->dim).dimpad, m.s8, m.s8_scale, m.xnorm2, m.s8_dnorm2, s.stream))
+        return -1;
+    return m.bf16 ? nk::build_shadow(rows, first, count, ix->dim, m.bf16_image(ix->dim).dimpad, m.bf16, m.xnorm2, m.bf16_dnorm2, s.stream) : 0;
 }
 
-// Bring the image of a shard up to date with rows [0, s.n) (converting only what is missing): the int8 image or the BF16
-// shadow + norms of an fp32 shard, or just the |x|^2 array of an fp16 / bf16 shard (scanned in place).  It is an optimisation: if its memory
-// cannot be had the shard simply goes without (TF32 filter / CUDA-core scan over the rows).
+// Bring the images of a shard up to date with rows [0, s.n) (converting only what is missing).  They are an optimisation: if
+// their memory cannot be had the shard simply goes without (TF32 filter / CUDA-core scan over the rows).
 static int shard_sync_shadow(NkIndex *ix, NkShard &s) {
+    ShardImages &m = s.img;
     const bool f32 = ix->dtype == NK_DTYPE_F32;
-    const bool wanted = ix->shadow_on && (s.owns || s.shadow_attached) && ix->dim >= 32 && s.n > 0 && (f32 ? ix->dim % 4 == 0 : ix->dim % 8 == 0);
+    const bool bf = f32 && ix->keeps(nk::RowImage::BF16), s8 = f32 && ix->keeps(nk::RowImage::S8);
+    const bool wanted = (f32 ? bf || s8 : ix->keeps(nk::RowImage::NATIVE)) && (s.owns || m.attached) && ix->dim >= 32 && s.n > 0 &&
+                        (f32 ? ix->dim % 4 == 0 : ix->dim % 8 == 0);
     if (!wanted) {
-        s.shadow_n = 0;
+        m.n = 0;
         return 0;
     }
-    const uint32_t dimpad = ix->dimpad(), dimpad8 = ix->dimpad8();
-    const bool bf = f32 && ix->bf16(), s8 = ix->s8();
-    if (s.shadow_cap < s.n) {
+    if (m.cap < s.n) {
         if (shard_drain(s)) return -1;
-        shard_drop_shadow(s);
+        m.release();
         const uint64_t cap = s.cap > s.n ? s.cap : s.n;
-        cudaError_t e = cudaMalloc((void **)&s.xnorm2, cap * 4);
-        if (e == cudaSuccess && bf) e = cudaMalloc(&s.shadow, cap * dimpad * 2);
-        if (e == cudaSuccess && bf) e = cudaMalloc((void **)&s.dnorm2, cap * 4);
+        cudaError_t e = cudaMalloc((void **)&m.xnorm2, cap * 4);
+        if (e == cudaSuccess && bf) e = cudaMalloc(&m.bf16, cap * m.bf16_image(ix->dim).row_bytes());
+        if (e == cudaSuccess && bf) e = cudaMalloc((void **)&m.bf16_dnorm2, cap * 4);
         if (e == cudaSuccess && s8) {
-            e = cudaMalloc(&s.img8, cap * dimpad8);
-            if (e == cudaSuccess) e = cudaMalloc((void **)&s.xscale, cap * 4);
-            if (e == cudaSuccess) e = cudaMalloc((void **)&s.d8norm2, cap * 4);
+            e = cudaMalloc(&m.s8, cap * m.s8_image(ix->dim).row_bytes());
+            if (e == cudaSuccess) e = cudaMalloc((void **)&m.s8_scale, cap * 4);
+            if (e == cudaSuccess) e = cudaMalloc((void **)&m.s8_dnorm2, cap * 4);
             if (e != cudaSuccess && bf) {  // the shard keeps its BF16 shadow and goes without the int8 image
                 cudaGetLastError();
-                if (s.img8) cudaFree(s.img8);
-                if (s.xscale) cudaFree(s.xscale);
-                if (s.d8norm2) cudaFree(s.d8norm2);
-                s.img8 = nullptr; s.xscale = s.d8norm2 = nullptr;
+                m.release(true);
                 e = cudaSuccess;
             }
         }
         if (e != cudaSuccess) {
             cudaGetLastError();
-            shard_drop_shadow(s);
+            m.release();
             return 0;
         }
-        s.shadow_cap = cap;
+        m.cap = cap;
     }
-    if (s.shadow_n < s.n) {
-        const float *rows = static_cast<const float *>(s.rows);
-        if (f32) {
-            if (s.img8 && nk::build_image_s8(rows, s.shadow_n, s.n - s.shadow_n, ix->dim, dimpad8, s.img8, s.xscale, s.xnorm2, s.d8norm2,
-                                             s.stream))
-                return -1;
-            if (s.shadow && nk::build_shadow(rows, s.shadow_n, s.n - s.shadow_n, ix->dim, dimpad, s.shadow, s.xnorm2, s.dnorm2, s.stream))
-                return -1;
-        } else if (nk::row_sqnorms16(s.rows, ix->dtype, s.shadow_n, s.n - s.shadow_n, ix->dim, s.xnorm2, s.stream)) {
-            return -1;
-        }
-        ix->stats.kernel_launches++;
-    }
-    s.shadow_n = s.n;
+    if (m.n < s.n && shard_image_build(ix, s, m.n, s.n - m.n)) return -1;
+    m.n = s.n;
     return 0;
-}
-static int shard_shadow_row(NkIndex *ix, NkShard &s, uint64_t local) {  // one row changed in place
-    if (!s.xnorm2 || local >= s.shadow_n) return 0;
-    ix->stats.kernel_launches++;
-    if (ix->dtype != NK_DTYPE_F32) return nk::row_sqnorms16(s.rows, ix->dtype, local, 1, ix->dim, s.xnorm2, s.stream);
-    const float *rows = static_cast<const float *>(s.rows);
-    if (s.img8 && nk::build_image_s8(rows, local, 1, ix->dim, ix->dimpad8(), s.img8, s.xscale, s.xnorm2, s.d8norm2, s.stream)) return -1;
-    return s.shadow ? nk::build_shadow(rows, local, 1, ix->dim, ix->dimpad(), s.shadow, s.xnorm2, s.dnorm2, s.stream) : 0;
 }
 
 // ---- cold-start feed (SURVEY.md §8(f)3) ---------------------------------------------------------------------------
@@ -396,58 +386,47 @@ static nk::ScanArgs shard_scan_args(const NkIndex *ix, const NkShard &s, const f
 // Has a search on the shard's int8 image overflowed its margin buffers since the last look?  Reads the counters copied
 // behind the last int8 search if they have landed (never waits); once true, the shard's kNN filter keeps to the BF16 shadow.
 static bool shard_s8_off(const NkShard &s) {
-    if (!s.s8_off && s.s8_ev && cudaEventQuery(s.s8_ev) == cudaSuccess) {
-        const int64_t seen = (int64_t)s.s8_h[0] + s.s8_h[1];
-        if (seen > s.s8_seen) s.s8_off = true;
-        s.s8_seen = seen;
+    const ShardImages &m = s.img;
+    if (!m.s8_off && m.s8_ev && cudaEventQuery(m.s8_ev) == cudaSuccess) {
+        const int64_t seen = (int64_t)m.s8_h[0] + m.s8_h[1];
+        if (seen > m.s8_seen) m.s8_off = true;
+        m.s8_seen = seen;
     }
-    return s.s8_off;
+    return m.s8_off;
 }
 
-// The int8 image serves the kNN filter where it wins: a shard large enough for the scan to be bound by HBM bytes (the same
-// 64 MB as AUTO's), k <= S8_MAX_K, and no earlier overflow on it.  Its margins are ~3x the BF16 shadow's, so at larger k
-// every CTA emits several times more rows for exact re-scoring (Q = 1024, k = 100: 5.6x slower, DESIGN §3.3), and range
-// searches would list more rows; those keep to the BF16 shadow where the shard has one.
+// The image a scan of shard s streams, if the shard has an up-to-date one (else kind NONE): a 16-bit shard's own rows, or
+// the int8 image or the BF16 shadow of an fp32 shard.  knn: a kNN filter search for the k best.  The int8 image serves it
+// where it wins: a shard large enough for the scan to be bound by HBM bytes (the same 64 MB as AUTO's), k <= S8_MAX_K, and
+// no earlier overflow on it.  Its margins are ~3x the BF16 shadow's, so at larger k every CTA emits several times more rows
+// for exact re-scoring (Q = 1024, k = 100: 5.6x slower, DESIGN §3.3), range searches would list more rows and k-means
+// assignment would leave more near-ties to its fix-up; those keep to the BF16 shadow where the shard has one.
 constexpr uint32_t S8_MAX_K = 16;
-static bool use_s8(const NkIndex *ix, const NkShard &s, const nk::ScanArgs &a, bool range) {
-    if (!s.img8) return false;
-    if (!s.shadow) return true;
-    return !range && a.k <= S8_MAX_K && (uint64_t)s.n * ix->dim * 4 >= (64ull << 20) && !shard_s8_off(s);
-}
-
-// a with the shard's image attached, if it has an up-to-date one: the int8 image or the BF16 shadow of an fp32 shard
-// (use_s8), or a 16-bit shard's own rows
-static nk::ScanArgs with_16bit_image(const NkIndex *ix, const NkShard &s, const nk::ScanArgs &a, bool range = false) {
-    nk::ScanArgs as = a;
-    if (s.xnorm2 && s.shadow_n == s.n) {
-        if (ix->dtype != NK_DTYPE_F32) {
-            as.shadow = s.rows; as.shadow_native = true; as.shadow_dimpad = ix->dimpad();
-        } else if (use_s8(ix, s, a, range)) {
-            as.shadow = s.img8; as.dnorm2 = s.d8norm2; as.xscale = s.xscale; as.shadow_dimpad = ix->dimpad8();
-        } else {
-            as.shadow = s.shadow; as.dnorm2 = s.dnorm2; as.shadow_dimpad = ix->dimpad();
-        }
-        as.xnorm2 = s.xnorm2;
-    }
-    return as;
+static nk::RowImage shard_image(const NkIndex *ix, const NkShard &s, bool knn, uint32_t k) {
+    const ShardImages &m = s.img;
+    if (!m.current(s.n)) return {};
+    if (ix->dtype != NK_DTYPE_F32) return nk::RowImage(nk::RowImage::NATIVE, s.rows, ix->dim, m.xnorm2);
+    const bool s8 = m.s8 && (!m.bf16 || (knn && k <= S8_MAX_K && (uint64_t)s.n * ix->dim * 4 >= (64ull << 20) && !shard_s8_off(s)));
+    return s8 ? m.s8_image(ix->dim) : m.bf16_image(ix->dim);
 }
 
 // Behind a search on the int8 image: copy the shard's overflow counters to pinned memory (read by shard_s8_off).
 static int shard_s8_watch(NkShard &s, cudaStream_t stream) {
-    if (!s.s8_ev) {
-        if (cudaEventCreateWithFlags(&s.s8_ev, cudaEventDisableTiming) != cudaSuccess ||
-            cudaMallocHost((void **)&s.s8_h, 2 * sizeof(int)) != cudaSuccess) {
+    ShardImages &m = s.img;
+    if (!m.s8_ev) {
+        if (cudaEventCreateWithFlags(&m.s8_ev, cudaEventDisableTiming) != cudaSuccess ||
+            cudaMallocHost((void **)&m.s8_h, 2 * sizeof(int)) != cudaSuccess) {
             nk::set_error("int8 image: event / pinned counters unavailable");
             return -1;
         }
     }
-    NK_CUDA_OK(cudaMemcpyAsync(s.s8_h, s.ws.flags + nk::FLAG_N_RETRY, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
-    NK_CUDA_OK(cudaEventRecord(s.s8_ev, stream));
+    NK_CUDA_OK(cudaMemcpyAsync(m.s8_h, s.ws.flags + nk::FLAG_N_RETRY, 2 * sizeof(int), cudaMemcpyDeviceToHost, stream));
+    NK_CUDA_OK(cudaEventRecord(m.s8_ev, stream));
     return 0;
 }
 
 // The path a scan of *a over shard s takes: the forced one (an error if it cannot serve the shape), or AUTO's pick.  *a gets
-// the shard's 16-bit image attached if the path is the 16-bit pass.  Range searches have no exact 3xTF32 mode.
+// the shard's image (shard_image) attached if the path is the 16-bit / int8 pass.  Range searches have no exact 3xTF32 mode.
 // AUTO: CUDA cores keep Q <= 4 (the single-kernel scan already streams the fewest bytes), tensor cores from 5 queries on.
 // With a BF16 shadow the filter streams half the bytes of the fp32 rows, so it serves every batch size once the shard is
 // large enough for bytes (not launches) to matter; small shards keep the CUDA-core scan at Q <= 4.  16-bit shards: the
@@ -457,15 +436,16 @@ static int plan_path(const NkIndex *ix, const NkShard &s, bool range, nk::ScanAr
         nk::set_error("nk_search_range: the exact 3xTF32 path has no range mode (use AUTO, SIMT, TENSOR_FILTER or TENSOR_SHADOW)");
         return -1;
     }
-    const nk::ScanArgs as = with_16bit_image(ix, s, *a, range);
+    nk::ScanArgs as = *a;
+    as.image = shard_image(ix, s, !range, a->k);
     const bool tensor_ok = !range && nk::scan_tensor_supported(s.di, *a);
     const bool filter_ok = ix->dtype == NK_DTYPE_F32 && nk::scan_tensor_filter_supported(s.di, *a);
-    const bool shadow_ok = as.shadow != nullptr && nk::shadow_pass_supported(s.di, as) && nk::scan_tensor_filter_supported(s.di, as);
+    const bool shadow_ok = nk::shadow_pass_supported(s.di, as) && nk::scan_tensor_filter_supported(s.di, as);
     int use = NK_PATH_SIMT;
     if (ix->path == NK_PATH_TENSOR || ix->path == NK_PATH_TENSOR_FILTER || ix->path == NK_PATH_TENSOR_SHADOW) {
         if (!(ix->path == NK_PATH_TENSOR ? tensor_ok : ix->path == NK_PATH_TENSOR_FILTER ? filter_ok : shadow_ok)) {
             nk::set_error("tensor path %d does not support this shape (dim=%u dtype=%d metric=%d Q=%u k=%u shadow=%d)", ix->path, ix->dim,
-                          ix->dtype, ix->metric, a->Q, a->k, (int)(as.shadow != nullptr));
+                          ix->dtype, ix->metric, a->Q, a->k, (int)(as.image.kind != nk::RowImage::NONE));
             return -1;
         }
         use = ix->path;
@@ -509,14 +489,10 @@ class ScanTimer {
 };
 
 // NkStats::bytes_scanned of `passes` scans of a on path `use`: every pass streams the a.n rows once per block of queries
-// (8 on CUDA cores, 64 in the exact 3xTF32 scan, 128 in the filters); the image pass streams the image, dimpad8 bytes (int8)
-// or dimpad bf16 per fp32 row.
+// (8 on CUDA cores, 64 in the exact 3xTF32 scan, 128 in the filters); the 16-bit / int8 pass streams the image's rows.
 static uint64_t scan_bytes(const NkIndex *ix, int use, const nk::ScanArgs &a, uint64_t passes) {
     const uint32_t width = use == NK_PATH_SIMT ? 8 : use == NK_PATH_TENSOR ? 64 : 128;
-    const uint64_t row_bytes = use != NK_PATH_TENSOR_SHADOW ? (uint64_t)ix->dim * ix->esz()
-                               : ix->dtype != NK_DTYPE_F32  ? (uint64_t)ix->dim * 2
-                               : a.xscale                   ? (uint64_t)ix->dimpad8()
-                                                            : (uint64_t)ix->dimpad() * 2;
+    const uint64_t row_bytes = use == NK_PATH_TENSOR_SHADOW ? a.image.row_bytes() : (uint64_t)ix->dim * ix->esz();
     return (uint64_t)a.n * row_bytes * ((a.Q + width - 1) / width) * passes;
 }
 
@@ -585,7 +561,7 @@ static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uin
         s.last_out_keys = out_keys;
     }
     ix->stats.bytes_scanned += scan_bytes(ix, use, a, 1);
-    if (use == NK_PATH_TENSOR_SHADOW && a.xscale && shard_s8_watch(s, stream)) return -1;
+    if (use == NK_PATH_TENSOR_SHADOW && a.image.kind == nk::RowImage::S8 && shard_s8_watch(s, stream)) return -1;
     return 0;
 }
 
@@ -636,10 +612,11 @@ NkIndex *nk_index_create(const int *device_ids, int n_devices, uint32_t dim, int
     }
     NkIndex *ix = new NkIndex();
     ix->dim = dim; ix->dtype = dtype; ix->metric = metric;
-    if (const char *e = getenv("NK_SHADOW")) {  // read once, at creation: unset / 1 both images, bf16 / int8 one of them, 0 none
-        if (strcmp(e, "int8") == 0) ix->image_bf16 = false;
-        else if (strcmp(e, "bf16") == 0) ix->image_s8 = false;
-        else ix->shadow_on = atoi(e) != 0;
+    if (const char *e = getenv("NK_SHADOW")) {  // read once, at creation
+        const unsigned native = 1u << nk::RowImage::NATIVE;
+        ix->images = strcmp(e, "int8") == 0 ? 1u << nk::RowImage::S8 | native
+                     : strcmp(e, "bf16") == 0 ? 1u << nk::RowImage::BF16 | native
+                     : atoi(e) != 0 ? ix->images : 0u;
     }
     ix->stats.dim = dim; ix->stats.n_devices = (uint32_t)n_devices;
     ix->shards.resize(n_devices);
@@ -676,11 +653,11 @@ void nk_index_release(NkIndex *ix) {
             cudaStreamDestroy(s.stream);
         }
         if (s.rows && s.owns) cudaFree(s.rows);
-        shard_drop_shadow(s);
+        s.img.release();
+        if (s.img.s8_h) cudaFreeHost(s.img.s8_h);
+        if (s.img.s8_ev) cudaEventDestroy(s.img.s8_ev);
         if (s.h_keys) cudaFreeHost(s.h_keys);
         if (s.h_res) cudaFreeHost(s.h_res);
-        if (s.s8_h) cudaFreeHost(s.s8_h);
-        if (s.s8_ev) cudaEventDestroy(s.s8_ev);
         for (int i = 0; i < 2; ++i) {
             if (s.stage[i]) cudaFreeHost(s.stage[i]);
             if (s.stage_ev[i]) cudaEventDestroy(s.stage_ev[i]);
@@ -710,13 +687,13 @@ static int repartition(NkIndex *ix, uint64_t n_rows, const WriteRows &write) {
         NkShard &s = ix->shards[g];
         const uint64_t cnt = n_rows * (g + 1) / G - n_rows * g / G;
         NK_CUDA_OK(cudaSetDevice(s.device));
-        if (!s.owns) { s.rows = nullptr; s.owns = true; s.cap = 0; s.shadow_attached = false; }
+        if (!s.owns) { s.rows = nullptr; s.owns = true; s.cap = 0; s.img.attached = false; }
         s.n = 0;
         s.tags_on = false;  // every tag back to 0
         if (shard_reserve_rows(ix, s, cnt, false)) return -1;
         if (write(s, off, cnt)) return -1;
         s.n = cnt;
-        s.shadow_n = 0;
+        s.img.n = 0;
         if (shard_sync_shadow(ix, s)) return -1;
         off += cnt;
     }
@@ -802,7 +779,7 @@ int nk_index_update_row(NkIndex *ix, uint64_t row, const void *row_host) {
     const size_t rb = (size_t)ix->dim * ix->esz();
     NK_CUDA_OK(cudaSetDevice(s->device));
     NK_CUDA_OK(cudaMemcpyAsync((char *)s->rows + local * rb, row_host, rb, cudaMemcpyHostToDevice, s->stream));
-    if (shard_shadow_row(ix, *s, local)) return -1;
+    if (s->img.xnorm2 && local < s->img.n && shard_image_build(ix, *s, local, 1)) return -1;
     NK_CUDA_OK(cudaStreamSynchronize(s->stream));
     ix->stats.bytes_h2d += rb;
     return 0;
@@ -837,7 +814,7 @@ int nk_index_remove_swap(NkIndex *ix, uint64_t row) {
         NK_CUDA_OK(cudaSetDevice(s->device));
         if (last->device == s->device) NK_CUDA_OK(cudaMemcpyAsync(dst, src, rb, cudaMemcpyDeviceToDevice, s->stream));
         else NK_CUDA_OK(cudaMemcpyPeerAsync(dst, s->device, src, last->device, rb, s->stream));
-        if (shard_shadow_row(ix, *s, local)) return -1;
+        if (s->img.xnorm2 && local < s->img.n && shard_image_build(ix, *s, local, 1)) return -1;
         NK_CUDA_OK(cudaStreamSynchronize(s->stream));
         if (last->tags_on || s->tags_on) {  // the last row's tag moves with its row
             uint64_t tag = 0;
@@ -851,7 +828,7 @@ int nk_index_remove_swap(NkIndex *ix, uint64_t row) {
         }
     }
     last->n -= 1;
-    if (last->shadow_n > last->n) last->shadow_n = last->n;
+    if (last->img.n > last->n) last->img.n = last->n;
     rebase(ix);
     return 0;
 }
@@ -899,9 +876,9 @@ int nk_index_attach_device_rows(NkIndex *ix, void *rows_dev, uint64_t n_rows) {
     if (s.rows && s.owns) NK_CUDA_OK(cudaFree(s.rows));
     // caller-owned rows may change behind the library's back (cuda_normalize_vectors runs right after NewBuffer,
     // gpu.go:2100-2106): no shadow until the caller says the rows are final (nk_index_refresh_shadow)
-    shard_drop_shadow(s);
+    s.img.release();
     drop_row_mask(ix);
-    s.rows = rows_dev; s.owns = false; s.n = n_rows; s.cap = n_rows; s.shadow_attached = false;
+    s.rows = rows_dev; s.owns = false; s.n = n_rows; s.cap = n_rows; s.img.attached = false;
     s.tags_on = false;  // every tag back to 0
     rebase(ix);
     return 0;
@@ -918,8 +895,8 @@ int nk_index_refresh_shadow(NkIndex *ix) {
     if (order.failed()) return -1;
     for (auto &s : ix->shards) {
         NK_CUDA_OK(cudaSetDevice(s.device));
-        if (!s.owns) s.shadow_attached = true;
-        s.shadow_n = 0;
+        if (!s.owns) s.img.attached = true;
+        s.img.n = 0;
         if (shard_sync_shadow(ix, s)) return -1;
         NK_CUDA_OK(cudaStreamSynchronize(s.stream));
     }
@@ -1075,7 +1052,8 @@ int nk_debug_filter_dump(NkIndex *ix, const float *queries_host, uint32_t Q, int
         if (nk::ws_reserve((void **)&s->ws.queries, &s->ws.queries_bytes, (size_t)Q * ix->dim * 4)) break;
         if (cudaMemcpyAsync(s->ws.queries, queries_host, (size_t)Q * ix->dim * 4, cudaMemcpyHostToDevice, s->stream) != cudaSuccess) break;
         if (cudaMemsetAsync(d, 0, cells * 8, s->stream) != cudaSuccess) break;
-        nk::ScanArgs a = with_16bit_image(ix, *s, shard_scan_args(ix, *s, s->ws.queries, Q, 1, s->stream));
+        nk::ScanArgs a = shard_scan_args(ix, *s, s->ws.queries, Q, 1, s->stream);
+        a.image = shard_image(ix, *s, true, 1);
         a.row_mask = nullptr;  // every pair (the dump ignores the score floor itself)
         if (nk::scan_filter_dump(s->di, a, s->ws, which, d, d + cells, Q, &ix->stats.kernel_launches)) break;
         if (cudaMemcpyAsync(est_host, d, cells * 4, cudaMemcpyDeviceToHost, s->stream) != cudaSuccess) break;
@@ -1488,12 +1466,7 @@ static int range_shard(NkIndex *ix, NkShard &s, uint32_t Q, const NkFilter *qfil
         a.row_base = s.base + from;
         if (a.row_mask) a.row_mask += from / 32;
         if (a.row_tags) a.row_tags += from;
-        if (a.shadow) {
-            a.shadow = static_cast<const char *>(a.shadow) + from * (a.shadow_native ? ix->dim * 2 : a.xscale ? a.shadow_dimpad : a.shadow_dimpad * 2);
-            a.xnorm2 += from;
-            if (a.dnorm2) a.dnorm2 += from;
-            if (a.xscale) a.xscale += from;
-        }
+        a.image = a.image.window(from);
     }
     ScanTimer timer(s);
     if (timer.attach(ix, &a)) return -1;
@@ -1816,7 +1789,7 @@ static int knn_graph_remap_locked(NkIndex *ix, const char *what, uint32_t k, uin
     if (gpath == NK_PATH_AUTO) {
         gpath = NK_PATH_TENSOR_SHADOW;
         for (NkShard *s : live)
-            if (!(s->xnorm2 && s->shadow_n == s->n)) gpath = NK_PATH_TENSOR_FILTER;
+            if (!s->img.current(s->n)) gpath = NK_PATH_TENSOR_FILTER;
     }
     struct PathGuard {
         NkIndex *ix; int saved;
@@ -2318,7 +2291,8 @@ static int assign_nearest(NkIndex *ix, const float *centroids_host, uint32_t K, 
     for (auto &s : ix->shards) {
         if (s.n == 0) continue;
         NK_CUDA_OK(cudaSetDevice(s.device));
-        const bool tensor = (s.shadow || s.img8) && s.shadow_n == s.n && nk::assign_tensor_supported(s.di, ix->dim, K, metric);
+        const nk::RowImage img = shard_image(ix, s, false, 0);
+        const bool tensor = img.kind != nk::RowImage::NONE && nk::assign_tensor_supported(s.di, ix->dim, K, metric);
         const uint32_t k = K < 2 ? K : 2u;
         NkIndex *cx = tensor ? nullptr : nk_index_create(&s.device, 1, ix->dim, NK_DTYPE_F32, metric);
         if (!tensor && !cx) return -1;
@@ -2350,14 +2324,9 @@ static int assign_nearest(NkIndex *ix, const float *centroids_host, uint32_t K, 
             if (e != cudaSuccess) rc = -1;
         }
         const float *rows = static_cast<const float *>(s.rows);
-        if (rc == 0 && tensor) {
-            // (the BF16 shadow where the shard has one: the int8 image's wider margins leave more near-ties to the fix-up)
-            rc = s.shadow ? nk::assign_tensor(s.di, rows, s.shadow, ix->dimpad(), nullptr, s.xnorm2, s.dnorm2, (uint32_t)s.n,
-                                              ix->dim, d_cen, K, metric, ties, d_asg, s.stream, &ix->stats.kernel_launches,
-                                              &s.ws.sub_gather, &s.ws.sub_gather_bytes)
-                          : nk::assign_tensor(s.di, rows, s.img8, ix->dimpad8(), s.xscale, s.xnorm2, s.d8norm2, (uint32_t)s.n, ix->dim, d_cen, K, metric, ties, d_asg,
-                                   s.stream, &ix->stats.kernel_launches, &s.ws.sub_gather, &s.ws.sub_gather_bytes);
-        }
+        if (rc == 0 && tensor)
+            rc = nk::assign_tensor(s.di, rows, img, (uint32_t)s.n, ix->dim, d_cen, K, metric, ties, d_asg, s.stream, &ix->stats.kernel_launches,
+                                   &s.ws.sub_gather, &s.ws.sub_gather_bytes);
         const uint64_t B = 8192;  // rows per fused search: amortises the ~12 fixed launches of a search over 8 scan launches
         for (uint64_t b = 0; rc == 0 && !tensor && b < s.n; b += B) {
             const uint32_t nb = (uint32_t)std::min<uint64_t>(B, s.n - b);

@@ -46,6 +46,35 @@ struct Workspace {
 };
 int ws_reserve(void **p, size_t *cur, size_t need);
 
+// What the filter's 16-bit / int8 pass streams in place of a shard's rows (scan_tensor_shadow.cu, DESIGN §2): the BF16
+// shadow or the int8 image of an fp32 shard, or the rows of an fp16 / bf16 shard scanned in place.
+struct RowImage {
+    enum Kind { NONE, BF16, S8, NATIVE };
+    Kind kind = NONE;
+    const void *data = nullptr;
+    uint32_t dimpad = 0;  // columns the scan covers: dim rounded up to one 128-byte swizzle row (64 16-bit / 128 int8 elements)
+    uint32_t stride = 0;  // row stride in elements: dimpad, or dim for rows scanned in place (columns past dim read as zero)
+    const float *xnorm2 = nullptr;  // per row |x|^2
+    const float *dnorm2 = nullptr;  // per row |x - image(x)|^2; nullptr for rows scanned in place (no residue)
+    const float *xscale = nullptr;  // int8 only: per row s, x ~ s * int8 row
+    RowImage() = default;
+    RowImage(Kind k, const void *d, uint32_t dim, const float *x2, const float *d2 = nullptr, const float *xs = nullptr)
+        : kind(k), data(d), dimpad(k == S8 ? (dim + 127) / 128 * 128 : (dim + 63) / 64 * 64), stride(k == NATIVE ? dim : dimpad),
+          xnorm2(x2), dnorm2(d2), xscale(xs) {}
+    uint32_t esz() const { return kind == S8 ? 1 : 2; }
+    uint64_t row_bytes() const { return (uint64_t)stride * esz(); }
+    // the image of rows [from, ..): the data and the per-row arrays move together
+    RowImage window(uint64_t from) const {
+        RowImage w = *this;
+        if (kind == NONE) return w;
+        w.data = static_cast<const char *>(data) + from * row_bytes();
+        w.xnorm2 += from;
+        if (dnorm2) w.dnorm2 += from;
+        if (xscale) w.xscale += from;
+        return w;
+    }
+};
+
 struct ScanArgs {
     const void *rows = nullptr;  // [n x dim] row-major, fp32 or fp16
     int dtype = NK_DTYPE_F32;
@@ -73,14 +102,7 @@ struct ScanArgs {
     // filtered (TAGS) instantiations, so unfiltered searches run unchanged code.
     const uint64_t *row_tags = nullptr;
     const NkFilter *qfilter = nullptr;
-    // optional image of an fp32 shard (scan_tensor_shadow.cu): rows of `shadow_dimpad` elements + per-row |x|^2 and
-    // |x - image(x)|^2; nullptr = none.  xscale != nullptr: the int8 image (x ~ xscale[row] * int8 row, stride shadow_dimpad
-    // bytes); otherwise the BF16 shadow (stride shadow_dimpad * 2 bytes)
-    const void *shadow = nullptr;
-    uint32_t shadow_dimpad = 0;
-    bool shadow_native = false;  // 16-bit corpus: shadow == rows (row stride dim * 2 bytes), dnorm2 == nullptr
-    const float *xnorm2 = nullptr, *dnorm2 = nullptr;
-    const float *xscale = nullptr;
+    RowImage image;  // what the 16-bit / int8 pass streams; kind NONE = no such pass
     // optional fused decode: the final (index, score) arrays [Q x k] are written by the last kernel of the path
     uint32_t *out_idx = nullptr;
     float *out_score = nullptr;
@@ -105,7 +127,7 @@ struct ScanArgs {
 int scan_simt(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *out_keys, uint64_t *launches);
 
 // Tensor-core scans (scan_tensor.cu, scan_tensor_shadow.cu): the exact 3xTF32 scan, and the filter (TF32 over fp32 rows, or
-// the 16-bit pass over a.shadow) with exact re-scoring.  scan_tensor_filter_tail queues the retry / exact stages a deferred
+// the 16-bit / int8 pass over a.image) with exact re-scoring.  scan_tensor_filter_tail queues the retry / exact stages a deferred
 // (a.defer_tail) filter search skipped.
 int scan_tensor(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *out_keys, uint64_t *launches);
 bool scan_tensor_supported(const DeviceInfo &di, const ScanArgs &a);
@@ -131,9 +153,8 @@ struct AssignTies {
 };
 // One pass of the 16-bit scan with an argmax epilogue.
 bool assign_tensor_supported(const DeviceInfo &di, uint32_t dim, uint32_t K, int metric);
-int assign_tensor(const DeviceInfo &di, const float *rows, const void *shadow, uint32_t dimpad, const float *xscale, const float *xnorm2,
-                  const float *dnorm2, uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric, AssignTies ties, uint32_t *assign_dev,
-                  cudaStream_t stream, uint64_t *launches, void **scratch, size_t *scratch_bytes);
+int assign_tensor(const DeviceInfo &di, const float *rows, const RowImage &img, uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K,
+                  int metric, AssignTies ties, uint32_t *assign_dev, cudaStream_t stream, uint64_t *launches, void **scratch, size_t *scratch_bytes);
 // From a k = min(2, K) search of the rows against the centroids (idx / sc: [n x k], euclidean scores as distances).
 int assign_from_search(const DeviceInfo &di, const float *rows, uint32_t n, uint32_t dim, const float *centroids_dev, uint32_t K, int metric,
                        const uint32_t *idx, const float *sc, uint32_t k, AssignTies ties, uint32_t *assign_dev, cudaStream_t stream,
@@ -148,7 +169,7 @@ int fatal_overflow(int flag, int *flags, cudaStream_t stream);
 // [Q][list_cap].  A fill counts every survivor, also those past list_cap.  range_qa mirrors the filter's padded per-query
 // arrays (Qpad + tc::QT_BIG), whose shared thresholds and fills sit at the same places.
 inline uint32_t range_qa(uint32_t Q) { return (Q + 63) / 64 * 64 + 256; }
-// 16-bit (a.shadow set) or TF32 filter scan with fixed thresholds: lists hold every pair whose UPPER bound reaches the threshold.
+// 16-bit / int8 (a.image set) or TF32 filter scan with fixed thresholds: lists hold every pair whose UPPER bound reaches the threshold.
 int scan_tensor_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint32_t list_cap, uint64_t *launches);
 // CUDA-core scan: lists hold every pair whose exact score reaches the threshold.
 int scan_simt_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint32_t list_cap, uint64_t *launches);

@@ -1020,14 +1020,22 @@ static void tc_print_prof(cudaStream_t stream, uint32_t num_tiles, uint32_t grid
 // (device, args).  Deterministic, so the host-driven retry of nk_search can rebuild it after the fact.
 struct FilterPlan {
     uint32_t Qpad, QA, num_tiles, grid, k_emit, dimpad, sample;
-    bool big;           // first stage = 16-bit pass (BF16 shadow of an fp32 shard, or an fp16 / bf16 corpus itself)
-    bool stage2;        // the TF32 filter over the fp32 rows exists as the retry stage (fp32 shards with a shadow)
+    bool big;           // first stage = 16-bit / int8 pass over a.image
+    bool s8;            // a.image is the int8 image
+    bool stage2;        // the TF32 filter over the fp32 rows exists as the retry stage (fp32 shards with an image)
     bool can_exact_tc;  // exact stage = 3xTF32 kernel (else the CUDA-core scan)
     float acc_c, margin_tf32;
     float *qhi, *qlo, *qnorm, *qa, *qb, *qscale;
     void *qbf16;        // the queries in the image's element type: bf16 / fp16, or int8 (with qscale) for an int8 image
     uint32_t max_groups_shadow;
     size_t fsmem;
+    // the fields every 16-bit / int8 pass of the plan shares; the caller sets the query range and the mode
+    ShadowPassArgs shadow_pass() const {
+        ShadowPassArgs sp{};
+        sp.grid = grid; sp.k_emit = k_emit; sp.dimpad = dimpad; sp.Qpad = Qpad;
+        sp.qbf16 = qbf16; sp.qnorm = qnorm; sp.qa = qa; sp.qb = qb; sp.qscale = qscale;
+        return sp;
+    }
 };
 
 static int make_filter_plan(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, FilterPlan *fp) {
@@ -1046,14 +1054,15 @@ static int make_filter_plan(const DeviceInfo &di, const ScanArgs &a, Workspace &
     f.acc_c = (float)a.dim * 2.384185791015625e-7f + 4e-6f;
     f.margin_tf32 = 9.765625e-4f + f.acc_c;
     f.big = shadow_pass_supported(di, a);
+    f.s8 = a.image.kind == RowImage::S8;
     f.stage2 = f.big && a.dtype == NK_DTYPE_F32 && tc_common_ok(di, a);
     f.can_exact_tc = scan_tensor_supported(di, a);  // euclidean / 16-bit rows have no 3xTF32 twin: overflow -> CUDA-core scan
     // 16-bit margins are ~6x wider than TF32's and clustered corpora put hundreds of rows per CTA inside them: the 16-bit
     // kernel has 1024-slot buffers and emits up to 512 entries per (CTA, query) (the finish step re-scores in rounds).  The
     // int8 image's margins are ~3x the BF16 shadow's: a CTA's local top 100 of 300k uniform rows already has ~550 rows inside
     // them, so it emits up to the whole prunable buffer at every k.
-    if (f.big) f.k_emit = a.k <= 160 && !a.xscale ? 512u : (uint32_t)(P_SHADOW - ROWS);
-    f.dimpad = f.big ? a.shadow_dimpad : (a.dim + 63) / 64 * 64;
+    if (f.big) f.k_emit = a.k <= 160 && !f.s8 ? 512u : (uint32_t)(P_SHADOW - ROWS);
+    f.dimpad = f.big ? a.image.dimpad : (a.dim + 63) / 64 * 64;
     const bool need_f32q = a.dtype == NK_DTYPE_F32;  // hi / lo arrays only serve passes over fp32 rows
     const size_t qaux_floats = (need_f32q ? (size_t)2 * f.Qpad * a.dim : 0) + (size_t)4 * f.QA;
     if (ws_reserve((void **)&ws.qaux, &ws.qaux_bytes, qaux_floats * 4 + (f.big ? (size_t)f.Qpad * f.dimpad * 2 : 0))) return -1;
@@ -1065,7 +1074,7 @@ static int make_filter_plan(const DeviceInfo &di, const ScanArgs &a, Workspace &
     f.qnorm = ws.qaux + (need_f32q ? (size_t)2 * f.Qpad * a.dim : 0);
     f.qa = f.qnorm + f.QA;
     f.qb = f.qa + f.QA;
-    f.qscale = a.xscale ? f.qb + f.QA : nullptr;
+    f.qscale = f.s8 ? f.qb + f.QA : nullptr;
     f.qbf16 = ws.qaux + qaux_floats;
     // G query groups leave each CTA 1/G of the grid for its queries, i.e. G times the rows — and G times the rows inside
     // the BF16 margin — per (CTA, query) buffer: large k keeps fewer groups so that k + margin rows stay inside k_emit
@@ -1140,8 +1149,8 @@ static int tf32_passes(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, c
 static PrepParams filter_prep_params(const ScanArgs &a, Workspace &ws, const FilterPlan &f) {
     PrepParams pp = prep_params(a, f.Qpad, f.dimpad);
     pp.acc_c = f.acc_c; pp.qhi = f.qhi;
-    pp.qbf = f.big && !a.xscale ? static_cast<uint16_t *>(f.qbf16) : nullptr; pp.qbf_f16 = a.dtype == NK_DTYPE_F16;
-    pp.qs8 = f.big && a.xscale ? static_cast<int8_t *>(f.qbf16) : nullptr; pp.qscale = f.qscale;
+    pp.qbf = f.big && !f.s8 ? static_cast<uint16_t *>(f.qbf16) : nullptr; pp.qbf_f16 = a.dtype == NK_DTYPE_F16;
+    pp.qs8 = f.big && f.s8 ? static_cast<int8_t *>(f.qbf16) : nullptr; pp.qscale = f.qscale;
     pp.qnorm = f.qnorm; pp.qa = f.qa; pp.qb = f.qb;
     pp.state = reinterpret_cast<uint32_t *>(ws.keys2); pp.QA = f.QA; pp.flags = ws.flags; pp.sample = f.sample;
     return pp;
@@ -1205,9 +1214,8 @@ int scan_tensor_filter(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, u
 
     if (a.ev_begin) NK_CUDA_OK(cudaEventRecord(a.ev_begin, a.stream));
     if (plan_launches(0, q_big, f.grid, f.max_groups_shadow, [&](uint32_t qt, uint32_t q0, uint32_t nq, uint32_t groups) {
-            ShadowPassArgs sp{};
-            sp.grid = f.grid; sp.k_emit = f.k_emit; sp.dimpad = f.dimpad; sp.Qpad = f.Qpad; sp.q0 = q0; sp.nq = nq; sp.qgroups = groups;
-            sp.qbf16 = f.qbf16; sp.qnorm = f.qnorm; sp.qa = f.qa; sp.qb = f.qb; sp.qscale = f.qscale; sp.presampled = f.sample != 0;
+            ShadowPassArgs sp = f.shadow_pass();
+            sp.q0 = q0; sp.nq = nq; sp.qgroups = groups; sp.presampled = f.sample != 0;
             return launch_shadow_pass((int)qt, di, a, ws, sp, launches);
         }))
         return -1;
@@ -1226,7 +1234,7 @@ int scan_tensor_filter(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, u
     return scan_tensor_filter_tail(di, a, ws, out_keys, launches);
 }
 
-// Range mode (nk_search_range, range.cu): the query prep, then the 16-bit pass (shadow attached) or the TF32 filter over the
+// Range mode (nk_search_range, range.cu): the query prep, then the 16-bit / int8 pass (a.image set) or the TF32 filter over the
 // fp32 rows with FIXED thresholds: ws.keys2 holds the order-preserving bits of every query's key-space threshold where the
 // filter keeps its shared thresholds (presampled: no flood tiles, nothing is published), and every pair whose upper bound
 // reaches it lands in ws.partial [Q][list_cap], fill counted in the list fills next to them (range_qa).  The caller
@@ -1247,9 +1255,8 @@ int scan_tensor_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, ui
     int rc;
     if (f.big) {
         rc = plan_launches(0, a.Q, f.grid, 4, [&](uint32_t qt, uint32_t q0, uint32_t nq, uint32_t groups) {
-            ShadowPassArgs sp{};
-            sp.grid = f.grid; sp.k_emit = f.k_emit; sp.dimpad = f.dimpad; sp.Qpad = f.Qpad; sp.q0 = q0; sp.nq = nq; sp.qgroups = groups;
-            sp.qbf16 = f.qbf16; sp.qnorm = f.qnorm; sp.qa = f.qa; sp.qb = f.qb; sp.qscale = f.qscale; sp.presampled = 1; sp.range = true; sp.list_cap = list_cap;
+            ShadowPassArgs sp = f.shadow_pass();
+            sp.q0 = q0; sp.nq = nq; sp.qgroups = groups; sp.presampled = 1; sp.range = true; sp.list_cap = list_cap;
             return launch_shadow_pass((int)qt, di, b, ws, sp, launches);
         });
     } else {
@@ -1284,9 +1291,8 @@ int scan_filter_dump(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, int
     pp.sample = 0;
     if (launch_prep(di, pp, b.stream, launches)) return -1;
     if (which == NK_PATH_TENSOR_SHADOW) {
-        ShadowPassArgs sp{};
-        sp.grid = f.grid; sp.k_emit = f.k_emit; sp.dimpad = f.dimpad; sp.Qpad = f.Qpad; sp.q0 = 0; sp.nq = b.Q; sp.qgroups = 1;
-        sp.qbf16 = f.qbf16; sp.qnorm = f.qnorm; sp.qa = f.qa; sp.qb = f.qb; sp.qscale = f.qscale; sp.presampled = 0;
+        ShadowPassArgs sp = f.shadow_pass();
+        sp.q0 = 0; sp.nq = b.Q; sp.qgroups = 1; sp.presampled = 0;
         sp.dump_est = est; sp.dump_bnd = bnd; sp.dump_ld = ld;
         if (launch_shadow_pass(64, di, b, ws, sp, launches)) return -1;
     } else {

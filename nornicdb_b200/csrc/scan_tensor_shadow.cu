@@ -28,7 +28,7 @@
 // extent of a TF32 slab: half the bytes per product of the TF32 kernel, which is shared-memory-bandwidth bound at 128
 // query columns.  Algorithmic HBM bytes per launch: n * dimpad * 2 (shadow) + n * 8 (norms).
 //
-// Int8 image (Opnd::S8; the kNN filter picks it per search, index_api.cu use_s8): rows of dimpad8 = ceil(d / 128) * 128 int8 with one fp32 scale per row, x ~ s_x xq,
+// Int8 image (Opnd::S8; the kNN filter picks it per search, index_api.cu shard_image): rows of dimpad8 = ceil(d / 128) * 128 int8 with one fp32 scale per row, x ~ s_x xq,
 // and int8 queries with one scale each.  The shared-memory layout is the same byte for byte (a 128-byte swizzle row holds 128
 // int8, one m64nQTk32 s8 MMA consumes the 32 B of one bf16 k16 MMA), the slab count halves, the exact s32 accumulators are
 // converted in place to float(acc) s_q and s_x joins the row's multiplier.  The bound above holds for any image xb, qb, with
@@ -590,11 +590,12 @@ static void sb_print_prof(cudaStream_t stream, uint32_t grid) {
             tend_max / 1e3, prune / g / 1e3, ftile / g, wait / g / 1e3);
 }
 
-// The 16-bit pass needs a 16-bit image of the rows: the BF16 shadow of an fp32 shard, or — fp16 / bf16 corpora — the rows
-// themselves (a.shadow == a.rows, shadow_native: no rounding residue on the row side, only the per-row |x|^2 array).
+// The 16-bit / int8 pass needs an image of the rows (a.image): the BF16 shadow or the int8 image of an fp32 shard, or —
+// fp16 / bf16 corpora — the rows themselves (no rounding residue on the row side, only the per-row |x|^2 array).
 bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a) {
-    if (di.cc < 90 || a.shadow == nullptr || a.xnorm2 == nullptr || a.k > 192 || a.dim > 32768 || a.dim < 32 || a.n == 0) return false;
-    if ((reinterpret_cast<uintptr_t>(a.rows) & 15) != 0 || (reinterpret_cast<uintptr_t>(a.shadow) & 15) != 0) return false;
+    if (di.cc < 90 || a.image.kind == RowImage::NONE || a.image.xnorm2 == nullptr || a.k > 192 || a.dim > 32768 || a.dim < 32 || a.n == 0)
+        return false;
+    if ((reinterpret_cast<uintptr_t>(a.rows) & 15) != 0 || (reinterpret_cast<uintptr_t>(a.image.data) & 15) != 0) return false;
     if (a.dtype == NK_DTYPE_F32) return a.dim % 4 == 0;
     return a.dim % 8 == 0;  // 16-bit rows: 16-byte TMA row stride and 128-bit exact re-scoring loads
 }
@@ -602,10 +603,9 @@ bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a) {
 template <int QT, ptx::Opnd OP, bool DUMP, bool TAGS, bool RANGE = false, bool ROWTHR = false, bool RFILT = false>
 static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
     using namespace sb;
-    const bool native = a.shadow_native;  // 16-bit corpus scanned in place: row stride dim * 2, columns past dim read as zero (TMA OOB fill)
     const uint32_t esz = OP == ptx::Opnd::S8 ? 1 : 2, kcols = 128 / esz;  // int8 image: 1-byte elements, 128 per swizzle row
-    const CUtensorMap *map_rows = tc_cached_map(ws, 4, a.shadow, a.n, native ? a.dim : sp.dimpad, esz, kcols, ROWS,
-                                                (uint64_t)(native ? a.dim : sp.dimpad) * esz, a.dtype);
+    // rows scanned in place have stride dim: the columns past dim read as zero (TMA OOB fill)
+    const CUtensorMap *map_rows = tc_cached_map(ws, 4, a.image.data, a.n, a.image.stride, esz, kcols, ROWS, a.image.row_bytes(), a.dtype);
     const CUtensorMap *map_q = tc_cached_map(ws, QT == 64 ? 5 : 6, sp.qbf16, sp.Qpad, sp.dimpad, esz, kcols, QT, (uint64_t)sp.dimpad * esz,
                                              a.dtype);  // rows past Qpad: zero
     if (!map_rows || !map_q) return -1;
@@ -617,8 +617,8 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
     if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, OP, DUMP, TAGS, RANGE, ROWTHR, RFILT>), di.device_id, smem))
         return -1;
     tc::Params p = pass_params(a, ws, sp);
-    p.nslab = sp.dimpad / kcols; p.qa = sp.qa; p.qb = sp.qb; p.xnorm2 = a.xnorm2; p.dnorm2 = a.dnorm2;
-    p.xscale = a.xscale; p.qscale = sp.qscale;
+    p.nslab = sp.dimpad / kcols; p.qa = sp.qa; p.qb = sp.qb; p.xnorm2 = a.image.xnorm2; p.dnorm2 = a.image.dnorm2;
+    p.xscale = a.image.xscale; p.qscale = sp.qscale;
     knn_scan_shadow_kernel<QT, OP, DUMP, TAGS, RANGE, ROWTHR, RFILT><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
     NK_CUDA_OK(cudaGetLastError());
     if (launches) ++*launches;
@@ -656,12 +656,11 @@ static int launch_shadow_pass_op(int qt, const DeviceInfo &di, const ScanArgs &a
                      : launch_shadow_pass_t<64, OP, false, false>(di, a, ws, sp, launches);
 }
 
-// fp32 shards with the int8 image run the s8 wgmma form, fp16 corpora the fp16 one, fp32 shards with the BF16 shadow and
-// bf16 corpora the bf16 one
+// the int8 image runs the s8 wgmma form, the BF16 shadow the bf16 one, rows scanned in place the form of their dtype
 int launch_shadow_pass(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
-    if (a.xscale) return launch_shadow_pass_op<ptx::Opnd::S8>(qt, di, a, ws, sp, launches);
-    return a.dtype == NK_DTYPE_F16 ? launch_shadow_pass_op<ptx::Opnd::F16>(qt, di, a, ws, sp, launches)
-                                   : launch_shadow_pass_op<ptx::Opnd::BF16>(qt, di, a, ws, sp, launches);
+    if (a.image.kind == RowImage::S8) return launch_shadow_pass_op<ptx::Opnd::S8>(qt, di, a, ws, sp, launches);
+    return a.image.kind == RowImage::NATIVE && a.dtype == NK_DTYPE_F16 ? launch_shadow_pass_op<ptx::Opnd::F16>(qt, di, a, ws, sp, launches)
+                                                                       : launch_shadow_pass_op<ptx::Opnd::BF16>(qt, di, a, ws, sp, launches);
 }
 
 }  // namespace nk
