@@ -57,10 +57,6 @@ struct NkShard {
     bool owns = true;
     uint64_t n = 0, cap = 0, base = 0;
     ShardImages img;
-    // last filter search (host-synchronous API): what the deferred retry tail needs
-    nk::ScanArgs last_args;
-    uint64_t *last_out_keys = nullptr;
-    bool last_filter = false;
     uint32_t *group = nullptr;  // node id per row (nk_index_set_row_groups), local rows
     size_t group_bytes = 0;
     bool group_on = false;
@@ -118,6 +114,16 @@ struct NkIndex {
         for (auto &s : shards) t += s.n;
         return t;
     }
+    uint64_t returnable_rows() const { return mask_on ? mask_alive : rows(); }  // rows that can be returned
+    uint64_t first_row(const NkShard &s) const { return s.base - row_base; }    // of a shard, relative to the index's first row
+};
+
+// An NVTX range (NK_RANGE_PUSH) that lasts to the end of the scope.
+struct ScopedRange {
+    explicit ScopedRange(const char *name) { NK_RANGE_PUSH(name); }
+    ~ScopedRange() { NK_RANGE_POP(); }
+    ScopedRange(const ScopedRange &) = delete;
+    ScopedRange &operator=(const ScopedRange &) = delete;
 };
 
 // ---- call order (include/nornic_knn.h, "Call order") ------------------------------------------------------------------
@@ -364,8 +370,8 @@ static void rebase(NkIndex *ix) {
 // Locate the shard holding global row `row` (relative to row_base).
 static NkShard *find_shard(NkIndex *ix, uint64_t row, uint64_t *local) {
     for (auto &s : ix->shards)
-        if (row >= s.base - ix->row_base && row < s.base - ix->row_base + s.n) {
-            *local = row - (s.base - ix->row_base);
+        if (row >= ix->first_row(s) && row < ix->first_row(s) + s.n) {
+            *local = row - ix->first_row(s);
             return &s;
         }
     return nullptr;
@@ -425,14 +431,15 @@ static int shard_s8_watch(NkShard &s, cudaStream_t stream) {
     return 0;
 }
 
-// The path a scan of *a over shard s takes: the forced one (an error if it cannot serve the shape), or AUTO's pick.  *a gets
+// The path a scan of *a over shard s takes when the call asks for `path` (the index's setting, nk_index_set_path, or the
+// one a graph call chose): the forced one (an error if it cannot serve the shape), or AUTO's pick.  *a gets
 // the shard's image (shard_image) attached if the path is the 16-bit / int8 pass.  Range searches have no exact 3xTF32 mode.
 // AUTO: CUDA cores keep Q <= 4 (the single-kernel scan already streams the fewest bytes), tensor cores from 5 queries on.
 // With a BF16 shadow the filter streams half the bytes of the fp32 rows, so it serves every batch size once the shard is
 // large enough for bytes (not launches) to matter; small shards keep the CUDA-core scan at Q <= 4.  16-bit shards: the
 // 16-bit tensor pass from 5 queries on.
-static int plan_path(const NkIndex *ix, const NkShard &s, bool range, nk::ScanArgs *a) {
-    if (range && ix->path == NK_PATH_TENSOR) {
+static int plan_path(const NkIndex *ix, const NkShard &s, int path, bool range, nk::ScanArgs *a) {
+    if (range && path == NK_PATH_TENSOR) {
         nk::set_error("nk_search_range: the exact 3xTF32 path has no range mode (use AUTO, SIMT, TENSOR_FILTER or TENSOR_SHADOW)");
         return -1;
     }
@@ -442,14 +449,14 @@ static int plan_path(const NkIndex *ix, const NkShard &s, bool range, nk::ScanAr
     const bool filter_ok = ix->dtype == NK_DTYPE_F32 && nk::scan_tensor_filter_supported(s.di, *a);
     const bool shadow_ok = nk::shadow_pass_supported(s.di, as) && nk::scan_tensor_filter_supported(s.di, as);
     int use = NK_PATH_SIMT;
-    if (ix->path == NK_PATH_TENSOR || ix->path == NK_PATH_TENSOR_FILTER || ix->path == NK_PATH_TENSOR_SHADOW) {
-        if (!(ix->path == NK_PATH_TENSOR ? tensor_ok : ix->path == NK_PATH_TENSOR_FILTER ? filter_ok : shadow_ok)) {
-            nk::set_error("tensor path %d does not support this shape (dim=%u dtype=%d metric=%d Q=%u k=%u shadow=%d)", ix->path, ix->dim,
+    if (path == NK_PATH_TENSOR || path == NK_PATH_TENSOR_FILTER || path == NK_PATH_TENSOR_SHADOW) {
+        if (!(path == NK_PATH_TENSOR ? tensor_ok : path == NK_PATH_TENSOR_FILTER ? filter_ok : shadow_ok)) {
+            nk::set_error("tensor path %d does not support this shape (dim=%u dtype=%d metric=%d Q=%u k=%u shadow=%d)", path, ix->dim,
                           ix->dtype, ix->metric, a->Q, a->k, (int)(as.image.kind != nk::RowImage::NONE));
             return -1;
         }
-        use = ix->path;
-    } else if (ix->path == NK_PATH_AUTO) {
+        use = path;
+    } else if (path == NK_PATH_AUTO) {
         const bool big_shard = (uint64_t)s.n * ix->dim * 4 >= (64ull << 20);
         if (a->Q >= 5) use = shadow_ok ? NK_PATH_TENSOR_SHADOW : filter_ok ? NK_PATH_TENSOR_FILTER : tensor_ok ? NK_PATH_TENSOR : NK_PATH_SIMT;
         else if (shadow_ok && big_shard && ix->dtype == NK_DTYPE_F32) use = NK_PATH_TENSOR_SHADOW;
@@ -519,16 +526,25 @@ static int run_scan_bigk(NkIndex *ix, NkShard &s, nk::ScanArgs a, uint64_t *out_
     return 0;
 }
 
-struct ScanOut {  // optional extras of run_scan
+// The retry / exact stages a host-synchronous filter search left unqueued, as a value its caller owns: run_scan fills it,
+// shard_status queues the stages from it once the host has seen a status word raised.
+struct DeferredTail {
+    bool pending = false;  // a filter scan ran and its tail has not been looked at yet
+    nk::ScanArgs args;     // the scan to re-issue (scan_tensor_filter_tail), without its timing events
+    uint64_t *out_keys = nullptr;
+};
+
+struct ScanOut {  // what a call asks of run_scan beyond the queries
+    explicit ScanOut(int path) : path(path) {}
+    int path;                      // the scan path of the call (plan_path)
     uint32_t *out_idx = nullptr;   // fused decode (single-shard searches)
     float *out_score = nullptr;
-    bool defer_tail = false;       // host-synchronous caller: retry stages are queued only if a flag was raised
+    DeferredTail *tail = nullptr;  // host-synchronous caller: retry stages are left to *tail, queued only if a flag was raised
     const NkFilter *qfilter = nullptr;  // per-query tag filters [Q] (device; the shard's tag array must be on)
 };
 
 static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uint32_t k, uint64_t *out_keys,
-                    cudaStream_t stream, const ScanOut &xo = ScanOut()) {
-    s.last_filter = false;
+                    cudaStream_t stream, const ScanOut &xo) {
     nk::ScanArgs a = shard_scan_args(ix, s, q_dev, Q, k, stream, xo.qfilter);
     if (k > NK_MAX_K) {
         if (run_scan_bigk(ix, s, a, out_keys)) return -1;
@@ -538,8 +554,8 @@ static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uin
         }
         return 0;
     }
-    a.out_idx = xo.out_idx; a.out_score = xo.out_score; a.defer_tail = xo.defer_tail;
-    const int use = plan_path(ix, s, false, &a);
+    a.out_idx = xo.out_idx; a.out_score = xo.out_score; a.defer_tail = xo.tail != nullptr;
+    const int use = plan_path(ix, s, xo.path, false, &a);
     if (use < 0) return -1;
     ScanTimer timer(s);
     if (timer.attach(ix, &a)) return -1;
@@ -553,12 +569,10 @@ static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uin
     ix->last_path = use;
     if (rc) return rc;
     timer.keep();
-    if (is_filter) {
-        s.last_filter = true;
-        s.last_args = a;
-        s.last_args.ev_begin = s.last_args.ev_end = nullptr;
-        s.last_args.main_launches = nullptr;
-        s.last_out_keys = out_keys;
+    if (is_filter && xo.tail) {  // the timer's events are gone by the time the tail runs
+        *xo.tail = DeferredTail{true, a, out_keys};
+        xo.tail->args.ev_begin = xo.tail->args.ev_end = nullptr;
+        xo.tail->args.main_launches = nullptr;
     }
     ix->stats.bytes_scanned += scan_bytes(ix, use, a, 1);
     if (use == NK_PATH_TENSOR_SHADOW && a.image.kind == nk::RowImage::S8 && shard_s8_watch(s, stream)) return -1;
@@ -567,26 +581,25 @@ static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uin
 
 // Host-synchronous searches defer the retry / exact stages of the filter paths.  h is the shard's status words, read after
 // the stream has drained: the fatal word set -> clear it and fail (-1); a deferred filter stage overflowed (adversarial
-// near-ties, NaN rows) -> queue the tail, and the caller waits and reads again (1); else the results stand (0).  The tail is
-// queued at most once per search.
-static int shard_status(NkIndex *ix, NkShard &s, const int *h) {
-    const bool tail = s.last_filter && s.last_args.defer_tail && (h[nk::FLAG_RETRY] || h[nk::FLAG_OVERFLOW]);
-    s.last_filter = false;
+// near-ties, NaN rows) -> queue the tail, and the caller waits and reads again (1); else the results stand (0).  tail: the
+// one run_scan filled for this search, nullptr if the call ran no filter scan.  It is queued at most once per search: the
+// first look clears it.
+static int shard_status(NkIndex *ix, NkShard &s, const int *h, DeferredTail *tail) {
+    const bool queue = tail && tail->pending && (h[nk::FLAG_RETRY] || h[nk::FLAG_OVERFLOW]);
+    if (tail) tail->pending = false;
     if (h[nk::FLAG_FATAL]) return nk::fatal_overflow(h[nk::FLAG_FATAL], s.ws.flags, s.stream);
-    if (!tail) return 0;
-    NK_RANGE_PUSH("nk:retry-tail");
-    const int rc = nk::scan_tensor_filter_tail(s.di, s.last_args, s.ws, s.last_out_keys, &ix->stats.kernel_launches);
-    NK_RANGE_POP();
-    return rc ? -1 : 1;
+    if (!queue) return 0;
+    ScopedRange range("nk:retry-tail");
+    return nk::scan_tensor_filter_tail(s.di, tail->args, s.ws, tail->out_keys, &ix->stats.kernel_launches) ? -1 : 1;
 }
 
 // shard_status on the status words alone, the retry tail included: 0 or -1.
-static int finish_deferred(NkIndex *ix, NkShard &s) {
+static int finish_deferred(NkIndex *ix, NkShard &s, DeferredTail *tail) {
     for (;;) {
         int h[nk::NK_FLAG_WORDS];
         NK_CUDA_OK(cudaMemcpyAsync(h, s.ws.flags, sizeof(h), cudaMemcpyDeviceToHost, s.stream));
         NK_CUDA_OK(cudaStreamSynchronize(s.stream));
-        const int st = shard_status(ix, s, h);
+        const int st = shard_status(ix, s, h, tail);
         if (st <= 0) return st;
     }
 }
@@ -1139,28 +1152,40 @@ static const NkFilter *stage_filters(NkIndex *ix, NkShard &s, const NkFilter *fi
     return s.ws.qfilter;
 }
 
+// What one call asks of every search it runs, passed down by reference: the scan path (the index's setting, or the one a
+// graph call chose) and the per-query tag filters of its queries.
+struct SearchOpts {
+    int path;
+    const NkFilter *filters_host = nullptr;  // [Q], nullptr: none
+};
+
 // One synchronous search of Q staged queries over the live (non-empty) shards, the index lock held: scan, deferred retry
 // tail, merge; writes ke results per query into out_idx / out_score [Q x k] (row stride k) and returns ke.
-static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const StageQueries &stage, const NkFilter *filters_host,
-                       uint32_t Q, uint32_t ke, uint32_t k, uint32_t *out_idx, float *out_score) {
+static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const StageQueries &stage, const SearchOpts &opts, uint32_t Q,
+                       uint32_t ke, uint32_t k, uint32_t *out_idx, float *out_score) {
     const size_t qbytes = (size_t)Q * ix->dim * sizeof(float);
     const bool single = live.size() == 1;
+    // one deferred tail per shard; a single shard's lives on the stack, so that search allocates nothing
+    DeferredTail tail0;
+    std::vector<DeferredTail> tails(single ? 0 : live.size());
+    const auto tail_of = [&](size_t i) { return single ? &tail0 : &tails[i]; };
 
     // Launch every shard asynchronously, then collect.  A single shard writes the decoded (index, score) arrays from
     // the last kernel of its path (no separate decode launch); the retry stages of the filter paths are deferred.
-    for (NkShard *s : live) {
+    for (size_t i = 0; i < live.size(); ++i) {
+        NkShard *s = live[i];
         NK_CUDA_OK(cudaSetDevice(s->device));
         if (nk::ws_reserve((void **)&s->ws.queries, &s->ws.queries_bytes, qbytes)) return -1;
         if (nk::ws_reserve((void **)&s->ws.keys, &s->ws.keys_bytes, (size_t)Q * ke * 8)) return -1;
-        ScanOut xo;
-        xo.defer_tail = true;
+        ScanOut xo(opts.path);
+        xo.tail = tail_of(i);
         if (single) {
             if (nk::ws_reserve((void **)&s->ws.out_idx, &s->ws.out_idx_bytes, (size_t)Q * ke * 4)) return -1;
             if (nk::ws_reserve((void **)&s->ws.out_score, &s->ws.out_score_bytes, (size_t)Q * ke * 4)) return -1;
             xo.out_idx = s->ws.out_idx; xo.out_score = s->ws.out_score;
         }
         if (stage(*s)) return -1;
-        if (filters_host && !(xo.qfilter = stage_filters(ix, *s, filters_host, Q))) return -1;
+        if (opts.filters_host && !(xo.qfilter = stage_filters(ix, *s, opts.filters_host, Q))) return -1;
         if (run_scan(ix, *s, s->ws.queries, Q, ke, s->ws.keys, s->stream, xo)) return -1;
     }
 
@@ -1178,7 +1203,7 @@ static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const St
             NK_CUDA_OK(cudaMemcpyAsync(hflags, s->ws.flags, sizeof(int) * nk::NK_FLAG_WORDS, cudaMemcpyDeviceToHost, s->stream));
             NK_CUDA_OK(cudaStreamSynchronize(s->stream));
             ix->stats.bytes_d2h += (uint64_t)Q * ke * 8;
-            if ((st = shard_status(ix, *s, hflags)) < 0) return -1;
+            if ((st = shard_status(ix, *s, hflags, &tail0)) < 0) return -1;
         }
         const uint32_t *hi = reinterpret_cast<const uint32_t *>(s->h_res);
         const float *hs = reinterpret_cast<const float *>(s->h_res + rbytes);
@@ -1201,9 +1226,10 @@ static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const St
         NK_CUDA_OK(cudaSetDevice(s->device));
         if (pinned_reserve((void **)&s->h_keys, &s->h_keys_bytes, kbytes)) return -1;
     }
-    for (NkShard *s : live) {
+    for (size_t i = 0; i < live.size(); ++i) {
+        NkShard *s = live[i];
         NK_CUDA_OK(cudaSetDevice(s->device));
-        if (finish_deferred(ix, *s) < 0) return -1;  // runs this shard's retry stages if it needs them
+        if (finish_deferred(ix, *s, tail_of(i)) < 0) return -1;  // runs this shard's retry stages if it needs them
         NK_CUDA_OK(cudaMemcpyAsync(s->h_keys, s->ws.keys, kbytes, cudaMemcpyDeviceToHost, s->stream));
         ix->stats.bytes_d2h += kbytes;
     }
@@ -1239,7 +1265,7 @@ static int search_host(NkIndex *ix, const float *queries_host, const NkFilter *f
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
-    const uint64_t N = ix->mask_on ? ix->mask_alive : ix->rows();  // rows that can be returned
+    const uint64_t N = ix->returnable_rows();
     if (k == 0 || N == 0 || Q == 0) return 0;  // cuda_bridge.go:644-646, gpu.go:1540-1542
     if (!queries_host || !out_idx || !out_score) { nk::set_error("null argument"); return -1; }
     const uint32_t ke = k > N ? (uint32_t)N : k;  // cuda_bridge.go:647-649
@@ -1247,8 +1273,7 @@ static int search_host(NkIndex *ix, const float *queries_host, const NkFilter *f
     const size_t qbytes = (size_t)Q * ix->dim * sizeof(float);
     ix->stats.searches++;
     ix->stats.queries += Q;
-    NK_RANGE_PUSH("nk_search");
-    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+    ScopedRange range("nk_search");
     ShardOrder order(ix);
     if (order.failed()) return -1;
 
@@ -1258,7 +1283,7 @@ static int search_host(NkIndex *ix, const float *queries_host, const NkFilter *f
         ix->stats.bytes_h2d += qbytes;
         return 0;
     };
-    return search_live(ix, live, upload, filters_host, Q, ke, k, out_idx, out_score);
+    return search_live(ix, live, upload, SearchOpts{ix->path, filters_host}, Q, ke, k, out_idx, out_score);
 }
 
 int nk_search(NkIndex *ix, const float *queries_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
@@ -1292,7 +1317,7 @@ static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, cons
         const bool filt = admit != nullptr;
         const NkFilter f = filt ? *admit : NkFilter{0, 0, 0};
         *stage = [ix, ids, nb, local, filt, f](NkShard &s) mutable {
-            for (uint32_t q = 0; q < nb; ++q) local[q] = ids[q] - (uint32_t)(s.base - ix->row_base);
+            for (uint32_t q = 0; q < nb; ++q) local[q] = ids[q] - (uint32_t)ix->first_row(s);
             if (nk::ws_reserve((void **)&s.ws.sub_rows, &s.ws.sub_rows_bytes, (size_t)nb * 4)) return -1;
             NK_CUDA_OK(cudaMemcpyAsync(s.ws.sub_rows, local.data(), (size_t)nb * 4, cudaMemcpyHostToDevice, s.stream));
             if (nk::gather_rows(s.rows, ix->dtype, ix->dim, s.ws.sub_rows, nb, s.ws.queries, true, s.stream)) return -1;
@@ -1353,11 +1378,11 @@ static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, cons
     return 0;
 }
 
-// The body of nk_search_rows and nk_search_rows_filtered (filters_host [Q] or nullptr), the index lock held and the ids
+// The body of nk_search_rows and nk_search_rows_filtered (opts.filters_host [Q] or nullptr), the index lock held and the ids
 // checked: returns ke, the entries written per query (the rest of each k-wide output row is left as it is).
-static int search_rows_locked(NkIndex *ix, const std::vector<NkShard *> &live, const uint32_t *rows_host, const NkFilter *filters_host,
+static int search_rows_locked(NkIndex *ix, const std::vector<NkShard *> &live, const uint32_t *rows_host, const SearchOpts &opts,
                               uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
-    const uint64_t N = ix->mask_on ? ix->mask_alive : ix->rows();  // rows that can be returned
+    const uint64_t N = ix->returnable_rows();
     const uint32_t kk = (uint32_t)std::min<uint64_t>((uint64_t)k + 1, N);  // asked of the scan
     const uint32_t ke = (uint32_t)std::min<uint64_t>(k, N);                // returned
     const uint32_t QB = std::min(Q, SEARCH_ROWS_BLOCK);
@@ -1368,7 +1393,8 @@ static int search_rows_locked(NkIndex *ix, const std::vector<NkShard *> &live, c
         const uint32_t *ids = rows_host + b;
         StageQueries stage;
         if (stage_row_block(ix, live, ids, nb, nullptr, &stage)) return -1;
-        if (search_live(ix, live, stage, filters_host ? filters_host + b : nullptr, nb, kk, kk, bidx.data(), bsc.data()) < 0) return -1;
+        const SearchOpts block{opts.path, opts.filters_host ? opts.filters_host + b : nullptr};
+        if (search_live(ix, live, stage, block, nb, kk, kk, bidx.data(), bsc.data()) < 0) return -1;
         for (uint32_t q = 0; q < nb; ++q) {
             const uint32_t self = (uint32_t)(ix->row_base + ids[q]);
             const uint32_t *ri = bidx.data() + (size_t)q * kk;
@@ -1396,7 +1422,7 @@ static int search_rows_host(NkIndex *ix, const char *what, const uint32_t *rows_
     if (k > NK_MAX_K_TOTAL - 1) { nk::set_error("%s: k=%u exceeds NK_MAX_K_TOTAL - 1 = %u", what, k, NK_MAX_K_TOTAL - 1); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
     const uint64_t total = ix->rows();
-    const uint64_t N = ix->mask_on ? ix->mask_alive : total;  // rows that can be returned
+    const uint64_t N = ix->returnable_rows();
     if (k == 0 || N == 0 || Q == 0) return 0;
     for (uint32_t q = 0; q < Q; ++q)
         if (rows_host[q] >= total) {
@@ -1405,11 +1431,10 @@ static int search_rows_host(NkIndex *ix, const char *what, const uint32_t *rows_
         }
     ix->stats.searches++;
     ix->stats.queries += Q;
-    NK_RANGE_PUSH(what);
-    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+    ScopedRange range(what);
     ShardOrder order(ix);
     if (order.failed()) return -1;
-    return search_rows_locked(ix, live_shards(ix), rows_host, filters_host, Q, k, out_idx, out_score);
+    return search_rows_locked(ix, live_shards(ix), rows_host, SearchOpts{ix->path, filters_host}, Q, k, out_idx, out_score);
 }
 
 int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
@@ -1443,23 +1468,36 @@ static float range_key_threshold(const NkIndex *ix, float t) {
     return std::max(key, ix->key_floor());
 }
 
-// One shard's range scan of the Q queries staged in s.ws.queries (qfilter: their per-query filters, on the device): path,
-// scan and exact re-scoring -> counts[Q] (host), *list_cap (range_scan_shard).  from > 0 (the self-join's triangular window):
-// only rows [from, s.n) are scanned, from a multiple of the 256-row scan tile, so the window's row-mask words, TMA base and
-// 16-byte alignment are those of the shard; the window gets its own TMA maps (tc_cached_map keys on the base).  pair_first:
-// see range_scan_shard.
-// row_thr (nk_knn_graph_update's reverse scan, device [s.n]): per-row thresholds, and row_keep (device mask words) takes the
-// place of the row mask: it selects the rows whose lists are updated, not the rows that may be returned.  row_filter (a
-// filtered graph, device [s.n]) and qtags (device [Q]): a pair (row, query) is listed only if the row's filter admits the
-// query's tag; qfilter must be set then.
-static int range_shard(NkIndex *ix, NkShard &s, uint32_t Q, const NkFilter *qfilter, const uint32_t *thr, uint64_t from,
-                       const uint64_t *pair_first, int *counts, uint32_t *list_cap, const float *row_thr = nullptr,
-                       const uint32_t *row_keep = nullptr, const NkFilter *row_filter = nullptr, const uint64_t *qtags = nullptr) {
+// One block of Q range queries as every shard it runs on scans it.  The queries are those the block's StageQueries wrote into
+// s.ws.queries; with `filtered` the same step wrote their per-query tag filters into s.ws.qfilter (stage_filters,
+// stage_row_block).
+struct RangeBlock {
+    int path;                              // the scan path of the call (plan_path)
+    uint32_t Q;
+    const uint32_t *thr;                   // [Q] thresholds in key space, as nk::ord_bits (host)
+    bool filtered = false;
+    const uint64_t *pair_first = nullptr;  // the self-join's triangle: see range_scan_shard
+    // The reverse scan of a k-NN graph update.  Every row has its own threshold, s.ws.row_thr [s.n], and the mask words behind
+    // them, s.ws.row_thr + s.n, TAKE THE PLACE OF the index's row mask: they select the rows whose lists are updated, not the
+    // rows that may be returned.  row_filters (a filtered graph; `filtered` must be set too): a pair (row, query) is listed only
+    // if the row's own filter, s.ws.row_filter [s.n], admits the query's tag, s.ws.qtags [Q].
+    bool reverse = false, row_filters = false;
+};
+
+// One shard's range scan of a block, rows [from, s.n): path, scan and exact re-scoring -> counts[Q] (host), *list_cap
+// (range_scan_shard).  from > 0 (the self-join's triangular window) is a multiple of the 256-row scan tile, so the window's
+// row-mask words, TMA base and 16-byte alignment are those of the shard; the window gets its own TMA maps (tc_cached_map keys
+// on the base).
+static int range_shard(NkIndex *ix, NkShard &s, const RangeBlock &b, uint64_t from, int *counts, uint32_t *list_cap) {
     // Paths: the 16-bit and TF32 filters with fixed thresholds, or the CUDA-core scan.
-    nk::ScanArgs a = shard_scan_args(ix, s, s.ws.queries, Q, 1, s.stream, qfilter);
-    const int use = plan_path(ix, s, true, &a);
+    nk::ScanArgs a = shard_scan_args(ix, s, s.ws.queries, b.Q, 1, s.stream, b.filtered ? s.ws.qfilter : nullptr);
+    const int use = plan_path(ix, s, b.path, true, &a);
     if (use < 0) return -1;
-    if (row_thr) { a.row_thr = row_thr; a.row_mask = row_keep; a.row_filter = row_filter; a.qtags = qtags; }
+    if (b.reverse) {
+        a.row_thr = s.ws.row_thr;
+        a.row_mask = reinterpret_cast<const uint32_t *>(s.ws.row_thr + s.n);
+        if (b.row_filters) { a.row_filter = s.ws.row_filter; a.qtags = s.ws.qtags; }
+    }
     if (from) {
         a.rows = static_cast<const char *>(a.rows) + from * ix->dim * ix->esz();
         a.n = (uint32_t)(s.n - from);
@@ -1471,34 +1509,58 @@ static int range_shard(NkIndex *ix, NkShard &s, uint32_t Q, const NkFilter *qfil
     ScanTimer timer(s);
     if (timer.attach(ix, &a)) return -1;
     int retried = 0;
-    if (nk::range_scan_shard(s.di, a, use != NK_PATH_SIMT, thr, s.ws, &ix->stats.kernel_launches, counts, list_cap, &retried, pair_first))
+    if (nk::range_scan_shard(s.di, a, use != NK_PATH_SIMT, b.thr, s.ws, &ix->stats.kernel_launches, counts, list_cap, &retried, b.pair_first))
         return -1;
     timer.keep();
-    s.last_filter = false;
     ix->last_path = use;
     ix->stats.bytes_scanned += scan_bytes(ix, use, a, retried ? 2 : 1);
     return 0;
 }
 
-// After range_shard on every shard of `shards`: each query's survivors, the shards' sorted runs merged into nk_search's order
-// (keys are unique across shards), appended to *out query after query.
-static int range_collect(NkIndex *ix, const std::vector<NkShard *> &shards, uint32_t Q, const std::vector<std::vector<int>> &counts,
-                         const std::vector<uint32_t> &list_cap, std::vector<uint64_t> *out) {
+// The shards a block of range queries runs on, and what their scans leave behind for range_collect.
+struct RangeShards {
+    std::vector<NkShard *> shards;
+    std::vector<uint64_t> from;            // per shard: the first row scanned (range_shard); empty: every shard from row 0
+    std::vector<std::vector<int>> counts;  // [shard][query] survivors
+    std::vector<uint32_t> list_cap;        // per shard (range_scan_shard)
+};
+
+// Run one block of range queries over on->shards: on each, reserve the query block, stage it and scan.  *per_query [b.Q]: each
+// query's survivors, summed over the shards (all zero if there is no shard to scan; `stage` is not called then).
+static int range_scan(NkIndex *ix, RangeShards *on, const StageQueries &stage, const RangeBlock &b, std::vector<uint64_t> *per_query) {
+    on->counts.assign(on->shards.size(), std::vector<int>(b.Q, 0));
+    on->list_cap.assign(on->shards.size(), 0);
+    per_query->assign(b.Q, 0);
+    for (size_t i = 0; i < on->shards.size(); ++i) {
+        NkShard &s = *on->shards[i];
+        NK_CUDA_OK(cudaSetDevice(s.device));
+        if (nk::ws_reserve((void **)&s.ws.queries, &s.ws.queries_bytes, (size_t)b.Q * ix->dim * sizeof(float))) return -1;
+        if (stage(s)) return -1;
+        if (range_shard(ix, s, b, on->from.empty() ? 0 : on->from[i], on->counts[i].data(), &on->list_cap[i])) return -1;
+        for (uint32_t q = 0; q < b.Q; ++q) (*per_query)[q] += (uint64_t)on->counts[i][q];
+    }
+    return 0;
+}
+
+// After range_scan: each of the Q queries' survivors, the shards' sorted runs merged into nk_search's order (keys are unique
+// across shards), appended to *out query after query.
+static int range_collect(NkIndex *ix, const RangeShards &on, uint32_t Q, std::vector<uint64_t> *out) {
+    const std::vector<NkShard *> &shards = on.shards;
     std::vector<std::vector<uint64_t>> keys(shards.size());
     std::vector<std::vector<uint64_t>> offs(shards.size(), std::vector<uint64_t>(Q + 1, 0));
     for (size_t i = 0; i < shards.size(); ++i) {
         NK_CUDA_OK(cudaSetDevice(shards[i]->device));
-        if (nk::range_sorted_keys(shards[i]->di, shards[i]->ws, shards[i]->stream, Q, counts[i].data(), list_cap[i], &keys[i],
+        if (nk::range_sorted_keys(shards[i]->di, shards[i]->ws, shards[i]->stream, Q, on.counts[i].data(), on.list_cap[i], &keys[i],
                                   &ix->stats.kernel_launches))
             return -1;
         ix->stats.bytes_d2h += keys[i].size() * 8;
-        for (uint32_t q = 0; q < Q; ++q) offs[i][q + 1] = offs[i][q] + (uint64_t)counts[i][q];
+        for (uint32_t q = 0; q < Q; ++q) offs[i][q + 1] = offs[i][q] + (uint64_t)on.counts[i][q];
     }
     std::vector<uint64_t> merged, tmp;
     for (uint32_t q = 0; q < Q; ++q) {
         merged.clear();
         for (size_t i = 0; i < shards.size(); ++i) {
-            tmp.resize(merged.size() + (size_t)counts[i][q]);
+            tmp.resize(merged.size() + (size_t)on.counts[i][q]);
             std::merge(merged.begin(), merged.end(), keys[i].begin() + offs[i][q], keys[i].begin() + offs[i][q + 1], tmp.begin(),
                        std::greater<uint64_t>());
             merged.swap(tmp);
@@ -1525,36 +1587,28 @@ int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresho
     }
     ix->stats.searches++;
     ix->stats.queries += Q;
-    NK_RANGE_PUSH("nk_search_range");
-    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+    ScopedRange range("nk_search_range");
     ShardOrder order(ix);
     if (order.failed()) return -1;
-    const std::vector<NkShard *> live = live_shards(ix);
+    RangeShards on{live_shards(ix)};
     const size_t qbytes = (size_t)Q * ix->dim * sizeof(float);
-    std::vector<std::vector<int>> counts(live.size(), std::vector<int>(Q, 0));
-    std::vector<uint32_t> list_cap(live.size());
-    for (size_t i = 0; i < live.size(); ++i) {
-        NkShard &s = *live[i];
-        NK_CUDA_OK(cudaSetDevice(s.device));
-        if (nk::ws_reserve((void **)&s.ws.queries, &s.ws.queries_bytes, qbytes)) return -1;
+    const StageQueries upload = [&](NkShard &s) {
         NK_CUDA_OK(cudaMemcpyAsync(s.ws.queries, queries_host, qbytes, cudaMemcpyHostToDevice, s.stream));
         ix->stats.bytes_h2d += qbytes;
-        const NkFilter *qfilter = nullptr;
-        if (filters_host && !(qfilter = stage_filters(ix, s, filters_host, Q))) return -1;
-        if (range_shard(ix, s, Q, qfilter, thr.data(), 0, nullptr, counts[i].data(), &list_cap[i])) return -1;
-    }
+        return filters_host && !stage_filters(ix, s, filters_host, Q) ? -1 : 0;
+    };
+    RangeBlock block{ix->path, Q, thr.data()};
+    block.filtered = filters_host != nullptr;
+    std::vector<uint64_t> per_query;
+    if (range_scan(ix, &on, upload, block, &per_query)) return -1;
     // offsets: the shards' survivors of query q are merged into one run
-    for (uint32_t q = 0; q < Q; ++q) {
-        uint64_t c = 0;
-        for (size_t i = 0; i < live.size(); ++i) c += (uint64_t)counts[i][q];
-        out_offsets[q + 1] = out_offsets[q] + c;
-    }
+    for (uint32_t q = 0; q < Q; ++q) out_offsets[q + 1] = out_offsets[q] + per_query[q];
     *out_total = out_offsets[Q];
     if (*out_total > capacity || *out_total == 0) return 0;
     if (!out_idx || !out_score) { nk::set_error("null argument"); return -1; }
     std::vector<uint64_t> keys;
     keys.reserve(*out_total);
-    if (range_collect(ix, live, Q, counts, list_cap, &keys)) return -1;
+    if (range_collect(ix, on, Q, &keys)) return -1;
     for (size_t j = 0; j < keys.size(); ++j) decode_key(ix->metric, keys[j], out_idx + j, out_score + j);
     return 0;
 }
@@ -1590,8 +1644,7 @@ int nk_search_pairs(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float thre
     if (n_rows == 0) return 0;
     ix->stats.searches++;
     ix->stats.queries += n_rows;
-    NK_RANGE_PUSH("nk_search_pairs");
-    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+    ScopedRange range("nk_search_pairs");
     ShardOrder order(ix);
     if (order.failed()) return -1;
 
@@ -1602,39 +1655,27 @@ int nk_search_pairs(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float thre
     const std::vector<uint32_t> thr(QB, nk::ord_bits(range_key_threshold(ix, threshold)));
     std::vector<uint32_t> ids(QB);
     std::vector<uint64_t> keys;  // the result so far, [out_offsets[0], out_offsets[b])
+    std::vector<uint64_t> per_query;
     for (uint64_t b = 0; b < n_rows; b += QB) {
         const uint32_t nb = (uint32_t)std::min<uint64_t>(QB, n_rows - b);
         const uint64_t s0 = first_row + b;  // the block's first row, relative to the index's first row
         for (uint32_t q = 0; q < nb; ++q) ids[q] = (uint32_t)(s0 + q);
-        std::vector<NkShard *> scan;
-        std::vector<uint64_t> from;
+        RangeShards scan;
         for (NkShard *s : live) {
-            const uint64_t lo = s->base - ix->row_base;
+            const uint64_t lo = ix->first_row(*s);
             if (lo + s->n <= s0 + 1) continue;  // every row at or below s0
-            scan.push_back(s);
-            from.push_back(lo <= s0 ? (s0 - lo) / SCAN_TILE_ROWS * SCAN_TILE_ROWS : 0);
+            scan.shards.push_back(s);
+            scan.from.push_back(lo <= s0 ? (s0 - lo) / SCAN_TILE_ROWS * SCAN_TILE_ROWS : 0);
         }
-        std::vector<std::vector<int>> counts(scan.size(), std::vector<int>(nb, 0));
-        std::vector<uint32_t> list_cap(scan.size());
-        if (!scan.empty()) {
-            StageQueries stage;
-            if (stage_row_block(ix, live, ids.data(), nb, admit ? &f : nullptr, &stage)) return -1;
-            const uint64_t pair_first = ix->row_base + s0;
-            for (size_t i = 0; i < scan.size(); ++i) {
-                NkShard &s = *scan[i];
-                NK_CUDA_OK(cudaSetDevice(s.device));
-                if (nk::ws_reserve((void **)&s.ws.queries, &s.ws.queries_bytes, (size_t)nb * ix->dim * sizeof(float))) return -1;
-                if (stage(s)) return -1;
-                if (range_shard(ix, s, nb, admit ? s.ws.qfilter : nullptr, thr.data(), from[i], &pair_first, counts[i].data(), &list_cap[i]))
-                    return -1;
-            }
-        }
-        for (uint32_t q = 0; q < nb; ++q) {
-            uint64_t c = 0;
-            for (size_t i = 0; i < scan.size(); ++i) c += (uint64_t)counts[i][q];
-            out_offsets[b + q + 1] = out_offsets[b + q] + c;
-        }
-        if (out_offsets[b + nb] > keys.size() && range_collect(ix, scan, nb, counts, list_cap, &keys)) return -1;
+        StageQueries stage;
+        if (!scan.shards.empty() && stage_row_block(ix, live, ids.data(), nb, admit ? &f : nullptr, &stage)) return -1;
+        const uint64_t pair_first = ix->row_base + s0;
+        RangeBlock block{ix->path, nb, thr.data()};
+        block.filtered = admit;
+        block.pair_first = &pair_first;
+        if (range_scan(ix, &scan, stage, block, &per_query)) return -1;
+        for (uint32_t q = 0; q < nb; ++q) out_offsets[b + q + 1] = out_offsets[b + q] + per_query[q];
+        if (out_offsets[b + nb] > keys.size() && range_collect(ix, scan, nb, &keys)) return -1;
     }
     *out_total = out_offsets[n_rows];
     if (*out_total > capacity || *out_total == 0) return 0;
@@ -1661,7 +1702,7 @@ static int admissible_rows(NkIndex *ix, std::vector<uint8_t> *ok) {
     if (!ix->mask_on) return 0;
     for (auto &s : ix->shards) {
         if (s.n == 0 || !s.mask_on) continue;
-        const uint64_t lo = s.base - ix->row_base;
+        const uint64_t lo = ix->first_row(s);
         std::vector<uint32_t> w((s.n + 31) / 32);
         NK_CUDA_OK(cudaSetDevice(s.device));
         NK_CUDA_OK(cudaMemcpyAsync(w.data(), s.mask, w.size() * 4, cudaMemcpyDeviceToHost, s.stream));
@@ -1677,7 +1718,7 @@ static int host_row_tags(NkIndex *ix, std::vector<uint64_t> *tags) {
     for (auto &s : ix->shards) {
         if (s.n == 0 || !s.tags_on) continue;
         NK_CUDA_OK(cudaSetDevice(s.device));
-        NK_CUDA_OK(cudaMemcpyAsync(tags->data() + (s.base - ix->row_base), s.tags, s.n * 8, cudaMemcpyDeviceToHost, s.stream));
+        NK_CUDA_OK(cudaMemcpyAsync(tags->data() + ix->first_row(s), s.tags, s.n * 8, cudaMemcpyDeviceToHost, s.stream));
         NK_CUDA_OK(cudaStreamSynchronize(s.stream));
         ix->stats.bytes_d2h += s.n * 8;
     }
@@ -1725,7 +1766,7 @@ static int graph_pair_keys_on(NkIndex *ix, const std::vector<NkShard *> &live, N
         if (n == 0) continue;
         arg.resize(3 * n);
         for (size_t i = 0; i < n; ++i) {
-            arg[i] = pr[idx[i]] - (uint32_t)(s.base - ix->row_base);
+            arg[i] = pr[idx[i]] - (uint32_t)ix->first_row(s);
             arg[n + i] = (uint32_t)(std::lower_bound(js.begin() + b, js.begin() + b + nb, pj[idx[i]]) - (js.begin() + b));
             arg[2 * n + i] = (uint32_t)(ix->row_base + pj[idx[i]]);
         }
@@ -1747,80 +1788,83 @@ static int graph_pair_keys_on(NkIndex *ix, const std::vector<NkShard *> &live, N
     return 0;
 }
 
-// The body of nk_knn_graph_remap and nk_knn_graph_update, the index lock held and the caller's own arguments checked (src
-// is non-null if the index has rows).  gi_in / gs_in [n_old x k] is the old graph, gi / gs [N x k] the output; they are one
+// One nk_knn_graph_remap / nk_knn_graph_update call, the index lock held and the caller's own arguments checked (src is
+// non-null if the index has rows).  gi_in / gs_in [n_old x k] is the old graph, gi / gs [N x k] the output; they are one
 // array only when every old row that is still named keeps its id (nk_knn_graph_update): each row's old list is read before
-// that row is written.  by_id: *n_lists_changed counts every row f < n_old whose list differs from old row f's, else only the
-// kept rows'.  filters [N] (nullptr: none): the graph of nk_search_rows_filtered, each row's list bounded by its own filter.
-// A kept row has the tag and the filter it had when the graph was built (the caller reports any other row as new), so the
-// rows searched again are the same; they are searched with their own filters, and the reverse scan also holds each pair
-// (r, c) to r's filter admitting c's tag.  Returns ke, or -1 with nothing written.
-static int knn_graph_remap_locked(NkIndex *ix, const char *what, uint32_t k, uint64_t n_old, const uint32_t *src, const NkFilter *filters,
-                                  const uint32_t *gi_in, const float *gs_in, uint32_t *gi, float *gs, bool by_id,
-                                  uint64_t *n_lists_changed) {
-    if (k == 0 || k > NK_GRAPH_MAX_K) { nk::set_error("%s: k=%u outside [1, %u]", what, k, NK_GRAPH_MAX_K); return -1; }
-    if (ix->path == NK_PATH_SIMT || ix->path == NK_PATH_TENSOR) {
-        nk::set_error("%s: the graph is kept on the filter paths (AUTO, TENSOR_FILTER or TENSOR_SHADOW), not path %d", what, ix->path);
-        return -1;
+// that row is written.  by_id: the lists counted as changed are those of every row f < n_old whose list differs from old row
+// f's, else only the kept rows'.  filters [N] (nullptr: none): the graph of nk_search_rows_filtered, each row's list bounded by
+// its own filter.  A kept row has the tag and the filter it had when the graph was built (the caller reports any other row as
+// new), so the rows searched again are the same; they are searched with their own filters, and the reverse scan also holds
+// each pair (r, c) to r's filter admitting c's tag.
+struct GraphCall {
+    const char *what;
+    uint32_t k;
+    uint64_t n_old;
+    const uint32_t *src;
+    const NkFilter *filters;
+    const uint32_t *gi_in; const float *gs_in;
+    uint32_t *gi; float *gs;
+    bool by_id;
+    uint64_t changed = 0;  // lists written that differ from the old graph's (by_id)
+    void write_list(uint64_t r, const uint32_t *li, const float *ls) {
+        if (r < n_old && (by_id || src[r] == r) && (memcmp(gi_in + r * k, li, (size_t)k * 4) || memcmp(gs_in + r * k, ls, (size_t)k * 4)))
+            ++changed;
+        memcpy(gi + r * k, li, (size_t)k * 4);
+        memcpy(gs + r * k, ls, (size_t)k * 4);
     }
-    const uint64_t N = ix->rows();
-    std::vector<uint32_t> now_at(n_old, NK_ROW_NEW);  // the current id of old row o, NK_ROW_NEW once it is gone
-    for (uint64_t f = 0; f < N; ++f) {
-        const uint32_t o = src[f];
-        if (o == NK_ROW_NEW) continue;
-        if (o >= n_old) {
-            nk::set_error("%s: src_of_row[%llu] = %u is not an old row (n_old=%llu)", what, (unsigned long long)f, o, (unsigned long long)n_old);
-            return -1;
-        }
-        if (now_at[o] != NK_ROW_NEW) {
-            nk::set_error("%s: old row %u is the source of rows %u and %llu", what, o, now_at[o], (unsigned long long)f);
-            return -1;
-        }
-        now_at[o] = (uint32_t)f;
-    }
-    for (uint64_t i = 0; i < n_old * k; ++i)
-        if (gi_in[i] != GRAPH_PAD && (gi_in[i] < ix->row_base || gi_in[i] - ix->row_base >= n_old)) {
-            nk::set_error("%s: entry %llu of the graph (row %u) is not an old row", what, (unsigned long long)i, gi_in[i]);
-            return -1;
-        }
-    const std::vector<NkShard *> live = live_shards(ix);
-    // the graph path: the forced one, or under AUTO the 16-bit pass where every live shard has a 16-bit image, else the TF32 filter
-    int gpath = ix->path;
-    if (gpath == NK_PATH_AUTO) {
-        gpath = NK_PATH_TENSOR_SHADOW;
-        for (NkShard *s : live)
-            if (!s->img.current(s->n)) gpath = NK_PATH_TENSOR_FILTER;
-    }
-    struct PathGuard {
-        NkIndex *ix; int saved;
-        ~PathGuard() { ix->path = saved; }
-    } path_guard{ix, ix->path};
-    ix->path = gpath;
-    for (NkShard *s : live) {
-        nk::ScanArgs a = shard_scan_args(ix, *s, nullptr, SEARCH_ROWS_BLOCK, k + 1, s->stream);
-        if (plan_path(ix, *s, false, &a) < 0) return -1;  // the error names the path and the shape
-    }
-    if (n_lists_changed) *n_lists_changed = 0;
-    ix->stats.searches++;
-    NK_RANGE_PUSH(what);
-    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
-    ShardOrder order(ix);
-    if (order.failed()) return -1;
-    if (gi != gi_in)  // kept rows start from their old lists
-        for (uint64_t f = 0; f < N; ++f)
-            if (src[f] == f) {
-                memcpy(gi + f * k, gi_in + f * k, (size_t)k * 4);
-                memcpy(gs + f * k, gs_in + f * k, (size_t)k * 4);
-            }
+};
 
-    // the rows to search again (R) and the queries of the reverse scan (C: new and moved rows)
-    std::vector<uint8_t> in_r(N, 0);
-    std::vector<uint32_t> C;
-    for (uint64_t f = 0; f < N; ++f)
-        if (src[f] != f) { in_r[f] = 1; C.push_back((uint32_t)f); }
-    const uint64_t adm = ix->mask_on ? ix->mask_alive : N;
-    const int ke = (int)std::min<uint64_t>(k, adm);
-    if (C.empty() && N == n_old) return ke;  // every row kept at its id
+// Is row r's old list that of a NaN row (every score -inf, decoded)?
+static bool graph_nan_list(const NkIndex *ix, const uint32_t *li, const float *ls) {
+    return li[0] != GRAPH_PAD && ls[0] == (ix->metric == NK_METRIC_EUCLIDEAN ? INFINITY : -INFINITY);
+}
+
+// Check src and the old graph's entries -> now_at [n_old]: the current id of old row o, NK_ROW_NEW once it is gone.
+static int graph_check(const NkIndex *ix, const GraphCall &g, std::vector<uint32_t> *now_at) {
+    const uint64_t N = ix->rows();
+    now_at->assign(g.n_old, NK_ROW_NEW);
+    for (uint64_t f = 0; f < N; ++f) {
+        const uint32_t o = g.src[f];
+        if (o == NK_ROW_NEW) continue;
+        if (o >= g.n_old) {
+            nk::set_error("%s: src_of_row[%llu] = %u is not an old row (n_old=%llu)", g.what, (unsigned long long)f, o,
+                          (unsigned long long)g.n_old);
+            return -1;
+        }
+        if ((*now_at)[o] != NK_ROW_NEW) {
+            nk::set_error("%s: old row %u is the source of rows %u and %llu", g.what, o, (*now_at)[o], (unsigned long long)f);
+            return -1;
+        }
+        (*now_at)[o] = (uint32_t)f;
+    }
+    for (uint64_t i = 0; i < g.n_old * g.k; ++i)
+        if (g.gi_in[i] != GRAPH_PAD && (g.gi_in[i] < ix->row_base || g.gi_in[i] - ix->row_base >= g.n_old)) {
+            nk::set_error("%s: entry %llu of the graph (row %u) is not an old row", g.what, (unsigned long long)i, g.gi_in[i]);
+            return -1;
+        }
+    return 0;
+}
+
+// The graph path: the forced one, or under AUTO the 16-bit pass where every live shard has a 16-bit image, else the TF32
+// filter; -1 if a live shard cannot serve it at the shape of the graph's searches (the error names the path and the shape).
+static int graph_path(const NkIndex *ix, const GraphCall &g, const std::vector<NkShard *> &live) {
+    int path = ix->path;
+    if (path == NK_PATH_AUTO) {
+        path = NK_PATH_TENSOR_SHADOW;
+        for (NkShard *s : live)
+            if (!s->img.current(s->n)) path = NK_PATH_TENSOR_FILTER;
+    }
+    for (NkShard *s : live) {
+        nk::ScanArgs a = shard_scan_args(ix, *s, nullptr, SEARCH_ROWS_BLOCK, g.k + 1, s->stream);
+        if (plan_path(ix, *s, path, false, &a) < 0) return -1;
+    }
+    return path;
+}
+
+// The rows to search again, R: in_r [N] comes in with the new and moved rows set and leaves with every row of R set.
+static int graph_rows_searched_again(NkIndex *ix, const GraphCall &g, const std::vector<uint32_t> &now_at, std::vector<uint8_t> *in_r) {
+    const uint64_t N = ix->rows();
+    const uint32_t k = g.k;
     // nk_search_rows treats a row specially while no more than k rows are admissible (its list drops one of them when the row
     // itself is not admissible): then every row is searched again.  Gone rows have no mask bit any more, so whether that held
     // when the graph was built is bounded: then every old list was short, and no more than k of the old rows still present
@@ -1829,259 +1873,313 @@ static int knn_graph_remap_locked(NkIndex *ix, const char *what, uint32_t k, uin
     // such rows the last slot a row drops is the (k+1)-th of its filtered order, and a list shorter than k holds every other
     // row its filter and the floor admit — its threshold is the floor, as for an unfiltered short list.  A list that is
     // full implies more than k rows passing the mask, filtered or not.
-    bool all = adm <= k;
+    bool all = ix->returnable_rows() <= k;
     if (!all) {
         bool full = false;
-        for (uint64_t o = 0; o < n_old && !full; ++o) full = gi_in[o * k + k - 1] != GRAPH_PAD;
+        for (uint64_t o = 0; o < g.n_old && !full; ++o) full = g.gi_in[o * k + k - 1] != GRAPH_PAD;
         if (!full) {
             std::vector<uint8_t> ok;
             if (admissible_rows(ix, &ok)) return -1;
             uint64_t still = 0;
-            for (uint64_t f = 0; f < N; ++f) still += src[f] != NK_ROW_NEW && ok[f];
+            for (uint64_t f = 0; f < N; ++f) still += g.src[f] != NK_ROW_NEW && ok[f];
             all = still <= k;
         }
     }
-    // A NaN row's list (every score -inf, decoded) comes from the exact stage its search block falls through to: its keys are
-    // that stage's, not warp_exact_score's, so such a row is searched again rather than merged.
-    const float nan_score = ix->metric == NK_METRIC_EUCLIDEAN ? INFINITY : -INFINITY;
     for (uint64_t r = 0; r < N; ++r) {
-        if (in_r[r]) continue;  // r is kept from here on: r < n_old
-        if (all || (gi_in[r * k] != GRAPH_PAD && gs_in[r * k] == nan_score)) { in_r[r] = 1; continue; }
+        if ((*in_r)[r]) continue;  // r is kept from here on: r < n_old
+        // A NaN row's list (every score -inf, decoded) comes from the exact stage its search block falls through to: its keys
+        // are that stage's, not warp_exact_score's, so such a row is searched again rather than merged.
+        if (all || graph_nan_list(ix, g.gi_in + r * k, g.gs_in + r * k)) { (*in_r)[r] = 1; continue; }
         for (uint32_t j = 0; j < k; ++j) {
-            const uint32_t e = gi_in[r * k + j];
-            if (e != GRAPH_PAD && now_at[e - ix->row_base] != e - ix->row_base) { in_r[r] = 1; break; }
+            const uint32_t e = g.gi_in[r * k + j];
+            if (e != GRAPH_PAD && now_at[e - ix->row_base] != e - ix->row_base) { (*in_r)[r] = 1; break; }
         }
     }
-    uint64_t n_changed_lists = 0;
-    auto write_list = [&](uint64_t r, const uint32_t *li, const float *ls) {
-        if (r < n_old && (by_id || src[r] == r) && (memcmp(gi_in + r * k, li, (size_t)k * 4) || memcmp(gs_in + r * k, ls, (size_t)k * 4)))
-            ++n_changed_lists;
-        memcpy(gi + r * k, li, (size_t)k * 4);
-        memcpy(gs + r * k, ls, (size_t)k * 4);
-    };
+    return 0;
+}
 
-    // reverse scan + merge for the kept rows outside R
-    bool reverse = false;
-    for (uint64_t r = 0; r < N && !reverse; ++r) reverse = !in_r[r];
-    if (reverse) {
-        for (NkShard *s : live) {  // per-row thresholds and the mask of rows outside R
-            const uint64_t lo = s->base - ix->row_base, words = (s->n + 31) / 32;
-            std::vector<float> thr(s->n + words);
-            uint32_t *keep = reinterpret_cast<uint32_t *>(thr.data() + s->n);
-            for (uint64_t w = 0; w < words; ++w) keep[w] = 0u;
-            for (uint64_t l = 0; l < s->n; ++l) {
-                const uint64_t r = lo + l;
-                thr[l] = INFINITY;
-                if (in_r[r]) continue;
-                keep[l >> 5] |= 1u << (l & 31);
-                thr[l] = gi_in[r * k + k - 1] != GRAPH_PAD ? range_key_threshold(ix, gs_in[r * k + k - 1]) : ix->key_floor();
-            }
-            NK_CUDA_OK(cudaSetDevice(s->device));
-            if (nk::ws_reserve((void **)&s->ws.row_thr, &s->ws.row_thr_bytes, thr.size() * 4)) return -1;
-            NK_CUDA_OK(cudaMemcpyAsync(s->ws.row_thr, thr.data(), thr.size() * 4, cudaMemcpyHostToDevice, s->stream));
-            if (filters) {  // each row's own filter, for the row side of the scan
-                if (nk::ws_reserve((void **)&s->ws.row_filter, &s->ws.row_filter_bytes, s->n * sizeof(NkFilter))) return -1;
-                NK_CUDA_OK(cudaMemcpyAsync(s->ws.row_filter, filters + lo, s->n * sizeof(NkFilter), cudaMemcpyHostToDevice, s->stream));
-                ix->stats.bytes_h2d += s->n * sizeof(NkFilter);
-            }
-            NK_CUDA_OK(cudaStreamSynchronize(s->stream));  // thr is pageable and goes out of scope
-            ix->stats.bytes_h2d += thr.size() * 4;
+// Before the reverse scan: every live shard gets its per-row thresholds and, behind them, the mask of the rows outside R
+// (s.ws.row_thr), and with filters each row's own filter for the row side of the scan (s.ws.row_filter).
+static int graph_upload_row_thresholds(NkIndex *ix, const GraphCall &g, const std::vector<NkShard *> &live, const std::vector<uint8_t> &in_r) {
+    const uint32_t k = g.k;
+    for (NkShard *s : live) {
+        const uint64_t lo = ix->first_row(*s), words = (s->n + 31) / 32;
+        std::vector<float> thr(s->n + words);
+        uint32_t *keep = reinterpret_cast<uint32_t *>(thr.data() + s->n);
+        for (uint64_t w = 0; w < words; ++w) keep[w] = 0u;
+        for (uint64_t l = 0; l < s->n; ++l) {
+            const uint64_t r = lo + l;
+            thr[l] = INFINITY;
+            if (in_r[r]) continue;
+            keep[l >> 5] |= 1u << (l & 31);
+            thr[l] = g.gi_in[r * k + k - 1] != GRAPH_PAD ? range_key_threshold(ix, g.gs_in[r * k + k - 1]) : ix->key_floor();
         }
-        // a filtered graph's queries also carry their tags, and always a per-query filter (the row-filtered scan is a mode
-        // of the tag-filtered one)
-        std::vector<uint64_t> tags, qtags;
-        if (filters && host_row_tags(ix, &tags)) return -1;
-        const bool qfilt = ix->mask_on || filters;
-        const NkFilter all_rows{0, 0, 0};  // masked-out queries get the filter that admits no row (stage_row_block)
-        const uint32_t QB = (uint32_t)std::min<size_t>(C.size(), SEARCH_ROWS_BLOCK);
-        const std::vector<uint32_t> floor_thr(QB, nk::ord_bits(ix->key_floor()));
-        std::vector<std::pair<uint32_t, uint64_t>> entrants;  // (kept row r, key of the new or moved row in r's list)
-        std::vector<uint64_t> keys;
-        for (size_t b = 0; b < C.size(); b += QB) {
-            const uint32_t nb = (uint32_t)std::min<size_t>(QB, C.size() - b);
-            StageQueries stage;
-            if (stage_row_block(ix, live, C.data() + b, nb, qfilt ? &all_rows : nullptr, &stage)) return -1;
-            if (filters) {
-                qtags.resize(nb);
-                for (uint32_t q = 0; q < nb; ++q) qtags[q] = tags[C[b + q]];
-            }
-            std::vector<std::vector<int>> counts(live.size(), std::vector<int>(nb, 0));
-            std::vector<uint32_t> list_cap(live.size());
-            for (size_t i = 0; i < live.size(); ++i) {
-                NkShard &s = *live[i];
-                NK_CUDA_OK(cudaSetDevice(s.device));
-                if (nk::ws_reserve((void **)&s.ws.queries, &s.ws.queries_bytes, (size_t)nb * ix->dim * sizeof(float))) return -1;
-                if (stage(s)) return -1;
-                if (filters) {  // read by the scan before range_shard's first synchronisation
-                    if (nk::ws_reserve((void **)&s.ws.qtags, &s.ws.qtags_bytes, (size_t)nb * 8)) return -1;
-                    NK_CUDA_OK(cudaMemcpyAsync(s.ws.qtags, qtags.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, s.stream));
-                    ix->stats.bytes_h2d += (uint64_t)nb * 8;
-                }
-                if (range_shard(ix, s, nb, qfilt ? s.ws.qfilter : nullptr, floor_thr.data(), 0, nullptr, counts[i].data(), &list_cap[i],
-                                s.ws.row_thr, reinterpret_cast<const uint32_t *>(s.ws.row_thr + s.n), filters ? s.ws.row_filter : nullptr,
-                                filters ? s.ws.qtags : nullptr))
-                    return -1;
-            }
-            keys.clear();
-            if (range_collect(ix, live, nb, counts, list_cap, &keys)) return -1;
-            size_t at = 0;
-            for (uint32_t q = 0; q < nb; ++q) {
-                uint64_t c = 0;
-                for (size_t i = 0; i < live.size(); ++i) c += (uint64_t)counts[i][q];
-                const uint64_t qrow = 0xffffffffull - (ix->row_base + C[b + q]);
-                for (uint64_t j = 0; j < c; ++j, ++at)
-                    entrants.emplace_back((uint32_t)(nk::key_row(keys[at]) - ix->row_base), (keys[at] & 0xffffffff00000000ull) | qrow);
-            }
+        NK_CUDA_OK(cudaSetDevice(s->device));
+        if (nk::ws_reserve((void **)&s->ws.row_thr, &s->ws.row_thr_bytes, thr.size() * 4)) return -1;
+        NK_CUDA_OK(cudaMemcpyAsync(s->ws.row_thr, thr.data(), thr.size() * 4, cudaMemcpyHostToDevice, s->stream));
+        if (g.filters) {
+            if (nk::ws_reserve((void **)&s->ws.row_filter, &s->ws.row_filter_bytes, s->n * sizeof(NkFilter))) return -1;
+            NK_CUDA_OK(cudaMemcpyAsync(s->ws.row_filter, g.filters + lo, s->n * sizeof(NkFilter), cudaMemcpyHostToDevice, s->stream));
+            ix->stats.bytes_h2d += s->n * sizeof(NkFilter);
         }
-        std::sort(entrants.begin(), entrants.end());
-        // keys of the touched rows' old entries, per shard of the row
-        std::vector<std::vector<uint64_t>> okeys(live.size());
-        std::vector<std::vector<uint32_t>> opr(live.size()), opj(live.size());
-        std::vector<uint32_t> touched;
-        for (size_t i = 0; i < entrants.size(); ++i)
-            if (i == 0 || entrants[i].first != entrants[i - 1].first) touched.push_back(entrants[i].first);
-        std::vector<size_t> shard_of(touched.size());
-        for (size_t t = 0; t < touched.size(); ++t) {
-            const uint32_t r = touched[t];
-            for (size_t i = 0; i < live.size(); ++i)
-                if (r >= live[i]->base - ix->row_base && r < live[i]->base - ix->row_base + live[i]->n) shard_of[t] = i;
-            for (uint32_t j = 0; j < k; ++j) {
-                const uint32_t e = gi_in[(uint64_t)r * k + j];
-                if (e == GRAPH_PAD) break;
-                opr[shard_of[t]].push_back(r);
-                opj[shard_of[t]].push_back((uint32_t)(e - ix->row_base));
-            }
+        NK_CUDA_OK(cudaStreamSynchronize(s->stream));  // thr is pageable and goes out of scope
+        ix->stats.bytes_h2d += thr.size() * 4;
+    }
+    return 0;
+}
+
+// The reverse scan for the kept rows outside R: the new and moved rows C, in blocks, are range queries over every live shard
+// with each row's own threshold -> *entrants, sorted: (kept row r, key of the new or moved row in r's list).
+using GraphEntrants = std::vector<std::pair<uint32_t, uint64_t>>;
+static int graph_reverse_scan(NkIndex *ix, const GraphCall &g, const std::vector<NkShard *> &live, int path, const std::vector<uint8_t> &in_r,
+                              const std::vector<uint32_t> &C, GraphEntrants *entrants) {
+    if (graph_upload_row_thresholds(ix, g, live, in_r)) return -1;
+    // a filtered graph's queries also carry their tags, and always a per-query filter (the row-filtered scan is a mode
+    // of the tag-filtered one)
+    std::vector<uint64_t> tags, qtags;
+    if (g.filters && host_row_tags(ix, &tags)) return -1;
+    const NkFilter all_rows{0, 0, 0};  // masked-out queries get the filter that admits no row (stage_row_block)
+    const uint32_t QB = (uint32_t)std::min<size_t>(C.size(), SEARCH_ROWS_BLOCK);
+    const std::vector<uint32_t> floor_thr(QB, nk::ord_bits(ix->key_floor()));
+    RangeBlock block{path, 0, floor_thr.data()};
+    block.filtered = ix->mask_on || g.filters;
+    block.reverse = true;
+    block.row_filters = g.filters != nullptr;
+    RangeShards on{live};
+    std::vector<uint64_t> keys, per_query;
+    for (size_t b = 0; b < C.size(); b += QB) {
+        const uint32_t nb = block.Q = (uint32_t)std::min<size_t>(QB, C.size() - b);
+        StageQueries stage_rows;
+        if (stage_row_block(ix, live, C.data() + b, nb, block.filtered ? &all_rows : nullptr, &stage_rows)) return -1;
+        if (g.filters) {
+            qtags.resize(nb);
+            for (uint32_t q = 0; q < nb; ++q) qtags[q] = tags[C[b + q]];
         }
-        for (size_t i = 0; i < live.size(); ++i)
-            if (!opr[i].empty() && graph_pair_keys_on(ix, live, *live[i], opr[i], opj[i], &okeys[i])) return -1;
-        // merge: each touched row's old entries and entrants in key space, the best k kept
-        std::vector<size_t> opos(live.size(), 0);
-        std::vector<uint64_t> cand;
-        std::vector<uint32_t> li(k);
-        std::vector<float> ls(k);
-        size_t e0 = 0;
-        for (size_t t = 0; t < touched.size(); ++t) {
-            const uint32_t r = touched[t];
-            cand.clear();
-            const size_t si = shard_of[t];
-            while (opos[si] < opr[si].size() && opr[si][opos[si]] == r) cand.push_back(okeys[si][opos[si]++]);
-            for (; e0 < entrants.size() && entrants[e0].first == r; ++e0) cand.push_back(entrants[e0].second);
-            const size_t take = std::min<size_t>(k, cand.size());
-            std::partial_sort(cand.begin(), cand.begin() + take, cand.end(), std::greater<uint64_t>());
-            for (uint32_t j = 0; j < k; ++j) {
-                if (j < take) decode_key(ix->metric, cand[j], &li[j], &ls[j]);
-                else { li[j] = GRAPH_PAD; ls[j] = 0.0f; }
-            }
-            write_list(r, li.data(), ls.data());
+        const StageQueries stage = [&](NkShard &s) {
+            if (stage_rows(s)) return -1;
+            if (!g.filters) return 0;
+            // the queries' tags: read by the scan before range_shard's first synchronisation
+            if (nk::ws_reserve((void **)&s.ws.qtags, &s.ws.qtags_bytes, (size_t)nb * 8)) return -1;
+            NK_CUDA_OK(cudaMemcpyAsync(s.ws.qtags, qtags.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, s.stream));
+            ix->stats.bytes_h2d += (uint64_t)nb * 8;
+            return 0;
+        };
+        if (range_scan(ix, &on, stage, block, &per_query)) return -1;
+        keys.clear();
+        if (range_collect(ix, on, nb, &keys)) return -1;
+        size_t at = 0;
+        for (uint32_t q = 0; q < nb; ++q) {
+            const uint64_t qrow = 0xffffffffull - (ix->row_base + C[b + q]);
+            for (uint64_t j = 0; j < per_query[q]; ++j, ++at)
+                entrants->emplace_back((uint32_t)(nk::key_row(keys[at]) - ix->row_base), (keys[at] & 0xffffffff00000000ull) | qrow);
         }
     }
+    std::sort(entrants->begin(), entrants->end());
+    return 0;
+}
 
-    // the rows of R, searched again.  A block with a NaN row among its queries overflows the filter and falls through to the
-    // exact stage, whose arithmetic differs: such a block is searched once more without its NaN rows (lists of -inf scores,
-    // the same on every path), so the other rows get the lists a rebuild gives them in blocks without a NaN query.
+// Merge the entrants into the lists of the rows they touch: each touched row's old entries, their keys recomputed as the
+// row's list scores them (graph_pair_keys_on, per shard of the row), and its entrants in key space, the best k kept.
+static int graph_merge_entrants(NkIndex *ix, GraphCall &g, const std::vector<NkShard *> &live, const GraphEntrants &entrants) {
+    const uint32_t k = g.k;
+    const size_t n_shards = ix->shards.size();
+    std::vector<std::vector<uint64_t>> okeys(n_shards);
+    std::vector<std::vector<uint32_t>> opr(n_shards), opj(n_shards);
+    std::vector<uint32_t> touched;
+    for (size_t i = 0; i < entrants.size(); ++i)
+        if (i == 0 || entrants[i].first != entrants[i - 1].first) touched.push_back(entrants[i].first);
+    std::vector<size_t> shard_of(touched.size());
+    for (size_t t = 0; t < touched.size(); ++t) {
+        const uint32_t r = touched[t];
+        uint64_t local;
+        shard_of[t] = (size_t)(find_shard(ix, r, &local) - ix->shards.data());
+        for (uint32_t j = 0; j < k; ++j) {
+            const uint32_t e = g.gi_in[(uint64_t)r * k + j];
+            if (e == GRAPH_PAD) break;
+            opr[shard_of[t]].push_back(r);
+            opj[shard_of[t]].push_back((uint32_t)(e - ix->row_base));
+        }
+    }
+    for (size_t i = 0; i < n_shards; ++i)
+        if (!opr[i].empty() && graph_pair_keys_on(ix, live, ix->shards[i], opr[i], opj[i], &okeys[i])) return -1;
+    std::vector<size_t> opos(n_shards, 0);
+    std::vector<uint64_t> cand;
+    std::vector<uint32_t> li(k);
+    std::vector<float> ls(k);
+    size_t e0 = 0;
+    for (size_t t = 0; t < touched.size(); ++t) {
+        const uint32_t r = touched[t];
+        cand.clear();
+        const size_t si = shard_of[t];
+        while (opos[si] < opr[si].size() && opr[si][opos[si]] == r) cand.push_back(okeys[si][opos[si]++]);
+        for (; e0 < entrants.size() && entrants[e0].first == r; ++e0) cand.push_back(entrants[e0].second);
+        const size_t take = std::min<size_t>(k, cand.size());
+        std::partial_sort(cand.begin(), cand.begin() + take, cand.end(), std::greater<uint64_t>());
+        for (uint32_t j = 0; j < k; ++j) {
+            if (j < take) decode_key(ix->metric, cand[j], &li[j], &ls[j]);
+            else { li[j] = GRAPH_PAD; ls[j] = 0.0f; }
+        }
+        g.write_list(r, li.data(), ls.data());
+    }
+    return 0;
+}
+
+// The rows of R, searched again.  A block with a NaN row among its queries overflows the filter and falls through to the
+// exact stage, whose arithmetic differs: such a block is searched once more without its NaN rows (lists of -inf scores,
+// the same on every path), so the other rows get the lists a rebuild gives them in blocks without a NaN query.
+static int graph_search_again(NkIndex *ix, GraphCall &g, const std::vector<NkShard *> &live, int path, const std::vector<uint8_t> &in_r) {
+    const uint32_t k = g.k;
     std::vector<uint32_t> rows;
-    for (uint64_t r = 0; r < N; ++r)
+    for (uint64_t r = 0; r < in_r.size(); ++r)
         if (in_r[r]) rows.push_back((uint32_t)r);
     std::vector<uint32_t> ri((size_t)std::min<size_t>(rows.size(), SEARCH_ROWS_BLOCK) * k), sub;
     std::vector<float> rs(ri.size());
     std::vector<NkFilter> rf;  // filters: the block's rows' own
-    auto row_filters = [&](const uint32_t *ids, uint32_t nb) -> const NkFilter * {
-        if (!filters) return nullptr;
-        rf.resize(nb);
-        for (uint32_t q = 0; q < nb; ++q) rf[q] = filters[ids[q]];
-        return rf.data();
+    auto search = [&](const uint32_t *ids, uint32_t nb) {
+        SearchOpts opts{path};
+        if (g.filters) {
+            rf.resize(nb);
+            for (uint32_t q = 0; q < nb; ++q) rf[q] = g.filters[ids[q]];
+            opts.filters_host = rf.data();
+        }
+        return search_rows_locked(ix, live, ids, opts, nb, k, ri.data(), rs.data());
     };
     for (size_t b = 0; b < rows.size(); b += SEARCH_ROWS_BLOCK) {
         uint32_t nb = (uint32_t)std::min<size_t>(SEARCH_ROWS_BLOCK, rows.size() - b);
         std::fill(ri.begin(), ri.end(), GRAPH_PAD);
         std::fill(rs.begin(), rs.end(), 0.0f);
         uint64_t exact0 = 0, exact1 = 0;
-        if (exact_stage_runs(ix, &exact0) ||
-            search_rows_locked(ix, live, rows.data() + b, row_filters(rows.data() + b, nb), nb, k, ri.data(), rs.data()) < 0 ||
-            exact_stage_runs(ix, &exact1))
-            return -1;
+        if (exact_stage_runs(ix, &exact0) || search(rows.data() + b, nb) < 0 || exact_stage_runs(ix, &exact1)) return -1;
         sub.clear();
         for (uint32_t q = 0; q < nb; ++q) {
-            const bool nan_row = ri[(size_t)q * k] != GRAPH_PAD && rs[(size_t)q * k] == nan_score;
-            if (exact1 == exact0 || nan_row) write_list(rows[b + q], ri.data() + (size_t)q * k, rs.data() + (size_t)q * k);
+            const uint32_t *li = ri.data() + (size_t)q * k;
+            const float *ls = rs.data() + (size_t)q * k;
+            if (exact1 == exact0 || graph_nan_list(ix, li, ls)) g.write_list(rows[b + q], li, ls);
             else sub.push_back(rows[b + q]);
         }
         if (sub.empty()) continue;
         nb = (uint32_t)sub.size();
-        if (search_rows_locked(ix, live, sub.data(), row_filters(sub.data(), nb), nb, k, ri.data(), rs.data()) < 0) return -1;
-        for (uint32_t q = 0; q < nb; ++q) write_list(sub[q], ri.data() + (size_t)q * k, rs.data() + (size_t)q * k);
+        if (search(sub.data(), nb) < 0) return -1;
+        for (uint32_t q = 0; q < nb; ++q) g.write_list(sub[q], ri.data() + (size_t)q * k, rs.data() + (size_t)q * k);
     }
-    if (n_lists_changed) *n_lists_changed = n_changed_lists;
+    return 0;
+}
+
+// The body of nk_knn_graph_remap and nk_knn_graph_update.  Returns ke, or -1 with nothing written; *n_lists_changed (nullable):
+// g.changed.
+static int knn_graph_remap_locked(NkIndex *ix, GraphCall g, uint64_t *n_lists_changed) {
+    if (g.k == 0 || g.k > NK_GRAPH_MAX_K) { nk::set_error("%s: k=%u outside [1, %u]", g.what, g.k, NK_GRAPH_MAX_K); return -1; }
+    if (ix->path == NK_PATH_SIMT || ix->path == NK_PATH_TENSOR) {
+        nk::set_error("%s: the graph is kept on the filter paths (AUTO, TENSOR_FILTER or TENSOR_SHADOW), not path %d", g.what, ix->path);
+        return -1;
+    }
+    const uint64_t N = ix->rows();
+    std::vector<uint32_t> now_at;
+    if (graph_check(ix, g, &now_at)) return -1;
+    const std::vector<NkShard *> live = live_shards(ix);
+    const int path = graph_path(ix, g, live);
+    if (path < 0) return -1;
+    if (n_lists_changed) *n_lists_changed = 0;
+    ix->stats.searches++;
+    ScopedRange range(g.what);
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
+    if (g.gi != g.gi_in)  // kept rows start from their old lists
+        for (uint64_t f = 0; f < N; ++f)
+            if (g.src[f] == f) {
+                memcpy(g.gi + f * g.k, g.gi_in + f * g.k, (size_t)g.k * 4);
+                memcpy(g.gs + f * g.k, g.gs_in + f * g.k, (size_t)g.k * 4);
+            }
+
+    // the rows to search again (R) and the queries of the reverse scan (C: new and moved rows)
+    std::vector<uint8_t> in_r(N, 0);
+    std::vector<uint32_t> C;
+    for (uint64_t f = 0; f < N; ++f)
+        if (g.src[f] != f) { in_r[f] = 1; C.push_back((uint32_t)f); }
+    const int ke = (int)std::min<uint64_t>(g.k, ix->returnable_rows());
+    if (C.empty() && N == g.n_old) return ke;  // every row kept at its id
+    if (graph_rows_searched_again(ix, g, now_at, &in_r)) return -1;
+
+    // reverse scan + merge for the kept rows outside R
+    bool reverse = false;
+    for (uint64_t r = 0; r < N && !reverse; ++r) reverse = !in_r[r];
+    if (reverse) {
+        GraphEntrants entrants;
+        if (graph_reverse_scan(ix, g, live, path, in_r, C, &entrants)) return -1;
+        if (graph_merge_entrants(ix, g, live, entrants)) return -1;
+    }
+    if (graph_search_again(ix, g, live, path, in_r)) return -1;
+    if (n_lists_changed) *n_lists_changed = g.changed;
     return ke;
 }
 
-static int knn_graph_remap_host(NkIndex *ix, const char *what, uint32_t k, uint64_t n_old, const uint32_t *src_of_row,
-                                const NkFilter *filters, const uint32_t *graph_idx_in, const float *graph_score_in,
-                                uint32_t *graph_idx_out, float *graph_score_out, uint64_t *n_lists_changed) {
+// The arguments of nk_knn_graph_remap[_filtered] checked, then the call itself.
+static int knn_graph_remap_host(NkIndex *ix, const GraphCall &g, uint64_t *n_lists_changed) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
-    if (!graph_idx_out || !graph_score_out || (n_old && (!graph_idx_in || !graph_score_in))) { nk::set_error("null argument"); return -1; }
+    if (!g.gi || !g.gs || (g.n_old && (!g.gi_in || !g.gs_in))) { nk::set_error("null argument"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
     const uint64_t N = ix->rows();
-    if (N && !src_of_row) { nk::set_error("null argument"); return -1; }
+    if (N && !g.src) { nk::set_error("null argument"); return -1; }
     // the output is written while the input is still read: overlapping arrays are refused
     auto overlap = [](const void *a, size_t na, const void *b, size_t nb) {
         const uintptr_t pa = (uintptr_t)a, pb = (uintptr_t)b;
         return na && nb && pa < pb + nb && pb < pa + na;
     };
-    const size_t in_bytes = (size_t)(n_old * k) * 4, out_bytes = (size_t)(N * k) * 4;
-    for (const void *in : {(const void *)graph_idx_in, (const void *)graph_score_in})
-        for (const void *out : {(const void *)graph_idx_out, (const void *)graph_score_out})
+    const size_t in_bytes = (size_t)(g.n_old * g.k) * 4, out_bytes = (size_t)(N * g.k) * 4;
+    for (const void *in : {(const void *)g.gi_in, (const void *)g.gs_in})
+        for (const void *out : {(const void *)g.gi, (const void *)g.gs})
             if (overlap(in, in_bytes, out, out_bytes)) {
-                nk::set_error("%s: the output arrays overlap the input graph", what);
+                nk::set_error("%s: the output arrays overlap the input graph", g.what);
                 return -1;
             }
-    return knn_graph_remap_locked(ix, what, k, n_old, src_of_row, filters, graph_idx_in, graph_score_in, graph_idx_out, graph_score_out,
-                                  false, n_lists_changed);
+    return knn_graph_remap_locked(ix, g, n_lists_changed);
 }
 
 int nk_knn_graph_remap(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row, const uint32_t *graph_idx_in,
                        const float *graph_score_in, uint32_t *graph_idx_out, float *graph_score_out, uint64_t *n_lists_changed) {
-    return knn_graph_remap_host(ix, "nk_knn_graph_remap", k, n_old, src_of_row, nullptr, graph_idx_in, graph_score_in, graph_idx_out,
-                                graph_score_out, n_lists_changed);
+    return knn_graph_remap_host(ix, GraphCall{"nk_knn_graph_remap", k, n_old, src_of_row, nullptr, graph_idx_in, graph_score_in,
+                                              graph_idx_out, graph_score_out, false}, n_lists_changed);
 }
 
 int nk_knn_graph_remap_filtered(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row, const NkFilter *filters_host,
                                 const uint32_t *graph_idx_in, const float *graph_score_in, uint32_t *graph_idx_out,
                                 float *graph_score_out, uint64_t *n_lists_changed) {
-    return knn_graph_remap_host(ix, "nk_knn_graph_remap_filtered", k, n_old, src_of_row, filters_host, graph_idx_in, graph_score_in,
-                                graph_idx_out, graph_score_out, n_lists_changed);
+    return knn_graph_remap_host(ix, GraphCall{"nk_knn_graph_remap_filtered", k, n_old, src_of_row, filters_host, graph_idx_in,
+                                              graph_score_in, graph_idx_out, graph_score_out, false}, n_lists_changed);
 }
 
-// An old row keeps its id; a rewritten row and every row from n_old on hold contents the graph never saw.  In place.
-static int knn_graph_update_host(NkIndex *ix, const char *what, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
-                                 const NkFilter *filters, uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed) {
+// An old row keeps its id; a rewritten row and every row from n_old on hold contents the graph never saw.  In place: g.src
+// and the input graph are filled in here.
+static int knn_graph_update_host(NkIndex *ix, GraphCall g, const uint32_t *changed_rows, uint32_t n_changed, uint64_t *n_lists_changed) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
-    if (!graph_idx || !graph_score || (n_changed && !changed_rows)) { nk::set_error("null argument"); return -1; }
+    if (!g.gi || !g.gs || (n_changed && !changed_rows)) { nk::set_error("null argument"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
     const uint64_t N = ix->rows();
-    if (n_old > N) { nk::set_error("%s: n_old=%llu exceeds the index's %llu rows", what, (unsigned long long)n_old, (unsigned long long)N); return -1; }
+    if (g.n_old > N) { nk::set_error("%s: n_old=%llu exceeds the index's %llu rows", g.what, (unsigned long long)g.n_old, (unsigned long long)N); return -1; }
     std::vector<uint32_t> src(N, NK_ROW_NEW);
-    for (uint64_t f = 0; f < n_old; ++f) src[f] = (uint32_t)f;
+    for (uint64_t f = 0; f < g.n_old; ++f) src[f] = (uint32_t)f;
     for (uint32_t i = 0; i < n_changed; ++i) {
-        if (changed_rows[i] >= n_old) { nk::set_error("%s: changed row %u is not an old row (n_old=%llu)", what, changed_rows[i], (unsigned long long)n_old); return -1; }
+        if (changed_rows[i] >= g.n_old) { nk::set_error("%s: changed row %u is not an old row (n_old=%llu)", g.what, changed_rows[i], (unsigned long long)g.n_old); return -1; }
         src[changed_rows[i]] = NK_ROW_NEW;
     }
-    return knn_graph_remap_locked(ix, what, k, n_old, src.data(), filters, graph_idx, graph_score, graph_idx, graph_score, true,
-                                  n_lists_changed);
+    g.src = src.data();
+    g.gi_in = g.gi;
+    g.gs_in = g.gs;
+    return knn_graph_remap_locked(ix, g, n_lists_changed);
 }
 
 int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
                         uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed) {
-    return knn_graph_update_host(ix, "nk_knn_graph_update", k, n_old, changed_rows, n_changed, nullptr, graph_idx, graph_score,
-                                 n_lists_changed);
+    return knn_graph_update_host(ix, GraphCall{"nk_knn_graph_update", k, n_old, nullptr, nullptr, nullptr, nullptr, graph_idx, graph_score, true},
+                                 changed_rows, n_changed, n_lists_changed);
 }
 
 int nk_knn_graph_update_filtered(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
                                  const NkFilter *filters_host, uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed) {
-    return knn_graph_update_host(ix, "nk_knn_graph_update_filtered", k, n_old, changed_rows, n_changed, filters_host, graph_idx,
-                                 graph_score, n_lists_changed);
+    return knn_graph_update_host(ix, GraphCall{"nk_knn_graph_update_filtered", k, n_old, nullptr, filters_host, nullptr, nullptr, graph_idx,
+                                               graph_score, true}, changed_rows, n_changed, n_lists_changed);
 }
 
 static int single_shard(NkIndex *ix, NkShard **out) {
@@ -2103,7 +2201,7 @@ static int search_keys_locked(NkIndex *ix, NkShard *s, const float *queries_dev,
         NK_CUDA_OK(cudaMemsetAsync(out_keys_dev, 0, (size_t)Q * k * 8, st));
         return (int)k;
     }
-    if (run_scan(ix, *s, queries_dev, Q, k, out_keys_dev, st)) return -1;
+    if (run_scan(ix, *s, queries_dev, Q, k, out_keys_dev, st, ScanOut(ix->path))) return -1;
     return (int)k;
 }
 
@@ -2140,7 +2238,7 @@ static int search_device(NkIndex *ix, const float *queries_dev, const NkFilter *
     if (nk::ws_reserve((void **)&s->ws.keys, &s->ws.keys_bytes, (size_t)Q * k * 8)) return -1;
     ix->stats.searches++;
     ix->stats.queries += Q;
-    ScanOut xo;
+    ScanOut xo(ix->path);
     xo.out_idx = out_idx_dev; xo.out_score = out_score_dev;  // decoded by the last kernel of the path
     if (filters_dev) {
         if (shard_tags_on(*s)) return -1;
@@ -2262,8 +2360,7 @@ int nk_score_subset(NkIndex *ix, const float *query_host, const uint32_t *rows_h
         cudaStreamSynchronize(s->stream);
         return -1;
     }
-    s->last_filter = false;
-    if (finish_deferred(ix, *s) < 0) return -1;
+    if (finish_deferred(ix, *s, nullptr) < 0) return -1;
     // positions within the subset -> global row ids (ties broken by subset position, like the stable
     // order of ScoreSubset's input list)
     for (uint32_t i = 0; i < ke; ++i) out_idx[i] = pos[i] < n_subset ? rows_host[pos[i]] : 0xffffffffu;
@@ -2472,8 +2569,7 @@ int nk_search_groups(NkIndex *ix, const float *query_host, uint32_t k, uint32_t 
     ShardOrder order(*s, s->stream);
     if (order.failed()) return -1;
     NK_CUDA_OK(cudaSetDevice(s->device));
-    NK_RANGE_PUSH("nk_search_groups");
-    struct Pop { ~Pop() { NK_RANGE_POP(); } } pop_on_exit;
+    ScopedRange range("nk_search_groups");
     if (nk::ws_reserve((void **)&s->ws.queries, &s->ws.queries_bytes, (size_t)ix->dim * 4)) return -1;
     if (nk::ws_reserve(&s->ws.scratch, &s->ws.scratch_bytes, (size_t)G * 8)) return -1;
     if (nk::ws_reserve((void **)&s->ws.keys, &s->ws.keys_bytes, (size_t)ke * 8)) return -1;
@@ -2493,8 +2589,7 @@ int nk_search_groups(NkIndex *ix, const float *query_host, uint32_t k, uint32_t 
     NK_CUDA_OK(cudaMemcpyAsync(out_group, s->ws.out_idx, (size_t)ke * 4, cudaMemcpyDeviceToHost, s->stream));
     NK_CUDA_OK(cudaMemcpyAsync(out_row, s->ws.out_idx + ke, (size_t)ke * 4, cudaMemcpyDeviceToHost, s->stream));
     NK_CUDA_OK(cudaMemcpyAsync(out_score, s->ws.out_score, (size_t)ke * 4, cudaMemcpyDeviceToHost, s->stream));
-    s->last_filter = false;
-    if (finish_deferred(ix, *s) < 0) return -1;
+    if (finish_deferred(ix, *s, nullptr) < 0) return -1;
     uint32_t found = 0;
     while (found < ke && out_group[found] != 0xffffffffu) ++found;
     return (int)found;
