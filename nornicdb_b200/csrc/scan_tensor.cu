@@ -283,7 +283,7 @@ __global__ void __launch_bounds__(PREP_THREADS) filter_prep_kernel(PrepParams p)
     }
 }
 
-// Score estimate of one accumulator fragment row of the TF32 scan (keep_fragment_row):
+// Score estimate of one accumulator fragment row of the TF32 scan (keep_fragment_rows):
 //   cosine     acc / |x|  (queries pre-normalised)       filter bound c
 //   dot        acc                                        filter bound c |x| |q|
 //   euclidean  -(|x|^2 + |q|^2 - 2 acc)   (filter only)   filter bound 2c |x| |q|
@@ -292,10 +292,12 @@ template <bool FILTER> struct Tf32Est {
     float mul, bnd, x2;
     const float *qn;
     bool euclid;
-    __device__ __forceinline__ float upper(float v, uint32_t qi) const {
+    struct Col { float qn; };  // the query's input, read once per column for all of a thread's rows
+    __device__ __forceinline__ Col col(uint32_t qi) const { return {FILTER ? qn[qi] : 0.0f}; }
+    __device__ __forceinline__ float upper(float v, const Col &c) const {
         float sc = v * mul;
         if (FILTER) {
-            const float q = qn[qi];
+            const float q = c.qn;
             if (euclid) sc -= tc::EUC_KEEP * fmaf(q, q, x2);
             sc = fmaf(bnd, q, sc);
         }
@@ -307,7 +309,7 @@ template <bool FILTER> struct Tf32Est {
 // TAGS: filtered search (per-query tag filters in the keep rule); the unfiltered instantiations are TAGS = false.
 // RANGE (filter mode only, nk_search_range): fixed per-query thresholds; full buffers are flushed to the lists, never pruned.
 // ROWTHR (with RANGE, the reverse scan of nk_knn_graph_update): a pair must also reach its row's threshold p.row_thr[row].
-// RFILT (with ROWTHR and TAGS, a filtered graph): the row's own filter must also admit the query's tag (keep_fragment_row);
+// RFILT (with ROWTHR and TAGS, a filtered graph): the row's own filter must also admit the query's tag (keep_fragment_rows);
 // the launch's query tags are staged in shared memory past Shared.
 template <int NT, int QT, bool DUMP, bool TAGS, bool RANGE = false, bool ROWTHR = false, bool RFILT = false>
 __global__ void __launch_bounds__(tc::THREADS, 1)
@@ -455,26 +457,26 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                 for (uint32_t qi = 0; qi < nq; ++qi) sh.cnt[qi] = (int)((it + 1) * ROWS);
 #pragma unroll
             for (uint32_t ri = 0; ri < 4; ++ri) {
-                const uint32_t h = ri >> 1, r = ri & 1;
-                const uint32_t rt = rbase + 64 * h + 8 * r;  // row within the tile
+                const uint32_t rt = rbase + 64 * (ri >> 1) + 8 * (ri & 1);  // row within the tile
                 const uint32_t row = tile * ROWS + rt;
                 const bool alive = row_alive(p, row);
-                Tf32Est<FILTER> est;
-                est.x2 = sh.xx[rt];
-                est.qn = sh.qn;
-                est.euclid = euclid;
-                const float xn = sqrtf(est.x2);
-                est.mul = 1.0f;
-                est.bnd = 0.0f;
-                if (cosine) est.mul = est.x2 > 0.0f ? 1.0f / xn : 0.0f;
+                Tf32Est<FILTER> est[1];
+                Tf32Est<FILTER> &e = est[0];
+                e.x2 = sh.xx[rt];
+                e.qn = sh.qn;
+                e.euclid = euclid;
+                const float xn = sqrtf(e.x2);
+                e.mul = 1.0f;
+                e.bnd = 0.0f;
+                if (cosine) e.mul = e.x2 > 0.0f ? 1.0f / xn : 0.0f;
                 if (FILTER) {
-                    est.bnd = cosine ? p.margin_c : bfac * xn;
-                    if (!cosine && alive && est.x2 < INFINITY && (lane & 3) == 0) atomicMax(&sh.maxxx, __float_as_uint(est.x2));  // NaN / Inf rows: kept, judged exactly
-                    if (euclid) est.mul = 2.0f;
+                    e.bnd = cosine ? p.margin_c : bfac * xn;
+                    if (!cosine && alive && e.x2 < INFINITY && (lane & 3) == 0) atomicMax(&sh.maxxx, __float_as_uint(e.x2));  // NaN / Inf rows: kept, judged exactly
+                    if (euclid) e.mul = 2.0f;
                 }
-                keep_fragment_row<QT, P, FILTER, DUMP && FILTER, TAGS, ROWTHR, RFILT>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq,
-                                                                                sh.tau, sh.qn, sh.cnt, my_cand,
-                                                                                ROWTHR && row < p.n ? __ldg(p.row_thr + row) : -INFINITY, qtag);
+                const float rthr[1] = {ROWTHR && row < p.n ? __ldg(p.row_thr + row) : -INFINITY};
+                keep_fragment_rows<QT, P, FILTER, DUMP && FILTER, TAGS, ROWTHR, RFILT>(p, est, acc, ri, alive ? 1u : 0u, tile * ROWS, rbase, flood, it,
+                                                                                 cbase, q0, nq, sh.tau, sh.qn, sh.cnt, my_cand, rthr, qtag);
             }
             // prune any buffer that could overflow during the next tile; the 8 consumer warps prune different
             // queries concurrently with a register-resident warp selection

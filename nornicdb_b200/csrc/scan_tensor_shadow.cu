@@ -197,9 +197,15 @@ int build_image_s8(const float *rows, uint64_t first, uint64_t count, uint32_t d
 // Debug timeline (NK_TC_DEBUG & 64): per-CTA globaltimer stamps, printed by launch_shadow_pass_t after a synchronize.
 //   [0] entry  [1] set-up done  [2] first accumulator ready  [3] last tile's epilogue done  [4] exit
 //   [5] ns in the prune section (epilogue warp 0)  [6] tile index of the first prune  [7] ns waiting for accumulators
-__device__ unsigned long long g_sb_prof[256][16];  // [8] all warps past the tile loop  [9] warp 0 done emitting  [10] live chunks  [11] entries emitted by warp 0
+//   [8] all warps past the tile loop  [9] warp 0 done emitting  [10] live chunks  [11] entries emitted by warp 0
+//   [12..14] emission stages.  The tile loop of epilogue thread 0, split (ns summed over its tiles): [15] tiles
+//   [16] waiting for the row inputs (|x|^2, |dx|^2, scale, mask word, row threshold) after the accumulators
+//   [17] int8 conversion, the rows' estimates and the keep rule  [18] the row maxima's shared atomics (one per warp and value)
+//   [19] the first EPI_BAR (arrival skew)  [20] prunes / flushes  [21] the second EPI_BAR  [22] threshold adoption
+__device__ unsigned long long g_sb_prof[256][24];
+__device__ float g_sb_sink;  // the timeline's row-input stamp stores their sum here: the store waits until they landed
 
-// Score estimate of one accumulator fragment row of the 16-bit scan (keep_fragment_row): the UPPER bound of the score,
+// Score estimate of one accumulator fragment row of the 16-bit scan (keep_fragment_rows): the UPPER bound of the score,
 // bound(row, q) = ra qa[q] + rb qb[q]:
 //   cosine     acc/|x|                        ra = |dx|/|x|   rb = 1
 //   dot        acc                            ra = |dx|       rb = |x|
@@ -208,9 +214,11 @@ struct Bf16Est {
     float mul, ra, rb, x2;
     const float *qa, *qb, *qn;
     bool euclid;
-    __device__ __forceinline__ float upper(float v, uint32_t qi) const {
-        float sc = fmaf(v, mul, fmaf(ra, qa[qi], rb * qb[qi]));
-        if (euclid) { const float q = qn[qi]; sc -= tc::EUC_KEEP * fmaf(q, q, x2); }
+    struct Col { float qa, qb, qn; };  // the query's inputs, read once per column for all of a thread's rows
+    __device__ __forceinline__ Col col(uint32_t qi) const { return {qa[qi], qb[qi], euclid ? qn[qi] : 0.0f}; }
+    __device__ __forceinline__ float upper(float v, const Col &c) const {
+        float sc = fmaf(v, mul, fmaf(ra, c.qa, rb * c.qb));
+        if (euclid) sc -= tc::EUC_KEEP * fmaf(c.qn, c.qn, x2);
         return sc;
     }
     __device__ __forceinline__ float bound(uint32_t qi) const { return fmaf(ra, qa[qi], rb * qb[qi]); }
@@ -221,7 +229,7 @@ struct Bf16Est {
 // corpora), fp16 (an fp16 corpus scanned in place) or int8 (the int8 image of an fp32 shard).  RANGE (nk_search_range): fixed per-query thresholds; full buffers are flushed to the
 // lists, never pruned, and the end of the launch flushes what is left.  ROWTHR (with RANGE, the reverse scan of
 // nk_knn_graph_update): a pair must also reach its row's threshold p.row_thr[row], loaded with the row's norms.  RFILT (with
-// ROWTHR and TAGS, a filtered graph): the row's own filter must also admit the query's tag (keep_fragment_row); the launch's
+// ROWTHR and TAGS, a filtered graph): the row's own filter must also admit the query's tag (keep_fragment_rows); the launch's
 // query tags are staged in shared memory past Shared.
 template <int QT, ptx::Opnd OP, bool DUMP, bool TAGS, bool RANGE, bool ROWTHR = false, bool RFILT = false>
 __global__ void __launch_bounds__(sb::NTHREADS, 1)
@@ -238,7 +246,10 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const bool prof = (p.debug & 64) && blockIdx.x < 256;
-    if (prof && tid == 0) { g_sb_prof[blockIdx.x][0] = globaltimer_ns(); g_sb_prof[blockIdx.x][6] = ~0ull; }
+    if (prof && tid == 0) {
+        g_sb_prof[blockIdx.x][0] = globaltimer_ns(); g_sb_prof[blockIdx.x][6] = ~0ull;
+        for (int i = 16; i <= 22; ++i) g_sb_prof[blockIdx.x][i] = 0;
+    }
     const uint32_t num_tiles = (p.n + ROWS - 1) / ROWS;
     const QueryGroup<QT> qg(p);
     const uint32_t sub = qg.sub, sgrid = qg.sgrid, q0 = qg.q0, qpad_off = qg.qpad_off, nq = qg.nq;
@@ -314,7 +325,8 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
         const int prune_trigger = min(prune_at, max(192, 4 * (int)p.k));
         const bool euclid = p.metric == NK_METRIC_EUCLIDEAN;
         const bool eprof = prof && ewarp == 0 && lane == 0;
-        unsigned long long t_prune = 0, t_wait = 0, t_a = 0;
+        unsigned long long t_wait = 0, t_a = 0;
+        unsigned long long *split = g_sb_prof[blockIdx.x < 256 ? blockIdx.x : 0];  // [16..22] (eprof only: no registers held)
         float acc[2][QT / 2];
 #pragma unroll
         for (int h = 0; h < 2; ++h)
@@ -323,9 +335,9 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
         uint32_t g = 0, it = 0;
         for (uint32_t tile = sub; tile < num_tiles; tile += sgrid, ++it) {
             if (eprof) t_a = globaltimer_ns();
-            // The epilogue's global inputs, loaded before the MMAs: |x|^2, |dx|^2 (int8 image: and the row's scale) and the
-            // mask word of this thread's 4 rows, and the shared threshold of query etid (it only grows: an earlier value is
-            // still a lower bound).
+            // The epilogue's row inputs, loaded before the MMAs: |x|^2, |dx|^2 (int8 image: and the row's scale), the mask word
+            // and (ROWTHR) the threshold of this thread's 4 rows; and the shared threshold of query etid (it only grows: an
+            // earlier value is still a lower bound).
             float x2[4], d2[4], rthr[4], xs[4];
             uint32_t mword[4];
 #pragma unroll
@@ -367,6 +379,21 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             ptx::wgmma_wait_all();
             ptx::fence_acc(acc[0]);
             ptx::fence_acc(acc[1]);
+            if (eprof) {
+                const unsigned long long t = globaltimer_ns();
+                t_wait += t - t_a;
+                if (it == 0) g_sb_prof[blockIdx.x][2] = t;
+                t_a = t;
+            }
+            if (eprof) {  // wait for the row inputs here, to time it
+                float s = 0.0f;
+#pragma unroll
+                for (uint32_t ri = 0; ri < 4; ++ri) s += x2[ri] + d2[ri] + xs[ri] + rthr[ri] + (float)mword[ri];
+                *(volatile float *)&g_sb_sink = s;
+                const unsigned long long t = globaltimer_ns();
+                split[16] += t - t_a;
+                t_a = t;
+            }
             if constexpr (S8) {
                 // exact int32 dot products of the int8 rows -> fp32 in the same registers, times the query's scale (the
                 // row's scale is part of the estimate's multiplier): acc = xq.qq s_q, the estimate (s_x xq).(s_q qq)
@@ -378,46 +405,57 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             }
             __syncwarp();
             if (lane == 0) { ptx::mbar_arrive(&sh.ring.aempty[prev_sa]); ptx::mbar_arrive(&sh.ring.bempty[prev_sb]); }
-            if (eprof) {
-                const unsigned long long t = globaltimer_ns();
-                t_wait += t - t_a;
-                if (it == 0) g_sb_prof[blockIdx.x][2] = t;
-            }
-            if (flood && it < 2 && ewarp == 0 && lane == 0)
-                for (uint32_t qi = 0; qi < nq; ++qi) sh.cnt[qi] = (int)((it + 1) * ROWS);
+            // the rows' estimates
+            Bf16Est est[4];
+            uint32_t alive = 0u;
+            uint32_t mx_ra = 0u, mx_rb = 0u, mx_xx = 0u;  // maxima (float bits) of the bound factors and |x|^2 of the alive rows
 #pragma unroll
             for (uint32_t ri = 0; ri < 4; ++ri) {
-                const uint32_t h = ri >> 1, r = ri & 1;
-                const uint32_t rt = rbase + 64 * h + 8 * r;  // row within the tile
-                const uint32_t row = tile * ROWS + rt;
-                const bool alive = row < p.n && ((mword[ri] >> (row & 31)) & 1u);
-                Bf16Est est;
-                est.x2 = x2[ri];
-                est.qa = sh.qa;
-                est.qb = sh.qb;
-                est.qn = sh.qn;
-                est.euclid = euclid;
-                const float xn = sqrtf(est.x2);
+                const uint32_t row = tile * ROWS + rbase + 64 * (ri >> 1) + 8 * (ri & 1);
+                const bool live = row < p.n && ((mword[ri] >> (row & 31)) & 1u);
+                alive |= live ? 1u << ri : 0u;
+                Bf16Est &e = est[ri];
+                e.x2 = x2[ri];
+                e.qa = sh.qa;
+                e.qb = sh.qb;
+                e.qn = sh.qn;
+                e.euclid = euclid;
+                const float xn = sqrtf(e.x2);
                 const float dxn = sqrtf(d2[ri]) * 1.0001f;
-                est.mul = 1.0f; est.ra = dxn; est.rb = xn;
+                e.mul = 1.0f; e.ra = dxn; e.rb = xn;
                 if (cosine) {
-                    est.mul = est.x2 > 0.0f ? 1.0f / xn : 0.0f;
-                    est.ra = dxn * est.mul * 1.000001f;
-                    est.rb = 1.0f;
+                    e.mul = e.x2 > 0.0f ? 1.0f / xn : 0.0f;
+                    e.ra = dxn * e.mul * 1.000001f;
+                    e.rb = 1.0f;
                 } else if (euclid) {
-                    est.mul = 2.0f; est.ra = 2.0f * dxn; est.rb = 2.0f * xn;
+                    e.mul = 2.0f; e.ra = 2.0f * dxn; e.rb = 2.0f * xn;
                 }
-                if (S8) est.mul *= xs[ri];  // (a NaN scale: a non-finite row, every estimate NaN -> kept)
-                if ((lane & 3) == 0 && alive && est.ra < INFINITY && est.rb < INFINITY) {  // NaN / Inf rows are kept anyway (score NaN -> +inf)
-                    atomicMax(&sh.max_ra, __float_as_uint(est.ra));
-                    if (!cosine) { atomicMax(&sh.max_rb, __float_as_uint(est.rb)); atomicMax(&sh.maxxx, __float_as_uint(est.x2)); }
+                if (S8) e.mul *= xs[ri];  // (a NaN scale: a non-finite row, every estimate NaN -> kept)
+                if (live && e.ra < INFINITY && e.rb < INFINITY) {  // NaN / Inf rows are kept anyway (score NaN -> +inf)
+                    mx_ra = max(mx_ra, __float_as_uint(e.ra));
+                    if (!cosine) { mx_rb = max(mx_rb, __float_as_uint(e.rb)); mx_xx = max(mx_xx, __float_as_uint(e.x2)); }
                 }
-                keep_fragment_row<QT, PB, true, DUMP, TAGS, ROWTHR, RFILT>(p, est, acc[h], r, row, rt, alive, flood, it, cbase, q0, nq, sh.tau, sh.qn,
-                                                                           sh.cnt, my_cand, rthr[ri], qtag);
             }
+            if (eprof) { const unsigned long long t = globaltimer_ns(); split[17] += t - t_a; t_a = t; }
+            {
+                // One atomic per warp and maximum.  This tile's prunes (after the first EPI_BAR) read the maxima over every
+                // row this CTA has seen, as per-row atomics would leave them.
+                const uint32_t wa = __reduce_max_sync(0xffffffffu, mx_ra);
+                const uint32_t wb = __reduce_max_sync(0xffffffffu, mx_rb), wx = __reduce_max_sync(0xffffffffu, mx_xx);
+                if (lane == 0) {
+                    atomicMax(&sh.max_ra, wa);
+                    if (!cosine) { atomicMax(&sh.max_rb, wb); atomicMax(&sh.maxxx, wx); }
+                }
+            }
+            if (eprof) { const unsigned long long t = globaltimer_ns(); split[18] += t - t_a; t_a = t; }
+            if (flood && it < 2 && ewarp == 0 && lane == 0)
+                for (uint32_t qi = 0; qi < nq; ++qi) sh.cnt[qi] = (int)((it + 1) * ROWS);
+            keep_fragment_rows<QT, PB, true, DUMP, TAGS, ROWTHR, RFILT>(p, est, acc, 0, alive, tile * ROWS, rbase, flood, it, cbase, q0, nq, sh.tau,
+                                                                        sh.qn, sh.cnt, my_cand, rthr, qtag);
+            if (eprof) { const unsigned long long t = globaltimer_ns(); split[17] += t - t_a; t_a = t; }
             // prune any buffer that could overflow during the next tile (8 warps, different queries concurrently)
             group_sync(EPI_BAR, EPI_NT);  // every push of this tile is visible
-            if (eprof) t_a = globaltimer_ns();
+            if (eprof) { const unsigned long long t = globaltimer_ns(); split[19] += t - t_a; t_a = t; }
             if constexpr (RANGE)
                 flush_tile<PB>(p, q0, nq, ewarp, lane, my_cand, sh.cnt);
             else
@@ -426,11 +464,16 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                                      if (eprof && g_sb_prof[blockIdx.x][6] == ~0ull) g_sb_prof[blockIdx.x][6] = it;
                                      prune(qi, out, out_len, max_keep, floor_tau, gcount);
                                  });
+            if (eprof) { const unsigned long long t = globaltimer_ns(); split[20] += t - t_a; t_a = t; }
             group_sync(EPI_BAR, EPI_NT);
-            if (eprof) t_prune += globaltimer_ns() - t_a;
+            if (eprof) { const unsigned long long t = globaltimer_ns(); split[21] += t - t_a; t_a = t; }
             if (!RANGE && etid < nq) sh.tau[etid] = raise_to_shared_tau(gt_pre, sh.tau[etid]);  // adopt the shared threshold
+            if (eprof) split[22] += globaltimer_ns() - t_a;
         }
-        if (eprof) { g_sb_prof[blockIdx.x][3] = globaltimer_ns(); g_sb_prof[blockIdx.x][5] = t_prune; g_sb_prof[blockIdx.x][7] = t_wait; }
+        if (eprof) {
+            unsigned long long *pr = g_sb_prof[blockIdx.x];
+            pr[3] = globaltimer_ns(); pr[5] = pr[20] + pr[21]; pr[7] = t_wait; pr[15] = it;
+        }
         ptx::setmaxnreg_dec<EMIT_REGS>();
         ptx::named_bar_arrive(REG_BAR, NTHREADS);
     }
@@ -561,7 +604,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
 }
 
 static void sb_print_prof(cudaStream_t stream, uint32_t grid) {
-    static unsigned long long h[256][16];
+    static unsigned long long h[256][24];
     cudaStreamSynchronize(stream);
     cudaMemcpyFromSymbol(h, g_sb_prof, sizeof(h));
     const uint32_t g = grid < 256 ? grid : 256;
@@ -588,6 +631,13 @@ static void sb_print_prof(cudaStream_t stream, uint32_t grid) {
             "exit min +%.1f avg +%.1f max +%.1f | prune section %.1f us (first at tile %.1f) | accumulator wait %.1f us\n",
             g, tend_max / 1e3, start_max / 1e3, setup / g / 1e3, first / g / 1e3, e3 / g / 1e3, e3_max / 1e3, tend_min / 1e3, ends / g / 1e3,
             tend_max / 1e3, prune / g / 1e3, ftile / g, wait / g / 1e3);
+    double split[24] = {};
+    for (uint32_t b = 0; b < g; ++b)
+        for (int i = 15; i <= 22; ++i) split[i] += (double)h[b][i];
+    fprintf(stderr, "[shadow prof] tile loop per CTA (us, epilogue thread 0, %.1f tiles): accumulator wait %.1f | row inputs %.1f | "
+            "conversion + keep rule %.1f | shared atomics %.1f | barrier 1 %.1f | prunes %.1f | barrier 2 %.1f | adoption %.1f\n",
+            split[15] / g, wait / g / 1e3, split[16] / g / 1e3, split[17] / g / 1e3, split[18] / g / 1e3, split[19] / g / 1e3,
+            split[20] / g / 1e3, split[21] / g / 1e3, split[22] / g / 1e3);
 }
 
 // The 16-bit / int8 pass needs an image of the rows (a.image): the BF16 shadow or the int8 image of an fp32 shard, or —

@@ -152,113 +152,169 @@ __device__ __forceinline__ bool row_alive(const Params &p, uint32_t row) {
     return row < p.n && (!p.mask || ((__ldg(p.mask + (row >> 5)) >> (row & 31)) & 1u));
 }
 
-// The filter's keep rule for one accumulator fragment row: thread = 1 row x QT/4 query columns cbase + 8 (j / 2) + j % 2
-// of acc (the row's 64-row half), r = which of the half's two fragment rows.  Buffers every (row, query) pair whose score
-// estimate can still reach the query's threshold.  The kernel supplies the estimate: est.upper(v, qi) is the UPPER bound
-// of the score from accumulator value v (exact mode: the score itself), est.bound(qi) its error bound before the
-// euclidean term (DUMP only), est.mul / est.x2 the row's scale and |x|^2.
-//   flood (first two tiles without a sampled threshold): every pair is placed directly at slot = tile-local row;
-//   otherwise a compact compare pass builds the mask of columns worth buffering (NaN passes) and the rare pushes run in a
-//   small out-of-line loop so the hot code stays short.
+// Element i of a thread's per-row array for a row index known only at run time: the register file is not indexable, so
+// select by compare (an indexed local array would live in local memory).
+template <class T, int N> __device__ __forceinline__ T pick_row(const T (&a)[N], uint32_t ri) {
+    T v = a[0];
+#pragma unroll
+    for (int i = 1; i < N; ++i)
+        if (ri == (uint32_t)i) v = a[i];
+    return v;
+}
+// Accumulator value of fragment row fr (tile rows rbase + 64 (fr / 2) + 8 (fr % 2)) in column slot jj (query cbase +
+// 8 (jj / 2) + jj % 2).
+template <int QT> __device__ __forceinline__ float frag_at(const float (&acc)[2][QT / 2], uint32_t fr, int jj) {
+    const int i = (jj >> 1) * 4 + (jj & 1);
+    return fr == 0 ? acc[0][i] : fr == 1 ? acc[0][i + 2] : fr == 2 ? acc[1][i] : acc[1][i + 2];
+}
+// ... for a column slot c known only at run time: select by compare.
+template <int QT> __device__ __forceinline__ float frag_value(const float (&acc)[2][QT / 2], uint32_t fr, uint32_t c) {
+    float v = 0.0f;
+#pragma unroll
+    for (int jj = 0; jj < QT / 4; ++jj)
+        if (c == (uint32_t)jj) v = frag_at<QT>(acc, fr, jj);
+    return v;
+}
+
+// The filter's keep rule for NR of a thread's 4 accumulator fragment rows: est[ri] is fragment row fr = fr0 + ri = tile row
+// rbase + 64 (fr / 2) + 8 (fr % 2) (corpus row row0 + that), QT/4 query columns cbase + 8 (j / 2) + j % 2.  Buffers every
+// (row, query) pair whose score estimate can still reach the query's threshold.  The kernel supplies one estimate per row:
+// est[ri].upper(v, col) is the UPPER bound of the score from accumulator value v (exact mode: the score itself) given the
+// query's inputs col = est[0].col(qi), est.bound(qi) its error bound before the euclidean term (DUMP only), est.mul /
+// est.x2 the row's scale and |x|^2.  alive: bit ri set = the row takes part.  The 16-bit / int8 scan passes all 4 rows at
+// once (NR = 4); the TF32 kernel, whose register budget is 168 rather than 240, one row at a time (NR = 1).
+//   flood (first two tiles without a sampled threshold): every pair is placed directly at slot = tile-local row, in a loop
+//   over the rows that is not unrolled: it runs on two tiles of a launch at most and stays out of the hot code.
+//   otherwise a compare pass over the columns reads each query's inputs and threshold from shared memory once for all NR
+//   rows and builds the masks of pairs worth buffering (NaN passes); the rare pushes run in a small loop that is not
+//   unrolled.
 // BOUNDED: a NaN estimate is undecidable here, so it is kept as +inf and the exact re-scoring judges; exact mode: -inf.
 // TAGS (filtered searches): a pair whose query does not admit the row's tag never enters a buffer — otherwise the pruned and
 // published thresholds would stop being lower bounds of the FILTERED k-th best score.  Flood tiles place it as key 0; the
 // compare pass loads the row's tag only when some column passed and clears the columns whose filter rejects it.
-// ROWTHR (the reverse scan of nk_knn_graph_update, range mode): a pair must also reach the ROW's threshold rthr.
+// ROWTHR (the reverse scan of nk_knn_graph_update, range mode): a pair must also reach the ROW's threshold rthr[ri].
 // RFILT (with ROWTHR and TAGS, the reverse scan of a filtered graph): the row's own filter p.row_filter[row] must also admit
 // the query's tag qtag[qi] (the CTA's query tags, in shared memory) — the mirror image of TAGS.  The row's filter is loaded
 // only for a fragment row with a pair that already reached both thresholds.
-template <int QT, int CAP, bool BOUNDED, bool DUMP, bool TAGS = false, bool ROWTHR = false, bool RFILT = false, class Est>
-__device__ __forceinline__ void keep_fragment_row(const Params &p, const Est &est, const float (&acc)[QT / 2], uint32_t r,
-                                                  uint32_t row, uint32_t rt, bool alive, bool flood, uint32_t it, uint32_t cbase,
-                                                  uint32_t q0, uint32_t nq, const float *tau, const float *qn, int *cnt,
-                                                  uint64_t *cand, float rthr = -INFINITY, const uint64_t *qtag = nullptr) {
+template <int QT, int CAP, bool BOUNDED, bool DUMP, bool TAGS = false, bool ROWTHR = false, bool RFILT = false, int NR, class Est>
+__device__ __forceinline__ void keep_fragment_rows(const Params &p, const Est (&est)[NR], const float (&acc)[2][QT / 2], uint32_t fr0,
+                                                   uint32_t alive, uint32_t row0, uint32_t rbase, bool flood, uint32_t it, uint32_t cbase,
+                                                   uint32_t q0, uint32_t nq, const float *tau, const float *qn, int *cnt, uint64_t *cand,
+                                                   const float (&rthr)[NR], const uint64_t *qtag = nullptr) {
     static_assert(!RFILT || (TAGS && ROWTHR), "the row-side filter is a mode of the filtered reverse scan");
-    float v[QT / 4];
+    if (DUMP) {  // tests only: score estimate and error bound per (row, query)
 #pragma unroll
-    for (int jj = 0; jj < QT / 4; ++jj) v[jj] = acc[(jj >> 1) * 4 + r * 2 + (jj & 1)];
-    if (DUMP && row < p.n) {  // tests only: score estimate and error bound per (row, query)
+        for (uint32_t ri = 0; ri < (uint32_t)NR; ++ri) {
+            const uint32_t fr = fr0 + ri, row = row0 + rbase + 64 * (fr >> 1) + 8 * (fr & 1);
+            if (row >= p.n) continue;
 #pragma unroll
-        for (int jj = 0; jj < QT / 4; ++jj) {
-            const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
-            if (qi >= nq) continue;
-            const float q = qn[qi];
-            float e = v[jj] * est.mul, b = est.bound(qi);
-            if (p.metric == NK_METRIC_EUCLIDEAN) { e -= fmaf(q, q, est.x2); b += EUC_EPS * fmaf(q, q, est.x2); }
-            p.dump_est[(size_t)row * p.dump_ld + q0 + qi] = e;
-            p.dump_bnd[(size_t)row * p.dump_ld + q0 + qi] = b;
+            for (int jj = 0; jj < QT / 4; ++jj) {
+                const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
+                if (qi >= nq) continue;
+                const float q = qn[qi];
+                float e = frag_at<QT>(acc, fr, jj) * est[ri].mul, b = est[ri].bound(qi);
+                if (p.metric == NK_METRIC_EUCLIDEAN) { e -= fmaf(q, q, est[ri].x2); b += EUC_EPS * fmaf(q, q, est[ri].x2); }
+                p.dump_est[(size_t)row * p.dump_ld + q0 + qi] = e;
+                p.dump_bnd[(size_t)row * p.dump_ld + q0 + qi] = b;
+            }
         }
     }
     if (flood && it < 2) {
         // Until the first prune (after this CTA's second tile) every threshold is -inf and EVERY (row, query) pair is
-        // buffered: no atomics, no register select.
-        const uint32_t slot = it * ROWS + rt;
-        const uint32_t grow = (uint32_t)(p.row_base + row);
-        uint32_t admit = ~0u;  // columns whose filter admits the row (a compact loop: the unrolled one below stays as it is)
-        if (TAGS) {
-            admit = 0u;
-            if (alive) {
-                const uint64_t tag = __ldg(p.row_tags + row);
+        // buffered: no atomics.
 #pragma unroll 1
-                for (uint32_t c = 0; c < (uint32_t)(QT / 4); ++c) {
-                    const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
-                    if (qi < nq && tag_admits(tag, p.qfilter + q0 + qi) && (!RFILT || tag_admits(qtag[qi], p.row_filter + row)))
-                        admit |= 1u << c;
+        for (uint32_t r = 0; r < (uint32_t)NR; ++r) {
+            const uint32_t ri = NR == 1 ? 0u : r;  // (one row: a constant, so the row's values stay compile-time selected)
+            const uint32_t fr = fr0 + ri, rt = rbase + 64 * (fr >> 1) + 8 * (fr & 1), row = row0 + rt;
+            const bool live = (alive >> ri) & 1u;
+            const Est e = pick_row(est, ri);
+            const uint32_t slot = it * ROWS + rt;
+            const uint32_t grow = (uint32_t)(p.row_base + row);
+            uint32_t admit = ~0u;  // columns whose filter admits the row
+            if (TAGS) {
+                admit = 0u;
+                if (live) {
+                    const uint64_t tag = __ldg(p.row_tags + row);
+#pragma unroll 1
+                    for (uint32_t c = 0; c < (uint32_t)(QT / 4); ++c) {
+                        const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
+                        if (qi < nq && tag_admits(tag, p.qfilter + q0 + qi) && (!RFILT || tag_admits(qtag[qi], p.row_filter + row)))
+                            admit |= 1u << c;
+                    }
+                }
+            }
+#pragma unroll
+            for (int jj = 0; jj < QT / 4; ++jj) {
+                const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
+                if (qi < nq) {
+                    float sc = e.upper(frag_at<QT>(acc, fr, jj), e.col(qi));
+                    if (sc != sc) sc = BOUNDED ? INFINITY : -INFINITY;
+                    const bool keep = live && sc >= p.min_score && ((admit >> jj) & 1u);
+                    cand[(size_t)qi * CAP + slot] = keep ? make_key(sc, grow) : 0ull;  // 0 = empty slot
                 }
             }
         }
+        return;
+    }
+    uint32_t pass[NR];
 #pragma unroll
-        for (int jj = 0; jj < QT / 4; ++jj) {
-            const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
-            if (qi < nq) {
-                float sc = est.upper(v[jj], qi);
-                if (sc != sc) sc = BOUNDED ? INFINITY : -INFINITY;
-                const bool keep = alive && sc >= p.min_score && ((admit >> jj) & 1u);
-                cand[(size_t)qi * CAP + slot] = keep ? make_key(sc, grow) : 0ull;  // 0 = empty slot
-            }
-        }
-    } else if (alive) {
-        uint32_t pass = 0;
+    for (int ri = 0; ri < NR; ++ri) pass[ri] = 0u;
 #pragma unroll
-        for (int jj = 0; jj < QT / 4; ++jj) {
-            const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
-            const float s0 = est.upper(v[jj], qi);
-            const float t = ROWTHR ? fmaxf(tau[qi], rthr) : tau[qi];
-            pass |= (!(s0 < t) && qi < nq) ? (1u << jj) : 0u;
+    for (int jj = 0; jj < QT / 4; ++jj) {
+        const uint32_t qi = cbase + 8 * (jj >> 1) + (jj & 1);
+        const typename Est::Col col = est[0].col(qi);
+        const float t = tau[qi];
+#pragma unroll
+        for (uint32_t ri = 0; ri < (uint32_t)NR; ++ri) {
+            const float s0 = est[ri].upper(frag_at<QT>(acc, fr0 + ri, jj), col);
+            const float tr = ROWTHR ? fmaxf(t, rthr[ri]) : t;
+            pass[ri] |= (!(s0 < tr) && qi < nq) ? (1u << jj) : 0u;
         }
-        if (TAGS && pass) {
+    }
+    uint32_t any = 0u;
+#pragma unroll
+    for (uint32_t ri = 0; ri < (uint32_t)NR; ++ri) {
+        if (!((alive >> ri) & 1u)) pass[ri] = 0u;
+        any |= pass[ri];
+    }
+    if (!any) return;
+#pragma unroll 1
+    for (uint32_t r = 0; r < (uint32_t)NR; ++r) {
+        const uint32_t ri = NR == 1 ? 0u : r;
+        uint32_t ps = pick_row(pass, ri);
+        if (!ps) continue;
+        const uint32_t fr = fr0 + ri, row = row0 + rbase + 64 * (fr >> 1) + 8 * (fr & 1);
+        const Est e = pick_row(est, ri);
+        const float rt = ROWTHR ? pick_row(rthr, ri) : -INFINITY;
+        if (TAGS) {
             const uint64_t tag = __ldg(p.row_tags + row);
-            uint32_t chk = pass;
+            uint32_t chk = ps;
 #pragma unroll 1
             while (chk) {
                 const uint32_t c = (uint32_t)__ffs((int)chk) - 1u;
                 chk &= chk - 1u;
-                if (!tag_admits(tag, p.qfilter + q0 + cbase + 8 * (c >> 1) + (c & 1))) pass &= ~(1u << c);
+                if (!tag_admits(tag, p.qfilter + q0 + cbase + 8 * (c >> 1) + (c & 1))) ps &= ~(1u << c);
             }
         }
-        if (RFILT && pass) {
+        if (RFILT && ps) {
             const NkFilter *rf = p.row_filter + row;
             const uint64_t all_of = __ldg(&rf->all_of), none_of = __ldg(&rf->none_of), any_of = __ldg(&rf->any_of);
-            uint32_t chk = pass;
+            uint32_t chk = ps;
 #pragma unroll 1
             while (chk) {
                 const uint32_t c = (uint32_t)__ffs((int)chk) - 1u;
                 chk &= chk - 1u;
-                if (!tag_admits(qtag[cbase + 8 * (c >> 1) + (c & 1)], all_of, none_of, any_of)) pass &= ~(1u << c);
+                if (!tag_admits(qtag[cbase + 8 * (c >> 1) + (c & 1)], all_of, none_of, any_of)) ps &= ~(1u << c);
             }
         }
 #pragma unroll 1
-        while (pass) {
-            const uint32_t c = (uint32_t)__ffs((int)pass) - 1u;
-            pass &= pass - 1u;
-            float val = 0.0f;
-#pragma unroll
-            for (uint32_t i = 0; i < (uint32_t)(QT / 4); ++i)  // the register file is not indexable: select by compare
-                if (c == i) val = v[i];
+        while (ps) {
+            const uint32_t c = (uint32_t)__ffs((int)ps) - 1u;
+            ps &= ps - 1u;
             const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
-            float sc = est.upper(val, qi);
+            float sc = e.upper(frag_value<QT>(acc, fr, c), e.col(qi));
             if (sc != sc) sc = BOUNDED ? INFINITY : -INFINITY;
-            if (sc >= (ROWTHR ? fmaxf(tau[qi], rthr) : tau[qi])) {
+            if (sc >= (ROWTHR ? fmaxf(tau[qi], rt) : tau[qi])) {
                 int pos = atomicAdd(&cnt[qi], 1);
                 if (pos < CAP) cand[(size_t)qi * CAP + pos] = make_key(sc, (uint32_t)(p.row_base + row));
                 else atomicExch(p.flags + FLAG_FATAL, 1);
