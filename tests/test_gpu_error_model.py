@@ -7,7 +7,8 @@ the tensor cores' fp32 accumulation — a constant round 1 only checked against 
 instantiation of the scan kernels writes (est, bnd) for every pair straight from the accumulator registers, and the test
 compares with the fp64 score on uniform, same-sign (no cancellation), huge / tiny scaled, sparse and heavy-cancellation
 data at d = 32 / 1024 / 4096: > 10^7 pairs per run.  The worst observed err / bnd is printed and must stay below 1 (it
-sits well below: the Cauchy-Schwarz bounds are loose by construction)."""
+sits well below: the Cauchy-Schwarz bounds are loose by construction).  An fp32 shard's image is pinned (NK_SHADOW):
+the BF16 shadow in the ("shadow", "f32") cases, the int8 image in its own test, d = 100 (not a multiple of 128) included."""
 import numpy as np
 import pytest
 
@@ -52,8 +53,19 @@ def _queries(rng, data, Q):
 
 @pytest.mark.parametrize("which,dtype", [("shadow", "f32"), ("filter", "f32"), ("shadow", "f16"), ("shadow", "bf16")])
 @pytest.mark.parametrize("d,n", [(32, 60_000), (1024, 40_000), (4096, 6000)])
-def test_filter_estimates_stay_inside_their_bounds(knn_lib, which, dtype, d, n, capsys):
+def test_filter_estimates_stay_inside_their_bounds(knn_lib, monkeypatch, which, dtype, d, n, capsys):
+    _check_bounds(monkeypatch, which, dtype, d, n, capsys, "bf16")
+
+
+@pytest.mark.parametrize("d,n", [(32, 60_000), (100, 40_000), (1024, 40_000), (4096, 6000)])
+def test_int8_image_estimates_stay_inside_their_bounds(knn_lib, monkeypatch, d, n, capsys):
+    _check_bounds(monkeypatch, "shadow", "f32", d, n, capsys, "int8")
+
+
+def _check_bounds(monkeypatch, which, dtype, d, n, capsys, image):
+    """image: the image of an fp32 shard the shadow dump reads (NK_SHADOW, read at index creation)"""
     from nornicdb_b200.knn import KnnIndex, from_bf16_bits, to_bf16_bits
+    monkeypatch.setenv("NK_SHADOW", image)
     rng = np.random.default_rng(d * 7 + n)
     Q = 64
     worst, pairs = {}, 0
@@ -88,6 +100,6 @@ def test_filter_estimates_stay_inside_their_bounds(knn_lib, which, dtype, d, n, 
             pairs += est.size
     top = sorted(worst.items(), key=lambda t: -t[1])[:3]
     with capsys.disabled():
-        print(f"\n[error model] {which}/{dtype} d={d}: {pairs:.3g} pairs, worst err/bound = {top[0][1]:.3f} "
+        print(f"\n[error model] {which}/{dtype}{'/' + image if (which, dtype) == ('shadow', 'f32') else ''} d={d}: {pairs:.3g} pairs, worst err/bound = {top[0][1]:.3f} "
               f"({top[0][0][0]}, {top[0][0][1]}); next {[(k[0], k[1], round(v, 3)) for k, v in top[1:]]}")
     assert top[0][1] < 1.0
