@@ -330,7 +330,7 @@ int assign_tensor(const DeviceInfo &di, const float *rows, const RowImage &img, 
         pp.acc_c = acc_c; pp.qnorm = qn; pp.qa = qa; pp.qb = qb;
         if (s8) { pp.qs8 = reinterpret_cast<int8_t *>(buf + off_q); pp.qscale = qsc; }
         else pp.qbf = reinterpret_cast<uint16_t *>(buf + off_q);
-        if (launch_prep(di, pp, stream, launches)) { rc = -1; break; }
+        if (launch_prep(di, a.mode, pp, stream, launches)) { rc = -1; break; }
         assign_mark_nonfinite_kernel<<<(K + 7) / 8, 256, 0, stream>>>(centroids_dev, K, dim, qb);
         CUtensorMap map_rows, map_q;
         if (tc_make_map(&map_rows, img.data, n, img.stride, esz, 128 / esz, ROWS, img.row_bytes())) { rc = -1; break; }

@@ -385,7 +385,7 @@ static nk::ScanArgs shard_scan_args(const NkIndex *ix, const NkShard &s, const f
     a.rows = s.rows; a.dtype = ix->dtype; a.n = (uint32_t)s.n; a.dim = ix->dim; a.row_base = s.base;
     a.queries = q_dev; a.Q = Q; a.k = k; a.metric = ix->metric; a.stream = stream;
     a.row_mask = s.mask_on ? s.mask : nullptr; a.min_score = ix->key_floor();
-    if (qfilter) { a.row_tags = s.tags; a.qfilter = qfilter; }
+    if (qfilter) { a.row_tags = s.tags; a.qfilter = qfilter; a.mode = nk::ScanMode::KNN_TAGS; }
     return a;
 }
 
@@ -1493,7 +1493,9 @@ static int range_shard(NkIndex *ix, NkShard &s, const RangeBlock &b, uint64_t fr
     nk::ScanArgs a = shard_scan_args(ix, s, s.ws.queries, b.Q, 1, s.stream, b.filtered ? s.ws.qfilter : nullptr);
     const int use = plan_path(ix, s, b.path, true, &a);
     if (use < 0) return -1;
+    a.mode = b.filtered ? nk::ScanMode::RANGE_TAGS : nk::ScanMode::RANGE;
     if (b.reverse) {
+        a.mode = b.row_filters ? nk::ScanMode::REVERSE_RFILT : b.filtered ? nk::ScanMode::REVERSE_TAGS : nk::ScanMode::REVERSE;
         a.row_thr = s.ws.row_thr;
         a.row_mask = reinterpret_cast<const uint32_t *>(s.ws.row_thr + s.n);
         if (b.row_filters) { a.row_filter = s.ws.row_filter; a.qtags = s.ws.qtags; }

@@ -75,6 +75,24 @@ struct RowImage {
     }
 };
 
+// What a scan keeps and which filters it applies: the 8 kinds of scan.  ScanArgs::mode is set where the pointers it reads
+// are attached (ScanArgs::check holds the two together); the tensor-core scan kernels take it as a template argument.
+//   KNN, KNN_TAGS           the k best rows per query: running thresholds, shared between CTAs; full buffers are pruned
+//   RANGE, RANGE_TAGS       every row that reaches a fixed per-query threshold: full buffers are flushed to the lists
+//   REVERSE, REVERSE_TAGS   the graph update's reverse scan: a range scan whose pairs must also reach their row's threshold (row_thr)
+//   REVERSE_RFILT           ... of a filtered graph: the row's own filter (row_filter) must also admit the query's tag (qtags)
+//   DUMP                    tests only (scan_filter_dump): a kNN filter pass that also writes every pair's estimate and bound
+// The *_TAGS modes and REVERSE_RFILT apply per-query tag filters (row_tags, qfilter): a pair takes part only if the query
+// admits the row's tag.  The range modes (RANGE .. REVERSE_RFILT) and the reverse modes (REVERSE ..) are contiguous.
+enum class ScanMode { KNN, KNN_TAGS, RANGE, RANGE_TAGS, REVERSE, REVERSE_TAGS, REVERSE_RFILT, DUMP };
+__host__ __device__ constexpr bool mode_tags(ScanMode m) {
+    return m == ScanMode::KNN_TAGS || m == ScanMode::RANGE_TAGS || m == ScanMode::REVERSE_TAGS || m == ScanMode::REVERSE_RFILT;
+}
+__host__ __device__ constexpr bool mode_range(ScanMode m) { return m >= ScanMode::RANGE && m <= ScanMode::REVERSE_RFILT; }
+__host__ __device__ constexpr bool mode_row_thr(ScanMode m) { return m >= ScanMode::REVERSE && m <= ScanMode::REVERSE_RFILT; }
+__host__ __device__ constexpr bool mode_row_filter(ScanMode m) { return m == ScanMode::REVERSE_RFILT; }
+__host__ __device__ constexpr bool mode_dump(ScanMode m) { return m == ScanMode::DUMP; }
+
 struct ScanArgs {
     const void *rows = nullptr;  // [n x dim] row-major, fp32 or fp16
     int dtype = NK_DTYPE_F32;
@@ -97,9 +115,9 @@ struct ScanArgs {
     // optional row filter (label / tombstone bitmask): bit r (LSB first in 32-bit words) set = local row r takes part;
     // nullptr = every row.  Honoured by every scan kernel.
     const uint32_t *row_mask = nullptr;
-    // optional per-query tag filters (nk_search_filtered): row_tags [n] (local rows) and qfilter [Q]; a (row, query) pair
-    // takes part only if tag_admits(row_tags[row], qfilter + q).  Both set or both nullptr; kernels that see them are the
-    // filtered (TAGS) instantiations, so unfiltered searches run unchanged code.
+    ScanMode mode = ScanMode::KNN;
+    // the tag modes (mode_tags): per-query tag filters, row_tags [n] (local rows) and qfilter [Q]; a (row, query) pair takes
+    // part only if tag_admits(row_tags[row], qfilter + q).  Unfiltered searches run kernels without the filter code.
     const uint64_t *row_tags = nullptr;
     const NkFilter *qfilter = nullptr;
     RowImage image;  // what the 16-bit / int8 pass streams; kind NONE = no such pass
@@ -112,14 +130,16 @@ struct ScanArgs {
     // filter paths: do not queue the retry / exact stages; the (host-synchronous) caller inspects the status words and
     // calls scan_tensor_filter_tail only when a stage overflowed
     bool defer_tail = false;
-    // range mode only, the reverse scan of nk_knn_graph_update: key-space threshold per local row [n]; a (row, query) pair is
-    // listed only if it reaches both the query's threshold and the row's (tensor-core filters, ROWTHR instantiations)
+    // the reverse modes (mode_row_thr): key-space threshold per local row [n]; a (row, query) pair is listed only if it
+    // reaches both the query's threshold and the row's
     const float *row_thr = nullptr;
-    // with row_thr, a filtered graph's reverse scan: row_filter [n] (local rows) and qtags [Q]; a (row, query) pair is also
-    // listed only if tag_admits(qtags[q], row_filter + row), the mirror image of row_tags / qfilter.  Needs qfilter as well
-    // (the ROWTHR + TAGS + RFILT instantiations).
+    // REVERSE_RFILT: row_filter [n] (local rows) and qtags [Q]; a (row, query) pair is also listed only if
+    // tag_admits(qtags[q], row_filter + row), the mirror image of row_tags / qfilter
     const NkFilter *row_filter = nullptr;
     const uint64_t *qtags = nullptr;
+    // 0 if a range (else kNN) scan, on the CUDA cores (no reverse modes) or not, serves the mode and exactly the pointers the
+    // mode reads are set; else set_error and -1.  No scan accepts DUMP: scan_filter_dump sets it on its own copy.
+    int check(bool range, bool cuda_cores) const;
 };
 
 // Fused distance + top-k scan on CUDA cores (small Q, any dim / dtype / alignment).

@@ -211,6 +211,7 @@ int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const
                      int *counts, uint32_t *list_cap_out, int *retried, const uint64_t *pair_first) {
     const uint32_t Q = a.Q, QA = range_qa(Q);
     *retried = 0;
+    if (a.check(true, !tensor)) return -1;
     if (ws_reserve((void **)&ws.keys2, &ws.keys2_bytes, (size_t)(2 * QA + 2 * Q) * 4 + (size_t)(Q + 1) * 8)) return -1;
     uint32_t list_cap = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(LIST0, ws.partial_bytes / ((size_t)Q * 8)), 0x7fffffffu);
     std::vector<int> fill(Q);
@@ -243,16 +244,15 @@ int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const
     rp.rows = a.rows; rp.dtype = a.dtype; rp.dim = a.dim; rp.row_base = a.row_base; rp.metric = a.metric; rp.queries = a.queries;
     rp.lists = ws.partial; rp.list_cap = list_cap; rp.fill = ws_fill(ws, Q); rp.thr = ws_thr(ws); rp.count = ws_count(ws, Q);
     rp.rescore = tensor ? 1 : 0; rp.row_thr = a.row_thr;
-    if (a.row_thr && !tensor) { set_error("internal: the per-row threshold scan runs on the tensor-core filters only"); return -1; }
     const size_t smem = tensor ? (size_t)a.dim * 4 : 0;
-    const void *kern = a.row_thr ? reinterpret_cast<const void *>(range_rescore_reverse_kernel)
+    const void *kern = mode_row_thr(a.mode) ? reinterpret_cast<const void *>(range_rescore_reverse_kernel)
                        : pair_first ? reinterpret_cast<const void *>(range_rescore_pairs_kernel) : reinterpret_cast<const void *>(range_rescore_kernel);
     if (smem > 48 * 1024 && tc_ensure_smem(kern, di.device_id, smem)) return -1;
     if (longest > 0)
         for (uint32_t q0 = 0; q0 < Q; q0 += MAX_GRID_Y) {
             rp.q_base = q0;
             const dim3 grid((longest + RS_ENTRIES - 1) / RS_ENTRIES, std::min(MAX_GRID_Y, Q - q0));
-            if (a.row_thr) range_rescore_reverse_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp);
+            if (mode_row_thr(a.mode)) range_rescore_reverse_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp);
             else if (pair_first) range_rescore_pairs_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp, *pair_first);
             else range_rescore_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp);
             NK_CUDA_OK(cudaGetLastError());

@@ -50,6 +50,14 @@ int fatal_overflow(int flag, int *flags, cudaStream_t stream) {
     return -1;
 }
 
+int ScanArgs::check(bool range, bool cuda_cores) const {
+    if (!mode_dump(mode) && mode_range(mode) == range && !(cuda_cores && mode_row_thr(mode)) && mode_tags(mode) == (qfilter != nullptr) &&
+        mode_row_thr(mode) == (row_thr != nullptr) && mode_row_filter(mode) == (row_filter != nullptr) && mode_row_filter(mode) == (qtags != nullptr))
+        return 0;
+    set_error("internal: scan mode %d does not fit this %s scan (%s) or its pointers", (int)mode, range ? "range" : "kNN", cuda_cores ? "CUDA cores" : "tensor");
+    return -1;
+}
+
 int query_device_info(int device_id, DeviceInfo *out) {
     cudaDeviceProp prop;
     NK_CUDA_OK(cudaGetDeviceProperties(&prop, device_id));

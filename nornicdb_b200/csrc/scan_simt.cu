@@ -318,7 +318,6 @@ __global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtArgs<RA
 
 // ---------------------------------------------------------------------------------------------
 template <bool RANGE> using SimtKernelT = void (*)(SimtArgs<RANGE>);
-typedef SimtKernelT<false> SimtKernel;
 
 template <typename T, bool VEC, bool EUCLID, bool TAGS, bool RANGE>
 static SimtKernelT<RANGE> pick_qt(int qt) {
@@ -350,11 +349,10 @@ static SimtKernelT<RANGE> pick_kernel_t(int dtype, bool vec, bool euclid, int qt
     if (vec) return euclid ? pick_qt<float, true, true, TAGS, RANGE>(qt) : pick_qt<float, true, false, TAGS, RANGE>(qt);
     return euclid ? pick_qt<float, false, true, TAGS, RANGE>(qt) : pick_qt<float, false, false, TAGS, RANGE>(qt);
 }
-static SimtKernel pick_kernel(int dtype, bool vec, bool euclid, int qt, bool tags) {
-    return tags ? pick_kernel_t<true, false>(dtype, vec, euclid, qt) : pick_kernel_t<false, false>(dtype, vec, euclid, qt);
-}
-static SimtKernelT<true> pick_range_kernel(int dtype, bool vec, bool euclid, int qt, bool tags) {
-    return tags ? pick_kernel_t<true, true>(dtype, vec, euclid, qt) : pick_kernel_t<false, true>(dtype, vec, euclid, qt);
+// The kernel of a scan in the mode a.mode: a kNN mode (RANGE = false) or a range mode (RANGE = true), as ScanArgs::check found.
+template <bool RANGE> static SimtKernelT<RANGE> pick_kernel(const ScanArgs &a, bool vec, int qt) {
+    const bool euclid = a.metric == NK_METRIC_EUCLIDEAN;
+    return mode_tags(a.mode) ? pick_kernel_t<true, RANGE>(a.dtype, vec, euclid, qt) : pick_kernel_t<false, RANGE>(a.dtype, vec, euclid, qt);
 }
 
 // cudaFuncSetAttribute + occupancy query once per (kernel, device, smem) instead of once per search
@@ -389,6 +387,7 @@ int simt_cap_for_k(uint32_t k) {
 }
 
 int scan_simt(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *out_keys, uint64_t *launches) {
+    if (a.check(false, true)) return -1;
     if (a.n == 0 || a.Q == 0 || a.k == 0) return 0;
     if (a.k > NK_MAX_K) {
         set_error("k=%u exceeds NK_MAX_K=%u", a.k, NK_MAX_K);
@@ -397,7 +396,6 @@ int scan_simt(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *
     const size_t esz = a.dtype == NK_DTYPE_F32 ? 4 : 2;
     const uint32_t vec_elems = a.dtype == NK_DTYPE_F32 ? 4 : 8;
     const bool vec = (a.dim % vec_elems == 0) && ((reinterpret_cast<uintptr_t>(a.rows) & 15) == 0);
-    const bool euclid = a.metric == NK_METRIC_EUCLIDEAN;
     const int P = simt_cap_for_k(a.k);
     const size_t smem_budget = 96 * 1024;  // keeps >= 2 CTAs per SM
     const uint32_t num_iv = (a.n + SIMT_RT - 1) / SIMT_RT;
@@ -417,7 +415,7 @@ int scan_simt(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *
             set_error("dim=%u too large for the SIMT scan (needs %zu B shared memory)", a.dim, smem);
             return -1;
         }
-        SimtKernel kern = pick_kernel(a.dtype, vec, euclid, qt, a.qfilter != nullptr);
+        const auto kern = pick_kernel<false>(a, vec, qt);
         if (simt_ensure(reinterpret_cast<const void *>(kern), di.device_id, smem)) return -1;
         int occ = simt_occupancy(reinterpret_cast<const void *>(kern), di.device_id, smem);
         // One grid for every query group of this search so the per-CTA partial lists line up.
@@ -467,7 +465,7 @@ int scan_simt_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint
             set_error("dim=%u too large for the SIMT scan (needs %zu B shared memory)", a.dim, smem);
             return -1;
         }
-        SimtKernelT<true> kern = pick_range_kernel(a.dtype, vec, a.metric == NK_METRIC_EUCLIDEAN, qt, a.qfilter != nullptr);
+        const auto kern = pick_kernel<true>(a, vec, qt);
         if (simt_ensure(reinterpret_cast<const void *>(kern), di.device_id, smem)) return -1;
         const int occ = simt_occupancy(reinterpret_cast<const void *>(kern), di.device_id, smem);
         uint32_t grid = (uint32_t)di.num_sms * (uint32_t)occ;

@@ -306,12 +306,8 @@ template <bool FILTER> struct Tf32Est {
     __device__ __forceinline__ float bound(uint32_t qi) const { return bnd * qn[qi]; }
 };
 
-// TAGS: filtered search (per-query tag filters in the keep rule); the unfiltered instantiations are TAGS = false.
-// RANGE (filter mode only, nk_search_range): fixed per-query thresholds; full buffers are flushed to the lists, never pruned.
-// ROWTHR (with RANGE, the reverse scan of nk_knn_graph_update): a pair must also reach its row's threshold p.row_thr[row].
-// RFILT (with ROWTHR and TAGS, a filtered graph): the row's own filter must also admit the query's tag (keep_fragment_rows);
-// the launch's query tags are staged in shared memory past Shared.
-template <int NT, int QT, bool DUMP, bool TAGS, bool RANGE = false, bool ROWTHR = false, bool RFILT = false>
+// M: the scan mode (kernels.cuh).  REVERSE_RFILT stages the launch's query tags in shared memory past Shared.
+template <int NT, int QT, ScanMode M>
 __global__ void __launch_bounds__(tc::THREADS, 1)
 knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_qhi,
                    const __grid_constant__ CUtensorMap map_qlo, tc::Params p) {
@@ -351,8 +347,8 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
         sh.cnt[tid] = 0;
         sh.qn[tid] = (FILTER && p.qnorm) ? p.qnorm[qpad_off + tid] : 1.0f;
     }
-    uint64_t *qtag = reinterpret_cast<uint64_t *>(smem_raw + (size_t)C::RING_BYTES + sizeof(Shared));  // RFILT only
-    if (RFILT && tid < QT) qtag[tid] = (uint32_t)tid < nq ? p.qtags[q0 + tid] : 0ull;
+    uint64_t *qtag = reinterpret_cast<uint64_t *>(smem_raw + (size_t)C::RING_BYTES + sizeof(Shared));  // REVERSE_RFILT only
+    if (mode_row_filter(M) && tid < QT) qtag[tid] = (uint32_t)tid < nq ? p.qtags[q0 + tid] : 0ull;
     __syncthreads();
     const bool flood = !(FILTER && p.presampled);  // first two tiles: every (row, query) pair is placed directly
     uint64_t *my_cand = p.cand + (size_t)blockIdx.x * QT * P;
@@ -474,17 +470,17 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
                     if (!cosine && alive && e.x2 < INFINITY && (lane & 3) == 0) atomicMax(&sh.maxxx, __float_as_uint(e.x2));  // NaN / Inf rows: kept, judged exactly
                     if (euclid) e.mul = 2.0f;
                 }
-                const float rthr[1] = {ROWTHR && row < p.n ? __ldg(p.row_thr + row) : -INFINITY};
-                keep_fragment_rows<QT, P, FILTER, DUMP && FILTER, TAGS, ROWTHR, RFILT>(p, est, acc, ri, alive ? 1u : 0u, tile * ROWS, rbase, flood, it,
-                                                                                 cbase, q0, nq, sh.tau, sh.qn, sh.cnt, my_cand, rthr, qtag);
+                const float rthr[1] = {mode_row_thr(M) && row < p.n ? __ldg(p.row_thr + row) : -INFINITY};
+                keep_fragment_rows<QT, P, FILTER, M>(p, est, acc, ri, alive ? 1u : 0u, tile * ROWS, rbase, flood, it, cbase, q0, nq, sh.tau, sh.qn,
+                                                     sh.cnt, my_cand, rthr, qtag);
             }
             // prune any buffer that could overflow during the next tile; the 8 consumer warps prune different
             // queries concurrently with a register-resident warp selection
             group_sync(EPI_BAR, EPI_THREADS);  // every push of this tile is visible
-            if constexpr (RANGE) flush_tile<P>(p, q0, nq, ewarp, lane, my_cand, sh.cnt);
+            if constexpr (mode_range(M)) flush_tile<P>(p, q0, nq, ewarp, lane, my_cand, sh.cnt);
             else prune_tile<FILTER>(p, q0, nq, ewarp, lane, sh.cnt, sh.tau, prune_at, prune_at, flood && it == 0, prune);
             group_sync(EPI_BAR, EPI_THREADS);
-            if (FILTER && !RANGE) adopt_shared_tau(p, q0, nq, tid - EPI_WARP0 * 32, sh.tau);
+            if (FILTER && !mode_range(M)) adopt_shared_tau(p, q0, nq, tid - EPI_WARP0 * 32, sh.tau);
         }
     }
 
@@ -492,7 +488,7 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
     // Every role has finished its tile loop here, so all 12 warps share the final prunes.
     __syncthreads();
     for (uint32_t qi = warp; qi < nq; qi += THREADS / 32) {
-        if (RANGE)
+        if (mode_range(M))
             flush_query(p, q0, qi, lane, my_cand + (size_t)qi * P, sh.cnt);
         else if (FILTER)
             emit_query(p, q0, qi, lane, my_cand + (size_t)qi * P, sh.cnt, sh.tau, prune);
@@ -884,7 +880,7 @@ int tc_debug_flags() { return tc_env_int("NK_TC_DEBUG", 0); }
 tc::Params pass_params(const ScanArgs &a, Workspace &ws, const tc::PassArgs &t) {
     tc::Params p{};
     p.n = a.n; p.dim = a.dim; p.row_base = a.row_base;
-    p.q0 = t.q0; p.nq = t.nq; p.k = a.k; p.qpad_off = t.q0; p.qgroups = t.qgroups; p.list_cap = t.range ? t.list_cap : t.grid * t.k_emit;
+    p.q0 = t.q0; p.nq = t.nq; p.k = a.k; p.qpad_off = t.q0; p.qgroups = t.qgroups; p.list_cap = mode_range(a.mode) ? t.list_cap : t.grid * t.k_emit;
     p.metric = a.metric; p.k_emit = t.k_emit; p.qnorm = t.qnorm;
     p.cand = ws.cand; p.partial = ws.partial; p.flags = ws.flags; p.debug = tc_debug_flags(); p.mask = a.row_mask;
     p.gtau = reinterpret_cast<uint32_t *>(ws.keys2); p.gcount = reinterpret_cast<int *>(ws.keys2) + (t.Qpad + tc::QT_BIG);
@@ -924,13 +920,11 @@ PrepParams prep_params(const ScanArgs &a, uint32_t Qpad, uint32_t dimpad) {
     return pp;
 }
 
-int launch_prep(const DeviceInfo &di, const PrepParams &pp, cudaStream_t stream, uint64_t *launches) {
+int launch_prep(const DeviceInfo &di, ScanMode mode, const PrepParams &pp, cudaStream_t stream, uint64_t *launches) {
     const size_t smem = (size_t)((pp.dim + 3) & ~3u) * 4 + (size_t)pp.sample * 8;
-    const bool tags = pp.qfilter != nullptr;
-    const void *kern = tags ? reinterpret_cast<const void *>(filter_prep_kernel<true>) : reinterpret_cast<const void *>(filter_prep_kernel<false>);
-    if (smem > 48 * 1024 && tc_ensure_smem(kern, di.device_id, smem)) return -1;
-    if (tags) filter_prep_kernel<true><<<pp.Qpad, PREP_THREADS, smem, stream>>>(pp);
-    else filter_prep_kernel<false><<<pp.Qpad, PREP_THREADS, smem, stream>>>(pp);
+    void (*kern)(PrepParams) = mode_tags(mode) ? filter_prep_kernel<true> : filter_prep_kernel<false>;
+    if (smem > 48 * 1024 && tc_ensure_smem(reinterpret_cast<const void *>(kern), di.device_id, smem)) return -1;
+    kern<<<pp.Qpad, PREP_THREADS, smem, stream>>>(pp);
     NK_CUDA_OK(cudaGetLastError());
     if (launches) ++*launches;
     return 0;
@@ -943,7 +937,7 @@ struct TcPassArgs : tc::PassArgs {
     const int *only_if;
     bool count_main;
 };
-template <int NT, int QT, bool DUMP = false, bool TAGS = false, bool RANGE = false, bool ROWTHR = false, bool RFILT = false>
+template <int NT, int QT, ScanMode M>
 static int launch_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const TcPassArgs &t, uint64_t *launches) {
     using namespace tc;
     const CUtensorMap *map_rows = tc_cached_map(ws, 0, a.rows, a.n, a.dim, 4, (uint32_t)BK, ROWS, (uint64_t)a.dim * 4);
@@ -951,42 +945,33 @@ static int launch_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws,
     const CUtensorMap *map_qhi = tc_cached_map(ws, QT == 64 ? 1 : 2, t.qhi, t.Qpad, a.dim, 4, (uint32_t)BK, QT, (uint64_t)a.dim * 4);
     const CUtensorMap *map_qlo = NT == 3 ? tc_cached_map(ws, 3, t.qlo, t.Qpad, a.dim, 4, (uint32_t)BK, QT, (uint64_t)a.dim * 4) : map_qhi;
     if (!map_rows || !map_qhi || !map_qlo) return -1;
-    const size_t smem = (size_t)Cfg<NT, QT>::RING_BYTES + sizeof(Shared) + (RFILT ? QT * sizeof(uint64_t) : 0) + 1024;
+    const size_t smem = (size_t)Cfg<NT, QT>::RING_BYTES + sizeof(Shared) + (mode_row_filter(M) ? QT * sizeof(uint64_t) : 0) + 1024;
     if (smem > di.max_smem_optin) {
         set_error("tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;
     }
-    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_tc_kernel<NT, QT, DUMP, TAGS, RANGE, ROWTHR, RFILT>), di.device_id, smem))
+    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_tc_kernel<NT, QT, M>), di.device_id, smem))
         return -1;
     Params p = pass_params(a, ws, t);
     p.nslab = (a.dim + BK - 1) / BK; p.margin_c = t.margin_c; p.only_if = t.only_if;
     // (asynchronous API: the early-exit retry / exact stages are programmatic dependents — their launch overlaps the kernel
     // before them.  Not for the host-synchronous API: measured 5-15 us slower per nk_search, the copy-out behind it waits longer)
-    NK_CUDA_OK(launch_pdl(knn_scan_tc_kernel<NT, QT, DUMP, TAGS, RANGE, ROWTHR, RFILT>, dim3(t.grid), dim3(THREADS), smem, a.stream, t.only_if != nullptr && !a.defer_tail, *map_rows, *map_qhi,
+    NK_CUDA_OK(launch_pdl(knn_scan_tc_kernel<NT, QT, M>, dim3(t.grid), dim3(THREADS), smem, a.stream, t.only_if != nullptr && !a.defer_tail, *map_rows, *map_qhi,
                           *map_qlo, p));
     if (launches) ++*launches;
     if (t.count_main && a.main_launches) ++*a.main_launches;
     return 0;
 }
-// Filtered searches (per-query tag filters) run the TAGS instantiation of the same kernel; range searches the RANGE one, and
-// the reverse scan of nk_knn_graph_update (per-row thresholds) the ROWTHR one, and that of a filtered graph (each row's own
-// filter, which needs the per-query filters too) the ROWTHR + RFILT one.
-template <int NT, int QT, bool DUMP = false>
+// One pass in the mode a.mode.  The exact 3xTF32 kernel serves the kNN modes only; the dump mode exists at QT = 64 only.
+template <int NT, int QT>
 static int launch_pass(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const TcPassArgs &t, uint64_t *launches) {
-    if constexpr (NT == 1 && !DUMP)
-        if (t.range && a.row_thr && a.row_filter) {
-            if (!a.qfilter || !a.qtags) { set_error("internal: the row-filtered reverse scan needs per-query filters and tags"); return -1; }
-            return launch_pass_t<NT, QT, false, true, true, true, true>(di, a, ws, t, launches);
-        }
-    if constexpr (NT == 1 && !DUMP)
-        if (t.range && a.row_thr)
-            return a.qfilter ? launch_pass_t<NT, QT, false, true, true, true>(di, a, ws, t, launches)
-                             : launch_pass_t<NT, QT, false, false, true, true>(di, a, ws, t, launches);
-    if constexpr (NT == 1 && !DUMP)
-        if (t.range)
-            return a.qfilter ? launch_pass_t<NT, QT, false, true, true>(di, a, ws, t, launches) : launch_pass_t<NT, QT, false, false, true>(di, a, ws, t, launches);
-    if (!DUMP && a.qfilter) return launch_pass_t<NT, QT, false, true>(di, a, ws, t, launches);
-    return launch_pass_t<NT, QT, DUMP, false>(di, a, ws, t, launches);
+    return tc::with_scan_mode(a.mode, [&](auto mode) {
+        constexpr ScanMode M = decltype(mode)::value;
+        if constexpr ((NT == 1 || M == ScanMode::KNN || M == ScanMode::KNN_TAGS) && (QT == 64 || !mode_dump(M)))
+            return launch_pass_t<NT, QT, M>(di, a, ws, t, launches);
+        set_error("internal: no %s kernel for scan mode %d at %d query columns", NT == 3 ? "3xTF32" : "TF32 filter", (int)M, QT);
+        return -1;
+    });
 }
 
 static void fin_print_prof(cudaStream_t stream, uint32_t Q) {
@@ -1110,7 +1095,7 @@ static int scan_tensor_exact(const DeviceInfo &di, const ScanArgs &a, Workspace 
     if (prep) {
         PrepParams pp = prep_params(a, Qpad, a.dim);
         pp.qhi = qhi; pp.qlo = qlo; pp.only_if = only_if;
-        if (launch_prep(di, pp, a.stream, launches)) return -1;
+        if (launch_prep(di, a.mode, pp, a.stream, launches)) return -1;
     }
     if (count_main && a.ev_begin) NK_CUDA_OK(cudaEventRecord(a.ev_begin, a.stream));
     for (uint32_t q0 = 0; q0 < a.Q; q0 += 64) {
@@ -1201,6 +1186,7 @@ int scan_tensor_filter_tail(const DeviceInfo &di, const ScanArgs &a, Workspace &
 // rescoring, decode).  Three launches in the common case; the retry / exact stages follow as scan_tensor_filter_tail.
 int scan_tensor_filter(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *out_keys, uint64_t *launches) {
     using namespace tc;
+    if (a.check(false, false)) return -1;
     if (a.n == 0 || a.Q == 0 || a.k == 0) return 0;
     if (!scan_tensor_filter_supported(di, a)) {
         set_error("tensor filter path: unsupported shape");
@@ -1212,7 +1198,7 @@ int scan_tensor_filter(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, u
 
     PrepParams pp = filter_prep_params(a, ws, f);
     pp.qlo = f.can_exact_tc ? f.qlo : nullptr;
-    if (launch_prep(di, pp, a.stream, launches)) return -1;
+    if (launch_prep(di, a.mode, pp, a.stream, launches)) return -1;
 
     if (a.ev_begin) NK_CUDA_OK(cudaEventRecord(a.ev_begin, a.stream));
     if (plan_launches(0, q_big, f.grid, f.max_groups_shadow, [&](uint32_t qt, uint32_t q0, uint32_t nq, uint32_t groups) {
@@ -1252,20 +1238,20 @@ int scan_tensor_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, ui
     PrepParams pp = filter_prep_params(b, ws, f);
     pp.state = nullptr;  // the thresholds and list fills are the caller's
     pp.sample = 0;
-    if (launch_prep(di, pp, a.stream, launches)) return -1;
+    if (launch_prep(di, a.mode, pp, a.stream, launches)) return -1;
     if (a.ev_begin) NK_CUDA_OK(cudaEventRecord(a.ev_begin, a.stream));
     int rc;
     if (f.big) {
         rc = plan_launches(0, a.Q, f.grid, 4, [&](uint32_t qt, uint32_t q0, uint32_t nq, uint32_t groups) {
             ShadowPassArgs sp = f.shadow_pass();
-            sp.q0 = q0; sp.nq = nq; sp.qgroups = groups; sp.presampled = 1; sp.range = true; sp.list_cap = list_cap;
+            sp.q0 = q0; sp.nq = nq; sp.qgroups = groups; sp.presampled = 1; sp.list_cap = list_cap;
             return launch_shadow_pass((int)qt, di, b, ws, sp, launches);
         });
     } else {
         rc = plan_launches(0, a.Q, f.grid, 4, [&](uint32_t qt, uint32_t q0, uint32_t nq, uint32_t groups) {
             TcPassArgs t{};
             t.grid = f.grid; t.k_emit = f.k_emit; t.Qpad = f.Qpad; t.q0 = q0; t.nq = nq; t.qgroups = groups; t.margin_c = f.margin_tf32;
-            t.qhi = f.qhi; t.qnorm = f.qnorm; t.count_main = true; t.presampled = 1; t.range = true; t.list_cap = list_cap;
+            t.qhi = f.qhi; t.qnorm = f.qnorm; t.count_main = true; t.presampled = 1; t.list_cap = list_cap;
             return qt == 128 ? launch_pass<1, 128>(di, b, ws, t, launches) : launch_pass<1, 64>(di, b, ws, t, launches);
         });
     }
@@ -1283,7 +1269,7 @@ int scan_filter_dump(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, int
     using namespace tc;
     if (a.Q == 0 || a.Q > 64 || a.n == 0) { set_error("dump: 1 <= Q <= 64 and n > 0 required"); return -1; }
     ScanArgs b = a;
-    b.k = 1; b.min_score = -INFINITY; b.defer_tail = true; b.out_idx = nullptr; b.out_score = nullptr;
+    b.k = 1; b.min_score = -INFINITY; b.defer_tail = true; b.out_idx = nullptr; b.out_score = nullptr; b.mode = ScanMode::DUMP;
     if (!scan_tensor_filter_supported(di, b)) { set_error("dump: unsupported shape"); return -1; }
     FilterPlan f;
     if (make_filter_plan(di, b, ws, &f)) return -1;
@@ -1291,7 +1277,7 @@ int scan_filter_dump(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, int
     if (which == NK_PATH_TENSOR_FILTER && a.dtype != NK_DTYPE_F32) { set_error("dump: TF32 pass needs fp32 rows"); return -1; }
     PrepParams pp = filter_prep_params(b, ws, f);
     pp.sample = 0;
-    if (launch_prep(di, pp, b.stream, launches)) return -1;
+    if (launch_prep(di, b.mode, pp, b.stream, launches)) return -1;
     if (which == NK_PATH_TENSOR_SHADOW) {
         ShadowPassArgs sp = f.shadow_pass();
         sp.q0 = 0; sp.nq = b.Q; sp.qgroups = 1; sp.presampled = 0;
@@ -1301,7 +1287,7 @@ int scan_filter_dump(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, int
         TcPassArgs t{};
         t.grid = f.grid; t.k_emit = f.k_emit; t.Qpad = f.Qpad; t.q0 = 0; t.nq = b.Q; t.qgroups = 1; t.margin_c = f.margin_tf32;
         t.qhi = f.qhi; t.qnorm = f.qnorm; t.dump_est = est; t.dump_bnd = bnd; t.dump_ld = ld;
-        if (launch_pass<1, 64, true>(di, b, ws, t, launches)) return -1;
+        if (launch_pass<1, 64>(di, b, ws, t, launches)) return -1;
     }
     return 0;
 }

@@ -224,14 +224,10 @@ struct Bf16Est {
     __device__ __forceinline__ float bound(uint32_t qi) const { return fmaf(ra, qa[qi], rb * qb[qi]); }
 };
 
-// TAGS: filtered search (per-query tag filters in the keep rule, read through the read-only cache: the shared-memory budget
-// is spent on the rings); the unfiltered instantiations are TAGS = false.  OP: the operand type, bf16 (BF16 shadow, bf16
-// corpora), fp16 (an fp16 corpus scanned in place) or int8 (the int8 image of an fp32 shard).  RANGE (nk_search_range): fixed per-query thresholds; full buffers are flushed to the
-// lists, never pruned, and the end of the launch flushes what is left.  ROWTHR (with RANGE, the reverse scan of
-// nk_knn_graph_update): a pair must also reach its row's threshold p.row_thr[row], loaded with the row's norms.  RFILT (with
-// ROWTHR and TAGS, a filtered graph): the row's own filter must also admit the query's tag (keep_fragment_rows); the launch's
-// query tags are staged in shared memory past Shared.
-template <int QT, ptx::Opnd OP, bool DUMP, bool TAGS, bool RANGE, bool ROWTHR = false, bool RFILT = false>
+// OP: the operand type, bf16 (BF16 shadow, bf16 corpora), fp16 (an fp16 corpus scanned in place) or int8 (the int8 image of
+// an fp32 shard).  M: the scan mode (kernels.cuh).  Tag filters are read through the read-only cache (shared memory is spent
+// on the rings); REVERSE_RFILT stages the launch's query tags in shared memory past Shared.
+template <int QT, ptx::Opnd OP, ScanMode M>
 __global__ void __launch_bounds__(sb::NTHREADS, 1)
 knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_q, tc::Params p) {
     using namespace sb;
@@ -271,8 +267,8 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
         sh.qb[tid] = p.qb[qpad_off + tid];
         if (S8) sh.qs[tid] = p.qscale[qpad_off + tid];
     }
-    uint64_t *qtag = reinterpret_cast<uint64_t *>(smem_raw + (size_t)C::RING_BYTES + sizeof(Shared));  // RFILT only
-    if (RFILT && tid < QT) qtag[tid] = (uint32_t)tid < nq ? p.qtags[q0 + tid] : 0ull;
+    uint64_t *qtag = reinterpret_cast<uint64_t *>(smem_raw + (size_t)C::RING_BYTES + sizeof(Shared));  // REVERSE_RFILT only
+    if (mode_row_filter(M) && tid < QT) qtag[tid] = (uint32_t)tid < nq ? p.qtags[q0 + tid] : 0ull;
     __syncthreads();
     const bool flood = !p.presampled;  // first two tiles: every (row, query) pair is placed directly
     if (prof && tid == 0) g_sb_prof[blockIdx.x][1] = globaltimer_ns();
@@ -336,7 +332,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
         for (uint32_t tile = sub; tile < num_tiles; tile += sgrid, ++it) {
             if (eprof) t_a = globaltimer_ns();
             // The epilogue's row inputs, loaded before the MMAs: |x|^2, |dx|^2 (int8 image: and the row's scale), the mask word
-            // and (ROWTHR) the threshold of this thread's 4 rows; and the shared threshold of query etid (it only grows: an
+            // and (reverse modes) the threshold of this thread's 4 rows; and the shared threshold of query etid (it only grows: an
             // earlier value is still a lower bound).
             float x2[4], d2[4], rthr[4], xs[4];
             uint32_t mword[4];
@@ -347,11 +343,11 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
                 x2[ri] = in ? __ldg(p.xnorm2 + row) : 0.0f;
                 d2[ri] = in && p.dnorm2 ? __ldg(p.dnorm2 + row) : 0.0f;  // 16-bit corpus: no residue
                 mword[ri] = in && p.mask ? __ldg(p.mask + (row >> 5)) : ~0u;
-                rthr[ri] = ROWTHR && in ? __ldg(p.row_thr + row) : -INFINITY;
+                rthr[ri] = mode_row_thr(M) && in ? __ldg(p.row_thr + row) : -INFINITY;
                 xs[ri] = S8 && in ? __ldg(p.xscale + row) : 1.0f;
             }
             const uint32_t etid = tid - EPI_WARP0 * 32;  // consumer thread: one query each (QT <= EPI_NT)
-            const uint32_t gt_pre = !RANGE && etid < nq ? __ldcg(p.gtau + q0 + etid) : 0u;
+            const uint32_t gt_pre = !mode_range(M) && etid < nq ? __ldcg(p.gtau + q0 + etid) : 0u;
             uint32_t prev_sa = 0, prev_sb = 0;
             for (uint32_t j = 0; j < nslab; ++j, ++g) {
                 const uint32_t sa = g % C::ASTAGES, sbq = g % C::BSTAGES;
@@ -450,13 +446,13 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             if (eprof) { const unsigned long long t = globaltimer_ns(); split[18] += t - t_a; t_a = t; }
             if (flood && it < 2 && ewarp == 0 && lane == 0)
                 for (uint32_t qi = 0; qi < nq; ++qi) sh.cnt[qi] = (int)((it + 1) * ROWS);
-            keep_fragment_rows<QT, PB, true, DUMP, TAGS, ROWTHR, RFILT>(p, est, acc, 0, alive, tile * ROWS, rbase, flood, it, cbase, q0, nq, sh.tau,
-                                                                        sh.qn, sh.cnt, my_cand, rthr, qtag);
+            keep_fragment_rows<QT, PB, true, M>(p, est, acc, 0, alive, tile * ROWS, rbase, flood, it, cbase, q0, nq, sh.tau, sh.qn, sh.cnt, my_cand,
+                                                rthr, qtag);
             if (eprof) { const unsigned long long t = globaltimer_ns(); split[17] += t - t_a; t_a = t; }
             // prune any buffer that could overflow during the next tile (8 warps, different queries concurrently)
             group_sync(EPI_BAR, EPI_NT);  // every push of this tile is visible
             if (eprof) { const unsigned long long t = globaltimer_ns(); split[19] += t - t_a; t_a = t; }
-            if constexpr (RANGE)
+            if constexpr (mode_range(M))
                 flush_tile<PB>(p, q0, nq, ewarp, lane, my_cand, sh.cnt);
             else
                 prune_tile<true>(p, q0, nq, ewarp, lane, sh.cnt, sh.tau, prune_trigger, prune_at, flood && it == 0,
@@ -467,7 +463,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
             if (eprof) { const unsigned long long t = globaltimer_ns(); split[20] += t - t_a; t_a = t; }
             group_sync(EPI_BAR, EPI_NT);
             if (eprof) { const unsigned long long t = globaltimer_ns(); split[21] += t - t_a; t_a = t; }
-            if (!RANGE && etid < nq) sh.tau[etid] = raise_to_shared_tau(gt_pre, sh.tau[etid]);  // adopt the shared threshold
+            if (!mode_range(M) && etid < nq) sh.tau[etid] = raise_to_shared_tau(gt_pre, sh.tau[etid]);  // adopt the shared threshold
             if (eprof) split[22] += globaltimer_ns() - t_a;
         }
         if (eprof) {
@@ -480,7 +476,7 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
 
     // ---- emit: everything inside this CTA's margin AND above the shared threshold goes to the query's shared list.
     __syncthreads();
-    if constexpr (RANGE) {  // range mode: what the last flushes left, whole (no staging: one buffer per warp at a time)
+    if constexpr (mode_range(M)) {  // range modes: what the last flushes left, whole (no staging: one buffer per warp at a time)
         for (uint32_t qi = warp; qi < nq; qi += NTHREADS / 32) flush_query(p, q0, qi, lane, my_cand + (size_t)qi * PB, sh.cnt);
     } else {
         // Fast path (buffers with <= k_emit entries, i.e. almost always all of them): no selection, the finish kernel selects
@@ -650,7 +646,7 @@ bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a) {
     return a.dim % 8 == 0;  // 16-bit rows: 16-byte TMA row stride and 128-bit exact re-scoring loads
 }
 
-template <int QT, ptx::Opnd OP, bool DUMP, bool TAGS, bool RANGE = false, bool ROWTHR = false, bool RFILT = false>
+template <int QT, ptx::Opnd OP, ScanMode M>
 static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
     using namespace sb;
     const uint32_t esz = OP == ptx::Opnd::S8 ? 1 : 2, kcols = 128 / esz;  // int8 image: 1-byte elements, 128 per swizzle row
@@ -659,17 +655,17 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
     const CUtensorMap *map_q = tc_cached_map(ws, QT == 64 ? 5 : 6, sp.qbf16, sp.Qpad, sp.dimpad, esz, kcols, QT, (uint64_t)sp.dimpad * esz,
                                              a.dtype);  // rows past Qpad: zero
     if (!map_rows || !map_q) return -1;
-    const size_t smem = (size_t)Cfg<QT>::RING_BYTES + sizeof(Shared) + (RFILT ? QT * sizeof(uint64_t) : 0) + 1024;
+    const size_t smem = (size_t)Cfg<QT>::RING_BYTES + sizeof(Shared) + (mode_row_filter(M) ? QT * sizeof(uint64_t) : 0) + 1024;
     if (smem > di.max_smem_optin) {
         set_error("shadow tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;
     }
-    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, OP, DUMP, TAGS, RANGE, ROWTHR, RFILT>), di.device_id, smem))
+    if (tc_ensure_smem(reinterpret_cast<const void *>(knn_scan_shadow_kernel<QT, OP, M>), di.device_id, smem))
         return -1;
     tc::Params p = pass_params(a, ws, sp);
     p.nslab = sp.dimpad / kcols; p.qa = sp.qa; p.qb = sp.qb; p.xnorm2 = a.image.xnorm2; p.dnorm2 = a.image.dnorm2;
     p.xscale = a.image.xscale; p.qscale = sp.qscale;
-    knn_scan_shadow_kernel<QT, OP, DUMP, TAGS, RANGE, ROWTHR, RFILT><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
+    knn_scan_shadow_kernel<QT, OP, M><<<sp.grid, NTHREADS, smem, a.stream>>>(*map_rows, *map_q, p);
     NK_CUDA_OK(cudaGetLastError());
     if (launches) ++*launches;
     if (a.main_launches) ++*a.main_launches;
@@ -677,33 +673,16 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
     return 0;
 }
 
+// One pass at qt = 64 or 128 query columns in the mode a.mode; the dump mode exists at QT = 64 only.
 template <ptx::Opnd OP>
 static int launch_shadow_pass_op(int qt, const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const ShadowPassArgs &sp, uint64_t *launches) {
-    if (sp.dump_est) return launch_shadow_pass_t<64, OP, true, false>(di, a, ws, sp, launches);
-    if (sp.range && a.row_thr && a.row_filter) {  // the reverse scan of a filtered graph: each row's own filter
-        if (!a.qfilter || !a.qtags) { set_error("internal: the row-filtered reverse scan needs per-query filters and tags"); return -1; }
-        return qt == 128 ? launch_shadow_pass_t<128, OP, false, true, true, true, true>(di, a, ws, sp, launches)
-                         : launch_shadow_pass_t<64, OP, false, true, true, true, true>(di, a, ws, sp, launches);
-    }
-    if (sp.range && a.row_thr) {  // the reverse scan of nk_knn_graph_update
-        if (a.qfilter)
-            return qt == 128 ? launch_shadow_pass_t<128, OP, false, true, true, true>(di, a, ws, sp, launches)
-                             : launch_shadow_pass_t<64, OP, false, true, true, true>(di, a, ws, sp, launches);
-        return qt == 128 ? launch_shadow_pass_t<128, OP, false, false, true, true>(di, a, ws, sp, launches)
-                         : launch_shadow_pass_t<64, OP, false, false, true, true>(di, a, ws, sp, launches);
-    }
-    if (sp.range) {
-        if (a.qfilter)
-            return qt == 128 ? launch_shadow_pass_t<128, OP, false, true, true>(di, a, ws, sp, launches)
-                             : launch_shadow_pass_t<64, OP, false, true, true>(di, a, ws, sp, launches);
-        return qt == 128 ? launch_shadow_pass_t<128, OP, false, false, true>(di, a, ws, sp, launches)
-                         : launch_shadow_pass_t<64, OP, false, false, true>(di, a, ws, sp, launches);
-    }
-    if (a.qfilter)
-        return qt == 128 ? launch_shadow_pass_t<128, OP, false, true>(di, a, ws, sp, launches)
-                         : launch_shadow_pass_t<64, OP, false, true>(di, a, ws, sp, launches);
-    return qt == 128 ? launch_shadow_pass_t<128, OP, false, false>(di, a, ws, sp, launches)
-                     : launch_shadow_pass_t<64, OP, false, false>(di, a, ws, sp, launches);
+    return tc::with_scan_mode(a.mode, [&](auto mode) {
+        constexpr ScanMode M = decltype(mode)::value;
+        if (qt != 128) return launch_shadow_pass_t<64, OP, M>(di, a, ws, sp, launches);
+        if constexpr (!mode_dump(M)) return launch_shadow_pass_t<128, OP, M>(di, a, ws, sp, launches);
+        set_error("internal: no 16-bit / int8 kernel for scan mode %d at 128 query columns", (int)M);
+        return -1;
+    });
 }
 
 // the int8 image runs the s8 wgmma form, the BF16 shadow the bf16 one, rows scanned in place the form of their dtype

@@ -3,6 +3,7 @@
 // set-up, the TMA producer loop and the filter epilogue (keep rule, per-tile prune / publish / adopt, emission fallback).
 #pragma once
 #include <cuda.h>
+#include <type_traits>
 
 #include "kernels.cuh"
 #ifdef __CUDACC__
@@ -67,13 +68,13 @@ struct Params {
                               // (filter_prep_kernel): no flood tiles, thresholds are adopted at kernel start
     float min_score;          // filter: caller's score floor (VectorIndex minSimilarity, vector_index.go:339-352): rows
                               // whose upper bound is below it are never buffered (-inf = none)
-    float *dump_est, *dump_bnd;  // DUMP kernels only (tests): per (row, query) score estimate and error bound, [n][dump_ld]
+    float *dump_est, *dump_bnd;  // dump mode only (tests): per (row, query) score estimate and error bound, [n][dump_ld]
     uint32_t dump_ld;
-    const uint64_t *row_tags; // TAGS kernels only: tag word per local row
-    const NkFilter *qfilter;  // TAGS kernels only: filter per query [Q], indexed like gtau (absolute query index)
-    const float *row_thr;     // ROWTHR kernels only: key-space threshold per local row (the reverse scan of nk_knn_graph_update)
-    const NkFilter *row_filter;  // RFILT kernels only: the filter of each local row's own k-NN list (filtered graphs)
-    const uint64_t *qtags;    // RFILT kernels only: tag word per query [Q], indexed like gtau; staged in shared memory per CTA
+    const uint64_t *row_tags; // tag modes only: tag word per local row
+    const NkFilter *qfilter;  // tag modes only: filter per query [Q], indexed like gtau (absolute query index)
+    const float *row_thr;     // reverse modes only: key-space threshold per local row (the reverse scan of nk_knn_graph_update)
+    const NkFilter *row_filter;  // REVERSE_RFILT only: the filter of each local row's own k-NN list (filtered graphs)
+    const uint64_t *qtags;    // REVERSE_RFILT only: tag word per query [Q], indexed like gtau; staged in shared memory per CTA
 };
 
 // What one scan launch covers: queries [q0, q0+nq) in `qgroups` query groups over a `grid`-CTA launch.  Both kernels'
@@ -82,11 +83,19 @@ struct PassArgs {
     uint32_t grid, k_emit, Qpad, q0, nq, qgroups;
     const float *qnorm;
     int presampled;
-    float *dump_est = nullptr, *dump_bnd = nullptr;  // test-only DUMP instantiations
+    float *dump_est = nullptr, *dump_bnd = nullptr;  // read under ScanMode::DUMP only (tests)
     uint32_t dump_ld = 0;
-    bool range = false;       // range mode (nk_search_range): gtau[] holds fixed thresholds, survivors go to lists of list_cap
-    uint32_t list_cap = 0;
+    uint32_t list_cap = 0;    // range modes: gtau[] holds fixed thresholds, survivors go to lists of list_cap
 };
+
+// Where a scan's run-time mode becomes its kernel's template argument: launch(std::integral_constant<ScanMode, M>{}) for M = m
+// (modes tried in order, DUMP last).  The launchers refuse with `if constexpr` the (kernel, mode) pairs that do not exist.
+template <ScanMode M = ScanMode::KNN, class Launch> int with_scan_mode(ScanMode m, Launch &&launch) {
+    if (m == M) return launch(std::integral_constant<ScanMode, M>{});
+    if constexpr (M != ScanMode::DUMP) return with_scan_mode<ScanMode((int)M + 1)>(m, launch);
+    set_error("internal: unknown scan mode %d", (int)m);
+    return -1;
+}
 
 #ifdef __CUDACC__
 // mbarriers of the two TMA rings (corpus slabs, query slabs) of a scan kernel; the first member of its shared state.
@@ -180,7 +189,7 @@ template <int QT> __device__ __forceinline__ float frag_value(const float (&acc)
 // rbase + 64 (fr / 2) + 8 (fr % 2) (corpus row row0 + that), QT/4 query columns cbase + 8 (j / 2) + j % 2.  Buffers every
 // (row, query) pair whose score estimate can still reach the query's threshold.  The kernel supplies one estimate per row:
 // est[ri].upper(v, col) is the UPPER bound of the score from accumulator value v (exact mode: the score itself) given the
-// query's inputs col = est[0].col(qi), est.bound(qi) its error bound before the euclidean term (DUMP only), est.mul /
+// query's inputs col = est[0].col(qi), est.bound(qi) its error bound before the euclidean term (dump mode only), est.mul /
 // est.x2 the row's scale and |x|^2.  alive: bit ri set = the row takes part.  The 16-bit / int8 scan passes all 4 rows at
 // once (NR = 4); the TF32 kernel, whose register budget is 168 rather than 240, one row at a time (NR = 1).
 //   flood (first two tiles without a sampled threshold): every pair is placed directly at slot = tile-local row, in a loop
@@ -189,20 +198,16 @@ template <int QT> __device__ __forceinline__ float frag_value(const float (&acc)
 //   rows and builds the masks of pairs worth buffering (NaN passes); the rare pushes run in a small loop that is not
 //   unrolled.
 // BOUNDED: a NaN estimate is undecidable here, so it is kept as +inf and the exact re-scoring judges; exact mode: -inf.
-// TAGS (filtered searches): a pair whose query does not admit the row's tag never enters a buffer — otherwise the pruned and
-// published thresholds would stop being lower bounds of the FILTERED k-th best score.  Flood tiles place it as key 0; the
-// compare pass loads the row's tag only when some column passed and clears the columns whose filter rejects it.
-// ROWTHR (the reverse scan of nk_knn_graph_update, range mode): a pair must also reach the ROW's threshold rthr[ri].
-// RFILT (with ROWTHR and TAGS, the reverse scan of a filtered graph): the row's own filter p.row_filter[row] must also admit
-// the query's tag qtag[qi] (the CTA's query tags, in shared memory) — the mirror image of TAGS.  The row's filter is loaded
-// only for a fragment row with a pair that already reached both thresholds.
-template <int QT, int CAP, bool BOUNDED, bool DUMP, bool TAGS = false, bool ROWTHR = false, bool RFILT = false, int NR, class Est>
+// M (ScanMode): tag modes: a pair whose query does not admit the row's tag never enters a buffer — else the pruned and
+// published thresholds would stop being lower bounds of the FILTERED k-th best score; flood tiles place it as key 0, the
+// compare pass loads the row's tag only when some column passed.  Reverse modes: a pair must also reach the ROW's threshold rthr[ri] and
+// (REVERSE_RFILT) be admitted by the row's own filter (qtag: the CTA's query tags), loaded only once both thresholds hold.
+template <int QT, int CAP, bool BOUNDED, ScanMode M, int NR, class Est>
 __device__ __forceinline__ void keep_fragment_rows(const Params &p, const Est (&est)[NR], const float (&acc)[2][QT / 2], uint32_t fr0,
                                                    uint32_t alive, uint32_t row0, uint32_t rbase, bool flood, uint32_t it, uint32_t cbase,
                                                    uint32_t q0, uint32_t nq, const float *tau, const float *qn, int *cnt, uint64_t *cand,
                                                    const float (&rthr)[NR], const uint64_t *qtag = nullptr) {
-    static_assert(!RFILT || (TAGS && ROWTHR), "the row-side filter is a mode of the filtered reverse scan");
-    if (DUMP) {  // tests only: score estimate and error bound per (row, query)
+    if (mode_dump(M)) {  // tests only: score estimate and error bound per (row, query)
 #pragma unroll
         for (uint32_t ri = 0; ri < (uint32_t)NR; ++ri) {
             const uint32_t fr = fr0 + ri, row = row0 + rbase + 64 * (fr >> 1) + 8 * (fr & 1);
@@ -231,14 +236,14 @@ __device__ __forceinline__ void keep_fragment_rows(const Params &p, const Est (&
             const uint32_t slot = it * ROWS + rt;
             const uint32_t grow = (uint32_t)(p.row_base + row);
             uint32_t admit = ~0u;  // columns whose filter admits the row
-            if (TAGS) {
+            if (mode_tags(M)) {
                 admit = 0u;
                 if (live) {
                     const uint64_t tag = __ldg(p.row_tags + row);
 #pragma unroll 1
                     for (uint32_t c = 0; c < (uint32_t)(QT / 4); ++c) {
                         const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
-                        if (qi < nq && tag_admits(tag, p.qfilter + q0 + qi) && (!RFILT || tag_admits(qtag[qi], p.row_filter + row)))
+                        if (qi < nq && tag_admits(tag, p.qfilter + q0 + qi) && (!mode_row_filter(M) || tag_admits(qtag[qi], p.row_filter + row)))
                             admit |= 1u << c;
                     }
                 }
@@ -267,7 +272,7 @@ __device__ __forceinline__ void keep_fragment_rows(const Params &p, const Est (&
 #pragma unroll
         for (uint32_t ri = 0; ri < (uint32_t)NR; ++ri) {
             const float s0 = est[ri].upper(frag_at<QT>(acc, fr0 + ri, jj), col);
-            const float tr = ROWTHR ? fmaxf(t, rthr[ri]) : t;
+            const float tr = mode_row_thr(M) ? fmaxf(t, rthr[ri]) : t;
             pass[ri] |= (!(s0 < tr) && qi < nq) ? (1u << jj) : 0u;
         }
     }
@@ -285,8 +290,8 @@ __device__ __forceinline__ void keep_fragment_rows(const Params &p, const Est (&
         if (!ps) continue;
         const uint32_t fr = fr0 + ri, row = row0 + rbase + 64 * (fr >> 1) + 8 * (fr & 1);
         const Est e = pick_row(est, ri);
-        const float rt = ROWTHR ? pick_row(rthr, ri) : -INFINITY;
-        if (TAGS) {
+        const float rt = mode_row_thr(M) ? pick_row(rthr, ri) : -INFINITY;
+        if (mode_tags(M)) {
             const uint64_t tag = __ldg(p.row_tags + row);
             uint32_t chk = ps;
 #pragma unroll 1
@@ -296,7 +301,7 @@ __device__ __forceinline__ void keep_fragment_rows(const Params &p, const Est (&
                 if (!tag_admits(tag, p.qfilter + q0 + cbase + 8 * (c >> 1) + (c & 1))) ps &= ~(1u << c);
             }
         }
-        if (RFILT && ps) {
+        if (mode_row_filter(M) && ps) {
             const NkFilter *rf = p.row_filter + row;
             const uint64_t all_of = __ldg(&rf->all_of), none_of = __ldg(&rf->none_of), any_of = __ldg(&rf->any_of);
             uint32_t chk = ps;
@@ -314,7 +319,7 @@ __device__ __forceinline__ void keep_fragment_rows(const Params &p, const Est (&
             const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
             float sc = e.upper(frag_value<QT>(acc, fr, c), e.col(qi));
             if (sc != sc) sc = BOUNDED ? INFINITY : -INFINITY;
-            if (sc >= (ROWTHR ? fmaxf(tau[qi], rt) : tau[qi])) {
+            if (sc >= (mode_row_thr(M) ? fmaxf(tau[qi], rt) : tau[qi])) {
                 int pos = atomicAdd(&cnt[qi], 1);
                 if (pos < CAP) cand[(size_t)qi * CAP + pos] = make_key(sc, (uint32_t)(p.row_base + row));
                 else atomicExch(p.flags + FLAG_FATAL, 1);
@@ -559,11 +564,12 @@ struct PrepParams {
     const uint32_t *mask;
     float min_score;
     const int *only_if;
-    const uint64_t *row_tags;  // per-query tag filters (both set or both nullptr): the sample counts admissible rows only
+    const uint64_t *row_tags;  // the tag modes' filters: the sample counts admissible rows only
     const NkFilter *qfilter;
 };
 // The fields taken from the search arguments: the queries, the metric and the shard (for the sample).
 PrepParams prep_params(const ScanArgs &a, uint32_t Qpad, uint32_t dimpad);
-int launch_prep(const DeviceInfo &di, const PrepParams &pp, cudaStream_t stream, uint64_t *launches);
+// The tag modes run the instantiation whose sample counts only the rows each query admits.
+int launch_prep(const DeviceInfo &di, ScanMode mode, const PrepParams &pp, cudaStream_t stream, uint64_t *launches);
 
 }  // namespace nk
