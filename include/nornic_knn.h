@@ -469,6 +469,23 @@ int nk_score_subset(NkIndex *ix, const float *query_host, const uint32_t *rows_h
 int nk_index_assign_nearest(NkIndex *ix, const float *centroids_host, uint32_t K, int metric, int32_t *assign_io,
                             uint64_t *changed);
 int nk_index_cluster_means(NkIndex *ix, const int32_t *assign_host, uint32_t K, float *centroids_io, uint32_t *counts_out);
+/* nk_index_kmeanspp = initCentroidsKMeansPlusPlus (kmeans.go:364-426) over every row of an fp32 index, on the device.
+ * The caller owns the randomness: first_row plays rand.Intn(n), u_host [K-1] (each in [0, 1); nullable when K == 1) plays
+ * rand.Float64() for seeds 1 .. K-1.  Outputs: seeds_out [K] row ids (relative to the index's first row);
+ * centroids_out (nullable) [K x dim] those rows; potential_out (nullable) [K]: the sum of every row's D² after seeds
+ * 0..c (the total seed c+1 is drawn from; the last entry is the k-means++ cost); min_d2_out (nullable) [rows]: each
+ * row's D² to its nearest seed; *rows_read (nullable): rows whose contents the passes read.  D² is squaredEuclidean
+ * bit for bit; seed 0 assigns it (a NaN stays NaN), later seeds lower it only where strictly smaller.  The pick: target
+ * = u T, where the weights are summed sequentially in chunks of 256 rows from each shard's first row, and the chunk sums
+ * sequentially in row order (P_j inclusive prefixes, T the total); seed = the first row i of the first chunk j with
+ * P_j >= target such that P_{j-1} + (the chunk's partial sum up to i) >= target, or the last row if no chunk qualifies
+ * (NaN).  This equals kmeans.go's pick except where target lies within the rounding of the running sums, and exactly
+ * where every sum is exact; the number of devices enters only through the chunk boundaries.  NK_KMPP_PRUNE=0 (read per
+ * call) computes every row of every pass instead of skipping the rows the triangle inequality proves unchanged: same
+ * outputs.  The row mask, tags and score floor are ignored.  Synchronous; -1 before any work for a null ix / seeds_out
+ * (/ u_host when K > 1), a non-fp32 index, K == 0 or K > rows, first_row >= rows, or any u that is NaN or outside [0, 1). */
+int nk_index_kmeanspp(NkIndex *ix, uint32_t K, uint64_t first_row, const double *u_host, uint32_t *seeds_out, float *centroids_out,
+                      double *potential_out, double *min_d2_out, uint64_t *rows_read);
 
 /* Synthetic fp32 query block from the shared generator, on the device of a single-device index. */
 int nk_fill_uniform_device(int device_id, float *out_dev, uint64_t n_rows, uint32_t dim, uint64_t seed,

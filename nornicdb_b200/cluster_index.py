@@ -10,8 +10,11 @@ Centroid bookkeeping (K x dim, tiny) stays on the host in the reference's arithm
 squares: squaredEuclidean kmeans.go:430-454).
 
 Deviations, stated: the reference seeds k-means++ / random init from Go's global math/rand stream, which cannot be
-reproduced; this mirror takes a numpy Generator (seedable) and, for corpora above `init_sample` rows, runs k-means++ on
-a uniform sample of the rows read back from the device.  `assign` selects which of the reference's two assignment rules
+reproduced; this mirror takes a numpy Generator (seedable).  By default, for corpora above `init_sample` rows, it runs
+k-means++ on the host over a uniform sample of the rows read back from the device.  `init_sample=None` seeds over every
+row as kmeans.go:364-426 does, on the device (`nk_index_kmeanspp`): the same draws (rng.integers(n), then one
+rng.random() per further seed), squaredEuclidean bit for bit, and the pick from chunked fp64 sums, which equals the
+reference's sequential one except where the target lies within the rounding of the running sums.  `assign` selects which of the reference's two assignment rules
 is used: "euclidean" (assignToCentroids, the CPU definition) or "cosine" (assignToCentroidsGPU, what the reference runs
 when its GPU manager is enabled).
 """
@@ -74,14 +77,14 @@ def squaredEuclidean(a: np.ndarray, b: np.ndarray) -> np.ndarray:
 
 class ClusterIndex(EmbeddingIndex):
     def __init__(self, dimensions: int, kmeansConfig: Optional[KMeansConfig] = None, devices: Sequence[int] = (0,),
-                 assign: str = "euclidean", rng: Optional[np.random.Generator] = None, init_sample: int = 200_000):
+                 assign: str = "euclidean", rng: Optional[np.random.Generator] = None, init_sample: Optional[int] = 200_000):
         super().__init__(dimensions, metric="cosine", devices=devices, dtype="f32")  # kmeans.go:200-229
         if assign not in ("euclidean", "cosine"):
             raise ValueError("assign must be 'euclidean' (kmeans.go:458) or 'cosine' (kmeans.go:491)")
         self.config = kmeansConfig or KMeansConfig()
         self.assign_metric = assign
         self.rng = rng or np.random.default_rng()
-        self.init_sample = int(init_sample)
+        self.init_sample = None if init_sample is None else int(init_sample)  # None: no sample, k-means++ on the device
         self.centroids: Optional[np.ndarray] = None      # [K x dim] float32
         self.assignments: Optional[np.ndarray] = None    # [N] int32
         self.clusterMap: Dict[int, List[int]] = {}
@@ -96,7 +99,7 @@ class ClusterIndex(EmbeddingIndex):
 
     # ---- initialisation (kmeans.go:335-427) ------------------------------------------------------------------------
     def _init_rows(self, n: int) -> np.ndarray:
-        if n <= self.init_sample:
+        if self.init_sample is None or n <= self.init_sample:
             return self._ix.read_rows(0, n)
         pick = np.sort(self.rng.choice(n, size=self.init_sample, replace=False))
         return np.stack([self._ix.read_rows(int(r), 1)[0] for r in pick])
@@ -138,6 +141,9 @@ class ClusterIndex(EmbeddingIndex):
                 cen = np.array(initial_centroids, dtype=np.float32, order="C", copy=True)
                 if cen.shape != (k, self.dimensions):
                     raise ValueError(f"initial_centroids must be [{k} x {self.dimensions}]")
+            elif self.init_sample is None and self.config.InitMethod == "kmeans++":
+                first = int(self.rng.integers(n))
+                cen = self._ix.kmeanspp(k, first, self.rng.random(k - 1)).centroids
             else:
                 rows = self._init_rows(n)
                 cen = self._init_kmeanspp(k, rows) if self.config.InitMethod == "kmeans++" else self._init_random(k, rows)

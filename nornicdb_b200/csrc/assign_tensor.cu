@@ -22,6 +22,7 @@
 #include "kernels.cuh"
 #include "ptx_sm90.cuh"
 #include "scan_tensor_shared.cuh"
+#include "sq_euclid.cuh"
 
 namespace nk {
 
@@ -217,25 +218,6 @@ assign_scan_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
             }
         }
     }
-}
-
-// squaredEuclidean (kmeans.go:430-454, oracle orc_sq_euclid64) bit for bit: fp32 differences, fp64 squares in four
-// interleaved sums, the tail into s0, then s0 + s1 + s2 + s3.  Explicit round-to-nearest intrinsics: nvcc would contract
-// a * b + c into an fma and change the rounding.
-__device__ __forceinline__ double sq_euclid64(const float *x, const float *c, uint32_t dim) {
-    double s0 = 0.0, s1 = 0.0, s2 = 0.0, s3 = 0.0;
-    uint32_t j = 0;
-    for (; j + 4 <= dim; j += 4) {
-        const double d0 = (double)__fsub_rn(x[j], c[j]), d1 = (double)__fsub_rn(x[j + 1], c[j + 1]);
-        const double d2 = (double)__fsub_rn(x[j + 2], c[j + 2]), d3 = (double)__fsub_rn(x[j + 3], c[j + 3]);
-        s0 = __dadd_rn(s0, __dmul_rn(d0, d0)); s1 = __dadd_rn(s1, __dmul_rn(d1, d1));
-        s2 = __dadd_rn(s2, __dmul_rn(d2, d2)); s3 = __dadd_rn(s3, __dmul_rn(d3, d3));
-    }
-    for (; j < dim; ++j) {
-        const double d = (double)__fsub_rn(x[j], c[j]);
-        s0 = __dadd_rn(s0, __dmul_rn(d, d));
-    }
-    return __dadd_rn(__dadd_rn(__dadd_rn(s0, s1), s2), s3);
 }
 
 // fp64 cosine of the fp32 inputs: 0 for a zero row or centroid, NaN for non-finite inputs (never wins)

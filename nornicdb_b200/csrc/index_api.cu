@@ -2525,6 +2525,144 @@ int nk_index_cluster_means(NkIndex *ix, const int32_t *assign_host, uint32_t K, 
     return 0;
 }
 
+// k-means++ seeding over every row (kmeans.go:364-426; include/nornic_knn.h, DESIGN §7 item 3).  Each shard keeps, in its
+// scratch, every row's D² and nearest seed, the sums of its chunks of 256 rows, the δ² of the newest seed to the earlier
+// ones and the grow-only list of the seeds so far.  Per seed: one pass per shard (kmeanspp_pass), then the pick on the
+// host from the chunk sums and the weights of the one chunk the target falls in, the same code for any number of devices.
+struct KmppShard {
+    NkShard *s = nullptr;
+    uint64_t first = 0, nch = 0;
+    double *d2 = nullptr, *sums = nullptr, *delta = nullptr;
+    uint32_t *near = nullptr;
+    float *seeds = nullptr;
+    unsigned long long *read = nullptr;
+    std::vector<double> h_sums;
+};
+
+int nk_index_kmeanspp(NkIndex *ix, uint32_t K, uint64_t first_row, const double *u_host, uint32_t *seeds_out, float *centroids_out,
+                      double *potential_out, double *min_d2_out, uint64_t *rows_read) {
+    nk::DeviceGuard _restore_device;
+    if (!ix || !seeds_out || (K > 1 && !u_host)) { nk::set_error("null argument"); return -1; }
+    if (ix->dtype != NK_DTYPE_F32) { nk::set_error("nk_index_kmeanspp: fp32 index required"); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
+    const uint64_t n = ix->rows();
+    if (K == 0 || K > n) { nk::set_error("nk_index_kmeanspp: K=%u outside [1, %llu rows]", K, (unsigned long long)n); return -1; }
+    if (first_row >= n) { nk::set_error("nk_index_kmeanspp: first_row %llu >= %llu rows", (unsigned long long)first_row, (unsigned long long)n); return -1; }
+    for (uint32_t c = 0; c + 1 < K; ++c)
+        if (!(u_host[c] >= 0.0 && u_host[c] < 1.0)) { nk::set_error("nk_index_kmeanspp: u[%u] = %g is not in [0, 1)", c, u_host[c]); return -1; }
+    bool prune = true;
+    if (const char *e = getenv("NK_KMPP_PRUNE"))
+        if (atoi(e) == 0) prune = false;
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
+    const uint32_t dim = ix->dim;
+    const size_t rowb = (size_t)dim * 4;
+    auto al = [](size_t b) { return (b + 255) & ~(size_t)255; };
+    std::vector<KmppShard> sh;
+    for (NkShard *s : live_shards(ix)) {
+        KmppShard k;
+        k.s = s; k.first = ix->first_row(*s); k.nch = (s->n + nk::KMPP_CHUNK - 1) / nk::KMPP_CHUNK;
+        const size_t o_near = al(s->n * 8), o_sums = o_near + al(s->n * 4), o_delta = o_sums + al(k.nch * 8),
+                     o_seeds = o_delta + al((size_t)K * 8), o_read = o_seeds + al((size_t)K * rowb);
+        NK_CUDA_OK(cudaSetDevice(s->device));
+        if (nk::ws_reserve(&s->ws.scratch, &s->ws.scratch_bytes, o_read + 256)) return -1;  // grow-only, reused across calls
+        unsigned char *base = static_cast<unsigned char *>(s->ws.scratch);
+        k.d2 = reinterpret_cast<double *>(base);
+        k.near = reinterpret_cast<uint32_t *>(base + o_near);
+        k.sums = reinterpret_cast<double *>(base + o_sums);
+        k.delta = reinterpret_cast<double *>(base + o_delta);
+        k.seeds = reinterpret_cast<float *>(base + o_seeds);
+        k.read = reinterpret_cast<unsigned long long *>(base + o_read);
+        k.h_sums.resize(k.nch);
+        NK_CUDA_OK(cudaMemsetAsync(k.read, 0, 8, s->stream));
+        sh.push_back(std::move(k));
+    }
+    auto owner = [&](uint64_t row) -> KmppShard & {
+        for (auto &k : sh)
+            if (row < k.first + k.s->n) return k;
+        return sh.back();
+    };
+    std::vector<float> crow(dim);
+    std::vector<double> prefix;  // P_j over every shard's chunks, in row order
+    std::vector<double> w(nk::KMPP_CHUNK);
+    uint64_t seed = first_row;
+    for (uint32_t c = 0; c < K; ++c) {
+        seeds_out[c] = (uint32_t)seed;
+        KmppShard &o = owner(seed);
+        NK_CUDA_OK(cudaSetDevice(o.s->device));
+        NK_CUDA_OK(cudaMemcpyAsync(crow.data(), static_cast<const float *>(o.s->rows) + (seed - o.first) * dim, rowb, cudaMemcpyDeviceToHost, o.s->stream));
+        NK_CUDA_OK(cudaStreamSynchronize(o.s->stream));
+        if (centroids_out) memcpy(centroids_out + (size_t)c * dim, crow.data(), rowb);
+        for (auto &k : sh) {
+            NkShard &s = *k.s;
+            NK_CUDA_OK(cudaSetDevice(s.device));
+            NK_CUDA_OK(cudaMemcpyAsync(k.seeds + (size_t)c * dim, crow.data(), rowb, cudaMemcpyHostToDevice, s.stream));
+            cudaEvent_t ev[2] = {nullptr, nullptr};
+            if (ix->timing_on) {
+                NK_CUDA_OK(cudaEventCreate(&ev[0]));
+                NK_CUDA_OK(cudaEventCreate(&ev[1]));
+                NK_CUDA_OK(cudaEventRecord(ev[0], s.stream));
+            }
+            uint64_t launches = 0;
+            const int rc = nk::kmeanspp_pass(s.di, static_cast<const float *>(s.rows), s.n, dim, k.seeds, c, k.delta, prune, k.d2, k.near,
+                                             k.sums, k.read, s.stream, &launches);
+            if (ev[0]) {
+                cudaEventRecord(ev[1], s.stream);
+                s.timing.emplace_back(ev[0], ev[1]);
+                s.timing_launches.push_back(launches);
+            }
+            if (rc) return -1;
+            ix->stats.kernel_launches += launches;
+            NK_CUDA_OK(cudaMemcpyAsync(k.h_sums.data(), k.sums, k.nch * 8, cudaMemcpyDeviceToHost, s.stream));
+        }
+        prefix.clear();
+        double T = 0.0;
+        for (auto &k : sh) {
+            NK_CUDA_OK(cudaSetDevice(k.s->device));
+            NK_CUDA_OK(cudaStreamSynchronize(k.s->stream));
+            for (double S : k.h_sums) prefix.push_back(T = T + S);
+        }
+        if (potential_out) potential_out[c] = T;
+        if (c + 1 == K) break;
+        // the next seed: the first chunk whose inclusive prefix reaches the target, then the first row of it whose running
+        // sum does; no chunk (a NaN sum or target): the last row, kmeans.go:397
+        const double target = u_host[c] * T;
+        const size_t j = std::find_if(prefix.begin(), prefix.end(), [&](double P) { return P >= target; }) - prefix.begin();
+        if (j == prefix.size()) { seed = n - 1; continue; }
+        size_t jj = j;
+        KmppShard *kj = nullptr;
+        for (auto &k : sh) {
+            if (jj < k.nch) { kj = &k; break; }
+            jj -= k.nch;
+        }
+        const uint64_t r0 = jj * nk::KMPP_CHUNK, cnt = std::min<uint64_t>(nk::KMPP_CHUNK, kj->s->n - r0);
+        NK_CUDA_OK(cudaSetDevice(kj->s->device));
+        NK_CUDA_OK(cudaMemcpyAsync(w.data(), kj->d2 + r0, cnt * 8, cudaMemcpyDeviceToHost, kj->s->stream));
+        NK_CUDA_OK(cudaStreamSynchronize(kj->s->stream));
+        const double before = j ? prefix[j - 1] : 0.0;
+        uint64_t pick = cnt - 1;  // reached at the latest by the chunk's last row: its running sum is S_j, added in the same order
+        double L = 0.0;
+        for (uint64_t i = 0; i < cnt; ++i) {
+            L = L + w[i];
+            if (before + L >= target) { pick = i; break; }
+        }
+        seed = kj->first + r0 + pick;
+    }
+    uint64_t total_read = 0;
+    for (auto &k : sh) {
+        NkShard &s = *k.s;
+        unsigned long long r = 0;
+        NK_CUDA_OK(cudaSetDevice(s.device));
+        if (min_d2_out) NK_CUDA_OK(cudaMemcpyAsync(min_d2_out + k.first, k.d2, s.n * 8, cudaMemcpyDeviceToHost, s.stream));
+        NK_CUDA_OK(cudaMemcpyAsync(&r, k.read, 8, cudaMemcpyDeviceToHost, s.stream));
+        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+        total_read += r;
+    }
+    ix->stats.bytes_scanned += total_read * rowb;
+    if (rows_read) *rows_read = total_read;
+    return 0;
+}
+
 // ---- best-of-chunks per node (db.index.vector.queryNodes, call_vector.go:177-256; SURVEY.md §8(f)2) -------------------------
 // Rows are chunk embeddings; group_of_row[r] = the node row r belongs to (ids in [0, n_groups)).  Stays set until a
 // row-count changing mutation (like the row mask, whose bits are positions).

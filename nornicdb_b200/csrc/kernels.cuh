@@ -245,6 +245,14 @@ int decode_group_keys(const uint64_t *keys, uint32_t k, int metric, const uint32
 int cluster_sums(const float *rows, uint64_t n, uint32_t dim, const int32_t *assign, uint32_t K, double *sums,
                  unsigned long long *counts, cudaStream_t s);
 int count_changed(const int32_t *a, const uint32_t *b, uint64_t n, unsigned long long *changed, cudaStream_t s);
+// k-means++ seeding (kmeanspp.cu): the pass of seed c (row c of the shard's [K x dim] seed list `seeds`) over a shard.  c = 0
+// sets d2 (and near = 0); c > 0 first computes delta[j] = sq_euclid64(seed c, seed j) for j < c, then lowers d2[i] (near[i]
+// = c) where the new distance is strictly smaller; rows the triangle inequality proves unchanged are skipped when `prune`.
+// chunk_sum[j] = sequential fp64 sum of d2 over rows [KMPP_CHUNK j, KMPP_CHUNK (j + 1)); *rows_read += rows computed.
+constexpr uint32_t KMPP_CHUNK = 256;
+int kmeanspp_pass(const DeviceInfo &di, const float *rows, uint64_t n, uint32_t dim, const float *seeds, uint32_t c, double *delta,
+                  bool prune, double *d2, uint32_t *near, double *chunk_sum, unsigned long long *rows_read, cudaStream_t stream,
+                  uint64_t *launches);
 int convert_f32_to_16(const float *src, void *dst, int dtype, size_t n, cudaStream_t s);  // fp16 / bf16, round to nearest even like the host's astype
 // out[r] = rows[idx[r]]: in the rows' dtype, or (out_f32) widened exactly to fp32
 int gather_rows(const void *rows, int dtype, uint32_t dim, const uint32_t *idx, uint32_t n_idx, void *out, bool out_f32,

@@ -6,7 +6,7 @@ time by one fused distance + top-k kernel per shard."""
 from __future__ import annotations
 
 import ctypes as C
-from typing import List, Optional, Sequence, Tuple
+from typing import List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -500,6 +500,33 @@ class KnnIndex:
         _check(self.lib.nk_index_cluster_means(self.ptr, a.ctypes.data_as(C.c_void_p), c.shape[0], c.ctypes.data_as(C.c_void_p),
                                                counts.ctypes.data_as(C.c_void_p)), "nk_index_cluster_means")
         return c, counts
+
+    def kmeanspp(self, K: int, first_row: int, u, min_d2: bool = False) -> "KmeansppSeeds":
+        """initCentroidsKMeansPlusPlus (kmeans.go:364-426) over every row, on the device: `first_row` plays rand.Intn(n) and
+        `u` (K-1 floats in [0, 1)) rand.Float64() for seeds 1 .. K-1.  Returns (seeds uint32 [K], centroids float32 [K x dim],
+        potential float64 [K]: the D² total after seeds 0..c, min_d2 float64 [rows] or None, rows_read)."""
+        K = int(K)
+        uu = np.ascontiguousarray(np.asarray(u, dtype=np.float64).reshape(-1))
+        if K < 1 or uu.size != K - 1:
+            raise KnnError(f"kmeanspp: K={K} needs K-1 uniforms, got {uu.size}")
+        seeds = np.empty(K, dtype=np.uint32)
+        cen = np.empty((K, self.dim), dtype=np.float32)
+        pot = np.empty(K, dtype=np.float64)
+        d2 = np.empty(len(self), dtype=np.float64) if min_d2 else None
+        read = C.c_uint64(0)
+        _check(self.lib.nk_index_kmeanspp(self.ptr, K, int(first_row), uu.ctypes.data_as(C.c_void_p) if uu.size else None,
+                                          seeds.ctypes.data_as(C.c_void_p), cen.ctypes.data_as(C.c_void_p),
+                                          pot.ctypes.data_as(C.c_void_p), d2.ctypes.data_as(C.c_void_p) if d2 is not None else None,
+                                          C.byref(read)), "nk_index_kmeanspp")
+        return KmeansppSeeds(seeds, cen, pot, d2, int(read.value))
+
+
+class KmeansppSeeds(NamedTuple):
+    seeds: np.ndarray
+    centroids: np.ndarray
+    potential: np.ndarray
+    min_d2: Optional[np.ndarray]
+    rows_read: int
 
 
 ALL_BITS = 0xFFFFFFFFFFFFFFFF
