@@ -252,7 +252,9 @@ int nk_search_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uint32_t
  * Tags live per shard in device memory (8 B per row) and follow the rows: append gives new rows tag 0, update_row keeps the
  * tag, remove_swap moves the last row's tag with its row; upload, upload_from_f32, fill_* and attach_device_rows reset every
  * tag to 0.
- * Not filtered: nk_search_groups, nk_score_subset, nk_search_keys_device, nk_search_sharded_device and the k-means calls. */
+ * Not filtered: nk_search_groups, nk_score_subset, nk_search_keys_device, nk_search_sharded_device and the k-means calls.
+ * Not windowed (value windows, below): nk_search_rows*, nk_search_pairs, the graph update and remap calls, nk_search_groups,
+ * nk_score_subset, nk_search_keys_device, nk_search_sharded_device, the exchange calls and the k-means calls. */
 typedef struct NkFilter {
     uint64_t all_of, none_of, any_of;
 } NkFilter;
@@ -265,6 +267,33 @@ int nk_search_filtered(NkIndex *ix, const float *queries_host, const NkFilter *f
  * has run the search. */
 int nk_search_filtered_device(NkIndex *ix, const float *queries_dev, const NkFilter *filters_dev, uint32_t Q, uint32_t k,
                               uint32_t *out_idx_dev, float *out_score_dev, void *stream);
+
+/* Per-query value windows: numeric range conditions (Qdrant Range / DatetimeRange, "the last 7 days", "under a price")
+ * evaluated inside the scan, in the same corpus pass as the tag filters.
+ * Every row carries one 64-bit VALUE KEY; rows that were never given a value have key 0.  Keys are compared as unsigned
+ * integers only: the caller encodes its numbers so that key order is number order (nornicdb_b200.knn.value_keys: int64
+ * v ^ 2^63; doubles by their order-preserving bit pattern; key 0 is kept for "no value").  Each query carries an NkWindow;
+ * row r is admissible for the query iff  lo <= value[r] <= hi  AND the query's tag filter admits tag[r] (NULL filters: every
+ * tag), with the row mask and the score floor as in nk_search_filtered.  {0, ~0} admits every row; lo > hi admits none; a
+ * window with lo >= 1 never admits a row without a value.
+ * Results, order, ties, padding (0xffffffff / 0), return values and the k clamp: those of nk_search_filtered /
+ * nk_search_filtered_device; the range call's size protocol: that of nk_search_range.  windows == NULL: each call IS its
+ * counterpart (same kernels, bit-identical output).  Any number of devices, as for the counterparts.
+ * Values live per shard in device memory (8 B per row) and follow the rows exactly as tags do: append gives new rows key 0,
+ * update_row keeps the key, remove_swap moves the last row's key with its row; upload, upload_from_f32, fill_* and
+ * attach_device_rows reset every key to 0. */
+typedef struct NkWindow {
+    uint64_t lo, hi; /* row r admissible iff lo <= value[r] <= hi (unsigned) */
+} NkWindow;
+/* Value keys of rows [first_row, first_row + n_rows) (global, relative to the index's first row); may span shards. */
+int nk_index_set_row_values(NkIndex *ix, uint64_t first_row, const uint64_t *keys_host, uint64_t n_rows);
+/* nk_search_filtered with one value window per query (windows_host [Q], NULL = none; filters_host NULL = no tag filter). */
+int nk_search_windowed(NkIndex *ix, const float *queries_host, const NkFilter *filters_host, const NkWindow *windows_host,
+                       uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score);
+/* nk_search_filtered_device with one value window per query: windows_dev [Q] device memory (NULL = none) that, like
+ * filters_dev, must stay valid until `stream` has run the search. */
+int nk_search_windowed_device(NkIndex *ix, const float *queries_dev, const NkFilter *filters_dev, const NkWindow *windows_dev,
+                              uint32_t Q, uint32_t k, uint32_t *out_idx_dev, float *out_score_dev, void *stream);
 
 /* ---- Search by stored row ----------------------------------------------------------------------------------------------
  * The k nearest OTHER rows of stored rows ("which nodes are like this node?", FindSimilar, OnStore's related-node search, the
@@ -307,6 +336,10 @@ int nk_search_rows_filtered(NkIndex *ix, const uint32_t *rows_host, const NkFilt
 int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresholds_host, const NkFilter *filters_host,
                     uint32_t Q, uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx, float *out_score,
                     uint64_t *out_total);
+/* nk_search_range with one value window per query (windows_host [Q], NULL = none: then nk_search_range bit for bit). */
+int nk_search_range_windowed(NkIndex *ix, const float *queries_host, const float *thresholds_host, const NkFilter *filters_host,
+                             const NkWindow *windows_host, uint32_t Q, uint64_t capacity, uint64_t *out_offsets,
+                             uint32_t *out_idx, float *out_score, uint64_t *out_total);
 
 /* ---- Similarity self-join ----------------------------------------------------------------------------------------------
  * Every pair of stored rows whose similarity reaches one threshold (near-duplicate detection, threshold auto-linking of a

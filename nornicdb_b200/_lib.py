@@ -77,6 +77,10 @@ SIGNATURES = {
     "nk_search_filtered": (_i, [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp]),
     "nk_search_filtered_device": (_i, [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp]),
     "nk_search_range": (_i, [_vp, _vp, _vp, _vp, C.c_uint32, _u64, _vp, _vp, _vp, _vp]),
+    "nk_index_set_row_values": (_i, [_vp, _u64, _vp, _u64]),
+    "nk_search_windowed": (_i, [_vp, _vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp]),
+    "nk_search_windowed_device": (_i, [_vp, _vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp]),
+    "nk_search_range_windowed": (_i, [_vp, _vp, _vp, _vp, _vp, C.c_uint32, _u64, _vp, _vp, _vp, _vp]),
     "nk_search_rows": (_i, [_vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp]),
     "nk_search_rows_filtered": (_i, [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp]),
     "nk_search_pairs": (_i, [_vp, _u64, _u64, C.c_float, _vp, _u64, _vp, _vp, _vp, _vp]),

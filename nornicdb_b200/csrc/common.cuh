@@ -118,6 +118,12 @@ __device__ __forceinline__ bool tag_admits(uint64_t tag, const NkFilter *f) {
     return tag_admits(tag, __ldg(&f->all_of), __ldg(&f->none_of), __ldg(&f->any_of));
 }
 #endif
+// Per-query value window (nk_search_windowed): may a row with value key v be returned for a query with window [lo, hi]?
+__host__ __device__ __forceinline__ bool window_admits(uint64_t v, uint64_t lo, uint64_t hi) { return lo <= v && v <= hi; }
+#ifdef __CUDACC__
+// The same against a device window array [Q] (16 B per query, shared by every row).
+__device__ __forceinline__ bool window_admits(uint64_t v, const NkWindow *w) { return window_admits(v, __ldg(&w->lo), __ldg(&w->hi)); }
+#endif
 
 // Counter-based U[-1,1) generator, bit-identical to oracle/knn_oracle.c orc_uniform_at().
 __host__ __device__ __forceinline__ uint64_t mix64(uint64_t z) {

@@ -76,6 +76,10 @@ struct NkShard {
     uint64_t *tags = nullptr;
     uint64_t tags_cap = 0;
     bool tags_on = false;
+    // value key per local row (nk_index_set_row_values), kept exactly like the tags; values_on = false: every key is 0
+    uint64_t *values = nullptr;
+    uint64_t values_cap = 0;
+    bool values_on = false;
     size_t cvt_bytes = 0;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> timing;  // pending scan-kernel event pairs
     std::vector<uint64_t> timing_launches;
@@ -208,31 +212,35 @@ static void decode_key(int metric, uint64_t key, uint32_t *row, float *score) {
     *score = metric == NK_METRIC_EUCLIDEAN ? sqrtf(std::max(-sc, 0.0f)) : sc;
 }
 
-// ---- per-row tag words (nk_search_filtered) ---------------------------------------------------------------------------
-// The array follows the rows: rows [old_n, s.n) are new and get tag 0; the capacity follows the row capacity.  Synchronous,
+// ---- per-row tag words (nk_search_filtered) and value keys (nk_search_windowed) -------------------------------------
+// One 64-bit word per row, in a shard array (words, cap, on) = (tags, tags_cap, tags_on) or (values, values_cap, values_on).
+// The array follows the rows: rows [old_n, s.n) are new and get word 0; the capacity follows the row capacity.  Synchronous,
 // so a search on any stream may read the array afterwards.
-static int shard_tags_grow(NkShard &s, uint64_t old_n) {
-    if (s.tags_cap < s.n) {
+static int shard_words_grow(NkShard &s, uint64_t *&words, uint64_t &words_cap, uint64_t old_n) {
+    if (words_cap < s.n) {
         const uint64_t cap = std::max<uint64_t>(std::max(s.cap, s.n), 16);
         uint64_t *p = nullptr;
         NK_CUDA_OK(cudaMalloc((void **)&p, cap * 8));
-        if (s.tags && old_n) NK_CUDA_OK(cudaMemcpyAsync(p, s.tags, old_n * 8, cudaMemcpyDeviceToDevice, s.stream));
+        if (words && old_n) NK_CUDA_OK(cudaMemcpyAsync(p, words, old_n * 8, cudaMemcpyDeviceToDevice, s.stream));
         if (shard_drain(s)) return -1;
-        if (s.tags) NK_CUDA_OK(cudaFree(s.tags));
-        s.tags = p;
-        s.tags_cap = cap;
+        if (words) NK_CUDA_OK(cudaFree(words));
+        words = p;
+        words_cap = cap;
     }
-    if (s.n > old_n) NK_CUDA_OK(cudaMemsetAsync(s.tags + old_n, 0, (s.n - old_n) * 8, s.stream));
+    if (s.n > old_n) NK_CUDA_OK(cudaMemsetAsync(words + old_n, 0, (s.n - old_n) * 8, s.stream));
     NK_CUDA_OK(cudaStreamSynchronize(s.stream));
     return 0;
 }
-// Make the shard's tag array real (all zero if the rows were never tagged since the last reset).
-static int shard_tags_on(NkShard &s) {
-    if (s.tags_on) return 0;
-    if (shard_tags_grow(s, 0)) return -1;
-    s.tags_on = true;
+// Make the array real (all zero if its words were never set since the last reset).
+static int shard_words_on(NkShard &s, uint64_t *&words, uint64_t &words_cap, bool &on) {
+    if (on) return 0;
+    if (shard_words_grow(s, words, words_cap, 0)) return -1;
+    on = true;
     return 0;
 }
+static int shard_tags_grow(NkShard &s, uint64_t old_n) { return shard_words_grow(s, s.tags, s.tags_cap, old_n); }
+static int shard_tags_on(NkShard &s) { return shard_words_on(s, s.tags, s.tags_cap, s.tags_on); }
+static int shard_values_on(NkShard &s) { return shard_words_on(s, s.values, s.values_cap, s.values_on); }
 
 // Convert rows [first, first+count) into every image the shard has (one launch counted): the int8 image and / or the BF16
 // shadow with their norms (fp32 shards), or the |x|^2 array (16-bit shards).
@@ -378,14 +386,16 @@ static NkShard *find_shard(NkIndex *ix, uint64_t row, uint64_t *local) {
 }
 
 // The scan of Q device queries over shard s as it stands: its rows, the row mask and the score floor; qfilter (per-query tag
-// filters [Q] on the device, nullptr = none) needs the shard's tag array on.
+// filters [Q] on the device, nullptr = none) needs the shard's tag array on; qwindow (per-query value windows [Q] on the
+// device, nullptr = none) needs qfilter and the shard's value array on.
 static nk::ScanArgs shard_scan_args(const NkIndex *ix, const NkShard &s, const float *q_dev, uint32_t Q, uint32_t k,
-                                    cudaStream_t stream, const NkFilter *qfilter = nullptr) {
+                                    cudaStream_t stream, const NkFilter *qfilter = nullptr, const NkWindow *qwindow = nullptr) {
     nk::ScanArgs a;
     a.rows = s.rows; a.dtype = ix->dtype; a.n = (uint32_t)s.n; a.dim = ix->dim; a.row_base = s.base;
     a.queries = q_dev; a.Q = Q; a.k = k; a.metric = ix->metric; a.stream = stream;
     a.row_mask = s.mask_on ? s.mask : nullptr; a.min_score = ix->key_floor();
     if (qfilter) { a.row_tags = s.tags; a.qfilter = qfilter; a.mode = nk::ScanMode::KNN_TAGS; }
+    if (qwindow) { a.row_values = s.values; a.qwindow = qwindow; a.mode = nk::ScanMode::KNN_WINDOW; }
     return a;
 }
 
@@ -541,11 +551,12 @@ struct ScanOut {  // what a call asks of run_scan beyond the queries
     float *out_score = nullptr;
     DeferredTail *tail = nullptr;  // host-synchronous caller: retry stages are left to *tail, queued only if a flag was raised
     const NkFilter *qfilter = nullptr;  // per-query tag filters [Q] (device; the shard's tag array must be on)
+    const NkWindow *qwindow = nullptr;  // per-query value windows [Q] (device; with qfilter, the shard's value array on)
 };
 
 static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uint32_t k, uint64_t *out_keys,
                     cudaStream_t stream, const ScanOut &xo) {
-    nk::ScanArgs a = shard_scan_args(ix, s, q_dev, Q, k, stream, xo.qfilter);
+    nk::ScanArgs a = shard_scan_args(ix, s, q_dev, Q, k, stream, xo.qfilter, xo.qwindow);
     if (k > NK_MAX_K) {
         if (run_scan_bigk(ix, s, a, out_keys)) return -1;
         if (xo.out_idx) {
@@ -678,6 +689,7 @@ void nk_index_release(NkIndex *ix) {
         if (s.cvt) cudaFree(s.cvt);
         if (s.mask) cudaFree(s.mask);
         if (s.tags) cudaFree(s.tags);
+        if (s.values) cudaFree(s.values);
         if (s.group) cudaFree(s.group);
         s.ws.release();
     }
@@ -703,6 +715,7 @@ static int repartition(NkIndex *ix, uint64_t n_rows, const WriteRows &write) {
         if (!s.owns) { s.rows = nullptr; s.owns = true; s.cap = 0; s.img.attached = false; }
         s.n = 0;
         s.tags_on = false;  // every tag back to 0
+        s.values_on = false;  // every value key back to 0
         if (shard_reserve_rows(ix, s, cnt, false)) return -1;
         if (write(s, off, cnt)) return -1;
         s.n = cnt;
@@ -773,6 +786,7 @@ int nk_index_append(NkIndex *ix, const void *rows_host, uint64_t n_rows) {
     if (stream_h2d(s, (char *)s.rows + s.n * rb, rows_host, n_rows * rb)) return -1;
     s.n += n_rows;
     if (s.tags_on && shard_tags_grow(s, s.n - n_rows)) return -1;  // appended rows: tag 0
+    if (s.values_on && shard_words_grow(s, s.values, s.values_cap, s.n - n_rows)) return -1;  // ... and value key 0
     if (shard_sync_shadow(ix, s)) return -1;  // converts only the appended rows (all of them if the shard was regrown)
     NK_CUDA_OK(cudaStreamSynchronize(s.stream));
     ix->stats.bytes_h2d += n_rows * rb;
@@ -839,6 +853,16 @@ int nk_index_remove_swap(NkIndex *ix, uint64_t row) {
             if (shard_tags_on(*s)) return -1;
             NK_CUDA_OK(cudaMemcpy(s->tags + local, &tag, 8, cudaMemcpyHostToDevice));
         }
+        if (last->values_on || s->values_on) {  // ... and so does its value key
+            uint64_t val = 0;
+            if (last->values_on) {
+                NK_CUDA_OK(cudaSetDevice(last->device));
+                NK_CUDA_OK(cudaMemcpy(&val, last->values + (last->n - 1), 8, cudaMemcpyDeviceToHost));
+            }
+            NK_CUDA_OK(cudaSetDevice(s->device));
+            if (shard_values_on(*s)) return -1;
+            NK_CUDA_OK(cudaMemcpy(s->values + local, &val, 8, cudaMemcpyHostToDevice));
+        }
     }
     last->n -= 1;
     if (last->img.n > last->n) last->img.n = last->n;
@@ -893,6 +917,7 @@ int nk_index_attach_device_rows(NkIndex *ix, void *rows_dev, uint64_t n_rows) {
     drop_row_mask(ix);
     s.rows = rows_dev; s.owns = false; s.n = n_rows; s.cap = n_rows; s.img.attached = false;
     s.tags_on = false;  // every tag back to 0
+    s.values_on = false;  // every value key back to 0
     rebase(ix);
     return 0;
 }
@@ -971,15 +996,17 @@ int nk_index_set_row_mask(NkIndex *ix, const uint32_t *mask_words, uint64_t n_bi
     return 0;
 }
 
-int nk_index_set_row_tags(NkIndex *ix, uint64_t first_row, const uint64_t *tags_host, uint64_t n_rows) {
+// nk_index_set_row_tags (values = false) / nk_index_set_row_values (values = true): words of rows [first_row, first_row + n_rows).
+static int set_row_words(NkIndex *ix, uint64_t first_row, const uint64_t *words_host, uint64_t n_rows, bool values) {
     nk::DeviceGuard _restore_device;
+    const char *what = values ? "values" : "tags";
     if (!ix) { nk::set_error("null index"); return -1; }
     if (n_rows == 0) return 0;
-    if (!tags_host) { nk::set_error("null tags"); return -1; }
+    if (!words_host) { nk::set_error("null %s", what); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
     const uint64_t total = ix->rows();
     if (first_row > total || n_rows > total - first_row) {
-        nk::set_error("row tags [%llu, %llu) out of range (index has %llu rows)", (unsigned long long)first_row,
+        nk::set_error("row %s [%llu, %llu) out of range (index has %llu rows)", what, (unsigned long long)first_row,
                       (unsigned long long)(first_row + n_rows), (unsigned long long)total);
         return -1;
     }
@@ -990,13 +1017,21 @@ int nk_index_set_row_tags(NkIndex *ix, uint64_t first_row, const uint64_t *tags_
         NkShard *s = find_shard(ix, first_row + i, &local);
         const uint64_t cnt = std::min<uint64_t>(n_rows - i, s->n - local);
         NK_CUDA_OK(cudaSetDevice(s->device));
-        if (shard_tags_on(*s)) return -1;
-        NK_CUDA_OK(cudaMemcpyAsync(s->tags + local, tags_host + i, cnt * 8, cudaMemcpyHostToDevice, s->stream));
+        if (values ? shard_values_on(*s) : shard_tags_on(*s)) return -1;
+        NK_CUDA_OK(cudaMemcpyAsync((values ? s->values : s->tags) + local, words_host + i, cnt * 8, cudaMemcpyHostToDevice, s->stream));
         NK_CUDA_OK(cudaStreamSynchronize(s->stream));
         ix->stats.bytes_h2d += cnt * 8;
         i += cnt;
     }
     return 0;
+}
+
+int nk_index_set_row_tags(NkIndex *ix, uint64_t first_row, const uint64_t *tags_host, uint64_t n_rows) {
+    return set_row_words(ix, first_row, tags_host, n_rows, false);
+}
+
+int nk_index_set_row_values(NkIndex *ix, uint64_t first_row, const uint64_t *keys_host, uint64_t n_rows) {
+    return set_row_words(ix, first_row, keys_host, n_rows, true);
 }
 
 int nk_index_set_path(NkIndex *ix, int path) {
@@ -1152,11 +1187,34 @@ static const NkFilter *stage_filters(NkIndex *ix, NkShard &s, const NkFilter *fi
     return s.ws.qfilter;
 }
 
+// Per-query value windows of a host search -> the shard workspace next to its filters, with the shard's tag and value arrays
+// on.  A windowed scan always applies a tag filter as well: without filters_host the filters staged are {0,0,0}, which admit
+// every row.  *qfilter / *qwindow: the device copies.
+static int stage_windows(NkIndex *ix, NkShard &s, const NkFilter *filters_host, const NkWindow *windows_host, uint32_t Q,
+                         const NkFilter **qfilter, const NkWindow **qwindow) {
+    if (filters_host) {
+        if (!(*qfilter = stage_filters(ix, s, filters_host, Q))) return -1;
+    } else {
+        if (shard_tags_on(s)) return -1;
+        if (nk::ws_reserve((void **)&s.ws.qfilter, &s.ws.qfilter_bytes, (size_t)Q * sizeof(NkFilter))) return -1;
+        NK_CUDA_OK(cudaMemsetAsync(s.ws.qfilter, 0, (size_t)Q * sizeof(NkFilter), s.stream));
+        *qfilter = s.ws.qfilter;
+    }
+    const size_t wbytes = (size_t)Q * sizeof(NkWindow);
+    if (shard_values_on(s)) return -1;
+    if (nk::ws_reserve((void **)&s.ws.qwindow, &s.ws.qwindow_bytes, wbytes)) return -1;
+    NK_CUDA_OK(cudaMemcpyAsync(s.ws.qwindow, windows_host, wbytes, cudaMemcpyHostToDevice, s.stream));
+    ix->stats.bytes_h2d += wbytes;
+    *qwindow = s.ws.qwindow;
+    return 0;
+}
+
 // What one call asks of every search it runs, passed down by reference: the scan path (the index's setting, or the one a
-// graph call chose) and the per-query tag filters of its queries.
+// graph call chose) and the per-query tag filters and value windows of its queries.
 struct SearchOpts {
     int path;
     const NkFilter *filters_host = nullptr;  // [Q], nullptr: none
+    const NkWindow *windows_host = nullptr;  // [Q], nullptr: none
 };
 
 // One synchronous search of Q staged queries over the live (non-empty) shards, the index lock held: scan, deferred retry
@@ -1185,7 +1243,11 @@ static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const St
             xo.out_idx = s->ws.out_idx; xo.out_score = s->ws.out_score;
         }
         if (stage(*s)) return -1;
-        if (opts.filters_host && !(xo.qfilter = stage_filters(ix, *s, opts.filters_host, Q))) return -1;
+        if (opts.windows_host) {
+            if (stage_windows(ix, *s, opts.filters_host, opts.windows_host, Q, &xo.qfilter, &xo.qwindow)) return -1;
+        } else if (opts.filters_host && !(xo.qfilter = stage_filters(ix, *s, opts.filters_host, Q))) {
+            return -1;
+        }
         if (run_scan(ix, *s, s->ws.queries, Q, ke, s->ws.keys, s->stream, xo)) return -1;
     }
 
@@ -1259,9 +1321,9 @@ static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const St
     return (int)ke;
 }
 
-// nk_search / nk_search_filtered: filters_host == nullptr is plain nk_search.
-static int search_host(NkIndex *ix, const float *queries_host, const NkFilter *filters_host, uint32_t Q, uint32_t k, uint32_t *out_idx,
-                       float *out_score) {
+// nk_search / nk_search_filtered / nk_search_windowed: filters_host == windows_host == nullptr is plain nk_search.
+static int search_host(NkIndex *ix, const float *queries_host, const NkFilter *filters_host, const NkWindow *windows_host, uint32_t Q,
+                       uint32_t k, uint32_t *out_idx, float *out_score) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
     std::lock_guard<std::mutex> lk(ix->mu);
@@ -1283,16 +1345,21 @@ static int search_host(NkIndex *ix, const float *queries_host, const NkFilter *f
         ix->stats.bytes_h2d += qbytes;
         return 0;
     };
-    return search_live(ix, live, upload, SearchOpts{ix->path, filters_host}, Q, ke, k, out_idx, out_score);
+    return search_live(ix, live, upload, SearchOpts{ix->path, filters_host, windows_host}, Q, ke, k, out_idx, out_score);
 }
 
 int nk_search(NkIndex *ix, const float *queries_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
-    return search_host(ix, queries_host, nullptr, Q, k, out_idx, out_score);
+    return search_host(ix, queries_host, nullptr, nullptr, Q, k, out_idx, out_score);
 }
 
 int nk_search_filtered(NkIndex *ix, const float *queries_host, const NkFilter *filters_host, uint32_t Q, uint32_t k,
                        uint32_t *out_idx, float *out_score) {
-    return search_host(ix, queries_host, filters_host, Q, k, out_idx, out_score);
+    return search_host(ix, queries_host, filters_host, nullptr, Q, k, out_idx, out_score);
+}
+
+int nk_search_windowed(NkIndex *ix, const float *queries_host, const NkFilter *filters_host, const NkWindow *windows_host,
+                       uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
+    return search_host(ix, queries_host, filters_host, windows_host, Q, k, out_idx, out_score);
 }
 
 // ---- search by stored row (DESIGN.md §3.5c) ---------------------------------------------------------------------------
@@ -1476,6 +1543,7 @@ struct RangeBlock {
     uint32_t Q;
     const uint32_t *thr;                   // [Q] thresholds in key space, as nk::ord_bits (host)
     bool filtered = false;
+    bool windowed = false;                 // (with `filtered`) the same step wrote per-query value windows into s.ws.qwindow
     const uint64_t *pair_first = nullptr;  // the self-join's triangle: see range_scan_shard
     // The reverse scan of a k-NN graph update.  Every row has its own threshold, s.ws.row_thr [s.n], and the mask words behind
     // them, s.ws.row_thr + s.n, TAKE THE PLACE OF the index's row mask: they select the rows whose lists are updated, not the
@@ -1490,10 +1558,10 @@ struct RangeBlock {
 // on the base).
 static int range_shard(NkIndex *ix, NkShard &s, const RangeBlock &b, uint64_t from, int *counts, uint32_t *list_cap) {
     // Paths: the 16-bit and TF32 filters with fixed thresholds, or the CUDA-core scan.
-    nk::ScanArgs a = shard_scan_args(ix, s, s.ws.queries, b.Q, 1, s.stream, b.filtered ? s.ws.qfilter : nullptr);
+    nk::ScanArgs a = shard_scan_args(ix, s, s.ws.queries, b.Q, 1, s.stream, b.filtered ? s.ws.qfilter : nullptr, b.windowed ? s.ws.qwindow : nullptr);
     const int use = plan_path(ix, s, b.path, true, &a);
     if (use < 0) return -1;
-    a.mode = b.filtered ? nk::ScanMode::RANGE_TAGS : nk::ScanMode::RANGE;
+    a.mode = b.windowed ? nk::ScanMode::RANGE_WINDOW : b.filtered ? nk::ScanMode::RANGE_TAGS : nk::ScanMode::RANGE;
     if (b.reverse) {
         a.mode = b.row_filters ? nk::ScanMode::REVERSE_RFILT : b.filtered ? nk::ScanMode::REVERSE_TAGS : nk::ScanMode::REVERSE;
         a.row_thr = s.ws.row_thr;
@@ -1506,6 +1574,7 @@ static int range_shard(NkIndex *ix, NkShard &s, const RangeBlock &b, uint64_t fr
         a.row_base = s.base + from;
         if (a.row_mask) a.row_mask += from / 32;
         if (a.row_tags) a.row_tags += from;
+        if (a.row_values) a.row_values += from;
         a.image = a.image.window(from);
     }
     ScanTimer timer(s);
@@ -1574,6 +1643,13 @@ static int range_collect(NkIndex *ix, const RangeShards &on, uint32_t Q, std::ve
 
 int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresholds_host, const NkFilter *filters_host, uint32_t Q,
                     uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total) {
+    return nk_search_range_windowed(ix, queries_host, thresholds_host, filters_host, nullptr, Q, capacity, out_offsets, out_idx, out_score,
+                                    out_total);
+}
+
+int nk_search_range_windowed(NkIndex *ix, const float *queries_host, const float *thresholds_host, const NkFilter *filters_host,
+                             const NkWindow *windows_host, uint32_t Q, uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx,
+                             float *out_score, uint64_t *out_total) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
     if (!out_offsets || !out_total) { nk::set_error("null argument"); return -1; }
@@ -1597,10 +1673,16 @@ int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresho
     const StageQueries upload = [&](NkShard &s) {
         NK_CUDA_OK(cudaMemcpyAsync(s.ws.queries, queries_host, qbytes, cudaMemcpyHostToDevice, s.stream));
         ix->stats.bytes_h2d += qbytes;
+        if (windows_host) {
+            const NkFilter *qf;
+            const NkWindow *qw;
+            return stage_windows(ix, s, filters_host, windows_host, Q, &qf, &qw);
+        }
         return filters_host && !stage_filters(ix, s, filters_host, Q) ? -1 : 0;
     };
     RangeBlock block{ix->path, Q, thr.data()};
-    block.filtered = filters_host != nullptr;
+    block.filtered = filters_host != nullptr || windows_host != nullptr;
+    block.windowed = windows_host != nullptr;
     std::vector<uint64_t> per_query;
     if (range_scan(ix, &on, upload, block, &per_query)) return -1;
     // offsets: the shards' survivors of query q are merged into one run
@@ -2220,9 +2302,10 @@ int nk_search_keys_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uin
     return search_keys_locked(ix, s, queries_dev, Q, k, out_keys_dev, st);
 }
 
-// nk_search_device / nk_search_filtered_device: filters_dev == nullptr is plain nk_search_device.
-static int search_device(NkIndex *ix, const float *queries_dev, const NkFilter *filters_dev, uint32_t Q, uint32_t k, uint32_t *out_idx_dev,
-                         float *out_score_dev, void *stream) {
+// nk_search_device / nk_search_filtered_device / nk_search_windowed_device: filters_dev == windows_dev == nullptr is plain
+// nk_search_device.
+static int search_device(NkIndex *ix, const float *queries_dev, const NkFilter *filters_dev, const NkWindow *windows_dev, uint32_t Q,
+                         uint32_t k, uint32_t *out_idx_dev, float *out_score_dev, void *stream) {
     nk::DeviceGuard _restore_device;
     NkShard *s;
     if (single_shard(ix, &s)) return -1;
@@ -2246,18 +2329,33 @@ static int search_device(NkIndex *ix, const float *queries_dev, const NkFilter *
         if (shard_tags_on(*s)) return -1;
         xo.qfilter = filters_dev;  // the caller keeps it valid until the stream has run (the blindly queued tail reads it too)
     }
+    if (windows_dev) {
+        if (shard_values_on(*s)) return -1;
+        if (!filters_dev) {  // a windowed scan also applies a tag filter: {0,0,0} for every query, staged on the caller's stream
+            if (shard_tags_on(*s)) return -1;
+            if (nk::ws_reserve((void **)&s->ws.qfilter, &s->ws.qfilter_bytes, (size_t)Q * sizeof(NkFilter))) return -1;
+            NK_CUDA_OK(cudaMemsetAsync(s->ws.qfilter, 0, (size_t)Q * sizeof(NkFilter), st));
+            xo.qfilter = s->ws.qfilter;
+        }
+        xo.qwindow = windows_dev;  // kept valid by the caller, as filters_dev
+    }
     if (run_scan(ix, *s, queries_dev, Q, k, s->ws.keys, st, xo)) return -1;
     return (int)k;
 }
 
 int nk_search_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uint32_t k, uint32_t *out_idx_dev,
                      float *out_score_dev, void *stream) {
-    return search_device(ix, queries_dev, nullptr, Q, k, out_idx_dev, out_score_dev, stream);
+    return search_device(ix, queries_dev, nullptr, nullptr, Q, k, out_idx_dev, out_score_dev, stream);
 }
 
 int nk_search_filtered_device(NkIndex *ix, const float *queries_dev, const NkFilter *filters_dev, uint32_t Q, uint32_t k,
                               uint32_t *out_idx_dev, float *out_score_dev, void *stream) {
-    return search_device(ix, queries_dev, filters_dev, Q, k, out_idx_dev, out_score_dev, stream);
+    return search_device(ix, queries_dev, filters_dev, nullptr, Q, k, out_idx_dev, out_score_dev, stream);
+}
+
+int nk_search_windowed_device(NkIndex *ix, const float *queries_dev, const NkFilter *filters_dev, const NkWindow *windows_dev,
+                              uint32_t Q, uint32_t k, uint32_t *out_idx_dev, float *out_score_dev, void *stream) {
+    return search_device(ix, queries_dev, filters_dev, windows_dev, Q, k, out_idx_dev, out_score_dev, stream);
 }
 
 // Device-resident searches cannot report a (never expected) candidate-buffer overflow when they return: this call waits

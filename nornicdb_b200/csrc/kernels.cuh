@@ -35,6 +35,7 @@ struct Workspace {
     float *row_thr = nullptr;     size_t row_thr_bytes = 0;    // nk_knn_graph_update: per-row thresholds [n], then keep-mask words
     NkFilter *row_filter = nullptr; size_t row_filter_bytes = 0;  // filtered graph update: each row's own filter [n]
     uint64_t *qtags = nullptr;    size_t qtags_bytes = 0;      // ... and the tags of the reverse scan's queries [Q]
+    NkWindow *qwindow = nullptr;  size_t qwindow_bytes = 0;    // staged per-query value windows (host API, next to the filters)
     // cached TMA descriptors (tc_cached_map): re-encoded only when the base pointer or shape changes
     struct MapSlot {
         alignas(64) unsigned char bytes[128];
@@ -75,18 +76,24 @@ struct RowImage {
     }
 };
 
-// What a scan keeps and which filters it applies: the 8 kinds of scan.  ScanArgs::mode is set where the pointers it reads
+// What a scan keeps and which filters it applies: the 10 kinds of scan.  ScanArgs::mode is set where the pointers it reads
 // are attached (ScanArgs::check holds the two together); the tensor-core scan kernels take it as a template argument.
 //   KNN, KNN_TAGS           the k best rows per query: running thresholds, shared between CTAs; full buffers are pruned
+//   KNN_WINDOW              ... with per-query value windows on top of the tag filters
 //   RANGE, RANGE_TAGS       every row that reaches a fixed per-query threshold: full buffers are flushed to the lists
+//   RANGE_WINDOW            ... with per-query value windows on top of the tag filters
 //   REVERSE, REVERSE_TAGS   the graph update's reverse scan: a range scan whose pairs must also reach their row's threshold (row_thr)
 //   REVERSE_RFILT           ... of a filtered graph: the row's own filter (row_filter) must also admit the query's tag (qtags)
 //   DUMP                    tests only (scan_filter_dump): a kNN filter pass that also writes every pair's estimate and bound
-// The *_TAGS modes and REVERSE_RFILT apply per-query tag filters (row_tags, qfilter): a pair takes part only if the query
-// admits the row's tag.  The range modes (RANGE .. REVERSE_RFILT) and the reverse modes (REVERSE ..) are contiguous.
-enum class ScanMode { KNN, KNN_TAGS, RANGE, RANGE_TAGS, REVERSE, REVERSE_TAGS, REVERSE_RFILT, DUMP };
+// The *_TAGS and *_WINDOW modes and REVERSE_RFILT apply per-query tag filters (row_tags, qfilter): a pair takes part only if
+// the query admits the row's tag.  The window modes also apply per-query value windows (row_values, qwindow): a pair takes
+// part only if the row's value key lies in the query's window.  The range modes (RANGE .. REVERSE_RFILT) and the reverse
+// modes (REVERSE ..) are contiguous.
+enum class ScanMode { KNN, KNN_TAGS, KNN_WINDOW, RANGE, RANGE_TAGS, RANGE_WINDOW, REVERSE, REVERSE_TAGS, REVERSE_RFILT, DUMP };
+__host__ __device__ constexpr bool mode_window(ScanMode m) { return m == ScanMode::KNN_WINDOW || m == ScanMode::RANGE_WINDOW; }
 __host__ __device__ constexpr bool mode_tags(ScanMode m) {
-    return m == ScanMode::KNN_TAGS || m == ScanMode::RANGE_TAGS || m == ScanMode::REVERSE_TAGS || m == ScanMode::REVERSE_RFILT;
+    return m == ScanMode::KNN_TAGS || m == ScanMode::RANGE_TAGS || m == ScanMode::REVERSE_TAGS || m == ScanMode::REVERSE_RFILT ||
+           mode_window(m);
 }
 __host__ __device__ constexpr bool mode_range(ScanMode m) { return m >= ScanMode::RANGE && m <= ScanMode::REVERSE_RFILT; }
 __host__ __device__ constexpr bool mode_row_thr(ScanMode m) { return m >= ScanMode::REVERSE && m <= ScanMode::REVERSE_RFILT; }
@@ -137,6 +144,10 @@ struct ScanArgs {
     // tag_admits(qtags[q], row_filter + row), the mirror image of row_tags / qfilter
     const NkFilter *row_filter = nullptr;
     const uint64_t *qtags = nullptr;
+    // the window modes (mode_window): value key per local row, row_values [n], and window per query, qwindow [Q]; a (row,
+    // query) pair takes part only if window_admits(row_values[row], qwindow + q) (and the tag filter admits it)
+    const uint64_t *row_values = nullptr;
+    const NkWindow *qwindow = nullptr;
     // 0 if a range (else kNN) scan, on the CUDA cores (no reverse modes) or not, serves the mode and exactly the pointers the
     // mode reads are set; else set_error and -1.  No scan accepts DUMP: scan_filter_dump sets it on its own copy.
     int check(bool range, bool cuda_cores) const;

@@ -54,7 +54,14 @@ struct SimtRangeParams : SimtParams {
     int *range_fill;            // list fill per query [Q], counts past list_cap
     uint32_t list_cap;          // `partial` is [Q][list_cap]
 };
-template <bool RANGE> using SimtArgs = std::conditional_t<RANGE, SimtRangeParams, SimtParams>;
+// WINDOW kernels (the window modes) take the value windows on top of either block, so the other kernels' parameter offsets
+// stay as they are.
+template <bool RANGE> struct SimtWindowParams : std::conditional_t<RANGE, SimtRangeParams, SimtParams> {
+    const uint64_t *row_values;  // value key per local row
+    const NkWindow *qwindow;     // window per query [Q]
+};
+template <bool RANGE, bool WINDOW = false>
+using SimtArgs = std::conditional_t<WINDOW, SimtWindowParams<RANGE>, std::conditional_t<RANGE, SimtRangeParams, SimtParams>>;
 
 // ---- element loaders -------------------------------------------------------------------------
 template <typename T, bool VEC> struct Lane;
@@ -127,10 +134,11 @@ __device__ __forceinline__ void warp_reduce_scatter(float (&v)[V], int lane) {
 }
 
 // TAGS: filtered search — the owner lane also tests its (row, query) pair against the query's tag filter.
+// WINDOW (with TAGS): windowed search — ... and against the query's value window.
 // RANGE (nk_search_range): the owner lane appends every pair whose exact score reaches the query's fixed threshold straight to
 // the query's list — no buffer, no prune, no emission, and the scores need no re-scoring.
-template <typename T, bool VEC, int QT, int R, bool EUCLID, bool TAGS, bool RANGE>
-__global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtArgs<RANGE> p) {
+template <typename T, bool VEC, int QT, int R, bool EUCLID, bool TAGS, bool RANGE, bool WINDOW>
+__global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtArgs<RANGE, WINDOW> p) {
     pdl_trigger();  // the merge launch behind this scan may begin (it waits for this grid before reading)
     pdl_wait();     // exact-stage twin of a filter search: programmatic dependent of the finish kernel
     if (p.only_if && *p.only_if == 0) return;
@@ -250,6 +258,9 @@ __global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtArgs<RA
             const uint32_t row = row0 + r;
             if ((lane % LPV) == 0 && row < n && (uint32_t)qi < p.nq && (!p.mask || ((p.mask[row >> 5] >> (row & 31)) & 1u)) &&
                 (!TAGS || tag_admits(__ldg(p.row_tags + row), p.qfilter + p.q0 + qi))) {
+                if constexpr (WINDOW) {
+                    if (!window_admits(__ldg(p.row_values + row), p.qwindow + p.q0 + qi)) continue;
+                }
                 if constexpr (EUCLID) {
                     s = -s;
                 } else if (p.metric == NK_METRIC_COSINE) {
@@ -317,42 +328,54 @@ __global__ void __launch_bounds__(SIMT_THREADS) knn_scan_simt_kernel(SimtArgs<RA
 }
 
 // ---------------------------------------------------------------------------------------------
-template <bool RANGE> using SimtKernelT = void (*)(SimtArgs<RANGE>);
+template <bool RANGE, bool WINDOW> using SimtKernelT = void (*)(SimtArgs<RANGE, WINDOW>);
 
-template <typename T, bool VEC, bool EUCLID, bool TAGS, bool RANGE>
-static SimtKernelT<RANGE> pick_qt(int qt) {
+template <typename T, bool VEC, bool EUCLID, bool TAGS, bool RANGE, bool WINDOW>
+static SimtKernelT<RANGE, WINDOW> pick_qt(int qt) {
     if constexpr (VEC) {
         switch (qt) {
-            case 8: return knn_scan_simt_kernel<T, VEC, 8, 4, EUCLID, TAGS, RANGE>;
-            case 4: return knn_scan_simt_kernel<T, VEC, 4, 8, EUCLID, TAGS, RANGE>;
-            case 2: return knn_scan_simt_kernel<T, VEC, 2, 8, EUCLID, TAGS, RANGE>;
-            default: return knn_scan_simt_kernel<T, VEC, 1, 8, EUCLID, TAGS, RANGE>;
+            case 8: return knn_scan_simt_kernel<T, VEC, 8, 4, EUCLID, TAGS, RANGE, WINDOW>;
+            case 4: return knn_scan_simt_kernel<T, VEC, 4, 8, EUCLID, TAGS, RANGE, WINDOW>;
+            case 2: return knn_scan_simt_kernel<T, VEC, 2, 8, EUCLID, TAGS, RANGE, WINDOW>;
+            default: return knn_scan_simt_kernel<T, VEC, 1, 8, EUCLID, TAGS, RANGE, WINDOW>;
         }
     } else {
         switch (qt) {
-            case 4: return knn_scan_simt_kernel<T, VEC, 4, 8, EUCLID, TAGS, RANGE>;
-            default: return knn_scan_simt_kernel<T, VEC, 1, 8, EUCLID, TAGS, RANGE>;
+            case 4: return knn_scan_simt_kernel<T, VEC, 4, 8, EUCLID, TAGS, RANGE, WINDOW>;
+            default: return knn_scan_simt_kernel<T, VEC, 1, 8, EUCLID, TAGS, RANGE, WINDOW>;
         }
     }
 }
 
-template <bool TAGS, bool RANGE>
-static SimtKernelT<RANGE> pick_kernel_t(int dtype, bool vec, bool euclid, int qt) {
+template <bool TAGS, bool RANGE, bool WINDOW>
+static SimtKernelT<RANGE, WINDOW> pick_kernel_t(int dtype, bool vec, bool euclid, int qt) {
     if (dtype == NK_DTYPE_F16) {
-        if (vec) return euclid ? pick_qt<__half, true, true, TAGS, RANGE>(qt) : pick_qt<__half, true, false, TAGS, RANGE>(qt);
-        return euclid ? pick_qt<__half, false, true, TAGS, RANGE>(qt) : pick_qt<__half, false, false, TAGS, RANGE>(qt);
+        if (vec) return euclid ? pick_qt<__half, true, true, TAGS, RANGE, WINDOW>(qt) : pick_qt<__half, true, false, TAGS, RANGE, WINDOW>(qt);
+        return euclid ? pick_qt<__half, false, true, TAGS, RANGE, WINDOW>(qt) : pick_qt<__half, false, false, TAGS, RANGE, WINDOW>(qt);
     }
     if (dtype == NK_DTYPE_BF16) {
-        if (vec) return euclid ? pick_qt<__nv_bfloat16, true, true, TAGS, RANGE>(qt) : pick_qt<__nv_bfloat16, true, false, TAGS, RANGE>(qt);
-        return euclid ? pick_qt<__nv_bfloat16, false, true, TAGS, RANGE>(qt) : pick_qt<__nv_bfloat16, false, false, TAGS, RANGE>(qt);
+        if (vec) return euclid ? pick_qt<__nv_bfloat16, true, true, TAGS, RANGE, WINDOW>(qt) : pick_qt<__nv_bfloat16, true, false, TAGS, RANGE, WINDOW>(qt);
+        return euclid ? pick_qt<__nv_bfloat16, false, true, TAGS, RANGE, WINDOW>(qt) : pick_qt<__nv_bfloat16, false, false, TAGS, RANGE, WINDOW>(qt);
     }
-    if (vec) return euclid ? pick_qt<float, true, true, TAGS, RANGE>(qt) : pick_qt<float, true, false, TAGS, RANGE>(qt);
-    return euclid ? pick_qt<float, false, true, TAGS, RANGE>(qt) : pick_qt<float, false, false, TAGS, RANGE>(qt);
+    if (vec) return euclid ? pick_qt<float, true, true, TAGS, RANGE, WINDOW>(qt) : pick_qt<float, true, false, TAGS, RANGE, WINDOW>(qt);
+    return euclid ? pick_qt<float, false, true, TAGS, RANGE, WINDOW>(qt) : pick_qt<float, false, false, TAGS, RANGE, WINDOW>(qt);
 }
-// The kernel of a scan in the mode a.mode: a kNN mode (RANGE = false) or a range mode (RANGE = true), as ScanArgs::check found.
-template <bool RANGE> static SimtKernelT<RANGE> pick_kernel(const ScanArgs &a, bool vec, int qt) {
+
+// Calls run(kern, params) with the kernel of a scan in the mode a.mode — a kNN mode (RANGE = false) or a range mode (RANGE =
+// true), as ScanArgs::check found — and params(p), which turns the parameter block p into the kernel's: p itself, or for
+// the window modes p with the windows appended.
+template <bool RANGE, class Run> static int with_simt_kernel(const ScanArgs &a, bool vec, int qt, Run run) {
     const bool euclid = a.metric == NK_METRIC_EUCLIDEAN;
-    return mode_tags(a.mode) ? pick_kernel_t<true, RANGE>(a.dtype, vec, euclid, qt) : pick_kernel_t<false, RANGE>(a.dtype, vec, euclid, qt);
+    if (mode_window(a.mode))
+        return run(pick_kernel_t<true, RANGE, true>(a.dtype, vec, euclid, qt), [&](const SimtArgs<RANGE> &p) {
+            SimtWindowParams<RANGE> w{};
+            static_cast<SimtArgs<RANGE> &>(w) = p;
+            w.row_values = a.row_values; w.qwindow = a.qwindow;
+            return w;
+        });
+    const auto same = [](const SimtArgs<RANGE> &p) { return p; };
+    return mode_tags(a.mode) ? run(pick_kernel_t<true, RANGE, false>(a.dtype, vec, euclid, qt), same)
+                             : run(pick_kernel_t<false, RANGE, false>(a.dtype, vec, euclid, qt), same);
 }
 
 // cudaFuncSetAttribute + occupancy query once per (kernel, device, smem) instead of once per search
@@ -415,26 +438,30 @@ int scan_simt(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *
             set_error("dim=%u too large for the SIMT scan (needs %zu B shared memory)", a.dim, smem);
             return -1;
         }
-        const auto kern = pick_kernel<false>(a, vec, qt);
-        if (simt_ensure(reinterpret_cast<const void *>(kern), di.device_id, smem)) return -1;
-        int occ = simt_occupancy(reinterpret_cast<const void *>(kern), di.device_id, smem);
-        // One grid for every query group of this search so the per-CTA partial lists line up.
-        if (grid_used == 0) {
-            grid_used = (uint32_t)di.num_sms * (uint32_t)occ;
-            if (grid_used > num_iv) grid_used = num_iv;
-            if (grid_used > max_grid) grid_used = max_grid;
-            if (ws_reserve((void **)&ws.cand, &ws.cand_bytes, (size_t)grid_used * 8 * P * 8)) return -1;
-            if (ws_reserve((void **)&ws.partial, &ws.partial_bytes, (size_t)a.Q * grid_used * a.k * 8)) return -1;
-        }
-        SimtParams p;
-        p.rows = a.rows; p.n = a.n; p.dim = a.dim; p.row_base = a.row_base;
-        p.queries = a.queries; p.q0 = q0; p.nq = left < (uint32_t)qt ? left : (uint32_t)qt; p.k = a.k;
-        p.metric = a.metric; p.P = P; p.cand = ws.cand; p.partial = ws.partial; p.flags = ws.flags; p.only_if = a.only_if; p.below = a.below; p.mask = a.row_mask; p.min_score = a.min_score;
-        p.row_tags = a.row_tags; p.qfilter = a.qfilter;
-        NK_CUDA_OK(launch_pdl(kern, dim3(grid_used), dim3(SIMT_THREADS), smem, a.stream, a.only_if != nullptr && !a.defer_tail, p));
+        const uint32_t nq = left < (uint32_t)qt ? left : (uint32_t)qt;
+        if (with_simt_kernel<false>(a, vec, qt, [&](auto kern, auto params) -> int {
+                if (simt_ensure(reinterpret_cast<const void *>(kern), di.device_id, smem)) return -1;
+                int occ = simt_occupancy(reinterpret_cast<const void *>(kern), di.device_id, smem);
+                // One grid for every query group of this search so the per-CTA partial lists line up.
+                if (grid_used == 0) {
+                    grid_used = (uint32_t)di.num_sms * (uint32_t)occ;
+                    if (grid_used > num_iv) grid_used = num_iv;
+                    if (grid_used > max_grid) grid_used = max_grid;
+                    if (ws_reserve((void **)&ws.cand, &ws.cand_bytes, (size_t)grid_used * 8 * P * 8)) return -1;
+                    if (ws_reserve((void **)&ws.partial, &ws.partial_bytes, (size_t)a.Q * grid_used * a.k * 8)) return -1;
+                }
+                SimtParams p;
+                p.rows = a.rows; p.n = a.n; p.dim = a.dim; p.row_base = a.row_base;
+                p.queries = a.queries; p.q0 = q0; p.nq = nq; p.k = a.k;
+                p.metric = a.metric; p.P = P; p.cand = ws.cand; p.partial = ws.partial; p.flags = ws.flags; p.only_if = a.only_if; p.below = a.below; p.mask = a.row_mask; p.min_score = a.min_score;
+                p.row_tags = a.row_tags; p.qfilter = a.qfilter;
+                NK_CUDA_OK(launch_pdl(kern, dim3(grid_used), dim3(SIMT_THREADS), smem, a.stream, a.only_if != nullptr && !a.defer_tail, params(p)));
+                return 0;
+            }))
+            return -1;
         if (launches) ++*launches;
         if (a.main_launches) ++*a.main_launches;
-        q0 += p.nq;
+        q0 += nq;
     }
     if (a.ev_end) NK_CUDA_OK(cudaEventRecord(a.ev_end, a.stream));
     // Fold the per-CTA lists: list l of query q starts at partial[(q*grid + l)*k].
@@ -465,21 +492,25 @@ int scan_simt_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint
             set_error("dim=%u too large for the SIMT scan (needs %zu B shared memory)", a.dim, smem);
             return -1;
         }
-        const auto kern = pick_kernel<true>(a, vec, qt);
-        if (simt_ensure(reinterpret_cast<const void *>(kern), di.device_id, smem)) return -1;
-        const int occ = simt_occupancy(reinterpret_cast<const void *>(kern), di.device_id, smem);
-        uint32_t grid = (uint32_t)di.num_sms * (uint32_t)occ;
-        if (grid > num_iv) grid = num_iv;
-        SimtRangeParams p{};
-        p.rows = a.rows; p.n = a.n; p.dim = a.dim; p.row_base = a.row_base;
-        p.queries = a.queries; p.q0 = q0; p.nq = left < (uint32_t)qt ? left : (uint32_t)qt; p.k = 1;
-        p.metric = a.metric; p.P = 0; p.partial = ws.partial; p.flags = ws.flags; p.mask = a.row_mask; p.min_score = a.min_score;
-        p.row_tags = a.row_tags; p.qfilter = a.qfilter;
-        p.range_tau = reinterpret_cast<const uint32_t *>(ws.keys2); p.range_fill = reinterpret_cast<int *>(ws.keys2) + QA; p.list_cap = list_cap;
-        NK_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(SIMT_THREADS), smem, a.stream, false, p));
+        const uint32_t nq = left < (uint32_t)qt ? left : (uint32_t)qt;
+        if (with_simt_kernel<true>(a, vec, qt, [&](auto kern, auto params) -> int {
+                if (simt_ensure(reinterpret_cast<const void *>(kern), di.device_id, smem)) return -1;
+                const int occ = simt_occupancy(reinterpret_cast<const void *>(kern), di.device_id, smem);
+                uint32_t grid = (uint32_t)di.num_sms * (uint32_t)occ;
+                if (grid > num_iv) grid = num_iv;
+                SimtRangeParams p{};
+                p.rows = a.rows; p.n = a.n; p.dim = a.dim; p.row_base = a.row_base;
+                p.queries = a.queries; p.q0 = q0; p.nq = nq; p.k = 1;
+                p.metric = a.metric; p.P = 0; p.partial = ws.partial; p.flags = ws.flags; p.mask = a.row_mask; p.min_score = a.min_score;
+                p.row_tags = a.row_tags; p.qfilter = a.qfilter;
+                p.range_tau = reinterpret_cast<const uint32_t *>(ws.keys2); p.range_fill = reinterpret_cast<int *>(ws.keys2) + QA; p.list_cap = list_cap;
+                NK_CUDA_OK(launch_pdl(kern, dim3(grid), dim3(SIMT_THREADS), smem, a.stream, false, params(p)));
+                return 0;
+            }))
+            return -1;
         if (launches) ++*launches;
         if (a.main_launches) ++*a.main_launches;
-        q0 += p.nq;
+        q0 += nq;
     }
     if (a.ev_end) NK_CUDA_OK(cudaEventRecord(a.ev_end, a.stream));
     return 0;

@@ -92,8 +92,8 @@ __device__ long long g_tc_prof[32];
 constexpr int PREP_THREADS = 1024;  // 32 warps: the sample scoring is latency-bound (one 4 KB row per warp at a time)
 
 // TAGS (filtered searches): the sample only counts rows the query admits, so a query with fewer than k admissible sample rows
-// starts at the score floor.
-template <bool TAGS>
+// starts at the score floor.  WINDOW (windowed searches, with TAGS): admitted means by the tag filter AND the value window.
+template <bool TAGS, bool WINDOW>
 __global__ void __launch_bounds__(PREP_THREADS) filter_prep_kernel(PrepParams p) {
     extern __shared__ __align__(16) unsigned char prep_smem[];
     float *qs = reinterpret_cast<float *>(prep_smem);                                  // raw query [dim]
@@ -216,7 +216,8 @@ __global__ void __launch_bounds__(PREP_THREADS) filter_prep_kernel(PrepParams p)
         return (lo == lo && lo > -INFINITY && lo < INFINITY) ? (uint64_t)ord_bits(lo) : 0ull;
     };
     auto admissible = [&](uint64_t r) -> bool {
-        return r < p.n && (!p.mask || ((__ldg(p.mask + (r >> 5)) >> (r & 31)) & 1u)) && (!TAGS || tag_admits(__ldg(p.row_tags + r), p.qfilter + row));
+        return r < p.n && (!p.mask || ((__ldg(p.mask + (r >> 5)) >> (r & 31)) & 1u)) && (!TAGS || tag_admits(__ldg(p.row_tags + r), p.qfilter + row)) &&
+               (!WINDOW || window_admits(__ldg(p.row_values + r), p.qwindow + row));
     };
     if (p.dtype == NK_DTYPE_F32 && p.metric != NK_METRIC_EUCLIDEAN) {
         // two rows per warp at a time: both rows' 128-bit loads are in flight together (the scoring is latency-bound:
@@ -886,6 +887,7 @@ tc::Params pass_params(const ScanArgs &a, Workspace &ws, const tc::PassArgs &t) 
     p.gtau = reinterpret_cast<uint32_t *>(ws.keys2); p.gcount = reinterpret_cast<int *>(ws.keys2) + (t.Qpad + tc::QT_BIG);
     p.presampled = t.presampled; p.min_score = a.min_score;
     p.row_tags = a.row_tags; p.qfilter = a.qfilter; p.row_thr = a.row_thr; p.row_filter = a.row_filter; p.qtags = a.qtags;
+    p.row_values = a.row_values; p.qwindow = a.qwindow;
     p.dump_est = t.dump_est; p.dump_bnd = t.dump_bnd; p.dump_ld = t.dump_ld;
     return p;
 }
@@ -916,13 +918,14 @@ PrepParams prep_params(const ScanArgs &a, uint32_t Qpad, uint32_t dimpad) {
     pp.q = a.queries; pp.Q = a.Q; pp.dim = a.dim; pp.dimpad = dimpad; pp.Qpad = Qpad;
     pp.normalise = a.metric == NK_METRIC_COSINE; pp.metric = a.metric;
     pp.rows = a.rows; pp.dtype = a.dtype; pp.n = a.n; pp.k = a.k; pp.mask = a.row_mask; pp.min_score = a.min_score;
-    pp.row_tags = a.row_tags; pp.qfilter = a.qfilter;
+    pp.row_tags = a.row_tags; pp.qfilter = a.qfilter; pp.row_values = a.row_values; pp.qwindow = a.qwindow;
     return pp;
 }
 
 int launch_prep(const DeviceInfo &di, ScanMode mode, const PrepParams &pp, cudaStream_t stream, uint64_t *launches) {
     const size_t smem = (size_t)((pp.dim + 3) & ~3u) * 4 + (size_t)pp.sample * 8;
-    void (*kern)(PrepParams) = mode_tags(mode) ? filter_prep_kernel<true> : filter_prep_kernel<false>;
+    void (*kern)(PrepParams) = mode_window(mode) ? filter_prep_kernel<true, true>
+                               : mode_tags(mode) ? filter_prep_kernel<true, false> : filter_prep_kernel<false, false>;
     if (smem > 48 * 1024 && tc_ensure_smem(reinterpret_cast<const void *>(kern), di.device_id, smem)) return -1;
     kern<<<pp.Qpad, PREP_THREADS, smem, stream>>>(pp);
     NK_CUDA_OK(cudaGetLastError());
@@ -962,12 +965,13 @@ static int launch_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws,
     if (t.count_main && a.main_launches) ++*a.main_launches;
     return 0;
 }
-// One pass in the mode a.mode.  The exact 3xTF32 kernel serves the kNN modes only; the dump mode exists at QT = 64 only.
+// One pass in the mode a.mode.  The exact 3xTF32 kernel serves the kNN modes only (the retry and exact stages of a filter
+// search re-run its arguments); the dump mode exists at QT = 64 only.
 template <int NT, int QT>
 static int launch_pass(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, const TcPassArgs &t, uint64_t *launches) {
     return tc::with_scan_mode(a.mode, [&](auto mode) {
         constexpr ScanMode M = decltype(mode)::value;
-        if constexpr ((NT == 1 || M == ScanMode::KNN || M == ScanMode::KNN_TAGS) && (QT == 64 || !mode_dump(M)))
+        if constexpr ((NT == 1 || M == ScanMode::KNN || M == ScanMode::KNN_TAGS || M == ScanMode::KNN_WINDOW) && (QT == 64 || !mode_dump(M)))
             return launch_pass_t<NT, QT, M>(di, a, ws, t, launches);
         set_error("internal: no %s kernel for scan mode %d at %d query columns", NT == 3 ? "3xTF32" : "TF32 filter", (int)M, QT);
         return -1;

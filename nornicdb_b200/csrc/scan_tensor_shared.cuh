@@ -75,6 +75,8 @@ struct Params {
     const float *row_thr;     // reverse modes only: key-space threshold per local row (the reverse scan of nk_knn_graph_update)
     const NkFilter *row_filter;  // REVERSE_RFILT only: the filter of each local row's own k-NN list (filtered graphs)
     const uint64_t *qtags;    // REVERSE_RFILT only: tag word per query [Q], indexed like gtau; staged in shared memory per CTA
+    const uint64_t *row_values;  // window modes only: value key per local row
+    const NkWindow *qwindow;     // window modes only: window per query [Q] (absolute query index; no padding, never read past Q)
 };
 
 // What one scan launch covers: queries [q0, q0+nq) in `qgroups` query groups over a `grid`-CTA launch.  Both kernels'
@@ -200,7 +202,10 @@ template <int QT> __device__ __forceinline__ float frag_value(const float (&acc)
 // BOUNDED: a NaN estimate is undecidable here, so it is kept as +inf and the exact re-scoring judges; exact mode: -inf.
 // M (ScanMode): tag modes: a pair whose query does not admit the row's tag never enters a buffer — else the pruned and
 // published thresholds would stop being lower bounds of the FILTERED k-th best score; flood tiles place it as key 0, the
-// compare pass loads the row's tag only when some column passed.  Reverse modes: a pair must also reach the ROW's threshold rthr[ri] and
+// compare pass loads the row's tag only when some column passed.  Window modes: the same for the row's value key and the
+// query's window, loaded and tested after the tag, and only for the columns the tag test kept (so only queries < nq: the
+// window array has Q entries, no padding).  The window's query index is summed in 32 bits before the one pointer add: the
+// 16-bit / int8 QT=128 instantiations then keep their register budget without spills.  Reverse modes: a pair must also reach the ROW's threshold rthr[ri] and
 // (REVERSE_RFILT) be admitted by the row's own filter (qtag: the CTA's query tags), loaded only once both thresholds hold.
 template <int QT, int CAP, bool BOUNDED, ScanMode M, int NR, class Est>
 __device__ __forceinline__ void keep_fragment_rows(const Params &p, const Est (&est)[NR], const float (&acc)[2][QT / 2], uint32_t fr0,
@@ -245,6 +250,18 @@ __device__ __forceinline__ void keep_fragment_rows(const Params &p, const Est (&
                         const uint32_t qi = cbase + 8 * (c >> 1) + (c & 1);
                         if (qi < nq && tag_admits(tag, p.qfilter + q0 + qi) && (!mode_row_filter(M) || tag_admits(qtag[qi], p.row_filter + row)))
                             admit |= 1u << c;
+                    }
+                }
+            }
+            if constexpr (mode_window(M)) {
+                if (admit) {  // only the columns the tag loop admitted: those are queries < nq, whose windows exist
+                    const uint64_t val = __ldg(p.row_values + row);
+                    uint32_t chk = admit;
+#pragma unroll 1
+                    while (chk) {
+                        const uint32_t c = (uint32_t)__ffs((int)chk) - 1u;
+                        chk &= chk - 1u;
+                        if (!window_admits(val, p.qwindow + (q0 + cbase + 8 * (c >> 1) + (c & 1)))) admit &= ~(1u << c);
                     }
                 }
             }
@@ -299,6 +316,18 @@ __device__ __forceinline__ void keep_fragment_rows(const Params &p, const Est (&
                 const uint32_t c = (uint32_t)__ffs((int)chk) - 1u;
                 chk &= chk - 1u;
                 if (!tag_admits(tag, p.qfilter + q0 + cbase + 8 * (c >> 1) + (c & 1))) ps &= ~(1u << c);
+            }
+        }
+        if constexpr (mode_window(M)) {
+            if (ps) {
+                const uint64_t val = __ldg(p.row_values + row);
+                uint32_t chk = ps;
+#pragma unroll 1
+                while (chk) {
+                    const uint32_t c = (uint32_t)__ffs((int)chk) - 1u;
+                    chk &= chk - 1u;
+                    if (!window_admits(val, p.qwindow + (q0 + cbase + 8 * (c >> 1) + (c & 1)))) ps &= ~(1u << c);
+                }
             }
         }
         if (mode_row_filter(M) && ps) {
@@ -566,10 +595,12 @@ struct PrepParams {
     const int *only_if;
     const uint64_t *row_tags;  // the tag modes' filters: the sample counts admissible rows only
     const NkFilter *qfilter;
+    const uint64_t *row_values;  // ... and the window modes' windows
+    const NkWindow *qwindow;
 };
 // The fields taken from the search arguments: the queries, the metric and the shard (for the sample).
 PrepParams prep_params(const ScanArgs &a, uint32_t Qpad, uint32_t dimpad);
-// The tag modes run the instantiation whose sample counts only the rows each query admits.
+// The tag and window modes run the instantiations whose sample counts only the rows each query admits.
 int launch_prep(const DeviceInfo &di, ScanMode mode, const PrepParams &pp, cudaStream_t stream, uint64_t *launches);
 
 }  // namespace nk

@@ -312,13 +312,47 @@ public:
             }
         return out;
     }
+    // Per-query value windows: value keys of rows [firstRow, firstRow + keys.size()) (row order of Add; 0 = no value, keys
+    // encoded by the caller so that key order is number order), then a batch whose queries each carry an NkWindow {lo, hi}
+    // (inclusive, unsigned) on top of an optional tag filter (filters empty = none, else one per query), in one corpus pass.
+    void SetRowValues(uint64_t firstRow, const std::vector<uint64_t> &keys) {
+        std::lock_guard<std::mutex> lk(mu_);
+        check(nk_index_set_row_values(ix_, firstRow, keys.data(), keys.size()));
+    }
+    std::vector<std::vector<SearchResult>> SearchBatchWindowed(const std::vector<float> &queries, const std::vector<NkFilter> &filters,
+                                                               const std::vector<NkWindow> &windows, uint32_t Q, int k) {
+        if (queries.size() != (size_t)Q * dims_) throw ErrInvalidDimensions();
+        if (!filters.empty() && filters.size() != Q) throw std::invalid_argument("gpu: one filter per query");
+        if (windows.size() != Q) throw std::invalid_argument("gpu: one window per query");
+        std::lock_guard<std::mutex> lk(mu_);
+        if (nodeIDs_.empty() || k <= 0) return std::vector<std::vector<SearchResult>>(Q);
+        std::vector<uint32_t> idx((size_t)Q * k);
+        std::vector<float> sc((size_t)Q * k);
+        int got = nk_search_windowed(ix_, queries.data(), filters.empty() ? nullptr : filters.data(), windows.data(), Q, (uint32_t)k,
+                                     idx.data(), sc.data());
+        if (got < 0) throw cuda::ErrKernelExecution(std::string("gpu: ") + nk_last_error());
+        std::vector<std::vector<SearchResult>> out(Q);
+        for (uint32_t q = 0; q < Q; ++q)
+            for (int i = 0; i < got; ++i) {
+                uint32_t r = idx[(size_t)q * k + i];
+                float s = sc[(size_t)q * k + i];
+                if (r < nodeIDs_.size()) out[q].push_back({nodeIDs_[r], s, 1.0f - s});  // 0xffffffff: fewer admissible rows than k
+            }
+        return out;
+    }
     // Every node whose similarity reaches the query's threshold (cosine / dot: minimum score; euclidean: maximum distance),
     // best first; filters empty = none, else one per query.  Sizes its buffers from the library's exact total.
     std::vector<std::vector<SearchResult>> SearchRange(const std::vector<float> &queries, const std::vector<float> &thresholds,
                                                        const std::vector<NkFilter> &filters, uint32_t Q) {
+        return SearchRange(queries, thresholds, filters, {}, Q);
+    }
+    // ... with one value window per query on top (windows empty = none: the call above).
+    std::vector<std::vector<SearchResult>> SearchRange(const std::vector<float> &queries, const std::vector<float> &thresholds,
+                                                       const std::vector<NkFilter> &filters, const std::vector<NkWindow> &windows, uint32_t Q) {
         if (queries.size() != (size_t)Q * dims_) throw ErrInvalidDimensions();
         if (thresholds.size() != Q) throw std::invalid_argument("gpu: one threshold per query");
         if (!filters.empty() && filters.size() != Q) throw std::invalid_argument("gpu: one filter per query");
+        if (!windows.empty() && windows.size() != Q) throw std::invalid_argument("gpu: one window per query");
         std::lock_guard<std::mutex> lk(mu_);
         std::vector<std::vector<SearchResult>> out(Q);
         if (nodeIDs_.empty() || Q == 0) return out;
@@ -327,8 +361,8 @@ public:
         std::vector<float> sc;
         uint64_t total = 0;
         for (int pass = 0; pass < 2; ++pass) {
-            if (nk_search_range(ix_, queries.data(), thresholds.data(), filters.empty() ? nullptr : filters.data(), Q, idx.size(), off.data(),
-                                idx.data(), sc.data(), &total) < 0)
+            if (nk_search_range_windowed(ix_, queries.data(), thresholds.data(), filters.empty() ? nullptr : filters.data(),
+                                         windows.empty() ? nullptr : windows.data(), Q, idx.size(), off.data(), idx.data(), sc.data(), &total) < 0)
                 throw cuda::ErrKernelExecution(std::string("gpu: ") + nk_last_error());
             if (total <= idx.size()) break;
             idx.resize(total);

@@ -6,6 +6,8 @@ time by one fused distance + top-k kernel per shard."""
 from __future__ import annotations
 
 import ctypes as C
+import datetime as _dt
+import math
 from typing import List, NamedTuple, Optional, Sequence, Tuple
 
 import numpy as np
@@ -397,24 +399,32 @@ class KnnIndex:
                                                 Q, k, idx.ctypes.data_as(C.c_void_p), sc.ctypes.data_as(C.c_void_p)), "nk_search_filtered")
         return idx[:, :ke], sc[:, :ke]
 
-    def search_range(self, queries, thresholds, filters=None) -> List[Tuple[np.ndarray, np.ndarray]]:
+    def search_range(self, queries, thresholds, filters=None, windows=None) -> List[Tuple[np.ndarray, np.ndarray]]:
         """Every admissible row whose score reaches the query's threshold (cosine / dot: minimum score; euclidean: maximum
         distance), one threshold per query (a scalar applies to all).  Returns one (idx uint32, score float32) pair per query,
-        in search()'s order.  The result buffer grows to the size the library reports (nk_search_range's size protocol)."""
+        in search()'s order.  The result buffer grows to the size the library reports (nk_search_range's size protocol).
+        windows: None, or per-query value windows as for search_windowed (nk_search_range_windowed)."""
         q = self._queries(queries)
         Q = q.shape[0]
         t = np.ascontiguousarray(np.broadcast_to(np.asarray(thresholds, dtype=np.float32), (Q,)))
         f = None if filters is None else as_filters(filters, Q)
+        w = None if windows is None else as_windows(windows, Q)
         off = np.zeros(Q + 1, dtype=np.uint64)
         total = C.c_uint64(0)
         cap = getattr(self, "_range_cap", 0)
         while True:
             idx = np.empty(max(cap, 1), dtype=np.uint32)
             sc = np.empty(max(cap, 1), dtype=np.float32)
-            _check(self.lib.nk_search_range(self.ptr, q.ctypes.data_as(C.c_void_p), t.ctypes.data_as(C.c_void_p),
-                                            None if f is None else f.ctypes.data_as(C.c_void_p), Q, cap,
-                                            off.ctypes.data_as(C.c_void_p), idx.ctypes.data_as(C.c_void_p),
-                                            sc.ctypes.data_as(C.c_void_p), C.byref(total)), "nk_search_range")
+            if w is None:
+                _check(self.lib.nk_search_range(self.ptr, q.ctypes.data_as(C.c_void_p), t.ctypes.data_as(C.c_void_p),
+                                                None if f is None else f.ctypes.data_as(C.c_void_p), Q, cap,
+                                                off.ctypes.data_as(C.c_void_p), idx.ctypes.data_as(C.c_void_p),
+                                                sc.ctypes.data_as(C.c_void_p), C.byref(total)), "nk_search_range")
+            else:
+                _check(self.lib.nk_search_range_windowed(self.ptr, q.ctypes.data_as(C.c_void_p), t.ctypes.data_as(C.c_void_p),
+                                                         None if f is None else f.ctypes.data_as(C.c_void_p), w.ctypes.data_as(C.c_void_p),
+                                                         Q, cap, off.ctypes.data_as(C.c_void_p), idx.ctypes.data_as(C.c_void_p),
+                                                         sc.ctypes.data_as(C.c_void_p), C.byref(total)), "nk_search_range_windowed")
             if total.value <= cap:
                 break
             cap = int(total.value)
@@ -456,6 +466,41 @@ class KnnIndex:
         """Device-resident filtered search: filters_ptr = device [Q x 3] uint64 (0 = no filter), valid until the stream ran."""
         return _check(self.lib.nk_search_filtered_device(self.ptr, q_ptr, filters_ptr or None, Q, k, out_idx_ptr, out_score_ptr, stream),
                       "nk_search_filtered_device")
+
+    # -- per-query value windows -------------------------------------------------------------------
+    def set_row_values(self, values, first_row: int = 0) -> None:
+        """Value keys of rows [first_row, first_row + len(values)); rows never given one have key 0 (no value).  `values`:
+        keys already encoded (uint64), or numbers (int64, float, datetime64), which are encoded with value_keys()."""
+        a = np.asarray(values).reshape(-1)
+        v = np.ascontiguousarray(a if a.dtype == np.uint64 else value_keys(a))
+        _check(self.lib.nk_index_set_row_values(self.ptr, int(first_row), v.ctypes.data_as(C.c_void_p), int(v.size)),
+               "nk_index_set_row_values")
+
+    def search_windowed(self, queries, k: int, windows, filters=None) -> Tuple[np.ndarray, np.ndarray]:
+        """search_filtered() with one value window per query on top: windows [Q x 2] uint64 (lo, hi), inclusive key bounds (one
+        pair applies to every query; window() turns Qdrant Range bounds into one), None = none.  Row r is admissible iff
+        lo <= value[r] <= hi and the query's tag filter (None = none) admits it.  Slots beyond a query's admissible rows hold
+        index 0xffffffff and score 0."""
+        q = self._queries(queries)
+        Q = q.shape[0]
+        f = None if filters is None else as_filters(filters, Q)
+        w = None if windows is None else as_windows(windows, Q)
+        k = int(k)
+        if k <= 0 or Q == 0:
+            return np.empty((Q, 0), np.uint32), np.empty((Q, 0), np.float32)
+        idx = np.empty((Q, k), dtype=np.uint32)
+        sc = np.empty((Q, k), dtype=np.float32)
+        ke = _check(self.lib.nk_search_windowed(self.ptr, q.ctypes.data_as(C.c_void_p), None if f is None else f.ctypes.data_as(C.c_void_p),
+                                                None if w is None else w.ctypes.data_as(C.c_void_p), Q, k,
+                                                idx.ctypes.data_as(C.c_void_p), sc.ctypes.data_as(C.c_void_p)), "nk_search_windowed")
+        return idx[:, :ke], sc[:, :ke]
+
+    def search_windowed_device(self, q_ptr: int, filters_ptr: int, windows_ptr: int, Q: int, k: int, out_idx_ptr: int,
+                               out_score_ptr: int, stream: int = 0) -> int:
+        """Device-resident windowed search: filters_ptr = device [Q x 3] uint64 (0 = no filter), windows_ptr = device [Q x 2]
+        uint64 (0 = no window), both valid until the stream ran."""
+        return _check(self.lib.nk_search_windowed_device(self.ptr, q_ptr, filters_ptr or None, windows_ptr or None, Q, k, out_idx_ptr,
+                                                         out_score_ptr, stream), "nk_search_windowed_device")
 
     def search_keys_device(self, q_ptr: int, Q: int, k: int, out_keys_ptr: int, stream: int = 0) -> int:
         return _check(self.lib.nk_search_keys_device(self.ptr, q_ptr, Q, k, out_keys_ptr, stream),
@@ -591,6 +636,112 @@ def admits(tags, all_of: int, none_of: int, any_of: int):
     t = np.asarray(tags, dtype=np.uint64)
     a, n, s = np.uint64(all_of), np.uint64(none_of), np.uint64(any_of)
     return ((t & a) == a) & ((t & n) == 0) & ((s == 0) | ((t & s) != 0))
+
+
+SIGN64 = 1 << 63
+ADMIT_ALL_WINDOW = (0, ALL_BITS)  # every row, with or without a value
+EMPTY_WINDOW = (ALL_BITS, 0)       # lo > hi: no row
+
+
+def value_keys(values) -> np.ndarray:
+    """Numbers -> the uint64 value keys of nk_index_set_row_values, in the same order as the numbers:
+      - integers (int64 range): v ^ 2^63;
+      - float64, and float32 widened exactly: -0.0 becomes +0.0, then ~bits if the sign bit is set, else bits | 2^63;
+      - datetime64: its int64 nanoseconds since the epoch, as an integer.
+    Raises on NaN and on INT64_MIN (NaT for datetimes), so key 0 always means "no value": a window with lo >= 1 never admits a
+    row that was not given one (Qdrant's rule for a missing key)."""
+    a = np.asarray(values)
+    if a.dtype.kind == "M":
+        a = a.astype("datetime64[ns]").astype(np.int64)
+    if a.dtype.kind == "b":
+        a = a.astype(np.int64)
+    if a.dtype.kind in "iu":
+        if a.dtype.kind == "u" and a.size and int(a.max()) > (1 << 63) - 1:
+            raise KnnError("value_keys: unsigned value above INT64_MAX")
+        v = a.astype(np.int64)
+        if (v == np.iinfo(np.int64).min).any():
+            raise KnnError("value_keys: INT64_MIN (or NaT) has no key: key 0 means 'no value'")
+        return v.view(np.uint64) ^ np.uint64(SIGN64)
+    if a.dtype.kind == "f":
+        f = a.astype(np.float64)
+        if np.isnan(f).any():
+            raise KnnError("value_keys: NaN has no key")
+        f = np.where(f == 0.0, 0.0, f)  # -0.0 -> +0.0
+        b = np.ascontiguousarray(f).view(np.uint64).reshape(f.shape)
+        neg = (b >> np.uint64(63)) != 0
+        return np.where(neg, ~b, b | np.uint64(SIGN64)).astype(np.uint64)
+    raise KnnError(f"value_keys: unsupported dtype {a.dtype}")
+
+
+_I64_MIN, _I64_MAX = -(1 << 63), (1 << 63) - 1
+
+
+def _closed_key(x, kind: Optional[str], op: str) -> int:
+    """One Qdrant Range bound (op: gt / gte / lt / lte) as the key of the closed bound it implies: the smallest admitted key
+    for gt / gte, the largest for lt / lte.  The result may fall outside [1, ALL_BITS] (ALL_BITS + 1 or 0): nothing admitted.
+    kind None infers int / float / datetime from the bound itself."""
+    if kind is None:
+        kind = ("datetime" if isinstance(x, (np.datetime64, _dt.datetime, _dt.date))
+                else "float" if isinstance(x, (float, np.floating)) else "int")
+    lower = op in ("gt", "gte")
+    if kind == "float":
+        k = int(value_keys(np.float64(x))[()])  # NaN refused there
+        return k + 1 if op == "gt" else k - 1 if op == "lt" else k
+    if kind == "datetime":
+        t = np.datetime64(x, "ns").astype(np.int64)
+        if t == _I64_MIN:
+            raise KnnError("window: NaT bound")
+        x = int(t)
+    elif kind != "int":
+        raise KnnError(f"window: unknown kind {kind!r} (int, float or datetime)")
+    # integer column: the closed integer bound t, rounded inward when the bound is fractional (Qdrant bounds are doubles)
+    if isinstance(x, (float, np.floating)):
+        f = float(x)
+        if math.isnan(f):
+            raise KnnError("window: NaN bound")
+        if math.isinf(f):
+            return (ALL_BITS + 1 if f > 0 else 1) if lower else (ALL_BITS if f > 0 else 0)
+        t = math.floor(f) + 1 if op == "gt" else math.ceil(f) if op == "gte" else math.ceil(f) - 1 if op == "lt" else math.floor(f)
+    else:
+        t = int(x) + (1 if op == "gt" else -1 if op == "lt" else 0)
+    if lower:
+        return ALL_BITS + 1 if t > _I64_MAX else max(t, _I64_MIN + 1) + (1 << 63)
+    return 0 if t < _I64_MIN + 1 else min(t, _I64_MAX) + (1 << 63)
+
+
+def window(gt=None, gte=None, lt=None, lte=None, kind: Optional[str] = None) -> Tuple[int, int]:
+    """Qdrant Range bounds (gt / gte / lt / lte, any subset; None = open) as the closed key window (lo, hi) of
+    search_windowed, over values encoded with value_keys().  kind: "int", "float" or "datetime" — the encoding of the
+    indexed values; None infers it from each bound (pass it when, e.g., integer bounds filter a float column).  A strict bound
+    steps one key inward; on an int (or datetime) column a fractional bound is rounded inward (gte=2.5 admits 3, lt=2.5
+    admits 2).  A bound past either end of the key space gives EMPTY_WINDOW.  Rows without a value (key 0) never match, as
+    a missing key never matches a Qdrant range: lo is at least 1."""
+    lo, hi = 1, ALL_BITS
+    for op, x in (("gt", gt), ("gte", gte), ("lt", lt), ("lte", lte)):
+        if x is None:
+            continue
+        k = _closed_key(x, kind, op)
+        if op in ("gt", "gte"):
+            lo = max(lo, k)
+        else:
+            hi = min(hi, k)
+    return (lo, hi) if lo <= hi else EMPTY_WINDOW
+
+
+def as_windows(windows, Q: int) -> np.ndarray:
+    """[Q x 2] uint64 (lo, hi) rows, C-contiguous: the NkWindow array layout.  A single (lo, hi) pair applies to every query."""
+    w = np.ascontiguousarray(np.asarray(windows, dtype=np.uint64)).reshape(-1, 2)
+    if w.shape[0] == 1 and Q != 1:
+        w = np.ascontiguousarray(np.broadcast_to(w, (Q, 2)))
+    if w.shape[0] != Q:
+        raise KnnError(f"windows: {w.shape[0]} rows for {Q} queries")
+    return w
+
+
+def window_admits(keys, lo: int, hi: int):
+    """The window predicate of nk_search_windowed on host value keys (numpy; tests, callers' bookkeeping)."""
+    k = np.asarray(keys, dtype=np.uint64)
+    return (k >= np.uint64(lo)) & (k <= np.uint64(hi))
 
 
 def synthetic_tags(n_rows: int, seed: int, row_base: int = 0) -> np.ndarray:

@@ -1,0 +1,30 @@
+"""The C++ host mirror's windowed calls (gpu::EmbeddingIndex::SetRowValues / SearchBatchWindowed / windowed SearchRange) compile
+against the C ABI, and answer a tiny dated batch on the GPU."""
+import os
+import subprocess
+
+import pytest
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+@pytest.fixture(scope="module")
+def windowed_binary(knn_lib, tmp_path_factory):
+    src = os.path.join(ROOT, "tests", "cpp", "windowed_mirror_test.cpp")
+    lib = os.path.join(ROOT, "nornicdb_b200", "libnornic_knn.so")
+    out = str(tmp_path_factory.mktemp("cpp") / "windowed_mirror_test")
+    subprocess.run(["/usr/bin/g++", "-std=c++17", "-O1", "-Wall", "-I", ROOT, src, "-L", os.path.dirname(lib), "-lnornic_knn",
+                    f"-Wl,-rpath,{os.path.dirname(lib)}", "-lpthread", "-o", out], check=True, cwd=ROOT)
+    return out
+
+
+def test_windowed_mirror_compiles(windowed_binary):
+    out = subprocess.run([windowed_binary, "--no-gpu"], capture_output=True, text=True)
+    assert out.returncode == 0 and "windowed mirror ok" in out.stdout
+
+
+@pytest.mark.gpu
+def test_windowed_mirror_on_gpu(windowed_binary):
+    out = subprocess.run([windowed_binary], capture_output=True, text=True, timeout=120)
+    assert out.returncode == 0, out.stdout + out.stderr
+    assert "windowed mirror ok" in out.stdout
