@@ -253,8 +253,9 @@ int nk_search_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uint32_t
  * tag, remove_swap moves the last row's tag with its row; upload, upload_from_f32, fill_* and attach_device_rows reset every
  * tag to 0.
  * Not filtered: nk_search_groups, nk_score_subset, nk_search_keys_device, nk_search_sharded_device and the k-means calls.
- * Not windowed (value windows, below): nk_search_rows*, nk_search_pairs, the graph update and remap calls, nk_search_groups,
- * nk_score_subset, nk_search_keys_device, nk_search_sharded_device, the exchange calls and the k-means calls. */
+ * Not windowed (value windows, below): the graph update and remap calls, nk_search_groups, nk_score_subset,
+ * nk_search_keys_device, nk_search_sharded_device, the exchange calls and the k-means calls (search by stored row and the
+ * self-join have windowed forms: nk_search_rows_windowed, nk_search_pairs_windowed). */
 typedef struct NkFilter {
     uint64_t all_of, none_of, any_of;
 } NkFilter;
@@ -320,6 +321,16 @@ int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t 
  * of 1024 queries. */
 int nk_search_rows_filtered(NkIndex *ix, const uint32_t *rows_host, const NkFilter *filters_host, uint32_t Q, uint32_t k,
                             uint32_t *out_idx, float *out_score);
+/* nk_search_rows_filtered with one value window per query (windows_host [Q], NULL = none: then nk_search_rows_filtered bit for
+ * bit), e.g. "nodes like this one from the last 7 days".  Query q gets the top k of the rows other than rows_host[q] that
+ * filters_host[q] (NULL = every tag) and windows_host[q] admit (nk_search_windowed's predicate), with the row mask and the score
+ * floor as in nk_search_rows.  The query row itself may lie outside its own window.  Return value, padding, blocks of 1024,
+ * devices, k limit, locking and refusals: those of nk_search_rows.
+ * Equals nk_search_windowed(the rows read back and widened, filters_host, windows_host, k' = min(k + 1, rows passing the row
+ * mask)) with the query's own row removed from each list (or, where it is not in the list, the last entry), bit for bit, for
+ * the same blocks of 1024 queries. */
+int nk_search_rows_windowed(NkIndex *ix, const uint32_t *rows_host, const NkFilter *filters_host, const NkWindow *windows_host,
+                            uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score);
 
 /* ---- Range search ------------------------------------------------------------------------------------------------------
  * Every admissible row whose score reaches the query's threshold (Cypher WHERE vector.similarity.* >= t, auto-links above a
@@ -366,6 +377,22 @@ int nk_search_range_windowed(NkIndex *ix, const float *queries_host, const float
  * filter for every query) with each list cut to the rows above its own query row, and emptied for inadmissible left rows. */
 int nk_search_pairs(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float threshold, const NkFilter *filter, uint64_t capacity,
                     uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total);
+/* nk_search_pairs with value conditions on both sides (near-duplicates within the same hour, auto-links only between rows close
+ * in time).  A pair {i, j} is returned iff nk_search_pairs returns it and
+ *   - `window` (one NkWindow, NULL = none) admits value[i] and value[j];
+ *   - max_gap != NK_NO_GAP (a BAND): value[i] != 0, value[j] != 0 and |value[i] - value[j]| <= max_gap.  max_gap is in key
+ *     units, which are value units for int64 and datetime64 (ns) columns encoded by nornicdb_b200.knn.value_keys.
+ * Both conditions are symmetric, so each unordered pair still appears once, under its lower id.  Left row i scans with the
+ * window [max(lo, value[i] - max_gap, 1), min(hi, value[i] + max_gap)] (saturating; without a band, [lo, hi]), computed on the
+ * device that holds it; a left row that fails the row mask, `filter`, `window` or the band's value rule gets the window that
+ * admits no row.  The scans run in the windowed range mode, so out-of-window pairs are never staged.
+ * Arguments, CSR layout, size protocol, refusals, locking and costs: those of nk_search_pairs.  window == NULL and max_gap ==
+ * NK_NO_GAP: nk_search_pairs, bit for bit (same kernels).
+ * Equals nk_search_pairs with the out-of-window and out-of-band pairs dropped, bit for bit (scores, order and CSR). */
+#define NK_NO_GAP 0xffffffffffffffffull
+int nk_search_pairs_windowed(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float threshold, const NkFilter *filter,
+                             const NkWindow *window, uint64_t max_gap, uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx,
+                             float *out_score, uint64_t *out_total);
 
 /* ---- k-NN graph update -------------------------------------------------------------------------------------------------
  * Keeps the k-NN graph of nk_search_rows exact across nk_index_append and nk_index_update_row without an O(N^2) rebuild.

@@ -1374,23 +1374,40 @@ constexpr uint32_t SEARCH_ROWS_BLOCK = 1024;
 // device that holds it.  *stage then writes the block into s.ws.queries (reserved by the caller) of any shard the search runs
 // on.  With one live shard only the ids cross PCIe and the rows are gathered straight into the query block; otherwise each
 // owner gathers its rows now, the block is assembled in pinned host memory and *stage sends it.  admit (nk_search_pairs):
-// *stage also writes the per-query filters into s.ws.qfilter, with the shard's tag array on: *admit for a row that passes the
-// row mask and *admit, the filter that admits no row otherwise, decided on the row's own device.
-static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, const uint32_t *ids, uint32_t nb, const NkFilter *admit,
+// *stage also writes the per-query filters into s.ws.qfilter, with the shard's tag array on: admit->f for a row that passes the
+// row mask and admit->f, the filter that admits no row otherwise, decided on the row's own device.  admit->windowed
+// (nk_search_pairs_windowed): each row's window (nk::row_windows) goes into s.ws.qwindow instead, with the shard's value array
+// on, and decides the row's admission alone (mask, filter, window and band: a refused row gets the window that admits no
+// row), so every query's filter is admit->f and row_filters does not run.
+struct RowAdmit {
+    NkFilter f{0, 0, 0};
+    bool windowed = false;
+    NkWindow w{0, ~0ull};
+    uint64_t gap = NK_NO_GAP;
+};
+static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, const uint32_t *ids, uint32_t nb, const RowAdmit *admit,
                            StageQueries *stage) {
     const size_t rb = (size_t)ix->dim * sizeof(float);
     std::vector<uint32_t> local(nb);
     if (live.size() == 1) {
         const bool filt = admit != nullptr;
-        const NkFilter f = filt ? *admit : NkFilter{0, 0, 0};
-        *stage = [ix, ids, nb, local, filt, f](NkShard &s) mutable {
+        const RowAdmit a = filt ? *admit : RowAdmit{};
+        const NkFilter f = a.f;
+        std::vector<NkFilter> every(a.windowed ? nb : 0, f);  // a windowed block's filters: f for every query
+        *stage = [ix, ids, nb, local, filt, f, a, every](NkShard &s) mutable {
             for (uint32_t q = 0; q < nb; ++q) local[q] = ids[q] - (uint32_t)ix->first_row(s);
             if (nk::ws_reserve((void **)&s.ws.sub_rows, &s.ws.sub_rows_bytes, (size_t)nb * 4)) return -1;
             NK_CUDA_OK(cudaMemcpyAsync(s.ws.sub_rows, local.data(), (size_t)nb * 4, cudaMemcpyHostToDevice, s.stream));
             if (nk::gather_rows(s.rows, ix->dtype, ix->dim, s.ws.sub_rows, nb, s.ws.queries, true, s.stream)) return -1;
             ix->stats.bytes_h2d += (uint64_t)nb * 4;
             ix->stats.kernel_launches++;
-            if (filt) {
+            if (a.windowed) {
+                if (!stage_filters(ix, s, every.data(), nb) || shard_values_on(s)) return -1;
+                if (nk::ws_reserve((void **)&s.ws.qwindow, &s.ws.qwindow_bytes, (size_t)nb * sizeof(NkWindow))) return -1;
+                if (nk::row_windows(s.ws.sub_rows, nb, s.mask_on ? s.mask : nullptr, s.tags, s.values, f, a.w, a.gap, s.ws.qwindow, s.stream))
+                    return -1;
+                ix->stats.kernel_launches++;
+            } else if (filt) {
                 if (shard_tags_on(s)) return -1;
                 if (nk::ws_reserve((void **)&s.ws.qfilter, &s.ws.qfilter_bytes, (size_t)nb * sizeof(NkFilter))) return -1;
                 if (nk::row_filters(s.ws.sub_rows, nb, s.mask_on ? s.mask : nullptr, s.tags, f, s.ws.qfilter, s.stream)) return -1;
@@ -1404,7 +1421,9 @@ static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, cons
     if (pinned_reserve((void **)&ix->h_qrows, &ix->h_qrows_bytes, 2 * nb * rb)) return -1;
     float *blk = ix->h_qrows, *part = ix->h_qrows + (size_t)nb * ix->dim;
     std::vector<uint32_t> pos(nb);
-    std::vector<NkFilter> filters(admit ? nb : 0), part_f(admit ? nb : 0);
+    const bool win = admit && admit->windowed;
+    std::vector<NkFilter> filters(admit ? nb : 0, win ? admit->f : NkFilter{0, 0, 0}), part_f(admit && !win ? nb : 0);
+    std::vector<NkWindow> windows(win ? nb : 0), part_w(win ? nb : 0);
     for (NkShard *o : live) {
         uint32_t m = 0;
         for (uint32_t q = 0; q < nb; ++q) {
@@ -1418,14 +1437,23 @@ static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, cons
         NK_CUDA_OK(cudaMemcpyAsync(o->ws.sub_rows, local.data(), (size_t)m * 4, cudaMemcpyHostToDevice, o->stream));
         if (nk::gather_rows(o->rows, ix->dtype, ix->dim, o->ws.sub_rows, m, o->ws.sub_gather, true, o->stream)) return -1;
         NK_CUDA_OK(cudaMemcpyAsync(part, o->ws.sub_gather, (size_t)m * rb, cudaMemcpyDeviceToHost, o->stream));
-        if (admit) {  // the owner's qfilter slot is free until the scan stages its own filters
+        if (admit && !win) {  // the owner's qfilter slot is free until the scan stages its own filters
             if (nk::ws_reserve((void **)&o->ws.qfilter, &o->ws.qfilter_bytes, (size_t)m * sizeof(NkFilter))) return -1;
-            if (nk::row_filters(o->ws.sub_rows, m, o->mask_on ? o->mask : nullptr, o->tags_on ? o->tags : nullptr, *admit, o->ws.qfilter,
+            if (nk::row_filters(o->ws.sub_rows, m, o->mask_on ? o->mask : nullptr, o->tags_on ? o->tags : nullptr, admit->f, o->ws.qfilter,
                                 o->stream))
                 return -1;
             NK_CUDA_OK(cudaMemcpyAsync(part_f.data(), o->ws.qfilter, (size_t)m * sizeof(NkFilter), cudaMemcpyDeviceToHost, o->stream));
             ix->stats.kernel_launches++;
             ix->stats.bytes_d2h += (uint64_t)m * sizeof(NkFilter);
+        }
+        if (win) {  // ... and so is its qwindow slot
+            if (nk::ws_reserve((void **)&o->ws.qwindow, &o->ws.qwindow_bytes, (size_t)m * sizeof(NkWindow))) return -1;
+            if (nk::row_windows(o->ws.sub_rows, m, o->mask_on ? o->mask : nullptr, o->tags_on ? o->tags : nullptr,
+                                o->values_on ? o->values : nullptr, admit->f, admit->w, admit->gap, o->ws.qwindow, o->stream))
+                return -1;
+            NK_CUDA_OK(cudaMemcpyAsync(part_w.data(), o->ws.qwindow, (size_t)m * sizeof(NkWindow), cudaMemcpyDeviceToHost, o->stream));
+            ix->stats.kernel_launches++;
+            ix->stats.bytes_d2h += (uint64_t)m * sizeof(NkWindow);
         }
         NK_CUDA_OK(cudaStreamSynchronize(o->stream));
         ix->stats.bytes_h2d += (uint64_t)m * 4;
@@ -1433,20 +1461,26 @@ static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, cons
         ix->stats.kernel_launches++;
         for (uint32_t i = 0; i < m; ++i) {
             memcpy(blk + (size_t)pos[i] * ix->dim, part + (size_t)i * ix->dim, rb);
-            if (admit) filters[pos[i]] = part_f[i];
+            if (admit && !win) filters[pos[i]] = part_f[i];
+            if (win) windows[pos[i]] = part_w[i];
         }
     }
-    *stage = [ix, blk, nb, rb, filters](NkShard &s) {
+    *stage = [ix, blk, nb, rb, filters, windows](NkShard &s) {
         NK_CUDA_OK(cudaMemcpyAsync(s.ws.queries, blk, (size_t)nb * rb, cudaMemcpyHostToDevice, s.stream));
         ix->stats.bytes_h2d += (uint64_t)nb * rb;
+        if (!windows.empty()) {
+            const NkFilter *qf;
+            const NkWindow *qw;
+            return stage_windows(ix, s, filters.data(), windows.data(), nb, &qf, &qw);
+        }
         if (!filters.empty() && !stage_filters(ix, s, filters.data(), nb)) return -1;
         return 0;
     };
     return 0;
 }
 
-// The body of nk_search_rows and nk_search_rows_filtered (opts.filters_host [Q] or nullptr), the index lock held and the ids
-// checked: returns ke, the entries written per query (the rest of each k-wide output row is left as it is).
+// The body of nk_search_rows, nk_search_rows_filtered and nk_search_rows_windowed (opts.filters_host / opts.windows_host [Q] or
+// nullptr), the index lock held and the ids checked: returns ke, the entries written per query (the rest of each k-wide output row is left as it is).
 static int search_rows_locked(NkIndex *ix, const std::vector<NkShard *> &live, const uint32_t *rows_host, const SearchOpts &opts,
                               uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
     const uint64_t N = ix->returnable_rows();
@@ -1460,7 +1494,7 @@ static int search_rows_locked(NkIndex *ix, const std::vector<NkShard *> &live, c
         const uint32_t *ids = rows_host + b;
         StageQueries stage;
         if (stage_row_block(ix, live, ids, nb, nullptr, &stage)) return -1;
-        const SearchOpts block{opts.path, opts.filters_host ? opts.filters_host + b : nullptr};
+        const SearchOpts block{opts.path, opts.filters_host ? opts.filters_host + b : nullptr, opts.windows_host ? opts.windows_host + b : nullptr};
         if (search_live(ix, live, stage, block, nb, kk, kk, bidx.data(), bsc.data()) < 0) return -1;
         for (uint32_t q = 0; q < nb; ++q) {
             const uint32_t self = (uint32_t)(ix->row_base + ids[q]);
@@ -1480,9 +1514,10 @@ static int search_rows_locked(NkIndex *ix, const std::vector<NkShard *> &live, c
     return (int)ke;
 }
 
-// nk_search_rows / nk_search_rows_filtered: filters_host == nullptr is plain nk_search_rows.
-static int search_rows_host(NkIndex *ix, const char *what, const uint32_t *rows_host, const NkFilter *filters_host, uint32_t Q, uint32_t k,
-                            uint32_t *out_idx, float *out_score) {
+// nk_search_rows / nk_search_rows_filtered / nk_search_rows_windowed: filters_host == windows_host == nullptr is plain
+// nk_search_rows.
+static int search_rows_host(NkIndex *ix, const char *what, const uint32_t *rows_host, const NkFilter *filters_host,
+                            const NkWindow *windows_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
     if (Q && (!rows_host || !out_idx || !out_score)) { nk::set_error("null argument"); return -1; }
@@ -1501,16 +1536,21 @@ static int search_rows_host(NkIndex *ix, const char *what, const uint32_t *rows_
     ScopedRange range(what);
     ShardOrder order(ix);
     if (order.failed()) return -1;
-    return search_rows_locked(ix, live_shards(ix), rows_host, SearchOpts{ix->path, filters_host}, Q, k, out_idx, out_score);
+    return search_rows_locked(ix, live_shards(ix), rows_host, SearchOpts{ix->path, filters_host, windows_host}, Q, k, out_idx, out_score);
 }
 
 int nk_search_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
-    return search_rows_host(ix, "nk_search_rows", rows_host, nullptr, Q, k, out_idx, out_score);
+    return search_rows_host(ix, "nk_search_rows", rows_host, nullptr, nullptr, Q, k, out_idx, out_score);
 }
 
 int nk_search_rows_filtered(NkIndex *ix, const uint32_t *rows_host, const NkFilter *filters_host, uint32_t Q, uint32_t k,
                             uint32_t *out_idx, float *out_score) {
-    return search_rows_host(ix, "nk_search_rows_filtered", rows_host, filters_host, Q, k, out_idx, out_score);
+    return search_rows_host(ix, "nk_search_rows_filtered", rows_host, filters_host, nullptr, Q, k, out_idx, out_score);
+}
+
+int nk_search_rows_windowed(NkIndex *ix, const uint32_t *rows_host, const NkFilter *filters_host, const NkWindow *windows_host,
+                            uint32_t Q, uint32_t k, uint32_t *out_idx, float *out_score) {
+    return search_rows_host(ix, "nk_search_rows_windowed", rows_host, filters_host, windows_host, Q, k, out_idx, out_score);
 }
 
 // ---- range search ---------------------------------------------------------------------------------------------------
@@ -1702,12 +1742,21 @@ int nk_search_range_windowed(NkIndex *ix, const float *queries_host, const float
 // device as nk_search_rows gathers them.  For a block starting at row s0 the scan skips every shard whose rows all lie at or
 // below s0, and in the shard holding s0 covers only the window from s0 rounded down to the 256-row scan tile; the re-scoring
 // kernel keeps row j for the block's query q only if j > s0 + q.  Left rows that fail the row mask or the filter get the filter
-// that admits no row, on the device that holds them.  Each block's merged survivors are staged in host memory (8 B per pair)
+// that admits no row, on the device that holds them.  A windowed join (a window, a band or both) also gives each left row its
+// own value window on that device (nk::row_windows) and scans in the windowed range mode: the band is symmetric, so the
+// triangle still holds each unordered pair once.  Each block's merged survivors are staged in host memory (8 B per pair)
 // until the whole stripe is done, so the offsets and the total are exact before anything is written.
 constexpr uint64_t SCAN_TILE_ROWS = 256;
 
 int nk_search_pairs(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float threshold, const NkFilter *filter, uint64_t capacity,
                     uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total) {
+    return nk_search_pairs_windowed(ix, first_row, n_rows, threshold, filter, nullptr, NK_NO_GAP, capacity, out_offsets, out_idx,
+                                    out_score, out_total);
+}
+
+int nk_search_pairs_windowed(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float threshold, const NkFilter *filter,
+                             const NkWindow *window, uint64_t max_gap, uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx,
+                             float *out_score, uint64_t *out_total) {
     nk::DeviceGuard _restore_device;
     if (!ix) { nk::set_error("null index"); return -1; }
     if (n_rows && (!out_offsets || !out_total)) { nk::set_error("null argument"); return -1; }
@@ -1733,8 +1782,12 @@ int nk_search_pairs(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float thre
     if (order.failed()) return -1;
 
     const std::vector<NkShard *> live = live_shards(ix);
-    const bool admit = filter || ix->mask_on;  // some left rows may be inadmissible: per-query filters
-    const NkFilter f = filter ? *filter : NkFilter{0, 0, 0};
+    RowAdmit adm;
+    adm.windowed = window || max_gap != NK_NO_GAP;  // per-query windows too (a windowed scan is also a tag-filtered one)
+    const bool admit = filter || ix->mask_on || adm.windowed;  // some left rows may be inadmissible: per-query filters
+    if (filter) adm.f = *filter;
+    if (window) adm.w = *window;
+    adm.gap = max_gap;
     const uint32_t QB = (uint32_t)std::min<uint64_t>(n_rows, SEARCH_ROWS_BLOCK);
     const std::vector<uint32_t> thr(QB, nk::ord_bits(range_key_threshold(ix, threshold)));
     std::vector<uint32_t> ids(QB);
@@ -1752,10 +1805,11 @@ int nk_search_pairs(NkIndex *ix, uint64_t first_row, uint64_t n_rows, float thre
             scan.from.push_back(lo <= s0 ? (s0 - lo) / SCAN_TILE_ROWS * SCAN_TILE_ROWS : 0);
         }
         StageQueries stage;
-        if (!scan.shards.empty() && stage_row_block(ix, live, ids.data(), nb, admit ? &f : nullptr, &stage)) return -1;
+        if (!scan.shards.empty() && stage_row_block(ix, live, ids.data(), nb, admit ? &adm : nullptr, &stage)) return -1;
         const uint64_t pair_first = ix->row_base + s0;
         RangeBlock block{ix->path, nb, thr.data()};
         block.filtered = admit;
+        block.windowed = adm.windowed;
         block.pair_first = &pair_first;
         if (range_scan(ix, &scan, stage, block, &per_query)) return -1;
         for (uint32_t q = 0; q < nb; ++q) out_offsets[b + q + 1] = out_offsets[b + q] + per_query[q];
@@ -2022,7 +2076,7 @@ static int graph_reverse_scan(NkIndex *ix, const GraphCall &g, const std::vector
     // of the tag-filtered one)
     std::vector<uint64_t> tags, qtags;
     if (g.filters && host_row_tags(ix, &tags)) return -1;
-    const NkFilter all_rows{0, 0, 0};  // masked-out queries get the filter that admits no row (stage_row_block)
+    const RowAdmit all_rows;  // masked-out queries get the filter that admits no row (stage_row_block)
     const uint32_t QB = (uint32_t)std::min<size_t>(C.size(), SEARCH_ROWS_BLOCK);
     const std::vector<uint32_t> floor_thr(QB, nk::ord_bits(ix->key_floor()));
     RangeBlock block{path, 0, floor_thr.data()};

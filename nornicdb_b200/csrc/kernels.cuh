@@ -272,5 +272,10 @@ int gather_rows(const void *rows, int dtype, uint32_t dim, const uint32_t *idx, 
 // row) and f admits its tag (tags nullptr = tag 0), else the filter that admits no row (all_of = none_of = ~0).
 int row_filters(const uint32_t *idx, uint32_t n_idx, const uint32_t *mask, const uint64_t *tags, NkFilter f, NkFilter *out,
                 cudaStream_t s);
+// Left-row windows of a windowed self-join (nk_search_pairs_windowed): out[r] = w, narrowed to [v - gap, v + gap] (saturating,
+// and never below key 1) where gap != NK_NO_GAP, if local row idx[r] passes the row mask and f, and its value key v (values
+// nullptr = key 0) lies in w and, under a band, is not 0; else the window that admits no row (lo = ~0, hi = 0).
+int row_windows(const uint32_t *idx, uint32_t n_idx, const uint32_t *mask, const uint64_t *tags, const uint64_t *values, NkFilter f,
+                NkWindow w, uint64_t gap, NkWindow *out, cudaStream_t s);
 
 }  // namespace nk

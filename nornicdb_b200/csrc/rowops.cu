@@ -226,6 +226,27 @@ __global__ void row_filters_kernel(const uint32_t *idx, uint32_t n_idx, const ui
     out[r] = in_mask && tag_admits(tag, f.all_of, f.none_of, f.any_of) ? f : NkFilter{~0ull, ~0ull, 0ull};
 }
 
+__global__ void row_windows_kernel(const uint32_t *idx, uint32_t n_idx, const uint32_t *mask, const uint64_t *tags, const uint64_t *values,
+                                   NkFilter f, NkWindow w, uint64_t gap, NkWindow *out) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= n_idx) return;
+    const uint32_t row = idx[r];
+    const bool in_mask = !mask || ((mask[row >> 5] >> (row & 31)) & 1u);
+    const uint64_t tag = tags ? tags[row] : 0ull;
+    const uint64_t v = values ? values[row] : 0ull;
+    const bool band = gap != NK_NO_GAP;
+    NkWindow o{~0ull, 0ull};  // admits no row
+    if (in_mask && tag_admits(tag, f.all_of, f.none_of, f.any_of) && window_admits(v, w.lo, w.hi) && (!band || v != 0)) {
+        o = w;
+        if (band) {  // [v - gap, v + gap], saturating, without key 0 (a row without a value is in no band)
+            const uint64_t lo = v > gap ? v - gap : 1ull, hi = v > ~0ull - gap ? ~0ull : v + gap;
+            o.lo = o.lo > lo ? o.lo : lo;
+            o.hi = o.hi < hi ? o.hi : hi;
+        }
+    }
+    out[r] = o;
+}
+
 // |x|^2 per row of a 16-bit corpus (fp32 accumulation of the exactly widened elements)
 template <typename T>
 __global__ void row_sqnorms16_kernel(const T *rows, uint64_t n, uint32_t dim, float *out) {
@@ -414,6 +435,13 @@ int row_filters(const uint32_t *idx, uint32_t n_idx, const uint32_t *mask, const
                 cudaStream_t s) {
     if (n_idx == 0) return 0;
     row_filters_kernel<<<(n_idx + 255) / 256, 256, 0, s>>>(idx, n_idx, mask, tags, f, out);
+    NK_CUDA_OK(cudaGetLastError());
+    return 0;
+}
+int row_windows(const uint32_t *idx, uint32_t n_idx, const uint32_t *mask, const uint64_t *tags, const uint64_t *values, NkFilter f,
+                NkWindow w, uint64_t gap, NkWindow *out, cudaStream_t s) {
+    if (n_idx == 0) return 0;
+    row_windows_kernel<<<(n_idx + 255) / 256, 256, 0, s>>>(idx, n_idx, mask, tags, values, f, w, gap, out);
     NK_CUDA_OK(cudaGetLastError());
     return 0;
 }

@@ -378,6 +378,12 @@ public:
     // both nodes must pass.  The join runs in stripes of at most stripeRows left rows, so the staging (8 B per pair) and the
     // cost of a call that outgrows its buffer stay bounded.  Sizes its buffers from the library's exact total.
     std::vector<SimilarPair> SearchPairs(float threshold, const NkFilter *filter = nullptr, uint64_t stripeRows = 1u << 16) {
+        return SearchPairs(threshold, filter, nullptr, NK_NO_GAP, stripeRows);
+    }
+    // ... with value conditions on both nodes: window = nullptr or one NkWindow both value keys must lie in; maxGap = a band,
+    // |key(A) - key(B)| <= maxGap with both keys set (NK_NO_GAP: none), e.g. near-duplicates within the same hour.
+    std::vector<SimilarPair> SearchPairs(float threshold, const NkFilter *filter, const NkWindow *window, uint64_t maxGap,
+                                         uint64_t stripeRows = 1u << 16) {
         std::lock_guard<std::mutex> lk(mu_);
         std::vector<SimilarPair> out;
         const uint64_t n = nk_index_rows(ix_);
@@ -389,7 +395,8 @@ public:
             std::vector<uint64_t> off(rows + 1);
             uint64_t total = 0;
             for (int pass = 0; pass < 2; ++pass) {
-                if (nk_search_pairs(ix_, first, rows, threshold, filter, idx.size(), off.data(), idx.data(), sc.data(), &total) < 0)
+                if (nk_search_pairs_windowed(ix_, first, rows, threshold, filter, window, maxGap, idx.size(), off.data(), idx.data(), sc.data(),
+                                             &total) < 0)
                     throw cuda::ErrKernelExecution(std::string("gpu: ") + nk_last_error());
                 if (total <= idx.size()) break;
                 idx.resize(total);
@@ -406,11 +413,19 @@ public:
     // (missing ids are ignored, as in ScoreSubset).  filters empty = none, else one tag filter per id (e.g. "same collection"):
     // each list then holds only nodes its filter admits.
     std::vector<std::vector<SearchResult>> SearchSimilar(const std::vector<std::string> &ids, int k, const std::vector<NkFilter> &filters = {}) {
+        return SearchSimilar(ids, k, filters, {});
+    }
+    // ... with one value window per id on top (windows empty = none: the call above), e.g. "nodes like this one from the last
+    // 7 days": each list then holds only nodes whose value key the id's window admits.
+    std::vector<std::vector<SearchResult>> SearchSimilar(const std::vector<std::string> &ids, int k, const std::vector<NkFilter> &filters,
+                                                         const std::vector<NkWindow> &windows) {
         if (!filters.empty() && filters.size() != ids.size()) throw std::invalid_argument("gpu: one filter per id");
+        if (!windows.empty() && windows.size() != ids.size()) throw std::invalid_argument("gpu: one window per id");
         std::lock_guard<std::mutex> lk(mu_);
         std::vector<std::vector<SearchResult>> out(ids.size());
         std::vector<uint32_t> rows;
         std::vector<NkFilter> f;
+        std::vector<NkWindow> w;
         std::vector<size_t> at;
         for (size_t i = 0; i < ids.size(); ++i) {
             auto it = idToIndex_.find(ids[i]);
@@ -418,13 +433,14 @@ public:
                 rows.push_back((uint32_t)it->second);
                 at.push_back(i);
                 if (!filters.empty()) f.push_back(filters[i]);
+                if (!windows.empty()) w.push_back(windows[i]);
             }
         }
         if (rows.empty() || k <= 0) return out;
         std::vector<uint32_t> idx(rows.size() * (size_t)k);
         std::vector<float> sc(rows.size() * (size_t)k);
-        int got = nk_search_rows_filtered(ix_, rows.data(), f.empty() ? nullptr : f.data(), (uint32_t)rows.size(), (uint32_t)k, idx.data(),
-                                          sc.data());
+        int got = nk_search_rows_windowed(ix_, rows.data(), f.empty() ? nullptr : f.data(), w.empty() ? nullptr : w.data(), (uint32_t)rows.size(),
+                                          (uint32_t)k, idx.data(), sc.data());
         if (got < 0) throw cuda::ErrKernelExecution(std::string("gpu: ") + nk_last_error());
         for (size_t j = 0; j < rows.size(); ++j)
             for (int i = 0; i < got; ++i) {

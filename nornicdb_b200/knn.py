@@ -244,25 +244,33 @@ class KnnIndex:
                                        sc.ctypes.data_as(C.c_void_p)), "nk_search")
         return idx[:, :ke], sc[:, :ke]
 
-    def search_rows(self, rows, k: int, filters=None) -> Tuple[np.ndarray, np.ndarray]:
+    def search_rows(self, rows, k: int, filters=None, windows=None) -> Tuple[np.ndarray, np.ndarray]:
         """The k nearest OTHER rows of stored rows: rows = row ids (< len(self), repeats allowed), each searched as stored now
         -> (idx [Q x k'] uint32, score [Q x k'] fp32), k' = min(k, admissible rows), with search()'s conventions.  A query
         with fewer admissible other rows gets index 0xffffffff and score 0 in its unused slots.  rows = every row id gives
         the k-NN graph of the index in one call (served in blocks of 1024 queries).  filters: None, or one tag filter per
         query ([Q x 3] uint64, as in search_filtered): query q then lists only rows its filter admits (its own row may be
-        refused by it) (nk_search_rows_filtered)."""
+        refused by it) (nk_search_rows_filtered).  windows: None, or one value window per query ([Q x 2] uint64, as in
+        search_windowed; one pair applies to every query): query q then lists only rows whose value key its window admits (its
+        own row may lie outside it); band_windows(keys[rows], below, above) gives "near this row's value"
+        (nk_search_rows_windowed)."""
         r = np.asarray(rows, dtype=np.int64).reshape(-1)
         if r.size and (r.min() < 0 or r.max() > 0xFFFFFFFF):
             raise KnnError("search_rows: row ids must be in [0, 2^32)")
         r = np.ascontiguousarray(r.astype(np.uint32))
         Q = r.size
         f = None if filters is None else as_filters(filters, Q)
+        w = None if windows is None else as_windows(windows, Q)
         k = int(k)
         if k <= 0 or Q == 0:
             return np.empty((Q, 0), np.uint32), np.empty((Q, 0), np.float32)
         idx = np.empty((Q, k), dtype=np.uint32)
         sc = np.empty((Q, k), dtype=np.float32)
-        if f is None:
+        if w is not None:
+            ke = _check(self.lib.nk_search_rows_windowed(self.ptr, r.ctypes.data_as(C.c_void_p), None if f is None else f.ctypes.data_as(C.c_void_p),
+                                                         w.ctypes.data_as(C.c_void_p), Q, k, idx.ctypes.data_as(C.c_void_p),
+                                                         sc.ctypes.data_as(C.c_void_p)), "nk_search_rows_windowed")
+        elif f is None:
             ke = _check(self.lib.nk_search_rows(self.ptr, r.ctypes.data_as(C.c_void_p), Q, k, idx.ctypes.data_as(C.c_void_p),
                                                 sc.ctypes.data_as(C.c_void_p)), "nk_search_rows")
         else:
@@ -433,27 +441,38 @@ class KnnIndex:
         return [(idx[o[i]:o[i + 1]].copy(), sc[o[i]:o[i + 1]].copy()) for i in range(Q)]
 
     def search_pairs(self, threshold: float, first_row: int = 0, n_rows: Optional[int] = None,
-                     filter=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+                     filter=None, window=None, max_gap=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
         """Similarity self-join: for each left row i of the stripe [first_row, first_row + n_rows) (default: to the end of the
         index), every admissible row j > i whose score against row i reaches `threshold` (cosine / dot: minimum score;
         euclidean: maximum distance), so each pair of the stripe appears once, under its lower row.  filter = one
         (all_of, none_of, any_of) tag filter for both sides, None = none.  Returns CSR arrays (offsets uint64 [n_rows + 1],
         idx uint32, score float32): row first_row + r's list is [offsets[r], offsets[r + 1]), in search()'s order.  The result
-        buffer grows to the size the library reports (nk_search_pairs' size protocol); a call that outgrows it joins twice."""
+        buffer grows to the size the library reports (nk_search_pairs' size protocol); a call that outgrows it joins twice.
+        window = one (lo, hi) value window for both sides, None = none.  max_gap = a band: a pair also needs both rows to have a
+        value and |key[i] - key[j]| <= max_gap, in key units (value units for int and datetime columns); an np.timedelta64 is
+        taken in nanoseconds.  None = no band (nk_search_pairs_windowed)."""
         first_row = int(first_row)
         n_rows = max(len(self) - first_row, 0) if n_rows is None else int(n_rows)
         if first_row < 0 or n_rows < 0:
             raise KnnError("search_pairs: first_row and n_rows must be >= 0")
         f = None if filter is None else as_filters(filter, 1)
+        w = None if window is None else as_windows(window, 1)
+        gap = NO_GAP if max_gap is None else _gap_keys(max_gap)
+        windowed = w is not None or gap != NO_GAP
         off = np.zeros(n_rows + 1, dtype=np.uint64)
         total = C.c_uint64(0)
         cap = getattr(self, "_pairs_cap", 0)
         while True:
             idx = np.empty(max(cap, 1), dtype=np.uint32)
             sc = np.empty(max(cap, 1), dtype=np.float32)
-            _check(self.lib.nk_search_pairs(self.ptr, first_row, n_rows, float(threshold), None if f is None else f.ctypes.data_as(C.c_void_p),
-                                            cap, off.ctypes.data_as(C.c_void_p), idx.ctypes.data_as(C.c_void_p),
-                                            sc.ctypes.data_as(C.c_void_p), C.byref(total)), "nk_search_pairs")
+            out = (cap, off.ctypes.data_as(C.c_void_p), idx.ctypes.data_as(C.c_void_p), sc.ctypes.data_as(C.c_void_p), C.byref(total))
+            fp = None if f is None else f.ctypes.data_as(C.c_void_p)
+            if windowed:
+                _check(self.lib.nk_search_pairs_windowed(self.ptr, first_row, n_rows, float(threshold), fp,
+                                                         None if w is None else w.ctypes.data_as(C.c_void_p), gap, *out),
+                       "nk_search_pairs_windowed")
+            else:
+                _check(self.lib.nk_search_pairs(self.ptr, first_row, n_rows, float(threshold), fp, *out), "nk_search_pairs")
             if total.value <= cap:
                 break
             cap = int(total.value)
@@ -736,6 +755,39 @@ def as_windows(windows, Q: int) -> np.ndarray:
     if w.shape[0] != Q:
         raise KnnError(f"windows: {w.shape[0]} rows for {Q} queries")
     return w
+
+
+NO_GAP = ALL_BITS  # nk_search_pairs_windowed: no band
+
+
+def _gap_keys(gap) -> int:
+    """A band width in key units: an int >= 0 (< NO_GAP), or an np.timedelta64 / datetime.timedelta, in nanoseconds."""
+    if isinstance(gap, (np.timedelta64, _dt.timedelta)):
+        g = np.timedelta64(gap).astype("timedelta64[ns]").astype(np.int64)
+        if g == _I64_MIN:
+            raise KnnError("max_gap: NaT")
+        gap = int(g)
+    elif isinstance(gap, (bool, np.bool_, float, np.floating)) or not isinstance(gap, (int, np.integer)):
+        raise KnnError(f"max_gap: an integer number of key units or a timedelta, not {type(gap).__name__}")
+    gap = int(gap)
+    if gap < 0 or gap >= NO_GAP:
+        raise KnnError(f"max_gap: {gap} outside [0, 2^64 - 1)")
+    return gap
+
+
+def band_windows(keys, below, above=None) -> np.ndarray:
+    """Per-row value windows [key - below, key + above] (above defaults to below), saturating at 1 and 2^64 - 1, as [n x 2]
+    uint64: the windows of a time-local k-NN graph or of "near this row" search_rows calls.  below / above are in key units
+    (ints, or np.timedelta64 in nanoseconds for datetime columns, as for search_pairs' max_gap).  A row without a value (key 0)
+    gets EMPTY_WINDOW, and no window admits key 0."""
+    k = np.asarray(keys, dtype=np.uint64).reshape(-1)
+    b = _gap_keys(below)
+    a = b if above is None else _gap_keys(above)
+    lo = np.where(k > np.uint64(b), k - np.uint64(b), np.uint64(1))
+    hi = np.where(k > np.uint64(ALL_BITS - a), np.uint64(ALL_BITS), k + np.uint64(a))
+    w = np.stack([lo, hi], axis=1).astype(np.uint64)
+    w[k == 0] = EMPTY_WINDOW
+    return np.ascontiguousarray(w)
 
 
 def window_admits(keys, lo: int, hi: int):
