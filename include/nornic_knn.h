@@ -253,9 +253,9 @@ int nk_search_device(NkIndex *ix, const float *queries_dev, uint32_t Q, uint32_t
  * tag, remove_swap moves the last row's tag with its row; upload, upload_from_f32, fill_* and attach_device_rows reset every
  * tag to 0.
  * Not filtered: nk_search_groups, nk_score_subset, nk_search_keys_device, nk_search_sharded_device and the k-means calls.
- * Not windowed (value windows, below): the graph update and remap calls, nk_search_groups, nk_score_subset,
- * nk_search_keys_device, nk_search_sharded_device, the exchange calls and the k-means calls (search by stored row and the
- * self-join have windowed forms: nk_search_rows_windowed, nk_search_pairs_windowed). */
+ * Not windowed (value windows, below): nk_search_groups, nk_score_subset, nk_search_keys_device, nk_search_sharded_device,
+ * the exchange calls and the k-means calls (search by stored row, the self-join and the graph calls have windowed forms:
+ * nk_search_rows_windowed, nk_search_pairs_windowed, nk_knn_graph_update_windowed, nk_knn_graph_remap_windowed). */
 typedef struct NkFilter {
     uint64_t all_of, none_of, any_of;
 } NkFilter;
@@ -458,6 +458,26 @@ int nk_knn_graph_update_filtered(NkIndex *ix, uint32_t k, uint64_t n_old, const 
 int nk_knn_graph_remap_filtered(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row, const NkFilter *filters_host,
                                 const uint32_t *graph_idx_in, const float *graph_score_in, uint32_t *graph_idx_out,
                                 float *graph_score_out, uint64_t *n_lists_changed);
+
+/* Windowed k-NN graphs: time-local graphs ("related events in the same week") kept exact across updates.  windows_host [N]:
+ * the value window of each current row's list, in current row order (knn.band_windows gives each row its own +-delta band);
+ * NULL = none: then the _filtered call bit for bit, running the same kernels.  filters_host [N] as in the _filtered calls
+ * (NULL = no tag filter).  The graph is what nk_search_rows_windowed(rows 0 .. N-1, filters_host, windows_host, k) returns,
+ * bit for bit (order, ties, scores, padding): row r's list holds only rows whose value key r's window admits.  On entry the
+ * old graph is that call's result at the time it was built.  Arguments, return value, refusals, the NaN caveat, locking and
+ * every other precondition: those of the unfiltered calls.
+ * One more precondition (not checked): every kept row has the tag, value key, filter and window its contents had when the
+ * graph was built.  Report a row whose value key or window changed as new contents, exactly like a rewritten row (a changed
+ * row, or NK_ROW_NEW).  A band window moves with its row's key, so re-valuing a row is such a report.
+ * Rows searched again are searched with their own filter and window, and the scan of new and moved rows also holds each
+ * pair (row r, new row c) to r's window admitting c's value key, inside the scan kernel. */
+int nk_knn_graph_update_windowed(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
+                                 const NkFilter *filters_host, const NkWindow *windows_host,
+                                 uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed);
+int nk_knn_graph_remap_windowed(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row,
+                                const NkFilter *filters_host, const NkWindow *windows_host,
+                                const uint32_t *graph_idx_in, const float *graph_score_in,
+                                uint32_t *graph_idx_out, float *graph_score_out, uint64_t *n_lists_changed);
 
 /* Multi-process sharding (one rank per GPU): emit this shard's sorted candidate list as packed 64-bit
  * keys [Q x k] (order-preserving score bits << 32 | ~row index; larger key = better), to be exchanged

@@ -90,6 +90,8 @@ SIGNATURES = {
     "nk_knn_graph_remap": (_i, [_vp, C.c_uint32, _u64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nk_knn_graph_update_filtered": (_i, [_vp, C.c_uint32, _u64, _vp, C.c_uint32, _vp, _vp, _vp, _vp]),
     "nk_knn_graph_remap_filtered": (_i, [_vp, C.c_uint32, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "nk_knn_graph_update_windowed": (_i, [_vp, C.c_uint32, _u64, _vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp]),
+    "nk_knn_graph_remap_windowed": (_i, [_vp, C.c_uint32, _u64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nk_search_keys_device":(_i, [_vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp]),
     "nk_merge_keys_device": (_i, [_i, _vp, C.c_uint32, C.c_uint32, C.c_uint32, _i, _vp, _vp, _vp]),
     "nk_score_subset": (_i, [_vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp]),

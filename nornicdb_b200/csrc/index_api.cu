@@ -1588,8 +1588,10 @@ struct RangeBlock {
     // The reverse scan of a k-NN graph update.  Every row has its own threshold, s.ws.row_thr [s.n], and the mask words behind
     // them, s.ws.row_thr + s.n, TAKE THE PLACE OF the index's row mask: they select the rows whose lists are updated, not the
     // rows that may be returned.  row_filters (a filtered graph; `filtered` must be set too): a pair (row, query) is listed only
-    // if the row's own filter, s.ws.row_filter [s.n], admits the query's tag, s.ws.qtags [Q].
-    bool reverse = false, row_filters = false;
+    // if the row's own filter, s.ws.row_filter [s.n], admits the query's tag, s.ws.qtags [Q].  row_windows (a windowed graph;
+    // `row_filters` must be set too): ... and if the row's own window, s.ws.row_window [s.n], admits the query's value key,
+    // s.ws.qvalues [Q].
+    bool reverse = false, row_filters = false, row_windows = false;
 };
 
 // One shard's range scan of a block, rows [from, s.n): path, scan and exact re-scoring -> counts[Q] (host), *list_cap
@@ -1603,10 +1605,12 @@ static int range_shard(NkIndex *ix, NkShard &s, const RangeBlock &b, uint64_t fr
     if (use < 0) return -1;
     a.mode = b.windowed ? nk::ScanMode::RANGE_WINDOW : b.filtered ? nk::ScanMode::RANGE_TAGS : nk::ScanMode::RANGE;
     if (b.reverse) {
-        a.mode = b.row_filters ? nk::ScanMode::REVERSE_RFILT : b.filtered ? nk::ScanMode::REVERSE_TAGS : nk::ScanMode::REVERSE;
+        a.mode = b.row_windows ? nk::ScanMode::REVERSE_RWINDOW
+                 : b.row_filters ? nk::ScanMode::REVERSE_RFILT : b.filtered ? nk::ScanMode::REVERSE_TAGS : nk::ScanMode::REVERSE;
         a.row_thr = s.ws.row_thr;
         a.row_mask = reinterpret_cast<const uint32_t *>(s.ws.row_thr + s.n);
         if (b.row_filters) { a.row_filter = s.ws.row_filter; a.qtags = s.ws.qtags; }
+        if (b.row_windows) { a.row_window = s.ws.row_window; a.qvalues = s.ws.qvalues; }
     }
     if (from) {
         a.rows = static_cast<const char *>(a.rows) + from * ix->dim * ix->esz();
@@ -1850,13 +1854,14 @@ static int admissible_rows(NkIndex *ix, std::vector<uint8_t> *ok) {
     return 0;
 }
 
-// The tag word of each current row (relative id) -> tags[rows()]; 0 where a shard has no tags.
-static int host_row_tags(NkIndex *ix, std::vector<uint64_t> *tags) {
-    tags->assign(ix->rows(), 0ull);
+// The tag word (values = false) or value key (values = true) of each current row (relative id) -> words[rows()]; 0 where a
+// shard has none.
+static int host_row_words(NkIndex *ix, bool values, std::vector<uint64_t> *words) {
+    words->assign(ix->rows(), 0ull);
     for (auto &s : ix->shards) {
-        if (s.n == 0 || !s.tags_on) continue;
+        if (s.n == 0 || !(values ? s.values_on : s.tags_on)) continue;
         NK_CUDA_OK(cudaSetDevice(s.device));
-        NK_CUDA_OK(cudaMemcpyAsync(tags->data() + ix->first_row(s), s.tags, s.n * 8, cudaMemcpyDeviceToHost, s.stream));
+        NK_CUDA_OK(cudaMemcpyAsync(words->data() + ix->first_row(s), values ? s.values : s.tags, s.n * 8, cudaMemcpyDeviceToHost, s.stream));
         NK_CUDA_OK(cudaStreamSynchronize(s.stream));
         ix->stats.bytes_d2h += s.n * 8;
     }
@@ -1933,13 +1938,17 @@ static int graph_pair_keys_on(NkIndex *ix, const std::vector<NkShard *> &live, N
 // f's, else only the kept rows'.  filters [N] (nullptr: none): the graph of nk_search_rows_filtered, each row's list bounded by
 // its own filter.  A kept row has the tag and the filter it had when the graph was built (the caller reports any other row as
 // new), so the rows searched again are the same; they are searched with their own filters, and the reverse scan also holds
-// each pair (r, c) to r's filter admitting c's tag.
+// each pair (r, c) to r's filter admitting c's tag.  windows [N] (nullptr: none): the graph of nk_search_rows_windowed, each
+// row's list bounded by its own window as well, in the same way: a kept row has the value key and the window it had, the rows
+// searched again are searched with their own windows, and the reverse scan holds each pair (r, c) to r's window admitting c's
+// value key.
 struct GraphCall {
     const char *what;
     uint32_t k;
     uint64_t n_old;
     const uint32_t *src;
     const NkFilter *filters;
+    const NkWindow *windows;
     const uint32_t *gi_in; const float *gs_in;
     uint32_t *gi; float *gs;
     bool by_id;
@@ -2037,7 +2046,9 @@ static int graph_rows_searched_again(NkIndex *ix, const GraphCall &g, const std:
 }
 
 // Before the reverse scan: every live shard gets its per-row thresholds and, behind them, the mask of the rows outside R
-// (s.ws.row_thr), and with filters each row's own filter for the row side of the scan (s.ws.row_filter).
+// (s.ws.row_thr), with filters each row's own filter for the row side of the scan (s.ws.row_filter), and with windows each
+// row's own window (s.ws.row_window).  A windowed scan is a row-filter scan: without filters its row filters are {0,0,0},
+// which admit every tag, written on the device.
 static int graph_upload_row_thresholds(NkIndex *ix, const GraphCall &g, const std::vector<NkShard *> &live, const std::vector<uint8_t> &in_r) {
     const uint32_t k = g.k;
     for (NkShard *s : live) {
@@ -2059,6 +2070,14 @@ static int graph_upload_row_thresholds(NkIndex *ix, const GraphCall &g, const st
             if (nk::ws_reserve((void **)&s->ws.row_filter, &s->ws.row_filter_bytes, s->n * sizeof(NkFilter))) return -1;
             NK_CUDA_OK(cudaMemcpyAsync(s->ws.row_filter, g.filters + lo, s->n * sizeof(NkFilter), cudaMemcpyHostToDevice, s->stream));
             ix->stats.bytes_h2d += s->n * sizeof(NkFilter);
+        } else if (g.windows) {
+            if (nk::ws_reserve((void **)&s->ws.row_filter, &s->ws.row_filter_bytes, s->n * sizeof(NkFilter))) return -1;
+            NK_CUDA_OK(cudaMemsetAsync(s->ws.row_filter, 0, s->n * sizeof(NkFilter), s->stream));
+        }
+        if (g.windows) {
+            if (nk::ws_reserve((void **)&s->ws.row_window, &s->ws.row_window_bytes, s->n * sizeof(NkWindow))) return -1;
+            NK_CUDA_OK(cudaMemcpyAsync(s->ws.row_window, g.windows + lo, s->n * sizeof(NkWindow), cudaMemcpyHostToDevice, s->stream));
+            ix->stats.bytes_h2d += s->n * sizeof(NkWindow);
         }
         NK_CUDA_OK(cudaStreamSynchronize(s->stream));  // thr is pageable and goes out of scope
         ix->stats.bytes_h2d += thr.size() * 4;
@@ -2072,33 +2091,44 @@ using GraphEntrants = std::vector<std::pair<uint32_t, uint64_t>>;
 static int graph_reverse_scan(NkIndex *ix, const GraphCall &g, const std::vector<NkShard *> &live, int path, const std::vector<uint8_t> &in_r,
                               const std::vector<uint32_t> &C, GraphEntrants *entrants) {
     if (graph_upload_row_thresholds(ix, g, live, in_r)) return -1;
-    // a filtered graph's queries also carry their tags, and always a per-query filter (the row-filtered scan is a mode
-    // of the tag-filtered one)
-    std::vector<uint64_t> tags, qtags;
-    if (g.filters && host_row_tags(ix, &tags)) return -1;
+    // a filtered graph's queries also carry their tags, a windowed graph's their value keys (and tag 0 without filters: its
+    // row filters admit every tag), and always a per-query filter (the row-filtered scan is a mode of the tag-filtered one)
+    std::vector<uint64_t> tags, values, qtags, qvalues;
+    if (g.filters && host_row_words(ix, false, &tags)) return -1;
+    if (g.windows && host_row_words(ix, true, &values)) return -1;
     const RowAdmit all_rows;  // masked-out queries get the filter that admits no row (stage_row_block)
     const uint32_t QB = (uint32_t)std::min<size_t>(C.size(), SEARCH_ROWS_BLOCK);
     const std::vector<uint32_t> floor_thr(QB, nk::ord_bits(ix->key_floor()));
     RangeBlock block{path, 0, floor_thr.data()};
-    block.filtered = ix->mask_on || g.filters;
+    block.filtered = ix->mask_on || g.filters || g.windows;
     block.reverse = true;
-    block.row_filters = g.filters != nullptr;
+    block.row_filters = g.filters || g.windows;
+    block.row_windows = g.windows != nullptr;
     RangeShards on{live};
     std::vector<uint64_t> keys, per_query;
     for (size_t b = 0; b < C.size(); b += QB) {
         const uint32_t nb = block.Q = (uint32_t)std::min<size_t>(QB, C.size() - b);
         StageQueries stage_rows;
         if (stage_row_block(ix, live, C.data() + b, nb, block.filtered ? &all_rows : nullptr, &stage_rows)) return -1;
-        if (g.filters) {
-            qtags.resize(nb);
-            for (uint32_t q = 0; q < nb; ++q) qtags[q] = tags[C[b + q]];
+        if (block.row_filters) {
+            qtags.assign(nb, 0ull);
+            if (g.filters)
+                for (uint32_t q = 0; q < nb; ++q) qtags[q] = tags[C[b + q]];
+        }
+        if (g.windows) {
+            qvalues.resize(nb);
+            for (uint32_t q = 0; q < nb; ++q) qvalues[q] = values[C[b + q]];
         }
         const StageQueries stage = [&](NkShard &s) {
             if (stage_rows(s)) return -1;
-            if (!g.filters) return 0;
-            // the queries' tags: read by the scan before range_shard's first synchronisation
+            if (!block.row_filters) return 0;
+            // the queries' tags and value keys: read by the scan before range_shard's first synchronisation
             if (nk::ws_reserve((void **)&s.ws.qtags, &s.ws.qtags_bytes, (size_t)nb * 8)) return -1;
             NK_CUDA_OK(cudaMemcpyAsync(s.ws.qtags, qtags.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, s.stream));
+            ix->stats.bytes_h2d += (uint64_t)nb * 8;
+            if (!g.windows) return 0;
+            if (nk::ws_reserve((void **)&s.ws.qvalues, &s.ws.qvalues_bytes, (size_t)nb * 8)) return -1;
+            NK_CUDA_OK(cudaMemcpyAsync(s.ws.qvalues, qvalues.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, s.stream));
             ix->stats.bytes_h2d += (uint64_t)nb * 8;
             return 0;
         };
@@ -2173,12 +2203,18 @@ static int graph_search_again(NkIndex *ix, GraphCall &g, const std::vector<NkSha
     std::vector<uint32_t> ri((size_t)std::min<size_t>(rows.size(), SEARCH_ROWS_BLOCK) * k), sub;
     std::vector<float> rs(ri.size());
     std::vector<NkFilter> rf;  // filters: the block's rows' own
+    std::vector<NkWindow> rw;  // windows: the block's rows' own
     auto search = [&](const uint32_t *ids, uint32_t nb) {
         SearchOpts opts{path};
         if (g.filters) {
             rf.resize(nb);
             for (uint32_t q = 0; q < nb; ++q) rf[q] = g.filters[ids[q]];
             opts.filters_host = rf.data();
+        }
+        if (g.windows) {
+            rw.resize(nb);
+            for (uint32_t q = 0; q < nb; ++q) rw[q] = g.windows[ids[q]];
+            opts.windows_host = rw.data();
         }
         return search_rows_locked(ix, live, ids, opts, nb, k, ri.data(), rs.data());
     };
@@ -2276,14 +2312,21 @@ static int knn_graph_remap_host(NkIndex *ix, const GraphCall &g, uint64_t *n_lis
 
 int nk_knn_graph_remap(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row, const uint32_t *graph_idx_in,
                        const float *graph_score_in, uint32_t *graph_idx_out, float *graph_score_out, uint64_t *n_lists_changed) {
-    return knn_graph_remap_host(ix, GraphCall{"nk_knn_graph_remap", k, n_old, src_of_row, nullptr, graph_idx_in, graph_score_in,
+    return knn_graph_remap_host(ix, GraphCall{"nk_knn_graph_remap", k, n_old, src_of_row, nullptr, nullptr, graph_idx_in, graph_score_in,
                                               graph_idx_out, graph_score_out, false}, n_lists_changed);
 }
 
 int nk_knn_graph_remap_filtered(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row, const NkFilter *filters_host,
                                 const uint32_t *graph_idx_in, const float *graph_score_in, uint32_t *graph_idx_out,
                                 float *graph_score_out, uint64_t *n_lists_changed) {
-    return knn_graph_remap_host(ix, GraphCall{"nk_knn_graph_remap_filtered", k, n_old, src_of_row, filters_host, graph_idx_in,
+    return knn_graph_remap_host(ix, GraphCall{"nk_knn_graph_remap_filtered", k, n_old, src_of_row, filters_host, nullptr, graph_idx_in,
+                                              graph_score_in, graph_idx_out, graph_score_out, false}, n_lists_changed);
+}
+
+int nk_knn_graph_remap_windowed(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *src_of_row, const NkFilter *filters_host,
+                                const NkWindow *windows_host, const uint32_t *graph_idx_in, const float *graph_score_in,
+                                uint32_t *graph_idx_out, float *graph_score_out, uint64_t *n_lists_changed) {
+    return knn_graph_remap_host(ix, GraphCall{"nk_knn_graph_remap_windowed", k, n_old, src_of_row, filters_host, windows_host, graph_idx_in,
                                               graph_score_in, graph_idx_out, graph_score_out, false}, n_lists_changed);
 }
 
@@ -2310,14 +2353,22 @@ static int knn_graph_update_host(NkIndex *ix, GraphCall g, const uint32_t *chang
 
 int nk_knn_graph_update(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
                         uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed) {
-    return knn_graph_update_host(ix, GraphCall{"nk_knn_graph_update", k, n_old, nullptr, nullptr, nullptr, nullptr, graph_idx, graph_score, true},
+    return knn_graph_update_host(ix, GraphCall{"nk_knn_graph_update", k, n_old, nullptr, nullptr, nullptr, nullptr, nullptr, graph_idx, graph_score,
+                                               true},
                                  changed_rows, n_changed, n_lists_changed);
 }
 
 int nk_knn_graph_update_filtered(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
                                  const NkFilter *filters_host, uint32_t *graph_idx, float *graph_score, uint64_t *n_lists_changed) {
-    return knn_graph_update_host(ix, GraphCall{"nk_knn_graph_update_filtered", k, n_old, nullptr, filters_host, nullptr, nullptr, graph_idx,
-                                               graph_score, true}, changed_rows, n_changed, n_lists_changed);
+    return knn_graph_update_host(ix, GraphCall{"nk_knn_graph_update_filtered", k, n_old, nullptr, filters_host, nullptr, nullptr, nullptr,
+                                               graph_idx, graph_score, true}, changed_rows, n_changed, n_lists_changed);
+}
+
+int nk_knn_graph_update_windowed(NkIndex *ix, uint32_t k, uint64_t n_old, const uint32_t *changed_rows, uint32_t n_changed,
+                                 const NkFilter *filters_host, const NkWindow *windows_host, uint32_t *graph_idx, float *graph_score,
+                                 uint64_t *n_lists_changed) {
+    return knn_graph_update_host(ix, GraphCall{"nk_knn_graph_update_windowed", k, n_old, nullptr, filters_host, windows_host, nullptr, nullptr,
+                                               graph_idx, graph_score, true}, changed_rows, n_changed, n_lists_changed);
 }
 
 static int single_shard(NkIndex *ix, NkShard **out) {

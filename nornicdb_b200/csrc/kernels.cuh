@@ -35,6 +35,8 @@ struct Workspace {
     float *row_thr = nullptr;     size_t row_thr_bytes = 0;    // nk_knn_graph_update: per-row thresholds [n], then keep-mask words
     NkFilter *row_filter = nullptr; size_t row_filter_bytes = 0;  // filtered graph update: each row's own filter [n]
     uint64_t *qtags = nullptr;    size_t qtags_bytes = 0;      // ... and the tags of the reverse scan's queries [Q]
+    NkWindow *row_window = nullptr; size_t row_window_bytes = 0;  // windowed graph update: each row's own window [n]
+    uint64_t *qvalues = nullptr;  size_t qvalues_bytes = 0;    // ... and the value keys of the reverse scan's queries [Q]
     NkWindow *qwindow = nullptr;  size_t qwindow_bytes = 0;    // staged per-query value windows (host API, next to the filters)
     // cached TMA descriptors (tc_cached_map): re-encoded only when the base pointer or shape changes
     struct MapSlot {
@@ -84,20 +86,24 @@ struct RowImage {
 //   RANGE_WINDOW            ... with per-query value windows on top of the tag filters
 //   REVERSE, REVERSE_TAGS   the graph update's reverse scan: a range scan whose pairs must also reach their row's threshold (row_thr)
 //   REVERSE_RFILT           ... of a filtered graph: the row's own filter (row_filter) must also admit the query's tag (qtags)
+//   REVERSE_RWINDOW         ... of a windowed graph: the row's own window (row_window) must also admit the query's value key
+//                           (qvalues); a row-filter mode too (the row filters of a graph without filters admit every tag)
 //   DUMP                    tests only (scan_filter_dump): a kNN filter pass that also writes every pair's estimate and bound
-// The *_TAGS and *_WINDOW modes and REVERSE_RFILT apply per-query tag filters (row_tags, qfilter): a pair takes part only if
-// the query admits the row's tag.  The window modes also apply per-query value windows (row_values, qwindow): a pair takes
-// part only if the row's value key lies in the query's window.  The range modes (RANGE .. REVERSE_RFILT) and the reverse
-// modes (REVERSE ..) are contiguous.
-enum class ScanMode { KNN, KNN_TAGS, KNN_WINDOW, RANGE, RANGE_TAGS, RANGE_WINDOW, REVERSE, REVERSE_TAGS, REVERSE_RFILT, DUMP };
+// The *_TAGS and *_WINDOW modes and the row-filter modes apply per-query tag filters (row_tags, qfilter): a pair takes part
+// only if the query admits the row's tag.  The window modes also apply per-query value windows (row_values, qwindow): a pair
+// takes part only if the row's value key lies in the query's window.  The range modes (RANGE .. REVERSE_RWINDOW) and the reverse
+// modes (REVERSE ..) are contiguous.  The queries' own windows play no part in a reverse scan: mode_window excludes
+// REVERSE_RWINDOW.
+enum class ScanMode { KNN, KNN_TAGS, KNN_WINDOW, RANGE, RANGE_TAGS, RANGE_WINDOW, REVERSE, REVERSE_TAGS, REVERSE_RFILT, REVERSE_RWINDOW, DUMP };
 __host__ __device__ constexpr bool mode_window(ScanMode m) { return m == ScanMode::KNN_WINDOW || m == ScanMode::RANGE_WINDOW; }
 __host__ __device__ constexpr bool mode_tags(ScanMode m) {
     return m == ScanMode::KNN_TAGS || m == ScanMode::RANGE_TAGS || m == ScanMode::REVERSE_TAGS || m == ScanMode::REVERSE_RFILT ||
-           mode_window(m);
+           m == ScanMode::REVERSE_RWINDOW || mode_window(m);
 }
-__host__ __device__ constexpr bool mode_range(ScanMode m) { return m >= ScanMode::RANGE && m <= ScanMode::REVERSE_RFILT; }
-__host__ __device__ constexpr bool mode_row_thr(ScanMode m) { return m >= ScanMode::REVERSE && m <= ScanMode::REVERSE_RFILT; }
-__host__ __device__ constexpr bool mode_row_filter(ScanMode m) { return m == ScanMode::REVERSE_RFILT; }
+__host__ __device__ constexpr bool mode_range(ScanMode m) { return m >= ScanMode::RANGE && m <= ScanMode::REVERSE_RWINDOW; }
+__host__ __device__ constexpr bool mode_row_thr(ScanMode m) { return m >= ScanMode::REVERSE && m <= ScanMode::REVERSE_RWINDOW; }
+__host__ __device__ constexpr bool mode_row_filter(ScanMode m) { return m == ScanMode::REVERSE_RFILT || m == ScanMode::REVERSE_RWINDOW; }
+__host__ __device__ constexpr bool mode_row_window(ScanMode m) { return m == ScanMode::REVERSE_RWINDOW; }
 __host__ __device__ constexpr bool mode_dump(ScanMode m) { return m == ScanMode::DUMP; }
 
 struct ScanArgs {
@@ -140,10 +146,14 @@ struct ScanArgs {
     // the reverse modes (mode_row_thr): key-space threshold per local row [n]; a (row, query) pair is listed only if it
     // reaches both the query's threshold and the row's
     const float *row_thr = nullptr;
-    // REVERSE_RFILT: row_filter [n] (local rows) and qtags [Q]; a (row, query) pair is also listed only if
-    // tag_admits(qtags[q], row_filter + row), the mirror image of row_tags / qfilter
+    // the row-filter modes (mode_row_filter): row_filter [n] (local rows) and qtags [Q]; a (row, query) pair is also listed only
+    // if tag_admits(qtags[q], row_filter + row), the mirror image of row_tags / qfilter
     const NkFilter *row_filter = nullptr;
     const uint64_t *qtags = nullptr;
+    // REVERSE_RWINDOW: row_window [n] (local rows) and qvalues [Q]; a (row, query) pair is also listed only if
+    // window_admits(qvalues[q], row_window + row), the mirror image of row_values / qwindow
+    const NkWindow *row_window = nullptr;
+    const uint64_t *qvalues = nullptr;
     // the window modes (mode_window): value key per local row, row_values [n], and window per query, qwindow [Q]; a (row,
     // query) pair takes part only if window_admits(row_values[row], qwindow + q) (and the tag filter admits it)
     const uint64_t *row_values = nullptr;

@@ -53,7 +53,8 @@ int fatal_overflow(int flag, int *flags, cudaStream_t stream) {
 int ScanArgs::check(bool range, bool cuda_cores) const {
     if (!mode_dump(mode) && mode_range(mode) == range && !(cuda_cores && mode_row_thr(mode)) && mode_tags(mode) == (qfilter != nullptr) &&
         mode_row_thr(mode) == (row_thr != nullptr) && mode_row_filter(mode) == (row_filter != nullptr) && mode_row_filter(mode) == (qtags != nullptr) &&
-        mode_window(mode) == (qwindow != nullptr) && mode_window(mode) == (row_values != nullptr))
+        mode_window(mode) == (qwindow != nullptr) && mode_window(mode) == (row_values != nullptr) &&
+        mode_row_window(mode) == (row_window != nullptr) && mode_row_window(mode) == (qvalues != nullptr))
         return 0;
     set_error("internal: scan mode %d does not fit this %s scan (%s) or its pointers", (int)mode, range ? "range" : "kNN", cuda_cores ? "CUDA cores" : "tensor");
     return -1;
@@ -86,7 +87,7 @@ int ws_reserve(void **p, size_t *cur, size_t need) {
 }
 
 int Workspace::release() {
-    void *ptrs[] = {cand, partial, keys, keys2, below, queries, qfilter, out_idx, out_score, qaux, rownorm, flags, sub_rows, sub_gather, scratch, row_thr, row_filter, qtags, qwindow};
+    void *ptrs[] = {cand, partial, keys, keys2, below, queries, qfilter, out_idx, out_score, qaux, rownorm, flags, sub_rows, sub_gather, scratch, row_thr, row_filter, qtags, qwindow, row_window, qvalues};
     for (void *q : ptrs)
         if (q) cudaFree(q);
     *this = Workspace();

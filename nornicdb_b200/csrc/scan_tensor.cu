@@ -307,7 +307,8 @@ template <bool FILTER> struct Tf32Est {
     __device__ __forceinline__ float bound(uint32_t qi) const { return bnd * qn[qi]; }
 };
 
-// M: the scan mode (kernels.cuh).  REVERSE_RFILT stages the launch's query tags in shared memory past Shared.
+// M: the scan mode (kernels.cuh).  The row-filter modes stage the launch's query tags (REVERSE_RWINDOW: and value keys) in
+// shared memory past Shared.
 template <int NT, int QT, ScanMode M>
 __global__ void __launch_bounds__(tc::THREADS, 1)
 knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_qhi,
@@ -348,8 +349,11 @@ knn_scan_tc_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_co
         sh.cnt[tid] = 0;
         sh.qn[tid] = (FILTER && p.qnorm) ? p.qnorm[qpad_off + tid] : 1.0f;
     }
-    uint64_t *qtag = reinterpret_cast<uint64_t *>(smem_raw + (size_t)C::RING_BYTES + sizeof(Shared));  // REVERSE_RFILT only
+    // row-filter modes only: the query tags [QT], then (REVERSE_RWINDOW) the query value keys [QT]
+    uint64_t *qtag = reinterpret_cast<uint64_t *>(smem_raw + (size_t)C::RING_BYTES + sizeof(Shared));
     if (mode_row_filter(M) && tid < QT) qtag[tid] = (uint32_t)tid < nq ? p.qtags[q0 + tid] : 0ull;
+    if constexpr (mode_row_window(M))
+        if (tid < QT) qtag[QT + tid] = (uint32_t)tid < nq ? p.qvalues[q0 + tid] : 0ull;
     __syncthreads();
     const bool flood = !(FILTER && p.presampled);  // first two tiles: every (row, query) pair is placed directly
     uint64_t *my_cand = p.cand + (size_t)blockIdx.x * QT * P;
@@ -887,7 +891,7 @@ tc::Params pass_params(const ScanArgs &a, Workspace &ws, const tc::PassArgs &t) 
     p.gtau = reinterpret_cast<uint32_t *>(ws.keys2); p.gcount = reinterpret_cast<int *>(ws.keys2) + (t.Qpad + tc::QT_BIG);
     p.presampled = t.presampled; p.min_score = a.min_score;
     p.row_tags = a.row_tags; p.qfilter = a.qfilter; p.row_thr = a.row_thr; p.row_filter = a.row_filter; p.qtags = a.qtags;
-    p.row_values = a.row_values; p.qwindow = a.qwindow;
+    p.row_values = a.row_values; p.qwindow = a.qwindow; p.row_window = a.row_window; p.qvalues = a.qvalues;
     p.dump_est = t.dump_est; p.dump_bnd = t.dump_bnd; p.dump_ld = t.dump_ld;
     return p;
 }
@@ -948,7 +952,8 @@ static int launch_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspace &ws,
     const CUtensorMap *map_qhi = tc_cached_map(ws, QT == 64 ? 1 : 2, t.qhi, t.Qpad, a.dim, 4, (uint32_t)BK, QT, (uint64_t)a.dim * 4);
     const CUtensorMap *map_qlo = NT == 3 ? tc_cached_map(ws, 3, t.qlo, t.Qpad, a.dim, 4, (uint32_t)BK, QT, (uint64_t)a.dim * 4) : map_qhi;
     if (!map_rows || !map_qhi || !map_qlo) return -1;
-    const size_t smem = (size_t)Cfg<NT, QT>::RING_BYTES + sizeof(Shared) + (mode_row_filter(M) ? QT * sizeof(uint64_t) : 0) + 1024;
+    const size_t smem = (size_t)Cfg<NT, QT>::RING_BYTES + sizeof(Shared) + (mode_row_filter(M) ? QT * sizeof(uint64_t) : 0) +
+                        (mode_row_window(M) ? QT * sizeof(uint64_t) : 0) + 1024;
     if (smem > di.max_smem_optin) {
         set_error("tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;

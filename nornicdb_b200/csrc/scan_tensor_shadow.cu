@@ -226,7 +226,8 @@ struct Bf16Est {
 
 // OP: the operand type, bf16 (BF16 shadow, bf16 corpora), fp16 (an fp16 corpus scanned in place) or int8 (the int8 image of
 // an fp32 shard).  M: the scan mode (kernels.cuh).  Tag filters are read through the read-only cache (shared memory is spent
-// on the rings); REVERSE_RFILT stages the launch's query tags in shared memory past Shared.
+// on the rings); the row-filter modes stage the launch's query tags (REVERSE_RWINDOW: and value keys) in shared memory past
+// Shared.
 template <int QT, ptx::Opnd OP, ScanMode M>
 __global__ void __launch_bounds__(sb::NTHREADS, 1)
 knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __grid_constant__ CUtensorMap map_q, tc::Params p) {
@@ -267,8 +268,11 @@ knn_scan_shadow_kernel(const __grid_constant__ CUtensorMap map_rows, const __gri
         sh.qb[tid] = p.qb[qpad_off + tid];
         if (S8) sh.qs[tid] = p.qscale[qpad_off + tid];
     }
-    uint64_t *qtag = reinterpret_cast<uint64_t *>(smem_raw + (size_t)C::RING_BYTES + sizeof(Shared));  // REVERSE_RFILT only
+    // row-filter modes only: the query tags [QT], then (REVERSE_RWINDOW) the query value keys [QT]
+    uint64_t *qtag = reinterpret_cast<uint64_t *>(smem_raw + (size_t)C::RING_BYTES + sizeof(Shared));
     if (mode_row_filter(M) && tid < QT) qtag[tid] = (uint32_t)tid < nq ? p.qtags[q0 + tid] : 0ull;
+    if constexpr (mode_row_window(M))
+        if (tid < QT) qtag[QT + tid] = (uint32_t)tid < nq ? p.qvalues[q0 + tid] : 0ull;
     __syncthreads();
     const bool flood = !p.presampled;  // first two tiles: every (row, query) pair is placed directly
     if (prof && tid == 0) g_sb_prof[blockIdx.x][1] = globaltimer_ns();
@@ -655,7 +659,8 @@ static int launch_shadow_pass_t(const DeviceInfo &di, const ScanArgs &a, Workspa
     const CUtensorMap *map_q = tc_cached_map(ws, QT == 64 ? 5 : 6, sp.qbf16, sp.Qpad, sp.dimpad, esz, kcols, QT, (uint64_t)sp.dimpad * esz,
                                              a.dtype);  // rows past Qpad: zero
     if (!map_rows || !map_q) return -1;
-    const size_t smem = (size_t)Cfg<QT>::RING_BYTES + sizeof(Shared) + (mode_row_filter(M) ? QT * sizeof(uint64_t) : 0) + 1024;
+    const size_t smem = (size_t)Cfg<QT>::RING_BYTES + sizeof(Shared) + (mode_row_filter(M) ? QT * sizeof(uint64_t) : 0) +
+                        (mode_row_window(M) ? QT * sizeof(uint64_t) : 0) + 1024;
     if (smem > di.max_smem_optin) {
         set_error("shadow tensor path needs %zu B shared memory (> %zu)", smem, di.max_smem_optin);
         return -1;

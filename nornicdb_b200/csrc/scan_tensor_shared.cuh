@@ -73,10 +73,12 @@ struct Params {
     const uint64_t *row_tags; // tag modes only: tag word per local row
     const NkFilter *qfilter;  // tag modes only: filter per query [Q], indexed like gtau (absolute query index)
     const float *row_thr;     // reverse modes only: key-space threshold per local row (the reverse scan of nk_knn_graph_update)
-    const NkFilter *row_filter;  // REVERSE_RFILT only: the filter of each local row's own k-NN list (filtered graphs)
-    const uint64_t *qtags;    // REVERSE_RFILT only: tag word per query [Q], indexed like gtau; staged in shared memory per CTA
+    const NkFilter *row_filter;  // row-filter modes only: the filter of each local row's own k-NN list (filtered graphs)
+    const uint64_t *qtags;    // row-filter modes only: tag word per query [Q], indexed like gtau; staged in shared memory per CTA
     const uint64_t *row_values;  // window modes only: value key per local row
     const NkWindow *qwindow;     // window modes only: window per query [Q] (absolute query index; no padding, never read past Q)
+    const NkWindow *row_window;  // REVERSE_RWINDOW only: the window of each local row's own k-NN list (windowed graphs)
+    const uint64_t *qvalues;     // REVERSE_RWINDOW only: value key per query [Q]; staged in shared memory per CTA past the tags
 };
 
 // What one scan launch covers: queries [q0, q0+nq) in `qgroups` query groups over a `grid`-CTA launch.  Both kernels'
@@ -206,7 +208,9 @@ template <int QT> __device__ __forceinline__ float frag_value(const float (&acc)
 // query's window, loaded and tested after the tag, and only for the columns the tag test kept (so only queries < nq: the
 // window array has Q entries, no padding).  The window's query index is summed in 32 bits before the one pointer add: the
 // 16-bit / int8 QT=128 instantiations then keep their register budget without spills.  Reverse modes: a pair must also reach the ROW's threshold rthr[ri] and
-// (REVERSE_RFILT) be admitted by the row's own filter (qtag: the CTA's query tags), loaded only once both thresholds hold.
+// (row-filter modes) be admitted by the row's own filter (qtag: the CTA's query tags), loaded only once both thresholds hold;
+// REVERSE_RWINDOW: and by the row's own window (qtag[QT + qi]: the CTA's query value keys), loaded only once a column passed the
+// filter.  The range modes have no later stage that could drop a pair the window refuses: this is where it is enforced.
 template <int QT, int CAP, bool BOUNDED, ScanMode M, int NR, class Est>
 __device__ __forceinline__ void keep_fragment_rows(const Params &p, const Est (&est)[NR], const float (&acc)[2][QT / 2], uint32_t fr0,
                                                    uint32_t alive, uint32_t row0, uint32_t rbase, bool flood, uint32_t it, uint32_t cbase,
@@ -262,6 +266,19 @@ __device__ __forceinline__ void keep_fragment_rows(const Params &p, const Est (&
                         const uint32_t c = (uint32_t)__ffs((int)chk) - 1u;
                         chk &= chk - 1u;
                         if (!window_admits(val, p.qwindow + (q0 + cbase + 8 * (c >> 1) + (c & 1)))) admit &= ~(1u << c);
+                    }
+                }
+            }
+            if constexpr (mode_row_window(M)) {
+                if (admit) {  // only the columns the tag loop admitted (queries < nq): the row's own window against their keys
+                    const NkWindow *rw = p.row_window + row;
+                    const uint64_t lo = __ldg(&rw->lo), hi = __ldg(&rw->hi);
+                    uint32_t chk = admit;
+#pragma unroll 1
+                    while (chk) {
+                        const uint32_t c = (uint32_t)__ffs((int)chk) - 1u;
+                        chk &= chk - 1u;
+                        if (!window_admits(qtag[QT + cbase + 8 * (c >> 1) + (c & 1)], lo, hi)) admit &= ~(1u << c);
                     }
                 }
             }
@@ -339,6 +356,19 @@ __device__ __forceinline__ void keep_fragment_rows(const Params &p, const Est (&
                 const uint32_t c = (uint32_t)__ffs((int)chk) - 1u;
                 chk &= chk - 1u;
                 if (!tag_admits(qtag[cbase + 8 * (c >> 1) + (c & 1)], all_of, none_of, any_of)) ps &= ~(1u << c);
+            }
+            if constexpr (mode_row_window(M)) {
+                if (ps) {
+                    const NkWindow *rw = p.row_window + row;
+                    const uint64_t lo = __ldg(&rw->lo), hi = __ldg(&rw->hi);
+                    chk = ps;
+#pragma unroll 1
+                    while (chk) {
+                        const uint32_t c = (uint32_t)__ffs((int)chk) - 1u;
+                        chk &= chk - 1u;
+                        if (!window_admits(qtag[QT + cbase + 8 * (c >> 1) + (c & 1)], lo, hi)) ps &= ~(1u << c);
+                    }
+                }
             }
         }
 #pragma unroll 1

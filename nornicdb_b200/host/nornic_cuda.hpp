@@ -230,7 +230,8 @@ public:
         } else {
             check(nk_index_append(ix_, embedding.data(), 1));
             if (graphK_) graphSrc_.push_back(NK_ROW_NEW);
-            tags_.push_back(0);  // nk_index_append: tag 0
+            tags_.push_back(0);    // nk_index_append: tag 0
+            values_.push_back(0);  // ... and value key 0
             idToIndex_[nodeID] = nodeIDs_.size();
             nodeIDs_.push_back(nodeID);
         }
@@ -250,8 +251,10 @@ public:
             graphSrc_[idx] = graphSrc_[last];
             graphSrc_.pop_back();
         }
-        tags_[idx] = tags_[last];  // the tag moves with its row
+        tags_[idx] = tags_[last];  // the tag and the value key move with their row
         tags_.pop_back();
+        values_[idx] = values_[last];
+        values_.pop_back();
         if (idx != last) {
             nodeIDs_[idx] = nodeIDs_[last];
             idToIndex_[nodeIDs_[idx]] = idx;
@@ -315,9 +318,14 @@ public:
     // Per-query value windows: value keys of rows [firstRow, firstRow + keys.size()) (row order of Add; 0 = no value, keys
     // encoded by the caller so that key order is number order), then a batch whose queries each carry an NkWindow {lo, hi}
     // (inclusive, unsigned) on top of an optional tag filter (filters empty = none, else one per query), in one corpus pass.
+    // A row whose value key changes is new contents to SimilarGraph's graph.
     void SetRowValues(uint64_t firstRow, const std::vector<uint64_t> &keys) {
         std::lock_guard<std::mutex> lk(mu_);
         check(nk_index_set_row_values(ix_, firstRow, keys.data(), keys.size()));
+        for (size_t i = 0; i < keys.size(); ++i) {
+            if (graphK_ && values_[firstRow + i] != keys[i]) graphSrc_[firstRow + i] = NK_ROW_NEW;
+            values_[firstRow + i] = keys[i];
+        }
     }
     std::vector<std::vector<SearchResult>> SearchBatchWindowed(const std::vector<float> &queries, const std::vector<NkFilter> &filters,
                                                                const std::vector<NkWindow> &windows, uint32_t Q, int k) {
@@ -456,34 +464,41 @@ public:
     // the last call rebuild it with nk_search_rows.  Lists in row order (the order of insertion, as swapped by Remove).  The
     // graph is built and updated on the 16-bit filter path (the TF32 filter if the shape has no 16-bit image), which the
     // update requires; other searches keep the automatic choice.  filters empty = none, else one tag filter per row (row
-    // order): each node's list holds only nodes its filter admits, e.g. one graph per collection of the shared index.  A node
-    // whose filter or tag (SetRowTags) changed since the last call is handed to the update as new contents.
-    std::vector<std::vector<SearchResult>> SimilarGraph(int k, const std::vector<NkFilter> &filters = {}) {
+    // order): each node's list holds only nodes its filter admits, e.g. one graph per collection of the shared index.  windows
+    // empty = none, else one value window per row (row order): each node's list holds only nodes whose value key (SetRowValues)
+    // its window admits, a time-local graph.  A node whose filter, window, tag (SetRowTags) or value key (SetRowValues) changed
+    // since the last call is handed to the update as new contents.
+    std::vector<std::vector<SearchResult>> SimilarGraph(int k, const std::vector<NkFilter> &filters = {}, const std::vector<NkWindow> &windows = {}) {
         std::lock_guard<std::mutex> lk(mu_);
         const uint64_t n = nodeIDs_.size();
         if (!filters.empty() && filters.size() != n) throw std::invalid_argument("gpu: one filter per node");
+        if (!windows.empty() && windows.size() != n) throw std::invalid_argument("gpu: one window per node");
         if (n == 0 || k <= 0) return std::vector<std::vector<SearchResult>>(n);
         auto filter_of = [&](uint64_t r) { return filters.empty() ? NkFilter{0, 0, 0} : filters[r]; };
         auto same_filter = [](const NkFilter &a, const NkFilter &b) { return a.all_of == b.all_of && a.none_of == b.none_of && a.any_of == b.any_of; };
+        auto window_of = [&](uint64_t r) { return windows.empty() ? NkWindow{0, ~0ull} : windows[r]; };  // none: every key
+        auto same_window = [](const NkWindow &a, const NkWindow &b) { return a.lo == b.lo && a.hi == b.hi; };
         const NkFilter *fp = filters.empty() ? nullptr : filters.data();
+        const NkWindow *wp = windows.empty() ? nullptr : windows.data();
         int got = -1;
         std::vector<uint32_t> gi(n * k, 0xffffffffu);
         std::vector<float> gs(n * k, 0.0f);
-        std::vector<uint32_t> src;  // graphSrc_ with the rows whose filter changed as new contents
+        std::vector<uint32_t> src;  // graphSrc_ with the rows whose filter or window changed as new contents
         if (graphK_ == (uint32_t)k) {
             src = graphSrc_;
             for (uint64_t f = 0; f < n; ++f)
-                if (src[f] != NK_ROW_NEW && !same_filter(filter_of(f), graphFilter_[src[f]])) src[f] = NK_ROW_NEW;
+                if (src[f] != NK_ROW_NEW && (!same_filter(filter_of(f), graphFilter_[src[f]]) || !same_window(window_of(f), graphWindow_[src[f]])))
+                    src[f] = NK_ROW_NEW;
         }
         for (int path : {NK_PATH_TENSOR_SHADOW, NK_PATH_TENSOR_FILTER}) {
             check(nk_index_set_path(ix_, path));
             if (graphK_ == (uint32_t)k) {
-                got = nk_knn_graph_remap_filtered(ix_, (uint32_t)k, graphRows_, src.data(), fp, graphIdx_.data(), graphScore_.data(), gi.data(),
+                got = nk_knn_graph_remap_windowed(ix_, (uint32_t)k, graphRows_, src.data(), fp, wp, graphIdx_.data(), graphScore_.data(), gi.data(),
                                                   gs.data(), nullptr);
             } else {
                 std::vector<uint32_t> rows(n);
                 for (uint64_t r = 0; r < n; ++r) rows[r] = (uint32_t)r;
-                got = nk_search_rows_filtered(ix_, rows.data(), fp, (uint32_t)n, (uint32_t)k, gi.data(), gs.data());
+                got = nk_search_rows_windowed(ix_, rows.data(), fp, wp, (uint32_t)n, (uint32_t)k, gi.data(), gs.data());
                 if (got >= 0) ++graphRebuilds_;
             }
             if (got >= 0) break;
@@ -496,7 +511,8 @@ public:
         graphScore_.swap(gs);
         graphSrc_.resize(n);
         graphFilter_.resize(n);
-        for (uint64_t r = 0; r < n; ++r) { graphSrc_[r] = (uint32_t)r; graphFilter_[r] = filter_of(r); }
+        graphWindow_.resize(n);
+        for (uint64_t r = 0; r < n; ++r) { graphSrc_[r] = (uint32_t)r; graphFilter_[r] = filter_of(r); graphWindow_[r] = window_of(r); }
         std::vector<std::vector<SearchResult>> out(n);
         for (uint64_t r = 0; r < n; ++r)
             for (int i = 0; i < got; ++i) {
@@ -529,6 +545,7 @@ public:
     bool IsGPUSynced() const { return gpuSynced_; }
     uint64_t GraphRebuilds() const { return graphRebuilds_; }  // SimilarGraph calls that searched every row
     std::vector<uint64_t> RowTags() { std::lock_guard<std::mutex> lk(mu_); return tags_; }  // the tag of each row, row order
+    std::vector<uint64_t> RowValues() { std::lock_guard<std::mutex> lk(mu_); return values_; }  // the value key of each row, row order
     int Count() const { return (int)nodeIDs_.size(); }                                   // gpu.go:2225
     bool Has(const std::string &id) const { return idToIndex_.count(id) != 0; }          // gpu.go:2279
     bool Get(const std::string &id, std::vector<float> *out) {                           // gpu.go:2287
@@ -569,7 +586,8 @@ public:
         check(nk_index_upload(ix_, data.data() + off, count));  // the blob streams straight into device memory
         gpuSynced_ = false;
         graphK_ = 0;
-        tags_.assign(count, 0);  // nk_index_upload: every tag 0
+        tags_.assign(count, 0);    // nk_index_upload: every tag 0
+        values_.assign(count, 0);  // ... and every value key 0
         nodeIDs_ = ids;
         idToIndex_.clear();
         for (uint32_t i = 0; i < count; ++i) idToIndex_[nodeIDs_[i]] = i;
@@ -590,7 +608,9 @@ private:
     std::vector<float> graphScore_;
     std::vector<uint32_t> graphSrc_;
     std::vector<NkFilter> graphFilter_;  // the filter of each graph row's list when it was made ({0,0,0}: none)
+    std::vector<NkWindow> graphWindow_;  // ... and its window ({0, ~0}: none)
     std::vector<uint64_t> tags_;         // the tag of each row, as on the device
+    std::vector<uint64_t> values_;       // the value key of each row, as on the device
     uint64_t graphRebuilds_ = 0;
     std::mutex mu_;
 };

@@ -289,8 +289,18 @@ class KnnIndex:
             raise KnnError(f"{what}: filters must be [{n} x 3] (one per current row), not {list(f.shape)}")
         return f
 
+    def _graph_windows(self, windows, what: str):
+        """windows of a graph call: None, or one [n x 2] uint64 (lo, hi) window per current row"""
+        if windows is None:
+            return None
+        n = len(self)
+        w = np.ascontiguousarray(np.asarray(windows, dtype=np.uint64))
+        if w.shape != (n, 2):
+            raise KnnError(f"{what}: windows must be [{n} x 2] (one per current row), not {list(w.shape)}")
+        return w
+
     def update_knn_graph(self, idx, score, n_old: int, changed=None, k: Optional[int] = None,
-                         filters=None) -> Tuple[np.ndarray, np.ndarray, int]:
+                         filters=None, windows=None) -> Tuple[np.ndarray, np.ndarray, int]:
         """Bring the k-NN graph search_rows(range(n_old), k) returned up to date after rows were appended (rows n_old ..
         len(self) - 1) and old rows rewritten (`changed`: their ids, repeats allowed) -> (idx, score, lists_changed): what
         search_rows(every row, k) returns now, k' = min(k, admissible rows) columns, and how many old rows' lists changed.
@@ -300,7 +310,11 @@ class KnnIndex:
         remove_swap, use remap_knn_graph (nk_knn_graph_update).
         filters: None, or one tag filter per current row ([len(self) x 3] uint64): the graph of search_rows(every row, k,
         filters), each list bounded by its row's own filter.  An old row whose tag or filter changed since the graph was built
-        must be listed in `changed`, like a rewritten row (nk_knn_graph_update_filtered)."""
+        must be listed in `changed`, like a rewritten row (nk_knn_graph_update_filtered).
+        windows: None, or one value window per current row ([len(self) x 2] uint64, as band_windows returns them): the graph
+        of search_rows(every row, k, filters, windows), a time-local graph.  An old row whose value key or window changed
+        since the graph was built must be listed in `changed`, like a retag; a band window moves with its row's key, so
+        re-valuing a row is such a change (nk_knn_graph_update_windowed)."""
         idx = np.asarray(idx, dtype=np.uint32)
         score = np.asarray(score, dtype=np.float32)
         n_old = int(n_old)
@@ -317,6 +331,7 @@ class KnnIndex:
             raise KnnError("update_knn_graph: changed row ids must be >= 0")
         ch = np.ascontiguousarray(ch.astype(np.uint32))
         f = self._graph_filters(filters, "update_knn_graph")
+        w = self._graph_windows(windows, "update_knn_graph")
         if k <= 0 or n == 0:
             return np.empty((n, 0), np.uint32), np.empty((n, 0), np.float32), 0
         gi = np.full((n, k), 0xFFFFFFFF, dtype=np.uint32)
@@ -325,7 +340,12 @@ class KnnIndex:
         gs[:n_old, :idx.shape[1]] = score
         changed_lists = C.c_uint64(0)
         chp = ch.ctypes.data_as(C.c_void_p) if ch.size else None
-        if f is None:
+        if w is not None:
+            ke = _check(self.lib.nk_knn_graph_update_windowed(self.ptr, k, n_old, chp, int(ch.size), None if f is None else f.ctypes.data_as(C.c_void_p),
+                                                              w.ctypes.data_as(C.c_void_p), gi.ctypes.data_as(C.c_void_p),
+                                                              gs.ctypes.data_as(C.c_void_p), C.byref(changed_lists)),
+                        "nk_knn_graph_update_windowed")
+        elif f is None:
             ke = _check(self.lib.nk_knn_graph_update(self.ptr, k, n_old, chp, int(ch.size), gi.ctypes.data_as(C.c_void_p),
                                                      gs.ctypes.data_as(C.c_void_p), C.byref(changed_lists)), "nk_knn_graph_update")
         else:
@@ -335,7 +355,7 @@ class KnnIndex:
         return gi[:, :ke], gs[:, :ke], int(changed_lists.value)
 
     def remap_knn_graph(self, idx, score, n_old: int, src, k: Optional[int] = None,
-                        filters=None) -> Tuple[np.ndarray, np.ndarray, int]:
+                        filters=None, windows=None) -> Tuple[np.ndarray, np.ndarray, int]:
         """Bring the k-NN graph search_rows(range(n_old), k) returned up to date after any mix of append, update_row and
         remove_swap -> (idx, score, lists_changed): what search_rows(every row, k) returns now, k' = min(k, admissible rows)
         columns, and how many rows that hold their old contents at their old id got a different list.  src: a GraphRowMap
@@ -344,7 +364,10 @@ class KnnIndex:
         (nk_knn_graph_remap).
         filters: None, or one tag filter per current row ([len(self) x 3] uint64, in current row order): the graph of
         search_rows(every row, k, filters).  A row whose tag or filter changed since the graph was built must be ROW_NEW in
-        src: record it with GraphRowMap.update_row, like a rewrite (nk_knn_graph_remap_filtered)."""
+        src: record it with GraphRowMap.update_row, like a rewrite (nk_knn_graph_remap_filtered).
+        windows: None, or one value window per current row ([len(self) x 2] uint64, in current row order): the graph of
+        search_rows(every row, k, filters, windows).  A row whose value key or window changed since the graph was built must
+        be ROW_NEW in src, like a retag: record it with GraphRowMap.update_row (nk_knn_graph_remap_windowed)."""
         idx = np.asarray(idx, dtype=np.uint32)
         score = np.asarray(score, dtype=np.float32)
         n_old = int(n_old)
@@ -361,6 +384,7 @@ class KnnIndex:
             raise KnnError("remap_knn_graph: src_of_row entries must be old row ids or ROW_NEW")
         s = np.ascontiguousarray(s.astype(np.uint32))
         f = self._graph_filters(filters, "remap_knn_graph")
+        w = self._graph_windows(windows, "remap_knn_graph")
         if k <= 0 or n == 0:
             return np.empty((n, 0), np.uint32), np.empty((n, 0), np.float32), 0
         oi = np.full((n_old, k), 0xFFFFFFFF, dtype=np.uint32)
@@ -372,7 +396,11 @@ class KnnIndex:
         changed_lists = C.c_uint64(0)
         graph = (oi.ctypes.data_as(C.c_void_p), osc.ctypes.data_as(C.c_void_p), gi.ctypes.data_as(C.c_void_p),
                  gs.ctypes.data_as(C.c_void_p), C.byref(changed_lists))
-        if f is None:
+        if w is not None:
+            ke = _check(self.lib.nk_knn_graph_remap_windowed(self.ptr, k, n_old, s.ctypes.data_as(C.c_void_p),
+                                                             None if f is None else f.ctypes.data_as(C.c_void_p),
+                                                             w.ctypes.data_as(C.c_void_p), *graph), "nk_knn_graph_remap_windowed")
+        elif f is None:
             ke = _check(self.lib.nk_knn_graph_remap(self.ptr, k, n_old, s.ctypes.data_as(C.c_void_p), *graph), "nk_knn_graph_remap")
         else:
             ke = _check(self.lib.nk_knn_graph_remap_filtered(self.ptr, k, n_old, s.ctypes.data_as(C.c_void_p),
@@ -632,7 +660,8 @@ class GraphRowMap:
 
     def update_row(self, row: int) -> None:
         """The row's contents changed (update_row).  For a filtered graph, also call it for a row whose tag or filter
-        changed: the graph treats such a row as rewritten."""
+        changed, and for a windowed graph for a row whose value key or window changed: the graph treats such a row as
+        rewritten."""
         self._src[self._row(row)] = ROW_NEW
 
     def remove_swap(self, row: int) -> None:
