@@ -479,6 +479,45 @@ int nk_knn_graph_remap_windowed(NkIndex *ix, uint32_t k, uint64_t n_old, const u
                                 const uint32_t *graph_idx_in, const float *graph_score_in,
                                 uint32_t *graph_idx_out, float *graph_score_out, uint64_t *n_lists_changed);
 
+/* ---- Self-join kept current --------------------------------------------------------------------------------------------
+ * The pairs of the whole-index self-join incident to a set of rows: on a write, every pair the changed rows now form (the
+ * edges to create; the edges to delete are those touching the changed or removed rows, which the caller knows).
+ * rows_host [n]: distinct relative ids.  Take nk_search_pairs_windowed(first_row = 0, n_rows = nk_index_rows(ix), threshold,
+ * filter, window, max_gap) on the graph path, keep its pairs {i, j} with at least one end listed, and group them by that
+ * listed end (a pair with both ends listed goes under the lower one): listed row rows_host[r] owns [out_offsets[r],
+ * out_offsets[r+1]) of out_idx (global ids of the other ends) / out_score, out_offsets [n + 1].  The result equals that, bit
+ * for bit: each score is the join's, with the lower row of the pair as the query (under cosine the two orientations can
+ * round differently), and each list is in nk_search's order.  Size protocol: nk_search_pairs'.
+ * The call runs on the graph path (nk_knn_graph_update) whatever AUTO would pick: every score is warp_exact_score's, so it
+ * equals the join run with TENSOR_SHADOW or TENSOR_FILTER forced (AUTO may run small joins on the CUDA cores).  Each block of
+ * 1024 listed rows scans every shard whole: about n / 1024 full-index range scans.
+ * Returns 0, or -1 with nk_last_error, before any work, for: a repeated or out-of-range id, a NaN threshold, a null pointer
+ * with n > 0, the SIMT or 3xTF32 path forced, or a shape without a filter path.  Synchronous; holds the index lock.
+ * nk_search_pairs_rows is the _windowed call with window == NULL and max_gap == NK_NO_GAP. */
+int nk_search_pairs_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t n, float threshold, const NkFilter *filter, uint64_t capacity,
+                         uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total);
+int nk_search_pairs_rows_windowed(NkIndex *ix, const uint32_t *rows_host, uint32_t n, float threshold, const NkFilter *filter,
+                                  const NkWindow *window, uint64_t max_gap, uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx,
+                                  float *out_score, uint64_t *out_total);
+
+/* Brings a stored self-join up to date after any mix of append, update_row, remove_swap, retags and re-valued rows.
+ * src_of_row [N] as for nk_knn_graph_remap: NK_ROW_NEW marks a row appended, rewritten, retagged or re-valued since.
+ * old_offsets [n_old + 1] / old_idx / old_score: what nk_search_pairs_windowed over the whole index (rows [0, n_old)) returned
+ * with the same threshold, filter, window and max_gap.  out_offsets [N + 1] / out_idx / out_score: on return, bit for bit, what
+ * that call over the whole index returns now on the graph path, under nk_search_pairs' size protocol.  *n_dropped (nullable):
+ * old pairs with an end that is gone, moved or NK_ROW_NEW; *n_found (nullable): pairs incident to the new and moved rows.
+ * Old pairs with both ends kept at their id are carried; every other old pair is dropped (a moved row counts as new: its id
+ * decides the orientation and the tie order); nk_search_pairs_rows_windowed of the new and moved rows adds the rest; each
+ * owner's list is merged in key space.  The merge is host C++, O(pairs) time and memory.  This is the verification and
+ * convenience path: a database that keeps the pairs as edges calls nk_search_pairs_rows_windowed on each write.
+ * Preconditions (not checked): the metric and the score floor are unchanged, and every kept row has its mask bit, tag and
+ * value key.  Refused before any output is written: those of nk_search_pairs_rows, a src_of_row value >= n_old other than
+ * NK_ROW_NEW or repeated, an old entry that is not an old row above its owner, old_offsets not starting at 0 or decreasing. */
+int nk_pairs_remap(NkIndex *ix, float threshold, const NkFilter *filter, const NkWindow *window, uint64_t max_gap, uint64_t n_old,
+                   const uint32_t *src_of_row, const uint64_t *old_offsets, const uint32_t *old_idx, const float *old_score,
+                   uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total,
+                   uint64_t *n_dropped, uint64_t *n_found);
+
 /* Multi-process sharding (one rank per GPU): emit this shard's sorted candidate list as packed 64-bit
  * keys [Q x k] (order-preserving score bits << 32 | ~row index; larger key = better), to be exchanged
  * (e.g. ncclAllGather of Q*k*8 bytes per rank) and merged with nk_merge_keys_device.  k <= NK_MAX_K_TOTAL: one shard's

@@ -86,6 +86,9 @@ SIGNATURES = {
     "nk_search_rows_windowed": (_i, [_vp, _vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp]),
     "nk_search_pairs": (_i, [_vp, _u64, _u64, C.c_float, _vp, _u64, _vp, _vp, _vp, _vp]),
     "nk_search_pairs_windowed": (_i, [_vp, _u64, _u64, C.c_float, _vp, _vp, _u64, _u64, _vp, _vp, _vp, _vp]),
+    "nk_search_pairs_rows": (_i, [_vp, _vp, C.c_uint32, C.c_float, _vp, _u64, _vp, _vp, _vp, _vp]),
+    "nk_search_pairs_rows_windowed": (_i, [_vp, _vp, C.c_uint32, C.c_float, _vp, _vp, _u64, _u64, _vp, _vp, _vp, _vp]),
+    "nk_pairs_remap": (_i, [_vp, C.c_float, _vp, _vp, _u64, _u64, _vp, _vp, _vp, _vp, _u64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nk_knn_graph_update": (_i, [_vp, C.c_uint32, _u64, _vp, C.c_uint32, _vp, _vp, _vp]),
     "nk_knn_graph_remap": (_i, [_vp, C.c_uint32, _u64, _vp, _vp, _vp, _vp, _vp, _vp]),
     "nk_knn_graph_update_filtered": (_i, [_vp, C.c_uint32, _u64, _vp, C.c_uint32, _vp, _vp, _vp, _vp]),

@@ -1592,6 +1592,9 @@ struct RangeBlock {
     // `row_filters` must be set too): ... and if the row's own window, s.ws.row_window [s.n], admits the query's value key,
     // s.ws.qvalues [Q].
     bool reverse = false, row_filters = false, row_windows = false;
+    // The pairs incident to listed rows (nk_search_pairs_rows): s.ws.pair_rows holds one bit per row of the shard for the
+    // listed rows, then the block's query rows (global ids); see nk::IncidentRows.
+    bool incident = false;
 };
 
 // One shard's range scan of a block, rows [from, s.n): path, scan and exact re-scoring -> counts[Q] (host), *list_cap
@@ -1624,7 +1627,10 @@ static int range_shard(NkIndex *ix, NkShard &s, const RangeBlock &b, uint64_t fr
     ScanTimer timer(s);
     if (timer.attach(ix, &a)) return -1;
     int retried = 0;
-    if (nk::range_scan_shard(s.di, a, use != NK_PATH_SIMT, b.thr, s.ws, &ix->stats.kernel_launches, counts, list_cap, &retried, b.pair_first))
+    nk::IncidentRows inc{nullptr, nullptr};
+    if (b.incident) inc = {s.ws.pair_rows + (s.n + 31) / 32, s.ws.pair_rows};  // reserved by pairs_rows_locked
+    if (nk::range_scan_shard(s.di, a, use != NK_PATH_SIMT, b.thr, s.ws, &ix->stats.kernel_launches, counts, list_cap, &retried, b.pair_first,
+                             b.incident ? &inc : nullptr))
         return -1;
     timer.keep();
     ix->last_path = use;
@@ -1992,9 +1998,10 @@ static int graph_check(const NkIndex *ix, const GraphCall &g, std::vector<uint32
     return 0;
 }
 
-// The graph path: the forced one, or under AUTO the 16-bit pass where every live shard has a 16-bit image, else the TF32
-// filter; -1 if a live shard cannot serve it at the shape of the graph's searches (the error names the path and the shape).
-static int graph_path(const NkIndex *ix, const GraphCall &g, const std::vector<NkShard *> &live) {
+// The graph path (the k-NN graph calls and the incident pairs of the self-join): the forced one, or under AUTO the 16-bit pass
+// where every live shard has a 16-bit image, else the TF32 filter; -1 if a live shard cannot serve it for a block of
+// SEARCH_ROWS_BLOCK queries asking k each (range: range queries) (the error names the path and the shape).
+static int graph_path(const NkIndex *ix, const std::vector<NkShard *> &live, uint32_t k, bool range) {
     int path = ix->path;
     if (path == NK_PATH_AUTO) {
         path = NK_PATH_TENSOR_SHADOW;
@@ -2002,8 +2009,8 @@ static int graph_path(const NkIndex *ix, const GraphCall &g, const std::vector<N
             if (!s->img.current(s->n)) path = NK_PATH_TENSOR_FILTER;
     }
     for (NkShard *s : live) {
-        nk::ScanArgs a = shard_scan_args(ix, *s, nullptr, SEARCH_ROWS_BLOCK, g.k + 1, s->stream);
-        if (plan_path(ix, *s, path, false, &a) < 0) return -1;
+        nk::ScanArgs a = shard_scan_args(ix, *s, nullptr, SEARCH_ROWS_BLOCK, k, s->stream);
+        if (plan_path(ix, *s, path, range, &a) < 0) return -1;
     }
     return path;
 }
@@ -2251,7 +2258,7 @@ static int knn_graph_remap_locked(NkIndex *ix, GraphCall g, uint64_t *n_lists_ch
     std::vector<uint32_t> now_at;
     if (graph_check(ix, g, &now_at)) return -1;
     const std::vector<NkShard *> live = live_shards(ix);
-    const int path = graph_path(ix, g, live);
+    const int path = graph_path(ix, live, g.k + 1, false);
     if (path < 0) return -1;
     if (n_lists_changed) *n_lists_changed = 0;
     ix->stats.searches++;
@@ -2369,6 +2376,271 @@ int nk_knn_graph_update_windowed(NkIndex *ix, uint32_t k, uint64_t n_old, const 
                                  uint64_t *n_lists_changed) {
     return knn_graph_update_host(ix, GraphCall{"nk_knn_graph_update_windowed", k, n_old, nullptr, filters_host, windows_host, nullptr, nullptr,
                                                graph_idx, graph_score, true}, changed_rows, n_changed, n_lists_changed);
+}
+
+// ---- the self-join kept current (DESIGN.md §3.5d, "Pairs incident to rows") ---------------------------------------------
+// The listed rows are range queries over every shard whole (no triangle), in blocks of SEARCH_ROWS_BLOCK gathered by
+// stage_row_block with the join's admission (a listed row the join would refuse gets the filter, or the window, that admits no
+// row), on the graph path.  range_rescore_incident_kernel drops each query's own row and the listed rows below it, and scores
+// every other pair with its lower row as the query: each key is the one the whole-index join gives the pair.
+struct PairsCall {
+    const char *what;
+    float threshold;
+    const NkFilter *filter;
+    const NkWindow *window;
+    uint64_t max_gap;
+};
+
+// The pairs of the whole-index join incident to rows[n] (relative ids, distinct, checked), the index lock held: row i's are
+// keys[off[i], off[i + 1]), in nk_search's order.
+static int pairs_rows_locked(NkIndex *ix, const PairsCall &c, int path, const std::vector<NkShard *> &live, const uint32_t *rows,
+                             uint32_t n, std::vector<uint64_t> *off, std::vector<uint64_t> *keys) {
+    off->assign((size_t)n + 1, 0);
+    keys->clear();
+    if (n == 0) return 0;
+    RowAdmit adm;  // the join's (nk_search_pairs_windowed)
+    adm.windowed = c.window || c.max_gap != NK_NO_GAP;
+    const bool admit = c.filter || ix->mask_on || adm.windowed;
+    if (c.filter) adm.f = *c.filter;
+    if (c.window) adm.w = *c.window;
+    adm.gap = c.max_gap;
+    const uint32_t QB = std::min(n, SEARCH_ROWS_BLOCK);
+    // every live shard: the bits of the listed rows it holds, room for a block's query rows behind them
+    for (NkShard *s : live) {
+        const uint64_t lo = ix->first_row(*s), words = (s->n + 31) / 32;
+        std::vector<uint32_t> bits(words, 0u);
+        for (uint32_t i = 0; i < n; ++i)
+            if (rows[i] >= lo && rows[i] - lo < s->n) bits[(rows[i] - lo) >> 5] |= 1u << ((rows[i] - lo) & 31);
+        NK_CUDA_OK(cudaSetDevice(s->device));
+        if (nk::ws_reserve((void **)&s->ws.pair_rows, &s->ws.pair_rows_bytes, (size_t)(words + QB) * 4)) return -1;
+        NK_CUDA_OK(cudaMemcpyAsync(s->ws.pair_rows, bits.data(), words * 4, cudaMemcpyHostToDevice, s->stream));
+        NK_CUDA_OK(cudaStreamSynchronize(s->stream));  // bits is pageable and goes out of scope
+        ix->stats.bytes_h2d += words * 4;
+    }
+    const std::vector<uint32_t> thr(QB, nk::ord_bits(range_key_threshold(ix, c.threshold)));
+    std::vector<uint32_t> qrow(QB);
+    std::vector<uint64_t> per_query;
+    RangeShards on{live};
+    for (uint32_t b = 0; b < n; b += QB) {
+        const uint32_t nb = std::min(QB, n - b);
+        for (uint32_t q = 0; q < nb; ++q) qrow[q] = (uint32_t)(ix->row_base + rows[b + q]);
+        StageQueries stage_rows;
+        if (stage_row_block(ix, live, rows + b, nb, admit ? &adm : nullptr, &stage_rows)) return -1;
+        const StageQueries stage = [&](NkShard &s) {
+            if (stage_rows(s)) return -1;
+            // the block's query rows behind the listed-row bits (range_shard's IncidentRows), read before its first synchronisation
+            NK_CUDA_OK(cudaMemcpyAsync(s.ws.pair_rows + (s.n + 31) / 32, qrow.data(), (size_t)nb * 4, cudaMemcpyHostToDevice, s.stream));
+            ix->stats.bytes_h2d += (uint64_t)nb * 4;
+            return 0;
+        };
+        RangeBlock block{path, nb, thr.data()};
+        block.filtered = admit;
+        block.windowed = adm.windowed;
+        block.incident = true;
+        if (range_scan(ix, &on, stage, block, &per_query)) return -1;
+        for (uint32_t q = 0; q < nb; ++q) (*off)[b + q + 1] = (*off)[b + q] + per_query[q];
+        if ((*off)[b + nb] > keys->size() && range_collect(ix, on, nb, keys)) return -1;
+    }
+    return 0;
+}
+
+// The checks every call of this section makes before any work, the index lock held.
+static int pairs_check(const NkIndex *ix, const PairsCall &c) {
+    if (c.threshold != c.threshold) { nk::set_error("%s: threshold is NaN", c.what); return -1; }
+    if (ix->path == NK_PATH_SIMT || ix->path == NK_PATH_TENSOR) {
+        nk::set_error("%s: the incident pairs are scanned on the filter paths (AUTO, TENSOR_FILTER or TENSOR_SHADOW), not path %d",
+                      c.what, ix->path);
+        return -1;
+    }
+    return 0;
+}
+
+static int pairs_rows_host(NkIndex *ix, const PairsCall &c, const uint32_t *rows_host, uint32_t n, uint64_t capacity,
+                           uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total) {
+    nk::DeviceGuard _restore_device;
+    if (!ix) { nk::set_error("null index"); return -1; }
+    if (n && (!rows_host || !out_offsets || !out_total)) { nk::set_error("null argument"); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
+    if (pairs_check(ix, c)) return -1;
+    const uint64_t total_rows = ix->rows();
+    std::vector<uint8_t> seen(n ? total_rows : 0, 0);
+    for (uint32_t i = 0; i < n; ++i) {
+        if (rows_host[i] >= total_rows) {
+            nk::set_error("%s: row %u (entry %u) out of range, index has %llu rows", c.what, rows_host[i], i, (unsigned long long)total_rows);
+            return -1;
+        }
+        if (seen[rows_host[i]]++) { nk::set_error("%s: row %u is listed twice", c.what, rows_host[i]); return -1; }
+    }
+    if (out_offsets) out_offsets[0] = 0;
+    if (out_total) *out_total = 0;
+    if (n == 0) return 0;
+    const std::vector<NkShard *> live = live_shards(ix);
+    const int path = graph_path(ix, live, 1, true);
+    if (path < 0) return -1;
+    ix->stats.searches++;
+    ix->stats.queries += n;
+    ScopedRange range(c.what);
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
+    std::vector<uint64_t> off, keys;
+    if (pairs_rows_locked(ix, c, path, live, rows_host, n, &off, &keys)) return -1;
+    memcpy(out_offsets, off.data(), ((size_t)n + 1) * 8);
+    *out_total = off[n];
+    if (*out_total > capacity || *out_total == 0) return 0;
+    if (!out_idx || !out_score) { nk::set_error("null argument"); return -1; }
+    for (size_t j = 0; j < keys.size(); ++j) decode_key(ix->metric, keys[j], out_idx + j, out_score + j);
+    return 0;
+}
+
+int nk_search_pairs_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t n, float threshold, const NkFilter *filter, uint64_t capacity,
+                         uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total) {
+    return pairs_rows_host(ix, PairsCall{"nk_search_pairs_rows", threshold, filter, nullptr, NK_NO_GAP}, rows_host, n, capacity, out_offsets,
+                           out_idx, out_score, out_total);
+}
+
+int nk_search_pairs_rows_windowed(NkIndex *ix, const uint32_t *rows_host, uint32_t n, float threshold, const NkFilter *filter,
+                                  const NkWindow *window, uint64_t max_gap, uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx,
+                                  float *out_score, uint64_t *out_total) {
+    return pairs_rows_host(ix, PairsCall{"nk_search_pairs_rows_windowed", threshold, filter, window, max_gap}, rows_host, n, capacity,
+                           out_offsets, out_idx, out_score, out_total);
+}
+
+// The remap: old pairs whose two ends are kept at their id are carried (their ids, orientation and keys cannot have changed),
+// every other old pair is dropped, and the pairs incident to the new and moved rows C are found by pairs_rows_locked.  Each
+// found pair goes to its lower end's list and is merged there with the carried entries in key space.  Carried keys come back
+// from the old scores (cosine / dot: the score is the key's); under euclidean two squared distances one ulp apart decode to one
+// distance, so the carried keys of a list that takes in found pairs are computed again on the device (graph_pair_keys_on).
+int nk_pairs_remap(NkIndex *ix, float threshold, const NkFilter *filter, const NkWindow *window, uint64_t max_gap, uint64_t n_old,
+                   const uint32_t *src_of_row, const uint64_t *old_offsets, const uint32_t *old_idx, const float *old_score,
+                   uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total,
+                   uint64_t *n_dropped, uint64_t *n_found) {
+    const PairsCall c{"nk_pairs_remap", threshold, filter, window, max_gap};
+    nk::DeviceGuard _restore_device;
+    if (!ix) { nk::set_error("null index"); return -1; }
+    if (!old_offsets || !out_offsets || !out_total) { nk::set_error("null argument"); return -1; }
+    std::lock_guard<std::mutex> lk(ix->mu);
+    if (pairs_check(ix, c)) return -1;
+    const uint64_t N = ix->rows();
+    if (N && !src_of_row) { nk::set_error("null argument"); return -1; }
+    if (n_old > 0xffffffffull) { nk::set_error("%s: n_old=%llu is past the 32-bit row ids", c.what, (unsigned long long)n_old); return -1; }
+    if (old_offsets[0] != 0) { nk::set_error("%s: old_offsets[0] = %llu, not 0", c.what, (unsigned long long)old_offsets[0]); return -1; }
+    for (uint64_t o = 0; o < n_old; ++o)
+        if (old_offsets[o + 1] < old_offsets[o]) { nk::set_error("%s: old_offsets decrease at row %llu", c.what, (unsigned long long)o); return -1; }
+    const uint64_t n_old_pairs = old_offsets[n_old];
+    if (n_old_pairs && (!old_idx || !old_score)) { nk::set_error("null argument"); return -1; }
+    std::vector<uint32_t> now_at(n_old, NK_ROW_NEW);
+    for (uint64_t f = 0; f < N; ++f) {
+        const uint32_t o = src_of_row[f];
+        if (o == NK_ROW_NEW) continue;
+        if (o >= n_old) {
+            nk::set_error("%s: src_of_row[%llu] = %u is not an old row (n_old=%llu)", c.what, (unsigned long long)f, o, (unsigned long long)n_old);
+            return -1;
+        }
+        if (now_at[o] != NK_ROW_NEW) { nk::set_error("%s: old row %u is the source of rows %u and %llu", c.what, o, now_at[o], (unsigned long long)f); return -1; }
+        now_at[o] = (uint32_t)f;
+    }
+    for (uint64_t o = 0; o < n_old; ++o)
+        for (uint64_t e = old_offsets[o]; e < old_offsets[o + 1]; ++e) {
+            const uint64_t j = (uint64_t)old_idx[e] - ix->row_base;
+            if (old_idx[e] < ix->row_base || j >= n_old || j <= o) {
+                nk::set_error("%s: entry %llu of old row %llu (row %u) is not an old row above it", c.what, (unsigned long long)e,
+                              (unsigned long long)o, old_idx[e]);
+                return -1;
+            }
+        }
+    out_offsets[0] = 0;
+    *out_total = 0;
+    if (n_dropped) *n_dropped = 0;
+    if (n_found) *n_found = 0;
+    auto kept = [&](uint64_t o) { return o < N && now_at[o] == o; };  // an old row still at its id
+    std::vector<uint32_t> C;  // new and moved rows
+    for (uint64_t f = 0; f < N; ++f)
+        if (src_of_row[f] != f) C.push_back((uint32_t)f);
+    const std::vector<NkShard *> live = live_shards(ix);
+    const int path = C.empty() ? 0 : graph_path(ix, live, 1, true);
+    if (path < 0) return -1;
+    ix->stats.searches++;
+    ix->stats.queries += C.size();
+    ScopedRange range(c.what);
+    ShardOrder order(ix);
+    if (order.failed()) return -1;
+    std::vector<uint64_t> coff, ckeys;
+    if (pairs_rows_locked(ix, c, path, live, C.data(), (uint32_t)C.size(), &coff, &ckeys)) return -1;
+    // the found pairs under their lower end: (owner, key), owners ascending, each owner's keys descending
+    std::vector<std::pair<uint32_t, uint64_t>> found;
+    found.reserve(ckeys.size());
+    for (size_t i = 0; i < C.size(); ++i)
+        for (uint64_t e = coff[i]; e < coff[i + 1]; ++e) {
+            const uint32_t j = (uint32_t)(nk::key_row(ckeys[e]) - ix->row_base);
+            if (j > C[i]) found.emplace_back(C[i], ckeys[e]);
+            else found.emplace_back(j, (ckeys[e] & 0xffffffff00000000ull) | (0xffffffffull - (ix->row_base + C[i])));
+        }
+    std::sort(found.begin(), found.end(), [](const std::pair<uint32_t, uint64_t> &a, const std::pair<uint32_t, uint64_t> &b) {
+        return a.first != b.first ? a.first < b.first : a.second > b.second;
+    });
+    // carried entries of every current row -> offsets; the keys of those that meet found pairs
+    std::vector<uint8_t> touched(N, 0);
+    for (const auto &p : found) touched[p.first] = 1;
+    uint64_t carried = 0;
+    std::vector<uint64_t> cnt(N, 0);
+    for (uint64_t r = 0; r < N && r < n_old; ++r) {
+        if (!kept(r)) continue;
+        for (uint64_t e = old_offsets[r]; e < old_offsets[r + 1]; ++e) cnt[r] += kept(old_idx[e] - ix->row_base);
+        carried += cnt[r];
+    }
+    for (const auto &p : found) ++cnt[p.first];
+    for (uint64_t r = 0; r < N; ++r) out_offsets[r + 1] = out_offsets[r] + cnt[r];
+    *out_total = out_offsets[N];
+    if (n_dropped) *n_dropped = n_old_pairs - carried;
+    if (n_found) *n_found = found.size();
+    if (*out_total > capacity || *out_total == 0) return 0;
+    if (!out_idx || !out_score) { nk::set_error("null argument"); return -1; }
+    std::vector<uint64_t> okey(ix->metric == NK_METRIC_EUCLIDEAN ? n_old_pairs : 0, 0ull);
+    if (!okey.empty()) {
+        const size_t n_shards = ix->shards.size();
+        std::vector<std::vector<uint32_t>> pr(n_shards), pj(n_shards);
+        std::vector<std::vector<uint64_t>> at(n_shards), keys(n_shards);
+        for (uint64_t r = 0; r < N && r < n_old; ++r) {
+            if (!touched[r] || !kept(r)) continue;
+            uint64_t local;
+            const size_t si = (size_t)(find_shard(ix, r, &local) - ix->shards.data());
+            for (uint64_t e = old_offsets[r]; e < old_offsets[r + 1]; ++e)
+                if (kept(old_idx[e] - ix->row_base)) {
+                    pr[si].push_back((uint32_t)r);
+                    pj[si].push_back((uint32_t)(old_idx[e] - ix->row_base));
+                    at[si].push_back(e);
+                }
+        }
+        for (size_t i = 0; i < n_shards; ++i) {
+            if (pr[i].empty()) continue;
+            if (graph_pair_keys_on(ix, live, ix->shards[i], pr[i], pj[i], &keys[i])) return -1;
+            for (size_t t = 0; t < at[i].size(); ++t) okey[at[i][t]] = keys[i][t];
+        }
+    }
+    std::vector<uint64_t> mine, merged;
+    size_t f0 = 0;
+    for (uint64_t r = 0; r < N; ++r) {
+        uint64_t w = out_offsets[r];
+        const bool old_list = r < n_old && kept(r);
+        if (!touched[r]) {  // the carried entries as they were
+            if (old_list)
+                for (uint64_t e = old_offsets[r]; e < old_offsets[r + 1]; ++e)
+                    if (kept(old_idx[e] - ix->row_base)) { out_idx[w] = old_idx[e]; out_score[w] = old_score[e]; ++w; }
+            continue;
+        }
+        mine.clear();
+        if (old_list)
+            for (uint64_t e = old_offsets[r]; e < old_offsets[r + 1]; ++e)
+                if (kept(old_idx[e] - ix->row_base)) mine.push_back(okey.empty() ? nk::make_key(old_score[e], old_idx[e]) : okey[e]);
+        const size_t f1 = f0;
+        while (f0 < found.size() && found[f0].first == r) ++f0;
+        merged.resize(mine.size() + (f0 - f1));
+        std::vector<uint64_t> fk(f0 - f1);
+        for (size_t i = f1; i < f0; ++i) fk[i - f1] = found[i].second;
+        std::merge(mine.begin(), mine.end(), fk.begin(), fk.end(), merged.begin(), std::greater<uint64_t>());
+        for (uint64_t key : merged) { decode_key(ix->metric, key, out_idx + w, out_score + w); ++w; }
+    }
+    return 0;
 }
 
 static int single_shard(NkIndex *ix, NkShard **out) {

@@ -38,6 +38,7 @@ struct Workspace {
     NkWindow *row_window = nullptr; size_t row_window_bytes = 0;  // windowed graph update: each row's own window [n]
     uint64_t *qvalues = nullptr;  size_t qvalues_bytes = 0;    // ... and the value keys of the reverse scan's queries [Q]
     NkWindow *qwindow = nullptr;  size_t qwindow_bytes = 0;    // staged per-query value windows (host API, next to the filters)
+    uint32_t *pair_rows = nullptr; size_t pair_rows_bytes = 0;  // nk_search_pairs_rows: listed-row bits [(n + 31) / 32], then query rows [Q]
     // cached TMA descriptors (tc_cached_map): re-encoded only when the base pointer or shape changes
     struct MapSlot {
         alignas(64) unsigned char bytes[128];
@@ -217,8 +218,16 @@ int scan_simt_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint
 // One shard's scan (tensor: the filter, else the CUDA-core scan) and exact re-scoring: survivors per query -> counts[Q] (host);
 // *list_cap = the list capacity the lists were filled with; *retried = 1 if the scan ran twice.  pair_first (the self-join,
 // nk_search_pairs): query q is stored row *pair_first + q (global id) and keeps only rows above it; nullptr = range search.
+// incident (nk_search_pairs_rows, tensor-core lists only): query q is stored row qrow[q] (global id, device [Q]); listed (device,
+// one bit per row of the shard) marks the rows listed in the call; each listed pair is kept under its lower listed end and
+// scored with its lower row as the query.
+struct IncidentRows {
+    const uint32_t *qrow;
+    const uint32_t *listed;
+};
 int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const uint32_t *thr_bits, Workspace &ws, uint64_t *launches,
-                     int *counts, uint32_t *list_cap, int *retried, const uint64_t *pair_first = nullptr);
+                     int *counts, uint32_t *list_cap, int *retried, const uint64_t *pair_first = nullptr,
+                     const IncidentRows *incident = nullptr);
 // After range_scan_shard: the shard's survivors, CSR by counts[Q], each query's run sorted -> *keys (host).
 int range_sorted_keys(const DeviceInfo &di, Workspace &ws, cudaStream_t stream, uint32_t Q, const int *counts, uint32_t list_cap,
                       std::vector<uint64_t> *keys, uint64_t *launches);

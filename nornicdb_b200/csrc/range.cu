@@ -7,7 +7,8 @@
 //   2. range_rescore_kernel re-scores every listed pair exactly in fp32 (warp_exact_score, the arithmetic of every filter
 //      path's finish) and keeps those that meet the threshold; the survivor counts come back to the host (size protocol).
 //      The self-join (nk_search_pairs) runs its twin range_rescore_pairs_kernel, which also drops every row at or below the
-//      query's own row; the reverse scan of nk_knn_graph_update runs range_rescore_reverse_kernel, which scores each pair as
+//      query's own row; the pairs incident to listed rows (nk_search_pairs_rows) run range_rescore_incident_kernel, which
+//      scores each pair with its lower row as the query; the reverse scan of nk_knn_graph_update runs range_rescore_reverse_kernel, which scores each pair as
 //      the listed row's k-NN list ranks the query (warp_pair_score) and also holds it to the row's threshold;
 //   3. range_compact_kernel packs the survivors of every query into one CSR array, range_sort_runs_kernel sorts runs of
 //      RUN keys per query in shared memory, range_merge_kernel merges sorted runs pairwise until each query's segment is
@@ -52,11 +53,17 @@ struct RescoreParams {
 // REVERSE (nk_knn_graph_update): query q is a new or rewritten stored row and each listed row r an old row whose k-NN list q
 // may enter.  The score is K(r, q), q's score in r's list (warp_pair_score: |q|^2 as a stored row's), and it must reach both
 // the query's threshold (the score floor) and r's own (the score of r's k-th entry).  Tensor-core lists only.
-template <bool PAIRS, bool REVERSE = false>
-__device__ __forceinline__ void rescore_lists(const RescoreParams &p, uint64_t pair_first) {
+// INCIDENT (nk_search_pairs_rows): query q is stored row c = qrow[q] (global id) and every listed row j forms the pair {c, j}
+// of the self-join, which scores it with the lower row as the query.  j == c is dropped, and so is j < c when j is listed
+// too (bit j - row_base of `listed`: the pair belongs to j's list); j > c is scored with c as the query (warp_exact_score),
+// j < c with j as the query (warp_pair_score: |c|^2 as a stored row's).  Tensor-core lists only.
+template <bool PAIRS, bool REVERSE = false, bool INCIDENT = false>
+__device__ __forceinline__ void rescore_lists(const RescoreParams &p, uint64_t pair_first, const uint32_t *qrow = nullptr,
+                                              const uint32_t *listed = nullptr) {
     extern __shared__ __align__(16) float qs[];  // the query, [dim]
     __shared__ float s_qq;
     __shared__ int s_cnt;
+    __shared__ float s_qx;  // INCIDENT: |q|^2 as a stored row's
     const uint32_t q = p.q_base + blockIdx.y;
     const int len = p.fill[q];
     const int i0 = blockIdx.x * RS_ENTRIES;
@@ -65,10 +72,10 @@ __device__ __forceinline__ void rescore_lists(const RescoreParams &p, uint64_t p
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     uint64_t *list = p.lists + (size_t)q * p.list_cap;
     const float thr = ord_to_float(p.thr[q]);
-    const uint64_t self = pair_first + q;  // PAIRS: keep rows > self
+    const uint64_t self = INCIDENT ? (uint64_t)qrow[q] : pair_first + q;  // PAIRS: keep rows > self
     if (tid == 0) s_cnt = 0;
     int mine = 0;
-    if (p.rescore) {
+    if (INCIDENT || p.rescore) {
         for (uint32_t j = tid; j < p.dim; j += RS_THREADS) qs[j] = p.queries[(size_t)q * p.dim + j];
         __syncthreads();
         if (REVERSE) {
@@ -82,6 +89,10 @@ __device__ __forceinline__ void rescore_lists(const RescoreParams &p, uint64_t p
 #pragma unroll
             for (int o = 16; o; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
             if (lane == 0) s_qq = a;
+            if (INCIDENT) {
+                const float x = warp_stored_sqnorm(qs, p.dtype, p.dim, lane);
+                if (lane == 0) s_qx = x;
+            }
         }
         __syncthreads();
         for (int i = i0 + warp; i < i1; i += RS_THREADS / 32) {
@@ -91,8 +102,13 @@ __device__ __forceinline__ void rescore_lists(const RescoreParams &p, uint64_t p
                 continue;
             }
             const size_t local = (size_t)(grow - (uint32_t)p.row_base);
-            const float sc = REVERSE ? warp_pair_score(p.rows, p.dtype, local, p.dim, qs, s_qq, p.metric, lane)
-                                     : warp_exact_score(p.rows, p.dtype, local, p.dim, qs, s_qq, p.metric, lane);
+            if (INCIDENT && (grow == self || (grow < self && (__ldg(listed + (local >> 5)) >> (local & 31) & 1u)))) {
+                if (lane == 0) list[i] = 0ull;
+                continue;
+            }
+            const float sc = REVERSE || (INCIDENT && grow < self)
+                                 ? warp_pair_score(p.rows, p.dtype, local, p.dim, qs, INCIDENT ? s_qx : s_qq, p.metric, lane)
+                                 : warp_exact_score(p.rows, p.dtype, local, p.dim, qs, s_qq, p.metric, lane);
             // (the graph keeps -inf scores, as filter_finish_kernel does under no floor)
             const bool keep = REVERSE ? sc >= thr && sc >= __ldg(p.row_thr + local) : sc > -INFINITY && sc >= thr;
             if (lane == 0) {
@@ -119,6 +135,9 @@ __global__ void __launch_bounds__(RS_THREADS) range_rescore_pairs_kernel(Rescore
     rescore_lists<true>(p, pair_first);
 }
 __global__ void __launch_bounds__(RS_THREADS) range_rescore_reverse_kernel(RescoreParams p) { rescore_lists<false, true>(p, 0); }
+__global__ void __launch_bounds__(RS_THREADS) range_rescore_incident_kernel(RescoreParams p, const uint32_t *qrow, const uint32_t *listed) {
+    rescore_lists<false, false, true>(p, 0, qrow, listed);
+}
 
 // The keys K(r, j) of given pairs (nk_knn_graph_update's merge), one warp per pair: r = local row rl[i] of `rows`, j = row
 // js_row[i] of the widened block js [.. x dim] (global id jid[i]).
@@ -208,10 +227,11 @@ constexpr uint32_t LIST0 = 1024;  // first list capacity per query (the workspac
 // Steps 1 and 2 on one shard: survivors per query -> counts[Q] (host); *list_cap = the list capacity the lists were filled
 // with (range_sorted_keys reads them); *retried = 1 if the scan ran twice.
 int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const uint32_t *thr_bits, Workspace &ws, uint64_t *launches,
-                     int *counts, uint32_t *list_cap_out, int *retried, const uint64_t *pair_first) {
+                     int *counts, uint32_t *list_cap_out, int *retried, const uint64_t *pair_first, const IncidentRows *incident) {
     const uint32_t Q = a.Q, QA = range_qa(Q);
     *retried = 0;
     if (a.check(true, !tensor)) return -1;
+    if (incident && !tensor) { set_error("internal: the incident pairs are re-scored from tensor-core lists only"); return -1; }
     if (ws_reserve((void **)&ws.keys2, &ws.keys2_bytes, (size_t)(2 * QA + 2 * Q) * 4 + (size_t)(Q + 1) * 8)) return -1;
     uint32_t list_cap = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(LIST0, ws.partial_bytes / ((size_t)Q * 8)), 0x7fffffffu);
     std::vector<int> fill(Q);
@@ -246,6 +266,7 @@ int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const
     rp.rescore = tensor ? 1 : 0; rp.row_thr = a.row_thr;
     const size_t smem = tensor ? (size_t)a.dim * 4 : 0;
     const void *kern = mode_row_thr(a.mode) ? reinterpret_cast<const void *>(range_rescore_reverse_kernel)
+                       : incident ? reinterpret_cast<const void *>(range_rescore_incident_kernel)
                        : pair_first ? reinterpret_cast<const void *>(range_rescore_pairs_kernel) : reinterpret_cast<const void *>(range_rescore_kernel);
     if (smem > 48 * 1024 && tc_ensure_smem(kern, di.device_id, smem)) return -1;
     if (longest > 0)
@@ -253,6 +274,7 @@ int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const
             rp.q_base = q0;
             const dim3 grid((longest + RS_ENTRIES - 1) / RS_ENTRIES, std::min(MAX_GRID_Y, Q - q0));
             if (mode_row_thr(a.mode)) range_rescore_reverse_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp);
+            else if (incident) range_rescore_incident_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp, incident->qrow, incident->listed);
             else if (pair_first) range_rescore_pairs_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp, *pair_first);
             else range_rescore_kernel<<<grid, RS_THREADS, smem, a.stream>>>(rp);
             NK_CUDA_OK(cudaGetLastError());

@@ -87,7 +87,7 @@ int ws_reserve(void **p, size_t *cur, size_t need) {
 }
 
 int Workspace::release() {
-    void *ptrs[] = {cand, partial, keys, keys2, below, queries, qfilter, out_idx, out_score, qaux, rownorm, flags, sub_rows, sub_gather, scratch, row_thr, row_filter, qtags, qwindow, row_window, qvalues};
+    void *ptrs[] = {cand, partial, keys, keys2, below, queries, qfilter, out_idx, out_score, qaux, rownorm, flags, sub_rows, sub_gather, scratch, row_thr, row_filter, qtags, qwindow, row_window, qvalues, pair_rows};
     for (void *q : ptrs)
         if (q) cudaFree(q);
     *this = Workspace();

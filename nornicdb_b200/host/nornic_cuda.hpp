@@ -227,9 +227,11 @@ public:
         if (it != idToIndex_.end()) {
             check(nk_index_update_row(ix_, it->second, embedding.data()));
             if (graphK_) graphSrc_[it->second] = NK_ROW_NEW;  // contents SimilarGraph's graph never saw
+            if (pairsOn_) pairsSrc_[it->second] = NK_ROW_NEW;  // ... nor SimilarPairs' join
         } else {
             check(nk_index_append(ix_, embedding.data(), 1));
             if (graphK_) graphSrc_.push_back(NK_ROW_NEW);
+            if (pairsOn_) pairsSrc_.push_back(NK_ROW_NEW);
             tags_.push_back(0);    // nk_index_append: tag 0
             values_.push_back(0);  // ... and value key 0
             idToIndex_[nodeID] = nodeIDs_.size();
@@ -250,6 +252,10 @@ public:
         if (graphK_) {  // the last row's contents move to idx, as on the device
             graphSrc_[idx] = graphSrc_[last];
             graphSrc_.pop_back();
+        }
+        if (pairsOn_) {
+            pairsSrc_[idx] = pairsSrc_[last];
+            pairsSrc_.pop_back();
         }
         tags_[idx] = tags_[last];  // the tag and the value key move with their row
         tags_.pop_back();
@@ -293,6 +299,7 @@ public:
         check(nk_index_set_row_tags(ix_, firstRow, tags.data(), tags.size()));
         for (size_t i = 0; i < tags.size(); ++i) {
             if (graphK_ && tags_[firstRow + i] != tags[i]) graphSrc_[firstRow + i] = NK_ROW_NEW;
+            if (pairsOn_ && tags_[firstRow + i] != tags[i]) pairsSrc_[firstRow + i] = NK_ROW_NEW;
             tags_[firstRow + i] = tags[i];
         }
     }
@@ -324,6 +331,7 @@ public:
         check(nk_index_set_row_values(ix_, firstRow, keys.data(), keys.size()));
         for (size_t i = 0; i < keys.size(); ++i) {
             if (graphK_ && values_[firstRow + i] != keys[i]) graphSrc_[firstRow + i] = NK_ROW_NEW;
+            if (pairsOn_ && values_[firstRow + i] != keys[i]) pairsSrc_[firstRow + i] = NK_ROW_NEW;
             values_[firstRow + i] = keys[i];
         }
     }
@@ -522,6 +530,118 @@ public:
             }
         return out;
     }
+    // Auto-link on write: every pair of the whole-index join (SearchPairs with the same threshold, filter, window and maxGap)
+    // that has an end among `ids`, each as {listed node, other node, score}, grouped by the listed node in the order of `ids`
+    // (a pair with both ends listed once, under the node with the lower row), best first within a group.  Missing and repeated
+    // ids are ignored.  Scores are the join's (nk_search_pairs_rows_windowed), on the filter path SimilarGraph uses.
+    std::vector<SimilarPair> PairsOfNodes(const std::vector<std::string> &ids, float threshold, const NkFilter *filter = nullptr,
+                                          const NkWindow *window = nullptr, uint64_t maxGap = NK_NO_GAP) {
+        std::lock_guard<std::mutex> lk(mu_);
+        std::vector<uint32_t> rows;
+        std::unordered_map<uint64_t, bool> seen;
+        for (auto &id : ids) {
+            auto it = idToIndex_.find(id);
+            if (it != idToIndex_.end() && !seen[it->second]) { seen[it->second] = true; rows.push_back((uint32_t)it->second); }
+        }
+        std::vector<SimilarPair> out;
+        if (rows.empty()) return out;
+        std::vector<uint64_t> off(rows.size() + 1);
+        std::vector<uint32_t> idx;
+        std::vector<float> sc;
+        on_graph_path([&] {
+            uint64_t total = 0;
+            for (int pass = 0; pass < 2; ++pass) {
+                if (nk_search_pairs_rows_windowed(ix_, rows.data(), (uint32_t)rows.size(), threshold, filter, window, maxGap, idx.size(), off.data(),
+                                                  idx.data(), sc.data(), &total) < 0)
+                    return -1;
+                if (total <= idx.size()) break;
+                idx.resize(total);
+                sc.resize(total);
+            }
+            return 0;
+        });
+        for (size_t r = 0; r < rows.size(); ++r)
+            for (uint64_t i = off[r]; i < off[r + 1]; ++i)
+                if (idx[i] < nodeIDs_.size()) out.push_back({nodeIDs_[rows[r]], nodeIDs_[idx[i]], sc[i]});
+        return out;
+    }
+    // The whole-index join (SearchPairs with the same arguments, in the same order) kept current across Add / AddBatch /
+    // Remove / SetRowTags / SetRowValues, as SimilarGraph keeps its graph: the index follows which row of the last join each
+    // row's contents came from (a rewritten, retagged or re-valued row is new contents), and the next call hands that map to
+    // nk_pairs_remap instead of joining again.  The first call, a new threshold, filter, window or maxGap, or a Deserialize
+    // since the last call rebuild the join in stripes of stripeRows left rows, as SearchPairs does.  Runs on the filter path
+    // SimilarGraph uses, which the remap requires.  The join is held in host memory, 8 B per pair.
+    std::vector<SimilarPair> SimilarPairs(float threshold, const NkFilter *filter = nullptr, const NkWindow *window = nullptr,
+                                          uint64_t maxGap = NK_NO_GAP, uint64_t stripeRows = 1u << 16) {
+        std::lock_guard<std::mutex> lk(mu_);
+        const uint64_t n = nodeIDs_.size();
+        const NkFilter f = filter ? *filter : NkFilter{0, 0, 0};
+        const NkWindow w = window ? *window : NkWindow{0, ~0ull};
+        const bool same = pairsOn_ && std::memcmp(&pairsT_, &threshold, 4) == 0 && pairsHasF_ == (filter != nullptr) &&
+                          pairsF_.all_of == f.all_of && pairsF_.none_of == f.none_of && pairsF_.any_of == f.any_of &&
+                          pairsHasW_ == (window != nullptr) && pairsW_.lo == w.lo && pairsW_.hi == w.hi && pairsGap_ == maxGap;
+        std::vector<uint64_t> off(n + 1, 0);
+        std::vector<uint32_t> idx;
+        std::vector<float> sc;
+        if (stripeRows == 0) stripeRows = 1;
+        on_graph_path([&] {
+            uint64_t total = 0;
+            if (same) {
+                for (int pass = 0; pass < 2; ++pass) {
+                    if (nk_pairs_remap(ix_, threshold, filter, window, maxGap, pairsRows_, pairsSrc_.data(), pairsOff_.data(), pairsIdx_.data(),
+                                       pairsScore_.data(), idx.size(), off.data(), idx.data(), sc.data(), &total, nullptr, nullptr) < 0)
+                        return -1;
+                    if (total <= idx.size()) return 0;
+                    idx.resize(total);
+                    sc.resize(total);
+                }
+                return 0;
+            }
+            idx.clear();
+            sc.clear();
+            std::vector<uint32_t> si;
+            std::vector<float> ss;
+            for (uint64_t first = 0; first < n; first += stripeRows) {  // stripes of the whole join, concatenated
+                const uint64_t rows = std::min<uint64_t>(stripeRows, n - first);
+                std::vector<uint64_t> so(rows + 1);
+                for (int pass = 0; pass < 2; ++pass) {
+                    if (nk_search_pairs_windowed(ix_, first, rows, threshold, filter, window, maxGap, si.size(), so.data(), si.data(), ss.data(),
+                                                 &total) < 0)
+                        return -1;
+                    if (total <= si.size()) break;
+                    si.resize(total);
+                    ss.resize(total);
+                }
+                for (uint64_t r = 0; r < rows; ++r) off[first + r + 1] = off[first] + so[r + 1];
+                idx.insert(idx.end(), si.begin(), si.begin() + total);
+                sc.insert(sc.end(), ss.begin(), ss.begin() + total);
+            }
+            ++pairsRebuilds_;
+            return 0;
+        });
+        idx.resize(off[n]);
+        sc.resize(off[n]);
+        pairsOn_ = true;
+        pairsT_ = threshold;
+        pairsHasF_ = filter != nullptr;
+        pairsF_ = f;
+        pairsHasW_ = window != nullptr;
+        pairsW_ = w;
+        pairsGap_ = maxGap;
+        pairsRows_ = n;
+        pairsOff_.swap(off);
+        pairsIdx_.swap(idx);
+        pairsScore_.swap(sc);
+        pairsSrc_.resize(n);
+        for (uint64_t r = 0; r < n; ++r) pairsSrc_[r] = (uint32_t)r;
+        std::vector<SimilarPair> out;
+        out.reserve(pairsIdx_.size());
+        for (uint64_t r = 0; r < n; ++r)
+            for (uint64_t i = pairsOff_[r]; i < pairsOff_[r + 1]; ++i)
+                if (pairsIdx_[i] < n) out.push_back({nodeIDs_[r], nodeIDs_[pairsIdx_[i]], pairsScore_[i]});
+        return out;
+    }
+    uint64_t PairsRebuilds() const { return pairsRebuilds_; }  // SimilarPairs calls that joined every row
     std::vector<SearchResult> ScoreSubset(const std::vector<float> &query, const std::vector<std::string> &ids) {  // gpu.go:1552-1616
         if ((int)query.size() != dims_) throw ErrInvalidDimensions();
         std::lock_guard<std::mutex> lk(mu_);
@@ -586,6 +706,7 @@ public:
         check(nk_index_upload(ix_, data.data() + off, count));  // the blob streams straight into device memory
         gpuSynced_ = false;
         graphK_ = 0;
+        pairsOn_ = false;
         tags_.assign(count, 0);    // nk_index_upload: every tag 0
         values_.assign(count, 0);  // ... and every value key 0
         nodeIDs_ = ids;
@@ -595,6 +716,17 @@ public:
 
 private:
     void check(int rc) { if (rc != 0) throw cuda::ErrKernelExecution(std::string("gpu: ") + nk_last_error()); }
+    // Run call() on the 16-bit filter path, or the TF32 filter if the shape has no 16-bit image (SimilarGraph's choice), then
+    // go back to AUTO; throw if neither serves it.
+    template <class F> void on_graph_path(F call) {
+        int rc = -1;
+        for (int path : {NK_PATH_TENSOR_SHADOW, NK_PATH_TENSOR_FILTER}) {
+            check(nk_index_set_path(ix_, path));
+            if ((rc = call()) >= 0) break;
+        }
+        check(nk_index_set_path(ix_, NK_PATH_AUTO));
+        if (rc < 0) throw cuda::ErrKernelExecution(std::string("gpu: ") + nk_last_error());
+    }
     int dims_;
     NkIndex *ix_ = nullptr;
     std::vector<std::string> nodeIDs_;
@@ -612,6 +744,20 @@ private:
     std::vector<uint64_t> tags_;         // the tag of each row, as on the device
     std::vector<uint64_t> values_;       // the value key of each row, as on the device
     uint64_t graphRebuilds_ = 0;
+    // SimilarPairs: the join of rows [0, pairsRows_) (CSR) with its arguments (pairsOn_ = false: none), and for each current row
+    // the join row its contents came from (NK_ROW_NEW: appended, rewritten, retagged or re-valued since)
+    bool pairsOn_ = false;
+    float pairsT_ = 0.0f;
+    bool pairsHasF_ = false, pairsHasW_ = false;
+    NkFilter pairsF_{0, 0, 0};
+    NkWindow pairsW_{0, ~0ull};
+    uint64_t pairsGap_ = NK_NO_GAP;
+    uint64_t pairsRows_ = 0;
+    std::vector<uint64_t> pairsOff_;
+    std::vector<uint32_t> pairsIdx_;
+    std::vector<float> pairsScore_;
+    std::vector<uint32_t> pairsSrc_;
+    uint64_t pairsRebuilds_ = 0;
     std::mutex mu_;
 };
 

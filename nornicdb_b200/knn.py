@@ -508,6 +508,83 @@ class KnnIndex:
         t = int(total.value)
         return off, idx[:t].copy(), sc[:t].copy()
 
+    def _pairs_args(self, filter, window, max_gap):
+        f = None if filter is None else as_filters(filter, 1)
+        w = None if window is None else as_windows(window, 1)
+        gap = NO_GAP if max_gap is None else _gap_keys(max_gap)
+        return (None if f is None else f.ctypes.data_as(C.c_void_p), None if w is None else w.ctypes.data_as(C.c_void_p), gap), (f, w)
+
+    def search_pairs_rows(self, rows, threshold: float, filter=None, window=None,
+                          max_gap=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """The pairs of the whole-index self-join (search_pairs over every row, with the same threshold, filter, window and
+        max_gap) that have at least one end among `rows` (distinct row ids), grouped by that end; a pair with both ends listed
+        goes under the lower one.  Scores are the join's (the lower row of the pair is the query), each list in search()'s
+        order.  Returns CSR arrays (offsets uint64 [len(rows) + 1], idx uint32, score float32): rows[r]'s pairs are
+        [offsets[r], offsets[r + 1]).  Runs on the graph path (TENSOR_SHADOW or TENSOR_FILTER), so it equals the join with that
+        path forced; SIMT or TENSOR forced is refused (nk_search_pairs_rows_windowed)."""
+        r = np.ascontiguousarray(np.asarray(rows, dtype=np.int64).reshape(-1))
+        if r.size and (r.min() < 0 or r.max() > 0xFFFFFFFF):
+            raise KnnError("search_pairs_rows: row ids must lie in [0, 2^32)")
+        r = np.ascontiguousarray(r.astype(np.uint32))
+        args, keep = self._pairs_args(filter, window, max_gap)
+        off = np.zeros(r.size + 1, dtype=np.uint64)
+        total = C.c_uint64(0)
+        cap = getattr(self, "_pairs_cap", 0)
+        while True:
+            idx = np.empty(max(cap, 1), dtype=np.uint32)
+            sc = np.empty(max(cap, 1), dtype=np.float32)
+            _check(self.lib.nk_search_pairs_rows_windowed(self.ptr, r.ctypes.data_as(C.c_void_p), int(r.size), float(threshold), *args,
+                                                          cap, off.ctypes.data_as(C.c_void_p), idx.ctypes.data_as(C.c_void_p),
+                                                          sc.ctypes.data_as(C.c_void_p), C.byref(total)),
+                   "nk_search_pairs_rows_windowed")
+            if total.value <= cap:
+                break
+            cap = int(total.value)
+            self._pairs_cap = cap
+        t = int(total.value)
+        return off, idx[:t].copy(), sc[:t].copy()
+
+    def remap_pairs(self, pairs, n_old: int, src, threshold: float, filter=None, window=None,
+                    max_gap=None) -> Tuple[np.ndarray, np.ndarray, np.ndarray, int, int]:
+        """Bring a stored self-join up to date after any mix of append, update_row, remove_swap, retags and re-valued rows.
+        pairs = (offsets, idx, score): what search_pairs(threshold, filter=, window=, max_gap=) over the whole index of n_old
+        rows returned.  src: a GraphRowMap that followed the changes (call update_row for a retagged or re-valued row too), or
+        its src_of_row.  Returns (offsets, idx, score, n_dropped, n_found): what that search_pairs call over every row returns
+        now on the graph path, bit for bit; the old pairs dropped (an end gone, moved or new) and the pairs found incident to
+        the new and moved rows (nk_pairs_remap)."""
+        oo, oi, osc = pairs
+        n_old = int(n_old)
+        oo = np.ascontiguousarray(np.asarray(oo, dtype=np.uint64).reshape(-1))
+        oi = np.ascontiguousarray(np.asarray(oi, dtype=np.uint32).reshape(-1))
+        osc = np.ascontiguousarray(np.asarray(osc, dtype=np.float32).reshape(-1))
+        if oo.size != n_old + 1 or oi.size != osc.size or int(oo[-1]) != oi.size:
+            raise KnnError("remap_pairs: pairs must be CSR over n_old rows (n_old + 1 offsets, offsets[-1] entries)")
+        s = np.asarray(src.src_of_row if isinstance(src, GraphRowMap) else src, dtype=np.int64).reshape(-1)
+        n = len(self)
+        if s.size != n:
+            raise KnnError(f"remap_pairs: src_of_row has {s.size} entries, the index {n} rows")
+        if s.size and (s.min() < 0 or s.max() > ROW_NEW):
+            raise KnnError("remap_pairs: src_of_row entries must be old row ids or ROW_NEW")
+        s = np.ascontiguousarray(s.astype(np.uint32))
+        args, keep = self._pairs_args(filter, window, max_gap)
+        off = np.zeros(n + 1, dtype=np.uint64)
+        total, dropped, found = C.c_uint64(0), C.c_uint64(0), C.c_uint64(0)
+        cap = getattr(self, "_pairs_cap", 0)
+        while True:
+            idx = np.empty(max(cap, 1), dtype=np.uint32)
+            sc = np.empty(max(cap, 1), dtype=np.float32)
+            _check(self.lib.nk_pairs_remap(self.ptr, float(threshold), *args, n_old, s.ctypes.data_as(C.c_void_p),
+                                           oo.ctypes.data_as(C.c_void_p), oi.ctypes.data_as(C.c_void_p), osc.ctypes.data_as(C.c_void_p),
+                                           cap, off.ctypes.data_as(C.c_void_p), idx.ctypes.data_as(C.c_void_p),
+                                           sc.ctypes.data_as(C.c_void_p), C.byref(total), C.byref(dropped), C.byref(found)),
+                   "nk_pairs_remap")
+            if total.value <= cap:
+                break
+            cap = int(total.value)
+            self._pairs_cap = cap
+        t = int(total.value)
+        return off, idx[:t].copy(), sc[:t].copy(), int(dropped.value), int(found.value)
+
     def search_filtered_device(self, q_ptr: int, filters_ptr: int, Q: int, k: int, out_idx_ptr: int, out_score_ptr: int,
                                stream: int = 0) -> int:
         """Device-resident filtered search: filters_ptr = device [Q x 3] uint64 (0 = no filter), valid until the stream ran."""
