@@ -94,7 +94,16 @@ enum { NK_DTYPE_F32 = 0, NK_DTYPE_F16 = 1, NK_DTYPE_BF16 = 2 };
  * streaming a BF16 shadow copy of the shard (half the HBM bytes; built at upload for library-owned fp32 shards unless
  * NK_SHADOW=0, +50% device memory; plus an int8 copy with one scale per row, +25%, a quarter of the fp32 bytes, which
  * serves k <= 16 on large shards), exact fp32 rescoring from the fp32 rows, device-side retry through TENSOR_FILTER
- * and then the exact scan.  All paths return identical index sets. */
+ * and then the exact scan.  All paths return identical index sets.
+ * Dimensions each path serves (the shared-memory limits as on an H100, 232 448 B per block):
+ *   SIMT           any d up to about 56 800 (the query row and the candidate buffer in shared memory);
+ *   TENSOR         fp32, cosine / dot, 32 <= d <= 12288, d % 4 == 0 (its accumulation error grows with d);
+ *   TENSOR_FILTER  fp32, 32 <= d <= 32768, d % 4 == 0;
+ *   TENSOR_SHADOW  32 <= d <= 32768, d % 4 == 0 for fp32 rows (BF16 shadow or int8 image), d % 8 == 0 for fp16 / bf16;
+ *   group search (nk_search_groups) up to about 57 800.
+ * A forced path that does not serve the shape fails; AUTO picks among the paths that do, and the filters' exact stage
+ * runs on SIMT where TENSOR does not serve.  Past the SIMT limit no path serves d: a search fails with nk_last_error
+ * naming d (DESIGN.md §3.5g). */
 enum { NK_PATH_AUTO = 0, NK_PATH_SIMT = 1, NK_PATH_TENSOR = 2, NK_PATH_TENSOR_FILTER = 3, NK_PATH_TENSOR_SHADOW = 4 };
 
 /* k up to NK_MAX_K is one fused pass; larger k (the reference accepts any k) is served by ceil(k/NK_MAX_K) passes
@@ -124,7 +133,8 @@ const char *nk_last_error(void);
 const char *nk_version(void);
 
 /* An index = one row-major [N x dim] corpus, row-sharded by contiguous ranges over n_devices GPUs of
- * this process (shard g holds rows [base_g, base_g + n_g)).  gpu.EmbeddingIndex storage, gpu.go:1224-1260. */
+ * this process (shard g holds rows [base_g, base_g + n_g)).  gpu.EmbeddingIndex storage, gpu.go:1224-1260.  Any dim is
+ * accepted; which search paths serve it is listed with NK_PATH_* above. */
 NkIndex *nk_index_create(const int *device_ids, int n_devices, uint32_t dim, int dtype, int metric);
 void nk_index_release(NkIndex *ix); /* NULL-safe */
 

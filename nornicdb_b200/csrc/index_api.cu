@@ -3193,7 +3193,7 @@ int nk_search_groups(NkIndex *ix, const float *query_host, uint32_t k, uint32_t 
     unsigned long long *best = static_cast<unsigned long long *>(s->ws.scratch);
     NK_CUDA_OK(cudaMemcpyAsync(s->ws.queries, query_host, (size_t)ix->dim * 4, cudaMemcpyHostToDevice, s->stream));
     NK_CUDA_OK(cudaMemsetAsync(best, 0, (size_t)G * 8, s->stream));
-    if (nk::group_best(s->rows, ix->dtype, s->n, ix->dim, s->base, s->ws.queries, ix->metric, s->group, s->mask_on ? s->mask : nullptr,
+    if (nk::group_best(s->di, s->rows, ix->dtype, s->n, ix->dim, s->base, s->ws.queries, ix->metric, s->group, s->mask_on ? s->mask : nullptr,
                        ix->key_floor(), best, s->stream))
         return -1;
     if (nk::topk_keys(s->di, best, G, ke, s->ws, s->ws.keys, s->stream)) return -1;

@@ -177,6 +177,12 @@ int scan_tensor_filter(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, u
 int scan_tensor_filter_tail(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *out_keys, uint64_t *launches);
 bool scan_tensor_filter_supported(const DeviceInfo &di, const ScanArgs &a);
 bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a);
+// Largest d the filters serve: the int8 image's integer accumulation is exact while 127^2 d < 2^31 (DESIGN §3.3).
+// scan_tensor_filter_supported also asks that the finish kernel's shared memory fit the device.
+constexpr uint32_t FILTER_MAX_DIM = 32768;
+// Largest d the exact 3xTF32 scan serves (scan_tensor_supported); above it the exact stage of a filter search, TENSOR and
+// AUTO use the CUDA-core scan.
+constexpr uint32_t TENSOR_EXACT_MAX_DIM = 12288;
 // Tests only: the filters' score estimates and error bounds for every (row, query) pair (nk_debug_filter_dump).
 int scan_filter_dump(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, int which, float *est, float *bnd, uint32_t ld, uint64_t *launches);
 // fp32 rows [first, first+count) -> bf16 shadow rows (stride dimpad) + |x|^2, |x - bf16(x)|^2
@@ -264,8 +270,21 @@ int fill_clustered(void *out, int dtype, uint64_t n_rows, uint32_t dim, uint64_t
 // |x|^2 of rows [first, first+count) of an fp16 / bf16 corpus -> out[first..]
 int row_sqnorms16(const void *rows, int dtype, uint64_t first, uint64_t count, uint32_t dim, float *out, cudaStream_t s);
 // best-of-chunks per node (queryNodes): best[group[r]] = max key over the node's rows; top-k over the node keys; decode
-int group_best(const void *rows, int dtype, uint64_t n, uint32_t dim, uint64_t row_base, const float *query, int metric,
-               const uint32_t *group, const uint32_t *mask, float min_score, unsigned long long *best, cudaStream_t s);
+// (the query is staged in 4 dim bytes of shared memory: refused only past the device's opt-in limit)
+int group_best(const DeviceInfo &di, const void *rows, int dtype, uint64_t n, uint32_t dim, uint64_t row_base, const float *query,
+               int metric, const uint32_t *group, const uint32_t *mask, float min_score, unsigned long long *best, cudaStream_t s);
+// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device) and size (scan_tensor.cu)
+int tc_ensure_smem(const void *func, int device, size_t smem);
+// Shared memory a launch of func needs besides its dynamic part, counted as `cuobjdump -res-usage` counts it: the static
+// shared memory plus the SMEM_RESERVED bytes the system reserves per block (so a fit errs by at most 1 KB on the safe
+// side).  smem_fits: dyn + that <= the device's opt-in limit.  Every path whose dynamic shared memory grows with d asks
+// here before it admits d, so the planner never promises a launch the device refuses.
+constexpr size_t SMEM_RESERVED = 1024;
+size_t kernel_static_smem(const void *func);
+bool smem_fits(const DeviceInfo &di, const void *func, size_t dyn);
+// Before a launch of func with dyn bytes of dynamic shared memory: an error naming `what` and dim if it cannot fit the
+// device, else the opt-in wherever static + dynamic pass the 48 KB a launch gets by default.
+int ensure_smem(const DeviceInfo &di, const void *func, size_t dyn, const char *what, uint32_t dim);
 int topk_keys(const DeviceInfo &di, const unsigned long long *keys, uint32_t n, uint32_t k, Workspace &ws, uint64_t *out_keys,
               cudaStream_t s);
 int decode_group_keys(const uint64_t *keys, uint32_t k, int metric, const uint32_t *group, uint64_t row_base, uint32_t *out_group,

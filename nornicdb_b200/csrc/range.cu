@@ -268,7 +268,7 @@ int range_scan_shard(const DeviceInfo &di, const ScanArgs &a, bool tensor, const
     const void *kern = mode_row_thr(a.mode) ? reinterpret_cast<const void *>(range_rescore_reverse_kernel)
                        : incident ? reinterpret_cast<const void *>(range_rescore_incident_kernel)
                        : pair_first ? reinterpret_cast<const void *>(range_rescore_pairs_kernel) : reinterpret_cast<const void *>(range_rescore_kernel);
-    if (smem > 48 * 1024 && tc_ensure_smem(kern, di.device_id, smem)) return -1;
+    if (ensure_smem(di, kern, smem, "range re-scoring", a.dim)) return -1;
     if (longest > 0)
         for (uint32_t q0 = 0; q0 < Q; q0 += MAX_GRID_Y) {
             rp.q_base = q0;

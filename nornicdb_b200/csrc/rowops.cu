@@ -445,15 +445,15 @@ int row_windows(const uint32_t *idx, uint32_t n_idx, const uint32_t *mask, const
     NK_CUDA_OK(cudaGetLastError());
     return 0;
 }
-int group_best(const void *rows, int dtype, uint64_t n, uint32_t dim, uint64_t row_base, const float *query, int metric,
-               const uint32_t *group, const uint32_t *mask, float min_score, unsigned long long *best, cudaStream_t s) {
+int group_best(const DeviceInfo &di, const void *rows, int dtype, uint64_t n, uint32_t dim, uint64_t row_base, const float *query,
+               int metric, const uint32_t *group, const uint32_t *mask, float min_score, unsigned long long *best, cudaStream_t s) {
     if (n == 0) return 0;
     const size_t smem = (size_t)dim * 4;
     const unsigned grid = warp_grid(n);
-    if (smem > 48 * 1024) {
-        set_error("group search: dim=%u too large", dim);
-        return -1;
-    }
+    const void *kern = dtype == NK_DTYPE_F16    ? reinterpret_cast<const void *>(group_best_kernel<__half>)
+                       : dtype == NK_DTYPE_BF16 ? reinterpret_cast<const void *>(group_best_kernel<__nv_bfloat16>)
+                                                : reinterpret_cast<const void *>(group_best_kernel<float>);
+    if (ensure_smem(di, kern, smem, "group search", dim)) return -1;
     if (dtype == NK_DTYPE_F16)
         group_best_kernel<__half><<<grid, 256, smem, s>>>((const __half *)rows, n, dim, row_base, query, metric, group, mask, min_score, best);
     else if (dtype == NK_DTYPE_BF16)

@@ -434,12 +434,12 @@ int scan_simt(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint64_t *
         if (!vec) qt = left >= 3 ? 4 : 1;
         while (qt > 1 && (size_t)P * 8 + (size_t)qt * a.dim * 4 > smem_budget) qt = vec ? qt / 2 : 1;
         size_t smem = (size_t)P * 8 + (size_t)qt * a.dim * 4;
-        if (smem > di.max_smem_optin) {
-            set_error("dim=%u too large for the SIMT scan (needs %zu B shared memory)", a.dim, smem);
-            return -1;
-        }
         const uint32_t nq = left < (uint32_t)qt ? left : (uint32_t)qt;
         if (with_simt_kernel<false>(a, vec, qt, [&](auto kern, auto params) -> int {
+                if (!smem_fits(di, reinterpret_cast<const void *>(kern), smem)) {
+                    set_error("dim=%u too large for the SIMT scan (needs %zu B shared memory)", a.dim, smem);
+                    return -1;
+                }
                 if (simt_ensure(reinterpret_cast<const void *>(kern), di.device_id, smem)) return -1;
                 int occ = simt_occupancy(reinterpret_cast<const void *>(kern), di.device_id, smem);
                 // One grid for every query group of this search so the per-CTA partial lists line up.
@@ -488,12 +488,12 @@ int scan_simt_range(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, uint
         if (!vec) qt = left >= 3 ? 4 : 1;
         while (qt > 1 && (size_t)qt * a.dim * 4 > smem_budget) qt = vec ? qt / 2 : 1;
         const size_t smem = (size_t)qt * a.dim * 4;  // the queries only: no candidate buffer
-        if (smem > di.max_smem_optin) {
-            set_error("dim=%u too large for the SIMT scan (needs %zu B shared memory)", a.dim, smem);
-            return -1;
-        }
         const uint32_t nq = left < (uint32_t)qt ? left : (uint32_t)qt;
         if (with_simt_kernel<true>(a, vec, qt, [&](auto kern, auto params) -> int {
+                if (!smem_fits(di, reinterpret_cast<const void *>(kern), smem)) {
+                    set_error("dim=%u too large for the SIMT scan (needs %zu B shared memory)", a.dim, smem);
+                    return -1;
+                }
                 if (simt_ensure(reinterpret_cast<const void *>(kern), di.device_id, smem)) return -1;
                 const int occ = simt_occupancy(reinterpret_cast<const void *>(kern), di.device_id, smem);
                 uint32_t grid = (uint32_t)di.num_sms * (uint32_t)occ;

@@ -520,6 +520,7 @@ constexpr int FINISH_THREADS = 1024;  // one CTA per query has an SM to itself: 
 constexpr int FINISH_CAP = 4096;
 constexpr int FINISH_WIN = FINISH_CAP - 256;  // list entries per round; the carried best k (<= 192) fits in the rest
 constexpr int FINISH_HI = 16384;              // score words of the list cached in shared memory (longer lists: read from L2)
+constexpr int FINISH_HI_SMALL = 8192;         // the same for query rows too long to fit beside FINISH_HI (make_filter_plan)
 constexpr uint32_t ORD_POS_INF = 0xFF800000u;  // ord_bits(+inf): the bound of a row whose score is undecidable (NaN)
 struct FinishParams {
     const void *rows;        // corpus shard (fp32, or fp16 for the fp16 tensor path)
@@ -550,12 +551,14 @@ struct FinishParams {
 //   [0] entry  [1] list cached  [2] k-th bound selected  [3] survivors gathered  [4] re-scored  [5] ranked  [6] exit  [7] list length
 __device__ unsigned long long g_fin_prof[256][8];
 
+// HI: score words of the list cached in shared memory (FINISH_HI, or FINISH_HI_SMALL where the query row needs the room)
+template <int HI>
 __global__ void __launch_bounds__(FINISH_THREADS) filter_finish_kernel(FinishParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
-    uint32_t *shi = reinterpret_cast<uint32_t *>(smem_raw);                                   // FINISH_HI score words of the list
-    uint64_t *sb = reinterpret_cast<uint64_t *>(smem_raw + FINISH_HI * 4);                    // FINISH_CAP bound keys
-    uint64_t *se = reinterpret_cast<uint64_t *>(smem_raw + FINISH_HI * 4 + FINISH_CAP * 8);   // FINISH_CAP exact keys
-    float *qs = reinterpret_cast<float *>(smem_raw + FINISH_HI * 4 + FINISH_CAP * 16);        // query
+    uint32_t *shi = reinterpret_cast<uint32_t *>(smem_raw);                            // HI score words of the list
+    uint64_t *sb = reinterpret_cast<uint64_t *>(smem_raw + HI * 4);                    // FINISH_CAP bound keys
+    uint64_t *se = reinterpret_cast<uint64_t *>(smem_raw + HI * 4 + FINISH_CAP * 8);   // FINISH_CAP exact keys
+    float *qs = reinterpret_cast<float *>(smem_raw + HI * 4 + FINISH_CAP * 16);        // query
     __shared__ float s_qq;
     __shared__ int s_count, s_last;
     pdl_trigger();
@@ -573,7 +576,7 @@ __global__ void __launch_bounds__(FINISH_THREADS) filter_finish_kernel(FinishPar
     // ONE pass over the list (L2): the score words go to shared memory — every selection pass below reads them from there
     // (the list was read five times from L2, each time a chain of dependent ~1 us loads: that, not the arithmetic, was the
     // finish step's cost).  Four independent loads per thread per iteration.
-    const bool cached = n <= FINISH_HI;
+    const bool cached = n <= HI;
     uint32_t umax = 0u, umin = 0xffffffffu;
     int ninf = 0;
     for (int i0 = tid; i0 < n; i0 += 4 * FINISH_THREADS) {
@@ -861,6 +864,31 @@ int tc_ensure_smem(const void *func, int device, size_t smem) {
     return 0;
 }
 
+// the prep kernel's dynamic shared memory: the query row (padded to float4) and the threshold sample's keys
+static size_t prep_smem_bytes(uint32_t dim, uint32_t sample) { return (size_t)((dim + 3) & ~3u) * 4 + (size_t)sample * 8; }
+
+size_t kernel_static_smem(const void *func) {
+    static std::mutex mu;
+    static std::map<const void *, size_t> known;
+    std::lock_guard<std::mutex> lk(mu);
+    auto it = known.find(func);
+    if (it != known.end()) return it->second;
+    cudaFuncAttributes fa{};
+    if (cudaFuncGetAttributes(&fa, func) != cudaSuccess) {
+        cudaGetLastError();
+        return (size_t)1 << 40;  // unknown (not cached): nothing fits
+    }
+    return known[func] = fa.sharedSizeBytes + SMEM_RESERVED;
+}
+bool smem_fits(const DeviceInfo &di, const void *func, size_t dyn) { return dyn + kernel_static_smem(func) <= di.max_smem_optin; }
+int ensure_smem(const DeviceInfo &di, const void *func, size_t dyn, const char *what, uint32_t dim) {
+    if (!smem_fits(di, func, dyn)) {
+        set_error("%s: dim=%u needs %zu B shared memory (> %zu)", what, dim, dyn + kernel_static_smem(func), di.max_smem_optin);
+        return -1;
+    }
+    return dyn + kernel_static_smem(func) > 48 * 1024 ? tc_ensure_smem(func, di.device_id, dyn) : 0;
+}
+
 static bool tc_common_ok(const DeviceInfo &di, const ScanArgs &a) {
     if (di.cc < 90) return false;
     if (a.dtype != NK_DTYPE_F32) return false;                      // fp16 / bf16 corpus: 16-bit tensor pass or CUDA cores
@@ -869,15 +897,38 @@ static bool tc_common_ok(const DeviceInfo &di, const ScanArgs &a) {
     if (a.n == 0 || a.k == 0) return false;
     return true;
 }
-// exact (3xTF32) mode: cosine / dot, k <= 255 (register-resident prune over a 512-slot buffer)
+// exact (3xTF32) mode: cosine / dot, k <= 255 (register-resident prune over a 512-slot buffer), d <= TENSOR_EXACT_MAX_DIM:
+// its scores fall below fp64 by about 3e-9 d |x||q| (the dropped lo*lo products and the MMA's truncating fp32 adds),
+// 1e-4 of a score of 0.4 |x||q| at d = 12288 (tests/test_gpu_dims.py); larger d take the CUDA-core scan
 bool scan_tensor_supported(const DeviceInfo &di, const ScanArgs &a) {
-    return tc_common_ok(di, a) && a.metric != NK_METRIC_EUCLIDEAN && a.k + tc::ROWS + 1 <= (uint32_t)tc::P;
+    return tc_common_ok(di, a) && a.metric != NK_METRIC_EUCLIDEAN && a.k + tc::ROWS + 1 <= (uint32_t)tc::P &&
+           a.dim <= TENSOR_EXACT_MAX_DIM &&
+           smem_fits(di, reinterpret_cast<const void *>(filter_prep_kernel<false, false>), prep_smem_bytes(a.dim, 0));
 }
+// The finish launch of a filter search over rows of `dim` elements: the FINISH_HI window wherever its dynamic shared
+// memory (cached score words, bound and exact keys, the query row) fits the device's opt-in limit beside the kernel's
+// static shared memory, else the FINISH_HI_SMALL window (lists longer than the window are read from L2).  kern == nullptr:
+// neither fits.  The planner (scan_tensor_filter_supported) and the launch (make_filter_plan) both ask here.
+struct FinishLaunch {
+    void (*kern)(FinishParams);
+    size_t smem;
+};
+static size_t finish_dyn_smem(int hi, uint32_t dim) { return (size_t)hi * 4 + (size_t)FINISH_CAP * 16 + (size_t)dim * 4; }
+static FinishLaunch finish_launch(const DeviceInfo &di, uint32_t dim) {
+    if (smem_fits(di, reinterpret_cast<const void *>(filter_finish_kernel<FINISH_HI>), finish_dyn_smem(FINISH_HI, dim)))
+        return {filter_finish_kernel<FINISH_HI>, finish_dyn_smem(FINISH_HI, dim)};
+    if (smem_fits(di, reinterpret_cast<const void *>(filter_finish_kernel<FINISH_HI_SMALL>), finish_dyn_smem(FINISH_HI_SMALL, dim)))
+        return {filter_finish_kernel<FINISH_HI_SMALL>, finish_dyn_smem(FINISH_HI_SMALL, dim)};
+    return {nullptr, 0};
+}
+
 // filter mode (1xTF32 over fp32 rows, or the 16-bit pass over a shadow / a 16-bit corpus) + exact rescoring: all three
-// metrics, k <= 192
+// metrics, k <= 192, d <= FILTER_MAX_DIM (the int8 image's exact integer accumulation, DESIGN §3.3) and a query row that
+// fits the finish kernel's shared memory on this device
 bool scan_tensor_filter_supported(const DeviceInfo &di, const ScanArgs &a) {
-    if (a.k > 192 || a.dim > 32768) return false;  // finish kernel keeps the query in shared memory
-    return tc_common_ok(di, a) || shadow_pass_supported(di, a);
+    if (a.k > 192 || a.dim > FILTER_MAX_DIM) return false;
+    if (!(tc_common_ok(di, a) || shadow_pass_supported(di, a))) return false;
+    return finish_launch(di, a.dim).kern != nullptr;
 }
 
 int tc_debug_flags() { return tc_env_int("NK_TC_DEBUG", 0); }
@@ -927,10 +978,10 @@ PrepParams prep_params(const ScanArgs &a, uint32_t Qpad, uint32_t dimpad) {
 }
 
 int launch_prep(const DeviceInfo &di, ScanMode mode, const PrepParams &pp, cudaStream_t stream, uint64_t *launches) {
-    const size_t smem = (size_t)((pp.dim + 3) & ~3u) * 4 + (size_t)pp.sample * 8;
+    const size_t smem = prep_smem_bytes(pp.dim, pp.sample);
     void (*kern)(PrepParams) = mode_window(mode) ? filter_prep_kernel<true, true>
                                : mode_tags(mode) ? filter_prep_kernel<true, false> : filter_prep_kernel<false, false>;
-    if (smem > 48 * 1024 && tc_ensure_smem(reinterpret_cast<const void *>(kern), di.device_id, smem)) return -1;
+    if (ensure_smem(di, reinterpret_cast<const void *>(kern), smem, "query prep", pp.dim)) return -1;
     kern<<<pp.Qpad, PREP_THREADS, smem, stream>>>(pp);
     NK_CUDA_OK(cudaGetLastError());
     if (launches) ++*launches;
@@ -1024,7 +1075,7 @@ struct FilterPlan {
     float *qhi, *qlo, *qnorm, *qa, *qb, *qscale;
     void *qbf16;        // the queries in the image's element type: bf16 / fp16, or int8 (with qscale) for an int8 image
     uint32_t max_groups_shadow;
-    size_t fsmem;
+    FinishLaunch finish;
     // the fields every 16-bit / int8 pass of the plan shares; the caller sets the query range and the mode
     ShadowPassArgs shadow_pass() const {
         ShadowPassArgs sp{};
@@ -1083,8 +1134,12 @@ static int make_filter_plan(const DeviceInfo &di, const ScanArgs &a, Workspace &
         if (f.sample < 128) f.sample = 128;
         if (f.sample > 2048) f.sample = 2048;
     }
-    f.fsmem = (size_t)FINISH_HI * 4 + (size_t)FINISH_CAP * 16 + (size_t)a.dim * 4;
-    if (tc_ensure_smem(reinterpret_cast<const void *>(filter_finish_kernel), di.device_id, f.fsmem)) return -1;
+    f.finish = finish_launch(di, a.dim);
+    if (!f.finish.kern) {
+        set_error("filter finish: dim=%u needs more shared memory than the device allows (%zu B)", a.dim, di.max_smem_optin);
+        return -1;
+    }
+    if (tc_ensure_smem(reinterpret_cast<const void *>(f.finish.kern), di.device_id, f.finish.smem)) return -1;
     return 0;
 }
 
@@ -1176,7 +1231,7 @@ int scan_tensor_filter_tail(const DeviceInfo &di, const ScanArgs &a, Workspace &
         FinishParams fp{};
         fill_finish(fp, a, ws, f, out_keys);
         fp.q_big = 0; fp.only_if = ws.flags + FLAG_RETRY; fp.mark_retry = 0;
-        NK_CUDA_OK(launch_pdl(filter_finish_kernel, dim3(a.Q), dim3(FINISH_THREADS), f.fsmem, a.stream, !a.defer_tail, fp));
+        NK_CUDA_OK(launch_pdl(f.finish.kern, dim3(a.Q), dim3(FINISH_THREADS), f.finish.smem, a.stream, !a.defer_tail, fp));
         if (launches) ++*launches;
     }
     ScanArgs b = a;
@@ -1223,7 +1278,7 @@ int scan_tensor_filter(const DeviceInfo &di, const ScanArgs &a, Workspace &ws, u
     fill_finish(fp, a, ws, f, out_keys);
     fp.q_big = q_big; fp.only_if = nullptr; fp.mark_retry = (f.stage2 && a.defer_tail) ? 1 : 0;
     fp.debug = tc_debug_flags() & 64;
-    NK_CUDA_OK(launch_pdl(filter_finish_kernel, dim3(a.Q), dim3(FINISH_THREADS), f.fsmem, a.stream, !a.defer_tail, fp));
+    NK_CUDA_OK(launch_pdl(f.finish.kern, dim3(a.Q), dim3(FINISH_THREADS), f.finish.smem, a.stream, !a.defer_tail, fp));
     if (launches) ++*launches;
     tc_print_prof(a.stream, f.num_tiles, f.grid, (a.dim + BK - 1) / BK);
     fin_print_prof(a.stream, a.Q);

@@ -643,7 +643,7 @@ static void sb_print_prof(cudaStream_t stream, uint32_t grid) {
 // The 16-bit / int8 pass needs an image of the rows (a.image): the BF16 shadow or the int8 image of an fp32 shard, or —
 // fp16 / bf16 corpora — the rows themselves (no rounding residue on the row side, only the per-row |x|^2 array).
 bool shadow_pass_supported(const DeviceInfo &di, const ScanArgs &a) {
-    if (di.cc < 90 || a.image.kind == RowImage::NONE || a.image.xnorm2 == nullptr || a.k > 192 || a.dim > 32768 || a.dim < 32 || a.n == 0)
+    if (di.cc < 90 || a.image.kind == RowImage::NONE || a.image.xnorm2 == nullptr || a.k > 192 || a.dim > FILTER_MAX_DIM || a.dim < 32 || a.n == 0)
         return false;
     if ((reinterpret_cast<uintptr_t>(a.rows) & 15) != 0 || (reinterpret_cast<uintptr_t>(a.image.data) & 15) != 0) return false;
     if (a.dtype == NK_DTYPE_F32) return a.dim % 4 == 0;

@@ -581,7 +581,6 @@ __device__ __forceinline__ float bf16_margin2(int metric, float max_ra, float ma
 // map_dtype (2-byte elements only): NK_DTYPE_F16 -> fp16 tensor, anything else -> bf16.
 int tc_make_map(CUtensorMap *m, const void *base, uint64_t rows, uint32_t cols, uint32_t elem_bytes, uint32_t box_cols,
                 uint32_t box_rows, uint64_t row_stride_bytes, int map_dtype = 0);
-int tc_ensure_smem(const void *func, int device, size_t smem);
 int tc_debug_flags();
 
 // Cached tensor map: cuTensorMapEncodeTiled runs only when (base, shape, box) changed since the last search.
