@@ -385,18 +385,27 @@ static NkShard *find_shard(NkIndex *ix, uint64_t row, uint64_t *local) {
     return nullptr;
 }
 
-// The scan of Q device queries over shard s as it stands: its rows, the row mask and the score floor; qfilter (per-query tag
-// filters [Q] on the device, nullptr = none) needs the shard's tag array on; qwindow (per-query value windows [Q] on the
-// device, nullptr = none) needs qfilter and the shard's value array on.
-static nk::ScanArgs shard_scan_args(const NkIndex *ix, const NkShard &s, const float *q_dev, uint32_t Q, uint32_t k,
-                                    cudaStream_t stream, const NkFilter *qfilter = nullptr, const NkWindow *qwindow = nullptr) {
+// The plain kNN scan (ScanMode::KNN) of Q device queries over shard s as it stands: its rows, the row mask and the score floor.
+static nk::ScanArgs shard_scan_args(const NkIndex *ix, const NkShard &s, const float *q_dev, uint32_t Q, uint32_t k, cudaStream_t stream) {
     nk::ScanArgs a;
     a.rows = s.rows; a.dtype = ix->dtype; a.n = (uint32_t)s.n; a.dim = ix->dim; a.row_base = s.base;
     a.queries = q_dev; a.Q = Q; a.k = k; a.metric = ix->metric; a.stream = stream;
     a.row_mask = s.mask_on ? s.mask : nullptr; a.min_score = ix->key_floor();
-    if (qfilter) { a.row_tags = s.tags; a.qfilter = qfilter; a.mode = nk::ScanMode::KNN_TAGS; }
-    if (qwindow) { a.row_values = s.values; a.qwindow = qwindow; a.mode = nk::ScanMode::KNN_WINDOW; }
     return a;
+}
+
+// Give *a mode m and what m reads on shard s: the shard's tag and value arrays (turned on by whoever staged the predicates); the
+// per-query filters and windows staged in the workspace (stage_predicates), or the caller's own device arrays qfilter /
+// qwindow where given (the device API); and for the reverse modes each row's threshold with the keep mask behind them, which
+// takes the place of the row mask, each row's own filter and window and the queries' tags and value keys (graph_reverse_scan).
+static void set_scan_mode(const NkShard &s, nk::ScanMode m, nk::ScanArgs *a, const NkFilter *qfilter = nullptr,
+                          const NkWindow *qwindow = nullptr) {
+    a->mode = m;
+    if (nk::mode_tags(m)) { a->row_tags = s.tags; a->qfilter = qfilter ? qfilter : s.ws.qfilter; }
+    if (nk::mode_window(m)) { a->row_values = s.values; a->qwindow = qwindow ? qwindow : s.ws.qwindow; }
+    if (nk::mode_row_thr(m)) { a->row_thr = s.ws.row_thr; a->row_mask = reinterpret_cast<const uint32_t *>(s.ws.row_thr + s.n); }
+    if (nk::mode_row_filter(m)) { a->row_filter = s.ws.row_filter; a->qtags = s.ws.qtags; }
+    if (nk::mode_row_window(m)) { a->row_window = s.ws.row_window; a->qvalues = s.ws.qvalues; }
 }
 
 // Has a search on the shard's int8 image overflowed its margin buffers since the last look?  Reads the counters copied
@@ -545,18 +554,20 @@ struct DeferredTail {
 };
 
 struct ScanOut {  // what a call asks of run_scan beyond the queries
-    explicit ScanOut(int path) : path(path) {}
+    explicit ScanOut(int path, nk::ScanMode mode = nk::ScanMode::KNN) : path(path), mode(mode) {}
     int path;                      // the scan path of the call (plan_path)
+    nk::ScanMode mode;             // KNN, KNN_TAGS or KNN_WINDOW (set_scan_mode)
     uint32_t *out_idx = nullptr;   // fused decode (single-shard searches)
     float *out_score = nullptr;
     DeferredTail *tail = nullptr;  // host-synchronous caller: retry stages are left to *tail, queued only if a flag was raised
-    const NkFilter *qfilter = nullptr;  // per-query tag filters [Q] (device; the shard's tag array must be on)
-    const NkWindow *qwindow = nullptr;  // per-query value windows [Q] (device; with qfilter, the shard's value array on)
+    const NkFilter *qfilter = nullptr;  // the device API's own per-query filters / windows [Q]; nullptr: the workspace's
+    const NkWindow *qwindow = nullptr;
 };
 
 static int run_scan(NkIndex *ix, NkShard &s, const float *q_dev, uint32_t Q, uint32_t k, uint64_t *out_keys,
                     cudaStream_t stream, const ScanOut &xo) {
-    nk::ScanArgs a = shard_scan_args(ix, s, q_dev, Q, k, stream, xo.qfilter, xo.qwindow);
+    nk::ScanArgs a = shard_scan_args(ix, s, q_dev, Q, k, stream);
+    set_scan_mode(s, xo.mode, &a, xo.qfilter, xo.qwindow);
     if (k > NK_MAX_K) {
         if (run_scan_bigk(ix, s, a, out_keys)) return -1;
         if (xo.out_idx) {
@@ -1176,36 +1187,35 @@ int nk_index_read_rows(NkIndex *ix, uint64_t row, uint64_t n_rows, void *rows_ho
 // Writes the Q fp32 queries of a search into s.ws.queries (already reserved) on s.stream; the device is s's.
 using StageQueries = std::function<int(NkShard &)>;
 
-// Per-query tag filters of a host search -> the shard workspace, next to the queries (the deferred retry tail reads them
-// after the call's first synchronisation), with the shard's tag array on.  The device copy, or nullptr on error.
-static const NkFilter *stage_filters(NkIndex *ix, NkShard &s, const NkFilter *filters_host, uint32_t Q) {
-    const size_t fbytes = (size_t)Q * sizeof(NkFilter);
-    if (shard_tags_on(s)) return nullptr;
-    if (nk::ws_reserve((void **)&s.ws.qfilter, &s.ws.qfilter_bytes, fbytes)) return nullptr;
-    NK_CUDA_OK_PTR(cudaMemcpyAsync(s.ws.qfilter, filters_host, fbytes, cudaMemcpyHostToDevice, s.stream));
-    ix->stats.bytes_h2d += fbytes;
-    return s.ws.qfilter;
+// n tag filters -> a grow-only device array *dev, on `stream`: filters_host [n], or with filters_host nullptr {0,0,0}, which
+// admit every tag (a window scan is also a tag scan, and a windowed graph's row filters are those of a graph without filters).
+static int put_filters(NkIndex *ix, NkFilter **dev, size_t *dev_bytes, const NkFilter *filters_host, uint64_t n, cudaStream_t stream) {
+    const size_t bytes = n * sizeof(NkFilter);
+    if (nk::ws_reserve((void **)dev, dev_bytes, bytes)) return -1;
+    if (!filters_host) {
+        NK_CUDA_OK(cudaMemsetAsync(*dev, 0, bytes, stream));
+        return 0;
+    }
+    NK_CUDA_OK(cudaMemcpyAsync(*dev, filters_host, bytes, cudaMemcpyHostToDevice, stream));
+    ix->stats.bytes_h2d += bytes;
+    return 0;
 }
 
-// Per-query value windows of a host search -> the shard workspace next to its filters, with the shard's tag and value arrays
-// on.  A windowed scan always applies a tag filter as well: without filters_host the filters staged are {0,0,0}, which admit
-// every row.  *qfilter / *qwindow: the device copies.
-static int stage_windows(NkIndex *ix, NkShard &s, const NkFilter *filters_host, const NkWindow *windows_host, uint32_t Q,
-                         const NkFilter **qfilter, const NkWindow **qwindow) {
-    if (filters_host) {
-        if (!(*qfilter = stage_filters(ix, s, filters_host, Q))) return -1;
-    } else {
-        if (shard_tags_on(s)) return -1;
-        if (nk::ws_reserve((void **)&s.ws.qfilter, &s.ws.qfilter_bytes, (size_t)Q * sizeof(NkFilter))) return -1;
-        NK_CUDA_OK(cudaMemsetAsync(s.ws.qfilter, 0, (size_t)Q * sizeof(NkFilter), s.stream));
-        *qfilter = s.ws.qfilter;
-    }
-    const size_t wbytes = (size_t)Q * sizeof(NkWindow);
+// The per-query predicates a scan in mode m reads, for Q queries -> shard s's workspace, on `stream`, next to the queries (the
+// deferred retry tail reads them after the call's first synchronisation): under a tag mode the shard's tag array on and the
+// filters in s.ws.qfilter (put_filters: filters_host, or {0,0,0}); under a window mode also the shard's value array on and
+// windows_host in s.ws.qwindow (nullptr: the windows are written on the device, or the caller passes its own).
+static int stage_predicates(NkIndex *ix, NkShard &s, cudaStream_t stream, nk::ScanMode m, uint32_t Q, const NkFilter *filters_host,
+                            const NkWindow *windows_host) {
+    if (!nk::mode_tags(m)) return 0;
+    if (shard_tags_on(s) || put_filters(ix, &s.ws.qfilter, &s.ws.qfilter_bytes, filters_host, Q, stream)) return -1;
+    if (!nk::mode_window(m)) return 0;
     if (shard_values_on(s)) return -1;
+    if (!windows_host) return 0;
+    const size_t wbytes = (size_t)Q * sizeof(NkWindow);
     if (nk::ws_reserve((void **)&s.ws.qwindow, &s.ws.qwindow_bytes, wbytes)) return -1;
-    NK_CUDA_OK(cudaMemcpyAsync(s.ws.qwindow, windows_host, wbytes, cudaMemcpyHostToDevice, s.stream));
+    NK_CUDA_OK(cudaMemcpyAsync(s.ws.qwindow, windows_host, wbytes, cudaMemcpyHostToDevice, stream));
     ix->stats.bytes_h2d += wbytes;
-    *qwindow = s.ws.qwindow;
     return 0;
 }
 
@@ -1222,6 +1232,7 @@ struct SearchOpts {
 static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const StageQueries &stage, const SearchOpts &opts, uint32_t Q,
                        uint32_t ke, uint32_t k, uint32_t *out_idx, float *out_score) {
     const size_t qbytes = (size_t)Q * ix->dim * sizeof(float);
+    const nk::ScanMode mode = opts.windows_host ? nk::ScanMode::KNN_WINDOW : opts.filters_host ? nk::ScanMode::KNN_TAGS : nk::ScanMode::KNN;
     const bool single = live.size() == 1;
     // one deferred tail per shard; a single shard's lives on the stack, so that search allocates nothing
     DeferredTail tail0;
@@ -1235,19 +1246,14 @@ static int search_live(NkIndex *ix, const std::vector<NkShard *> &live, const St
         NK_CUDA_OK(cudaSetDevice(s->device));
         if (nk::ws_reserve((void **)&s->ws.queries, &s->ws.queries_bytes, qbytes)) return -1;
         if (nk::ws_reserve((void **)&s->ws.keys, &s->ws.keys_bytes, (size_t)Q * ke * 8)) return -1;
-        ScanOut xo(opts.path);
+        ScanOut xo(opts.path, mode);
         xo.tail = tail_of(i);
         if (single) {
             if (nk::ws_reserve((void **)&s->ws.out_idx, &s->ws.out_idx_bytes, (size_t)Q * ke * 4)) return -1;
             if (nk::ws_reserve((void **)&s->ws.out_score, &s->ws.out_score_bytes, (size_t)Q * ke * 4)) return -1;
             xo.out_idx = s->ws.out_idx; xo.out_score = s->ws.out_score;
         }
-        if (stage(*s)) return -1;
-        if (opts.windows_host) {
-            if (stage_windows(ix, *s, opts.filters_host, opts.windows_host, Q, &xo.qfilter, &xo.qwindow)) return -1;
-        } else if (opts.filters_host && !(xo.qfilter = stage_filters(ix, *s, opts.filters_host, Q))) {
-            return -1;
-        }
+        if (stage(*s) || stage_predicates(ix, *s, s->stream, mode, Q, opts.filters_host, opts.windows_host)) return -1;
         if (run_scan(ix, *s, s->ws.queries, Q, ke, s->ws.keys, s->stream, xo)) return -1;
     }
 
@@ -1370,50 +1376,72 @@ int nk_search_windowed(NkIndex *ix, const float *queries_host, const NkFilter *f
 // whatever Q is, the whole index included; one host synchronisation per block.
 constexpr uint32_t SEARCH_ROWS_BLOCK = 1024;
 
-// The queries of a block of stored rows ids[nb] (relative to the index's first row), each read and widened to fp32 on the
-// device that holds it.  *stage then writes the block into s.ws.queries (reserved by the caller) of any shard the search runs
-// on.  With one live shard only the ids cross PCIe and the rows are gathered straight into the query block; otherwise each
-// owner gathers its rows now, the block is assembled in pinned host memory and *stage sends it.  admit (nk_search_pairs):
-// *stage also writes the per-query filters into s.ws.qfilter, with the shard's tag array on: admit->f for a row that passes the
-// row mask and admit->f, the filter that admits no row otherwise, decided on the row's own device.  admit->windowed
-// (nk_search_pairs_windowed): each row's window (nk::row_windows) goes into s.ws.qwindow instead, with the shard's value array
-// on, and decides the row's admission alone (mask, filter, window and band: a refused row gets the window that admits no
-// row), so every query's filter is admit->f and row_filters does not run.
+// What stage_row_block writes beside a block of stored-row queries, by the mode of the scan they run in.  Under a tag mode
+// (the self-join's and the reverse scan's range modes) each query's filter goes into s.ws.qfilter, with the shard's tag array
+// on: f for a row that passes the row mask and f (nk::row_filters), the filter that admits no row otherwise, decided on the
+// row's own device.  Under a window mode (a windowed self-join: a window w, a band gap or both) each row's window
+// (nk::row_windows) goes into s.ws.qwindow instead, with the shard's value array on, and decides the row's admission alone
+// (mask, filter, window and band: a refused row gets the window that admits no row), so every query's filter is f and
+// row_filters does not run.  The other modes (KNN, RANGE, REVERSE) write nothing beside the queries.
 struct RowAdmit {
+    nk::ScanMode mode = nk::ScanMode::KNN;
     NkFilter f{0, 0, 0};
-    bool windowed = false;
     NkWindow w{0, ~0ull};
     uint64_t gap = NK_NO_GAP;
 };
-static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, const uint32_t *ids, uint32_t nb, const RowAdmit *admit,
+
+// The admission of a self-join's left rows (nk_search_pairs_windowed, nk_search_pairs_rows_windowed): the call's filter, window and
+// band and the index's row mask, and the range mode the join scans in.
+static RowAdmit join_admit(const NkIndex *ix, const NkFilter *filter, const NkWindow *window, uint64_t max_gap) {
+    RowAdmit adm;
+    adm.mode = window || max_gap != NK_NO_GAP ? nk::ScanMode::RANGE_WINDOW
+               : filter || ix->mask_on        ? nk::ScanMode::RANGE_TAGS  // some left rows may be inadmissible: per-query filters
+                                              : nk::ScanMode::RANGE;
+    if (filter) adm.f = *filter;
+    if (window) adm.w = *window;
+    adm.gap = max_gap;
+    return adm;
+}
+
+// The admission (RowAdmit, a tag or window mode) of m rows of shard o, their local ids in o.ws.sub_rows: one launch on o's
+// stream, into o.ws.qwindow (nk::row_windows) under a window mode, else into o.ws.qfilter (nk::row_filters).
+static int admit_rows(NkIndex *ix, NkShard &o, uint32_t m, const RowAdmit &adm) {
+    const uint32_t *mask = o.mask_on ? o.mask : nullptr;
+    const uint64_t *tags = o.tags_on ? o.tags : nullptr;
+    if (nk::mode_window(adm.mode)) {
+        if (nk::ws_reserve((void **)&o.ws.qwindow, &o.ws.qwindow_bytes, (size_t)m * sizeof(NkWindow))) return -1;
+        if (nk::row_windows(o.ws.sub_rows, m, mask, tags, o.values_on ? o.values : nullptr, adm.f, adm.w, adm.gap, o.ws.qwindow, o.stream))
+            return -1;
+    } else {
+        if (nk::ws_reserve((void **)&o.ws.qfilter, &o.ws.qfilter_bytes, (size_t)m * sizeof(NkFilter))) return -1;
+        if (nk::row_filters(o.ws.sub_rows, m, mask, tags, adm.f, o.ws.qfilter, o.stream)) return -1;
+    }
+    ix->stats.kernel_launches++;
+    return 0;
+}
+
+// The queries of a block of stored rows ids[nb] (relative to the index's first row), each read and widened to fp32 on the
+// device that holds it, and their admission under adm.  *stage then writes the block into s.ws.queries (reserved by the
+// caller) of any shard the search runs on, the admission beside it.  With one live shard only the ids cross PCIe, the rows
+// are gathered straight into the query block and the admission is written in place; otherwise each owner gathers its rows and
+// admits them now, the block is assembled in pinned host memory and *stage sends it.
+static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, const uint32_t *ids, uint32_t nb, const RowAdmit &adm,
                            StageQueries *stage) {
     const size_t rb = (size_t)ix->dim * sizeof(float);
+    const bool admit = nk::mode_tags(adm.mode), win = nk::mode_window(adm.mode);
     std::vector<uint32_t> local(nb);
     if (live.size() == 1) {
-        const bool filt = admit != nullptr;
-        const RowAdmit a = filt ? *admit : RowAdmit{};
-        const NkFilter f = a.f;
-        std::vector<NkFilter> every(a.windowed ? nb : 0, f);  // a windowed block's filters: f for every query
-        *stage = [ix, ids, nb, local, filt, f, a, every](NkShard &s) mutable {
+        std::vector<NkFilter> every(win ? nb : 0, adm.f);  // a windowed block's filters: f for every query
+        *stage = [ix, ids, nb, local, adm, admit, win, every](NkShard &s) mutable {
             for (uint32_t q = 0; q < nb; ++q) local[q] = ids[q] - (uint32_t)ix->first_row(s);
             if (nk::ws_reserve((void **)&s.ws.sub_rows, &s.ws.sub_rows_bytes, (size_t)nb * 4)) return -1;
             NK_CUDA_OK(cudaMemcpyAsync(s.ws.sub_rows, local.data(), (size_t)nb * 4, cudaMemcpyHostToDevice, s.stream));
             if (nk::gather_rows(s.rows, ix->dtype, ix->dim, s.ws.sub_rows, nb, s.ws.queries, true, s.stream)) return -1;
             ix->stats.bytes_h2d += (uint64_t)nb * 4;
             ix->stats.kernel_launches++;
-            if (a.windowed) {
-                if (!stage_filters(ix, s, every.data(), nb) || shard_values_on(s)) return -1;
-                if (nk::ws_reserve((void **)&s.ws.qwindow, &s.ws.qwindow_bytes, (size_t)nb * sizeof(NkWindow))) return -1;
-                if (nk::row_windows(s.ws.sub_rows, nb, s.mask_on ? s.mask : nullptr, s.tags, s.values, f, a.w, a.gap, s.ws.qwindow, s.stream))
-                    return -1;
-                ix->stats.kernel_launches++;
-            } else if (filt) {
-                if (shard_tags_on(s)) return -1;
-                if (nk::ws_reserve((void **)&s.ws.qfilter, &s.ws.qfilter_bytes, (size_t)nb * sizeof(NkFilter))) return -1;
-                if (nk::row_filters(s.ws.sub_rows, nb, s.mask_on ? s.mask : nullptr, s.tags, f, s.ws.qfilter, s.stream)) return -1;
-                ix->stats.kernel_launches++;
-            }
-            return 0;
+            if (!admit) return 0;
+            if (win ? stage_predicates(ix, s, s.stream, adm.mode, nb, every.data(), nullptr) : shard_tags_on(s)) return -1;
+            return admit_rows(ix, s, nb, adm);
         };
         return 0;
     }
@@ -1421,8 +1449,7 @@ static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, cons
     if (pinned_reserve((void **)&ix->h_qrows, &ix->h_qrows_bytes, 2 * nb * rb)) return -1;
     float *blk = ix->h_qrows, *part = ix->h_qrows + (size_t)nb * ix->dim;
     std::vector<uint32_t> pos(nb);
-    const bool win = admit && admit->windowed;
-    std::vector<NkFilter> filters(admit ? nb : 0, win ? admit->f : NkFilter{0, 0, 0}), part_f(admit && !win ? nb : 0);
+    std::vector<NkFilter> filters(admit ? nb : 0, adm.f), part_f(admit && !win ? nb : 0);
     std::vector<NkWindow> windows(win ? nb : 0), part_w(win ? nb : 0);
     for (NkShard *o : live) {
         uint32_t m = 0;
@@ -1437,23 +1464,11 @@ static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, cons
         NK_CUDA_OK(cudaMemcpyAsync(o->ws.sub_rows, local.data(), (size_t)m * 4, cudaMemcpyHostToDevice, o->stream));
         if (nk::gather_rows(o->rows, ix->dtype, ix->dim, o->ws.sub_rows, m, o->ws.sub_gather, true, o->stream)) return -1;
         NK_CUDA_OK(cudaMemcpyAsync(part, o->ws.sub_gather, (size_t)m * rb, cudaMemcpyDeviceToHost, o->stream));
-        if (admit && !win) {  // the owner's qfilter slot is free until the scan stages its own filters
-            if (nk::ws_reserve((void **)&o->ws.qfilter, &o->ws.qfilter_bytes, (size_t)m * sizeof(NkFilter))) return -1;
-            if (nk::row_filters(o->ws.sub_rows, m, o->mask_on ? o->mask : nullptr, o->tags_on ? o->tags : nullptr, admit->f, o->ws.qfilter,
-                                o->stream))
-                return -1;
-            NK_CUDA_OK(cudaMemcpyAsync(part_f.data(), o->ws.qfilter, (size_t)m * sizeof(NkFilter), cudaMemcpyDeviceToHost, o->stream));
-            ix->stats.kernel_launches++;
-            ix->stats.bytes_d2h += (uint64_t)m * sizeof(NkFilter);
-        }
-        if (win) {  // ... and so is its qwindow slot
-            if (nk::ws_reserve((void **)&o->ws.qwindow, &o->ws.qwindow_bytes, (size_t)m * sizeof(NkWindow))) return -1;
-            if (nk::row_windows(o->ws.sub_rows, m, o->mask_on ? o->mask : nullptr, o->tags_on ? o->tags : nullptr,
-                                o->values_on ? o->values : nullptr, admit->f, admit->w, admit->gap, o->ws.qwindow, o->stream))
-                return -1;
-            NK_CUDA_OK(cudaMemcpyAsync(part_w.data(), o->ws.qwindow, (size_t)m * sizeof(NkWindow), cudaMemcpyDeviceToHost, o->stream));
-            ix->stats.kernel_launches++;
-            ix->stats.bytes_d2h += (uint64_t)m * sizeof(NkWindow);
+        if (admit) {  // the owner's qfilter / qwindow slot is free until the scan stages its own
+            if (admit_rows(ix, *o, m, adm)) return -1;
+            if (win) NK_CUDA_OK(cudaMemcpyAsync(part_w.data(), o->ws.qwindow, (size_t)m * sizeof(NkWindow), cudaMemcpyDeviceToHost, o->stream));
+            else NK_CUDA_OK(cudaMemcpyAsync(part_f.data(), o->ws.qfilter, (size_t)m * sizeof(NkFilter), cudaMemcpyDeviceToHost, o->stream));
+            ix->stats.bytes_d2h += (uint64_t)m * (win ? sizeof(NkWindow) : sizeof(NkFilter));
         }
         NK_CUDA_OK(cudaStreamSynchronize(o->stream));
         ix->stats.bytes_h2d += (uint64_t)m * 4;
@@ -1461,20 +1476,14 @@ static int stage_row_block(NkIndex *ix, const std::vector<NkShard *> &live, cons
         ix->stats.kernel_launches++;
         for (uint32_t i = 0; i < m; ++i) {
             memcpy(blk + (size_t)pos[i] * ix->dim, part + (size_t)i * ix->dim, rb);
-            if (admit && !win) filters[pos[i]] = part_f[i];
             if (win) windows[pos[i]] = part_w[i];
+            else if (admit) filters[pos[i]] = part_f[i];
         }
     }
-    *stage = [ix, blk, nb, rb, filters, windows](NkShard &s) {
+    *stage = [ix, blk, nb, rb, mode = adm.mode, filters, windows](NkShard &s) {
         NK_CUDA_OK(cudaMemcpyAsync(s.ws.queries, blk, (size_t)nb * rb, cudaMemcpyHostToDevice, s.stream));
         ix->stats.bytes_h2d += (uint64_t)nb * rb;
-        if (!windows.empty()) {
-            const NkFilter *qf;
-            const NkWindow *qw;
-            return stage_windows(ix, s, filters.data(), windows.data(), nb, &qf, &qw);
-        }
-        if (!filters.empty() && !stage_filters(ix, s, filters.data(), nb)) return -1;
-        return 0;
+        return stage_predicates(ix, s, s.stream, mode, nb, filters.data(), windows.data());
     };
     return 0;
 }
@@ -1493,7 +1502,7 @@ static int search_rows_locked(NkIndex *ix, const std::vector<NkShard *> &live, c
         const uint32_t nb = std::min(QB, Q - b);
         const uint32_t *ids = rows_host + b;
         StageQueries stage;
-        if (stage_row_block(ix, live, ids, nb, nullptr, &stage)) return -1;
+        if (stage_row_block(ix, live, ids, nb, RowAdmit{}, &stage)) return -1;
         const SearchOpts block{opts.path, opts.filters_host ? opts.filters_host + b : nullptr, opts.windows_host ? opts.windows_host + b : nullptr};
         if (search_live(ix, live, stage, block, nb, kk, kk, bidx.data(), bsc.data()) < 0) return -1;
         for (uint32_t q = 0; q < nb; ++q) {
@@ -1576,22 +1585,15 @@ static float range_key_threshold(const NkIndex *ix, float t) {
 }
 
 // One block of Q range queries as every shard it runs on scans it.  The queries are those the block's StageQueries wrote into
-// s.ws.queries; with `filtered` the same step wrote their per-query tag filters into s.ws.qfilter (stage_filters,
-// stage_row_block).
+// s.ws.queries; the same step wrote what the block's mode reads beside them (set_scan_mode: stage_predicates, stage_row_block,
+// and for the reverse scan of a k-NN graph update graph_reverse_scan, whose per-row thresholds and keep mask select the rows
+// whose lists are updated, not the rows that may be returned).
 struct RangeBlock {
     int path;                              // the scan path of the call (plan_path)
+    nk::ScanMode mode;                     // a range mode
     uint32_t Q;
     const uint32_t *thr;                   // [Q] thresholds in key space, as nk::ord_bits (host)
-    bool filtered = false;
-    bool windowed = false;                 // (with `filtered`) the same step wrote per-query value windows into s.ws.qwindow
     const uint64_t *pair_first = nullptr;  // the self-join's triangle: see range_scan_shard
-    // The reverse scan of a k-NN graph update.  Every row has its own threshold, s.ws.row_thr [s.n], and the mask words behind
-    // them, s.ws.row_thr + s.n, TAKE THE PLACE OF the index's row mask: they select the rows whose lists are updated, not the
-    // rows that may be returned.  row_filters (a filtered graph; `filtered` must be set too): a pair (row, query) is listed only
-    // if the row's own filter, s.ws.row_filter [s.n], admits the query's tag, s.ws.qtags [Q].  row_windows (a windowed graph;
-    // `row_filters` must be set too): ... and if the row's own window, s.ws.row_window [s.n], admits the query's value key,
-    // s.ws.qvalues [Q].
-    bool reverse = false, row_filters = false, row_windows = false;
     // The pairs incident to listed rows (nk_search_pairs_rows): s.ws.pair_rows holds one bit per row of the shard for the
     // listed rows, then the block's query rows (global ids); see nk::IncidentRows.
     bool incident = false;
@@ -1603,18 +1605,10 @@ struct RangeBlock {
 // on the base).
 static int range_shard(NkIndex *ix, NkShard &s, const RangeBlock &b, uint64_t from, int *counts, uint32_t *list_cap) {
     // Paths: the 16-bit and TF32 filters with fixed thresholds, or the CUDA-core scan.
-    nk::ScanArgs a = shard_scan_args(ix, s, s.ws.queries, b.Q, 1, s.stream, b.filtered ? s.ws.qfilter : nullptr, b.windowed ? s.ws.qwindow : nullptr);
+    nk::ScanArgs a = shard_scan_args(ix, s, s.ws.queries, b.Q, 1, s.stream);
+    set_scan_mode(s, b.mode, &a);
     const int use = plan_path(ix, s, b.path, true, &a);
     if (use < 0) return -1;
-    a.mode = b.windowed ? nk::ScanMode::RANGE_WINDOW : b.filtered ? nk::ScanMode::RANGE_TAGS : nk::ScanMode::RANGE;
-    if (b.reverse) {
-        a.mode = b.row_windows ? nk::ScanMode::REVERSE_RWINDOW
-                 : b.row_filters ? nk::ScanMode::REVERSE_RFILT : b.filtered ? nk::ScanMode::REVERSE_TAGS : nk::ScanMode::REVERSE;
-        a.row_thr = s.ws.row_thr;
-        a.row_mask = reinterpret_cast<const uint32_t *>(s.ws.row_thr + s.n);
-        if (b.row_filters) { a.row_filter = s.ws.row_filter; a.qtags = s.ws.qtags; }
-        if (b.row_windows) { a.row_window = s.ws.row_window; a.qvalues = s.ws.qvalues; }
-    }
     if (from) {
         a.rows = static_cast<const char *>(a.rows) + from * ix->dim * ix->esz();
         a.n = (uint32_t)(s.n - from);
@@ -1691,6 +1685,19 @@ static int range_collect(NkIndex *ix, const RangeShards &on, uint32_t Q, std::ve
     return 0;
 }
 
+// The end of a call that returns CSR lists, its offsets written: *out_total = total and, if the lists fit capacity (else the
+// caller calls again with room) and are not empty, collect(&keys) gives them in order and they are written decoded.
+static int write_csr(const NkIndex *ix, uint64_t total, uint64_t capacity, uint32_t *out_idx, float *out_score, uint64_t *out_total,
+                     const std::function<int(std::vector<uint64_t> *)> &collect) {
+    *out_total = total;
+    if (total > capacity || total == 0) return 0;
+    if (!out_idx || !out_score) { nk::set_error("null argument"); return -1; }
+    std::vector<uint64_t> keys;
+    if (collect(&keys)) return -1;
+    for (size_t j = 0; j < keys.size(); ++j) decode_key(ix->metric, keys[j], out_idx + j, out_score + j);
+    return 0;
+}
+
 int nk_search_range(NkIndex *ix, const float *queries_host, const float *thresholds_host, const NkFilter *filters_host, uint32_t Q,
                     uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total) {
     return nk_search_range_windowed(ix, queries_host, thresholds_host, filters_host, nullptr, Q, capacity, out_offsets, out_idx, out_score,
@@ -1720,31 +1727,23 @@ int nk_search_range_windowed(NkIndex *ix, const float *queries_host, const float
     if (order.failed()) return -1;
     RangeShards on{live_shards(ix)};
     const size_t qbytes = (size_t)Q * ix->dim * sizeof(float);
+    const RangeBlock block{ix->path, windows_host   ? nk::ScanMode::RANGE_WINDOW
+                                     : filters_host ? nk::ScanMode::RANGE_TAGS
+                                                    : nk::ScanMode::RANGE,
+                           Q, thr.data()};
     const StageQueries upload = [&](NkShard &s) {
         NK_CUDA_OK(cudaMemcpyAsync(s.ws.queries, queries_host, qbytes, cudaMemcpyHostToDevice, s.stream));
         ix->stats.bytes_h2d += qbytes;
-        if (windows_host) {
-            const NkFilter *qf;
-            const NkWindow *qw;
-            return stage_windows(ix, s, filters_host, windows_host, Q, &qf, &qw);
-        }
-        return filters_host && !stage_filters(ix, s, filters_host, Q) ? -1 : 0;
+        return stage_predicates(ix, s, s.stream, block.mode, Q, filters_host, windows_host);
     };
-    RangeBlock block{ix->path, Q, thr.data()};
-    block.filtered = filters_host != nullptr || windows_host != nullptr;
-    block.windowed = windows_host != nullptr;
     std::vector<uint64_t> per_query;
     if (range_scan(ix, &on, upload, block, &per_query)) return -1;
     // offsets: the shards' survivors of query q are merged into one run
     for (uint32_t q = 0; q < Q; ++q) out_offsets[q + 1] = out_offsets[q] + per_query[q];
-    *out_total = out_offsets[Q];
-    if (*out_total > capacity || *out_total == 0) return 0;
-    if (!out_idx || !out_score) { nk::set_error("null argument"); return -1; }
-    std::vector<uint64_t> keys;
-    keys.reserve(*out_total);
-    if (range_collect(ix, on, Q, &keys)) return -1;
-    for (size_t j = 0; j < keys.size(); ++j) decode_key(ix->metric, keys[j], out_idx + j, out_score + j);
-    return 0;
+    return write_csr(ix, out_offsets[Q], capacity, out_idx, out_score, out_total, [&](std::vector<uint64_t> *keys) {
+        keys->reserve(out_offsets[Q]);
+        return range_collect(ix, on, Q, keys);
+    });
 }
 
 // ---- similarity self-join (DESIGN.md §3.5d) ---------------------------------------------------------------------------
@@ -1792,12 +1791,7 @@ int nk_search_pairs_windowed(NkIndex *ix, uint64_t first_row, uint64_t n_rows, f
     if (order.failed()) return -1;
 
     const std::vector<NkShard *> live = live_shards(ix);
-    RowAdmit adm;
-    adm.windowed = window || max_gap != NK_NO_GAP;  // per-query windows too (a windowed scan is also a tag-filtered one)
-    const bool admit = filter || ix->mask_on || adm.windowed;  // some left rows may be inadmissible: per-query filters
-    if (filter) adm.f = *filter;
-    if (window) adm.w = *window;
-    adm.gap = max_gap;
+    const RowAdmit adm = join_admit(ix, filter, window, max_gap);
     const uint32_t QB = (uint32_t)std::min<uint64_t>(n_rows, SEARCH_ROWS_BLOCK);
     const std::vector<uint32_t> thr(QB, nk::ord_bits(range_key_threshold(ix, threshold)));
     std::vector<uint32_t> ids(QB);
@@ -1815,21 +1809,18 @@ int nk_search_pairs_windowed(NkIndex *ix, uint64_t first_row, uint64_t n_rows, f
             scan.from.push_back(lo <= s0 ? (s0 - lo) / SCAN_TILE_ROWS * SCAN_TILE_ROWS : 0);
         }
         StageQueries stage;
-        if (!scan.shards.empty() && stage_row_block(ix, live, ids.data(), nb, admit ? &adm : nullptr, &stage)) return -1;
+        if (!scan.shards.empty() && stage_row_block(ix, live, ids.data(), nb, adm, &stage)) return -1;
         const uint64_t pair_first = ix->row_base + s0;
-        RangeBlock block{ix->path, nb, thr.data()};
-        block.filtered = admit;
-        block.windowed = adm.windowed;
+        RangeBlock block{ix->path, adm.mode, nb, thr.data()};
         block.pair_first = &pair_first;
         if (range_scan(ix, &scan, stage, block, &per_query)) return -1;
         for (uint32_t q = 0; q < nb; ++q) out_offsets[b + q + 1] = out_offsets[b + q] + per_query[q];
         if (out_offsets[b + nb] > keys.size() && range_collect(ix, scan, nb, &keys)) return -1;
     }
-    *out_total = out_offsets[n_rows];
-    if (*out_total > capacity || *out_total == 0) return 0;
-    if (!out_idx || !out_score) { nk::set_error("null argument"); return -1; }
-    for (size_t j = 0; j < keys.size(); ++j) decode_key(ix->metric, keys[j], out_idx + j, out_score + j);
-    return 0;
+    return write_csr(ix, out_offsets[n_rows], capacity, out_idx, out_score, out_total, [&](std::vector<uint64_t> *out) {
+        out->swap(keys);
+        return 0;
+    });
 }
 
 // ---- k-NN graph update and remap (DESIGN.md §3.5e) ----------------------------------------------------------------------
@@ -1889,50 +1880,59 @@ static int exact_stage_runs(NkIndex *ix, uint64_t *out) {
     return 0;
 }
 
-// The keys K(r, j) of pairs (r, j) (relative ids), r all on shard s -> keys[i].
-static int graph_pair_keys_on(NkIndex *ix, const std::vector<NkShard *> &live, NkShard &s, const std::vector<uint32_t> &pr,
-                              const std::vector<uint32_t> &pj, std::vector<uint64_t> *keys) {
+// The keys K(r, j) of pairs (pr[i], pj[i]) (relative ids) -> keys[i], computed on the shard that holds r: each shard's distinct j
+// are gathered in blocks of SEARCH_ROWS_BLOCK (stage_row_block) and every block's pairs are scored in one launch.
+static int pair_keys(NkIndex *ix, const std::vector<NkShard *> &live, const std::vector<uint32_t> &pr, const std::vector<uint32_t> &pj,
+                     std::vector<uint64_t> *keys) {
     keys->assign(pr.size(), 0ull);
-    std::vector<uint32_t> js(pj);  // distinct j, staged in blocks of SEARCH_ROWS_BLOCK
-    std::sort(js.begin(), js.end());
-    js.erase(std::unique(js.begin(), js.end()), js.end());
-    std::vector<uint32_t> order(pr.size());
-    for (size_t i = 0; i < order.size(); ++i) order[i] = (uint32_t)i;
-    std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return pj[a] < pj[b]; });
-    size_t at = 0;
-    for (size_t b = 0; b < js.size(); b += SEARCH_ROWS_BLOCK) {
-        const uint32_t nb = (uint32_t)std::min<size_t>(SEARCH_ROWS_BLOCK, js.size() - b);
-        StageQueries stage;
-        if (stage_row_block(ix, live, js.data() + b, nb, nullptr, &stage)) return -1;
-        NK_CUDA_OK(cudaSetDevice(s.device));
-        if (nk::ws_reserve((void **)&s.ws.queries, &s.ws.queries_bytes, (size_t)nb * ix->dim * sizeof(float))) return -1;
-        if (stage(s)) return -1;
-        const uint32_t last = js[b + nb - 1];
-        std::vector<uint32_t> arg;  // [r local | slot of j | global j]
-        std::vector<uint32_t> idx;
-        for (; at < order.size() && pj[order[at]] <= last; ++at) idx.push_back(order[at]);
-        const size_t n = idx.size();
-        if (n == 0) continue;
-        arg.resize(3 * n);
-        for (size_t i = 0; i < n; ++i) {
-            arg[i] = pr[idx[i]] - (uint32_t)ix->first_row(s);
-            arg[n + i] = (uint32_t)(std::lower_bound(js.begin() + b, js.begin() + b + nb, pj[idx[i]]) - (js.begin() + b));
-            arg[2 * n + i] = (uint32_t)(ix->row_base + pj[idx[i]]);
+    std::vector<std::vector<uint32_t>> of_shard(ix->shards.size());  // the pairs whose r each shard holds, in order
+    for (size_t i = 0; i < pr.size(); ++i) {
+        uint64_t local;
+        of_shard[find_shard(ix, pr[i], &local) - ix->shards.data()].push_back((uint32_t)i);
+    }
+    for (size_t si = 0; si < of_shard.size(); ++si) {
+        if (of_shard[si].empty()) continue;
+        NkShard &s = ix->shards[si];
+        std::vector<uint32_t> order(of_shard[si]), js(order.size());  // distinct j, staged in blocks of SEARCH_ROWS_BLOCK
+        for (size_t i = 0; i < order.size(); ++i) js[i] = pj[order[i]];
+        std::sort(js.begin(), js.end());
+        js.erase(std::unique(js.begin(), js.end()), js.end());
+        std::sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) { return pj[a] < pj[b]; });
+        size_t at = 0;
+        for (size_t b = 0; b < js.size(); b += SEARCH_ROWS_BLOCK) {
+            const uint32_t nb = (uint32_t)std::min<size_t>(SEARCH_ROWS_BLOCK, js.size() - b);
+            StageQueries stage;
+            if (stage_row_block(ix, live, js.data() + b, nb, RowAdmit{}, &stage)) return -1;
+            NK_CUDA_OK(cudaSetDevice(s.device));
+            if (nk::ws_reserve((void **)&s.ws.queries, &s.ws.queries_bytes, (size_t)nb * ix->dim * sizeof(float))) return -1;
+            if (stage(s)) return -1;
+            const uint32_t last = js[b + nb - 1];
+            std::vector<uint32_t> arg;  // [r local | slot of j | global j]
+            std::vector<uint32_t> idx;
+            for (; at < order.size() && pj[order[at]] <= last; ++at) idx.push_back(order[at]);
+            const size_t n = idx.size();
+            if (n == 0) continue;
+            arg.resize(3 * n);
+            for (size_t i = 0; i < n; ++i) {
+                arg[i] = pr[idx[i]] - (uint32_t)ix->first_row(s);
+                arg[n + i] = (uint32_t)(std::lower_bound(js.begin() + b, js.begin() + b + nb, pj[idx[i]]) - (js.begin() + b));
+                arg[2 * n + i] = (uint32_t)(ix->row_base + pj[idx[i]]);
+            }
+            if (nk::ws_reserve(&s.ws.scratch, &s.ws.scratch_bytes, n * 12 + n * 8 + 8)) return -1;
+            uint32_t *d_arg = static_cast<uint32_t *>(s.ws.scratch);
+            uint64_t *d_out = reinterpret_cast<uint64_t *>(static_cast<char *>(s.ws.scratch) + (n * 12 + 7) / 8 * 8);
+            std::vector<uint64_t> out(n);
+            NK_CUDA_OK(cudaMemcpyAsync(d_arg, arg.data(), n * 12, cudaMemcpyHostToDevice, s.stream));
+            if (nk::graph_pair_keys(s.rows, ix->dtype, ix->dim, ix->metric, s.ws.queries, d_arg, d_arg + n, d_arg + 2 * n, (uint32_t)n, d_out,
+                                    s.stream))
+                return -1;
+            NK_CUDA_OK(cudaMemcpyAsync(out.data(), d_out, n * 8, cudaMemcpyDeviceToHost, s.stream));
+            NK_CUDA_OK(cudaStreamSynchronize(s.stream));
+            ix->stats.kernel_launches++;
+            ix->stats.bytes_h2d += n * 12;
+            ix->stats.bytes_d2h += n * 8;
+            for (size_t i = 0; i < n; ++i) (*keys)[idx[i]] = out[i];
         }
-        if (nk::ws_reserve(&s.ws.scratch, &s.ws.scratch_bytes, n * 12 + n * 8 + 8)) return -1;
-        uint32_t *d_arg = static_cast<uint32_t *>(s.ws.scratch);
-        uint64_t *d_out = reinterpret_cast<uint64_t *>(static_cast<char *>(s.ws.scratch) + (n * 12 + 7) / 8 * 8);
-        std::vector<uint64_t> out(n);
-        NK_CUDA_OK(cudaMemcpyAsync(d_arg, arg.data(), n * 12, cudaMemcpyHostToDevice, s.stream));
-        if (nk::graph_pair_keys(s.rows, ix->dtype, ix->dim, ix->metric, s.ws.queries, d_arg, d_arg + n, d_arg + 2 * n, (uint32_t)n, d_out,
-                                s.stream))
-            return -1;
-        NK_CUDA_OK(cudaMemcpyAsync(out.data(), d_out, n * 8, cudaMemcpyDeviceToHost, s.stream));
-        NK_CUDA_OK(cudaStreamSynchronize(s.stream));
-        ix->stats.kernel_launches++;
-        ix->stats.bytes_h2d += n * 12;
-        ix->stats.bytes_d2h += n * 8;
-        for (size_t i = 0; i < n; ++i) (*keys)[idx[i]] = out[i];
     }
     return 0;
 }
@@ -1972,24 +1972,30 @@ static bool graph_nan_list(const NkIndex *ix, const uint32_t *li, const float *l
     return li[0] != GRAPH_PAD && ls[0] == (ix->metric == NK_METRIC_EUCLIDEAN ? INFINITY : -INFINITY);
 }
 
-// Check src and the old graph's entries -> now_at [n_old]: the current id of old row o, NK_ROW_NEW once it is gone.
-static int graph_check(const NkIndex *ix, const GraphCall &g, std::vector<uint32_t> *now_at) {
+// Check src [rows()] (the old row each current row holds, or NK_ROW_NEW) -> now_at [n_old]: the current id of old row o,
+// NK_ROW_NEW once it is gone.
+static int check_src_of_row(const NkIndex *ix, const char *what, const uint32_t *src, uint64_t n_old, std::vector<uint32_t> *now_at) {
     const uint64_t N = ix->rows();
-    now_at->assign(g.n_old, NK_ROW_NEW);
+    now_at->assign(n_old, NK_ROW_NEW);
     for (uint64_t f = 0; f < N; ++f) {
-        const uint32_t o = g.src[f];
+        const uint32_t o = src[f];
         if (o == NK_ROW_NEW) continue;
-        if (o >= g.n_old) {
-            nk::set_error("%s: src_of_row[%llu] = %u is not an old row (n_old=%llu)", g.what, (unsigned long long)f, o,
-                          (unsigned long long)g.n_old);
+        if (o >= n_old) {
+            nk::set_error("%s: src_of_row[%llu] = %u is not an old row (n_old=%llu)", what, (unsigned long long)f, o, (unsigned long long)n_old);
             return -1;
         }
         if ((*now_at)[o] != NK_ROW_NEW) {
-            nk::set_error("%s: old row %u is the source of rows %u and %llu", g.what, o, (*now_at)[o], (unsigned long long)f);
+            nk::set_error("%s: old row %u is the source of rows %u and %llu", what, o, (*now_at)[o], (unsigned long long)f);
             return -1;
         }
         (*now_at)[o] = (uint32_t)f;
     }
+    return 0;
+}
+
+// Check src and the old graph's entries -> now_at [n_old] (check_src_of_row).
+static int graph_check(const NkIndex *ix, const GraphCall &g, std::vector<uint32_t> *now_at) {
+    if (check_src_of_row(ix, g.what, g.src, g.n_old, now_at)) return -1;
     for (uint64_t i = 0; i < g.n_old * g.k; ++i)
         if (g.gi_in[i] != GRAPH_PAD && (g.gi_in[i] < ix->row_base || g.gi_in[i] - ix->row_base >= g.n_old)) {
             nk::set_error("%s: entry %llu of the graph (row %u) is not an old row", g.what, (unsigned long long)i, g.gi_in[i]);
@@ -2052,11 +2058,11 @@ static int graph_rows_searched_again(NkIndex *ix, const GraphCall &g, const std:
     return 0;
 }
 
-// Before the reverse scan: every live shard gets its per-row thresholds and, behind them, the mask of the rows outside R
-// (s.ws.row_thr), with filters each row's own filter for the row side of the scan (s.ws.row_filter), and with windows each
-// row's own window (s.ws.row_window).  A windowed scan is a row-filter scan: without filters its row filters are {0,0,0},
-// which admit every tag, written on the device.
-static int graph_upload_row_thresholds(NkIndex *ix, const GraphCall &g, const std::vector<NkShard *> &live, const std::vector<uint8_t> &in_r) {
+// Before the reverse scan in mode m: every live shard gets its per-row thresholds and, behind them, the mask of the rows outside
+// R (s.ws.row_thr), under a row-filter mode each row's own filter for the row side of the scan (s.ws.row_filter: put_filters,
+// {0,0,0} for a windowed graph without filters), and under REVERSE_RWINDOW each row's own window (s.ws.row_window).
+static int graph_upload_row_thresholds(NkIndex *ix, const GraphCall &g, nk::ScanMode m, const std::vector<NkShard *> &live,
+                                       const std::vector<uint8_t> &in_r) {
     const uint32_t k = g.k;
     for (NkShard *s : live) {
         const uint64_t lo = ix->first_row(*s), words = (s->n + 31) / 32;
@@ -2073,15 +2079,10 @@ static int graph_upload_row_thresholds(NkIndex *ix, const GraphCall &g, const st
         NK_CUDA_OK(cudaSetDevice(s->device));
         if (nk::ws_reserve((void **)&s->ws.row_thr, &s->ws.row_thr_bytes, thr.size() * 4)) return -1;
         NK_CUDA_OK(cudaMemcpyAsync(s->ws.row_thr, thr.data(), thr.size() * 4, cudaMemcpyHostToDevice, s->stream));
-        if (g.filters) {
-            if (nk::ws_reserve((void **)&s->ws.row_filter, &s->ws.row_filter_bytes, s->n * sizeof(NkFilter))) return -1;
-            NK_CUDA_OK(cudaMemcpyAsync(s->ws.row_filter, g.filters + lo, s->n * sizeof(NkFilter), cudaMemcpyHostToDevice, s->stream));
-            ix->stats.bytes_h2d += s->n * sizeof(NkFilter);
-        } else if (g.windows) {
-            if (nk::ws_reserve((void **)&s->ws.row_filter, &s->ws.row_filter_bytes, s->n * sizeof(NkFilter))) return -1;
-            NK_CUDA_OK(cudaMemsetAsync(s->ws.row_filter, 0, s->n * sizeof(NkFilter), s->stream));
-        }
-        if (g.windows) {
+        if (nk::mode_row_filter(m) &&
+            put_filters(ix, &s->ws.row_filter, &s->ws.row_filter_bytes, g.filters ? g.filters + lo : nullptr, s->n, s->stream))
+            return -1;
+        if (nk::mode_row_window(m)) {
             if (nk::ws_reserve((void **)&s->ws.row_window, &s->ws.row_window_bytes, s->n * sizeof(NkWindow))) return -1;
             NK_CUDA_OK(cudaMemcpyAsync(s->ws.row_window, g.windows + lo, s->n * sizeof(NkWindow), cudaMemcpyHostToDevice, s->stream));
             ix->stats.bytes_h2d += s->n * sizeof(NkWindow);
@@ -2097,27 +2098,28 @@ static int graph_upload_row_thresholds(NkIndex *ix, const GraphCall &g, const st
 using GraphEntrants = std::vector<std::pair<uint32_t, uint64_t>>;
 static int graph_reverse_scan(NkIndex *ix, const GraphCall &g, const std::vector<NkShard *> &live, int path, const std::vector<uint8_t> &in_r,
                               const std::vector<uint32_t> &C, GraphEntrants *entrants) {
-    if (graph_upload_row_thresholds(ix, g, live, in_r)) return -1;
-    // a filtered graph's queries also carry their tags, a windowed graph's their value keys (and tag 0 without filters: its
-    // row filters admit every tag), and always a per-query filter (the row-filtered scan is a mode of the tag-filtered one)
+    // a windowed graph's scan holds each pair to the row's window and its filter (those of a graph without filters admit every
+    // tag), a filtered graph's to the row's filter; every mode but REVERSE applies per-query filters (masked-out queries get
+    // the filter that admits no row, stage_row_block)
+    const RowAdmit all_rows{g.windows ? nk::ScanMode::REVERSE_RWINDOW
+                            : g.filters ? nk::ScanMode::REVERSE_RFILT
+                            : ix->mask_on ? nk::ScanMode::REVERSE_TAGS
+                                          : nk::ScanMode::REVERSE};
+    if (graph_upload_row_thresholds(ix, g, all_rows.mode, live, in_r)) return -1;
+    // a filtered graph's queries also carry their tags, a windowed graph's their value keys (and tag 0 without filters)
     std::vector<uint64_t> tags, values, qtags, qvalues;
     if (g.filters && host_row_words(ix, false, &tags)) return -1;
     if (g.windows && host_row_words(ix, true, &values)) return -1;
-    const RowAdmit all_rows;  // masked-out queries get the filter that admits no row (stage_row_block)
     const uint32_t QB = (uint32_t)std::min<size_t>(C.size(), SEARCH_ROWS_BLOCK);
     const std::vector<uint32_t> floor_thr(QB, nk::ord_bits(ix->key_floor()));
-    RangeBlock block{path, 0, floor_thr.data()};
-    block.filtered = ix->mask_on || g.filters || g.windows;
-    block.reverse = true;
-    block.row_filters = g.filters || g.windows;
-    block.row_windows = g.windows != nullptr;
+    RangeBlock block{path, all_rows.mode, 0, floor_thr.data()};
     RangeShards on{live};
     std::vector<uint64_t> keys, per_query;
     for (size_t b = 0; b < C.size(); b += QB) {
         const uint32_t nb = block.Q = (uint32_t)std::min<size_t>(QB, C.size() - b);
         StageQueries stage_rows;
-        if (stage_row_block(ix, live, C.data() + b, nb, block.filtered ? &all_rows : nullptr, &stage_rows)) return -1;
-        if (block.row_filters) {
+        if (stage_row_block(ix, live, C.data() + b, nb, all_rows, &stage_rows)) return -1;
+        if (nk::mode_row_filter(block.mode)) {
             qtags.assign(nb, 0ull);
             if (g.filters)
                 for (uint32_t q = 0; q < nb; ++q) qtags[q] = tags[C[b + q]];
@@ -2128,12 +2130,12 @@ static int graph_reverse_scan(NkIndex *ix, const GraphCall &g, const std::vector
         }
         const StageQueries stage = [&](NkShard &s) {
             if (stage_rows(s)) return -1;
-            if (!block.row_filters) return 0;
+            if (!nk::mode_row_filter(block.mode)) return 0;
             // the queries' tags and value keys: read by the scan before range_shard's first synchronisation
             if (nk::ws_reserve((void **)&s.ws.qtags, &s.ws.qtags_bytes, (size_t)nb * 8)) return -1;
             NK_CUDA_OK(cudaMemcpyAsync(s.ws.qtags, qtags.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, s.stream));
             ix->stats.bytes_h2d += (uint64_t)nb * 8;
-            if (!g.windows) return 0;
+            if (!nk::mode_row_window(block.mode)) return 0;
             if (nk::ws_reserve((void **)&s.ws.qvalues, &s.ws.qvalues_bytes, (size_t)nb * 8)) return -1;
             NK_CUDA_OK(cudaMemcpyAsync(s.ws.qvalues, qvalues.data(), (size_t)nb * 8, cudaMemcpyHostToDevice, s.stream));
             ix->stats.bytes_h2d += (uint64_t)nb * 8;
@@ -2154,39 +2156,28 @@ static int graph_reverse_scan(NkIndex *ix, const GraphCall &g, const std::vector
 }
 
 // Merge the entrants into the lists of the rows they touch: each touched row's old entries, their keys recomputed as the
-// row's list scores them (graph_pair_keys_on, per shard of the row), and its entrants in key space, the best k kept.
+// row's list scores them (pair_keys), and its entrants in key space, the best k kept.
 static int graph_merge_entrants(NkIndex *ix, GraphCall &g, const std::vector<NkShard *> &live, const GraphEntrants &entrants) {
     const uint32_t k = g.k;
-    const size_t n_shards = ix->shards.size();
-    std::vector<std::vector<uint64_t>> okeys(n_shards);
-    std::vector<std::vector<uint32_t>> opr(n_shards), opj(n_shards);
-    std::vector<uint32_t> touched;
+    std::vector<uint32_t> touched, opr, opj;
     for (size_t i = 0; i < entrants.size(); ++i)
         if (i == 0 || entrants[i].first != entrants[i - 1].first) touched.push_back(entrants[i].first);
-    std::vector<size_t> shard_of(touched.size());
-    for (size_t t = 0; t < touched.size(); ++t) {
-        const uint32_t r = touched[t];
-        uint64_t local;
-        shard_of[t] = (size_t)(find_shard(ix, r, &local) - ix->shards.data());
+    for (const uint32_t r : touched)
         for (uint32_t j = 0; j < k; ++j) {
             const uint32_t e = g.gi_in[(uint64_t)r * k + j];
             if (e == GRAPH_PAD) break;
-            opr[shard_of[t]].push_back(r);
-            opj[shard_of[t]].push_back((uint32_t)(e - ix->row_base));
+            opr.push_back(r);
+            opj.push_back((uint32_t)(e - ix->row_base));
         }
-    }
-    for (size_t i = 0; i < n_shards; ++i)
-        if (!opr[i].empty() && graph_pair_keys_on(ix, live, ix->shards[i], opr[i], opj[i], &okeys[i])) return -1;
-    std::vector<size_t> opos(n_shards, 0);
+    std::vector<uint64_t> okeys;
+    if (pair_keys(ix, live, opr, opj, &okeys)) return -1;
     std::vector<uint64_t> cand;
     std::vector<uint32_t> li(k);
     std::vector<float> ls(k);
-    size_t e0 = 0;
-    for (size_t t = 0; t < touched.size(); ++t) {
-        const uint32_t r = touched[t];
+    size_t o0 = 0, e0 = 0;
+    for (const uint32_t r : touched) {
         cand.clear();
-        const size_t si = shard_of[t];
-        while (opos[si] < opr[si].size() && opr[si][opos[si]] == r) cand.push_back(okeys[si][opos[si]++]);
+        for (; o0 < opr.size() && opr[o0] == r; ++o0) cand.push_back(okeys[o0]);
         for (; e0 < entrants.size() && entrants[e0].first == r; ++e0) cand.push_back(entrants[e0].second);
         const size_t take = std::min<size_t>(k, cand.size());
         std::partial_sort(cand.begin(), cand.begin() + take, cand.end(), std::greater<uint64_t>());
@@ -2398,12 +2389,7 @@ static int pairs_rows_locked(NkIndex *ix, const PairsCall &c, int path, const st
     off->assign((size_t)n + 1, 0);
     keys->clear();
     if (n == 0) return 0;
-    RowAdmit adm;  // the join's (nk_search_pairs_windowed)
-    adm.windowed = c.window || c.max_gap != NK_NO_GAP;
-    const bool admit = c.filter || ix->mask_on || adm.windowed;
-    if (c.filter) adm.f = *c.filter;
-    if (c.window) adm.w = *c.window;
-    adm.gap = c.max_gap;
+    const RowAdmit adm = join_admit(ix, c.filter, c.window, c.max_gap);
     const uint32_t QB = std::min(n, SEARCH_ROWS_BLOCK);
     // every live shard: the bits of the listed rows it holds, room for a block's query rows behind them
     for (NkShard *s : live) {
@@ -2425,7 +2411,7 @@ static int pairs_rows_locked(NkIndex *ix, const PairsCall &c, int path, const st
         const uint32_t nb = std::min(QB, n - b);
         for (uint32_t q = 0; q < nb; ++q) qrow[q] = (uint32_t)(ix->row_base + rows[b + q]);
         StageQueries stage_rows;
-        if (stage_row_block(ix, live, rows + b, nb, admit ? &adm : nullptr, &stage_rows)) return -1;
+        if (stage_row_block(ix, live, rows + b, nb, adm, &stage_rows)) return -1;
         const StageQueries stage = [&](NkShard &s) {
             if (stage_rows(s)) return -1;
             // the block's query rows behind the listed-row bits (range_shard's IncidentRows), read before its first synchronisation
@@ -2433,9 +2419,7 @@ static int pairs_rows_locked(NkIndex *ix, const PairsCall &c, int path, const st
             ix->stats.bytes_h2d += (uint64_t)nb * 4;
             return 0;
         };
-        RangeBlock block{path, nb, thr.data()};
-        block.filtered = admit;
-        block.windowed = adm.windowed;
+        RangeBlock block{path, adm.mode, nb, thr.data()};
         block.incident = true;
         if (range_scan(ix, &on, stage, block, &per_query)) return -1;
         for (uint32_t q = 0; q < nb; ++q) (*off)[b + q + 1] = (*off)[b + q] + per_query[q];
@@ -2485,11 +2469,10 @@ static int pairs_rows_host(NkIndex *ix, const PairsCall &c, const uint32_t *rows
     std::vector<uint64_t> off, keys;
     if (pairs_rows_locked(ix, c, path, live, rows_host, n, &off, &keys)) return -1;
     memcpy(out_offsets, off.data(), ((size_t)n + 1) * 8);
-    *out_total = off[n];
-    if (*out_total > capacity || *out_total == 0) return 0;
-    if (!out_idx || !out_score) { nk::set_error("null argument"); return -1; }
-    for (size_t j = 0; j < keys.size(); ++j) decode_key(ix->metric, keys[j], out_idx + j, out_score + j);
-    return 0;
+    return write_csr(ix, off[n], capacity, out_idx, out_score, out_total, [&](std::vector<uint64_t> *out) {
+        out->swap(keys);
+        return 0;
+    });
 }
 
 int nk_search_pairs_rows(NkIndex *ix, const uint32_t *rows_host, uint32_t n, float threshold, const NkFilter *filter, uint64_t capacity,
@@ -2509,7 +2492,7 @@ int nk_search_pairs_rows_windowed(NkIndex *ix, const uint32_t *rows_host, uint32
 // every other old pair is dropped, and the pairs incident to the new and moved rows C are found by pairs_rows_locked.  Each
 // found pair goes to its lower end's list and is merged there with the carried entries in key space.  Carried keys come back
 // from the old scores (cosine / dot: the score is the key's); under euclidean two squared distances one ulp apart decode to one
-// distance, so the carried keys of a list that takes in found pairs are computed again on the device (graph_pair_keys_on).
+// distance, so the carried keys of a list that takes in found pairs are computed again on the device (pair_keys).
 int nk_pairs_remap(NkIndex *ix, float threshold, const NkFilter *filter, const NkWindow *window, uint64_t max_gap, uint64_t n_old,
                    const uint32_t *src_of_row, const uint64_t *old_offsets, const uint32_t *old_idx, const float *old_score,
                    uint64_t capacity, uint64_t *out_offsets, uint32_t *out_idx, float *out_score, uint64_t *out_total,
@@ -2528,17 +2511,8 @@ int nk_pairs_remap(NkIndex *ix, float threshold, const NkFilter *filter, const N
         if (old_offsets[o + 1] < old_offsets[o]) { nk::set_error("%s: old_offsets decrease at row %llu", c.what, (unsigned long long)o); return -1; }
     const uint64_t n_old_pairs = old_offsets[n_old];
     if (n_old_pairs && (!old_idx || !old_score)) { nk::set_error("null argument"); return -1; }
-    std::vector<uint32_t> now_at(n_old, NK_ROW_NEW);
-    for (uint64_t f = 0; f < N; ++f) {
-        const uint32_t o = src_of_row[f];
-        if (o == NK_ROW_NEW) continue;
-        if (o >= n_old) {
-            nk::set_error("%s: src_of_row[%llu] = %u is not an old row (n_old=%llu)", c.what, (unsigned long long)f, o, (unsigned long long)n_old);
-            return -1;
-        }
-        if (now_at[o] != NK_ROW_NEW) { nk::set_error("%s: old row %u is the source of rows %u and %llu", c.what, o, now_at[o], (unsigned long long)f); return -1; }
-        now_at[o] = (uint32_t)f;
-    }
+    std::vector<uint32_t> now_at;
+    if (check_src_of_row(ix, c.what, src_of_row, n_old, &now_at)) return -1;
     for (uint64_t o = 0; o < n_old; ++o)
         for (uint64_t e = old_offsets[o]; e < old_offsets[o + 1]; ++e) {
             const uint64_t j = (uint64_t)old_idx[e] - ix->row_base;
@@ -2597,25 +2571,19 @@ int nk_pairs_remap(NkIndex *ix, float threshold, const NkFilter *filter, const N
     if (!out_idx || !out_score) { nk::set_error("null argument"); return -1; }
     std::vector<uint64_t> okey(ix->metric == NK_METRIC_EUCLIDEAN ? n_old_pairs : 0, 0ull);
     if (!okey.empty()) {
-        const size_t n_shards = ix->shards.size();
-        std::vector<std::vector<uint32_t>> pr(n_shards), pj(n_shards);
-        std::vector<std::vector<uint64_t>> at(n_shards), keys(n_shards);
+        std::vector<uint32_t> pr, pj;
+        std::vector<uint64_t> at, keys;
         for (uint64_t r = 0; r < N && r < n_old; ++r) {
             if (!touched[r] || !kept(r)) continue;
-            uint64_t local;
-            const size_t si = (size_t)(find_shard(ix, r, &local) - ix->shards.data());
             for (uint64_t e = old_offsets[r]; e < old_offsets[r + 1]; ++e)
                 if (kept(old_idx[e] - ix->row_base)) {
-                    pr[si].push_back((uint32_t)r);
-                    pj[si].push_back((uint32_t)(old_idx[e] - ix->row_base));
-                    at[si].push_back(e);
+                    pr.push_back((uint32_t)r);
+                    pj.push_back((uint32_t)(old_idx[e] - ix->row_base));
+                    at.push_back(e);
                 }
         }
-        for (size_t i = 0; i < n_shards; ++i) {
-            if (pr[i].empty()) continue;
-            if (graph_pair_keys_on(ix, live, ix->shards[i], pr[i], pj[i], &keys[i])) return -1;
-            for (size_t t = 0; t < at[i].size(); ++t) okey[at[i][t]] = keys[i][t];
-        }
+        if (pair_keys(ix, live, pr, pj, &keys)) return -1;
+        for (size_t t = 0; t < at.size(); ++t) okey[at[t]] = keys[t];
     }
     std::vector<uint64_t> mine, merged;
     size_t f0 = 0;
@@ -2700,22 +2668,13 @@ static int search_device(NkIndex *ix, const float *queries_dev, const NkFilter *
     if (nk::ws_reserve((void **)&s->ws.keys, &s->ws.keys_bytes, (size_t)Q * k * 8)) return -1;
     ix->stats.searches++;
     ix->stats.queries += Q;
-    ScanOut xo(ix->path);
+    ScanOut xo(ix->path, windows_dev ? nk::ScanMode::KNN_WINDOW : filters_dev ? nk::ScanMode::KNN_TAGS : nk::ScanMode::KNN);
     xo.out_idx = out_idx_dev; xo.out_score = out_score_dev;  // decoded by the last kernel of the path
-    if (filters_dev) {
-        if (shard_tags_on(*s)) return -1;
-        xo.qfilter = filters_dev;  // the caller keeps it valid until the stream has run (the blindly queued tail reads it too)
-    }
-    if (windows_dev) {
-        if (shard_values_on(*s)) return -1;
-        if (!filters_dev) {  // a windowed scan also applies a tag filter: {0,0,0} for every query, staged on the caller's stream
-            if (shard_tags_on(*s)) return -1;
-            if (nk::ws_reserve((void **)&s->ws.qfilter, &s->ws.qfilter_bytes, (size_t)Q * sizeof(NkFilter))) return -1;
-            NK_CUDA_OK(cudaMemsetAsync(s->ws.qfilter, 0, (size_t)Q * sizeof(NkFilter), st));
-            xo.qfilter = s->ws.qfilter;
-        }
-        xo.qwindow = windows_dev;  // kept valid by the caller, as filters_dev
-    }
+    // the caller's filters and windows are read in place: the caller keeps them valid until the stream has run (the blindly
+    // queued tail reads them too); a windowed scan without filters gets {0,0,0} staged on the caller's stream
+    xo.qfilter = filters_dev; xo.qwindow = windows_dev;
+    if (filters_dev ? shard_tags_on(*s) : stage_predicates(ix, *s, st, xo.mode, Q, nullptr, nullptr)) return -1;
+    if (windows_dev && shard_values_on(*s)) return -1;
     if (run_scan(ix, *s, queries_dev, Q, k, s->ws.keys, st, xo)) return -1;
     return (int)k;
 }
