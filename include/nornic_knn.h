@@ -62,7 +62,10 @@ size_t cuda_buffer_size(CudaBuffer *buf);            /* cuda_bridge.go:201 */
 /* cuda_bridge.go:205.  Copies min(count*4, size) bytes; 0 / -1. */
 int cuda_buffer_copy_to_host(CudaBuffer *buf, float *host_data, size_t count);
 
-/* cuda_bridge.go:231.  norms[i] = ||vectors[i]||2.  One kernel (the reference issues n cublasSnrm2 calls). */
+/* cuda_bridge.go:231.  norms[i] = ||vectors[i]||2.  One kernel (the reference issues n cublasSnrm2 calls).  Like
+ * cublasSnrm2 it neither overflows nor underflows in between: a row whose fp32 sum of squares is not finite or below 2^-100
+ * is summed again scaled by a power of two, so rows of elements near 1e25 or 1e-30 get a finite, accurate norm.  A NaN
+ * element gives NaN, an inf element inf. */
 int cuda_compute_norms(CudaDevice *dev, CudaBuffer *vectors, CudaBuffer *norms, unsigned int n, unsigned int dims);
 /* cuda_bridge.go:249.  In place; rows with norm <= 1e-10 are left untouched (cuda_bridge.go:267). */
 int cuda_normalize_vectors(CudaDevice *dev, CudaBuffer *vectors, unsigned int n, unsigned int dims);
@@ -73,7 +76,9 @@ int cuda_cosine_similarity(CudaDevice *dev, CudaBuffer *embeddings, CudaBuffer *
                            unsigned int n, unsigned int dims, int normalized);
 /* cuda_bridge.go:327.  out_indices/out_scores are HOST arrays of length k; k is clamped to n; result
  * sorted by score descending, ties by lowest index first (the strict '>' forward scan of
- * cuda_bridge.go:356-371).  Selection runs on the device; only k pairs cross PCIe. */
+ * cuda_bridge.go:356-371).  As in that scan, only scores > -1e30f enter: NaN, -inf and anything at or below -1e30f never
+ * do, and slots no score reached are (0, -1e30f).  -0.0 and +0.0 are equal (ties by index); each score is returned with
+ * its own bits.  Any n up to 2^32 - 1.  Selection runs on the device; only k pairs cross PCIe. */
 int cuda_topk(CudaDevice *dev, CudaBuffer *scores, unsigned int *out_indices, float *out_scores, unsigned int n,
               unsigned int k);
 

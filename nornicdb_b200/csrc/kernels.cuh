@@ -262,6 +262,8 @@ int row_scores(const float *rows, const float *query, float *scores, uint32_t n,
                cudaStream_t s);
 int topk_scores(const DeviceInfo &di, const float *scores, uint32_t n, uint32_t k, Workspace &ws, uint64_t *out_keys,
                 cudaStream_t s, const uint64_t *below = nullptr);
+// keys [k] of topk_scores -> (row, scores[row]), and (0, -1e30f) for an empty slot: cuda_topk's output.
+int decode_topk_scores(const uint64_t *keys, uint32_t k, const float *scores, uint32_t *out_idx, float *out_score, cudaStream_t s);
 // below[q] = keys[q*k + k-1] (the smallest key pass p returned): the exclusion bound of pass p+1.
 int update_below(const uint64_t *keys, uint32_t Q, uint32_t k, uint64_t *below, cudaStream_t s);
 int fill_uniform(void *out, int dtype, uint64_t n_rows, uint32_t dim, uint64_t seed, uint64_t row_base, cudaStream_t s);

@@ -121,6 +121,9 @@ CudaBuffer *cuda_create_buffer(CudaDevice *dev, float *host_data, size_t count, 
         err = cudaMalloc((void **)&buf->data, buf->size ? buf->size : 4);
         if (err == cudaSuccess && host_data && buf->size)
             err = cudaMemcpy(buf->data, host_data, buf->size, cudaMemcpyHostToDevice);
+        // a pageable cudaMemcpy may return before its DMA has landed, and the calls below run on the device's non-blocking
+        // stream, which does not wait for the legacy stream: finish the copy here, as the header promises
+        if (err == cudaSuccess && host_data && buf->size) err = cudaStreamSynchronize(cudaStreamLegacy);
         if (err != cudaSuccess) {
             nk::set_error("%s", cudaGetErrorString(err));
             cudaGetLastError();
@@ -249,7 +252,7 @@ int cuda_topk(CudaDevice *dev, CudaBuffer *scores, unsigned int *out_indices, fl
             done += kp;
         }
     }
-    if (nk::decode_keys(ws.keys, 1, k, NK_METRIC_DOT, ws.out_idx, ws.out_score, dev->stream)) return -1;
+    if (nk::decode_topk_scores(ws.keys, k, scores->data, ws.out_idx, ws.out_score, dev->stream)) return -1;
     NK_CUDA_OK(cudaMemcpyAsync(out_indices, ws.out_idx, (size_t)k * 4, cudaMemcpyDeviceToHost, dev->stream));
     NK_CUDA_OK(cudaMemcpyAsync(out_scores, ws.out_score, (size_t)k * 4, cudaMemcpyDeviceToHost, dev->stream));
     NK_CUDA_OK(cudaStreamSynchronize(dev->stream));

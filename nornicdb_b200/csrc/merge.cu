@@ -295,13 +295,16 @@ __global__ void __launch_bounds__(TOPK_THREADS) topk_scores_kernel(const float *
     }
     __syncthreads();
     uint64_t *my = cand + (size_t)blockIdx.x * P;
-    const uint32_t num_iv = (n + TOPK_IV - 1) / TOPK_IV;
-    for (uint32_t iv = blockIdx.x; iv < num_iv; iv += gridDim.x) {
-        for (uint32_t i = iv * TOPK_IV + threadIdx.x; i < (iv + 1) * TOPK_IV && i < n; i += TOPK_THREADS) {
-            float s = scores[i];
-            if (s != s) s = -INFINITY;
-            if (s >= s_tau) {
-                const uint64_t key = make_key(s, i);
+    const uint64_t num_iv = ((uint64_t)n + TOPK_IV - 1) / TOPK_IV;  // 64-bit: n may be up to 2^32 - 1
+    for (uint64_t iv = blockIdx.x; iv < num_iv; iv += gridDim.x) {
+        const uint64_t end = (iv + 1) * TOPK_IV < n ? (iv + 1) * TOPK_IV : n;
+        for (uint64_t i = iv * TOPK_IV + threadIdx.x; i < end; i += TOPK_THREADS) {
+            const float s = scores[i];
+            // the reference's slots start at -1e30f and admit only s > slot: NaN, -inf and scores <= -1e30f never enter.
+            // -0.0 enters as +0.0 (its '>' cannot tell them apart), so the two tie by row; the output score is re-read from
+            // scores[row] (decode_topk_scores), which keeps the sign.
+            if (s == s && s > -1e30f && s >= s_tau) {
+                const uint64_t key = make_key(s == 0.0f ? 0.0f : s, (uint32_t)i);
                 if (!below || key < below[0]) {
                     int pos = atomicAdd(&s_cnt, 1);
                     if (pos < P) my[pos] = key;
@@ -332,9 +335,10 @@ __global__ void __launch_bounds__(TOPK_THREADS) topk_keys_kernel(const unsigned 
     }
     __syncthreads();
     uint64_t *my = cand + (size_t)blockIdx.x * P;
-    const uint32_t num_iv = (n + TOPK_IV - 1) / TOPK_IV;
-    for (uint32_t iv = blockIdx.x; iv < num_iv; iv += gridDim.x) {
-        for (uint32_t i = iv * TOPK_IV + threadIdx.x; i < (iv + 1) * TOPK_IV && i < n; i += TOPK_THREADS) {
+    const uint64_t num_iv = ((uint64_t)n + TOPK_IV - 1) / TOPK_IV;
+    for (uint64_t iv = blockIdx.x; iv < num_iv; iv += gridDim.x) {
+        const uint64_t end = (iv + 1) * TOPK_IV < n ? (iv + 1) * TOPK_IV : n;
+        for (uint64_t i = iv * TOPK_IV + threadIdx.x; i < end; i += TOPK_THREADS) {
             const uint64_t key = keys[i];
             if (key && key_score(key) >= s_tau) {
                 int pos = atomicAdd(&s_cnt, 1);
@@ -382,9 +386,9 @@ int topk_keys(const DeviceInfo &di, const unsigned long long *keys, uint32_t n, 
         return -1;
     }
     int P = (int)next_pow2(k + TOPK_IV + 1);
-    uint32_t num_iv = (n + TOPK_IV - 1) / TOPK_IV;
+    const uint64_t num_iv = ((uint64_t)n + TOPK_IV - 1) / TOPK_IV;  // 64-bit: in 32 bits it wraps to 0 for n > 2^32 - 1024
     uint32_t grid = (uint32_t)di.num_sms * 2;
-    if (grid > num_iv) grid = num_iv;
+    if (grid > num_iv) grid = (uint32_t)num_iv;
     if (ws_reserve((void **)&ws.cand, &ws.cand_bytes, (size_t)grid * P * 8)) return -1;
     if (ws_reserve((void **)&ws.partial, &ws.partial_bytes, (size_t)grid * k * 8)) return -1;
     size_t smem = (size_t)P * 8;
@@ -409,9 +413,9 @@ int topk_scores(const DeviceInfo &di, const float *scores, uint32_t n, uint32_t 
         return -1;
     }
     int P = (int)next_pow2(k + TOPK_IV + 1);
-    uint32_t num_iv = (n + TOPK_IV - 1) / TOPK_IV;
+    const uint64_t num_iv = ((uint64_t)n + TOPK_IV - 1) / TOPK_IV;  // 64-bit: in 32 bits it wraps to 0 for n > 2^32 - 1024
     uint32_t grid = (uint32_t)di.num_sms * 2;
-    if (grid > num_iv) grid = num_iv;
+    if (grid > num_iv) grid = (uint32_t)num_iv;
     if (ws_reserve((void **)&ws.cand, &ws.cand_bytes, (size_t)grid * P * 8)) return -1;
     if (ws_reserve((void **)&ws.partial, &ws.partial_bytes, (size_t)grid * k * 8)) return -1;
     size_t smem = (size_t)P * 8;
@@ -419,6 +423,22 @@ int topk_scores(const DeviceInfo &di, const float *scores, uint32_t n, uint32_t 
     topk_scores_kernel<<<grid, TOPK_THREADS, smem, s>>>(scores, n, k, P, ws.cand, ws.partial, ws.flags, below);
     NK_CUDA_OK(cudaGetLastError());
     return merge_keys(ws.partial, grid, k, 0, 1, k, out_keys, s);
+}
+
+// keys [k] of topk_scores -> the reference's (index, score) slots: score = scores[row], bit for bit (a -0.0 stays -0.0), and
+// (0, -1e30f) for a slot no admissible score reached, as the reference leaves its unfilled slots (cuda_bridge.go:349-353).
+__global__ void decode_topk_scores_kernel(const uint64_t *keys, uint32_t k, const float *scores, uint32_t *out_idx, float *out_score) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= k) return;
+    const uint64_t key = keys[i];
+    out_idx[i] = key ? key_row(key) : 0u;
+    out_score[i] = key ? scores[key_row(key)] : -1e30f;
+}
+int decode_topk_scores(const uint64_t *keys, uint32_t k, const float *scores, uint32_t *out_idx, float *out_score, cudaStream_t s) {
+    if (k == 0) return 0;
+    decode_topk_scores_kernel<<<(k + 127) / 128, 128, 0, s>>>(keys, k, scores, out_idx, out_score);
+    NK_CUDA_OK(cudaGetLastError());
+    return 0;
 }
 
 }  // namespace nk

@@ -1,6 +1,6 @@
 // rowops.cu — one-pass row kernels behind the legacy ABI and index maintenance.
 //
-//   row_norms       replaces n x cublasSnrm2                  (cuda_bridge.go:231-246)
+//   row_norms       replaces n x cublasSnrm2                  (cuda_bridge.go:231-246), overflow- and underflow-safe like it
 //   normalize_rows  replaces n x cublasSnrm2 + D2H + n x cublasSscal (cuda_bridge.go:249-284)
 //   row_scores      replaces cublasSgemv                      (cuda_bridge.go:290-318)
 //   fill_uniform / fill_clustered   synthetic corpora generated in HBM (bench / tests); the uniform one is bit-identical
@@ -14,6 +14,7 @@
 // overflow uint32 at n*dim >= 2^32, cuda_kernels.cu:195,274,298).  Grids are sized from the device's SM count.
 // HBM-bound; algorithmic bytes: norms / scores n*dim*4 (read once), normalize 2*n*dim*4 (read + write; the row is re-read
 // from L1/L2 for the scaling pass).
+#include <float.h>
 #include <type_traits>
 
 #include "kernels.cuh"
@@ -45,6 +46,29 @@ static inline unsigned warp_grid(uint64_t n, int per_sm = 16) {
     if (blocks == 0) blocks = 1;
     return (unsigned)blocks;
 }
+// Norm of a row whose fp32 sum of squares `a` (the warp-uniform result of the fast path) is not finite, or below 2^-100
+// where subnormal squares lose precision: elements beyond ~1e19 overflow it, elements below ~1e-19 underflow it; cublasSnrm2,
+// which the reference calls, does neither.  As BLAS nrm2 does, the row is summed again scaled by the power of two that
+// brings its largest |x| into [0.5, 1), and the root scaled back.  Rows of ordinary magnitude never get here, so they keep
+// the fast path's bits.  A NaN element gives NaN, an inf element inf, a zero row 0.
+__device__ __noinline__ float scaled_row_norm(const float *p, uint32_t dim, uint32_t lane, float a) {
+    if (a != a) return a;
+    float m = 0.0f;
+    for (uint32_t j = lane; j < dim; j += 32) m = fmaxf(m, fabsf(p[j]));
+#pragma unroll
+    for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if (m == 0.0f || isinf(m)) return m;
+    int e;
+    frexpf(m, &e);
+    float t = 0.0f;
+    for (uint32_t j = lane; j < dim; j += 32) {
+        const float x = scalbnf(p[j], -e);
+        t = fmaf(x, x, t);
+    }
+    return scalbnf(sqrtf(warp_sum(t)), e);
+}
+__device__ __forceinline__ bool needs_scaling(float a) { return !(a >= 0x1p-100f && a <= FLT_MAX); }
+
 static inline bool vec4_ok(const void *p, uint32_t dim) { return dim % 4 == 0 && (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 template <bool VEC>
@@ -67,7 +91,8 @@ __global__ void row_norms_kernel(const float *rows, float *norms, uint32_t n, ui
             }
         }
         a = warp_sum(a);
-        if (lane == 0) norms[r] = sqrtf(a);
+        const float nrm = needs_scaling(a) ? scaled_row_norm(p, dim, lane, a) : sqrtf(a);
+        if (lane == 0) norms[r] = nrm;
     }
 }
 
@@ -84,7 +109,8 @@ __global__ void normalize_rows_kernel(float *rows, uint32_t n, uint32_t dim) {
                 const float4 v = p4[j];
                 a = fmaf(v.x, v.x, a); a = fmaf(v.y, v.y, a); a = fmaf(v.z, v.z, a); a = fmaf(v.w, v.w, a);
             }
-            const float nrm = sqrtf(warp_sum(a));
+            a = warp_sum(a);
+            const float nrm = needs_scaling(a) ? scaled_row_norm(p, dim, lane, a) : sqrtf(a);
             if (nrm > 1e-10f) {  // cuda_bridge.go:267: rows with norm <= 1e-10 are left untouched
                 const float inv = 1.0f / nrm;
                 for (uint32_t j = lane; j < dim / 4; j += 32) {
@@ -95,7 +121,8 @@ __global__ void normalize_rows_kernel(float *rows, uint32_t n, uint32_t dim) {
             }
         } else {
             for (uint32_t j = lane; j < dim; j += 32) a = fmaf(p[j], p[j], a);
-            const float nrm = sqrtf(warp_sum(a));
+            a = warp_sum(a);
+            const float nrm = needs_scaling(a) ? scaled_row_norm(p, dim, lane, a) : sqrtf(a);
             if (nrm > 1e-10f) {
                 const float inv = 1.0f / nrm;
                 for (uint32_t j = lane; j < dim; j += 32) p[j] *= inv;
@@ -140,7 +167,7 @@ __global__ void row_scores_kernel(const float *rows, const float *query, float *
                 scores[r] = d;
             } else {
                 float den = sqrtf(xx * qq);
-                scores[r] = den > 0.0f ? d / den : 0.0f;
+                scores[r] = den == 0.0f ? 0.0f : d / den;  // 0 for a zero row or query; a NaN element stays NaN
             }
         }
     }
